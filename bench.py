@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - alignments/sec of the ffsubsync hot path on B200 (BASELINE.json metric).
+"""bench.py - alignments/sec of the ffsubsync hot path on H100 (BASELINE.json metric).
 
 A "step" = one pass of the whole hot path (VAD on 2 h of 16 kHz PCM -> K=5 ratio candidates
 rasterised -> windowed FFT correlation + exact re-score -> max over ratios) over one batch of
@@ -7,9 +7,11 @@ synthetic pairs per GPU.  `value` counts whole-job alignments (pairs) per second
 already resident in HBM; `e2e` is the same call through the C ABI with HOST (pinned) buffers,
 H2D/D2H inside the timed region.  `--impl reference` times the reference's own CPU algorithm
 (numpy complex128 FFT aligner + the numpy restatement of the detector, oracle/) on the host
-cores of the same box.
+cores of the same box.  `--dump-outputs DIR` writes what the last timed step returned
+(best_score / best_offset / best_k of every pair, float64) as DIR/<name>.npy; the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 
-    python bench.py --gpus 1 --steps 5 --warmup 3
+    python bench.py --gpus 1 --steps 5 --warmup 3 [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         --master-port 29500 bench.py --gpus 8 --steps 5 --warmup 3
 """
@@ -46,7 +48,7 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json, copy bandwidth)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3), not a measured figure"
 
 
 class ClockSampler:
@@ -138,8 +140,8 @@ class ClockSampler:
 def workload_config(world, B, K):
     """The `config` object both arms print (same keys and values: the reference arm times a bounded
     sample of THIS workload, see its cpu_baseline.sample)."""
-    name = ("BASELINE configs[3]: 4096 two-hour pairs sharded over 8 GPUs (512 per GPU)"
-            if (world == 8 and B == 512) else
+    name = ("BASELINE configs[3]: 2048 two-hour pairs sharded over 8 GPUs (256 per GPU)"
+            if (world == 8 and B == 256) else
             "BASELINE configs[2]: batch of 256 two-hour pairs per GPU" if B == 256 else
             "batch of %d two-hour pairs per GPU (BASELINE configs[2] workload at another batch size)" % B)
     return {"workload": name + ", with the VAD of configs[1]: 16 kHz mono s16le PCM -> energy/ZCR "
@@ -148,12 +150,13 @@ def workload_config(world, B, K):
 
 
 def default_pairs(world):
-    """BASELINE configs[2]: 256 two-hour pairs on one GPU; configs[3]: 4096 pairs over 8 GPUs =
-    512 per GPU.  (2 and 4 GPUs keep 256 per GPU.)  B2_BENCH_PAIRS / --pairs override."""
+    """BASELINE configs[2]: 256 two-hour pairs on one GPU; configs[3]: 2048 pairs over 8 GPUs =
+    256 per GPU (59 GB of PCM: what fits an 80 GB H100 beside the workspaces).  B2_BENCH_PAIRS /
+    --pairs override."""
     env = os.environ.get("B2_BENCH_PAIRS")
     if env:
         return int(env)
-    return 512 if world >= 8 else 256
+    return 256
 
 
 _CHECK_JOBS = []   # filled before the worker pool forks (the PCM of a pair is 230 MB: inherited, not pickled)
@@ -235,16 +238,6 @@ def verify_against_oracle(bs, pairs, pcm_d, pcm_off, ratios, n_sample, seed):
             "mismatches": bad[:8], "oracle_seconds": round(time.perf_counter() - t0, 1),
             "what": "b2_sync_batch on the full batch vs oracle (numpy detector + complex128 FFTAligner + "
                     "MaxScoreAligner) on a seeded sample; offsets exact, scores <= 1e-5 relative"}
-
-
-def measured_traffic():
-    """DRAM bytes per launch of the dominant kernel from this round's `ncu --set full` capture
-    (profiles/r2_vad_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep)."""
-    p = os.path.join(ROOT, "profiles", "r2_vad_traffic.json")
-    if os.path.exists(p):
-        with open(p) as fh:
-            return json.load(fh)
-    return None
 
 
 def run_gpu(args):
@@ -358,6 +351,11 @@ def run_gpu(args):
     drain()
     ev1.record(stream)
     torch.cuda.synchronize()
+    if args.dump_outputs:   # what the last timed step returned (gathered over ranks on rank 0)
+        last = state["last"] if gather else None
+        dumped = ({k: last[:, i] for i, k in enumerate(("best_score", "best_offset", "best_k"))}
+                  if last is not None else out)
+        dumped = {k: v.cpu().numpy().astype(np.float64) for k, v in dumped.items()}
     if world > 1:
         torch.distributed.barrier()
     steps = done
@@ -411,25 +409,15 @@ def run_gpu(args):
                                              memspace=_native.B2_DEVICE), args.steps)
         stages = {"vad_ms": vad_ms, "rasterize_ms": ras_ms, "align_ms": ali_ms}
         achieved = BYTES_VAD * B / (vad_ms * 1e-3) / 1e9
-        tr = measured_traffic()
-        traffic = traffic_src = None
-        if tr:
-            ratio = tr["dram_bytes_per_launch"] / float(tr["algorithmic_bytes_per_launch"])
-            traffic = BYTES_VAD * B * ratio
-            traffic_src = ("ncu --set full dram__bytes_read.sum + dram__bytes_write.sum of a %d-pair launch "
-                           "(%s), x%.4f of its algorithmic bytes, scaled to this launch's pairs"
-                           % (tr["pairs"], tr["source"], ratio))
         roofline = {"kernel": "vad_lane_kernel<20, 1> (b2_vad_energy_zcr over the whole batch, all SMs)", "bound": "hbm", "achieved": achieved, "peak": peak,
-                    "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,
-                    "peak_source": peak_src,
-                    "frac_note": "the peak is a COPY bandwidth (read+write mix); this kernel is 98.8 %% reads, "
-                                 "which HBM3e serves faster than a copy - frac > 1 is not an error. Against the "
-                                 "8000 GB/s data-sheet figure: %.3f" % (achieved / 8000.0),
+                    "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
+                    "frac_note": "algorithmic bytes (PCM read + signal written) over the event-timed kernel; "
+                                 "against the 3350 GB/s H100 SXM data-sheet figure: %.3f" % (achieved / 3350.0),
                     "algorithmic_bytes_per_launch": BYTES_VAD * B,
                     "stages_note": "stages_ms time b2_vad_energy_zcr / b2_rasterize / b2_align_batch called "
                                    "one by one; the timed step calls b2_sync_batch, which replaces the float "
                                    "rasteriser by bit masks (no rasterize_ms on that path) and, from 96 pairs on, "
-                                   "runs the VAD of sub-batches 2 and 3 on 80 SMs beside the alignment of the "
+                                   "runs the VAD of sub-batches 2 and 3 on 54 % of the SMs beside the alignment of the "
                                    "previous sub-batch (the step is shorter than vad_ms + align_ms)",
                     "whole_path": {"achieved": (BYTES_VAD + bytes_align(K)) * B * steps
                                    / (elapsed_ms * 1e-3) / 1e9 if world == 1 else None,
@@ -482,7 +470,7 @@ def run_gpu(args):
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "int64 VAD; f32 FFT nomination + f64 exact re-score", "data": "synthetic",
             "config": dict(workload_config(world, B, K),
-                           l2_policy="inputs (%.1f GB PCM per GPU) are far larger than the 126 MB L2" % (B * 0.2304),
+                           l2_policy="inputs (%.1f GB PCM per GPU) are far larger than the 50 MB L2" % (B * 0.2304),
                            parallelism="pairs block-sharded, dp%d" % world,
                            call=("b2_sync_batch(B2_DEVICE): every step ordered after the previous one" if args.ordered_calls
                                  else "b2_sync_batch(B2_DEVICE_RESIDENT): the PCM is resident and constant, so the VAD of "
@@ -496,6 +484,10 @@ def run_gpu(args):
             "roofline": roofline, "e2e": e2e, "cpu_baseline": cpu_base,
         }
         print(json.dumps(line))
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for k, v in dumped.items():
+                np.save(os.path.join(args.dump_outputs, k + ".npy"), v)
     if world > 1:
         torch.distributed.barrier()
         torch.distributed.destroy_process_group()
@@ -541,9 +533,8 @@ def _cpu_setup(ratios):
 
 def available_cores():
     """Host cores this process may actually use: the container's CPU quota (cgroup v2 cpu.max, v1
-    cfs_quota) when there is one, else the affinity mask.  On the bench pod os.cpu_count() says 128
-    but cpu.max is "1600000 100000" = 16 cores: 16 workers give 4.9 alignments/s, 32 give 3.1, 128
-    give 1.9 (profiles/r2a_cpu_sweep.json) - oversubscribing the quota only adds context switches.
+    cfs_quota) when there is one, else the affinity mask: in a container os.cpu_count() can report
+    far more cores than the quota grants, and oversubscribing the quota only adds context switches.
     B2_CPU_WORKERS overrides."""
     if os.environ.get("B2_CPU_WORKERS"):
         return max(1, int(os.environ["B2_CPU_WORKERS"])), "B2_CPU_WORKERS"
@@ -629,8 +620,8 @@ def run_reference(args):
                          "cores_source": quota_src, "kind": "port",
                          "sample": "%d two-hour pairs per step, one per worker process" % per_step},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
-        "note": "the reference is pure Python and cannot travel to the GPU box; this is the oracle port of "
-                "its algorithm (pinned to the reference by tests/golden) on all host cores",
+        "note": "this is the oracle port of the reference's algorithm (pinned to the reference by "
+                "tests/golden) on all host cores",
     }
     print(json.dumps(line))
 
@@ -642,17 +633,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--pairs", type=int, default=0,
-                    help="2 h pairs per GPU per step (default: BASELINE configs[2] = 256 on 1/2/4 GPUs, "
-                         "configs[3] = 512 per GPU on 8 GPUs; 59 / 118 GB of PCM per GPU)")
+                    help="2 h pairs per GPU per step (default: 256 = BASELINE configs[2] on 1 GPU, configs[3] "
+                         "on 8 GPUs; 59 GB of PCM per GPU)")
     ap.add_argument("--min-seconds", type=float, default=0.0,
                     help="1 GPU only: repeat the K timed steps until the timed region is at least this long "
-                         "(sustained-clock runs for profiles/; `steps` in the output is what actually ran)")
+                         "(sustained-clock runs; `steps` in the output is what actually ran)")
     ap.add_argument("--oracle-pairs", type=int, default=8,
                     help="pairs of the batch cross-checked against the oracle after the timed region")
     ap.add_argument("--no-oracle-check", action="store_true")
     ap.add_argument("--ratios", type=int, default=5)
     ap.add_argument("--e2e-pairs", type=int, default=4)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (float64 .npy per output) into DIR")
     ap.add_argument("--ordered-calls", action="store_true",
                     help="timed steps call b2_sync_batch with B2_DEVICE instead of B2_DEVICE_RESIDENT (A/B)")
     args = ap.parse_args()

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI in include/ffsubsync_b200.h.
 
-There is deliberately NO CPU fallback: if the CUDA library is missing or no B200 is visible,
+There is deliberately NO CPU fallback: if the CUDA library is missing or no H100 is visible,
 every compute entry point raises.  Build the library with ``python __graft_entry__.py``.
 """
 import ctypes
@@ -131,7 +131,7 @@ class Handle:
         st = self.lib.b2_create(int(device), ctypes.byref(h))
         if st != 0:
             raise NativeError(st, "b2_create(device=%d)" % device,
-                              "no usable sm_100 CUDA device; this package has no CPU path")
+                              "no usable sm_90 (H100) CUDA device; this package has no CPU path")
         self.h = h
         self.device = device
 

@@ -50,7 +50,7 @@ extern "C" int b2_create(int device, b2_handle* out) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete h; return B2_ERR_CUDA; }
   h->sm_count = prop.multiProcessorCount;
-  if (prop.major != 10) {  // built for sm_100a only: fail loudly instead of falling back
+  if (prop.major != 9 || prop.minor != 0) {  // built for sm_90a only: fail loudly instead of falling back
     delete h;
     return B2_ERR_UNSUPPORTED;
   }
@@ -79,8 +79,6 @@ extern "C" int b2_create(int device, b2_handle* out) {
     return B2_ERR_CUDA;
   }
   h->log2_quirk_mask = compute_log2_quirk_mask();
-  const char* acc = getenv("B2_ACC");  // A/B switch for profiling: "reg" keeps the accumulators in registers
-  h->acc_in_tmem = !(acc && strcmp(acc, "reg") == 0);
   *out = h;
   return B2_OK;
 }
@@ -278,8 +276,8 @@ static cudaEvent_t next_event(b2_ctx* h) {
 
 // ---- helpers for B2_HOST calls -------------------------------------------------------------
 // Large PAGEABLE inputs (a numpy array of PCM: 230 MB per 2 h signal): cudaMemcpyAsync stages them
-// through the driver's bounce buffer with one thread at ~11 GB/s (measured: 19.9 ms per 230 MB against
-// 4.2 ms from pinned memory, profiles/r2e_latency_single_pair.json).  Here the copy goes through two
+// through the driver's bounce buffer with one thread, several times slower than a copy from pinned
+// memory.  Here the copy goes through two
 // pinned 32 MB buffers filled by kCopyThreads host threads while the previous buffer is on the bus.
 static const size_t kBounceBytes = (size_t)32 << 20;
 static const int kCopyThreads = 6;
@@ -963,14 +961,14 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
   // the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler keeps the
   // two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); with the
   // lane-group kernel (every SM's issue slots to reach the HBM roofline) partitioning never paid
-  // (profiles/r2a_partition_probe.txt).  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
-  // Defaults (measured on 256 two-hour pairs, tools/pipeline_probe.py: 3 sub-batches x 80 of 148 SMs =
-  // 11.16 ms per step against 12.49 unpipelined; 2-6 sub-batches and 74-86 SMs are within 4 %); small
-  // batches stay unpipelined (the alignment of a third of a small batch is launch- and tail-bound).
+  // (tools/partition_probe.py).  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
+  // Defaults: 3 sub-batches, the later VADs on 54 % of the SMs (71 of an H100's 132; tools/pipeline_probe.py
+  // sweeps both); small batches stay unpipelined (the alignment of a third of a small batch is launch- and
+  // tail-bound).
   int n_sub = 1, vad_sms = 0;
   if (B >= 96 && b2i_vad_lane_eligible(pcm_off, B, fpw)) {
     n_sub = 3;
-    vad_sms = (h->sm_count * 80 + 74) / 148;
+    vad_sms = (h->sm_count * 54 + 50) / 100;
   }
   if (const char* e = getenv("B2_SUBBATCHES")) n_sub = std::max(1, std::min(B, atoi(e)));
   if (const char* e = getenv("B2_VAD_SMS")) vad_sms = std::max(0, std::min(h->sm_count, atoi(e)));

@@ -1,5 +1,5 @@
-// Shared plumbing for the B200 ffsubsync hot-path library (internal; the ABI is
-// include/ffsubsync_b200.h).  sm_100a only.
+// Shared plumbing for the ffsubsync hot-path library (internal; the ABI is
+// include/ffsubsync_b200.h).  sm_90a (H100) only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -33,13 +33,12 @@ struct HostBuf {  // pinned
 
 struct b2_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
   std::string err;
   int64_t launches = 0;
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
-  int acc_in_tmem = 1;           // correlation accumulators in tensor memory (B2_ACC=reg: registers)
   int vad_ctas_per_sm = 0;       // 0 = as many as fit; set to 1 while b2_sync_batch pipelines
   int vad_partition_sms = 0;     // > 0: the VAD launches 512-consumer CTAs, one per SM, on this many SMs
   int corr_max_ctas = 0;         // > 0: persistent correlation kernels use at most this many CTAs

@@ -64,7 +64,7 @@ __device__ __forceinline__ void l2_prefetch_floats(const float* p, int n) {
 
 // Persistent over the reference blocks (one CTA per SM): twiddle tables are built once per CTA
 // and the next item's samples are pulled into L2 while the current one is transformed.
-__global__ void __maxnreg__(96)  // leaves registers for a co-resident VAD CTA (see sub_correlate_kernel)
+__global__ void __maxnreg__(96)  // leaves registers for a co-resident VAD CTA of b2_sync_batch's pipeline
     ref_spectra_kernel(const float* __restrict__ ref, const SpecItem* __restrict__ items, int n_items,
                        float4* __restrict__ spec, float* __restrict__ spec_energy) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -99,113 +99,15 @@ __global__ void __maxnreg__(96)  // leaves registers for a co-resident VAD CTA (
   }
 }
 
-// ---- tensor memory as accumulator storage ------------------------------------------------------
-// The 64 accumulator floats of each thread (conj(A)*B summed over the blocks) do not fit next to
-// the butterfly registers without pinning the kernel at 128 registers x 512 threads = the whole
-// register file.  Blackwell's tensor memory (256 KB per SM, unused by this path otherwise) holds
-// them instead: warp w owns lanes 32*(w%4).., columns 64*(w/4)..; each thread moves 16 columns at
-// a time with tcgen05.ld / tcgen05.st (32x32b shape = one 32-bit column per register).
-constexpr int kTmemCols = 256;
-
-__device__ __forceinline__ uint32_t smem_addr_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_addr_u32(smem_dst)),
-               "r"(kTmemCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // one full warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kTmemCols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-      "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-      "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])),
-      "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-      "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// acc (tensor memory) += conj(A) * B for one block.  Column group g holds the thread's pair slots
-// 4g..4g+3 as (cp.x, cp.y, cq.x, cq.y) each; the load of group g+1 is in flight while group g is
-// updated.  FIRST: nothing accumulated yet, start from zero instead of loading.
-// DEPTH = how many slots ahead the stored reference spectrum is read (measured on the 148-pair
-// bench: 2, 4 and 8 give 7.20 / 7.23 / 7.23 ms per step - the loads are not the limiter).
-template <bool FIRST, int DEPTH>
-__device__ __forceinline__ void accumulate_block_tmem(uint32_t taddr, const float2* buf,
-                                                      const Tables& t, const PairCtx& pc, int tid,
-                                                      const float4* __restrict__ spec) {
-  float4 bq[DEPTH];
-#pragma unroll
-  for (int d = 0; d < DEPTH; ++d) bq[d] = __ldg(spec + tid + d * kThreads);
-  float cur[16], nxt[16];
-  if (!FIRST) {
-    tmem_ld16(taddr, cur);
-    tmem_wait_ld();
-  }
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    if (FIRST) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) cur[i] = 0.f;
-    } else if (g + 1 < 4) {
-      tmem_ld16(taddr + 16 * (g + 1), nxt);
-    }
-#pragma unroll
-    for (int uu = 0; uu < 4; ++uu) {
-      const int u = 4 * g + uu;
-      const float4 b = bq[u % DEPTH];
-      if (u + DEPTH < 16) bq[u % DEPTH] = __ldg(spec + tid + (u + DEPTH) * kThreads);
-      float2 dp, dq;
-      product_terms(buf, t, pc, tid, u, b, dp, dq);
-      cur[4 * uu + 0] += dp.x;
-      cur[4 * uu + 1] += dp.y;
-      cur[4 * uu + 2] += dq.x;
-      cur[4 * uu + 3] += dq.y;
-    }
-    tmem_st16(taddr + 16 * g, cur);
-    if (!FIRST && g + 1 < 4) {
-      tmem_wait_ld();
-#pragma unroll
-      for (int i = 0; i < 16; ++i) cur[i] = nxt[i];
-    }
-  }
-  tmem_wait_st();
-}
-
 // BITS = false: the subtitle signal is a float array in global memory (b2_align_batch).
 // BITS = true : it is a bit mask, one bit per frame (b2_sync_batch: raster_bits_kernel writes the
 //   K masks of a pair straight from the cue list, 1/32 of the bytes of the float signals, and the
 //   exact re-score reads the same masks).  The words of block blk+1 are fetched while block blk is
 //   transformed (registers -> shared memory, double buffered).
-template <bool TMEM, bool BITS, int DEPTH = 2>
+// The 64 accumulator floats of each thread (conj(A)*B summed over the blocks) live in registers:
+// 128 registers x 512 threads is the whole register file of an SM, and shared memory is taken by
+// the transform buffer (a further 128 KB of accumulators would exceed the 227 KB a block may use).
+template <bool BITS>
 __device__ __forceinline__ void sub_correlate_body(
     const float* __restrict__ sub, const SubJob* __restrict__ jobs, const float4* __restrict__ spec,
     const float* __restrict__ spec_energy, int L, float* __restrict__ scores,
@@ -216,7 +118,6 @@ __device__ __forceinline__ void sub_correlate_body(
   float2* fine32 = tw1024 + 1024;
   uint32_t* bit_words = reinterpret_cast<uint32_t*>(smem_raw + kSmemBytes);  // [2][kP/32] (BITS only)
   __shared__ float red[kThreads / 32];
-  __shared__ uint32_t tmem_base_s;
   const int tid = threadIdx.x;
   const SubJob job = jobs[blockIdx.x];
   float* out = scores + job.score_off;
@@ -233,17 +134,7 @@ __device__ __forceinline__ void sub_correlate_body(
     uint32_t* dst = bit_words + (job.blk_lo & 1) * (kP / 32);
     for (int w = tid; w < wpb; w += kThreads) dst[w] = __ldg(src + w);
   }
-  uint32_t taddr = 0;
-  if (TMEM) {
-    if (tid < 32) tmem_alloc(&tmem_base_s);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
   __syncthreads();
-  if (TMEM) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int warp = tid >> 5;
-    taddr = tmem_base_s + (uint32_t)(((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * 64);
-  }
   const Tables t{tw1024, fine32};
   const PairCtx pc = pair_ctx(t, tid);
   SubState st;
@@ -273,12 +164,7 @@ __device__ __forceinline__ void sub_correlate_body(
       st.ss += forward_block(buf, t, tid, s);
     }
     const size_t item = (size_t)(job.spec_base + (blk - job.blk_lo));
-    if (TMEM) {
-      if (blk == job.blk_lo) accumulate_block_tmem<true, DEPTH>(taddr, buf, t, pc, tid, spec + item * kPairs);
-      else accumulate_block_tmem<false, DEPTH>(taddr, buf, t, pc, tid, spec + item * kPairs);
-    } else {
-      sub_accumulate(st, buf, t, pc, tid, spec + item * kPairs);
-    }
+    sub_accumulate(st, buf, t, pc, tid, spec + item * kPairs);
     er += spec_energy[item];
     if (BITS) {  // the other buffer was last read in block blk-1's first pass
       uint32_t* dst = bit_words + ((blk + 1) & 1) * (kP / 32);
@@ -286,19 +172,6 @@ __device__ __forceinline__ void sub_correlate_body(
       dst[tid + kThreads] = nw1;
     }
     __syncthreads();  // buf is rewritten by the next block's first pass
-  }
-  if (TMEM) {  // accumulators back into registers for the retangle
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      float v[16];
-      tmem_ld16(taddr + 16 * g, v);
-      tmem_wait_ld();
-#pragma unroll
-      for (int uu = 0; uu < 4; ++uu) {
-        st.cp[4 * g + uu] = make_float2(v[4 * uu + 0], v[4 * uu + 1]);
-        st.cq[4 * g + uu] = make_float2(v[4 * uu + 2], v[4 * uu + 3]);
-      }
-    }
   }
   sub_retangle_store(st, buf, t, pc, tid);
   __syncthreads();
@@ -338,52 +211,23 @@ __device__ __forceinline__ void sub_correlate_body(
     }
     job_energy[job.energy_slot] = make_float4(e, er, c2, (float)(job.blk_hi - job.blk_lo));
   }
-  if (TMEM) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (tid < 32) tmem_dealloc(tmem_base_s);
-  }
 }
 
-// Product kernel: accumulators in tensor memory, 96 registers per thread so that 16 K registers
-// and 88 KB of shared memory per SM stay free for a co-resident VAD CTA of the next sub-batch
-// (b2_sync_batch's optional sub-batch pipeline, B2_SUBBATCHES).  Measured: the co-resident VAD CTA
-// cannot keep enough bytes in flight in that space, the overlap gains 2 % (profiles/README.md), so
-// the pipeline is off by default; a 128-register variant of this kernel is not faster either.
-constexpr int kSubRegs = 96;
-__global__ void __maxnreg__(kSubRegs)
+// Product kernel, one CTA of 512 threads per SM (accumulators in registers, see above).
+__global__ void __launch_bounds__(kThreads, 1)
     sub_correlate_kernel(const float* __restrict__ sub, const SubJob* __restrict__ jobs,
                          const float4* __restrict__ spec, const float* __restrict__ spec_energy,
                          int L, float* __restrict__ scores, float4* __restrict__ job_energy) {
-  sub_correlate_body<true, false>(sub, jobs, spec, spec_energy, L, scores, job_energy, nullptr);
+  sub_correlate_body<false>(sub, jobs, spec, spec_energy, L, scores, job_energy, nullptr);
 }
 
 // b2_sync_batch: subtitle signals as bit masks (no float subtitle signal in HBM).
-__global__ void __maxnreg__(kSubRegs)
+__global__ void __launch_bounds__(kThreads, 1)
     sub_correlate_bits_kernel(const SubJob* __restrict__ jobs, const float4* __restrict__ spec,
                               const float* __restrict__ spec_energy, int L,
                               float* __restrict__ scores, float4* __restrict__ job_energy,
                               const uint32_t* __restrict__ sub_bits) {
-  sub_correlate_body<true, true>(nullptr, jobs, spec, spec_energy, L, scores, job_energy, sub_bits);
-}
-
-// A/B variant (B2_ACC=reg): accumulators in registers, 128 registers per thread.
-__global__ void __launch_bounds__(kThreads, 1)
-    sub_correlate_regacc_kernel(const float* __restrict__ sub, const SubJob* __restrict__ jobs,
-                                const float4* __restrict__ spec,
-                                const float* __restrict__ spec_energy, int L,
-                                float* __restrict__ scores, float4* __restrict__ job_energy) {
-  sub_correlate_body<false, false>(sub, jobs, spec, spec_energy, L, scores, job_energy, nullptr);
-}
-
-// Same for the bit-mask path (compute-sanitizer's synccheck does not model tcgen05.alloc; the
-// sanitizer runs use B2_ACC=reg).
-__global__ void __launch_bounds__(kThreads, 1)
-    sub_correlate_bits_regacc_kernel(const SubJob* __restrict__ jobs, const float4* __restrict__ spec,
-                                     const float* __restrict__ spec_energy, int L,
-                                     float* __restrict__ scores, float4* __restrict__ job_energy,
-                                     const uint32_t* __restrict__ sub_bits) {
-  sub_correlate_body<false, true>(nullptr, jobs, spec, spec_energy, L, scores, job_energy, sub_bits);
+  sub_correlate_body<true>(nullptr, jobs, spec, spec_energy, L, scores, job_energy, sub_bits);
 }
 
 // ---- candidate selection ---------------------------------------------------------------------
@@ -744,8 +588,6 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
     B2_TRY(b2i_raster_bits_launch(h, cue_src, B, K, sub_off, bits_off.data(), d_bits));
     B2_CUDA(h, cudaFuncSetAttribute(sub_correlate_bits_kernel,
                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesBits));
-    B2_CUDA(h, cudaFuncSetAttribute(sub_correlate_bits_regacc_kernel,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesBits));
   }
   void* d_cand;
   B2_TRY(b2i_ws(h, b2_ctx::WS_CAND, J * kCandMax * (8 * kRescoreSeg + 8) + J * 12 + 64, &d_cand));
@@ -823,8 +665,6 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
                                   (int)kSmemBytes));
   B2_CUDA(h, cudaFuncSetAttribute(sub_correlate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)kSmemBytes));
-  B2_CUDA(h, cudaFuncSetAttribute(sub_correlate_regacc_kernel,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
 
   // Work is issued in groups so that the reference spectra of a group fit the workspace cap.
   const size_t kSpecBytes = (size_t)kPairs * 16;
@@ -854,17 +694,11 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
                                                                     spec, spec_energy);
       B2_CHECK_LAUNCH(h, "ref_spectra_kernel");
     }
-    if (cue_mode && h->acc_in_tmem)
+    if (cue_mode)
       sub_correlate_bits_kernel<<<(unsigned)jobs.size(), kThreads, kSmemBytesBits, h->stream>>>(
           d_jobs, spec, spec_energy, L, scores, job_energy, d_bits);
-    else if (cue_mode)
-      sub_correlate_bits_regacc_kernel<<<(unsigned)jobs.size(), kThreads, kSmemBytesBits, h->stream>>>(
-          d_jobs, spec, spec_energy, L, scores, job_energy, d_bits);
-    else if (h->acc_in_tmem)
-      sub_correlate_kernel<<<(unsigned)jobs.size(), kThreads, kSmemBytes, h->stream>>>(
-          d_sub, d_jobs, spec, spec_energy, L, scores, job_energy);
     else
-      sub_correlate_regacc_kernel<<<(unsigned)jobs.size(), kThreads, kSmemBytes, h->stream>>>(
+      sub_correlate_kernel<<<(unsigned)jobs.size(), kThreads, kSmemBytes, h->stream>>>(
           d_sub, d_jobs, spec, spec_energy, L, scores, job_energy);
     B2_CHECK_LAUNCH(h, "sub_correlate_kernel");
     items.clear();

@@ -40,17 +40,15 @@ CORR_HD float2 cmul(float2 a, float2 b) {
 CORR_HD float2 cmul_conj_a(float2 a, float2 b) {  // conj(a) * b
   return make_float2(a.x * b.x + a.y * b.y, a.x * b.y - a.y * b.x);
 }
-// Blackwell packed fp32x2 arithmetic (SASS FADD2 / FFMA2): one instruction per complex add.
+// Componentwise complex add and fused multiply-add.  Hopper has no packed fp32x2 instructions,
+// so each is two scalar FADD / FFMA; the fused form is spelled out so that the device result does
+// not depend on the compiler's contraction choices.
 CORR_HD float2 padd(float2 a, float2 b) {
-#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ >= 1000
-  return __fadd2_rn(a, b);
-#else
   return make_float2(a.x + b.x, a.y + b.y);
-#endif
 }
 CORR_HD float2 pfma(float2 a, float2 b, float2 c) {  // a*b + c, componentwise
-#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ >= 1000
-  return __ffma2_rn(a, b, c);
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 #else
   return make_float2(a.x * b.x + c.x, a.y * b.y + c.y);
 #endif
@@ -304,7 +302,7 @@ struct BlockSource {
 // The 16 complex inputs (32 samples) of one first-pass butterfly, j + q*1024, q = 0..15.
 // All global loads are issued back to back with clamped (always valid) addresses and masked
 // afterwards, so that the 16 (or 32) loads of a thread are in flight together; a branchy
-// per-element version serialised them on the memory latency (profiles/r1: 56 % long-scoreboard).
+// per-element version serialised them on the memory latency.
 CORR_HD void load_block16(const BlockSource& s, int j, float2 (&v)[16]) {
   if (s.t_hi <= s.t_lo) {
 #pragma unroll
@@ -642,8 +640,7 @@ CORR_HD void product_terms(const float2* buf, const Tables& t, const PairCtx& c,
 }
 
 // Consumer: acc += conj(A) * B for the subtitle block spectrum in buf and the stored B.
-// (Register-accumulator form; the device kernel keeps the accumulators in tensor memory instead,
-// see sub_correlate_kernel - this form is what tests/host_emul runs.)
+// (Used by sub_correlate_kernel on the device and by tests/host_emul on the CPU.)
 CORR_HD void sub_accumulate(SubState& st, const float2* buf, const Tables& t, const PairCtx& c,
                             int tid, const float4* spec) {
   // the stored reference spectrum is read two slots ahead of its use (L2 latency)

@@ -684,9 +684,8 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   int wpt = 1;
   if (const char* e = getenv("B2_VAD_WPT")) wpt = std::max(1, std::min(8, atoi(e)));  // tuning knob
   p.fpw = fpw;
-  // Measured after the per-tile overhead was cut (tools/vad_tune.py, 100 x 2 h signals at 16 kHz):
-  // 4 stages x 2 CTAs/SM 7.25 TB/s, 2 x 3 CTAs 7.06, 2 x 4 CTAs 5.63, 4 x 1 CTA 4.59 - ring depth
-  // now matters more than resident warps, so the ring is 4 deep when two such CTAs fit an SM.
+  // Ring depth matters more than resident warps (tools/vad_tune.py sweeps stages x CTAs per SM),
+  // so the ring is 4 deep when two such CTAs fit an SM.
   int stages = consumers == 512 ? kMaxStages : 4;
   if (const char* e = getenv("B2_VAD_STAGES")) stages = std::max(2, std::min(kMaxStages, atoi(e)));  // tuning knob
   const size_t ring_cap = consumers == 512 ? 216 * 1024 : 200 * 1024;

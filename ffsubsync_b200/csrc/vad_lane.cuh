@@ -4,7 +4,7 @@
 //
 // Why: with 4 lanes per window (vad.cu's original layout) the per-window bookkeeping - shuffles,
 // 64-bit sums, predicates - costs as many instructions as the arithmetic (3.25 instructions per byte
-// and lane: the kernel saturates the issue slots of all 148 SMs to reach the HBM roofline, nothing can
+// and lane: the kernel saturates the issue slots of every SM to reach the HBM roofline, nothing can
 // share the GPU with it).  Here a lane streams its window with 17 instructions per 16 bytes:
 //   energy    x = 256 h + l (h = signed high byte, l = unsigned low byte)
 //             sum x^2 = 65536 sum h^2 + 512 sum h l + sum l^2 : three 4-way byte dot products per 4 samples

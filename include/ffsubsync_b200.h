@@ -1,5 +1,5 @@
 /*
- * ffsubsync_b200.h - C ABI of the B200-native ffsubsync alignment hot path.
+ * ffsubsync_b200.h - C ABI of the H100-native ffsubsync alignment hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / C++ types.  Each entry
  * point names the piece of the reference (smacke/ffsubsync, paths relative to the reference

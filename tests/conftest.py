@@ -13,7 +13,7 @@ for p in (ROOT, GOLDEN_DIR):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def _cuda_device_count() -> int:
@@ -34,7 +34,7 @@ def _cuda_device_count() -> int:
 def pytest_collection_modifyitems(config, items):
     gpu_items = [it for it in items if it.get_closest_marker("gpu")]
     if gpu_items and _cuda_device_count() == 0:
-        skip = pytest.mark.skip(reason="no CUDA device visible (gpu tests run on the B200 box)")
+        skip = pytest.mark.skip(reason="no CUDA device visible (gpu tests run on an H100)")
         for it in gpu_items:
             it.add_marker(skip)
 

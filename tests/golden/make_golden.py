@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in this directory by running the REAL reference.
 
-Run in the build container only (it reads /root/reference, which does not exist on the GPU
-box):   python tests/golden/make_golden.py
+Run where a checkout of the reference is available (FFSUBSYNC_REFERENCE names it; the tests only
+read the fixtures this writes):   FFSUBSYNC_REFERENCE=<checkout> python tests/golden/make_golden.py
 
 The reference package cannot be imported normally here (ffmpeg-python, srt, pysubs2, tqdm
 wheels are absent), so the hot-path modules are imported by path behind stub modules for the
@@ -22,7 +22,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import cases  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("FFSUBSYNC_REFERENCE", "ffsubsync-reference")  # checkout of smacke/ffsubsync v0.5.0
 
 
 def load_reference():
@@ -359,7 +359,7 @@ def main():
     gen_maxscore(mods, out)
     gen_segment_starts(mods, out)
     gen_misc(mods, out)
-    out["_meta"] = {"reference": "smacke/ffsubsync @ /root/reference (v0.5.0)",
+    out["_meta"] = {"reference": "smacke/ffsubsync (v0.5.0)",
                     "numpy": np.__version__, "python": sys.version.split()[0],
                     "generator": "tests/golden/make_golden.py"}
     with open(os.path.join(HERE, "golden.json"), "w") as fh:

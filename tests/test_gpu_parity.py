@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI / the
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI / the
 reference-shaped Python API, against the oracle and the committed golden fixtures.
 
 Bars: integer/index results bit-exact; correlation scores within 1e-5 relative (north_star)."""

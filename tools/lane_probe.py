@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Lane-per-window VAD kernel (csrc/vad_lane.cuh) against the lane-group kernel, and the SM-partitioned
 overlap it is meant to enable: VAD on X SMs (one CTA per SM) next to the correlation kernels on the other
-148 - X SMs, two streams.
+remaining SMs, two streams.
 
     python tools/lane_probe.py [pairs]
 """
@@ -24,6 +24,7 @@ KNOBS = ("B2_VAD_BATCH", "B2_VAD_WPL", "B2_VAD_LAYOUT", "B2_VAD_GRID", "B2_VAD_S
 def main():
     B = int(sys.argv[1]) if len(sys.argv) > 1 else 74
     dev = torch.device("cuda", 0)
+    nsm = torch.cuda.get_device_properties(dev).multi_processor_count
     h1, h2 = _native.Handle(0), _native.Handle(0)
     s1, s2 = torch.cuda.Stream(priority=-1), torch.cuda.Stream()
     h1.set_stream(s1.cuda_stream)
@@ -92,20 +93,20 @@ def main():
           "lane + align back to back %.3f ms" % (B, tg, gb / tg * 1e3, tv0, gb / tv0 * 1e3, ta0, tv0 + ta0), flush=True)
     print("--- lane VAD alone, one CTA per SM on X SMs")
     for wpl, batch in (("1", "2"), ("1", "3"), ("1", "4"), ("1", "5"), ("1", "6"), ("2", "1"), ("2", "2")):
-        for X in (148, 90, 74):
+        for X in (nsm, 90, 74):
             os.environ.update(B2_VAD_WPL=wpl, B2_VAD_BATCH=batch, B2_VAD_GRID=str(X))
             tv = timed([vad])
             print("wpl=%s batch=%s X=%3d: %.3f ms = %.0f GB/s = %.1f GB/s per SM"
                   % (wpl, batch, X, tv, gb / tv * 1e3, gb / tv * 1e3 / X), flush=True)
     clear()
-    print("--- both together: lane VAD on X SMs, correlation on 148 - X CTAs")
+    print("--- both together: lane VAD on X SMs, correlation on nsm - X CTAs")
     for X in (74, 86, 100):
-        os.environ.update(B2_VAD_WPL="1", B2_VAD_BATCH=os.environ.get("LANE_PROBE_BATCH", "4"), B2_VAD_GRID=str(X), B2_CORR_MAX_CTAS=str(148 - X))
+        os.environ.update(B2_VAD_WPL="1", B2_VAD_BATCH=os.environ.get("LANE_PROBE_BATCH", "4"), B2_VAD_GRID=str(X), B2_CORR_MAX_CTAS=str(nsm - X))
         tv = timed([vad])
         ta = timed([align])
         tb = timed([vad, align])
         print("X=%3d: vad alone %.3f ms, align alone on %d CTAs %.3f ms, both %.3f ms  (unpartitioned sum %.3f)"
-              % (X, tv, 148 - X, ta, tb, tv0 + ta0), flush=True)
+              % (X, tv, nsm - X, ta, tb, tv0 + ta0), flush=True)
     clear()
 
 

@@ -1,5 +1,5 @@
-// Integer pipe throughput on sm_100a: byte / halfword dot products against IMAD, LOP3, PRMT.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o int_pipes int_pipes.cu && ./int_pipes
+// Integer pipe throughput on sm_90a (H100): byte / halfword dot products against IMAD, LOP3, PRMT.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o int_pipes int_pipes.cu && ./int_pipes
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdint.h>

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """SM-partitioning probe (VERDICT r1 item 4): the HBM-bound VAD on X SMs (one 512-consumer CTA per
 SM, ring filling its shared memory) next to the FP32/shared-memory-bound correlation kernels on the
-other 148 - X SMs (neither kernel fits beside the other on one SM, so the block scheduler keeps them
+other remaining SMs (neither kernel fits beside the other on one SM, so the block scheduler keeps them
 apart), on two streams, the VAD stream at high priority.
 
     python tools/partition_probe.py [pairs]
@@ -25,6 +25,7 @@ FPW, FR = 160, 16000
 def main():
     B = int(sys.argv[1]) if len(sys.argv) > 1 else 74
     dev = torch.device("cuda", 0)
+    nsm = torch.cuda.get_device_properties(dev).multi_processor_count
     h1, h2 = _native.Handle(0), _native.Handle(0)
     s1, s2 = torch.cuda.Stream(priority=-1), torch.cuda.Stream()
     h1.set_stream(s1.cuda_stream)
@@ -80,7 +81,7 @@ def main():
           % (B, tv0, gb / tv0 * 1e3, ta0, tv0 + ta0), flush=True)
     print("--- VAD alone, one CTA per SM on X SMs")
     for consumers, stages in (("512", "5"), ("512", "4"), ("256", "10"), ("256", "8")):
-        for X in (148, 120, 100, 90, 80, 74, 64, 48):
+        for X in (nsm, 120, 100, 90, 80, 74, 64, 48):
             os.environ.update(B2_VAD_CONSUMERS=consumers, B2_VAD_STAGES=stages, B2_VAD_CTAS_FORCE="1",
                               B2_VAD_GRID=str(X))
             tv = timed([vad])
@@ -91,12 +92,12 @@ def main():
     print("--- both together: VAD on X SMs (512 consumers, 5 stages), correlation on the rest")
     for X in (60, 68, 74, 80, 86, 92, 100):
         os.environ.update(B2_VAD_CONSUMERS="512", B2_VAD_STAGES="5", B2_VAD_CTAS_FORCE="1", B2_VAD_GRID=str(X),
-                          B2_CORR_MAX_CTAS=str(148 - X))
+                          B2_CORR_MAX_CTAS=str(nsm - X))
         tv = timed([vad])
         ta = timed([align])
         tb = timed([vad, align])
         print("X=%3d: vad alone %.3f ms, align alone (ref_spectra on %d CTAs) %.3f ms, both %.3f ms  (default sum %.3f)"
-              % (X, tv, 148 - X, ta, tb, tv0 + ta0), flush=True)
+              % (X, tv, nsm - X, ta, tb, tv0 + ta0), flush=True)
 
 
 if __name__ == "__main__":

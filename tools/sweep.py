@@ -28,7 +28,7 @@ from ffsubsync_b200.batch import BatchSynchronizer  # noqa: E402
 from ffsubsync_b200.synth import BENCH_RATIOS, make_pairs  # noqa: E402
 
 FPW, FR = 160, 16000
-PCM_BUDGET = 125e9   # bytes of resident PCM per GPU (180 GB HBM; workspaces and signals need the rest)
+PCM_BUDGET = 55e9    # bytes of resident PCM per GPU (80 GB HBM; workspaces and signals need the rest)
 
 
 def peak():

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Launches the VAD kernel in its SM-partitioned shape (one 512-consumer CTA per SM on X SMs) so that
-ncu can show why an SM cannot go faster (profiles/r2_partition_negative.md).
+ncu can show why an SM cannot go faster.
 
     B2_VAD_CONSUMERS=512 B2_VAD_CTAS_FORCE=1 B2_VAD_STAGES=5 B2_VAD_GRID=74 \
       ncu --set full --clock-control none -k regex:vad_energy -s 2 -c 1 -o gpurun_out/r2_vad_x74 python tools/vad_partition_ncu.py
