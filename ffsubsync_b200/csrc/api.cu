@@ -1,7 +1,7 @@
 // C-ABI entry points (include/ffsubsync_b200.h): handle lifecycle, workspace management and
 // the host<->device staging that turns B2_HOST calls into the device path.  All arithmetic
-// lives in the kernels (vad.cu, raster.cu, corr.cu, select.cu); nothing here computes results
-// on the CPU.
+// lives in the kernels (vad.cu, tokenizer.cu, raster.cu, corr.cu, bigfft.cu); nothing here computes
+// results on the CPU.
 #include <math.h>
 
 #include <chrono>
@@ -921,7 +921,6 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
   // the generic aligner (the b2_align_batch path) reads them back.
   bool fused = true;
   if (const char* e = getenv("B2_FUSED_RASTER")) fused = atoi(e) != 0;
-  B2CueSource cue_src{cue_start_s, cue_end_s, cue_keep, cue_off, ratios, sample_rate, start_seconds};
 
   void *d_refsig, *d_subsig = nullptr, *d_res;
   // a chained resident call (see below) writes the buffer the previous call is not reading any more
@@ -953,18 +952,32 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
   // only the best ratio of each pair is reported unless the per-ratio arrays are requested:
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   const int winner_only = (!all_score && !all_offset) ? 1 : 0;
+  // rasterise (float signals only if !fused) -> align -> reduce the pairs [b0, b1) on the caller's stream
+  auto enqueue_chain = [&](int b0, int b1) -> int {
+    const int nb = b1 - b0;
+    const size_t j0 = (size_t)b0 * K;
+    if (!fused)
+      B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + b0, nb, ratios, K, 0, nullptr,
+                               sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
+    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + b0, ratios, sample_rate, start_seconds};
+    B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + b0, (const float*)d_subsig,
+                            sub_off.data() + j0, nb, K, max_offset_samples, o_score + j0, o_offset + j0,
+                            d_status + j0, winner_only, fused ? &src : nullptr));
+    return b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nb, K, max_offset_samples,
+                             o_bs + b0, o_bo + b0, o_bk + b0);
+  };
 
   // Software pipeline over sub-batches of pairs.  The VAD (HBM-bound) of every sub-batch is queued on the
   // internal high-priority stream: sub-batch 0 on the whole GPU, the later ones on `vad_sms` SMs only (one
   // lane-per-window CTA per SM, csrc/vad.cu); the rasterisation / correlation / reduction of sub-batch i
   // (FP32- and shared-memory bound) follows on the caller's stream as soon as its VAD is done and runs on
   // the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler keeps the
-  // two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); with the
-  // lane-group kernel (every SM's issue slots to reach the HBM roofline) partitioning never paid
-  // (tools/partition_probe.py).  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
-  // Defaults: 3 sub-batches, the later VADs on 54 % of the SMs (71 of an H100's 132; tools/pipeline_probe.py
-  // sweeps both); small batches stay unpipelined (the alignment of a third of a small batch is launch- and
-  // tail-bound).
+  // two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); the
+  // lane-group kernel needs every SM's issue slots to reach the HBM roofline, so partitioning never paid
+  // with it.  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
+  // Defaults: 3 sub-batches of equal size, the later VADs on 54 % of the SMs (71 of an H100's 132;
+  // tools/pipeline_probe.py sweeps both); small batches stay unpipelined (the alignment of a third of a small
+  // batch is launch- and tail-bound).
   int n_sub = 1, vad_sms = 0;
   if (B >= 96 && b2i_vad_lane_eligible(pcm_off, B, fpw)) {
     n_sub = 3;
@@ -972,42 +985,14 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
   }
   if (const char* e = getenv("B2_SUBBATCHES")) n_sub = std::max(1, std::min(B, atoi(e)));
   if (const char* e = getenv("B2_VAD_SMS")) vad_sms = std::max(0, std::min(h->sm_count, atoi(e)));
-  // probe knobs (tools/pipeline_probe.py): share of the pairs in the first sub-batch (its VAD has nothing to
-  // overlap with; 0 = even split), and a cap on the persistent correlation grid while a VAD holds vad_sms SMs
-  int head_pct = 0, corr_cap = 0;
-  if (const char* e = getenv("B2_PIPE_HEAD_PCT")) head_pct = std::max(0, std::min(90, atoi(e)));
-  if (const char* e = getenv("B2_PIPE_CORR_CAP")) corr_cap = atoi(e) != 0;
   if (n_sub == 1) {
     B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off, B, fpw, non_speech_label, (int64_t)fpw * energy_threshold, z_lo,
                           z_hi, (float*)d_refsig, ref_off.data()));
-    if (!fused)
-      B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off, B, ratios, K, 0, nullptr,
-                               sample_rate, start_seconds, (float*)d_subsig, sub_off.data()));
-    B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data(), (const float*)d_subsig, sub_off.data(),
-                            B, K, max_offset_samples, o_score, o_offset, d_status, winner_only,
-                            fused ? &cue_src : nullptr));
-    B2_TRY(b2i_reduce_launch(h, o_score, o_offset, d_status, B, K, max_offset_samples, o_bs, o_bo, o_bk));
+    B2_TRY(enqueue_chain(0, B));
   } else {
     if (n_sub > b2_ctx::kEvents - 2) n_sub = b2_ctx::kEvents - 2;
-    std::vector<int> cut(n_sub + 1);
+    std::vector<int> cut(n_sub + 1);   // n_sub <= B: no sub-batch is empty
     for (int i = 0; i <= n_sub; ++i) cut[i] = (int)((int64_t)B * i / n_sub);
-    if (head_pct > 0 && n_sub > 1) {
-      const int head = std::max(1, std::min(B - (n_sub - 1), (int)((int64_t)B * head_pct / 100)));
-      for (int i = 1; i <= n_sub; ++i) cut[i] = head + (int)((int64_t)(B - head) * (i - 1) / (n_sub - 1));
-    }
-    if (const char* e = getenv("B2_PIPE_CUTS")) {   // probe knob: explicit first pairs of sub-batches 1.., e.g. "54,135,197"
-      std::vector<int> c{0};
-      for (const char* q = e; *q;) {
-        char* end = nullptr;
-        const long v = strtol(q, &end, 10);
-        if (end == q) break;
-        if (v > c.back() && v < B && (int)c.size() < b2_ctx::kEvents - 2) c.push_back((int)v);
-        q = *end ? end + 1 : end;
-      }
-      c.push_back(B);
-      cut = c;
-      n_sub = (int)cut.size() - 1;
-    }
     std::vector<cudaEvent_t> vad_done(n_sub);
     cudaEvent_t inputs_ready = next_event(h);
     B2_CUDA(h, cudaEventRecord(inputs_ready, h->stream));
@@ -1040,10 +1025,9 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
         const int b0 = cut[i], b1 = cut[i + 1];
         h->vad_partition_sms = (i > 0 || prev_busy) ? vad_sms : 0;
         if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
-        const int st = b1 > b0 ? b2i_vad_launch(h, d_pcm, pcm_off + b0, b1 - b0, fpw, non_speech_label,
-                                                (int64_t)fpw * energy_threshold, z_lo, z_hi, (float*)d_refsig,
-                                                ref_off.data() + b0)
-                               : B2_OK;
+        const int st = b2i_vad_launch(h, d_pcm, pcm_off + b0, b1 - b0, fpw, non_speech_label,
+                                      (int64_t)fpw * energy_threshold, z_lo, z_hi, (float*)d_refsig,
+                                      ref_off.data() + b0);
         h->vad_partition_sms = 0;
         if (st != B2_OK) return st;
         vad_done[i] = next_event(h);
@@ -1053,32 +1037,10 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
     }
     host_ms[0] = host_now();
     for (int i = 0; i < n_sub; ++i) {
-      const int b0 = cut[i], b1 = cut[i + 1];
-      const int nb = b1 - b0;
       if (resident && i == n_sub - 1) B2_CUDA(h, cudaEventRecord(h->resident_fence, h->stream));
       B2_CUDA(h, cudaStreamWaitEvent(h->stream, vad_done[i], 0));
       if (trace) B2_CUDA(h, cudaEventRecord(tev[3 + 4 * i], h->stream));
-      if (nb == 0) {
-        if (trace) B2_CUDA(h, cudaEventRecord(tev[4 + 4 * i], h->stream));
-        continue;
-      }
-      struct CapScope {   // restores the handle's grid cap on every exit path
-        b2_ctx* h;
-        int saved;
-        ~CapScope() { h->corr_max_ctas = saved; }
-      } cap_scope{h, h->corr_max_ctas};
-      if (corr_cap && i + 1 < n_sub && vad_sms > 0 && vad_sms < h->sm_count) h->corr_max_ctas = h->sm_count - vad_sms;
-      const size_t j0 = (size_t)b0 * K;
-      if (!fused)
-        B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + b0, nb, ratios, K, 0, nullptr,
-                                 sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
-      B2CueSource sub_src = cue_src;
-      sub_src.cue_off = cue_off + b0;
-      B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + b0, (const float*)d_subsig,
-                              sub_off.data() + j0, nb, K, max_offset_samples, o_score + j0, o_offset + j0,
-                              d_status + j0, winner_only, fused ? &sub_src : nullptr));
-      B2_TRY(b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nb, K, max_offset_samples,
-                               o_bs + b0, o_bo + b0, o_bk + b0));
+      B2_TRY(enqueue_chain(cut[i], cut[i + 1]));
       if (trace) B2_CUDA(h, cudaEventRecord(tev[4 + 4 * i], h->stream));
       host_ms[i + 1] = host_now();
     }
@@ -1095,8 +1057,8 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
         cudaEventElapsedTime(&ms, tev[0], tev[k]);
         return ms;
       };
-      fprintf(stderr, "[b2 pipe] B=%d n_sub=%d vad_sms=%d head_pct=%d corr_cap=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
-              B, n_sub, vad_sms, head_pct, corr_cap, (int)chained, (int)prev_busy, host_ms[0]);
+      fprintf(stderr, "[b2 pipe] B=%d n_sub=%d vad_sms=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
+              B, n_sub, vad_sms, (int)chained, (int)prev_busy, host_ms[0]);
       for (int i = 0; i < n_sub; ++i)
         fprintf(stderr, "[b2 pipe]  sub %d pairs %4d..%4d  VAD %7.3f -> %7.3f ms   chain %7.3f -> %7.3f ms   host enqueued chain at %.3f ms\n",
                 i, cut[i], cut[i + 1], at(1 + 4 * i), at(2 + 4 * i), at(3 + 4 * i), at(4 + 4 * i), host_ms[i + 1]);

@@ -39,9 +39,7 @@ struct b2_ctx {
   std::string err;
   int64_t launches = 0;
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
-  int vad_ctas_per_sm = 0;       // 0 = as many as fit; set to 1 while b2_sync_batch pipelines
-  int vad_partition_sms = 0;     // > 0: the VAD launches 512-consumer CTAs, one per SM, on this many SMs
-  int corr_max_ctas = 0;         // > 0: persistent correlation kernels use at most this many CTAs
+  int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
   // B2_DEVICE_RESIDENT chaining of b2_sync_batch calls (api.cu): `resident_fence` is recorded on the caller's
   // stream before the LAST sub-batch's correlation chain of a pipelined call, `resident_done` after it; the
   // next resident call (if no other entry point ran in between: `resident_fence_valid`) starts its VAD behind
@@ -67,8 +65,8 @@ struct b2_ctx {
   MetaSlot meta[2][kMetaSlots];
   uint64_t meta_seq[2] = {0, 0};
   int ring = 0;                    // ring in use: 0 = caller-facing stream, 1 = internal stream2
-  // b2_sync_batch overlaps the VAD of sub-batch i+1 (stream) with the alignment of sub-batch i
-  // (stream2); events from a small pool order the two
+  // b2_sync_batch overlaps the VAD of sub-batch i+1 (stream2) with the alignment of sub-batch i
+  // (stream); events from a small pool order the two
   // b2_vad_stream_*: ring of pinned/device chunk buffers (H2D + kernel + D2H of chunk i in flight
   // while the caller produces chunk i+1)
   struct VadStream {

@@ -686,10 +686,8 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
     const SubJob* d_jobs = (const SubJob*)b2i_meta_put(&a, jobs.data(), jobs.size() * sizeof(SubJob));
     B2_TRY(b2i_meta_commit(&a));
     if (!items.empty()) {
-      // persistent: one CTA per SM - or per SM the pipeline leaves to the correlation stage
-      int max_ctas = h->corr_max_ctas > 0 ? std::min(h->corr_max_ctas, h->sm_count) : h->sm_count;
-      if (const char* e = getenv("B2_CORR_MAX_CTAS")) max_ctas = std::max(1, std::min(h->sm_count, atoi(e)));  // probe knob
-      const unsigned grid = (unsigned)std::min<size_t>(items.size(), (size_t)max_ctas);
+      // persistent: one CTA per SM
+      const unsigned grid = (unsigned)std::min<size_t>(items.size(), (size_t)h->sm_count);
       ref_spectra_kernel<<<grid, kThreads, kSmemBytes, h->stream>>>(d_ref, d_items, (int)items.size(),
                                                                     spec, spec_energy);
       B2_CHECK_LAUNCH(h, "ref_spectra_kernel");

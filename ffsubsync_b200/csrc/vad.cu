@@ -19,9 +19,9 @@
 
 namespace {
 
-// consumer threads per CTA: 256 (two such CTAs share an SM: the default, whole-GPU launch) or 512
-// (one CTA per SM with a ring of up to 10 stages: the SM-partitioned launch that shares the GPU
-// with the correlation kernels, b2_sync_batch pipeline)
+// lane-group kernel: 256 consumer threads per CTA (two such CTAs share an SM), a ring of up to
+// kMaxStages stages
+constexpr int kConsumerThreads = 256;
 constexpr int kMaxStages = 10;
 // lane-per-window kernel (vad_lane.cuh): tiles of 32 windows per consumer WARP, in a ring of up to
 // kLaneMaxStages stages that fills the SM's shared memory; the producer warp claims and stages kLaneBatch
@@ -246,7 +246,6 @@ __device__ __forceinline__ TileDesc end_tile() {
   return d;
 }
 
-template <int kConsumerThreads>
 __global__ void __launch_bounds__(kConsumerThreads + 32) vad_energy_zcr_kernel(VadParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   unsigned char* data = smem;
@@ -651,13 +650,7 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   if (((uintptr_t)d_pcm & 15) != 0)
     B2_FAIL(h, B2_ERR_BAD_ARG, "vad: device PCM pointer must be 16-byte aligned");
   VadParams p;
-  // CTA shape.  Default: 256 consumer threads, two CTAs per SM.  SM-partitioned launch
-  // (h->vad_partition_sms > 0, set by b2_sync_batch's pipeline): 512 consumer threads, ONE CTA per
-  // SM with a ring that fills its shared memory, on that many SMs only - the correlation kernels of
-  // the previous sub-batch own the other SMs.  B2_VAD_CONSUMERS / B2_VAD_GRID: tuning knobs.
-  int consumers = h->vad_partition_sms > 0 ? 512 : 256;
-  if (const char* e = getenv("B2_VAD_CONSUMERS")) consumers = atoi(e) >= 512 ? 512 : 256;
-  p.consumers = consumers;
+  p.consumers = kConsumerThreads;
   // lanes per window G: the vector path needs the window's C 16-byte chunks to split evenly over
   // the lanes; prefer an odd chunks-per-lane count (conflict-free LDS.128) and tiles <= 64 KB
   const int C = fpw / 8;
@@ -666,7 +659,7 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   for (int g = 32; g >= 2 && p.fast; g >>= 1) {
     if (C % g != 0) continue;
     const int cpl = C / g;
-    const long long tile = (long long)(consumers / g) * fpw * 2;
+    const long long tile = (long long)(kConsumerThreads / g) * fpw * 2;
     const int score = ((cpl & 1) ? 4 : 0) + (tile <= 65536 ? 2 : 0) + (cpl >= 3 ? 1 : 0);
     if (score > best_score) { best_score = score; G = g; }
   }
@@ -686,13 +679,12 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   p.fpw = fpw;
   // Ring depth matters more than resident warps (tools/vad_tune.py sweeps stages x CTAs per SM),
   // so the ring is 4 deep when two such CTAs fit an SM.
-  int stages = consumers == 512 ? kMaxStages : 4;
+  int stages = 4;
   if (const char* e = getenv("B2_VAD_STAGES")) stages = std::max(2, std::min(kMaxStages, atoi(e)));  // tuning knob
-  const size_t ring_cap = consumers == 512 ? 216 * 1024 : 200 * 1024;
   for (;;) {
-    p.tw = wpt * (consumers / G);
+    p.tw = wpt * (kConsumerThreads / G);
     p.stage_bytes = ((p.tw * fpw * 2 + 32) + 127) & ~127;
-    if ((size_t)stages * p.stage_bytes <= ring_cap) break;
+    if ((size_t)stages * p.stage_bytes <= 200 * 1024) break;
     if (wpt > 1) --wpt;
     else if (stages > 2) --stages;
     else break;
@@ -771,24 +763,17 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
     B2_CUDA(h, cudaFuncSetAttribute(lk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // tiles are claimed kLaneBatch at a time: no point in more CTAs than claims
     long long grid = std::min<long long>((p.total_tiles + kLanePipes * p.batch - 1) / (kLanePipes * p.batch), (long long)h->sm_count);
+    // b2_sync_batch's pipeline: this many SMs for the VAD, the rest for the correlation kernels
     if (h->vad_partition_sms > 0) grid = std::min<long long>(grid, h->vad_partition_sms);
-    if (const char* e = getenv("B2_VAD_GRID")) grid = std::max<long long>(1, std::min<long long>(grid, atoll(e)));
     lk<<<(unsigned)grid, kLaneConsumers + 32 * kLanePipes, smem, h->stream>>>(p);
     B2_CHECK_LAUNCH(h, "vad_lane_kernel");
     return B2_OK;
   }
-  if (consumers == 512 && smem < 116 * 1024) smem = 116 * 1024;  // never two of these on one SM
-  auto kernel = consumers == 512 ? vad_energy_zcr_kernel<512> : vad_energy_zcr_kernel<256>;
-  B2_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(vad_energy_zcr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (220 * 1024) / smem));
-  // when the correlation kernels of the previous sub-batch run concurrently (b2_sync_batch
-  // pipeline) one VAD CTA per SM leaves room (139 KB smem, 48 K registers) for one of theirs
-  if (h->vad_ctas_per_sm > 0) per_sm = std::min(per_sm, h->vad_ctas_per_sm);
   if (const char* f = getenv("B2_VAD_CTAS_FORCE")) per_sm = std::max(1, atoi(f));  // profiling knob
-  long long grid = std::min<long long>(p.total_tiles, (long long)h->sm_count * per_sm);
-  if (h->vad_partition_sms > 0) grid = std::min<long long>(grid, h->vad_partition_sms);
-  if (const char* e = getenv("B2_VAD_GRID")) grid = std::max<long long>(1, std::min<long long>(grid, atoll(e)));
-  kernel<<<(unsigned)grid, consumers + 32, smem, h->stream>>>(p);
+  const long long grid = std::min<long long>(p.total_tiles, (long long)h->sm_count * per_sm);
+  vad_energy_zcr_kernel<<<(unsigned)grid, kConsumerThreads + 32, smem, h->stream>>>(p);
   B2_CHECK_LAUNCH(h, "vad_energy_zcr_kernel");
   return B2_OK;
 }

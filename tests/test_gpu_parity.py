@@ -74,6 +74,52 @@ def test_vad_full_scale_samples(handle):
     assert np.array_equal(out.astype(np.float64), vo.energy_zcr_detect(pcm, 100, 16000, 0.0, 100000, 0, 160))
 
 
+# (frame_rate, samples per signal): up to 8 two-hour signals, where every CTA of the lane-per-window kernel
+# reuses its ring many times
+_LANE_CASES = {"%d-%dx%d" % (fr, b, nw): (fr, [nw * (fr // 100)] * b) for fr, b, nw in (
+    (16000, 1, 64), (16000, 1, 65), (16000, 1, 640), (16000, 1, 5000), (16000, 3, 20000), (16000, 2, 200000),
+    (16000, 8, 720000), (8000, 2, 100000))}
+# window counts that are no multiple of a tile, partial last windows, an empty signal and a buffer end that is
+# not 16-byte aligned; every signal starts 16-byte aligned, so the lane-per-window kernel still takes the batch
+_LANE_CASES["16000-ragged"] = (16000, [160 * 1000 + 88, 0, 160 * 37 - 72, 160 * 4001, 160 + 8, 160 * 777 - 5])
+
+
+@pytest.mark.parametrize("frame_rate, lengths", list(_LANE_CASES.values()), ids=list(_LANE_CASES))
+def test_vad_lane_kernel_equals_lane_group_kernel(handle, monkeypatch, frame_rate, lengths):
+    """The default VAD (lane-per-window kernel at 8 and 16 kHz) and the lane-group kernel
+    (B2_VAD_LAYOUT=group) give bit-identical windows on the same device PCM, and both equal plain
+    torch arithmetic on that PCM."""
+    import torch
+    from ffsubsync_b200 import _native
+    fpw = frame_rate // 100
+    pcm_off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    n_out = sum(-(-n // fpw) for n in lengths)
+    n_syn = -(-int(pcm_off[-1]) // fpw)
+    cls = torch.from_numpy(np.random.RandomState(n_syn % 9973).randint(0, 3, n_syn).astype(np.uint8)).cuda()
+    pcm = torch.empty(n_syn * fpw, dtype=torch.int16, device="cuda")
+    lane, group = (torch.full((n_out,), -7.0, dtype=torch.float32, device="cuda") for _ in range(2))
+    torch.cuda.synchronize()   # the handle launches on its own stream
+    handle.synth_pcm(cls.data_ptr(), n_syn, fpw, 5, out=pcm.data_ptr(), memspace=_native.B2_DEVICE)
+    handle.vad_energy_zcr(pcm.data_ptr(), pcm_off, frame_rate, 100, 0.5, 100000, out=lane.data_ptr(),
+                          memspace=_native.B2_DEVICE)
+    monkeypatch.setenv("B2_VAD_LAYOUT", "group")
+    handle.vad_energy_zcr(pcm.data_ptr(), pcm_off, frame_rate, 100, 0.5, 100000, out=group.data_ptr(),
+                          memspace=_native.B2_DEVICE)
+    handle.synchronize()
+    assert torch.equal(lane, group)
+    want = []
+    for a, b in zip(pcm_off[:-1].tolist(), pcm_off[1:].tolist()):
+        n_full = (b - a) // fpw
+        x = pcm[a:a + n_full * fpw].view(n_full, fpw)
+        e = x.to(torch.int64).square().sum(1)
+        z = ((x[:, 1:] < 0) != (x[:, :-1] < 0)).sum(1)
+        speech = (e >= fpw * 100000) & (z <= (3 * fpw) // 8)
+        want.append(speech.float() * 0.5 + 0.5)   # 1.0 or the non-speech label 0.5
+        if (b - a) % fpw:
+            want.append(torch.full((1,), 0.5, device="cuda"))   # partial last window: non-speech
+    assert torch.equal(lane, torch.cat(want))
+
+
 def test_device_memspace_is_ordered_on_the_callers_stream(handle):
     """B2_DEVICE calls only enqueue work on the stream given to b2_set_stream; torch ops queued on
     the same stream right after must see the results (no host synchronisation in between).  Covers

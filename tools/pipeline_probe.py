@@ -4,7 +4,6 @@ one resident batch, a sweep over B2_SUBBATCHES x B2_VAD_SMS x B2_VAD_BATCH; ever
 unpipelined results bit for bit.
 
     python tools/pipeline_probe.py [pairs [n_combos]]
-    PIPE_PROBE=schedule python tools/pipeline_probe.py [pairs]   # head share / correlation grid cap instead
 """
 import os
 import sys
@@ -19,7 +18,7 @@ from ffsubsync_b200.batch import BatchSynchronizer  # noqa: E402
 from ffsubsync_b200.synth import BENCH_RATIOS, make_pairs  # noqa: E402
 
 FPW, FR = 160, 16000
-KNOBS = ("B2_SUBBATCHES", "B2_VAD_SMS", "B2_VAD_BATCH", "B2_VAD_LAYOUT", "B2_VAD_EVICT_FIRST", "B2_PIPE_HEAD_PCT", "B2_PIPE_CORR_CAP", "B2_PIPE_CUTS", "B2_PIPE_TRACE")
+KNOBS = ("B2_SUBBATCHES", "B2_VAD_SMS", "B2_VAD_BATCH", "B2_VAD_LAYOUT", "B2_VAD_EVICT_FIRST", "B2_PIPE_TRACE")
 
 
 def main():
@@ -82,39 +81,14 @@ def main():
     combos = []
     for sub, sms in ((2, 80), (3, 80), (4, 80)):
         combos.append({"B2_SUBBATCHES": str(sub), "B2_VAD_SMS": str(sms), "B2_VAD_BATCH": "5", "B2_VAD_EVICT_FIRST": "1"})
-    if os.environ.get("PIPE_PROBE") == "schedule":
-        def cuts(*sizes):
-            acc, out = 0, []
-            for x in sizes[:-1]:
-                acc += int(round(x * B / float(sum(sizes))))
-                out.append(str(acc))
-            return ",".join(out)
-        combos = [dict(B2_SUBBATCHES="3", B2_VAD_SMS="80"),
-                  dict(B2_SUBBATCHES="3", B2_VAD_SMS="80", B2_PIPE_CORR_CAP="1"),
-                  dict(B2_SUBBATCHES="4", B2_VAD_SMS="80"),
-                  dict(B2_SUBBATCHES="6", B2_VAD_SMS="80"),
-                  dict(B2_SUBBATCHES="3", B2_VAD_SMS="80", B2_PIPE_HEAD_PCT="25"),
-                  dict(B2_SUBBATCHES="4", B2_VAD_SMS="80", B2_PIPE_HEAD_PCT="15"),
-                  dict(B2_SUBBATCHES="4", B2_VAD_SMS="80", B2_PIPE_HEAD_PCT="15", B2_PIPE_CORR_CAP="1"),
-                  dict(B2_VAD_SMS="80", B2_PIPE_CUTS=cuts(54, 68, 75, 59)),
-                  dict(B2_VAD_SMS="80", B2_PIPE_CUTS=cuts(40, 81, 81, 54)),
-                  dict(B2_VAD_SMS="80", B2_PIPE_CUTS=cuts(27, 68, 68, 64, 29)),
-                  dict(B2_VAD_SMS="80", B2_PIPE_CUTS=cuts(54, 81, 62, 59), B2_PIPE_CORR_CAP="1"),
-                  dict(B2_VAD_SMS="86", B2_PIPE_CUTS=cuts(50, 75, 75, 56)),
-                  dict(B2_VAD_SMS="74", B2_PIPE_CUTS=cuts(54, 74, 74, 54)),
-                  dict(B2_VAD_SMS="80", B2_PIPE_CUTS=cuts(68, 100, 88))]
-        combos = [dict(c, B2_VAD_BATCH="5", B2_VAD_EVICT_FIRST="1") for c in combos]
     if len(sys.argv) > 2:
         combos = combos[: int(sys.argv[2])]
     for env in combos:
         ms, got = run(env)
-        if os.environ.get("PIPE_PROBE") == "schedule":
-            sys.stdout.flush()
-            run(dict(env, B2_PIPE_TRACE="1"), steps=1)   # device timeline of one call on stderr
         same = all(np.array_equal(ref[k], got[k]) for k in ref)
-        print("evict_first=%s sub=%2s vad_sms=%3s batch=%s head_pct=%s corr_cap=%s cuts=%s: %.3f ms/step (%.0f alignments/s, %.3f x), identical=%s"
-              % (env.get("B2_VAD_EVICT_FIRST", "-"), env.get("B2_SUBBATCHES", "-"), env["B2_VAD_SMS"], env["B2_VAD_BATCH"],
-                 env.get("B2_PIPE_HEAD_PCT", "-"), env.get("B2_PIPE_CORR_CAP", "-"), env.get("B2_PIPE_CUTS", "-"), ms, B / ms * 1e3, ms0 / ms, same),
+        print("evict_first=%s sub=%2s vad_sms=%3s batch=%s: %.3f ms/step (%.0f alignments/s, %.3f x), identical=%s"
+              % (env["B2_VAD_EVICT_FIRST"], env["B2_SUBBATCHES"], env["B2_VAD_SMS"], env["B2_VAD_BATCH"], ms, B / ms * 1e3,
+                 ms0 / ms, same),
               flush=True)
 
 

@@ -3,13 +3,13 @@
 
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
 
-Sizes are tiny (the sanitizer slows kernels 10-100x) but cover: the VAD's TMA/mbarrier ring on the
-vector path, the generic path, ragged tails and the 512-consumer partitioned shape; the auditok
-energy + tokenizer scan; both rasterisers; boundaries; blend; the correlation kernels with tensor
-memory accumulators (float and bit-mask subtitle signals, a multi-block job, the split-block small
-batch path), candidate selection, exact re-score, pick and the ratio reduction; b2_sync_batch with
-and without the sub-batch pipeline.  Results are checked against the oracle so that a run under
-the sanitizer is also a parity run.
+Sizes are tiny (the sanitizer slows kernels 10-100x) but cover: the TMA/mbarrier rings of both VAD
+kernels (lane-group: vector path, generic path, ragged tails; lane-per-window: multi-signal batches,
+one CTA reusing its ring many times); the auditok energy + tokenizer scan; both rasterisers;
+boundaries; blend; the correlation kernels (float and bit-mask subtitle signals, a multi-block job,
+the split-block small batch path), candidate selection, exact re-score, pick and the ratio
+reduction; b2_sync_batch with and without the sub-batch pipeline.  Results are checked against the
+oracle so that a run under the sanitizer is also a parity run.
 """
 import os
 import sys
@@ -31,32 +31,25 @@ from oracle import vad_oracle as vo  # noqa: E402
 def main():
     h = _native.get_handle(0)
     rng = np.random.RandomState(0)
-    # ---- VAD: vector path, generic path (441-sample windows), ragged tail, partitioned shape
+    # ---- VAD: vector path, generic path (441-sample windows), ragged tail
     for fr in (16000, 44100):
         fpw = vo.frames_per_window(fr, 100)
         pcm = vo.synth_pcm(rng.randint(0, 3, 700).astype(np.uint8), fpw, seed=3)[: 700 * fpw - 5]
         got, _ = h.vad_energy_zcr(pcm, [0, len(pcm)], fr, 100, 0.0, 100000)
         assert np.array_equal(got.astype(np.float64), vo.energy_zcr_detect(pcm, 100, fr, 0.0)), fr
     # lane-per-window kernel (16 kHz and 8 kHz, aligned multi-signal batch, ragged last window) against the
-    # lane-group kernel on the same input, then in its SM-partitioned shape (grid capped)
+    # lane-group kernel on the same input
     for fr in (16000, 8000):
         fpw = vo.frames_per_window(fr, 100)
         pcm = vo.synth_pcm(rng.randint(0, 3, 2600).astype(np.uint8), fpw, seed=5)[: 2600 * fpw - 3]
         offs = [0, fpw * 1000, fpw * 1800, len(pcm)]
         want = np.concatenate([vo.energy_zcr_detect(pcm[a:b], 100, fr, 0.0) for a, b in zip(offs[:-1], offs[1:])])
-        for env in ({}, {"B2_VAD_LAYOUT": "group"}, {"B2_VAD_GRID": "3"}, {"B2_VAD_BATCH": "2", "B2_VAD_STAGES": "4"}):
+        for env in ({}, {"B2_VAD_LAYOUT": "group"}, {"B2_VAD_BATCH": "2", "B2_VAD_STAGES": "4"}):
             os.environ.update(env)
             got, _ = h.vad_energy_zcr(pcm, offs, fr, 100, 0.0, 100000)
             for k in env:
                 os.environ.pop(k)
             assert np.array_equal(got.astype(np.float64), want), (fr, env)
-    os.environ.update(B2_VAD_CONSUMERS="512", B2_VAD_CTAS_FORCE="1", B2_VAD_GRID="5")
-    pcm = vo.synth_pcm(rng.randint(0, 3, 3000).astype(np.uint8), 160, seed=4)
-    got, _ = h.vad_energy_zcr(pcm, [0, 160 * 1000, len(pcm)], 16000, 100, 0.0, 100000)
-    assert np.array_equal(got.astype(np.float64), np.concatenate(
-        [vo.energy_zcr_detect(pcm[: 160 * 1000], 100, 16000, 0.0), vo.energy_zcr_detect(pcm[160 * 1000:], 100, 16000, 0.0)]))
-    for k in ("B2_VAD_CONSUMERS", "B2_VAD_CTAS_FORCE", "B2_VAD_GRID"):
-        os.environ.pop(k)
     # ---- auditok: energy + tokenizer
     amp = np.repeat(rng.choice([0.8, 1.2], 60), rng.choice([3, 30, 120], 60))[:2000]
     pcm = np.round(rng.randn(len(amp) * 160) * 316.2 * np.repeat(amp, 160)).astype(np.int16)[:-9]
@@ -91,8 +84,10 @@ def main():
     args = (pcm, [0, n_win * 160, 2 * n_win * 160], np.tile(starts, 2), np.tile(ends, 2), cue_off)
     base = bs.sync_host(*args)
     assert list(base[1]) == [200, 200] and list(base[2]) == [0, 0], base
-    for env in ({"B2_SUBBATCHES": "2"}, {"B2_SUBBATCHES": "2", "B2_VAD_SMS": "2"}):
-        os.environ.update(env)   # sub-batch pipeline: VAD on the internal stream, later sub-batches on B2_VAD_SMS SMs
+    # sub-batch pipeline: VAD on the internal stream; with B2_VAD_SMS=1 the second sub-batch's VAD is one
+    # lane-per-window CTA that reuses its ring for all 938 tiles of its 30 000 windows
+    for env in ({"B2_SUBBATCHES": "2"}, {"B2_SUBBATCHES": "2", "B2_VAD_SMS": "1"}):
+        os.environ.update(env)
         piped = bs.sync_host(*args)
         for k in env:
             os.environ.pop(k)
