@@ -3,6 +3,7 @@
 There is deliberately NO CPU fallback: if the CUDA library is missing or no H100 is visible,
 every compute entry point raises.  Build the library with ``python __graft_entry__.py``.
 """
+import contextlib
 import ctypes
 import os
 import threading
@@ -27,7 +28,7 @@ EXPORTS = [
     "b2_rasterize_lengths", "b2_rasterize", "b2_blend_signals", "b2_first_last_nonzero", "b2_align_batch",
     "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
-    "b2_vad_auditok",
+    "b2_vad_auditok", "b2_capture_nominations",
 ]
 
 
@@ -95,6 +96,7 @@ def load() -> ctypes.CDLL:
         lib.b2_auditok_energy_floor.restype = _i64
         lib.b2_vad_auditok.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _f64, _f64,
                                        _f64, _i64, _f64, _i64, _vp, _vp, ctypes.c_int]
+        lib.b2_capture_nominations.argtypes = [_vp, _vp, _i64, _vp, _vp, _vp]
         _lib = lib
         return lib
 
@@ -376,6 +378,32 @@ class Handle:
                                     memspace)
         self._check(st, "b2_sync_batch")
         return best_score, best_offset, best_k, all_score, all_offset
+
+    # -- diagnostics (tests) --------------------------------------------------------------------
+    @contextlib.contextmanager
+    def capture_nominations(self, n_jobs: int, stride: int):
+        """While the block runs, the aligner calls on this handle copy their nomination stage (fp32
+        window scores, fp32 maximum and tau, candidate count) for jobs 0 .. n_jobs-1 into device
+        arrays (b2_capture_nominations).  Yields a dict that holds numpy arrays once the block has
+        exited: win [n_jobs, 2] int64, stat [n_jobs, 2] float32, cand [n_jobs] int32 and
+        scores [n_jobs, stride] float32 (row j valid up to win[j, 1])."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        t = dict(scores=torch.zeros((n_jobs, stride), dtype=torch.float32, device=dev),
+                 win=torch.zeros((n_jobs, 2), dtype=torch.int64, device=dev),
+                 stat=torch.zeros((n_jobs, 2), dtype=torch.float32, device=dev),
+                 cand=torch.zeros(n_jobs, dtype=torch.int32, device=dev))
+        torch.cuda.synchronize(dev)   # the zero fills run on torch's stream, the captures on the handle's
+        self._check(self.lib.b2_capture_nominations(self.h, t["scores"].data_ptr(), int(stride), t["win"].data_ptr(),
+                                                    t["stat"].data_ptr(), t["cand"].data_ptr()),
+                    "b2_capture_nominations")
+        out = {}
+        try:
+            yield out
+        finally:
+            self._check(self.lib.b2_capture_nominations(self.h, None, 0, None, None, None), "b2_capture_nominations")
+            self.synchronize()
+            out.update({k: v.cpu().numpy() for k, v in t.items()})
 
 
 def _default_device() -> int:

@@ -827,13 +827,27 @@ extern "C" int b2_align_batch(b2_handle h, const float* ref, const int64_t* ref_
     d_status = d_offset + J;
   }
   B2_TRY(b2i_align_launch(h, d_ref, ref_off, d_sub, sub_off, B, K, max_offset_samples, d_score,
-                          d_offset, d_status, /*winner_only=*/0, /*cue_src=*/nullptr));
+                          d_offset, d_status, /*winner_only=*/0, /*cue_src=*/nullptr, /*capture_j0=*/0));
   if (memspace == B2_HOST) {
     B2_TRY(copy_out(h, score, d_score, J * 8));
     B2_TRY(copy_out(h, offset, d_offset, J * 4));
     B2_TRY(copy_out(h, status, d_status, J * 4));
     B2_CUDA(h, cudaStreamSynchronize(h->stream));
   }
+  return B2_OK;
+}
+
+extern "C" int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* win, float* stat,
+                                      int32_t* cand) {
+  B2_ENTER(h);
+  h->capture = B2Capture{};
+  if (!scores) return B2_OK;
+  if (stride <= 0 || !win || !stat || !cand) B2_FAIL(h, B2_ERR_BAD_ARG, "capture: bad arguments");
+  B2_TRY(check_device_ptr(h, scores, "capture: scores"));
+  B2_TRY(check_device_ptr(h, win, "capture: win"));
+  B2_TRY(check_device_ptr(h, stat, "capture: stat"));
+  B2_TRY(check_device_ptr(h, cand, "capture: cand"));
+  h->capture = B2Capture{scores, (long long)stride, (long long*)win, stat, cand};
   return B2_OK;
 }
 
@@ -962,7 +976,7 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
     const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + b0, ratios, sample_rate, start_seconds};
     B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + b0, (const float*)d_subsig,
                             sub_off.data() + j0, nb, K, max_offset_samples, o_score + j0, o_offset + j0,
-                            d_status + j0, winner_only, fused ? &src : nullptr));
+                            d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
     return b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nb, K, max_offset_samples,
                              o_bs + b0, o_bo + b0, o_bk + b0);
   };

@@ -439,7 +439,7 @@ int launch_cols_q(b2_ctx* h, int q1, bool inverse, const float* d_sig, const uin
 int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int B, int K,
                   std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
                   const std::vector<long long>& idx_hi, const std::vector<long long>& n_pad, int winner_only,
-                  const B2CandBuffers& cb, const SelJob** d_sel_out) {
+                  const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0) {
   B2Range range("b2:align_big (four-step FFT per signal)");
   const size_t J = (size_t)B * K;
   // transform size of a pair = the largest padded length among its live ratios (more zero padding
@@ -513,6 +513,9 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
   B2_CUDA(h, cudaMemsetAsync(cb.cand_cnt, 0, J * sizeof(int), h->stream));   // jobs that are not live: no candidates
   big_init_stat_kernel<<<(unsigned)((J + 255) / 256), 256, 0, h->stream>>>(cb.job_stat, (int)J);
   B2_CHECK_LAUNCH(h, "big_init_stat_kernel");
+  // capture: the jobs that join no group (empty input, all masked) now, the others after their group
+  const bool capture = h->capture.scores != nullptr;
+  if (capture) B2_TRY(b2i_capture_launch(h, d_sel, nullptr, (int)J, nullptr, cb, capture_j0));
   if (groups.empty()) return B2_OK;
 
   void *d_g, *d_s;
@@ -568,11 +571,16 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
     }
     const int n_ref = (int)xr.size(), n_sub = (int)xs.size();
     if (n_sub == 0) continue;
+    std::vector<int> jlist;   // capture only: the group's global job indices
+    if (capture)
+      for (const BigJob& jb : jobs) jlist.push_back(jb.j);
     MetaArena ga;
-    B2_TRY(b2i_meta_begin(h, &ga, (xr.size() + xs.size()) * sizeof(BigXform) + jobs.size() * sizeof(BigJob) + 256));
+    B2_TRY(b2i_meta_begin(h, &ga, (xr.size() + xs.size()) * sizeof(BigXform) + jobs.size() * sizeof(BigJob) +
+                                      jlist.size() * sizeof(int) + 256));
     const BigXform* d_xr = (const BigXform*)b2i_meta_put(&ga, xr.data(), xr.size() * sizeof(BigXform));
     const BigXform* d_xs = (const BigXform*)b2i_meta_put(&ga, xs.data(), xs.size() * sizeof(BigXform));
     const BigJob* d_jobs = (const BigJob*)b2i_meta_put(&ga, jobs.data(), jobs.size() * sizeof(BigJob));
+    const int* d_jlist = capture ? (const int*)b2i_meta_put(&ga, jlist.data(), jlist.size() * sizeof(int)) : nullptr;
     B2_TRY(b2i_meta_commit(&ga));
     float* ref_energy = tile_arr;
     float* sub_energy = ref_energy + (size_t)n_ref * tiles_per;
@@ -599,6 +607,8 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
                                                     chunk_cnt, cb.cand_off, cb.cand_cnt, cb.work_list,
                                                     cb.work_count);
     B2_CHECK_LAUNCH(h, "big_select_kernel");
+    // before the next group overwrites the score workspace
+    if (capture) B2_TRY(b2i_capture_launch(h, d_sel, d_jlist, n_sub, scores, cb, capture_j0));
   }
   return B2_OK;
 }

@@ -31,6 +31,15 @@ struct HostBuf {  // pinned
   size_t cap = 0;
 };
 
+// b2_capture_nominations: caller-owned device arrays the aligner copies its nomination stage into
+struct B2Capture {
+  float* scores = nullptr;  // nullptr: capture off
+  long long stride = 0;
+  long long* win = nullptr;
+  float* stat = nullptr;
+  int* cand = nullptr;
+};
+
 struct b2_ctx {
   int device = 0;
   int sm_count = 132;
@@ -40,6 +49,7 @@ struct b2_ctx {
   int64_t launches = 0;
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
   int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
+  B2Capture capture;             // set by b2_capture_nominations (tests)
   // B2_DEVICE_RESIDENT chaining of b2_sync_batch calls (api.cu): `resident_fence` is recorded on the caller's
   // stream before the LAST sub-batch's correlation chain of a pipelined call, `resident_done` after it; the
   // next resident call (if no other entry point ran in between: `resident_fence_valid`) starts its VAD behind
@@ -185,10 +195,13 @@ struct B2CueSource {
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);
+// capture_j0: global index of job 0 of this call in the arrays of b2_capture_nominations (b2_sync_batch's
+// sub-batches align a range of pairs at a time)
 int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host,
                      const float* d_sub, const int64_t* sub_off_host, int B, int K,
                      int64_t max_offset_samples, double* d_score, int32_t* d_offset,
-                     int32_t* d_status, int winner_only, const B2CueSource* cue_src);
+                     int32_t* d_status, int winner_only, const B2CueSource* cue_src,
+                     long long capture_j0);
 int b2i_reduce_launch(b2_ctx* h, const double* d_score, const int32_t* d_offset,
                       const int32_t* d_status, int B, int K, int64_t max_offset_samples,
                       double* d_best_score, int32_t* d_best_offset, int32_t* d_best_k);

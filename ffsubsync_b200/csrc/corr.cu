@@ -476,6 +476,35 @@ __global__ void __launch_bounds__(128) pick_kernel(const SelJob* __restrict__ jo
   status[job.out_index] = cnt > kCandMax ? B2_ALIGN_CAND_OVERFLOW : B2_ALIGN_OK;
 }
 
+// ---- diagnostics: b2_capture_nominations ----------------------------------------------------------
+// One CTA per job: the fp32 scores of its surviving window (m_lo..m_hi, offset o_first + m), its
+// (maximum, tau) and its candidate count, as the selection kernels left them.
+__global__ void __launch_bounds__(256) capture_nominations_kernel(const SelJob* __restrict__ jobs,
+                                                                   const int* __restrict__ jlist,
+                                                                   const float* __restrict__ scores,
+                                                                   const float2* __restrict__ job_stat,
+                                                                   const int* __restrict__ cand_cnt,
+                                                                   B2Capture cap, long long j0) {
+  const int j = jlist ? jlist[blockIdx.x] : (int)blockIdx.x;
+  const SelJob job = jobs[j];
+  const bool live = job.kind == 0 && job.m_lo <= job.m_hi;
+  if (live && !scores) return;  // written by the launch that has its scores
+  const long long g = j0 + j;
+  const int n = live ? job.m_hi - job.m_lo + 1 : 0;
+  if (threadIdx.x == 0) {
+    const float2 s = job_stat[j];
+    cap.win[2 * g] = live ? (long long)job.o_first + job.m_lo : 0;
+    cap.win[2 * g + 1] = n;
+    cap.stat[2 * g] = s.x;
+    cap.stat[2 * g + 1] = s.y;
+    cap.cand[g] = cand_cnt[j];
+  }
+  if (n == 0) return;
+  const float* c = scores + job.score_off + job.m_lo;
+  float* out = cap.scores + g * cap.stride;
+  for (int i = threadIdx.x; i < n; i += 256) out[i] = c[i];
+}
+
 // ---- host planning ----------------------------------------------------------------------------
 long long padded_length(const b2_ctx* h, long long n) {
   // int(2 ** math.ceil(math.log(n, 2))), aligners.py:67-68, libm quirks included
@@ -493,10 +522,19 @@ long long floor_div(long long a, long long b) {
 
 }  // namespace
 
+int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
+                       const B2CandBuffers& cb, long long j0) {
+  if (n <= 0) return B2_OK;
+  capture_nominations_kernel<<<(unsigned)n, 256, 0, h->stream>>>(d_sel, d_jlist, scores, cb.job_stat, cb.cand_cnt,
+                                                                  h->capture, j0);
+  B2_CHECK_LAUNCH(h, "capture_nominations_kernel");
+  return B2_OK;
+}
+
 int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, const float* d_sub,
                      const int64_t* sub_off, int B, int K, int64_t max_offset_samples,
                      double* d_score, int32_t* d_offset, int32_t* d_status, int winner_only,
-                     const B2CueSource* cue_src) {
+                     const B2CueSource* cue_src, long long capture_j0) {
   B2Range range("b2:align (ref_spectra, sub_correlate, select, rescore, pick)");
   const size_t J = (size_t)B * K;
   // cue mode (b2_sync_batch): the subtitle signals exist only as bit masks, rasterised from the cue
@@ -576,6 +614,12 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
         for (int k = 0; k < K; ++k) sel[(size_t)b * K + k].no_prune = 1;
     }
   }
+  const bool capture = h->capture.scores != nullptr;
+  if (capture)
+    for (size_t j = 0; j < J; ++j)
+      if (sel[j].kind == 0 && (long long)sel[j].m_hi - sel[j].m_lo + 1 > h->capture.stride)
+        B2_FAIL(h, B2_ERR_BAD_ARG, "capture: job %lld has %lld surviving offsets, stride %lld",
+                capture_j0 + (long long)j, (long long)sel[j].m_hi - sel[j].m_lo + 1, h->capture.stride);
   // offsets per tile: Wt = 1 (mod 32) so that L = P - Wt + 1 is a multiple of 32 (vector loads,
   // whole words of the speech bit mask per block), at most P/2 + 1
   const int Wt = (int)(max_w <= kP / 2 + 1 ? 32 * ((max_w + 30) / 32) + 1 : (kP / 2 + 1));
@@ -611,7 +655,8 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
   }
   if (use_big) {
     const SelJob* d_sel_big = nullptr;
-    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, B, K, sel, idx_lo, idx_hi, n_pad, winner_only, cb, &d_sel_big));
+    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, B, K, sel, idx_lo, idx_hi, n_pad, winner_only, cb, &d_sel_big,
+                         capture_j0));
     return b2i_rescore_pick(h, d_sel_big, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
   }
 
@@ -769,6 +814,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
                                                                 cb.cand_off, cb.cand_cnt, cb.work_list,
                                                                 cb.work_count);
   B2_CHECK_LAUNCH(h, "select_candidates_kernel");
+  if (capture) B2_TRY(b2i_capture_launch(h, d_sel, nullptr, (int)J, scores, cb, capture_j0));
   return b2i_rescore_pick(h, d_sel, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
 }
 

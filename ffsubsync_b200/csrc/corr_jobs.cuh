@@ -62,10 +62,15 @@ struct B2CandBuffers {
 int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_ref, const float* d_sub,
                      const uint32_t* d_bits, const B2CandBuffers& cb, double* d_score, int32_t* d_offset,
                      int32_t* d_status);
+// b2_capture_nominations (corr.cu): copies the window scores, job_stat and cand_cnt of n jobs into
+// h->capture at global index j0 + j, after the selection kernels.  Jobs d_jlist[0..n) (NULL: 0..n-1);
+// with scores == NULL only the jobs without a live window are written.
+int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
+                       const B2CandBuffers& cb, long long j0);
 // Large-window path (bigfft.cu).  sel: host copy of the jobs (kind / R / S / offsets filled in by the
 // planner; this call sets o_first, m_lo, m_hi, score_off), surviving index range per job in idx_lo /
 // idx_hi (half open, in the reference's conv[] index space), padded lengths n_pad per pair.
 int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int B, int K,
                   std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
                   const std::vector<long long>& idx_hi, const std::vector<long long>& n_pad, int winner_only,
-                  const B2CandBuffers& cb, const SelJob** d_sel_out);
+                  const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0);

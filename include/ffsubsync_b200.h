@@ -194,6 +194,22 @@ int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B
                   double* all_score /* [B*K] or NULL */, int32_t* all_offset /* or NULL */,
                   int memspace);
 
+/* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
+ * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
+ * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
+ * the exact float64 re-score.  While set, every aligner stage on this handle (b2_align_batch,
+ * b2_sync_batch) also writes, for each (pair, ratio) j = b*K + k of the call, into caller-owned DEVICE
+ * arrays (on the handle's stream):
+ *   win[2j], win[2j+1]    first surviving offset, number of surviving offsets (0: empty / all masked)
+ *   stat[2j], stat[2j+1]  fp32 maximum over the window, round-off bound tau
+ *   cand[j]               offsets with fp32 score >= max - tau (uncapped count); -1 = B2_ALIGN_APPROX
+ *   scores[j*stride + i]  fp32 score of offset win[2j] + i, 0 <= i < win[2j+1]
+ * The arrays must hold B*K entries (x2 for win and stat).  A window longer than stride fails the call
+ * with B2_ERR_BAD_ARG.  scores == NULL clears the capture.  Not for production use: each capture costs
+ * one extra launch per alignment (per group of the large-window path). */
+int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* win, float* stat,
+                           int32_t* cand);
+
 /* ---- synthetic PCM (bench / tests): counter-hash generator replayable in numpy -------------
  * oracle/vad_oracle.py:synth_pcm.  window_class: uint8 per 10 ms window (0 silence, 1 voiced,
  * 2 loud hiss), device or host per memspace; writes n_windows*fpw int16 samples. */

@@ -109,6 +109,35 @@ def multi_segment_case(true_scale: float, true_shift: float, sr: int = 100):
     return ref_full, sub
 
 
+# Signal families that stress the round-off bound tau of the nomination stage: large means (the
+# ||c||_2 term of tau dominates), flat or periodic correlation landscapes, exact ties, wide dynamic range.
+SIGNAL_FAMILIES = ["random", "ones", "zeros", "period2", "period_block", "sparse", "wide", "ramp"]
+
+
+def signal_family(name, n, rng, level=1.0):
+    """float32 signal of family ``name`` and length ``n``; two-level families take the value ``level``."""
+    if name == "random":
+        return (rng.rand(n) > rng.uniform(0.2, 0.8)).astype(np.float32) * np.float32(level)
+    if name == "ones":
+        return np.full(n, level, np.float32)
+    if name == "zeros":
+        return np.zeros(n, np.float32)
+    if name == "period2":
+        return (np.arange(n) % 2).astype(np.float32) * np.float32(level)
+    if name == "period_block":   # period = the block length of the +-60 s window (L = 20 736)
+        return ((np.arange(n) // 10368) % 2).astype(np.float32) * np.float32(level)
+    if name == "sparse":         # multi-segment reference: a few 60 s windows of speech, zero elsewhere
+        x = np.zeros(n, np.float32)
+        for s in rng.randint(0, max(1, n - 6000), 6):
+            x[s:s + 6000] = (rng.rand(len(x[s:s + 6000])) > 0.5) * np.float32(level)
+        return x
+    if name == "wide":           # float levels spanning 1e-3 ... 1e3
+        return (10.0 ** rng.uniform(-3, 3, n) * rng.choice([0.0, 1.0], n)).astype(np.float32)
+    if name == "ramp":
+        return np.linspace(0.0, level, n).astype(np.float32)
+    raise ValueError(name)
+
+
 def synthetic_cues(seed: int, duration_s: float):
     rng = np.random.RandomState(seed)
     t = 5.0

@@ -1177,23 +1177,7 @@ def test_ffmpeg_and_ffprobe_subprocess_branches(handle, tmp_path, monkeypatch):
 
 # ================================================= adversarial signal families (round-off bound, ties)
 
-def _adv_family(name, n, rng, level=1.0):
-    if name == "random":
-        return (rng.rand(n) > rng.uniform(0.2, 0.8)).astype(np.float32) * np.float32(level)
-    if name == "ones":
-        return np.full(n, level, np.float32)
-    if name == "period2":
-        return (np.arange(n) % 2).astype(np.float32) * np.float32(level)
-    if name == "period_block":
-        return ((np.arange(n) // 10368) % 2).astype(np.float32) * np.float32(level)
-    if name == "sparse":
-        x = np.zeros(n, np.float32)
-        for s in rng.randint(0, max(1, n - 6000), 6):
-            x[s:s + 6000] = (rng.rand(len(x[s:s + 6000])) > 0.5) * np.float32(level)
-        return x
-    if name == "wide":
-        return (10.0 ** rng.uniform(-3, 3, n) * rng.choice([0.0, 1.0], n)).astype(np.float32)
-    raise ValueError(name)
+_adv_family = cases.signal_family
 
 
 @pytest.mark.parametrize("mos", [6000, None])

@@ -78,6 +78,11 @@ def test_no_cpu_fallback_without_gpu(built):
         FFTAligner().fit([1, 0, 1], [1, 0])
     with pytest.raises(_native.NativeError):
         _make_energy_zcr_detector(100, 16000, 0.0)
+    with pytest.raises(_native.NativeError):
+        with _native.get_handle().capture_nominations(1, 16):
+            pass
+    # the entry point itself refuses a handle-less call instead of recording anything
+    assert _native.load().b2_capture_nominations(None, None, 0, None, None, None) == -1
     src = open(os.path.join(ROOT, "ffsubsync_b200", "aligners.py")).read() + \
         open(os.path.join(ROOT, "ffsubsync_b200", "speech_transformers.py")).read() + \
         open(os.path.join(ROOT, "ffsubsync_b200", "_native.py")).read()
@@ -230,30 +235,8 @@ def test_kernel_chain_emulation(built, R, S, o_t, W, mode):
 # |fp32 score - exact score| of the kernel chain (run thread by thread on the CPU) against the
 # worst-case bound tau the candidate selection uses, on adversarial signal families.
 
-def _family(name, n, rng, level=1.0):
-    if name == "random":
-        return (rng.rand(n) > rng.uniform(0.2, 0.8)).astype(np.float32) * np.float32(level)
-    if name == "ones":
-        return np.full(n, level, np.float32)
-    if name == "zeros":
-        return np.zeros(n, np.float32)
-    if name == "period2":
-        return (np.arange(n) % 2).astype(np.float32) * np.float32(level)
-    if name == "period_block":   # period = the block length of the +-60 s window (L = 20 736)
-        return ((np.arange(n) // 10368) % 2).astype(np.float32) * np.float32(level)
-    if name == "sparse":         # multi-segment reference: a few 60 s windows of speech, zero elsewhere
-        x = np.zeros(n, np.float32)
-        for s in rng.randint(0, max(1, n - 6000), 6):
-            x[s:s + 6000] = (rng.rand(len(x[s:s + 6000])) > 0.5) * np.float32(level)
-        return x
-    if name == "wide":           # float levels spanning 1e-3 ... 1e3
-        return (10.0 ** rng.uniform(-3, 3, n) * rng.choice([0.0, 1.0], n)).astype(np.float32)
-    if name == "ramp":
-        return np.linspace(0.0, level, n).astype(np.float32)
-    raise ValueError(name)
-
-
-_FAMILIES = ["random", "ones", "zeros", "period2", "period_block", "sparse", "wide", "ramp"]
+_family = cases.signal_family
+_FAMILIES = cases.SIGNAL_FAMILIES
 
 
 def _roundoff_case(fam_r, fam_s, R, S, o_t, W, seed, mode=0):
