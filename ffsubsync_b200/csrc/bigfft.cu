@@ -6,9 +6,9 @@
 // four-step complex FFT of M = N/2 = M1 x 1024 points (bigfft.cuh): columns (F1), rows + untangle
 // [+ product + inverse rows] (F2), inverse columns (F3).  The reference spectrum of a pair is computed
 // once and reused by its K ratio candidates.  The N fp32 scores only nominate candidates (same
-// worst-case round-off bound tau, same exact float64 re-score and argmax as the windowed path);
-// selection over the N-sized score arrays is parallel: per-tile maxima from F3, a counting pass over
-// 32 768-offset chunks and an ordered compaction of the chunks that hold candidates.
+// worst-case round-off bound tau, same selection, exact float64 re-score and argmax as the windowed
+// path); the maximum over the N-sized score arrays comes from per-tile maxima of F3, and the selection
+// (corr.cu) counts hits per 4 096-offset chunk and compacts only the chunks that hold candidates.
 //
 // HBM traffic per (pair, ratio) at N = 2^21: F1 3 + 8 MB, F2 16 + 8 MB, F3 8 + 8 MB, selection 8 MB
 // (+ 27 MB / K for the reference) against ~105 MFLOP per transform: memory and FP32 work are balanced,
@@ -45,7 +45,6 @@ struct BigJob {          // one (pair, ratio) of the group
   int x_sub, x_ref;      // transform indices inside the group
 };
 
-constexpr int kChunk = 4096;    // offsets per counting CTA
 constexpr int kFineCap = (1 << kMaxQ1) + (1 << (kMaxQ1 - 4)) + (1 << (kMaxQ1 - 8)) + 4;   // skewed size
 constexpr size_t kBigSmemBytes = kSmemBytes + 1024 * 8 + (size_t)kSkew1024 * 8 + (size_t)kFineCap * 8 + 16 * 8 + 64;
 
@@ -214,7 +213,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
 }
 
-// ---- selection over N-sized score arrays -----------------------------------------------------------
+// ---- window maximum over N-sized score arrays ------------------------------------------------------
 // per job: fp32 maximum over the surviving window and the round-off bound tau (corr_jobs.cuh)
 __global__ void __launch_bounds__(256) big_stat_kernel(const BigJob* __restrict__ jobs, int tiles_per,
                                                         const float* __restrict__ ref_energy,
@@ -246,8 +245,8 @@ __global__ void __launch_bounds__(256) big_stat_kernel(const BigJob* __restrict_
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    const float tau = kU * (kTauFwd * sqrtf(s_es[0] * s_er[0]) + kTauInv * sqrtf(s_cn[0]));
-    job_stat[jb.j] = make_float2(s_mx[0], tau * 1.0001f + 1e-30f);
+    const float tau = tau_bound(kTauFwd, sqrtf(s_es[0] * s_er[0]), kTauInv, sqrtf(s_cn[0]));
+    job_stat[jb.j] = make_float2(s_mx[0], nomination_tau(tau));
   }
 }
 
@@ -256,150 +255,6 @@ __global__ void __launch_bounds__(256) big_stat_kernel(const BigJob* __restrict_
 __global__ void big_init_stat_kernel(float2* __restrict__ job_stat, int n) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j < n) job_stat[j] = make_float2(-INFINITY, 0.f);
-}
-
-// The cut of a job: fp32 maximum minus tau; with winner_only a ratio that by the bound tau cannot be the
-// pair's best keeps only its fp32 argmax (same rule as select_candidates_kernel in corr.cu).
-__device__ __forceinline__ float job_cut(const float2* __restrict__ job_stat, int j, int K, int winner_only,
-                                         bool& approx_only) {
-  const float2 stat = job_stat[j];
-  float cut = stat.x - stat.y;
-  approx_only = false;
-  if (winner_only) {   // callers pass winner_only = 0 for a job with no_prune set
-    const int b0 = (j / K) * K;
-    float best_floor = -INFINITY;
-    for (int k = 0; k < K; ++k) {
-      const float2 s = job_stat[b0 + k];
-      best_floor = fmaxf(best_floor, s.x - s.y);
-    }
-    if (stat.x + stat.y < best_floor) {
-      approx_only = true;
-      cut = stat.x;
-    }
-  }
-  return cut;
-}
-
-__global__ void __launch_bounds__(256) big_count_kernel(const SelJob* __restrict__ sel,
-                                                         const BigJob* __restrict__ jobs,
-                                                         const float* __restrict__ scores,
-                                                         const float2* __restrict__ job_stat, int K,
-                                                         int winner_only, int n_chunks,
-                                                         int* __restrict__ chunk_cnt) {
-  const BigJob jb = jobs[blockIdx.y];
-  const SelJob job = sel[jb.j];
-  __shared__ int s_cnt[8];
-  int cnt = 0;
-  if (job.kind == 0 && job.m_lo <= job.m_hi) {
-    bool approx;
-    const float cut = job_cut(job_stat, jb.j, K, winner_only && !job.no_prune, approx);
-    const float* c = scores + job.score_off;
-    const int lo = max(job.m_lo, (int)blockIdx.x * kChunk), hi = min(job.m_hi, (int)(blockIdx.x + 1) * kChunk - 1);
-    for (int m = lo + threadIdx.x; m <= hi; m += 256) cnt += c[m] >= cut;
-  }
-  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-  if ((threadIdx.x & 31) == 0) s_cnt[threadIdx.x >> 5] = cnt;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int tot = 0;
-    for (int w = 0; w < 8; ++w) tot += s_cnt[w];
-    chunk_cnt[(size_t)blockIdx.y * n_chunks + blockIdx.x] = tot;
-  }
-}
-
-// Ordered compaction: candidates from the LARGEST offset down (np.argmax keeps the lowest index =
-// largest offset among equal values), at most kCandMax; only chunks that hold candidates are walked.
-__global__ void __launch_bounds__(256) big_select_kernel(const SelJob* __restrict__ sel,
-                                                          const BigJob* __restrict__ jobs,
-                                                          const float* __restrict__ scores,
-                                                          const float2* __restrict__ job_stat, int K,
-                                                          int winner_only, int n_chunks,
-                                                          const int* __restrict__ chunk_cnt,
-                                                          int* __restrict__ cand_off, int* __restrict__ cand_cnt,
-                                                          int* __restrict__ work_list,
-                                                          int* __restrict__ work_count) {
-  const BigJob jb = jobs[blockIdx.x];
-  const SelJob job = sel[jb.j];
-  const int tid = threadIdx.x;
-  __shared__ int scount;
-  __shared__ int swarp[8];
-  if (job.kind != 0 || job.m_lo > job.m_hi) {
-    if (tid == 0) cand_cnt[jb.j] = 0;
-    return;
-  }
-  bool approx_only;
-  const float cut = job_cut(job_stat, jb.j, K, winner_only && !job.no_prune, approx_only);
-  const float* c = scores + job.score_off;
-  // 1. the (at most kCandMax) highest chunks that hold candidates, in descending order, and the total
-  __shared__ int hit_chunk[kCandMax];
-  __shared__ int n_hit, s_total;
-  if (tid == 0) {
-    scount = 0;
-    n_hit = 0;
-    s_total = 0;
-  }
-  __syncthreads();
-  const int* cnt = chunk_cnt + (size_t)blockIdx.x * n_chunks;
-  for (int top = n_chunks - 1; top >= 0; top -= 256) {
-    const int ch = top - tid;
-    const int here = ch >= 0 ? cnt[ch] : 0;
-    const unsigned ball = __ballot_sync(0xffffffffu, here > 0);
-    int wsum = here;
-    for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-    if ((tid & 31) == 0) {
-      swarp[tid >> 5] = __popc(ball);
-      atomicAdd(&s_total, wsum);
-    }
-    __syncthreads();
-    int before = n_hit;
-    for (int w = 0; w < (tid >> 5); ++w) before += swarp[w];
-    before += __popc(ball & ((1u << (tid & 31)) - 1u));
-    if (here > 0 && before < kCandMax) hit_chunk[before] = ch;
-    __syncthreads();
-    if (tid == 0) {
-      int tot = 0;
-      for (int w = 0; w < 8; ++w) tot += swarp[w];
-      n_hit += tot;
-    }
-    __syncthreads();
-  }
-  const int total = s_total;
-  const int n_walk = min(n_hit, kCandMax);
-  // 2. ordered compaction inside those chunks
-  for (int h = 0; h < n_walk; ++h) {
-    if (scount >= kCandMax) break;   // uniform: scount is read after a barrier
-    const int ch = hit_chunk[h];
-    const int lo = max(job.m_lo, ch * kChunk), hi = min(job.m_hi, (ch + 1) * kChunk - 1);
-    for (int top = hi; top >= lo; top -= 256) {
-      const int m = top - tid;
-      const bool hit = (m >= lo) && (c[m] >= cut);
-      const unsigned ball = __ballot_sync(0xffffffffu, hit);
-      if ((tid & 31) == 0) swarp[tid >> 5] = __popc(ball);
-      __syncthreads();
-      int before = scount;
-      for (int w = 0; w < (tid >> 5); ++w) before += swarp[w];
-      before += __popc(ball & ((1u << (tid & 31)) - 1u));
-      if (hit && before < kCandMax) cand_off[(size_t)jb.j * kCandMax + before] = job.o_first + m;
-      __syncthreads();
-      if (tid == 0) {
-        int tot = 0;
-        for (int w = 0; w < 8; ++w) tot += swarp[w];
-        scount += tot;
-      }
-      __syncthreads();
-    }
-  }
-  if (approx_only) {  // slot 0 holds the largest offset attaining the fp32 maximum
-    if (tid == 0) cand_cnt[jb.j] = -1;
-    return;
-  }
-  if (tid == 0) {
-    cand_cnt[jb.j] = total;
-    scount = min(total, kCandMax);
-    swarp[0] = atomicAdd(work_count, scount);
-  }
-  __syncthreads();
-  if (tid < scount) work_list[swarp[0] + tid] = (jb.j << 5) | tid;
 }
 
 template <int Q1>
@@ -571,16 +426,15 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
     }
     const int n_ref = (int)xr.size(), n_sub = (int)xs.size();
     if (n_sub == 0) continue;
-    std::vector<int> jlist;   // capture only: the group's global job indices
-    if (capture)
-      for (const BigJob& jb : jobs) jlist.push_back(jb.j);
+    std::vector<int> jlist;   // the group's global job indices (selection, capture)
+    for (const BigJob& jb : jobs) jlist.push_back(jb.j);
     MetaArena ga;
     B2_TRY(b2i_meta_begin(h, &ga, (xr.size() + xs.size()) * sizeof(BigXform) + jobs.size() * sizeof(BigJob) +
                                       jlist.size() * sizeof(int) + 256));
     const BigXform* d_xr = (const BigXform*)b2i_meta_put(&ga, xr.data(), xr.size() * sizeof(BigXform));
     const BigXform* d_xs = (const BigXform*)b2i_meta_put(&ga, xs.data(), xs.size() * sizeof(BigXform));
     const BigJob* d_jobs = (const BigJob*)b2i_meta_put(&ga, jobs.data(), jobs.size() * sizeof(BigJob));
-    const int* d_jlist = capture ? (const int*)b2i_meta_put(&ga, jlist.data(), jlist.size() * sizeof(int)) : nullptr;
+    const int* d_jlist = (const int*)b2i_meta_put(&ga, jlist.data(), jlist.size() * sizeof(int));
     B2_TRY(b2i_meta_commit(&ga));
     float* ref_energy = tile_arr;
     float* sub_energy = ref_energy + (size_t)n_ref * tiles_per;
@@ -600,14 +454,8 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
     big_stat_kernel<<<n_sub, 256, 0, h->stream>>>(d_jobs, tiles_per, ref_energy, sub_energy, tile_max, tile_cn,
                                                   cb.job_stat);
     B2_CHECK_LAUNCH(h, "big_stat_kernel");
-    big_count_kernel<<<dim3(n_chunks, n_sub), 256, 0, h->stream>>>(d_sel, d_jobs, scores, cb.job_stat, K,
-                                                                   winner_only, n_chunks, chunk_cnt);
-    B2_CHECK_LAUNCH(h, "big_count_kernel");
-    big_select_kernel<<<n_sub, 256, 0, h->stream>>>(d_sel, d_jobs, scores, cb.job_stat, K, winner_only, n_chunks,
-                                                    chunk_cnt, cb.cand_off, cb.cand_cnt, cb.work_list,
-                                                    cb.work_count);
-    B2_CHECK_LAUNCH(h, "big_select_kernel");
     // before the next group overwrites the score workspace
+    B2_TRY(b2i_select_launch(h, d_sel, d_jlist, n_sub, scores, n_chunks, K, winner_only, chunk_cnt, cb));
     if (capture) B2_TRY(b2i_capture_launch(h, d_sel, d_jlist, n_sub, scores, cb, capture_j0));
   }
   return B2_OK;

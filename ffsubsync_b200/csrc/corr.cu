@@ -230,11 +230,8 @@ __global__ void __launch_bounds__(kThreads, 1)
   sub_correlate_body<true>(nullptr, jobs, spec, spec_energy, L, scores, job_energy, sub_bits);
 }
 
-// ---- candidate selection ---------------------------------------------------------------------
-// Per (pair, ratio): approximate maximum over the surviving window, then every offset whose
-// fp32 score is within tau of it, taken from the LARGEST offset down (np.argmax returns the
-// lowest index = largest offset among equal values), at most kCandMax of them.
-// Phase 1: fp32 maximum of the surviving window and the round-off bound tau, per (pair, ratio).
+// ---- window maximum ----------------------------------------------------------------------------
+// fp32 maximum of the surviving window and the round-off bound tau, per (pair, ratio).
 __global__ void __launch_bounds__(256) window_max_kernel(const SelJob* __restrict__ jobs,
                                                           float* __restrict__ scores,
                                                           const float4* __restrict__ job_energy,
@@ -279,76 +276,165 @@ __global__ void __launch_bounds__(256) window_max_kernel(const SelJob* __restric
         blocks = fmaxf(blocks, e.w);
       }
       const float fwd = kTauFwd + fmaxf(0.f, blocks - (float)kTauBlocks);
-      tau = fmaxf(tau, kU * (fwd * sqrtf(ex * ey) + (kTauInv + (float)(job.n_split - 1)) * cn));
+      tau = fmaxf(tau, tau_bound(fwd, sqrtf(ex * ey), kTauInv + (float)(job.n_split - 1), cn));
     }
-    job_stat[blockIdx.x] = make_float2(smax[0], tau * 1.0001f + 1e-30f);
+    job_stat[blockIdx.x] = make_float2(smax[0], nomination_tau(tau));
   }
 }
 
-// Phase 2.  With winner_only (b2_sync_batch when only the best ratio is wanted) a (pair, ratio)
-// whose fp32 maximum cannot reach the best ratio's even after round-off (mx + tau < max_k (mx_k -
-// tau_k)) is not re-scored: it reports its fp32 maximum and is flagged B2_ALIGN_APPROX.
-__global__ void __launch_bounds__(256) select_candidates_kernel(
-    const SelJob* __restrict__ jobs, const float* __restrict__ scores,
-    const float2* __restrict__ job_stat, int K, int winner_only, int* __restrict__ cand_off,
-    int* __restrict__ cand_cnt, int* __restrict__ work_list, int* __restrict__ work_count) {
-  const SelJob job = jobs[blockIdx.x];
-  const int tid = threadIdx.x;
-  __shared__ int scount;
-  __shared__ int swarp[8];
-  if (job.kind != 0 || job.m_lo > job.m_hi) {
-    if (tid == 0) cand_cnt[blockIdx.x] = 0;
-    return;
-  }
-  const float* c = scores + job.score_off;
-  const float2 stat = job_stat[blockIdx.x];
-  float cut = stat.x - stat.y;
-  bool approx_only = false;
+// ---- candidate selection (both paths) --------------------------------------------------------------
+// Per (pair, ratio): every offset whose fp32 score is within tau of the fp32 maximum (job_stat), taken
+// from the LARGEST offset down (np.argmax returns the lowest index = largest offset among equal values;
+// offset o = o_first + m, so that is the largest m), at most kCandMax of them.  nominate_count_kernel
+// counts the hits per kChunk-offset chunk of m, nominate_select_kernel walks only the chunks that hold
+// hits.  Job i of a launch is jlist[i] (NULL: i).
+
+// The cut of a job: fp32 maximum minus tau.  With winner_only (b2_sync_batch when only the best ratio
+// is wanted) a (pair, ratio) whose fp32 maximum cannot reach the best ratio's even after round-off
+// (mx + tau < max_k (mx_k - tau_k)) is not re-scored: it keeps only its fp32 argmax (cut = mx) and is
+// flagged B2_ALIGN_APPROX.  Off for a pair with no_prune set.
+__device__ __forceinline__ float nomination_cut(const SelJob& job, const float2* __restrict__ job_stat, int j,
+                                                int K, int winner_only, bool& approx_only) {
+  const float2 stat = job_stat[j];
+  approx_only = false;
   if (winner_only && !job.no_prune) {
-    const int b0 = (blockIdx.x / K) * K;
+    const int b0 = (j / K) * K;
     float best_floor = -INFINITY;
     for (int k = 0; k < K; ++k) {
       const float2 s = job_stat[b0 + k];
       best_floor = fmaxf(best_floor, s.x - s.y);
     }
-    if (stat.x + stat.y < best_floor) {  // cannot win: keep only the fp32 argmax (largest offset)
+    if (stat.x + stat.y < best_floor) {
       approx_only = true;
-      cut = stat.x;
+      return stat.x;
     }
   }
-  if (tid == 0) scount = 0;
-  __syncthreads();
-  // walk m from high to low so that slots fill in order of increasing index m_hi - m ... wait:
-  // offset o = o_first + m, so the largest offset is the largest m.
-  for (int top = job.m_hi; top >= job.m_lo; top -= 256) {
-    const int m = top - tid;
-    const bool hit = (m >= job.m_lo) && (c[m] >= cut);
-    const unsigned ball = __ballot_sync(0xffffffffu, hit);
-    if ((tid & 31) == 0) swarp[tid >> 5] = __popc(ball);
+  return stat.x - stat.y;
+}
+
+// Grid: jobs on x, chunks on y (a grid-stride loop: a window may have more than 65 535 chunks).
+__global__ void __launch_bounds__(256) nominate_count_kernel(const SelJob* __restrict__ sel,
+                                                              const int* __restrict__ jlist,
+                                                              const float* __restrict__ scores,
+                                                              const float2* __restrict__ job_stat, int K,
+                                                              int winner_only, int n_chunks,
+                                                              int* __restrict__ chunk_cnt) {
+  const int j = jlist ? jlist[blockIdx.x] : (int)blockIdx.x;
+  const SelJob job = sel[j];
+  if (job.kind != 0 || job.m_lo > job.m_hi) return;  // nominate_select_kernel reads no count
+  __shared__ int s_cnt[8];
+  bool approx;
+  const float cut = nomination_cut(job, job_stat, j, K, winner_only, approx);
+  const float* c = scores + job.score_off;
+  for (int ch = blockIdx.y; ch < n_chunks; ch += gridDim.y) {
+    const int lo = max(job.m_lo, ch * kChunk), hi = min(job.m_hi, ch * kChunk + (kChunk - 1));
+    int cnt = 0;
+    for (int m = lo + threadIdx.x; m <= hi; m += 256) cnt += c[m] >= cut;
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0) s_cnt[threadIdx.x >> 5] = cnt;
     __syncthreads();
-    int before = scount;
+    if (threadIdx.x == 0) {
+      int tot = 0;
+      for (int w = 0; w < 8; ++w) tot += s_cnt[w];
+      chunk_cnt[(size_t)blockIdx.x * n_chunks + ch] = tot;
+    }
+    __syncthreads();  // s_cnt is rewritten by the next chunk
+  }
+}
+
+// Ordered compaction, one CTA per job; publishes the job's candidates to the re-score work list.
+__global__ void __launch_bounds__(256) nominate_select_kernel(const SelJob* __restrict__ sel,
+                                                               const int* __restrict__ jlist,
+                                                               const float* __restrict__ scores,
+                                                               const float2* __restrict__ job_stat, int K,
+                                                               int winner_only, int n_chunks,
+                                                               const int* __restrict__ chunk_cnt,
+                                                               int* __restrict__ cand_off,
+                                                               int* __restrict__ cand_cnt,
+                                                               int* __restrict__ work_list,
+                                                               int* __restrict__ work_count) {
+  const int j = jlist ? jlist[blockIdx.x] : (int)blockIdx.x;
+  const SelJob job = sel[j];
+  const int tid = threadIdx.x;
+  __shared__ int scount;
+  __shared__ int swarp[8];
+  if (job.kind != 0 || job.m_lo > job.m_hi) {
+    if (tid == 0) cand_cnt[j] = 0;
+    return;
+  }
+  bool approx_only;
+  const float cut = nomination_cut(job, job_stat, j, K, winner_only, approx_only);
+  const float* c = scores + job.score_off;
+  // 1. the (at most kCandMax) highest chunks that hold candidates, in descending order, and the total
+  __shared__ int hit_chunk[kCandMax];
+  __shared__ int n_hit, s_total;
+  if (tid == 0) {
+    scount = 0;
+    n_hit = 0;
+    s_total = 0;
+  }
+  __syncthreads();
+  const int* cnt = chunk_cnt + (size_t)blockIdx.x * n_chunks;
+  for (int top = n_chunks - 1; top >= 0; top -= 256) {
+    const int ch = top - tid;
+    const int here = ch >= 0 ? cnt[ch] : 0;
+    const unsigned ball = __ballot_sync(0xffffffffu, here > 0);
+    int wsum = here;
+    for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
+    if ((tid & 31) == 0) {
+      swarp[tid >> 5] = __popc(ball);
+      atomicAdd(&s_total, wsum);
+    }
+    __syncthreads();
+    int before = n_hit;
     for (int w = 0; w < (tid >> 5); ++w) before += swarp[w];
     before += __popc(ball & ((1u << (tid & 31)) - 1u));
-    if (hit && before < kCandMax) cand_off[(size_t)blockIdx.x * kCandMax + before] = job.o_first + m;
+    if (here > 0 && before < kCandMax) hit_chunk[before] = ch;
     __syncthreads();
     if (tid == 0) {
       int tot = 0;
       for (int w = 0; w < 8; ++w) tot += swarp[w];
-      scount += tot;
+      n_hit += tot;
     }
     __syncthreads();
   }
+  const int total = s_total;
+  const int n_walk = min(n_hit, kCandMax);
+  // 2. ordered compaction inside those chunks
+  for (int h = 0; h < n_walk; ++h) {
+    if (scount >= kCandMax) break;  // uniform: scount is read after a barrier
+    const int ch = hit_chunk[h];
+    const int lo = max(job.m_lo, ch * kChunk), hi = min(job.m_hi, ch * kChunk + (kChunk - 1));
+    for (int top = hi; top >= lo; top -= 256) {
+      const int m = top - tid;
+      const bool hit = (m >= lo) && (c[m] >= cut);
+      const unsigned ball = __ballot_sync(0xffffffffu, hit);
+      if ((tid & 31) == 0) swarp[tid >> 5] = __popc(ball);
+      __syncthreads();
+      int before = scount;
+      for (int w = 0; w < (tid >> 5); ++w) before += swarp[w];
+      before += __popc(ball & ((1u << (tid & 31)) - 1u));
+      if (hit && before < kCandMax) cand_off[(size_t)j * kCandMax + before] = job.o_first + m;
+      __syncthreads();
+      if (tid == 0) {
+        int tot = 0;
+        for (int w = 0; w < 8; ++w) tot += swarp[w];
+        scount += tot;
+      }
+      __syncthreads();
+    }
+  }
   if (approx_only) {  // slot 0 holds the largest offset attaining the fp32 maximum
-    if (tid == 0) cand_cnt[blockIdx.x] = -1;
+    if (tid == 0) cand_cnt[j] = -1;
     return;
   }
   if (tid == 0) {
-    cand_cnt[blockIdx.x] = scount;
-    scount = min(scount, kCandMax);
+    cand_cnt[j] = total;
+    scount = min(total, kCandMax);
     swarp[0] = atomicAdd(work_count, scount);  // slots in the global re-score work list
   }
   __syncthreads();
-  if (tid < scount) work_list[swarp[0] + tid] = ((int)blockIdx.x << 5) | tid;
+  if (tid < scount) work_list[swarp[0] + tid] = (j << 5) | tid;
 }
 
 // ---- exact re-score ----------------------------------------------------------------------------
@@ -522,6 +608,20 @@ long long floor_div(long long a, long long b) {
 
 }  // namespace
 
+int b2i_select_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
+                      int n_chunks, int K, int winner_only, int* chunk_cnt, const B2CandBuffers& cb) {
+  if (n <= 0) return B2_OK;
+  const dim3 grid((unsigned)n, (unsigned)std::min(n_chunks, 65535));
+  nominate_count_kernel<<<grid, 256, 0, h->stream>>>(d_sel, d_jlist, scores, cb.job_stat, K, winner_only,
+                                                     n_chunks, chunk_cnt);
+  B2_CHECK_LAUNCH(h, "nominate_count_kernel");
+  nominate_select_kernel<<<(unsigned)n, 256, 0, h->stream>>>(d_sel, d_jlist, scores, cb.job_stat, K, winner_only,
+                                                             n_chunks, chunk_cnt, cb.cand_off, cb.cand_cnt,
+                                                             cb.work_list, cb.work_count);
+  B2_CHECK_LAUNCH(h, "nominate_select_kernel");
+  return B2_OK;
+}
+
 int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
                        const B2CandBuffers& cb, long long j0) {
   if (n <= 0) return B2_OK;
@@ -682,12 +782,13 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
     n_split = (int)std::max<long long>(1, std::min<long long>(ceil_div64(2LL * h->sm_count, n_jobs_total),
                                                                max_blocks / 4));
   if (const char* e = getenv("B2_ALIGN_SPLIT")) n_split = std::max(1, atoi(e));  // test / tuning knob
-  long long score_total = 0, energy_total = 0;
+  long long score_total = 0, energy_total = 0, max_score_len = 0;
   for (int b = 0; b < B; ++b) {
     PairPlan& p = pp[b];
     for (int k = 0; k < K; ++k) {
       SelJob& s = sel[(size_t)b * K + k];
       if (s.kind != 0) continue;
+      max_score_len = std::max(max_score_len, (long long)p.n_tiles * Wt);
       s.o_first = (int)p.o_min;
       s.m_lo -= (int)p.o_min;
       s.m_hi -= (int)p.o_min;
@@ -700,11 +801,13 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
     }
   }
 
+  const int n_chunks = (int)std::max<long long>(1, ceil_div64(max_score_len, kChunk));
   void* d_scores;
-  B2_TRY(b2i_ws(h, b2_ctx::WS_SCORES, (size_t)(score_total + 16) * 4 + (size_t)(energy_total + 2) * 16,
-                &d_scores));
+  B2_TRY(b2i_ws(h, b2_ctx::WS_SCORES,
+                (size_t)(score_total + 16) * 4 + (size_t)(energy_total + 2) * 16 + J * n_chunks * 4, &d_scores));
   float* scores = (float*)d_scores;
   float4* job_energy = (float4*)((char*)d_scores + (((size_t)(score_total + 16) * 4 + 15) & ~size_t(15)));
+  int* chunk_cnt = (int*)(job_energy + energy_total);
 
   B2_CUDA(h, cudaFuncSetAttribute(ref_spectra_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)kSmemBytes));
@@ -810,10 +913,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
   B2_CUDA(h, cudaMemsetAsync(cb.work_count, 0, sizeof(int), h->stream));
   window_max_kernel<<<(unsigned)J, 256, 0, h->stream>>>(d_sel, scores, job_energy, cb.job_stat, Wt);
   B2_CHECK_LAUNCH(h, "window_max_kernel");
-  select_candidates_kernel<<<(unsigned)J, 256, 0, h->stream>>>(d_sel, scores, cb.job_stat, K, winner_only,
-                                                                cb.cand_off, cb.cand_cnt, cb.work_list,
-                                                                cb.work_count);
-  B2_CHECK_LAUNCH(h, "select_candidates_kernel");
+  B2_TRY(b2i_select_launch(h, d_sel, nullptr, (int)J, scores, n_chunks, K, winner_only, chunk_cnt, cb));
   if (capture) B2_TRY(b2i_capture_launch(h, d_sel, nullptr, (int)J, scores, cb, capture_j0));
   return b2i_rescore_pick(h, d_sel, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
 }

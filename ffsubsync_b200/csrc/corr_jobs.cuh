@@ -1,5 +1,6 @@
 // Types and constants shared by the two correlation paths (corr.cu: overlap-save windows;
-// bigfft.cu: one large FFT per signal) and their common tail (exact re-score, pick).
+// bigfft.cu: one large FFT per signal) and their common tail (candidate selection, exact re-score,
+// pick).
 #pragma once
 #include <stdint.h>
 
@@ -27,6 +28,19 @@ constexpr float kTauFwd = 512.0f;
 constexpr float kTauInv = 192.0f;
 constexpr int kTauBlocks = 64;  // block count covered by kTauFwd
 
+// The bound above for one score array: fwd = kTauFwd (plus one per block beyond kTauBlocks),
+// sqrt_e = sqrt(Es*Er), inv = kTauInv + n_split - 1, cn = ||c||_2.
+__device__ __forceinline__ float tau_bound(float fwd, float sqrt_e, float inv, float cn) {
+  return kU * (fwd * sqrt_e + inv * cn);
+}
+// The tau a job nominates with (job_stat.y): the largest tau_bound of its score arrays, padded so that
+// the bound's own fp32 evaluation cannot cut off a candidate, and kept above 0.
+__device__ __forceinline__ float nomination_tau(float tau) { return tau * 1.0001f + 1e-30f; }
+
+// Offsets per chunk of the candidate selection: counting splits a window into chunks of m, the ordered
+// compaction walks only the chunks that hold candidates.
+constexpr int kChunk = 4096;
+
 struct SelJob {        // one (pair, ratio)
   long long ref_off, sub_off, score_off;
   int R, S, o_first;   // offset of scores[score_off]
@@ -49,8 +63,9 @@ constexpr int kBigMinTiles = 4;
 int bigfft_min_log2n();
 int bigfft_max_log2n();
 
-// Common tail (corr.cu): exact float64 re-score of the nominated candidates and the argmax.
-// cand_off / cand_cnt / work_list / work_count / job_stat as filled by either path's selection.
+// Common tail (corr.cu): candidate selection, exact float64 re-score of the nominated candidates and
+// the argmax.  job_stat is filled by either path (window_max_kernel, big_stat_kernel); cand_off /
+// cand_cnt / work_list / work_count by the selection.
 struct B2CandBuffers {
   double* cand_partial;
   float2* job_stat;
@@ -59,6 +74,12 @@ struct B2CandBuffers {
   int* work_list;
   int* work_count;
 };
+// Candidates of n jobs: every offset whose fp32 score is within tau of the job's fp32 maximum, largest
+// offset first, at most kCandMax, appended to the re-score work list.  Jobs d_jlist[0..n) (NULL:
+// 0..n-1); a job's score array covers m < n_chunks * kChunk; chunk_cnt holds n * n_chunks ints.
+// winner_only: a ratio that cannot be its pair's best keeps only its fp32 argmax (B2_ALIGN_APPROX).
+int b2i_select_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
+                      int n_chunks, int K, int winner_only, int* chunk_cnt, const B2CandBuffers& cb);
 int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_ref, const float* d_sub,
                      const uint32_t* d_bits, const B2CandBuffers& cb, double* d_score, int32_t* d_offset,
                      int32_t* d_status);

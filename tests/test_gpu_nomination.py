@@ -306,22 +306,26 @@ def _plateau_ref(R, centre, width):
     return ref
 
 
-@pytest.mark.parametrize("path", ["tiled", "large-window"])
+@pytest.mark.parametrize("path", ["tiled", "tiled-chunk", "large-window"])
 def test_selection_plateaus_of_32_and_33(handle, path):
-    """Plateaus of exactly 32 (fits the re-score budget) and 33 (B2_ALIGN_CAND_OVERFLOW) tied candidates,
-    straddling a 256-offset step of select_candidates_kernel (tiled) or the boundary m = 32 768 of the
-    large-window path's 4 096-offset counting chunks."""
+    """Plateaus of exactly 32 (fits the re-score budget) and 33 (B2_ALIGN_CAND_OVERFLOW) tied candidates
+    across the boundaries of the selection's walk: on the tiled path a 256-offset step of the ordered
+    compaction ("tiled") and the boundary m = 4 096 of the 4 096-offset counting chunks ("tiled-chunk"),
+    on the large-window path the chunk boundary m = 32 768."""
     sub = np.ones(1, np.float32)
-    if path == "tiled":
+    if path.startswith("tiled"):
         mos, R = 6000, 70000
-        o_hi = ao.offset_range(R, 1, mos)[1]
-        centre = o_hi - 256 * 10 + 1         # offsets o_hi - 256 k and o_hi - 256 k + 1 are in different steps
+        o_lo, o_hi = ao.offset_range(R, 1, mos)
+        if path == "tiled":
+            centre = o_hi - 256 * 10 + 1     # offsets o_hi - 256 k and o_hi - 256 k + 1 are in different steps
+        else:
+            centre = o_lo + 4096             # m = offset - o_lo (the window's first offset is m = 0)
     else:
         mos, R = None, 70000
         centre = 32768 - 1 + 1               # m = offset + 1: the chunk boundary m = 32 768 is offset 32 767
     pairs = [(_plateau_ref(R, centre, w), [sub]) for w in (32, 33)]
     cap, out, sigs = _align(handle, pairs, 1, mos)
-    _check_jobs(cap, sigs, mos, _Exact(), (path, "float"), out=out)
+    _check_jobs(cap, sigs, mos, _Exact(), ("tiled" if path.startswith("tiled") else path, "float"), out=out)
     assert list(cap["cand"]) == [32, 33]
     assert [int(s) & 4 for s in out[2]] == [0, 4]
     for b, w in enumerate((32, 33)):

@@ -235,6 +235,27 @@ def test_more_than_65535_signals_in_one_call(handle):
         assert _score_ok(bs[b], results[wk][0])
 
 
+def test_align_batch_more_than_65535_tiled_jobs(handle):
+    """b2_align_batch on the overlap-save path with 17 000 pairs x 4 ratios = 68 000 (pair, ratio) jobs:
+    every per-job launch indexes jobs with grid.x (grid.y stops at 65 535).  Random binary signals of a
+    few hundred frames, so the float64 correlation rounds to the exact integer scores; every job against
+    the oracle's argmax (ties -> largest offset)."""
+    rs = np.random.RandomState(65536)
+    B, K, mos = 17000, 4, 150
+    refs = [(rs.rand(rs.randint(300, 400)) > 0.5).astype(np.float32) for _ in range(B)]
+    subs = [(rs.rand(rs.randint(200, 300)) > 0.5).astype(np.float32) for _ in range(B * K)]
+    ref_off = np.concatenate([[0], np.cumsum([len(r) for r in refs])])
+    sub_off = np.concatenate([[0], np.cumsum([len(s) for s in subs])])
+    score, off, st = handle.align_batch(np.concatenate(refs), ref_off, np.concatenate(subs), sub_off, B, K, mos)
+    assert len(off) == B * K and np.all(st == 0)
+    for j, sub in enumerate(subs):
+        conv = np.round(ao.correlation(refs[j // K], sub))
+        N, S = len(conv), len(sub)
+        lo, hi = ao.surviving_index_range(N, S, mos)
+        idx = lo + int(np.argmax(conv[lo:hi]))
+        assert (off[j], score[j]) == (N - 1 - idx - S, conv[idx]), j
+
+
 def test_vad_stream_matches_per_chunk_detection(handle):
     """b2_vad_stream_*: every pushed chunk is detected like one detector call (ceil(n/fpw) windows,
     partial last window non-speech, odd trailing byte dropped); the ring (3 slots) wraps, chunk
