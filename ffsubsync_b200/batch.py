@@ -80,6 +80,43 @@ class BatchSynchronizer:
         assert K == len(self.ratios)
         return out
 
+    def sync_device_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, out=None,
+                           all_out=None, inputs_resident: bool = False):
+        """sync_device for several subtitle tracks per video (``ffs movie.mkv -i en.srt de.srt ...``):
+        pcm holds the V videos back to back, pcm_off: [V+1] sample offsets (host); track t (cue list
+        cue_off[t] .. cue_off[t+1]) is synced against video track_video[t] (host, non-decreasing).  Each
+        video's PCM is read and run through the VAD once, however many tracks it has.  out: optional dict
+        of CUDA tensors best_score f64[T], best_offset i32[T], best_k i32[T]; all_out: optional
+        {"score": f64[T*K], "offset": i32[T*K]}.  Returns out; nothing is synchronised.  inputs_resident
+        as for sync_device (resident calls of both methods chain with each other)."""
+        import torch
+        T = len(track_video)
+        dev = pcm.device
+        if out is None:
+            out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
+                   "best_offset": torch.empty(T, dtype=torch.int32, device=dev),
+                   "best_k": torch.empty(T, dtype=torch.int32, device=dev)}
+        a_s = all_out["score"].data_ptr() if all_out else None
+        a_o = all_out["offset"].data_ptr() if all_out else None
+        self.handle.sync_tracks(
+            pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
+            self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
+            self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
+            out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o,
+            memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+        return out
+
+    def sync_host_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None,
+                         want_all=False):
+        """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
+        results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
+        track."""
+        res = self.handle.sync_tracks(
+            pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
+            self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
+            self.start_seconds, self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
+        return res if want_all else res[:3]
+
     def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None):
         """Same as sync_device but starting from reference speech SIGNALS (100 Hz float32, all pairs
         back to back; numpy array or CUDA tensor) instead of PCM - the replay path of the

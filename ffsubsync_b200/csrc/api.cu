@@ -826,8 +826,8 @@ extern "C" int b2_align_batch(b2_handle h, const float* ref, const int64_t* ref_
     d_offset = (int32_t*)(d_score + J);
     d_status = d_offset + J;
   }
-  B2_TRY(b2i_align_launch(h, d_ref, ref_off, d_sub, sub_off, B, K, max_offset_samples, d_score,
-                          d_offset, d_status, /*winner_only=*/0, /*cue_src=*/nullptr, /*capture_j0=*/0));
+  B2_TRY(b2i_align_launch(h, d_ref, ref_off, B, /*trk_off=*/nullptr, d_sub, sub_off, B, K, max_offset_samples,
+                          d_score, d_offset, d_status, /*winner_only=*/0, /*cue_src=*/nullptr, /*capture_j0=*/0));
   if (memspace == B2_HOST) {
     B2_TRY(copy_out(h, score, d_score, J * 8));
     B2_TRY(copy_out(h, offset, d_offset, J * 4));
@@ -895,41 +895,59 @@ extern "C" int b2_reduce_ratios(b2_handle h, const double* score, const int32_t*
 
 // ---- whole hot path --------------------------------------------------------------------------
 // VideoSpeechTransformer.fit (VAD) -> K x (SubtitleScaler + SubtitleSpeechTransformer) ->
-// MaxScoreAligner(FFTAligner).fit_transform, for B pairs (ffsubsync/ffsubsync.py:637,196-235).
-extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
-                             int frame_rate, int sample_rate, float non_speech_label,
-                             int64_t energy_threshold, int z_lo, int z_hi,
-                             const double* cue_start_s, const double* cue_end_s,
-                             const uint8_t* cue_keep, const int64_t* cue_off, const double* ratios,
-                             int K, double start_seconds, int64_t max_offset_samples,
-                             double* best_score, int32_t* best_offset, int32_t* best_k,
-                             double* all_score, int32_t* all_offset, int memspace) {
-  B2_ENTER(h);
-  B2Range range("b2_sync_batch");
+// MaxScoreAligner(FFTAligner).fit_transform (ffsubsync/ffsubsync.py:637,196-235), for V videos and T
+// subtitle tracks: track t is synced against video track_video[t] (non-decreasing; NULL: V == T, track t
+// against video t - b2_sync_batch).  Each video's PCM goes through the VAD once; its reference spectra
+// serve the K ratio jobs t*K + k of every one of its tracks.
+static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm, const int64_t* pcm_off, int V,
+                            const int32_t* track_video, int T, int frame_rate, int sample_rate,
+                            float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                            const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                            const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                            int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                            int32_t* best_k, double* all_score, int32_t* all_offset, int memspace) {
   const bool resident = memspace == B2_DEVICE_RESIDENT;
   if (resident) memspace = B2_DEVICE;
-  if (B < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
-    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_batch: bad arguments");
-  if (B == 0) return B2_OK;
-  if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_batch: null output");
+  const char* who = track_video ? "sync_tracks" : "sync_batch";
+  if (V < 0 || T < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad arguments", who);
+  if (track_video) {
+    for (int t = 0; t < T; ++t)
+      if (track_video[t] < 0 || track_video[t] >= V || (t > 0 && track_video[t] < track_video[t - 1]))
+        B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: track_video[%d] = %d is out of [0, %d) or decreases", t,
+                (int)track_video[t], V);
+    for (int t = 0; t < T; ++t)
+      if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: cue_off not monotone at %d", t);
+  }
+  if (T == 0) return B2_OK;
+  if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null output", who);
   const int fpw = b2_vad_frames_per_window(frame_rate, sample_rate);
-  if (fpw <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_batch: bad frame_rate/sample_rate");
+  if (fpw <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
   if (z_lo < 0) z_lo = 0;
   if (z_hi < 0) z_hi = (3 * fpw) / 8;
-  const size_t J = (size_t)B * K;
-  std::vector<int64_t> ref_off(B + 1), sub_off(J + 1), lengths(J);
-  ref_off[0] = 0;
-  for (int b = 0; b < B; ++b) {
-    const int64_t n = pcm_off[b + 1] - pcm_off[b];
-    if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_batch: pcm_off not monotone");
-    ref_off[b + 1] = ref_off[b] + (n + fpw - 1) / fpw;
+  // trk_off[v]: first track of video v
+  std::vector<int> trk_off(V + 1);
+  for (int v = 0, t = 0; v <= V; ++v) {
+    if (track_video)
+      while (t < T && track_video[t] < v) ++t;
+    else
+      t = v;
+    trk_off[v] = t;
   }
-  if (b2_rasterize_lengths(cue_end_s, cue_off, B, ratios, K, 0, sample_rate, lengths.data()) != B2_OK)
-    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_batch: bad cue list / ratios");
+  const size_t J = (size_t)T * K;
+  std::vector<int64_t> ref_off(V + 1), sub_off(J + 1), lengths(J);
+  ref_off[0] = 0;
+  for (int v = 0; v < V; ++v) {
+    const int64_t n = pcm_off[v + 1] - pcm_off[v];
+    if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
+    ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
+  }
+  if (b2_rasterize_lengths(cue_end_s, cue_off, T, ratios, K, 0, sample_rate, lengths.data()) != B2_OK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad cue list / ratios", who);
   sub_off[0] = 0;
   for (size_t j = 0; j < J; ++j) sub_off[j + 1] = sub_off[j] + lengths[j];
 
-  // Default: the K subtitle signals of a pair are never materialised as floats - the cue list is
+  // Default: the K subtitle signals of a track are never materialised as floats - the cue list is
   // rasterised into bit masks (1 bit per frame) that the correlation kernel and the exact re-score
   // read.  B2_FUSED_RASTER=0 (A/B and test knob): raster_cues_kernel writes float signals to HBM and
   // the generic aligner (the b2_align_batch path) reads them back.
@@ -938,24 +956,30 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
 
   void *d_refsig, *d_subsig = nullptr, *d_res;
   // a chained resident call (see below) writes the buffer the previous call is not reading any more
-  const bool chained_candidate = resident && _b2_fence_was_valid;
+  const bool chained_candidate = resident && fence_was_valid;
   const int refsig_slot = chained_candidate && h->refsig_parity == 0 ? b2_ctx::WS_SIG_REF2 : b2_ctx::WS_SIG_REF;
-  B2_TRY(b2i_ws(h, refsig_slot, (size_t)ref_off[B] * 4 + 64, &d_refsig));
+  B2_TRY(b2i_ws(h, refsig_slot, (size_t)ref_off[V] * 4 + 64, &d_refsig));
   if (!fused) B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_SUB, (size_t)sub_off[J] * 4 + 64, &d_subsig));
-  B2_TRY(b2i_ws(h, b2_ctx::WS_MISC, J * 16 + (size_t)B * 16 + 256, &d_res));
+  B2_TRY(b2i_ws(h, b2_ctx::WS_MISC, J * 16 + (size_t)T * 16 + 256, &d_res));
   double* d_score = (double*)d_res;
   double* d_bs = d_score + J;
-  int32_t* d_offset = (int32_t*)(d_bs + B);
+  int32_t* d_offset = (int32_t*)(d_bs + T);
   int32_t* d_status = d_offset + J;
   int32_t* d_bo = d_status + J;
-  int32_t* d_bk = d_bo + B;
+  int32_t* d_bk = d_bo + T;
 
-  B2_CHECK_DEV(h, memspace, pcm, "sync_batch: pcm");
-  B2_CHECK_DEV(h, memspace, best_score, "sync_batch: best_score");
+  B2_CHECK_DEV(h, memspace, pcm, track_video ? "sync_tracks: pcm" : "sync_batch: pcm");
+  B2_CHECK_DEV(h, memspace, best_score, track_video ? "sync_tracks: best_score" : "sync_batch: best_score");
+  if (track_video) {   // b2_sync_batch has always checked the two above only
+    B2_CHECK_DEV(h, memspace, best_offset, "sync_tracks: best_offset");
+    B2_CHECK_DEV(h, memspace, best_k, "sync_tracks: best_k");
+    B2_CHECK_DEV(h, memspace, all_score, "sync_tracks: all_score");
+    B2_CHECK_DEV(h, memspace, all_offset, "sync_tracks: all_offset");
+  }
   const int16_t* d_pcm = pcm;
   if (memspace == B2_HOST) {
     void* dp;
-    B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, pcm, (size_t)pcm_off[B] * 2, &dp));
+    B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, pcm, (size_t)pcm_off[V] * 2, &dp));
     d_pcm = (const int16_t*)dp;
   }
   double* o_score = (memspace == B2_DEVICE && all_score) ? all_score : d_score;
@@ -963,55 +987,71 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
   double* o_bs = memspace == B2_DEVICE ? best_score : d_bs;
   int32_t* o_bo = memspace == B2_DEVICE ? best_offset : d_bo;
   int32_t* o_bk = memspace == B2_DEVICE ? best_k : d_bk;
-  // only the best ratio of each pair is reported unless the per-ratio arrays are requested:
+  // only the best ratio of each track is reported unless the per-ratio arrays are requested:
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   const int winner_only = (!all_score && !all_offset) ? 1 : 0;
-  // rasterise (float signals only if !fused) -> align -> reduce the pairs [b0, b1) on the caller's stream
-  auto enqueue_chain = [&](int b0, int b1) -> int {
-    const int nb = b1 - b0;
-    const size_t j0 = (size_t)b0 * K;
+  // rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
+  // caller's stream
+  std::vector<int> chain_trk;
+  auto enqueue_chain = [&](int v0, int v1) -> int {
+    const int t0 = trk_off[v0], nt = trk_off[v1] - t0;
+    const size_t j0 = (size_t)t0 * K;
+    chain_trk.resize(v1 - v0 + 1);
+    for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = trk_off[v] - t0;
     if (!fused)
-      B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + b0, nb, ratios, K, 0, nullptr,
+      B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + t0, nt, ratios, K, 0, nullptr,
                                sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
-    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + b0, ratios, sample_rate, start_seconds};
-    B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + b0, (const float*)d_subsig,
-                            sub_off.data() + j0, nb, K, max_offset_samples, o_score + j0, o_offset + j0,
-                            d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
-    return b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nb, K, max_offset_samples,
-                             o_bs + b0, o_bo + b0, o_bk + b0);
+    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds};
+    B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
+                            (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
+                            o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
+    return b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nt, K, max_offset_samples,
+                             o_bs + t0, o_bo + t0, o_bk + t0);
   };
 
-  // Software pipeline over sub-batches of pairs.  The VAD (HBM-bound) of every sub-batch is queued on the
+  // Software pipeline over sub-batches of videos.  The VAD (HBM-bound) of every sub-batch is queued on the
   // internal high-priority stream: sub-batch 0 on the whole GPU, the later ones on `vad_sms` SMs only (one
-  // lane-per-window CTA per SM, csrc/vad.cu); the rasterisation / correlation / reduction of sub-batch i
-  // (FP32- and shared-memory bound) follows on the caller's stream as soon as its VAD is done and runs on
-  // the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler keeps the
-  // two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); the
+  // lane-per-window CTA per SM, csrc/vad.cu); the rasterisation / correlation / reduction of the tracks of
+  // sub-batch i (FP32- and shared-memory bound) follows on the caller's stream as soon as its VAD is done and
+  // runs on the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler keeps
+  // the two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); the
   // lane-group kernel needs every SM's issue slots to reach the HBM roofline, so partitioning never paid
   // with it.  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
-  // Defaults: 3 sub-batches of equal size, the later VADs on 54 % of the SMs (71 of an H100's 132;
+  // Defaults: 3 sub-batches, the later VADs on 54 % of the SMs (71 of an H100's 132;
   // tools/pipeline_probe.py sweeps both); small batches stay unpipelined (the alignment of a third of a small
   // batch is launch- and tail-bound).
+  // Sub-batches are cut at video boundaries (a video's tracks run in the chain behind its own VAD) and
+  // balanced by track count, since the chain's work scales with tracks: cut i is the first video whose
+  // tracks start at or after track T*i/n_sub.  With one track per video these are T*i/n_sub exactly.
+  // Cuts that would leave a sub-batch without tracks are dropped; a video without tracks has its VAD run in
+  // the sub-batch of the next video that has tracks (trailing ones: of the last).  Where the cuts fall
+  // changes no result.
   int n_sub = 1, vad_sms = 0;
-  if (B >= 96 && b2i_vad_lane_eligible(pcm_off, B, fpw)) {
+  if (T >= 96 && b2i_vad_lane_eligible(pcm_off, V, fpw)) {
     n_sub = 3;
     vad_sms = (h->sm_count * 54 + 50) / 100;
   }
-  if (const char* e = getenv("B2_SUBBATCHES")) n_sub = std::max(1, std::min(B, atoi(e)));
+  if (const char* e = getenv("B2_SUBBATCHES")) n_sub = std::max(1, std::min(T, atoi(e)));
   if (const char* e = getenv("B2_VAD_SMS")) vad_sms = std::max(0, std::min(h->sm_count, atoi(e)));
+  n_sub = std::min(n_sub, b2_ctx::kEvents - 2);
+  std::vector<int> cut(1, 0);   // video cuts; every sub-batch holds at least one track
+  for (int i = 1; i < n_sub; ++i) {
+    const int target = (int)((int64_t)T * i / n_sub);
+    const int v = (int)(std::lower_bound(trk_off.begin(), trk_off.end(), target) - trk_off.begin());
+    if (trk_off[v] > trk_off[cut.back()] && trk_off[v] < T) cut.push_back(v);
+  }
+  cut.push_back(V);
+  n_sub = (int)cut.size() - 1;
   if (n_sub == 1) {
-    B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off, B, fpw, non_speech_label, (int64_t)fpw * energy_threshold, z_lo,
+    B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off, V, fpw, non_speech_label, (int64_t)fpw * energy_threshold, z_lo,
                           z_hi, (float*)d_refsig, ref_off.data()));
-    B2_TRY(enqueue_chain(0, B));
+    B2_TRY(enqueue_chain(0, V));
   } else {
-    if (n_sub > b2_ctx::kEvents - 2) n_sub = b2_ctx::kEvents - 2;
-    std::vector<int> cut(n_sub + 1);   // n_sub <= B: no sub-batch is empty
-    for (int i = 0; i <= n_sub; ++i) cut[i] = (int)((int64_t)B * i / n_sub);
     std::vector<cudaEvent_t> vad_done(n_sub);
     cudaEvent_t inputs_ready = next_event(h);
     B2_CUDA(h, cudaEventRecord(inputs_ready, h->stream));
     // B2_PIPE_TRACE=1 (diagnostic; synchronises): device timeline of the sub-batches and host enqueue times
-    const bool trace = getenv("B2_PIPE_TRACE") != nullptr;
+  const bool trace = getenv("B2_PIPE_TRACE") != nullptr;
     std::vector<cudaEvent_t> tev;   // t0, then per sub-batch: VAD start, VAD end, chain start, chain end
     std::vector<double> host_ms(n_sub + 1, 0.0);
     const auto host_t0 = std::chrono::steady_clock::now();
@@ -1021,9 +1061,10 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
       for (auto& e : tev) B2_CUDA(h, cudaEventCreate(&e));
       B2_CUDA(h, cudaEventRecord(tev[0], h->stream));
     }
-    // B2_DEVICE_RESIDENT, previous entry point on this handle = a pipelined resident b2_sync_batch: the VAD
-    // starts behind that call's fence (everything on the caller's stream up to, not including, its last
-    // correlation chain) and overlaps that chain like a further sub-batch - on vad_sms SMs if it is still running.
+    // B2_DEVICE_RESIDENT, previous entry point on this handle = a pipelined resident b2_sync_batch or
+    // b2_sync_tracks: the VAD starts behind that call's fence (everything on the caller's stream up to, not
+    // including, its last correlation chain) and overlaps that chain like a further sub-batch - on vad_sms
+    // SMs if it is still running.
     // It writes the other reference-signal buffer (the chain still reads the previous one); the chains of the
     // call before that, which read this buffer, precede the fence.
     const bool chained = chained_candidate;
@@ -1036,12 +1077,12 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
       Stream2Scope on2(h);
       B2_CUDA(h, cudaStreamWaitEvent(h->stream, chained ? h->resident_fence : inputs_ready, 0));
       for (int i = 0; i < n_sub; ++i) {
-        const int b0 = cut[i], b1 = cut[i + 1];
+        const int v0 = cut[i], v1 = cut[i + 1];
         h->vad_partition_sms = (i > 0 || prev_busy) ? vad_sms : 0;
         if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
-        const int st = b2i_vad_launch(h, d_pcm, pcm_off + b0, b1 - b0, fpw, non_speech_label,
+        const int st = b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label,
                                       (int64_t)fpw * energy_threshold, z_lo, z_hi, (float*)d_refsig,
-                                      ref_off.data() + b0);
+                                      ref_off.data() + v0);
         h->vad_partition_sms = 0;
         if (st != B2_OK) return st;
         vad_done[i] = next_event(h);
@@ -1071,20 +1112,52 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
         cudaEventElapsedTime(&ms, tev[0], tev[k]);
         return ms;
       };
-      fprintf(stderr, "[b2 pipe] B=%d n_sub=%d vad_sms=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
-              B, n_sub, vad_sms, (int)chained, (int)prev_busy, host_ms[0]);
+      fprintf(stderr, "[b2 pipe] V=%d T=%d n_sub=%d vad_sms=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
+              V, T, n_sub, vad_sms, (int)chained, (int)prev_busy, host_ms[0]);
       for (int i = 0; i < n_sub; ++i)
-        fprintf(stderr, "[b2 pipe]  sub %d pairs %4d..%4d  VAD %7.3f -> %7.3f ms   chain %7.3f -> %7.3f ms   host enqueued chain at %.3f ms\n",
+        fprintf(stderr, "[b2 pipe]  sub %d videos %4d..%4d  VAD %7.3f -> %7.3f ms   chain %7.3f -> %7.3f ms   host enqueued chain at %.3f ms\n",
                 i, cut[i], cut[i + 1], at(1 + 4 * i), at(2 + 4 * i), at(3 + 4 * i), at(4 + 4 * i), host_ms[i + 1]);
       for (auto& e : tev) cudaEventDestroy(e);
     }
   }
   if (memspace == B2_DEVICE) return B2_OK;
-  B2_TRY(copy_out(h, best_score, d_bs, (size_t)B * 8));
-  B2_TRY(copy_out(h, best_offset, d_bo, (size_t)B * 4));
-  B2_TRY(copy_out(h, best_k, d_bk, (size_t)B * 4));
+  B2_TRY(copy_out(h, best_score, d_bs, (size_t)T * 8));
+  B2_TRY(copy_out(h, best_offset, d_bo, (size_t)T * 4));
+  B2_TRY(copy_out(h, best_k, d_bk, (size_t)T * 4));
   if (all_score) B2_TRY(copy_out(h, all_score, d_score, J * 8));
   if (all_offset) B2_TRY(copy_out(h, all_offset, d_offset, J * 4));
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
+}
+
+extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
+                             int frame_rate, int sample_rate, float non_speech_label,
+                             int64_t energy_threshold, int z_lo, int z_hi,
+                             const double* cue_start_s, const double* cue_end_s,
+                             const uint8_t* cue_keep, const int64_t* cue_off, const double* ratios,
+                             int K, double start_seconds, int64_t max_offset_samples,
+                             double* best_score, int32_t* best_offset, int32_t* best_k,
+                             double* all_score, int32_t* all_offset, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_batch");
+  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, B, nullptr, B, frame_rate, sample_rate,
+                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
+                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
+                          all_offset, memspace);
+}
+
+extern "C" int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                              const int32_t* track_video, int T, int frame_rate, int sample_rate,
+                              float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                              const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                              const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                              int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                              int32_t* best_k, double* all_score, int32_t* all_offset, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: null track_video");
+  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
+                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
+                          all_offset, memspace);
 }

@@ -4,8 +4,9 @@
 // Instead of tiling the N candidate offsets in 16 385-wide windows (corr.cu; every tile re-transforms
 // every block) each signal gets ONE real FFT of the padded length N = 2^k >= R + S, computed as a
 // four-step complex FFT of M = N/2 = M1 x 1024 points (bigfft.cuh): columns (F1), rows + untangle
-// [+ product + inverse rows] (F2), inverse columns (F3).  The reference spectrum of a pair is computed
-// once and reused by its K ratio candidates.  The N fp32 scores only nominate candidates (same
+// [+ product + inverse rows] (F2), inverse columns (F3).  The reference spectrum of a video is computed
+// once (per slice of its tracks, when they exceed the workspace budget) and reused by the K ratio
+// candidates of each of its tracks.  The N fp32 scores only nominate candidates (same
 // worst-case round-off bound tau, same selection, exact float64 re-score and argmax as the windowed
 // path); the maximum over the N-sized score arrays comes from per-tile maxima of F3, and the selection
 // (corr.cu) counts hits per 4 096-offset chunk and compacts only the chunks that hold candidates.
@@ -291,19 +292,18 @@ int launch_cols_q(b2_ctx* h, int q1, bool inverse, const float* d_sig, const uin
 
 }  // namespace
 
-int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int B, int K,
-                  std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
+int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int V,
+                  const int* trk_off, int K, std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
                   const std::vector<long long>& idx_hi, const std::vector<long long>& n_pad, int winner_only,
                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0) {
   B2Range range("b2:align_big (four-step FFT per signal)");
-  const size_t J = (size_t)B * K;
-  // transform size of a pair = the largest padded length among its live ratios (more zero padding
-  // changes nothing: each job's offsets and surviving window come from ITS OWN padded length)
-  std::map<int, std::vector<int>> pairs_by_q1;
-  for (int b = 0; b < B; ++b) {
+  const size_t J = (size_t)trk_off[V] * K;
+  // transform size of a video = the largest padded length among the live jobs of its tracks (more zero
+  // padding changes nothing: each job's offsets and surviving window come from ITS OWN padded length)
+  std::map<int, std::vector<int>> videos_by_q1;
+  for (int v = 0; v < V; ++v) {
     long long n_max = 0;
-    for (int k = 0; k < K; ++k) {
-      const size_t j = (size_t)b * K + k;
+    for (size_t j = (size_t)trk_off[v] * K; j < (size_t)trk_off[v + 1] * K; ++j) {
       SelJob& s = sel[j];
       if (s.kind != 0) continue;
       n_max = std::max(n_max, n_pad[j]);
@@ -316,37 +316,51 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
     if (n_max == 0) continue;
     int lg = 0;
     while ((1LL << lg) < n_max) ++lg;
-    pairs_by_q1[lg - 11].push_back(b);
+    videos_by_q1[lg - 11].push_back(v);
   }
-  // group = as many pairs as keep the work arrays within the workspace budget
+  // A group is as many slices as keep the work arrays within the workspace budget.  A slice is a range of
+  // tracks of one video with its own reference transform: a whole video when its K ratio jobs per track fit,
+  // else as many tracks as fit (one track at least - a track's K jobs stay together, the winner-only test of
+  // the selection compares them).
   size_t budget = (size_t)4 << 30;
   if (const char* e = getenv("B2_BIG_WS_MB")) budget = (size_t)std::max(64, atoi(e)) << 20;
-  struct Group { int q1; std::vector<int> pairs; };
+  struct Slice { int t0, t1; };
+  struct Group { int q1; std::vector<Slice> slices; };
   std::vector<Group> groups;
-  for (auto& kv : pairs_by_q1) {
+  for (auto& kv : videos_by_q1) {
     const size_t m = (size_t)1 << (kv.first + 10);
-    const size_t per_pair = m * 8 + (size_t)K * (m * 8 + m * 2 * 4);
-    const size_t cap = std::max<size_t>(1, budget / per_pair);
-    for (size_t i = 0; i < kv.second.size(); i += cap)
-      groups.push_back({kv.first, std::vector<int>(kv.second.begin() + i,
-                                                   kv.second.begin() + std::min(kv.second.size(), i + cap))});
+    const size_t per_ref = m * 8, per_track = (size_t)K * (m * 8 + m * 2 * 4);
+    const size_t max_tracks = std::max<size_t>(1, budget > per_ref ? (budget - per_ref) / per_track : 0);
+    size_t used = 0;
+    for (int v : kv.second) {
+      for (int t0 = trk_off[v]; t0 < trk_off[v + 1]; t0 += (int)max_tracks) {
+        const int t1 = (int)std::min<size_t>(trk_off[v + 1], t0 + max_tracks);
+        const size_t cost = per_ref + (size_t)(t1 - t0) * per_track;
+        if (groups.empty() || groups.back().q1 != kv.first || (used + cost > budget && used > 0)) {
+          groups.push_back({kv.first, {}});
+          used = 0;
+        }
+        groups.back().slices.push_back({t0, t1});
+        used += cost;
+      }
+    }
   }
   // score_off is group-local (the score workspace is reused by the next group)
   size_t max_g = 0, max_scores = 0, max_tiles = 0, max_cnt = 0;
   for (auto& g : groups) {
     const size_t m = (size_t)1 << (g.q1 + 10), n = 2 * m;
     size_t n_sub = 0;
-    for (int b : g.pairs)
-      for (int k = 0; k < K; ++k) {
-        SelJob& s = sel[(size_t)b * K + k];
+    for (const Slice& sl : g.slices)
+      for (size_t j = (size_t)sl.t0 * K; j < (size_t)sl.t1 * K; ++j) {
+        SelJob& s = sel[j];
         if (s.kind != 0) continue;
         s.score_off = (long long)(n_sub * n);
         ++n_sub;
       }
     const size_t tiles_per = ((size_t)1 << g.q1) / 16;
-    max_g = std::max(max_g, (g.pairs.size() + n_sub) * m);
+    max_g = std::max(max_g, (g.slices.size() + n_sub) * m);
     max_scores = std::max(max_scores, n_sub * n);
-    max_tiles = std::max(max_tiles, (g.pairs.size() + 3 * n_sub) * tiles_per);
+    max_tiles = std::max(max_tiles, (g.slices.size() + 3 * n_sub) * tiles_per);
     max_cnt = std::max(max_cnt, n_sub * ((n + kChunk - 1) / kChunk));
   }
   // The job table is read by kernels of EVERY group and by the common tail, i.e. long after later
@@ -391,13 +405,12 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
     const int tiles_per = (1 << q1) / 16;
     std::vector<BigXform> xr, xs;
     std::vector<BigJob> jobs;
-    for (size_t pi = 0; pi < g.pairs.size(); ++pi) {
-      const int b = g.pairs[pi];
+    for (size_t pi = 0; pi < g.slices.size(); ++pi) {
+      const Slice& sl = g.slices[pi];
       BigXform r;
       memset(&r, 0, sizeof(r));
       bool have_ref = false;
-      for (int k = 0; k < K; ++k) {
-        const size_t j = (size_t)b * K + k;
+      for (size_t j = (size_t)sl.t0 * K; j < (size_t)sl.t1 * K; ++j) {
         const SelJob& s = sel[j];
         if (s.kind != 0) continue;
         if (!have_ref) {
@@ -416,13 +429,13 @@ int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint3
         x.S = s.S;
         x.m_lo = s.m_lo;
         x.m_hi = s.m_hi;
-        x.g_off = (long long)((g.pairs.size() + xs.size()) * m);
+        x.g_off = (long long)((g.slices.size() + xs.size()) * m);
         x.spec_off = r.g_off;
         x.score_off = s.score_off;
         jobs.push_back({(int)j, (int)xs.size(), (int)pi});
         xs.push_back(x);
       }
-      xr.push_back(r);   // a pair without live jobs keeps a zero-length dummy (never referenced)
+      xr.push_back(r);   // a slice without live jobs keeps a zero-length dummy (never referenced)
     }
     const int n_ref = (int)xr.size(), n_sub = (int)xs.size();
     if (n_sub == 0) continue;

@@ -196,8 +196,10 @@ struct B2CueSource {
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);
 // capture_j0: global index of job 0 of this call in the arrays of b2_capture_nominations (b2_sync_batch's
-// sub-batches align a range of pairs at a time)
-int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host,
+// sub-batches align a range of pairs at a time).  ref_off_host has V+1 entries; reference v is shared by
+// the tracks trk_off[v] .. trk_off[v+1]-1 (trk_off[V] == B), each with K ratio jobs t*K + k.  trk_off == NULL:
+// V == B, reference b belongs to pair b alone.
+int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host, int V, const int* trk_off,
                      const float* d_sub, const int64_t* sub_off_host, int B, int K,
                      int64_t max_offset_samples, double* d_score, int32_t* d_offset,
                      int32_t* d_status, int winner_only, const B2CueSource* cue_src,

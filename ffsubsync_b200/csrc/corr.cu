@@ -12,8 +12,8 @@
 // L = P - W + 1 samples; each block and the P reference samples it can meet are transformed with
 // a P = 2^15 point real FFT that lives entirely in shared memory, conj(A)*B is accumulated over
 // the blocks in registers, and ONE inverse transform yields the W scores (overlap-save
-// correlation).  The reference-side spectra are computed once per pair and reused by all K
-// ratio candidates.  The fp32 scores only nominate candidates: every offset within a first-order
+// correlation).  The reference-side spectra are computed once per video and reused by all K
+// ratio candidates of each of its subtitle tracks (b2_sync_batch: one track per video).  The fp32 scores only nominate candidates: every offset within a first-order
 // worst-case round-off bound (tau, below) of the maximum is re-scored exactly (float64 direct sum), so the returned
 // offset and score do not depend on FFT round-off.  Offset ranges wider than P/2 are tiled.
 #include <math.h>
@@ -631,12 +631,19 @@ int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n
   return B2_OK;
 }
 
-int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, const float* d_sub,
-                     const int64_t* sub_off, int B, int K, int64_t max_offset_samples,
+int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off,
+                     const float* d_sub, const int64_t* sub_off, int B, int K, int64_t max_offset_samples,
                      double* d_score, int32_t* d_offset, int32_t* d_status, int winner_only,
                      const B2CueSource* cue_src, long long capture_j0) {
   B2Range range("b2:align (ref_spectra, sub_correlate, select, rescore, pick)");
   const size_t J = (size_t)B * K;
+  std::vector<int> ident;   // no track table: reference b is read by pair b alone
+  if (!trk_off) {
+    ident.resize(B + 1);
+    for (int b = 0; b <= B; ++b) ident[b] = b;
+    trk_off = ident.data();
+    V = B;
+  }
   // cue mode (b2_sync_batch): the subtitle signals exist only as bit masks, rasterised from the cue
   // list by raster_bits_kernel below (sub_off then only carries the signal lengths)
   const bool cue_mode = cue_src != nullptr;
@@ -646,73 +653,77 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
       bits_off[j + 1] = bits_off[j] + ((sub_off[j + 1] - sub_off[j]) + kP) / 32 + 1;
   std::vector<SelJob> sel(J);
   std::vector<long long> idx_lo(J, 0), idx_hi(J, 0), n_pad(J, 0);
+  // one plan per reference (video): its window covers the live jobs of all its tracks, whose K ratio jobs
+  // are [trk_off[v] * K, trk_off[v + 1] * K)
   struct PairPlan { long long o_min, o_max; int n_tiles; bool any; };
-  std::vector<PairPlan> pp(B);
+  std::vector<PairPlan> pp(V);
   long long max_w = 1;
   bool big_ok = true;   // every live job's padded length suits the large-window path
-  for (int b = 0; b < B; ++b) {
-    const long long R = ref_off[b + 1] - ref_off[b];
-    if (R < 0 || R > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad reference length at %d", b);
-    PairPlan& p = pp[b];
+  const long long mo_clamped =
+      std::max<long long>(-(1LL << 40), std::min<long long>(1LL << 40, max_offset_samples));
+  for (int v = 0; v < V; ++v) {
+    const long long R = ref_off[v + 1] - ref_off[v];
+    if (R < 0 || R > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad reference length at %d", v);
+    PairPlan& p = pp[v];
     p.any = false;
     p.o_min = 0;
     p.o_max = -1;
-    for (int k = 0; k < K; ++k) {
-      const size_t j = (size_t)b * K + k;
-      const long long S = sub_off[j + 1] - sub_off[j];
-      if (S < 0 || S > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad subtitle length at %zu", j);
-      SelJob& s = sel[j];
-      memset(&s, 0, sizeof(s));
-      s.ref_off = ref_off[b];
-      s.sub_off = sub_off[j];
-      s.R = (int)R;
-      s.S = (int)S;
-      s.out_index = (int)j;
-      s.bits_off = cue_mode ? bits_off[j] : -1;
-      s.sub_level = cue_mode ? (float)std::min(1.0 / cue_src->ratios[k], 1.0) : 0.f;  // speech_transformers.py:977
-      if (R == 0 || S == 0) {  // aligners.py:58-66
-        s.kind = 1;
-        continue;
+    for (int b = trk_off[v]; b < trk_off[v + 1]; ++b) {
+      long long t_min = 0, t_max = -1;   // window of this track's K jobs (winner-only pruning is per track)
+      bool t_any = false;
+      for (int k = 0; k < K; ++k) {
+        const size_t j = (size_t)b * K + k;
+        const long long S = sub_off[j + 1] - sub_off[j];
+        if (S < 0 || S > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad subtitle length at %zu", j);
+        SelJob& s = sel[j];
+        memset(&s, 0, sizeof(s));
+        s.ref_off = ref_off[v];
+        s.sub_off = sub_off[j];
+        s.R = (int)R;
+        s.S = (int)S;
+        s.out_index = (int)j;
+        s.bits_off = cue_mode ? bits_off[j] : -1;
+        s.sub_level = cue_mode ? (float)std::min(1.0 / cue_src->ratios[k], 1.0) : 0.f;  // speech_transformers.py:977
+        if (R == 0 || S == 0) {  // aligners.py:58-66
+          s.kind = 1;
+          continue;
+        }
+        const long long N = padded_length(h, R + S);
+        long long lo = 0, hi = N;  // surviving index range, aligners.py:31-43 with slice semantics
+        if (max_offset_samples != B2_MAX_OFFSET_NONE) {
+          // any int64 width, negative ones included, through the reference's slice arithmetic; widths
+          // are clamped to +-2^40 first (beyond every padded length, so the result is unchanged)
+          const long long mo = mo_clamped;
+          const long long a = N - 1 - mo - S;
+          const long long bb = N - 1 + mo - S;
+          lo = a >= 0 ? std::min(a, N) : std::max(a + N, 0LL);
+          hi = bb >= 0 ? std::min(bb, N) : std::max(bb + N, 0LL);
+        }
+        if (lo >= hi) {
+          s.kind = 2;
+          s.masked_offset = (int)(N - 1 - S);
+          continue;
+        }
+        const long long o_lo = N - S - hi, o_hi = N - 1 - S - lo;  // aligners.py:47
+        idx_lo[j] = lo;
+        idx_hi[j] = hi;
+        n_pad[j] = N;
+        if (N < (1LL << (bigfft_min_log2n())) || N > (1LL << bigfft_max_log2n())) big_ok = false;
+        s.kind = 0;
+        s.m_lo = (int)o_lo;  // temporarily absolute offsets; rebased below
+        s.m_hi = (int)o_hi;
+        t_min = t_any ? std::min(t_min, o_lo) : o_lo;
+        t_max = t_any ? std::max(t_max, o_hi) : o_hi;
+        t_any = true;
       }
-      const long long N = padded_length(h, R + S);
-      long long lo = 0, hi = N;  // surviving index range, aligners.py:31-43 with slice semantics
-      if (max_offset_samples != B2_MAX_OFFSET_NONE) {
-        // any int64 width, negative ones included, through the reference's slice arithmetic; widths
-        // are clamped to +-2^40 first (beyond every padded length, so the result is unchanged)
-        const long long mo = std::max<long long>(-(1LL << 40), std::min<long long>(1LL << 40, max_offset_samples));
-        const long long a = N - 1 - mo - S;
-        const long long bb = N - 1 + mo - S;
-        lo = a >= 0 ? std::min(a, N) : std::max(a + N, 0LL);
-        hi = bb >= 0 ? std::min(bb, N) : std::max(bb + N, 0LL);
-      }
-      if (lo >= hi) {
-        s.kind = 2;
-        s.masked_offset = (int)(N - 1 - S);
-        continue;
-      }
-      const long long o_lo = N - S - hi, o_hi = N - 1 - S - lo;  // aligners.py:47
-      idx_lo[j] = lo;
-      idx_hi[j] = hi;
-      n_pad[j] = N;
-      if (N < (1LL << (bigfft_min_log2n())) || N > (1LL << bigfft_max_log2n())) big_ok = false;
-      s.kind = 0;
-      s.m_lo = (int)o_lo;  // temporarily absolute offsets; rebased below
-      s.m_hi = (int)o_hi;
-      if (!p.any) {
-        p.o_min = o_lo;
-        p.o_max = o_hi;
-        p.any = true;
-      } else {
-        p.o_min = std::min(p.o_min, o_lo);
-        p.o_max = std::max(p.o_max, o_hi);
-      }
-    }
-    if (p.any) max_w = std::max(max_w, p.o_max - p.o_min + 1);
-    if (p.any && max_offset_samples != B2_MAX_OFFSET_NONE) {
-      const long long mo = std::max<long long>(-(1LL << 40), std::min<long long>(1LL << 40, max_offset_samples));
-      if (std::max(llabs(p.o_min), llabs(p.o_max)) > mo)
+      if (!t_any) continue;
+      p.o_min = p.any ? std::min(p.o_min, t_min) : t_min;
+      p.o_max = p.any ? std::max(p.o_max, t_max) : t_max;
+      p.any = true;
+      if (max_offset_samples != B2_MAX_OFFSET_NONE && std::max(llabs(t_min), llabs(t_max)) > mo_clamped)
         for (int k = 0; k < K; ++k) sel[(size_t)b * K + k].no_prune = 1;
     }
+    if (p.any) max_w = std::max(max_w, p.o_max - p.o_min + 1);
   }
   const bool capture = h->capture.scores != nullptr;
   if (capture)
@@ -755,8 +766,8 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
   }
   if (use_big) {
     const SelJob* d_sel_big = nullptr;
-    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, B, K, sel, idx_lo, idx_hi, n_pad, winner_only, cb, &d_sel_big,
-                         capture_j0));
+    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, V, trk_off, K, sel, idx_lo, idx_hi, n_pad, winner_only, cb,
+                         &d_sel_big, capture_j0));
     return b2i_rescore_pick(h, d_sel_big, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
   }
 
@@ -767,11 +778,11 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
   // linear) into its own partial score array, and window_max_kernel adds the partial arrays in a
   // fixed order.  Costs one extra inverse transform per chunk, so chunks keep >= 4 blocks.
   long long n_jobs_total = 0, max_blocks = 1;
-  for (int b = 0; b < B; ++b) {
-    PairPlan& p = pp[b];
+  for (int v = 0; v < V; ++v) {
+    PairPlan& p = pp[v];
     p.n_tiles = p.any ? (int)ceil_div64(p.o_max - p.o_min + 1, Wt) : 0;
-    for (int k = 0; k < K; ++k) {
-      const SelJob& s = sel[(size_t)b * K + k];
+    for (size_t j = (size_t)trk_off[v] * K; j < (size_t)trk_off[v + 1] * K; ++j) {
+      const SelJob& s = sel[j];
       if (s.kind != 0) continue;
       n_jobs_total += p.n_tiles;
       max_blocks = std::max<long long>(max_blocks, ceil_div64(s.S, L));
@@ -783,10 +794,10 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
                                                                max_blocks / 4));
   if (const char* e = getenv("B2_ALIGN_SPLIT")) n_split = std::max(1, atoi(e));  // test / tuning knob
   long long score_total = 0, energy_total = 0, max_score_len = 0;
-  for (int b = 0; b < B; ++b) {
-    PairPlan& p = pp[b];
-    for (int k = 0; k < K; ++k) {
-      SelJob& s = sel[(size_t)b * K + k];
+  for (int v = 0; v < V; ++v) {
+    PairPlan& p = pp[v];
+    for (size_t j = (size_t)trk_off[v] * K; j < (size_t)trk_off[v + 1] * K; ++j) {
+      SelJob& s = sel[j];
       if (s.kind != 0) continue;
       max_score_len = std::max(max_score_len, (long long)p.n_tiles * Wt);
       s.o_first = (int)p.o_min;
@@ -852,13 +863,15 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
     return B2_OK;
   };
 
-  for (int b = 0; b < B; ++b) {
-    const PairPlan& p = pp[b];
+  // the reference blocks of a (video, tile) are transformed once and read by every track and ratio of the video
+  for (int v = 0; v < V; ++v) {
+    const PairPlan& p = pp[v];
     if (!p.any) continue;
-    const long long R = ref_off[b + 1] - ref_off[b];
+    const long long R = ref_off[v + 1] - ref_off[v];
+    const size_t j_lo = (size_t)trk_off[v] * K, j_hi = (size_t)trk_off[v + 1] * K;
     long long nblk_max = 0;
-    for (int k = 0; k < K; ++k) {
-      const SelJob& s = sel[(size_t)b * K + k];
+    for (size_t j = j_lo; j < j_hi; ++j) {
+      const SelJob& s = sel[j];
       if (s.kind == 0) nblk_max = std::max<long long>(nblk_max, ceil_div64(s.S, L));
     }
     for (int tile = 0; tile < p.n_tiles; ++tile) {
@@ -870,13 +883,13 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, cons
       const long long spec_base = (long long)items.size();
       for (long long blk = blk_lo; blk < blk_hi; ++blk) {
         SpecItem it;
-        it.ref_off = ref_off[b];
+        it.ref_off = ref_off[v];
         it.R = (int)R;
         it.i0 = (int)(blk * L + o_t);
         items.push_back(it);
       }
-      for (int k = 0; k < K; ++k) {
-        const SelJob& s = sel[(size_t)b * K + k];
+      for (size_t j = j_lo; j < j_hi; ++j) {
+        const SelJob& s = sel[j];
         if (s.kind != 0) continue;
         const long long job_hi = std::min<long long>(blk_hi, ceil_div64(s.S, L));
         const long long n_blk = std::max(0LL, job_hi - blk_lo);

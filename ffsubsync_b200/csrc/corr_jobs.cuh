@@ -90,8 +90,9 @@ int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n
                        const B2CandBuffers& cb, long long j0);
 // Large-window path (bigfft.cu).  sel: host copy of the jobs (kind / R / S / offsets filled in by the
 // planner; this call sets o_first, m_lo, m_hi, score_off), surviving index range per job in idx_lo /
-// idx_hi (half open, in the reference's conv[] index space), padded lengths n_pad per pair.
-int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int B, int K,
-                  std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
+// idx_hi (half open, in the reference's conv[] index space), padded lengths n_pad per job.  Reference v
+// is read by the K ratio jobs of each of its tracks trk_off[v] .. trk_off[v+1]-1.
+int b2i_align_big(b2_ctx* h, const float* d_ref, const float* d_sub, const uint32_t* d_bits, int V,
+                  const int* trk_off, int K, std::vector<SelJob>& sel, const std::vector<long long>& idx_lo,
                   const std::vector<long long>& idx_hi, const std::vector<long long>& n_pad, int winner_only,
                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0);

@@ -13,6 +13,7 @@ The same functions run on the ``gloo`` backend with CPU tensors (tests, world_si
 import os
 from typing import List, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -98,22 +99,62 @@ def shard_candidates(n_candidates: int, rank: int, world: int) -> List[int]:
     return list(range(rank, n_candidates, world))
 
 
+def shard_videos(track_video, rank: int, world: int) -> Tuple[int, int, int, int]:
+    """Block sharding of videos with several subtitle tracks (track_video: non-decreasing video index of
+    each track, as for BatchSynchronizer.sync_device_tracks).  Rank g owns the videos [v0, v1) and their
+    tracks [t0, t1); a video's tracks never straddle two ranks, and the rank boundaries are the first
+    videos whose tracks start at or after track g*T/G, so ranks hold about equal numbers of tracks.
+    The videos are those up to the last one with tracks (V = track_video[-1] + 1); one without tracks
+    goes with the previous video that has tracks.  Returns (v0, v1, t0, t1)."""
+    track_video = np.asarray(track_video, dtype=np.int64)
+    T = len(track_video)
+    V = int(track_video[-1]) + 1 if T else 0
+
+    def cut(g):
+        if g >= world:
+            return V, T
+        t = (g * T) // world
+        while 0 < t < T and track_video[t] == track_video[t - 1]:   # move up to the start of the next video
+            t += 1
+        return (int(track_video[t]) if t < T else V), t
+
+    (v0, t0), (v1, t1) = cut(rank), cut(rank + 1)
+    return (0 if rank == 0 else v0), v1, t0, t1
+
+
+def _gather_blocks(local: torch.Tensor, counts: List[Tuple[int, int]], rank: int, world: int, dst: Optional[int],
+                   group) -> Optional[torch.Tensor]:
+    """Rank r holds rows [lo_r, hi_r) of the result: pad every block to the largest, one
+    all_gather_into_tensor, concatenate in rank order on ``dst`` (every rank when dst is None)."""
+    width = max(max(hi - lo for lo, hi in counts), 1)
+    padded = torch.zeros((width,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+    padded[: local.shape[0]] = local
+    out = torch.empty((world * width,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+    dist.all_gather_into_tensor(out, padded, group=group)
+    if dst is not None and rank != dst:
+        return None
+    out = out.view((world, width) + tuple(local.shape[1:]))
+    return torch.cat([out[r, : hi - lo] for r, (lo, hi) in enumerate(counts)], dim=0)
+
+
 def gather_pair_results(local: torch.Tensor, n_pairs: int, rank: int, world: int, dst: int = 0,
                         group=None) -> Optional[torch.Tensor]:
     """local: [n_local, C] results of this rank's block of pairs (any dtype, same on all ranks).
     Returns [n_pairs, C] in global pair order on ``dst`` (None elsewhere).  One collective."""
     if world == 1:
         return local
-    counts = [shard_pairs(n_pairs, r, world) for r in range(world)]
-    width = max(hi - lo for lo, hi in counts)
-    padded = torch.zeros((width,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
-    padded[: local.shape[0]] = local
-    out = torch.empty((world * width,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
-    dist.all_gather_into_tensor(out, padded, group=group)
-    if rank != dst:
-        return None
-    out = out.view((world, width) + tuple(local.shape[1:]))
-    return torch.cat([out[r, : hi - lo] for r, (lo, hi) in enumerate(counts)], dim=0)
+    return _gather_blocks(local, [shard_pairs(n_pairs, r, world) for r in range(world)], rank, world, dst, group)
+
+
+def gather_track_results(local: torch.Tensor, track_video, rank: int, world: int, dst: Optional[int] = 0,
+                         group=None) -> Optional[torch.Tensor]:
+    """local: [t1 - t0, C] results of the tracks shard_videos() gave this rank (per-rank counts differ).
+    Returns [T, C] in global track order on ``dst`` (on every rank when dst is None, None elsewhere).
+    One collective."""
+    if world == 1:
+        return local
+    counts = [shard_videos(track_video, r, world)[2:] for r in range(world)]
+    return _gather_blocks(local, counts, rank, world, dst, group)
 
 
 def allgather_candidate_results(local: torch.Tensor, n_candidates: int, rank: int, world: int,

@@ -194,6 +194,27 @@ int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B
                   double* all_score /* [B*K] or NULL */, int32_t* all_offset /* or NULL */,
                   int memspace);
 
+/* ---- the whole hot path for several subtitle tracks per video ------------------------------
+ * `ffs movie.mkv -i en.srt de.srt ...` (ffsubsync/ffsubsync.py:637 + the loop of try_sync over
+ * args.srtin, :186-235) for V videos and T tracks in one call: track t (cue list
+ * cue_off[t] .. cue_off[t+1]) is synced against the PCM of video track_video[t].  track_video is a host
+ * array, non-decreasing, every entry in [0, V).  Each video's PCM goes through the VAD once and its
+ * reference spectra are shared by all its tracks.  Track t gets exactly what b2_sync_batch returns for the
+ * pair (PCM of video track_video[t], cue list t): best_*[t], and all_*[t*K + k] when requested.
+ * A video without tracks is legal; its VAD still runs (its PCM is read, nothing of it is returned).
+ * memspace as for b2_sync_batch (B2_HOST, B2_DEVICE, B2_DEVICE_RESIDENT; resident calls chain with
+ * b2_sync_batch calls too).  B2_ERR_BAD_ARG for a track_video entry out of range or smaller than the one
+ * before, a non-monotone pcm_off or cue_off, a null output or, with B2_DEVICE, a host pointer among pcm
+ * and the outputs. */
+int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /* [V+1] */, int V,
+                   const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                   float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                   const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                   const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                   int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                   double* all_score /* [T*K] or NULL */, int32_t* all_offset /* [T*K] or NULL */,
+                   int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
