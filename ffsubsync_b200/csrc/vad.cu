@@ -15,6 +15,7 @@
 // straight out of shared memory (conflict-free LDS.128) and release the stage through its
 // "empty" mbarrier - no CTA-wide barrier on the steady-state path.
 #include "common.cuh"
+#include "vad_group.cuh"
 #include "vad_lane.cuh"
 
 namespace {
@@ -98,64 +99,6 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_
       : "memory");
 }
 
-// One 32-bit word = samples (x0 = low half, x1 = high half).
-//   energy: x^2 = x*lo8(x) + 256*x*hi8(x) (lo8 unsigned, hi8 signed) -> two 2-way 16x8 dot products
-//   crossings: f = [x0 : previous sample]; (w ^ f) carries prev->x0 in bit 15, x0->x1 in bit 31
-__device__ __forceinline__ void accum_word(uint32_t w, uint32_t prev, int& e_lo, int& e_hi,
-                                           uint32_t& z128) {
-  const uint32_t perm = __byte_perm(w, 0u, 0x3120);  // bytes [lo8(x0), lo8(x1), hi8(x0), hi8(x1)]
-  asm("dp2a.lo.s32.u32 %0, %1, %2, %0;" : "+r"(e_lo) : "r"(w), "r"(perm));
-  asm("dp2a.hi.s32.s32 %0, %1, %2, %0;" : "+r"(e_hi) : "r"(w), "r"(perm));
-  const uint32_t f = __funnelshift_l(prev, w, 16);
-  // bytes 1 and 3 of the masked word are 0x80 per crossing: a 4-way byte dot product with ones
-  // adds 128 per crossing (one IDP.4A instead of POPC + IADD)
-  z128 = __dp4a((w ^ f) & 0x80008000u, 0x01010101u, z128);
-}
-
-// Lane g of a window owns the contiguous 16-byte chunks [g*CPL, (g+1)*CPL).
-template <int CPL>
-__device__ __forceinline__ void window_part_fast(const unsigned char* wbase, int g, int cpl_rt,
-                                                 long long& e, int& z) {
-  const int cpl = CPL > 0 ? CPL : cpl_rt;
-  const unsigned char* cbase = wbase + 16 * g * cpl;
-  uint32_t pw = 0;
-  if (g > 0) pw = *reinterpret_cast<const uint32_t*>(cbase - 4);
-  // two independent accumulator sets: the IDP chains are latency-bound otherwise (a CTA that shares
-  // its SM with the correlation kernel has only 8 consumer warps to hide them)
-  int e_lo = 0, e_hi = 0, f_lo = 0, f_hi = 0;
-  uint32_t z128 = 0, y128 = 0;
-  if (CPL > 0) {
-    uint4 v[CPL > 0 ? CPL : 1];
-#pragma unroll
-    for (int c = 0; c < CPL; ++c) v[c] = *reinterpret_cast<const uint4*>(cbase + 16 * c);
-    if (g == 0) pw = v[0].x << 16;  // first sample of the window: no crossing before it
-#pragma unroll
-    for (int c = 0; c < CPL; ++c) {
-      accum_word(v[c].x, pw, e_lo, e_hi, z128);
-      accum_word(v[c].y, v[c].x, f_lo, f_hi, y128);
-      accum_word(v[c].z, v[c].y, e_lo, e_hi, z128);
-      accum_word(v[c].w, v[c].z, f_lo, f_hi, y128);
-      pw = v[c].w;
-    }
-  } else {
-    for (int c = 0; c < cpl; ++c) {
-      const uint4 v = *reinterpret_cast<const uint4*>(cbase + 16 * c);
-      if (c == 0 && g == 0) pw = v.x << 16;
-      accum_word(v.x, pw, e_lo, e_hi, z128);
-      accum_word(v.y, v.x, f_lo, f_hi, y128);
-      accum_word(v.z, v.y, e_lo, e_hi, z128);
-      accum_word(v.w, v.z, f_lo, f_hi, y128);
-      pw = v.w;
-      if ((c & 15) == 15) {  // keep the 32-bit partial sums far from overflow
-        e += (long long)e_lo + (long long)f_lo + ((long long)e_hi + (long long)f_hi) * 256LL;
-        e_lo = e_hi = f_lo = f_hi = 0;
-      }
-    }
-  }
-  e += (long long)e_lo + (long long)f_lo + ((long long)e_hi + (long long)f_hi) * 256LL;
-  z += (int)((z128 + y128) >> 7);
-}
-
 // Sum (e, z) over the G lanes of a window (G a power of two <= 32, lanes contiguous).
 template <int GT>
 __device__ __forceinline__ void lane_group_sum(int G, long long& e, int& z) {
@@ -189,7 +132,7 @@ __device__ __forceinline__ void consume_tile_fast(const VadParams& p, const Tile
     const bool full = active && avail >= fpw;
     const bool tail = active && !full && avail > 0 && p.tail_emin != nullptr;
     if (full) {
-      window_part_fast<CPL>(span + (size_t)wl * fpw * 2, g, p.cpl, e, z);
+      vadgroup::window_part_fast<CPL>(span + (size_t)wl * fpw * 2, g, p.cpl, e, z);
     } else if (tail) {  // at most one window per signal: plain 16-bit loop over the samples it has
       const short* xs = reinterpret_cast<const short*>(span + (size_t)wl * fpw * 2);
       for (int i = g; i < (int)avail; i += p.G) e += (long long)xs[i] * xs[i];
@@ -724,6 +667,9 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
     if (const char* e = getenv("B2_VAD_EVICT_FIRST")) p.evict_first = atoi(e) != 0;   // A/B knob
     p.batch = kLaneBatch;
     if (const char* e = getenv("B2_VAD_BATCH")) p.batch = std::max(1, std::min(16, atoi(e)));   // tuning knob
+    // lane l of a producer pass stages into stage0 + l, wrapped once: a batch deeper than the ring would run
+    // past the pipeline's stages (and two lanes of one pass would share a stage)
+    p.batch = std::min(p.batch, stages);
     smem = (size_t)kLanePipes * stages * p.stage_bytes + 2 * kLaneMaxStages * sizeof(uint64_t) +
            kLaneMaxStages * sizeof(TileDesc) + 64;
     for (int b = 0; b < B; ++b) {

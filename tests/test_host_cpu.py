@@ -466,9 +466,15 @@ def test_bigfft_roundoff_adversarial(built):
 
 def test_vad_lane_arithmetic_emulation(built):
     """csrc/vad_lane.cuh (byte dot products, circular chunk order) == sum x^2 / sign changes, for every
-    instantiated window size, every start chunk, int16 extremes; and the bank-group bijection."""
+    instantiated window size, every start chunk, int16 extremes; and the bank-group bijection.  Also
+    csrc/vad_group.cuh (dp2a energy split, lane-boundary word, runtime-CPL flushes) for every
+    (chunks per lane, lanes per window) pair of the lane-group kernel's vector path."""
     exe = os.path.join(ROOT, "tests", "host_emul", "vad_emul")
     out = subprocess.run([exe, "140"], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout
-    assert out.stdout.startswith("ok "), out.stdout
-    assert int(out.stdout.split()[1]) > 50000
+    lines = out.stdout.splitlines()
+    assert lines[-1].startswith("ok "), out.stdout
+    assert int(lines[-1].split()[1]) > 50000
+    for cpl, g in ((5, 4), (15, 4), (5, 2), (15, 2), (5, 8), (15, 8), (1, 32), (17, 2)):
+        row = [ln for ln in lines if ln.startswith("group CPL=%d" % cpl) and " G=%d " % g in ln]
+        assert len(row) == 1 and row[0].endswith(" 0 mismatches") and " 0 windows" not in row[0], (cpl, g, out.stdout)
