@@ -1001,7 +1001,8 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     if (!fused)
       B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + t0, nt, ratios, K, 0, nullptr,
                                sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
-    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds};
+    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds,
+                          non_speech_label};
     B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
                             (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
                             o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));

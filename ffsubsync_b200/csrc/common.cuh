@@ -59,7 +59,7 @@ struct b2_ctx {
   int refsig_parity = 0;
   // named grow-only workspaces
   enum { WS_STAGE_IN0, WS_STAGE_IN1, WS_STAGE_OUT, WS_META, WS_SPEC, WS_SCORES, WS_CAND,
-         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_COUNT };
+         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_COUNT };
   DeviceBuf ws[WS_COUNT];
   HostBuf pinned[4];
   cudaEvent_t pinned_ev[4] = {};   // recorded after the last async copy out of pinned[i]
@@ -192,6 +192,7 @@ struct B2CueSource {
   const double* ratios;      // [K]
   int sample_rate;
   double start_seconds;
+  float ref_label;           // the reference is this call's VAD output: every value is 1.0f or ref_label
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);

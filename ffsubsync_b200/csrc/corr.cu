@@ -19,6 +19,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 #include "corr.cuh"
@@ -758,11 +759,45 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   // Large windows (FFTAligner's default max_offset_samples=None, or a mask wider than a few tiles):
   // the overlap-save path would recompute every block for every 16 385-offset tile; one padded-length
   // FFT per signal (four-step, bigfft.cu) is cheaper from kBigMinTiles tiles on.
-  // B2_ALIGN_PATH=tiled|big: test / A-B knob.
+  // B2_ALIGN_PATH=tiled|big|runs: test / A-B knob.
   bool use_big = big_ok && max_w > (long long)kBigMinTiles * (kP / 2 + 1);
-  if (const char* e = getenv("B2_ALIGN_PATH")) {
-    if (!strcmp(e, "tiled")) use_big = false;
-    if (!strcmp(e, "big") && big_ok) use_big = true;
+  const char* path_env = getenv("B2_ALIGN_PATH");
+  const bool force_runs = path_env && !strcmp(path_env, "runs");
+  if (path_env) {
+    if (!strcmp(path_env, "tiled") || force_runs) use_big = false;
+    if (!strcmp(path_env, "big") && big_ok) use_big = true;
+  }
+  // Cue mode with the reference from this call's VAD (two levels, 1.0f and the label): the run path
+  // (runcorr.cu) scores every offset of the window from the cue runs, exactly up to a float64 margin, when
+  // its work (cues x window) is below the FFT blocks it replaces for every live job.  A capture of the fp32
+  // nominations (b2_capture_nominations) probes the FFT paths and keeps them.
+  if (cue_mode && !capture && !use_big && std::isfinite(cue_src->ref_label) &&
+      !(path_env && !strcmp(path_env, "tiled"))) {
+    bool fits = true, pays = true;
+    int max_runs = 1;
+    for (int v = 0; v < V && fits; ++v) {
+      const long long n_tiles_v = pp[v].any ? ceil_div64(pp[v].o_max - pp[v].o_min + 1, Wt) : 0;
+      for (int b = trk_off[v]; b < trk_off[v + 1]; ++b) {
+        const long long cues = cue_src->cue_off[b + 1] - cue_src->cue_off[b];  // runs of a mask <= its cues
+        for (int k = 0; k < K; ++k) {
+          const SelJob& s = sel[(size_t)b * K + k];
+          if (s.kind != 0) continue;
+          const long long w = (long long)s.m_hi - s.m_lo + 1;
+          if (w > kRunMaxWindow || cues > kRunMaxCues || llabs((long long)s.m_lo) > (1LL << 30) ||
+              llabs((long long)s.m_hi) > (1LL << 30))
+            fits = false;
+          if ((double)cues * (double)w > kRunCostPerBlock * (double)(n_tiles_v * (ceil_div64(s.S, L) + 1)))
+            pays = false;
+          max_runs = std::max<int>(max_runs, (int)std::min<long long>(cues, kRunMaxCues));
+        }
+      }
+    }
+    if (fits && (pays || force_runs)) {
+      const SelJob* d_sel_runs = nullptr;
+      B2_TRY(b2i_align_runs(h, d_ref, ref_off, V, trk_off, K, sel, d_bits, max_runs, cue_src->ref_label, winner_only,
+                            cb, &d_sel_runs));
+      return b2i_rescore_pick(h, d_sel_runs, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
+    }
   }
   if (use_big) {
     const SelJob* d_sel_big = nullptr;

@@ -88,6 +88,19 @@ int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_re
 // with scores == NULL only the jobs without a live window are written.
 int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
                        const B2CandBuffers& cb, long long j0);
+// Run path (runcorr.cu): cue mode with a two-level reference (1.0f / ref_label).  sel: host copy of the jobs
+// as the planner left them (absolute offsets in m_lo / m_hi; this call rebases them on each job's own window),
+// subtitle bit masks in d_bits, at most max_runs cue runs per job.  Fills cand_off / cand_cnt / job_stat /
+// work_list / work_count like the selection; the caller then runs b2i_rescore_pick on *d_sel_out.
+int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
+                   std::vector<SelJob>& sel, const uint32_t* d_bits, int max_runs, float ref_label, int winner_only,
+                   const B2CandBuffers& cb, const SelJob** d_sel_out);
+// The run path is chosen per call when every live job has cues x window <= kRunCostPerBlock x (its FFT block
+// transforms): the break-even measured in the bench step on an H100 (DESIGN.md section 4, "K4r").
+// kRunMaxCues bounds the shared memory of a job's run table (3 ints per run).
+constexpr double kRunCostPerBlock = 5.6e5;
+constexpr int kRunMaxCues = 16384;
+constexpr int kRunMaxWindow = 32 * 1024;  // 32 offsets per thread, 1024 threads
 // Large-window path (bigfft.cu).  sel: host copy of the jobs (kind / R / S / offsets filled in by the
 // planner; this call sets o_first, m_lo, m_hi, score_off), surviving index range per job in idx_lo /
 // idx_hi (half open, in the reference's conv[] index space), padded lengths n_pad per job.  Reference v

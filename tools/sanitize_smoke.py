@@ -7,7 +7,7 @@ Sizes are tiny (the sanitizer slows kernels 10-100x) but cover: the TMA/mbarrier
 kernels (lane-group: vector path, generic path, ragged tails; lane-per-window: multi-signal batches,
 one CTA reusing its ring many times); the auditok energy + tokenizer scan; both rasterisers;
 boundaries; blend; the correlation kernels (float and bit-mask subtitle signals, a multi-block job,
-the split-block small batch path), candidate selection, exact re-score, pick and the ratio
+the split-block small batch path), the run path (reference bits, run correlation), candidate selection, exact re-score, pick and the ratio
 reduction; b2_sync_batch with and without the sub-batch pipeline.  Results are checked against the
 oracle so that a run under the sanitizer is also a parity run.
 """
@@ -92,6 +92,20 @@ def main():
         for k in env:
             os.environ.pop(k)
         assert all(np.array_equal(a, b) for a, b in zip(base, piped)), env
+    # the run path (the default for these cue-mode calls) against the overlap-save FFT path, per ratio too
+    for env in ({"B2_ALIGN_PATH": "runs"}, {"B2_ALIGN_PATH": "tiled"}):
+        os.environ.update(env)
+        other = bs.sync_host(*args)
+        for k in env:
+            os.environ.pop(k)
+        assert all(np.array_equal(a, b) for a, b in zip(base, other)), env
+    j_all = h.sync_batch(pcm, [0, n_win * 160, 2 * n_win * 160], 16000, 100, 0.0, 100000, -1, -1, np.tile(starts, 2),
+                         np.tile(ends, 2), None, cue_off, BENCH_RATIOS, 0.0, 6000, want_all=True)
+    os.environ["B2_ALIGN_PATH"] = "tiled"
+    j_fft = h.sync_batch(pcm, [0, n_win * 160, 2 * n_win * 160], 16000, 100, 0.0, 100000, -1, -1, np.tile(starts, 2),
+                         np.tile(ends, 2), None, cue_off, BENCH_RATIOS, 0.0, 6000, want_all=True)
+    os.environ.pop("B2_ALIGN_PATH")
+    assert all(np.array_equal(a, b) for a, b in zip(j_all, j_fft))
     h.synchronize()
     print("sanitize_smoke ok")
 
