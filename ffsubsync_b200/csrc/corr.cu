@@ -565,17 +565,18 @@ __global__ void __launch_bounds__(128) pick_kernel(const SelJob* __restrict__ jo
 
 // ---- diagnostics: b2_capture_nominations ----------------------------------------------------------
 // One CTA per job: the fp32 scores of its surviving window (m_lo..m_hi, offset o_first + m), its
-// (maximum, tau) and its candidate count, as the selection kernels left them.
+// (maximum, tau) and its candidate count, as the selection kernels left them.  scores_written: the run
+// path's kernel has written the window scores; only (maximum, epsilon) and the count are left.
 __global__ void __launch_bounds__(256) capture_nominations_kernel(const SelJob* __restrict__ jobs,
                                                                    const int* __restrict__ jlist,
                                                                    const float* __restrict__ scores,
                                                                    const float2* __restrict__ job_stat,
                                                                    const int* __restrict__ cand_cnt,
-                                                                   B2Capture cap, long long j0) {
+                                                                   B2Capture cap, long long j0, int scores_written) {
   const int j = jlist ? jlist[blockIdx.x] : (int)blockIdx.x;
   const SelJob job = jobs[j];
   const bool live = job.kind == 0 && job.m_lo <= job.m_hi;
-  if (live && !scores) return;  // written by the launch that has its scores
+  if (live && !scores && !scores_written) return;  // written by the launch that has its scores
   const long long g = j0 + j;
   const int n = live ? job.m_hi - job.m_lo + 1 : 0;
   if (threadIdx.x == 0) {
@@ -586,7 +587,7 @@ __global__ void __launch_bounds__(256) capture_nominations_kernel(const SelJob* 
     cap.stat[2 * g + 1] = s.y;
     cap.cand[g] = cand_cnt[j];
   }
-  if (n == 0) return;
+  if (n == 0 || scores_written) return;
   const float* c = scores + job.score_off + job.m_lo;
   float* out = cap.scores + g * cap.stride;
   for (int i = threadIdx.x; i < n; i += 256) out[i] = c[i];
@@ -624,10 +625,10 @@ int b2i_select_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n,
 }
 
 int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
-                       const B2CandBuffers& cb, long long j0) {
+                       const B2CandBuffers& cb, long long j0, bool scores_written) {
   if (n <= 0) return B2_OK;
   capture_nominations_kernel<<<(unsigned)n, 256, 0, h->stream>>>(d_sel, d_jlist, scores, cb.job_stat, cb.cand_cnt,
-                                                                  h->capture, j0);
+                                                                  h->capture, j0, scores_written ? 1 : 0);
   B2_CHECK_LAUNCH(h, "capture_nominations_kernel");
   return B2_OK;
 }
@@ -769,9 +770,10 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   }
   // Cue mode with the reference from this call's VAD (two levels, 1.0f and the label): the run path
   // (runcorr.cu) scores every offset of the window from the cue runs, exactly up to a float64 margin, when
-  // its work (cues x window) is below the FFT blocks it replaces for every live job.  A capture of the fp32
-  // nominations (b2_capture_nominations) probes the FFT paths and keeps them.
-  if (cue_mode && !capture && !use_big && std::isfinite(cue_src->ref_label) &&
+  // its work (cues x window) is below the FFT blocks it replaces for every live job.  A capture of the
+  // nominations (b2_capture_nominations) probes the FFT paths and keeps them, unless B2_ALIGN_PATH=runs asks
+  // for the run path (then its float64 scores are captured).
+  if (cue_mode && (!capture || force_runs) && !use_big && std::isfinite(cue_src->ref_label) &&
       !(path_env && !strcmp(path_env, "tiled"))) {
     bool fits = true, pays = true;
     int max_runs = 1;
@@ -795,7 +797,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
     if (fits && (pays || force_runs)) {
       const SelJob* d_sel_runs = nullptr;
       B2_TRY(b2i_align_runs(h, d_ref, ref_off, V, trk_off, K, sel, d_bits, max_runs, cue_src->ref_label, winner_only,
-                            cb, &d_sel_runs));
+                            cb, &d_sel_runs, capture_j0));
       return b2i_rescore_pick(h, d_sel_runs, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
     }
   }

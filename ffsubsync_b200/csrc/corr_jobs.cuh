@@ -85,16 +85,18 @@ int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_re
                      int32_t* d_status);
 // b2_capture_nominations (corr.cu): copies the window scores, job_stat and cand_cnt of n jobs into
 // h->capture at global index j0 + j, after the selection kernels.  Jobs d_jlist[0..n) (NULL: 0..n-1);
-// with scores == NULL only the jobs without a live window are written.
+// with scores == NULL only the jobs without a live window are written, unless scores_written (the run
+// path, whose kernel writes the scores itself): then every job's win / stat / cand are written.
 int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
-                       const B2CandBuffers& cb, long long j0);
+                       const B2CandBuffers& cb, long long j0, bool scores_written = false);
 // Run path (runcorr.cu): cue mode with a two-level reference (1.0f / ref_label).  sel: host copy of the jobs
 // as the planner left them (absolute offsets in m_lo / m_hi; this call rebases them on each job's own window),
 // subtitle bit masks in d_bits, at most max_runs cue runs per job.  Fills cand_off / cand_cnt / job_stat /
-// work_list / work_count like the selection; the caller then runs b2i_rescore_pick on *d_sel_out.
+// work_list / work_count like the selection; the caller then runs b2i_rescore_pick on *d_sel_out.  Under a
+// capture the float64 scores (rounded to float32), job_stat and cand_cnt go to it at global index capture_j0 + j.
 int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
                    std::vector<SelJob>& sel, const uint32_t* d_bits, int max_runs, float ref_label, int winner_only,
-                   const B2CandBuffers& cb, const SelJob** d_sel_out);
+                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0);
 // The run path is chosen per call when every live job has cues x window <= kRunCostPerBlock x (its FFT block
 // transforms): the break-even measured in the bench step on an H100 (DESIGN.md section 4, "K4r").
 // kRunMaxCues bounds the shared memory of a job's run table (3 ints per run).

@@ -96,13 +96,17 @@ __global__ void __launch_bounds__(1024) ref_bits_kernel(const float* __restrict_
 
 // One CTA per (track, ratio) job: blockDim.x / 32 >= ceil(window / 32) threads, thread t owning the offsets
 // o_lo + 32 t .. + 31.  Dynamic shared memory: 3 x max_runs ints (run starts, ends, lengths before).
+// CAPTURE (b2_capture_nominations): every score also goes, rounded to float32, to the capture row of the job
+// (cap.scores[(cap_j0 + j) * cap.stride + offset - o_lo]) from the loop that takes the maximum.
+template <bool CAPTURE>
 __global__ void __launch_bounds__(kMaxThreads) run_corr_kernel(const SelJob* __restrict__ sel,
                                                                 const long long* __restrict__ job_q,
                                                                 const uint2* __restrict__ q_all,
                                                                 const uint32_t* __restrict__ sub_bits,
                                                                 float ref_label, int max_runs,
                                                                 RunStat* __restrict__ stat,
-                                                                int* __restrict__ cand_off) {
+                                                                int* __restrict__ cand_off,
+                                                                B2Capture cap, long long cap_j0) {
   extern __shared__ int rsm[];
   int* ra = rsm;
   int* rb = ra + max_runs;
@@ -172,6 +176,7 @@ __global__ void __launch_bounds__(kMaxThreads) run_corr_kernel(const SelJob* __r
     for (int i = 0; i < 32; ++i) {
       if (i < n_mine) {
         const double g = rc_score(q, R, S, ra, rb, rl, nr, o0 + i, um, lv);
+        if (CAPTURE) cap.scores[(cap_j0 + j) * cap.stride + kOffsetsPerThread * tid + i] = (float)g;
         if (g >= best) {  // increasing offsets: ties go to the largest
           best = g;
           barg = o0 + i;
@@ -267,7 +272,7 @@ __global__ void __launch_bounds__(128) run_finalize_kernel(const SelJob* __restr
 
 int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
                    std::vector<SelJob>& sel, const uint32_t* d_bits, int max_runs, float ref_label, int winner_only,
-                   const B2CandBuffers& cb, const SelJob** d_sel_out) {
+                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0) {
   B2Range range("b2:align runs (ref_bits, run_corr, finalize)");
   const size_t J = sel.size();
   std::vector<RunRef> vids;
@@ -312,12 +317,16 @@ int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
   }
   max_runs = std::max(1, max_runs);
   const size_t smem = (size_t)3 * max_runs * sizeof(int);
-  B2_CUDA(h, cudaFuncSetAttribute(run_corr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  run_corr_kernel<<<(unsigned)J, (unsigned)max_thr, smem, h->stream>>>(d_sel, d_job_q, q, d_bits, ref_label, max_runs,
-                                                                      stat, cb.cand_off);
+  const bool capture = h->capture.scores != nullptr;
+  auto kernel = capture ? run_corr_kernel<true> : run_corr_kernel<false>;
+  B2_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)J, (unsigned)max_thr, smem, h->stream>>>(d_sel, d_job_q, q, d_bits, ref_label, max_runs, stat,
+                                                             cb.cand_off, h->capture, capture_j0);
   B2_CHECK_LAUNCH(h, "run_corr_kernel");
   B2_CUDA(h, cudaMemsetAsync(cb.work_count, 0, sizeof(int), h->stream));
   run_finalize_kernel<<<(unsigned)((J + 127) / 128), 128, 0, h->stream>>>(d_sel, (int)J, K, winner_only, stat, cb);
   B2_CHECK_LAUNCH(h, "run_finalize_kernel");
+  // the window scores are in the capture already: win / stat / cand as the finalize left them
+  if (capture) B2_TRY(b2i_capture_launch(h, d_sel, nullptr, (int)J, nullptr, cb, capture_j0, /*scores_written=*/true));
   return B2_OK;
 }

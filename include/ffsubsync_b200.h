@@ -227,7 +227,12 @@ int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /* [V
  *   scores[j*stride + i]  fp32 score of offset win[2j] + i, 0 <= i < win[2j+1]
  * The arrays must hold B*K entries (x2 for win and stat).  A window longer than stride fails the call
  * with B2_ERR_BAD_ARG.  scores == NULL clears the capture.  Not for production use: each capture costs
- * one extra launch per alignment (per group of the large-window path). */
+ * one extra launch per alignment (per group of the large-window path).
+ * A capture keeps cue-mode calls on the FFT paths, unless the environment sets B2_ALIGN_PATH=runs and the
+ * run path fits the call; then the fields hold the run path's nomination stage:
+ *   scores                its float64 score of each offset (exact counts, see DESIGN.md 4 "K4r"), rounded to fp32
+ *   stat[2j], stat[2j+1]  float64 maximum and margin epsilon in place of tau, both rounded to fp32
+ *   cand[j]               offsets with score >= max - epsilon (uncapped count); -1 = B2_ALIGN_APPROX */
 int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* win, float* stat,
                            int32_t* cand);
 

@@ -28,8 +28,12 @@ int main(int argc, char** argv) {
   fclose(f);
   if (W < 1 || W > kMaxWindow) return 5;
 
-  // packed reference, laid out as ref_bits_kernel writes it
-  std::vector<uint2> q(rc_ref_entries(R));
+  // packed reference, laid out as ref_bits_kernel writes it, between kPoison poison entries on each side
+  // (every bit set, a huge prefix): a read outside q[0] .. q[(R >> 5) + 2] changes a score or a UM count
+  constexpr int kPoison = 64;
+  const long long n_q = rc_ref_entries(R);
+  std::vector<uint2> q_guarded(n_q + 2 * kPoison, make_uint2(0xffffffffu, 0x40000000u));
+  uint2* q = q_guarded.data() + kPoison;
   q[0] = make_uint2(0u, 0u);
   int below = 0;
   for (int w = 0; w <= (R >> 5) + 1; ++w) {
@@ -65,12 +69,12 @@ int main(int argc, char** argv) {
     const int o0 = o_lo + kOffsetsPerThread * tid;
     const int n_mine = W - kOffsetsPerThread * tid < kOffsetsPerThread ? W - kOffsetsPerThread * tid : kOffsetsPerThread;
     int cnt[32], base;
-    rc_thread_counts(q.data(), R, ra.data(), rb.data(), nr, o0, cnt, base);
+    rc_thread_counts(q, R, ra.data(), rb.data(), nr, o0, cnt, base);
     int um = base;
     for (int i = 0; i < n_mine; ++i) {
       const int m = kOffsetsPerThread * tid + i;
       um_out[m] = um;
-      score[m] = rc_score(q.data(), R, S, ra.data(), rb.data(), rl.data(), nr, o0 + i, um, l);
+      score[m] = rc_score(q, R, S, ra.data(), rb.data(), rl.data(), nr, o0 + i, um, l);
       um += cnt[i] - nr;
     }
   }

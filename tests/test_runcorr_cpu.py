@@ -196,6 +196,21 @@ def test_widest_window():
     _check(m, u, R - 16000, 32 * 1024, 0.96, 0.3)
 
 
+@pytest.mark.parametrize("n_runs", [7, 8, 14, 15])
+def test_anticorrelated_reference_fills_the_counters(n_runs):
+    """A reference that is the complement of the mask at a planted offset: speech just after every run end,
+    silence at every run start, so every run adds 2 to the same 4-bit counter (7 runs fill it to 14; the
+    flush every kRunsPerFlush runs must come before it wraps).  Run counts on both sides of the flushes."""
+    rng = np.random.RandomState(n_runs)
+    S, R, o_star = 600, 2000, 777
+    u = _runs(S, [(20 + 40 * i, 1 + i % 5) for i in range(n_runs)])
+    m = (rng.rand(R) < 0.5).astype(np.uint8)
+    m[o_star:o_star + S] = 1 - u
+    for level, label in [(1.0, 0.0), (0.96, 0.3)]:
+        score, _ = _check(m, u, o_star - 100, 224, level, label)
+    assert score[100] == score.min()   # every frame disagrees at the planted offset (last call: level 0.96)
+
+
 def test_two_hour_bound_size():
     """eps for a 2 h pair (720 000 frames each side) is about 1e-4 - the figure DESIGN.md quotes."""
     rng = np.random.RandomState(4)
