@@ -10,6 +10,7 @@
 #include <thread>
 
 #include "common.cuh"
+#include "raster_math.cuh"
 
 // Entry guard: the handle's device is current for the duration of the call and the caller
 // thread's previous device is restored on every return path.
@@ -682,35 +683,107 @@ extern "C" int b2_synth_pcm(b2_handle h, const uint8_t* window_class, int64_t n_
 }
 
 // ---- rasteriser ----------------------------------------------------------------------------
-static double scaled_seconds_host(double t, double ratio) {
-  // timedelta(seconds=t*ratio).total_seconds(): see raster.cu (same arithmetic, host copy used
-  // only to size the output arrays).
-  volatile double x = t * ratio;
-  double whole;
-  double frac = modf(x, &whole);
-  volatile double fus = frac * 1e6;
-  long long us = (long long)whole * 1000000LL + (long long)nearbyint(fus);
-  return (double)us / 1e6;
+// Bits of |x| as an integer: ordered like |x| for every double, with inf above every finite value and
+// NaN above inf, so one integer maximum over a cue array finds its largest or non-finite time.
+static inline uint64_t magnitude_bits(double x) {
+  uint64_t u;
+  memcpy(&u, &x, 8);
+  return u & 0x7fffffffffffffffull;
 }
 
-extern "C" int b2_rasterize_lengths(const double* cue_end_s, const int64_t* cue_off, int B,
-                                    const double* ratios, int K, int per_pair_ratios,
-                                    int sample_rate, int64_t* lengths) {
+static inline double from_bits(uint64_t u) {
+  double x;
+  memcpy(&x, &u, 8);
+  return x;
+}
+
+// The cue arithmetic (raster_math.cuh) reproduces the reference for finite times with
+// |t| * ratio < B2_MAX_CUE_SECONDS; fl(|t| * r) is monotone in |t| and r, so the largest magnitude and
+// the largest ratio of a pair decide.  NaN and inf fail the comparison.
+static inline bool cue_magnitude_ok(uint64_t max_bits, double r_max) {
+  return from_bits(max_bits) * r_max < B2_MAX_CUE_SECONDS;
+}
+
+static inline bool ratio_ok(double r) { return r > 0.0 && r < INFINITY; }
+
+// Why the cues of pairs [0, B) cannot be rasterised exactly, or nullptr: start_seconds, a ratio that is
+// not finite and positive, or a cue time (start or end; either array may be null = not checked) beyond
+// the limit above.  For non-finite times the reference raises in timedelta.  Metadata cues count: the
+// reference scales them too.  *at: the offending ratio or cue index, *val its value.
+static const char* bad_cue_input(const double* cue_start_s, const double* cue_end_s, const int64_t* cue_off,
+                                 int B, const double* ratios, int K, int per_pair_ratios, double start_seconds,
+                                 int64_t* at, double* val) {
+  *at = -1;
+  *val = start_seconds;
+  if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS)) return "start_seconds is not finite or too large";
+  for (int b = 0; b < B; ++b) {
+    double r_max = 0.0;
+    for (int k = 0; k < K; ++k) {
+      const size_t i = per_pair_ratios ? (size_t)b * K + k : (size_t)k;
+      *at = (int64_t)i;
+      *val = ratios[i];
+      if (!ratio_ok(ratios[i])) return "ratio is not a finite positive number";
+      r_max = std::max(r_max, ratios[i]);
+    }
+    const int64_t c0 = cue_off[b], c1 = cue_off[b + 1];
+    for (const double* t : {cue_start_s, cue_end_s}) {
+      if (!t) continue;
+      // one branch-free pass (four independent chains); the offending cue is looked for only on failure
+      uint64_t m4[4] = {0, 0, 0, 0};
+      int64_t c = c0;
+      for (; c + 4 <= c1; c += 4)
+        for (int i = 0; i < 4; ++i) m4[i] = std::max(m4[i], magnitude_bits(t[c + i]));
+      for (; c < c1; ++c) m4[0] = std::max(m4[0], magnitude_bits(t[c]));
+      if (cue_magnitude_ok(std::max(std::max(m4[0], m4[1]), std::max(m4[2], m4[3])), r_max)) continue;
+      for (int64_t c = c0; c < c1; ++c)
+        if (!cue_magnitude_ok(magnitude_bits(t[c]), r_max)) {
+          *at = c;
+          *val = t[c];
+          return t == cue_start_s ? "cue start time times ratio is not finite or too large"
+                                  : "cue end time times ratio is not finite or too large";
+        }
+    }
+  }
+  return nullptr;
+}
+
+// b2_rasterize_lengths, also checking the start times when cue_start_s is not null (b2_sync_batch: one
+// pass over the cues for both)
+static int rasterize_lengths(const double* cue_start_s, const double* cue_end_s, const int64_t* cue_off, int B,
+                             const double* ratios, int K, int per_pair_ratios, int sample_rate, int64_t* lengths) {
   if (B < 0 || K < 0 || !cue_off || (!ratios && K) || !lengths || sample_rate <= 0)
     return B2_ERR_BAD_ARG;
   for (int b = 0; b < B; ++b) {
     // max over cues of scaled(end) == scaled(max end) for ratio > 0: the product, the microsecond
-    // rounding and the division are all monotone non-decreasing (speech_transformers.py:958-960)
-    double max_end = 0.0;
-    bool any = false;
-    for (int64_t c = cue_off[b]; c < cue_off[b + 1]; ++c)
-      if (!any || cue_end_s[c] > max_end) { max_end = cue_end_s[c]; any = true; }
+    // rounding and the division are all monotone non-decreasing (speech_transformers.py:958-960).
+    // The same pass finds the largest magnitude for the input check (see bad_cue_input).
+    // (four independent chains: this runs over every cue of every b2_sync_batch call).  A NaN end
+    // fails the check, so max_end may ignore it.
+    const int64_t c0 = cue_off[b], c1 = cue_off[b + 1];
+    const bool any = c1 > c0;
+    double e4[4];
+    uint64_t m4[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 4; ++i) e4[i] = any ? cue_end_s[c0] : 0.0;
+    int64_t c = c0;
+    for (; c + 4 <= c1; c += 4)
+      for (int i = 0; i < 4; ++i) {
+        e4[i] = std::max(e4[i], cue_end_s[c + i]);
+        m4[i] = std::max(m4[i], magnitude_bits(cue_end_s[c + i]));
+        if (cue_start_s) m4[i] = std::max(m4[i], magnitude_bits(cue_start_s[c + i]));
+      }
+    for (; c < c1; ++c) {
+      e4[0] = std::max(e4[0], cue_end_s[c]);
+      m4[0] = std::max(m4[0], magnitude_bits(cue_end_s[c]));
+      if (cue_start_s) m4[0] = std::max(m4[0], magnitude_bits(cue_start_s[c]));
+    }
+    const double max_end = std::max(std::max(e4[0], e4[1]), std::max(e4[2], e4[3]));
+    const uint64_t m = std::max(std::max(m4[0], m4[1]), std::max(m4[2], m4[3]));
     for (int k = 0; k < K; ++k) {
       double r = per_pair_ratios ? ratios[(size_t)b * K + k] : ratios[k];
-      if (!(r > 0.0)) return B2_ERR_BAD_ARG;
+      if (!ratio_ok(r) || !cue_magnitude_ok(m, r)) return B2_ERR_BAD_ARG;
       double max_time = 0.0;
       if (any) {
-        double e = scaled_seconds_host(max_end, r);
+        double e = b2_scaled_seconds(max_end, r);
         if (e > max_time) max_time = e;
       }
       volatile double prod = max_time * (double)sample_rate;
@@ -718,6 +791,12 @@ extern "C" int b2_rasterize_lengths(const double* cue_end_s, const int64_t* cue_
     }
   }
   return B2_OK;
+}
+
+extern "C" int b2_rasterize_lengths(const double* cue_end_s, const int64_t* cue_off, int B,
+                                    const double* ratios, int K, int per_pair_ratios,
+                                    int sample_rate, int64_t* lengths) {
+  return rasterize_lengths(nullptr, cue_end_s, cue_off, B, ratios, K, per_pair_ratios, sample_rate, lengths);
 }
 
 extern "C" int b2_rasterize(b2_handle h, const double* cue_start_s, const double* cue_end_s,
@@ -731,6 +810,11 @@ extern "C" int b2_rasterize(b2_handle h, const double* cue_start_s, const double
   if (B == 0 || K == 0) return B2_OK;
   if (!ratios || (cue_off[B] && (!cue_start_s || !cue_end_s)))
     B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize: null cue/ratio arrays");
+  int64_t at;
+  double val;
+  if (const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, B, ratios, K, per_pair_ratios,
+                                      start_seconds, &at, &val))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize: %s (index %lld: %g)", why, (long long)at, val);
   int64_t total = out_off[(size_t)B * K];
   if (total && !out) B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize: null output");
   float* d_out = out;
@@ -942,8 +1026,15 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
     ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
   }
-  if (b2_rasterize_lengths(cue_end_s, cue_off, T, ratios, K, 0, sample_rate, lengths.data()) != B2_OK)
-    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad cue list / ratios", who);
+  // the lengths pass checks the cue times and ratios too; the offending input is looked for on failure
+  if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
+      rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, ratios, K, 0, sample_rate, lengths.data()) != B2_OK) {
+    int64_t bad_at;
+    double bad_val;
+    const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, T, ratios, K, 0, start_seconds, &bad_at, &bad_val);
+    if (!why) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad cue list / ratios", who);
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: %s (index %lld: %g)", who, why, (long long)bad_at, bad_val);
+  }
   sub_off[0] = 0;
   for (size_t j = 0; j < J; ++j) sub_off[j + 1] = sub_off[j] + lengths[j];
 

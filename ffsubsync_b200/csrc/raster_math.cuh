@@ -1,28 +1,78 @@
-// Bit-exact device restatement of the reference's cue arithmetic, shared by the stand-alone
-// rasteriser (raster.cu) and the correlation kernel that rasterises subtitle blocks on the fly
-// (corr.cu).  Reference: SubtitleScaler.fit (ffsubsync/subtitle_transformers.py:35-47) +
-// SubtitleSpeechTransformer.fit (ffsubsync/speech_transformers.py:957-980).
+// Bit-exact restatement of the reference's cue arithmetic, shared by both rasterisers (raster.cu:
+// raster_cues_kernel, raster_bits_kernel), by b2_rasterize_lengths on the host (api.cu) and by the
+// CPU emulator tests/host_emul/raster_emul.cu.  Reference: SubtitleScaler.fit
+// (ffsubsync/subtitle_transformers.py:35-47) + SubtitleSpeechTransformer.fit
+// (ffsubsync/speech_transformers.py:957-980).
+//
+// Valid for finite times with |t * ratio| < B2_MAX_CUE_SECONDS and |start_seconds| below it too: there
+// every microsecond count is an exact double, so (double)us / 1e6 is the correctly rounded quotient
+// Python's int / int gives.  Callers reject everything else (api.cu) - the reference raises in
+// timedelta for non-finite times, and beyond 2^63 us the integer product below overflows.
+// On the host the intrinsics are the plain IEEE operations; the host half must be compiled without
+// FMA contraction (-ffp-contract=off).
 #pragma once
+#include <math.h>
+
 #include <cuda_runtime.h>
+
+// 2^53 microseconds (about 285 years) in seconds
+#define B2_MAX_CUE_SECONDS 9007199254.740992
+
+#ifdef __CUDACC__
+#define RASTER_HD __host__ __device__ __forceinline__
+#else
+#define RASTER_HD inline
+#endif
+
+RASTER_HD double b2_rm_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+RASTER_HD double b2_rm_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+
+RASTER_HD double b2_rm_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+RASTER_HD long long b2_rm_rint(double x) {  // half-to-even (the host's default rounding mode)
+#ifdef __CUDA_ARCH__
+  return __double2ll_rn(x);
+#else
+  return llrint(x);
+#endif
+}
 
 // timedelta(seconds=t*ratio).total_seconds(): whole seconds exact, fractional part * 1e6 rounded
 // half-to-even to integer microseconds, then one correctly rounded division (no FMA contraction).
-__device__ __forceinline__ double b2_scaled_seconds(double t, double ratio) {
-  const double x = __dmul_rn(t, ratio);
+RASTER_HD double b2_scaled_seconds(double t, double ratio) {
+  const double x = b2_rm_mul(t, ratio);
   double whole;
   const double frac = modf(x, &whole);
-  const long long us = (long long)whole * 1000000LL + __double2ll_rn(__dmul_rn(frac, 1e6));
-  return __ddiv_rn((double)us, 1e6);
+  const long long us = (long long)whole * 1000000LL + b2_rm_rint(b2_rm_mul(frac, 1e6));
+  return b2_rm_div((double)us, 1e6);
 }
 
 // samples[first:last] of a length-n array with Python slice semantics (negative index wraps once).
-__device__ __forceinline__ void b2_cue_bounds(double start_s, double end_s, double ratio,
-                                              double start_seconds, int sample_rate, long long n,
-                                              long long& first, long long& last) {
+RASTER_HD void b2_cue_bounds(double start_s, double end_s, double ratio, double start_seconds,
+                             int sample_rate, long long n, long long& first, long long& last) {
   const double st = b2_scaled_seconds(start_s, ratio);
   const double en = b2_scaled_seconds(end_s, ratio);
-  first = __double2ll_rn(__dmul_rn(__dsub_rn(st, start_seconds), (double)sample_rate));
-  last = first + __double2ll_rn(__dmul_rn(__dsub_rn(en, st), (double)sample_rate));
+  first = b2_rm_rint(b2_rm_mul(b2_rm_sub(st, start_seconds), (double)sample_rate));
+  last = first + b2_rm_rint(b2_rm_mul(b2_rm_sub(en, st), (double)sample_rate));
   if (first < 0) { first += n; if (first < 0) first = 0; } else if (first > n) first = n;
   if (last < 0) { last += n; if (last < 0) last = 0; } else if (last > n) last = n;
 }

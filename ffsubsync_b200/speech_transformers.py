@@ -187,7 +187,13 @@ class ComputeSpeechFrameBoundariesMixin:
         return self.end_frame_ - self.start_frame_
 
     def fit_boundaries(self, speech_frames: np.ndarray) -> "ComputeSpeechFrameBoundariesMixin":
-        x = np.asarray(speech_frames, dtype=np.float32)
+        # the kernel tests float32 x > 0.5f; rounding the float64 signal UP to float32 keeps the
+        # reference's float64 test (0.5 is a float32, so x > 0.5 <=> round_up(x) > 0.5): a level of
+        # 0.500000005 (ratio 1.99999998) would round to nearest 0.5f and find no speech
+        x64 = np.asarray(speech_frames, dtype=np.float64)
+        x = x64.astype(np.float32)
+        low = x < x64
+        x[low] = np.nextafter(x[low], np.float32(np.inf))
         if len(x):
             first, last = _native.get_handle().first_last_nonzero(x, [0, len(x)])
             if last[0] >= 0:

@@ -138,7 +138,11 @@ int b2_vad_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int 
  * ratio ratios[b*K+k] when per_pair_ratios != 0, else ratios[k].  The written level is
  * min(1/ratio, 1) (speech_transformers.py:977) unless levels (same shape as ratios) is given:
  * SubtitleSpeechTransformer alone = ratios of 1.0 (times already scaled) + levels.
- * b2_rasterize_lengths computes len = int(max_end*sample_rate)+2 per (b,k) on the host. */
+ * b2_rasterize_lengths computes len = int(max_end*sample_rate)+2 per (b,k) on the host.
+ * The cue arithmetic is the reference's bit for bit for finite positive ratios, finite cue times t with
+ * |t|*ratio < 2^53 us (9007199254.740992 s, about 285 years) and |start_seconds| below the same limit;
+ * everything else (the reference raises in timedelta for non-finite times) is B2_ERR_BAD_ARG, here and
+ * in b2_sync_batch / b2_sync_tracks.  Metadata cues (keep == 0) are checked too. */
 int b2_rasterize_lengths(const double* cue_end_s, const int64_t* cue_off, int B,
                          const double* ratios, int K, int per_pair_ratios, int sample_rate,
                          int64_t* lengths /* [B*K] */);
