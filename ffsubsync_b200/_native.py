@@ -28,8 +28,9 @@ EXPORTS = [
     "b2_rasterize_lengths", "b2_rasterize", "b2_blend_signals", "b2_first_last_nonzero", "b2_align_batch",
     "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
-    "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks",
+    "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
 ]
+GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
 
 
 class NativeError(RuntimeError):
@@ -87,6 +88,10 @@ def load() -> ctypes.CDLL:
         lib.b2_sync_tracks.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                        _f32, _i64, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, _vp,
                                        ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_sync_tracks_gss.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_int, _f32, _i64, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp,
+                                           _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                           ctypes.c_int]
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -416,6 +421,47 @@ class Handle:
                                      _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset), memspace)
         self._check(st, "b2_sync_tracks")
         return best_score, best_offset, best_k, all_score, all_offset
+
+    def sync_tracks_gss(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
+                        energy_threshold: int, z_lo: int, z_hi: int, cue_start_s, cue_end_s, cue_keep,
+                        cue_off, ratios, start_seconds: float, max_offset_samples: Optional[int],
+                        best_score=None, best_offset=None, best_k=None, all_score=None, all_offset=None,
+                        gss_ratio=None, gss_evals=None, want_all: bool = False, want_evals: bool = False,
+                        memspace: int = B2_HOST):
+        """sync_tracks with the golden-section search as candidate K (b2_sync_tracks_gss).  Outputs per track:
+        best_* [T] (best_k == K: the search won), all_* [T*(K+1)] (column K: the search's candidate),
+        gss_ratio [T] (NaN for an empty reference), gss_evals [T*17].  Raises NativeError with status
+        B2_ERR_UNSUPPORTED (-6) outside the envelope of the device-driven rounds."""
+        pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        V, T = len(pcm_off) - 1, len(track_video)
+        if len(cue_off) != T + 1:
+            raise NativeError(-1, "b2_sync_tracks_gss", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        K = len(ratios)
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
+        mos = _mask_width(max_offset_samples)
+        if memspace == B2_HOST:
+            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
+            best_score = np.empty(T, dtype=np.float64)
+            best_offset = np.empty(T, dtype=np.int32)
+            best_k = np.empty(T, dtype=np.int32)
+            gss_ratio = np.empty(T, dtype=np.float64)
+            if want_all:
+                all_score = np.empty(T * (K + 1), dtype=np.float64)
+                all_offset = np.empty(T * (K + 1), dtype=np.int32)
+            if want_evals:
+                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
+        st = self.lib.b2_sync_tracks_gss(self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate,
+                                         sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
+                                         int(z_hi), _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep),
+                                         _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos,
+                                         _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(all_score),
+                                         _ptr(all_offset), _ptr(gss_ratio), _ptr(gss_evals), memspace)
+        self._check(st, "b2_sync_tracks_gss")
+        return best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals
 
     # -- diagnostics (tests) --------------------------------------------------------------------
     @contextlib.contextmanager

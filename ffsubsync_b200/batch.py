@@ -30,13 +30,29 @@ def load_serialized_speech(paths, non_speech_label: float = 0.0):
     return (np.concatenate(sigs) if sigs else np.zeros(0, np.float32)), off
 
 
+def _is_unsupported(e: Exception) -> bool:
+    return isinstance(e, _native.NativeError) and e.status == -6   # B2_ERR_UNSUPPORTED
+
+
 class BatchSynchronizer:
-    def __init__(self, ratios: Sequence[float], frame_rate: int = 16000, sample_rate: int = SAMPLE_RATE,
+    """``ratios``: the framerate ratio grid in list order.  A trailing ``None`` adds the golden-section search
+    over [0.9, 1.1] as one more candidate, last in list order, the way the reference's list carries ``--gss``
+    (``constants.framerate_ratios_to_try(gss=True)``); results then gain ``gss_ratio`` and ``best_k == K``
+    (K = the grid's length) means the search won."""
+
+    def __init__(self, ratios: Sequence[Optional[float]], frame_rate: int = 16000, sample_rate: int = SAMPLE_RATE,
                  non_speech_label: float = 0.0, energy_threshold: int = DEFAULT_ENERGY_THRESHOLD,
                  z_lo: int = -1, z_hi: int = -1, start_seconds: float = 0.0,
                  max_offset_seconds: Optional[float] = DEFAULT_MAX_OFFSET_SECONDS,
                  device: Optional[int] = None) -> None:
-        self.ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        ratios = list(ratios)
+        self.gss = bool(ratios) and ratios[-1] is None
+        grid = ratios[:-1] if self.gss else ratios
+        if any(r is None for r in grid):
+            raise ValueError("None (the golden-section search) may only be the last entry of ratios")
+        if self.gss and not grid:
+            raise ValueError("the golden-section search (None) needs at least one grid ratio before it")
+        self.ratios = np.ascontiguousarray(grid, dtype=np.float64)
         self.frame_rate = frame_rate
         self.sample_rate = sample_rate
         self.non_speech_label = non_speech_label
@@ -65,6 +81,9 @@ class BatchSynchronizer:
         B = len(pcm_off) - 1
         K = len(self.ratios)
         dev = pcm.device
+        if self.gss:   # the identity track map: pair b is track b of video b
+            return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
+                                           cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident)
         if out is None:
             out = {"best_score": torch.empty(B, dtype=torch.float64, device=dev),
                    "best_offset": torch.empty(B, dtype=torch.int32, device=dev),
@@ -88,7 +107,9 @@ class BatchSynchronizer:
         video's PCM is read and run through the VAD once, however many tracks it has.  out: optional dict
         of CUDA tensors best_score f64[T], best_offset i32[T], best_k i32[T]; all_out: optional
         {"score": f64[T*K], "offset": i32[T*K]}.  Returns out; nothing is synchronised.  inputs_resident
-        as for sync_device (resident calls of both methods chain with each other)."""
+        as for sync_device (resident calls of both methods chain with each other).
+        With the golden-section search (a trailing None in ratios) out also holds gss_ratio f64[T] and all_out
+        is {"score": f64[T*(K+1)], "offset": i32[T*(K+1)]} with column K the search's candidate."""
         import torch
         T = len(track_video)
         dev = pcm.device
@@ -96,8 +117,29 @@ class BatchSynchronizer:
             out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
                    "best_offset": torch.empty(T, dtype=torch.int32, device=dev),
                    "best_k": torch.empty(T, dtype=torch.int32, device=dev)}
+        if self.gss and "gss_ratio" not in out:
+            out["gss_ratio"] = torch.empty(T, dtype=torch.float64, device=dev)
         a_s = all_out["score"].data_ptr() if all_out else None
         a_o = all_out["offset"].data_ptr() if all_out else None
+        if self.gss:
+            try:
+                self.handle.sync_tracks_gss(
+                    pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
+                    self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
+                    self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
+                    out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o, out["gss_ratio"].data_ptr(),
+                    memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+            except _native.NativeError as e:
+                if not _is_unsupported(e):
+                    raise
+                res = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep,
+                                        want_all=all_out is not None)
+                for key, v in zip(("best_score", "best_offset", "best_k", "gss_ratio"), res[:4]):
+                    out[key].copy_(torch.from_numpy(v))
+                if all_out:
+                    all_out["score"].copy_(torch.from_numpy(res[4]))
+                    all_out["offset"].copy_(torch.from_numpy(res[5]))
+            return out
         self.handle.sync_tracks(
             pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
             self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
@@ -110,7 +152,21 @@ class BatchSynchronizer:
                          want_all=False):
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
-        track."""
+        track, and gss_ratio last with the golden-section search."""
+        if self.gss:
+            try:
+                r = self.handle.sync_tracks_gss(
+                    pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
+                    self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
+                    self.start_seconds, self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
+                res = r[:5] + (r[5],)
+            except _native.NativeError as e:
+                if not _is_unsupported(e):
+                    raise
+                bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end,
+                                                                cue_off, cue_keep, want_all=want_all)
+                res = (bs, bo, bk, a_s, a_o, ratio)
+            return res if want_all else res[:3] + res[5:]
         res = self.handle.sync_tracks(
             pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
             self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
@@ -122,7 +178,9 @@ class BatchSynchronizer:
         back to back; numpy array or CUDA tensor) instead of PCM - the replay path of the
         reference's test-case bundles: ``ref.npz{"speech"}`` + ``in.srt``
         (ffsubsync/ffsubsync.py:338-343,639-644; DeserializeSpeechTransformer).
-        Returns (best_score f64[B], best_offset i32[B], best_k i32[B]) as numpy arrays."""
+        Returns (best_score f64[B], best_offset i32[B], best_k i32[B]) as numpy arrays, and gss_ratio f64[B]
+        last with the golden-section search (gss_batch.gss_align_batch on the same signals, merged as
+        candidate K by gss_batch.combine_gss)."""
         import torch
         h = self.handle
         ref_off = np.ascontiguousarray(ref_off, dtype=np.int64)
@@ -148,7 +206,14 @@ class BatchSynchronizer:
                         best_score=bs.data_ptr(), best_offset=bo.data_ptr(), best_k=bk.data_ptr(),
                         memspace=_native.B2_DEVICE)
         h.synchronize()
-        return bs.cpu().numpy(), bo.cpu().numpy(), bk.cpu().numpy()
+        if not self.gss:
+            return bs.cpu().numpy(), bo.cpu().numpy(), bk.cpu().numpy()
+        from .gss_batch import combine_gss, gss_align_batch
+        g = gss_align_batch(ref, ref_off, cue_start, cue_end, cue_off, cue_keep, self.max_offset_samples,
+                            self.sample_rate, self.start_seconds, handle=h)
+        bs, bo, bk, ratio, _, _ = combine_gss(bs.cpu().numpy(), bo.cpu().numpy(), bk.cpu().numpy(), g, K,
+                                              self.max_offset_samples)
+        return bs, bo, bk, ratio
 
     def sync_device_candidate_sharded(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None,
                                       rank: int = 0, world: int = 1, group=None):
@@ -160,9 +225,13 @@ class BatchSynchronizer:
         (NCCL, 24 B per candidate) and b2_reduce_ratios applies the |offset| filter and the
         first-in-list tie rule on every rank, so all ranks hold the same (score, offset, ratio index)
         as a single-GPU run.  pcm: int16 CUDA tensor, same on every rank.  Returns CUDA tensors
-        (best_score f64[B], best_offset i32[B], best_k i32[B])."""
+        (best_score f64[B], best_offset i32[B], best_k i32[B]).  Not available with the golden-section search:
+        its 17 evaluations are sequential per pair, so they cannot be dealt over ranks like grid candidates."""
         import torch
         from . import distributed
+        if self.gss:
+            raise ValueError("sync_device_candidate_sharded shards the ratio grid; it does not run the "
+                             "golden-section search (None in ratios)")
         h = self.handle
         self.use_torch_stream()   # torch ops and NCCL below are ordered against our kernels by the stream
         pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
@@ -206,9 +275,47 @@ class BatchSynchronizer:
 
     def sync_host(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None, want_all=False):
         """pcm: int16 numpy array (ideally backed by pinned memory).  Blocks until results are on
-        the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset])."""
+        the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]), and gss_ratio last
+        with the golden-section search."""
+        if self.gss:
+            return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
+                                         cue_end, cue_off, cue_keep, want_all=want_all)
         res = self.handle.sync_batch(
             pcm, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold,
             self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds,
             self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
         return res if want_all else res[:3]
+
+    def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False):
+        """The golden-section search outside the envelope of b2_sync_tracks_gss, composed of the public steps:
+        the VAD (b2_vad_energy_zcr), the grid (b2_sync_tracks), gss_align_batch on each track's reference
+        signal and the reference's combine.  pcm: int16 numpy array or CUDA tensor.  Returns numpy arrays
+        (best_score, best_offset, best_k, gss_ratio, all_score, all_offset) (all_* None unless want_all)."""
+        import torch
+        from .gss_batch import combine_gss, gss_align_batch
+        h = self.handle
+        pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        K = len(self.ratios)
+        on_device = not isinstance(pcm, np.ndarray)
+        if on_device:
+            h.synchronize()
+            torch.cuda.synchronize(pcm.device)
+            pcm_host = pcm.cpu().numpy()
+        else:
+            pcm_host = pcm
+        grid = h.sync_tracks(pcm_host, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end,
+                             cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples,
+                             want_all=True, memspace=_native.B2_HOST)
+        ref, ref_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                                        self.energy_threshold, self.z_lo, self.z_hi)
+        # one copy of its video's reference signal per track
+        parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
+        t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
+        t_ref = np.concatenate(parts).astype(np.float32) if parts else np.zeros(0, np.float32)
+        g = gss_align_batch(t_ref, t_off, cue_start, cue_end, cue_off, cue_keep, self.max_offset_samples,
+                            self.sample_rate, self.start_seconds, handle=h)
+        bs, bo, bk, ratio, a_s, a_o = combine_gss(grid[0], grid[1], grid[2], g, K, self.max_offset_samples,
+                                                  grid[3], grid[4])
+        return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))

@@ -5,11 +5,14 @@
 #include <math.h>
 
 #include <chrono>
+#include <cmath>
 #include <algorithm>
 #include <atomic>
 #include <thread>
 
 #include "common.cuh"
+#include "corr_jobs.cuh"
+#include "job_plan.cuh"
 #include "raster_math.cuh"
 
 // Entry guard: the handle's device is current for the duration of the call and the caller
@@ -781,13 +784,7 @@ static int rasterize_lengths(const double* cue_start_s, const double* cue_end_s,
     for (int k = 0; k < K; ++k) {
       double r = per_pair_ratios ? ratios[(size_t)b * K + k] : ratios[k];
       if (!ratio_ok(r) || !cue_magnitude_ok(m, r)) return B2_ERR_BAD_ARG;
-      double max_time = 0.0;
-      if (any) {
-        double e = b2_scaled_seconds(max_end, r);
-        if (e > max_time) max_time = e;
-      }
-      volatile double prod = max_time * (double)sample_rate;
-      lengths[(size_t)b * K + k] = (int64_t)prod + 2;  // speech_transformers.py:962
+      lengths[(size_t)b * K + k] = b2_signal_length(any ? max_end : 0.0, r, sample_rate);
     }
   }
   return B2_OK;
@@ -989,10 +986,11 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
                             const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
                             const int64_t* cue_off, const double* ratios, int K, double start_seconds,
                             int64_t max_offset_samples, double* best_score, int32_t* best_offset,
-                            int32_t* best_k, double* all_score, int32_t* all_offset, int memspace) {
+                            int32_t* best_k, double* all_score, int32_t* all_offset, int memspace,
+                            bool gss = false, double* gss_ratio = nullptr, double* gss_evals = nullptr) {
   const bool resident = memspace == B2_DEVICE_RESIDENT;
   if (resident) memspace = B2_DEVICE;
-  const char* who = track_video ? "sync_tracks" : "sync_batch";
+  const char* who = gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
   if (V < 0 || T < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
     B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad arguments", who);
   if (track_video) {
@@ -1003,8 +1001,23 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     for (int t = 0; t < T; ++t)
       if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: cue_off not monotone at %d", t);
   }
+  if (gss) {
+    // the envelope of the device-driven rounds (DESIGN.md section 4 "K8g"): every round runs on the run path
+    // (compared with half the window bound: 2 * max_offset_samples overflows for widths from 2^62 on)
+    if (max_offset_samples == B2_MAX_OFFSET_NONE || max_offset_samples < 0 ||
+        max_offset_samples > (int64_t)(kRunMaxWindow / 2))
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: max_offset_samples must lie in [0, %d] (a window of at most "
+              "2 max_offset_samples <= %d offsets, one CTA of the run path)", kRunMaxWindow / 2, kRunMaxWindow);
+    if (!std::isfinite(non_speech_label))
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: non_speech_label must be finite (the run path's two-level reference)");
+    for (int t = 0; t < T; ++t)
+      if (cue_off[t + 1] - cue_off[t] > kRunMaxCues)
+        B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: track %d has %lld cues, more than %d", t,
+                (long long)(cue_off[t + 1] - cue_off[t]), kRunMaxCues);
+  }
   if (T == 0) return B2_OK;
   if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null output", who);
+  if (gss && !gss_ratio) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null gss_ratio", who);
   const int fpw = b2_vad_frames_per_window(frame_rate, sample_rate);
   if (fpw <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
   if (z_lo < 0) z_lo = 0;
@@ -1037,6 +1050,24 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   }
   sub_off[0] = 0;
   for (size_t j = 0; j < J; ++j) sub_off[j + 1] = sub_off[j] + lengths[j];
+  // GSS: each track's largest cue end (its signal length at any ratio), the cue times checked at the
+  // interval's upper end as well
+  std::vector<double> max_end;
+  if (gss) {
+    const double r_hi = B2_GSS_HI;
+    std::vector<int64_t> len_hi(T);
+    if (rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, &r_hi, 1, 0, sample_rate, len_hi.data()) != B2_OK) {
+      int64_t bad_at;
+      double bad_val;
+      const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, T, &r_hi, 1, 0, start_seconds, &bad_at, &bad_val);
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: at ratio %g: %s (index %lld: %g)", who, r_hi, why ? why : "bad cue list",
+              (long long)bad_at, bad_val);
+    }
+    max_end.assign(T, 0.0);
+    for (int t = 0; t < T; ++t)
+      for (int64_t c = cue_off[t]; c < cue_off[t + 1]; ++c)
+        max_end[t] = c == cue_off[t] ? cue_end_s[c] : std::max(max_end[t], cue_end_s[c]);
+  }
 
   // Default: the K subtitle signals of a track are never materialised as floats - the cue list is
   // rasterised into bit masks (1 bit per frame) that the correlation kernel and the exact re-score
@@ -1067,14 +1098,37 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     B2_CHECK_DEV(h, memspace, all_score, "sync_tracks: all_score");
     B2_CHECK_DEV(h, memspace, all_offset, "sync_tracks: all_offset");
   }
+  if (gss) {
+    B2_CHECK_DEV(h, memspace, gss_ratio, "sync_tracks_gss: gss_ratio");
+    B2_CHECK_DEV(h, memspace, gss_evals, "sync_tracks_gss: gss_evals");
+  }
+  // GSS: the grid's per-ratio results stay in the workspace (all_* then hold K + 1 columns, written by the
+  // combine); host calls stage the GSS outputs in a second workspace
+  const size_t JG = (size_t)T * (K + 1);
+  double *g_all_score = nullptr, *g_ratio = gss_ratio, *g_evals = gss_evals;
+  int32_t* g_all_offset = nullptr;
+  if (gss) {
+    void* d_go;
+    B2_TRY(b2i_ws(h, b2_ctx::WS_GSS_OUT, JG * 12 + (size_t)T * 8 * (1 + kGssEvals) + 256, &d_go));
+    double* hs = (double*)d_go;
+    double* hr = hs + JG;
+    double* he = hr + T;
+    int32_t* ho = (int32_t*)(he + (size_t)T * kGssEvals);
+    g_all_score = all_score ? (memspace == B2_DEVICE ? all_score : hs) : nullptr;
+    g_all_offset = all_offset ? (memspace == B2_DEVICE ? all_offset : ho) : nullptr;
+    if (memspace != B2_DEVICE) {
+      g_ratio = hr;
+      g_evals = gss_evals ? he : nullptr;
+    }
+  }
   const int16_t* d_pcm = pcm;
   if (memspace == B2_HOST) {
     void* dp;
     B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, pcm, (size_t)pcm_off[V] * 2, &dp));
     d_pcm = (const int16_t*)dp;
   }
-  double* o_score = (memspace == B2_DEVICE && all_score) ? all_score : d_score;
-  int32_t* o_offset = (memspace == B2_DEVICE && all_offset) ? all_offset : d_offset;
+  double* o_score = (memspace == B2_DEVICE && all_score && !gss) ? all_score : d_score;
+  int32_t* o_offset = (memspace == B2_DEVICE && all_offset && !gss) ? all_offset : d_offset;
   double* o_bs = memspace == B2_DEVICE ? best_score : d_bs;
   int32_t* o_bo = memspace == B2_DEVICE ? best_offset : d_bo;
   int32_t* o_bk = memspace == B2_DEVICE ? best_k : d_bk;
@@ -1097,8 +1151,15 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
                             (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
                             o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
-    return b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nt, K, max_offset_samples,
-                             o_bs + t0, o_bo + t0, o_bk + t0);
+    B2_TRY(b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nt, K, max_offset_samples,
+                             o_bs + t0, o_bo + t0, o_bk + t0));
+    if (!gss || nt == 0) return B2_OK;
+    const size_t a0 = (size_t)t0 * (K + 1);
+    const B2GssOut go{o_bs + t0, o_bo + t0, o_bk + t0, o_score + j0, o_offset + j0,
+                      g_all_score ? g_all_score + a0 : nullptr, g_all_offset ? g_all_offset + a0 : nullptr,
+                      g_ratio + t0, g_evals ? g_evals + (size_t)t0 * kGssEvals : nullptr};
+    return b2i_gss_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(), K, src,
+                          max_end.data() + t0, max_offset_samples, go);
   };
 
   // Software pipeline over sub-batches of videos.  The VAD (HBM-bound) of every sub-batch is queued on the
@@ -1216,8 +1277,15 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   B2_TRY(copy_out(h, best_score, d_bs, (size_t)T * 8));
   B2_TRY(copy_out(h, best_offset, d_bo, (size_t)T * 4));
   B2_TRY(copy_out(h, best_k, d_bk, (size_t)T * 4));
-  if (all_score) B2_TRY(copy_out(h, all_score, d_score, J * 8));
-  if (all_offset) B2_TRY(copy_out(h, all_offset, d_offset, J * 4));
+  if (gss) {
+    if (all_score) B2_TRY(copy_out(h, all_score, g_all_score, JG * 8));
+    if (all_offset) B2_TRY(copy_out(h, all_offset, g_all_offset, JG * 4));
+    B2_TRY(copy_out(h, gss_ratio, g_ratio, (size_t)T * 8));
+    if (gss_evals) B2_TRY(copy_out(h, gss_evals, g_evals, (size_t)T * kGssEvals * 8));
+  } else {
+    if (all_score) B2_TRY(copy_out(h, all_score, d_score, J * 8));
+    if (all_offset) B2_TRY(copy_out(h, all_offset, d_offset, J * 4));
+  }
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
 }
@@ -1252,4 +1320,21 @@ extern "C" int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pc
                           non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
                           ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
                           all_offset, memspace);
+}
+
+extern "C" int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                  const int32_t* track_video, int T, int frame_rate, int sample_rate,
+                                  float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                                  const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                  const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                  int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                  int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                  double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_gss");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_gss: null track_video");
+  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
+                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
+                          all_offset, memspace, /*gss=*/true, gss_ratio, gss_evals);
 }

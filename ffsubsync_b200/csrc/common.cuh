@@ -59,7 +59,7 @@ struct b2_ctx {
   int refsig_parity = 0;
   // named grow-only workspaces
   enum { WS_STAGE_IN0, WS_STAGE_IN1, WS_STAGE_OUT, WS_META, WS_SPEC, WS_SCORES, WS_CAND,
-         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_COUNT };
+         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_GSS, WS_GSS_OUT, WS_COUNT };
   DeviceBuf ws[WS_COUNT];
   HostBuf pinned[4];
   cudaEvent_t pinned_ev[4] = {};   // recorded after the last async copy out of pinned[i]
@@ -196,6 +196,20 @@ struct B2CueSource {
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);
+// The same cue list already on the device (the GSS rounds upload it once per chain): DEVICE arrays,
+// cue_off[n_sig + 1] absolute into start / end / keep.
+struct B2CueDev {
+  const double* start;
+  const double* end;
+  const uint8_t* keep;       // may be null
+  const long long* cue_off;
+  int sample_rate;
+  double start_seconds;
+};
+// Zeroes n_sig masks of sig_words words each (signal b at d_bits + b * sig_words) and rasterises signal b at
+// the ratio d_ratio[b] and length d_len[b] (device arrays written by an earlier kernel).  No host upload.
+int b2i_raster_bits_dev_launch(b2_ctx* h, const B2CueDev& cues, int n_sig, int64_t max_cues, const double* d_ratio,
+                               const long long* d_len, long long sig_words, uint32_t* d_bits);
 // capture_j0: global index of job 0 of this call in the arrays of b2_capture_nominations (b2_sync_batch's
 // sub-batches align a range of pairs at a time).  ref_off_host has V+1 entries; reference v is shared by
 // the tracks trk_off[v] .. trk_off[v+1]-1 (trk_off[V] == B), each with K ratio jobs t*K + k.  trk_off == NULL:
@@ -208,3 +222,23 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host,
 int b2i_reduce_launch(b2_ctx* h, const double* d_score, const int32_t* d_offset,
                       const int32_t* d_status, int B, int K, int64_t max_offset_samples,
                       double* d_best_score, int32_t* d_best_offset, int32_t* d_best_k);
+// Golden-section search over the ratio for the tracks [0, T) of one chain (runcorr.cu, DESIGN.md section 4
+// "K8g"), after the grid chain wrote its reduced (score, offset, k) to bs / bo / bk and its per-ratio results
+// to g_score / g_offset [T*K].  Everything is enqueued on h->stream without a synchronisation.  ref_off_host
+// [V+1] and trk_off[V+1] as for b2i_align_launch; max_end[t]: the track's largest cue end (0 without cues).
+// Writes gss_ratio[t] (NaN for an empty reference), evals[t * kGssEvals + r] when evals is not null, merges the
+// GSS candidate into bs / bo / bk, and, when a_score / a_offset are not null, the grid's K results plus the
+// candidate into a_*[t * (K + 1) + k].
+struct B2GssOut {
+  double* bs;
+  int32_t* bo;
+  int32_t* bk;
+  const double* g_score;
+  const int32_t* g_offset;
+  double* a_score;     // may be null
+  int32_t* a_offset;   // may be null
+  double* gss_ratio;
+  double* evals;       // may be null
+};
+int b2i_gss_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host, int V, const int* trk_off, int K,
+                   const B2CueSource& src, const double* max_end, int64_t max_offset_samples, const B2GssOut& out);

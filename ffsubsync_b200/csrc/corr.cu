@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "corr.cuh"
 #include "corr_jobs.cuh"
+#include "job_plan.cuh"
 
 namespace {
 
@@ -594,14 +595,6 @@ __global__ void __launch_bounds__(256) capture_nominations_kernel(const SelJob* 
 }
 
 // ---- host planning ----------------------------------------------------------------------------
-long long padded_length(const b2_ctx* h, long long n) {
-  // int(2 ** math.ceil(math.log(n, 2))), aligners.py:67-68, libm quirks included
-  int k = 0;
-  while ((1LL << k) < n) ++k;
-  if ((1LL << k) == n && (h->log2_quirk_mask >> k) & 1ULL) ++k;
-  return 1LL << k;
-}
-
 long long floor_div(long long a, long long b) {
   long long q = a / b;
   if ((a % b != 0) && ((a < 0) != (b < 0))) --q;
@@ -686,29 +679,16 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
         s.out_index = (int)j;
         s.bits_off = cue_mode ? bits_off[j] : -1;
         s.sub_level = cue_mode ? (float)std::min(1.0 / cue_src->ratios[k], 1.0) : 0.f;  // speech_transformers.py:977
-        if (R == 0 || S == 0) {  // aligners.py:58-66
-          s.kind = 1;
+        // aligners.py:31-66: empty input, padded length, surviving index range (job_plan.cuh)
+        const B2JobPlan jp = b2_plan_job(R, S, max_offset_samples, h->log2_quirk_mask);
+        if (jp.kind != 0) {
+          s.kind = jp.kind;
+          s.masked_offset = jp.masked_offset;
           continue;
         }
-        const long long N = padded_length(h, R + S);
-        long long lo = 0, hi = N;  // surviving index range, aligners.py:31-43 with slice semantics
-        if (max_offset_samples != B2_MAX_OFFSET_NONE) {
-          // any int64 width, negative ones included, through the reference's slice arithmetic; widths
-          // are clamped to +-2^40 first (beyond every padded length, so the result is unchanged)
-          const long long mo = mo_clamped;
-          const long long a = N - 1 - mo - S;
-          const long long bb = N - 1 + mo - S;
-          lo = a >= 0 ? std::min(a, N) : std::max(a + N, 0LL);
-          hi = bb >= 0 ? std::min(bb, N) : std::max(bb + N, 0LL);
-        }
-        if (lo >= hi) {
-          s.kind = 2;
-          s.masked_offset = (int)(N - 1 - S);
-          continue;
-        }
-        const long long o_lo = N - S - hi, o_hi = N - 1 - S - lo;  // aligners.py:47
-        idx_lo[j] = lo;
-        idx_hi[j] = hi;
+        const long long N = jp.N, o_lo = jp.o_lo, o_hi = jp.o_hi;
+        idx_lo[j] = jp.lo;
+        idx_hi[j] = jp.hi;
         n_pad[j] = N;
         if (N < (1LL << (bigfft_min_log2n())) || N > (1LL << bigfft_max_log2n())) big_ok = false;
         s.kind = 0;

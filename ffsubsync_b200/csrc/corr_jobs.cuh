@@ -103,6 +103,23 @@ int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
 constexpr double kRunCostPerBlock = 5.6e5;
 constexpr int kRunMaxCues = 16384;
 constexpr int kRunMaxWindow = 32 * 1024;  // 32 offsets per thread, 1024 threads
+// GSS rounds (gss.cu kernels, driven by b2i_gss_launch in runcorr.cu).  One lane per track of the chain.
+struct GssTrack {
+  long long ref_off;   // element offset of its video's reference signal
+  long long bits_off;  // word offset of its mask (capacity planned at the interval's upper end)
+  double max_end;      // largest unscaled cue end, 0 without cues
+  int R;               // reference length
+};
+struct B2GssLane;
+// Round r: consumes the exact score of round r - 1 (prev_score[t]), writes the job of round r (sel[t], a
+// run-path job with its own window), its ratio x[t] and length len[t], and evals[t * kGssEvals + r].
+int b2i_gss_step_launch(b2_ctx* h, int r, int T, const GssTrack* d_trk, B2GssLane* d_lane, const double* prev_score,
+                        SelJob* d_sel, double* d_x, long long* d_len, double* evals, long long max_offset_samples,
+                        int sample_rate);
+// After the last round: the GSS candidate (x, score, offset, status of the last round) against the grid's
+// reduced result under MaxScoreAligner.transform's rule, candidate K last in list order.
+int b2i_gss_combine_launch(b2_ctx* h, int T, int K, const GssTrack* d_trk, const double* d_x, const double* r_score,
+                           const int32_t* r_offset, long long max_offset_samples, const B2GssOut& out);
 // Large-window path (bigfft.cu).  sel: host copy of the jobs (kind / R / S / offsets filled in by the
 // planner; this call sets o_first, m_lo, m_hi, score_off), surviving index range per job in idx_lo /
 // idx_hi (half open, in the reference's conv[] index space), padded lengths n_pad per job.  Reference v

@@ -67,15 +67,21 @@ struct RasterBitsParams {
   uint32_t* bits;              // zeroed by the caller
   int K, sample_rate, sig_base;  // blockIdx.y + sig_base = signal (grid.y is limited to 65535)
   double start_seconds;
+  // device-driven ratios (the GSS rounds, K = 1): when set, signal b has ratio sig_ratio[b], length
+  // sig_len[b] and its mask at bits + b * sig_words; ratios / sig_off / bits_off are not read
+  const double* sig_ratio;
+  const long long* sig_len;
+  long long sig_words;
 };
 
 __global__ void __launch_bounds__(256) raster_bits_kernel(RasterBitsParams p) {
   const int sig = blockIdx.y + p.sig_base;
   const int b = sig / p.K;
-  const double ratio = p.ratios[sig - b * p.K];
+  const bool dev = p.sig_ratio != nullptr;
+  const double ratio = dev ? p.sig_ratio[sig] : p.ratios[sig - b * p.K];
   const long long c0 = p.cue_off[b], c1 = p.cue_off[b + 1];
-  const long long n = p.sig_off[sig + 1] - p.sig_off[sig];
-  uint32_t* out = p.bits + p.bits_off[sig];
+  const long long n = dev ? p.sig_len[sig] : p.sig_off[sig + 1] - p.sig_off[sig];
+  uint32_t* out = p.bits + (dev ? sig * p.sig_words : p.bits_off[sig]);
   for (long long c = c0 + (long long)blockIdx.x * blockDim.x + threadIdx.x; c < c1;
        c += (long long)gridDim.x * blockDim.x) {
     if (p.keep && !p.keep[c]) continue;
@@ -252,9 +258,38 @@ int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, cons
   p.K = K;
   p.sample_rate = src->sample_rate;
   p.start_seconds = src->start_seconds;
+  p.sig_ratio = nullptr;
+  p.sig_len = nullptr;
+  p.sig_words = 0;
   for (size_t j0 = 0; j0 < J; j0 += 65535) {
     p.sig_base = (int)j0;
     dim3 grid((unsigned)std::min<int64_t>((max_cues + 255) / 256, 64), (unsigned)std::min<size_t>(J - j0, 65535));
+    raster_bits_kernel<<<grid, 256, 0, h->stream>>>(p);
+    B2_CHECK_LAUNCH(h, "raster_bits_kernel");
+  }
+  return B2_OK;
+}
+
+int b2i_raster_bits_dev_launch(b2_ctx* h, const B2CueDev& cues, int n_sig, int64_t max_cues, const double* d_ratio,
+                               const long long* d_len, long long sig_words, uint32_t* d_bits) {
+  if (n_sig <= 0) return B2_OK;
+  B2_CUDA(h, cudaMemsetAsync(d_bits, 0, (size_t)n_sig * sig_words * 4, h->stream));
+  if (max_cues == 0) return B2_OK;
+  RasterBitsParams p{};
+  p.start_s = cues.start;
+  p.end_s = cues.end;
+  p.keep = cues.keep;
+  p.cue_off = cues.cue_off;
+  p.bits = d_bits;
+  p.K = 1;
+  p.sample_rate = cues.sample_rate;
+  p.start_seconds = cues.start_seconds;
+  p.sig_ratio = d_ratio;
+  p.sig_len = d_len;
+  p.sig_words = sig_words;
+  for (int j0 = 0; j0 < n_sig; j0 += 65535) {
+    p.sig_base = j0;
+    dim3 grid((unsigned)std::min<int64_t>((max_cues + 255) / 256, 64), (unsigned)std::min(n_sig - j0, 65535));
     raster_bits_kernel<<<grid, 256, 0, h->stream>>>(p);
     B2_CHECK_LAUNCH(h, "raster_bits_kernel");
   }

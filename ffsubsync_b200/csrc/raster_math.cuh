@@ -66,6 +66,17 @@ RASTER_HD double b2_scaled_seconds(double t, double ratio) {
   return b2_rm_div((double)us, 1e6);
 }
 
+// Signal length int(max_time * sample_rate) + 2 (speech_transformers.py:958-962), max_time the largest
+// scaled cue end and at least 0.  max_end: the largest unscaled cue end (0 for a track without cues).
+// The max over cues of the scaled end is the scaled max end because the product, the microsecond
+// rounding and the division are all monotone non-decreasing for ratio > 0.
+RASTER_HD long long b2_signal_length(double max_end, double ratio, int sample_rate) {
+  double max_time = 0.0;
+  const double e = b2_scaled_seconds(max_end, ratio);
+  if (e > max_time) max_time = e;
+  return (long long)b2_rm_mul(max_time, (double)sample_rate) + 2;
+}
+
 // samples[first:last] of a length-n array with Python slice semantics (negative index wraps once).
 RASTER_HD void b2_cue_bounds(double start_s, double end_s, double ratio, double start_seconds,
                              int sample_rate, long long n, long long& first, long long& last) {

@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "corr_jobs.cuh"
+#include "job_plan.cuh"
 #include "runcorr.cuh"
 
 namespace {
@@ -329,4 +330,118 @@ int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
   // the window scores are in the capture already: win / stat / cand as the finalize left them
   if (capture) B2_TRY(b2i_capture_launch(h, d_sel, nullptr, (int)J, nullptr, cb, capture_j0, /*scores_written=*/true));
   return B2_OK;
+}
+
+// ---- GSS rounds (b2_sync_tracks_gss) ----------------------------------------------------------------
+// One chain's golden-section search, queued on h->stream with no synchronisation: the packed reference once,
+// then per round gss_step_kernel (the round's ratio, length and run-path job per track, from the previous
+// round's exact score) -> zero + rasterise the masks at those ratios -> run_corr_kernel -> run_finalize_kernel
+// (K = 1) -> rescore_kernel -> pick_kernel, and finally the combine.  Every host-side input of a round is
+// uploaded once per chain, in one metadata arena that no later arena of the chain can recycle (the rounds
+// begin none).
+int b2i_gss_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
+                   const B2CueSource& src, const double* max_end, int64_t max_offset_samples, const B2GssOut& out) {
+  B2Range range("b2:gss rounds (step, raster_bits, run_corr, finalize, rescore, pick) x 17");
+  const int T = trk_off[V] - trk_off[0];
+  if (T <= 0) return B2_OK;
+  // the mask's window holds at most 2 max_offset_samples offsets whatever the length (DESIGN.md "K8g");
+  // the caller has checked that this fits one CTA and that every track has at most kRunMaxCues cues
+  if (max_offset_samples < 0 || max_offset_samples > kMaxWindow / 2)
+    B2_FAIL(h, B2_ERR_UNSUPPORTED, "gss: max_offset_samples %lld is outside [0, %d]", (long long)max_offset_samples,
+            kMaxWindow / 2);
+  const long long w_bound = std::max<long long>(1, 2 * (long long)max_offset_samples);
+  const int max_thr = (int)(32 * ceil_div64(ceil_div64(w_bound, kOffsetsPerThread), 32));
+  std::vector<GssTrack> trk(T);
+  std::vector<RunRef> vids;
+  std::vector<long long> job_q(T, 0);
+  long long q_total = 0, sig_words = 1;
+  int max_runs = 1;
+  const long long c0 = src.cue_off[0], nc = src.cue_off[T] - c0;
+  for (int v = 0; v < V; ++v) {
+    const long long R = ref_off[v + 1] - ref_off[v];
+    if (R < 0 || R > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "gss: bad reference length at %d", v);
+    if (trk_off[v + 1] == trk_off[v]) continue;
+    vids.push_back(RunRef{(long long)ref_off[v], q_total, (int)R});
+    for (int t = trk_off[v]; t < trk_off[v + 1]; ++t) {
+      // the mask capacity at the interval's upper end: the length is monotone in the ratio
+      const long long s_max = b2_signal_length(max_end[t], B2_GSS_HI, src.sample_rate);
+      if (s_max > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "gss: subtitle signal of track %d too long", t);
+      sig_words = std::max(sig_words, (s_max >> 5) + 2);
+      trk[t] = GssTrack{(long long)ref_off[v], 0, max_end[t], (int)R};
+      job_q[t] = q_total;
+      max_runs = std::max<int>(max_runs, (int)std::min<long long>(src.cue_off[t + 1] - src.cue_off[t], kRunMaxCues));
+    }
+    q_total += rc_ref_entries((int)R);
+  }
+  long long max_cues = 0;
+  for (int t = 0; t < T; ++t) {
+    trk[t].bits_off = (long long)t * sig_words;
+    max_cues = std::max<long long>(max_cues, src.cue_off[t + 1] - src.cue_off[t]);
+  }
+  std::vector<long long> cue_rel(T + 1);
+  for (int t = 0; t <= T; ++t) cue_rel[t] = src.cue_off[t] - c0;
+
+  // device workspace of the chain
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~size_t(255); return o; };
+  const size_t o_q = take((size_t)q_total * 8), o_stat = take((size_t)T * sizeof(RunStat)),
+               o_lane = take((size_t)T * sizeof(B2GssLane)), o_sel = take((size_t)T * sizeof(SelJob)),
+               o_x = take((size_t)T * 8), o_len = take((size_t)T * 8), o_rs = take((size_t)T * 8),
+               o_ro = take((size_t)T * 4), o_rst = take((size_t)T * 4), o_bits = take((size_t)T * sig_words * 4),
+               o_cp = take((size_t)T * kCandMax * kRescoreSeg * 8), o_js = take((size_t)T * 8),
+               o_co = take((size_t)T * kCandMax * 4), o_cc = take((size_t)T * 4),
+               o_wl = take((size_t)T * kCandMax * 4), o_wc = take(16);
+  void* d_ws;
+  B2_TRY(b2i_ws(h, b2_ctx::WS_GSS, at + 256, &d_ws));
+  char* base = (char*)d_ws;
+  uint2* q = (uint2*)(base + o_q);
+  RunStat* stat = (RunStat*)(base + o_stat);
+  B2GssLane* lane = (B2GssLane*)(base + o_lane);
+  SelJob* d_sel = (SelJob*)(base + o_sel);
+  double* d_x = (double*)(base + o_x);
+  long long* d_len = (long long*)(base + o_len);
+  double* r_score = (double*)(base + o_rs);
+  int32_t* r_offset = (int32_t*)(base + o_ro);
+  int32_t* r_status = (int32_t*)(base + o_rst);
+  uint32_t* d_bits = (uint32_t*)(base + o_bits);
+  B2CandBuffers cb;
+  cb.cand_partial = (double*)(base + o_cp);
+  cb.job_stat = (float2*)(base + o_js);
+  cb.cand_off = (int*)(base + o_co);
+  cb.cand_cnt = (int*)(base + o_cc);
+  cb.work_list = (int*)(base + o_wl);
+  cb.work_count = (int*)(base + o_wc);
+
+  MetaArena a;
+  B2_TRY(b2i_meta_begin(h, &a, (size_t)nc * 17 + (size_t)(T + 1) * 8 + (size_t)T * (sizeof(GssTrack) + 8) +
+                                   vids.size() * sizeof(RunRef) + 1024));
+  B2CueDev cues;
+  cues.start = (const double*)b2i_meta_put(&a, src.cue_start + c0, (size_t)nc * 8);
+  cues.end = (const double*)b2i_meta_put(&a, src.cue_end + c0, (size_t)nc * 8);
+  cues.keep = src.cue_keep ? (const uint8_t*)b2i_meta_put(&a, src.cue_keep + c0, (size_t)nc) : nullptr;
+  cues.cue_off = (const long long*)b2i_meta_put(&a, cue_rel.data(), (size_t)(T + 1) * 8);
+  cues.sample_rate = src.sample_rate;
+  cues.start_seconds = src.start_seconds;
+  const GssTrack* d_trk = (const GssTrack*)b2i_meta_put(&a, trk.data(), (size_t)T * sizeof(GssTrack));
+  const long long* d_job_q = (const long long*)b2i_meta_put(&a, job_q.data(), (size_t)T * 8);
+  const RunRef* d_vids = (const RunRef*)b2i_meta_put(&a, vids.data(), vids.size() * sizeof(RunRef));
+  B2_TRY(b2i_meta_commit(&a));
+
+  ref_bits_kernel<<<(unsigned)vids.size(), 1024, 0, h->stream>>>(d_ref, d_vids, q);
+  B2_CHECK_LAUNCH(h, "ref_bits_kernel");
+  const size_t smem = (size_t)3 * max_runs * sizeof(int);
+  B2_CUDA(h, cudaFuncSetAttribute(run_corr_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  for (int r = 0; r < kGssEvals; ++r) {
+    B2_TRY(b2i_gss_step_launch(h, r, T, d_trk, lane, r_score, d_sel, d_x, d_len,
+                               out.evals, max_offset_samples, src.sample_rate));
+    B2_TRY(b2i_raster_bits_dev_launch(h, cues, T, max_cues, d_x, d_len, sig_words, d_bits));
+    run_corr_kernel<false><<<(unsigned)T, (unsigned)max_thr, smem, h->stream>>>(
+        d_sel, d_job_q, q, d_bits, src.ref_label, max_runs, stat, cb.cand_off, B2Capture{}, 0);
+    B2_CHECK_LAUNCH(h, "run_corr_kernel");
+    B2_CUDA(h, cudaMemsetAsync(cb.work_count, 0, sizeof(int), h->stream));
+    run_finalize_kernel<<<(unsigned)((T + 127) / 128), 128, 0, h->stream>>>(d_sel, T, 1, /*winner_only=*/0, stat, cb);
+    B2_CHECK_LAUNCH(h, "run_finalize_kernel");
+    B2_TRY(b2i_rescore_pick(h, d_sel, (size_t)T, d_ref, nullptr, d_bits, cb, r_score, r_offset, r_status));
+  }
+  return b2i_gss_combine_launch(h, T, K, d_trk, d_x, r_score, r_offset, max_offset_samples, out);
 }

@@ -137,24 +137,34 @@ def _gather_blocks(local: torch.Tensor, counts: List[Tuple[int, int]], rank: int
     return torch.cat([out[r, : hi - lo] for r, (lo, hi) in enumerate(counts)], dim=0)
 
 
-def gather_pair_results(local: torch.Tensor, n_pairs: int, rank: int, world: int, dst: int = 0,
-                        group=None) -> Optional[torch.Tensor]:
-    """local: [n_local, C] results of this rank's block of pairs (any dtype, same on all ranks).
-    Returns [n_pairs, C] in global pair order on ``dst`` (None elsewhere).  One collective."""
+def _gather_any(local, counts, rank, world, dst, group):
+    """A tensor, or a dict of per-row tensors such as BatchSynchronizer.sync_device's output (best_*, and
+    gss_ratio with the golden-section search): every entry is gathered the same way, one collective each."""
+    if not isinstance(local, dict):
+        return _gather_blocks(local, counts, rank, world, dst, group)
+    out = {k: _gather_blocks(v, counts, rank, world, dst, group) for k, v in local.items()}
+    return None if dst is not None and rank != dst else out
+
+
+def gather_pair_results(local, n_pairs: int, rank: int, world: int, dst: int = 0, group=None):
+    """local: [n_local, C] results of this rank's block of pairs (any dtype, same on all ranks), or a dict
+    of such tensors (e.g. sync_device's output, which carries gss_ratio with the golden-section search).
+    Returns [n_pairs, C] (or the dict of them) in global pair order on ``dst`` (None elsewhere).  One
+    collective per tensor."""
     if world == 1:
         return local
-    return _gather_blocks(local, [shard_pairs(n_pairs, r, world) for r in range(world)], rank, world, dst, group)
+    return _gather_any(local, [shard_pairs(n_pairs, r, world) for r in range(world)], rank, world, dst, group)
 
 
-def gather_track_results(local: torch.Tensor, track_video, rank: int, world: int, dst: Optional[int] = 0,
-                         group=None) -> Optional[torch.Tensor]:
-    """local: [t1 - t0, C] results of the tracks shard_videos() gave this rank (per-rank counts differ).
-    Returns [T, C] in global track order on ``dst`` (on every rank when dst is None, None elsewhere).
-    One collective."""
+def gather_track_results(local, track_video, rank: int, world: int, dst: Optional[int] = 0, group=None):
+    """local: [t1 - t0, C] results of the tracks shard_videos() gave this rank (per-rank counts differ), or a
+    dict of such tensors (e.g. sync_device_tracks' output, which carries gss_ratio with the golden-section
+    search).  Returns [T, C] (or the dict of them) in global track order on ``dst`` (on every rank when dst is
+    None, None elsewhere).  One collective per tensor."""
     if world == 1:
         return local
     counts = [shard_videos(track_video, r, world)[2:] for r in range(world)]
-    return _gather_blocks(local, counts, rank, world, dst, group)
+    return _gather_any(local, counts, rank, world, dst, group)
 
 
 def allgather_candidate_results(local: torch.Tensor, n_candidates: int, rank: int, world: int,

@@ -99,3 +99,29 @@ def gss_align_batch(ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None,
         if k == n - 2:
             last = (s[:, 0].copy(), o[:, 0].copy(), x.copy(), st[:, 0].copy())
     return GssResult(last[0], last[1].astype(np.int32), last[2], np.stack(evals, axis=1), last[3].astype(np.int32))
+
+
+def combine_gss(best_score, best_offset, best_k, gss: GssResult, K: int, max_offset_samples: Optional[int],
+                all_score=None, all_offset=None):
+    """MaxScoreAligner.transform (ffsubsync/aligners.py:154-167) over the candidates [grid, GSS] of every
+    track, given the grid's reduced result (b2_sync_tracks) and the search's last evaluation: the GSS candidate
+    is number K, last in list order, so it wins only with a strictly higher score; it goes through the same
+    |offset| filter, and a track whose reference is empty (status B2_ALIGN_EMPTY) keeps the grid's answer
+    and gets ratio NaN.  all_*: the grid's [T*K] per-ratio results, returned as [T*(K+1)] with column K the
+    candidate.  Returns (best_score, best_offset, best_k, gss_ratio, all_score, all_offset) as numpy arrays."""
+    bs = np.array(best_score, dtype=np.float64)
+    bo = np.array(best_offset, dtype=np.int32)
+    bk = np.array(best_k, dtype=np.int32)
+    T = len(bk)
+    live = (np.asarray(gss.status) & _native.ALIGN_EMPTY) == 0
+    ok = live if max_offset_samples is None else live & (np.abs(gss.offset.astype(np.int64)) <= max_offset_samples)
+    win = ok & ((bk < 0) | (gss.score > bs))
+    bs[win], bo[win], bk[win] = gss.score[win], gss.offset[win], K
+    ratio = np.where(live, gss.ratio, np.nan)
+    a_s = a_o = None
+    if all_score is not None:
+        a_s = np.concatenate([np.asarray(all_score, np.float64).reshape(T, K), gss.score[:, None]], axis=1).reshape(-1)
+    if all_offset is not None:
+        a_o = np.concatenate([np.asarray(all_offset, np.int32).reshape(T, K),
+                              gss.offset.astype(np.int32)[:, None]], axis=1).reshape(-1)
+    return bs, bo, bk, ratio, a_s, a_o

@@ -219,6 +219,29 @@ int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /* [V
                    double* all_score /* [T*K] or NULL */, int32_t* all_offset /* [T*K] or NULL */,
                    int memspace);
 
+/* ---- the grid plus the golden-section search over the ratio (--gss) ----------------------------
+ * `ffs movie.mkv -i a.srt ... --gss`: the reference's ratio list is the grid plus a golden-section search
+ * (ffsubsync/ffsubsync.py:131-142; MaxScoreAligner.fit_gss, ffsubsync/aligners.py:111-129;
+ * ffsubsync/golden_section_search.py:15-74).  Track t gets exactly what the reference's try_sync returns for the
+ * candidates [ratios[0..K-1], GSS]: the GSS candidate is the (score, offset) of the 17th evaluation of the search
+ * over [0.9, 1.1] with tolerance 1e-4 (fixed), and it goes through the same |offset| <= max_offset_samples filter
+ * and first-wins tie rule as a (K+1)-th ratio: best_k[t] == K means it won, and on an exact tie a grid ratio wins.
+ * Arguments as for b2_sync_tracks, plus gss_ratio[T] (the 17th point; NaN for a track whose video has no
+ * windows, which gets best_k = -1 and is not searched) and gss_evals[T*17] (every point in evaluation order, or
+ * NULL).  all_score / all_offset, when given, are [T*(K+1)]: column K holds the GSS candidate.  memspace as for
+ * b2_sync_tracks; resident calls chain with b2_sync_batch / b2_sync_tracks in either order.  The 17 rounds run
+ * on the handle's stream without a host synchronisation (DESIGN.md section 4 "K8g").  B2_ERR_UNSUPPORTED unless
+ * 0 <= max_offset_samples <= 16384 (every mask window then holds at most 2*max_offset_samples <= 32768 offsets),
+ * every track has at most 16384 cues and non_speech_label is finite; the message names the limit. */
+int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /* [V+1] */, int V,
+                       const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                       float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                       const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                       const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                       int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                       double* all_score /* [T*(K+1)] or NULL */, int32_t* all_offset /* [T*(K+1)] or NULL */,
+                       double* gss_ratio /* [T] */, double* gss_evals /* [T*17] or NULL */, int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
