@@ -29,6 +29,7 @@ EXPORTS = [
     "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
+    "b2_sync_tracks_auditok",
 ]
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
 
@@ -92,6 +93,10 @@ def load() -> ctypes.CDLL:
                                            ctypes.c_int, _f32, _i64, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp,
                                            _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                            ctypes.c_int]
+        lib.b2_sync_tracks_auditok.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int,
+                                               ctypes.c_int, _f64, _f64, _f64, _i64, _f64, _i64, _vp, _vp, _vp,
+                                               _vp, _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               _vp, ctypes.c_int]
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -462,6 +467,57 @@ class Handle:
                                          _ptr(all_offset), _ptr(gss_ratio), _ptr(gss_evals), memspace)
         self._check(st, "b2_sync_tracks_gss")
         return best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals
+
+    def sync_tracks_auditok(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int,
+                            non_speech_label: float, cue_start_s, cue_end_s, cue_keep, cue_off, ratios,
+                            start_seconds: float, max_offset_samples: Optional[int], chunk_samples: int,
+                            energy_threshold_db: float = 50.0, min_length: Optional[float] = None,
+                            max_length: Optional[int] = None, max_continuous_silence: Optional[float] = None,
+                            gss: bool = False, best_score=None, best_offset=None, best_k=None, all_score=None,
+                            all_offset=None, gss_ratio=None, gss_evals=None, want_all: bool = False,
+                            want_evals: bool = False, memspace: int = B2_HOST):
+        """sync_tracks / sync_tracks_gss with the reference's auditok detector (b2_sync_tracks_auditok): each video
+        is cut into detector calls of chunk_samples samples (0: one call).  Detector defaults as for vad_auditok.
+        Returns (best_score, best_offset, best_k, all_score, all_offset), plus (gss_ratio, gss_evals) with
+        gss=True (all_* then [T*(K+1)])."""
+        pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        V, T = len(pcm_off) - 1, len(track_video)
+        if len(cue_off) != T + 1:
+            raise NativeError(-1, "b2_sync_tracks_auditok", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        K = len(ratios)
+        min_length = 0.2 * sample_rate if min_length is None else min_length
+        max_length = int(5 * sample_rate) if max_length is None else max_length
+        max_continuous_silence = 0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
+        mos = _mask_width(max_offset_samples)
+        cols = K + 1 if gss else K
+        if memspace == B2_HOST:
+            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
+            best_score = np.empty(T, dtype=np.float64)
+            best_offset = np.empty(T, dtype=np.int32)
+            best_k = np.empty(T, dtype=np.int32)
+            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
+            if want_all:
+                all_score = np.empty(T * cols, dtype=np.float64)
+                all_offset = np.empty(T * cols, dtype=np.int32)
+            if gss and want_evals:
+                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
+        elif gss and gss_ratio is None:
+            raise ValueError("sync_tracks_auditok(gss=True) on device memory needs gss_ratio")
+        st = self.lib.b2_sync_tracks_auditok(
+            self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate, sample_rate,
+            float(non_speech_label), float(energy_threshold_db), float(min_length), int(max_length),
+            float(max_continuous_silence), int(chunk_samples), _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep),
+            _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos, _ptr(best_score), _ptr(best_offset),
+            _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
+            _ptr(gss_evals) if gss else None, memspace)
+        self._check(st, "b2_sync_tracks_auditok")
+        res = (best_score, best_offset, best_k, all_score, all_offset)
+        return res + (gss_ratio, gss_evals) if gss else res
 
     # -- diagnostics (tests) --------------------------------------------------------------------
     @contextlib.contextmanager

@@ -15,7 +15,8 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _native
-from .constants import DEFAULT_ENERGY_THRESHOLD, DEFAULT_MAX_OFFSET_SECONDS, SAMPLE_RATE
+from .constants import (BATCH_VADS, DEFAULT_ENERGY_THRESHOLD, DEFAULT_MAX_OFFSET_SECONDS, SAMPLE_RATE,
+                        detector_chunk_bytes)
 
 
 def load_serialized_speech(paths, non_speech_label: float = 0.0):
@@ -38,13 +39,25 @@ class BatchSynchronizer:
     """``ratios``: the framerate ratio grid in list order.  A trailing ``None`` adds the golden-section search
     over [0.9, 1.1] as one more candidate, last in list order, the way the reference's list carries ``--gss``
     (``constants.framerate_ratios_to_try(gss=True)``); results then gain ``gss_ratio`` and ``best_k == K``
-    (K = the grid's length) means the search won."""
+    (K = the grid's length) means the search won.
+
+    ``vad``: the detector that turns PCM into the reference signal.  ``"energy_zcr"`` (default) is this package's
+    energy / zero-crossing detector; ``"auditok"`` is the reference's auditok detector (``--vad auditok``) with its
+    default constants (50 dB, min 0.2 s, max 5 s, 0.25 s of continuous silence), run over the reference's chunk loop
+    (one detector call per 100 s).  ``energy_threshold`` / ``z_lo`` / ``z_hi`` belong to the energy detector and must
+    stay at their defaults with ``"auditok"``."""
 
     def __init__(self, ratios: Sequence[Optional[float]], frame_rate: int = 16000, sample_rate: int = SAMPLE_RATE,
                  non_speech_label: float = 0.0, energy_threshold: int = DEFAULT_ENERGY_THRESHOLD,
                  z_lo: int = -1, z_hi: int = -1, start_seconds: float = 0.0,
                  max_offset_seconds: Optional[float] = DEFAULT_MAX_OFFSET_SECONDS,
-                 device: Optional[int] = None) -> None:
+                 device: Optional[int] = None, vad: str = "energy_zcr") -> None:
+        if vad not in BATCH_VADS:
+            raise ValueError("vad must be one of %s, not %r" % (", ".join(BATCH_VADS), vad))
+        if vad == "auditok" and (energy_threshold != DEFAULT_ENERGY_THRESHOLD or z_lo != -1 or z_hi != -1):
+            raise ValueError("energy_threshold / z_lo / z_hi configure the energy_zcr detector; vad='auditok' "
+                             "does not read them")
+        self.vad = vad
         ratios = list(ratios)
         self.gss = bool(ratios) and ratios[-1] is None
         grid = ratios[:-1] if self.gss else ratios
@@ -62,6 +75,19 @@ class BatchSynchronizer:
         # MaxScoreAligner.__init__ (ffsubsync/aligners.py:98-101)
         self.max_offset_samples = None if max_offset_seconds is None else abs(int(max_offset_seconds * sample_rate))
         self.handle = _native.get_handle(device)
+        # auditok: samples per detector call, as VideoSpeechTransformer._chunks reads them
+        self.chunk_samples = detector_chunk_bytes(frame_rate, sample_rate) // 2
+
+    @property
+    def auditok(self) -> bool:
+        return self.vad == "auditok"
+
+    def _auditok_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, gss: bool, **kw):
+        """b2_sync_tracks_auditok with this synchroniser's settings (grid, or grid + search with gss)."""
+        return self.handle.sync_tracks_auditok(
+            pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label, cue_start, cue_end,
+            cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples, self.chunk_samples, gss=gss,
+            **kw)
 
     def use_torch_stream(self) -> None:
         """Launch on torch's current stream (so torch events / NCCL ops order against our kernels)."""
@@ -81,7 +107,7 @@ class BatchSynchronizer:
         B = len(pcm_off) - 1
         K = len(self.ratios)
         dev = pcm.device
-        if self.gss:   # the identity track map: pair b is track b of video b
+        if self.gss or self.auditok:   # the identity track map: pair b is track b of video b
             return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
                                            cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident)
         if out is None:
@@ -121,14 +147,27 @@ class BatchSynchronizer:
             out["gss_ratio"] = torch.empty(T, dtype=torch.float64, device=dev)
         a_s = all_out["score"].data_ptr() if all_out else None
         a_o = all_out["offset"].data_ptr() if all_out else None
+        memspace = _native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE
+        if self.auditok and not self.gss:
+            self._auditok_tracks(pcm.data_ptr(), pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
+                                 best_score=out["best_score"].data_ptr(), best_offset=out["best_offset"].data_ptr(),
+                                 best_k=out["best_k"].data_ptr(), all_score=a_s, all_offset=a_o, memspace=memspace)
+            return out
         if self.gss:
             try:
+                if self.auditok:
+                    self._auditok_tracks(pcm.data_ptr(), pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep,
+                                         True, best_score=out["best_score"].data_ptr(),
+                                         best_offset=out["best_offset"].data_ptr(), best_k=out["best_k"].data_ptr(),
+                                         all_score=a_s, all_offset=a_o, gss_ratio=out["gss_ratio"].data_ptr(),
+                                         memspace=memspace)
+                    return out
                 self.handle.sync_tracks_gss(
                     pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
                     self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
                     self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
                     out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o, out["gss_ratio"].data_ptr(),
-                    memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+                    memspace=memspace)
             except _native.NativeError as e:
                 if not _is_unsupported(e):
                     raise
@@ -144,8 +183,7 @@ class BatchSynchronizer:
             pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
             self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
             self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
-            out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o,
-            memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+            out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o, memspace=memspace)
         return out
 
     def sync_host_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None,
@@ -153,12 +191,21 @@ class BatchSynchronizer:
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
         track, and gss_ratio last with the golden-section search."""
+        if self.auditok and not self.gss:
+            res = self._auditok_tracks(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
+                                       want_all=want_all, memspace=_native.B2_HOST)
+            return res if want_all else res[:3]
         if self.gss:
             try:
-                r = self.handle.sync_tracks_gss(
-                    pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
-                    self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
-                    self.start_seconds, self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
+                if self.auditok:
+                    r = self._auditok_tracks(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, True,
+                                             want_all=want_all, memspace=_native.B2_HOST)
+                else:
+                    r = self.handle.sync_tracks_gss(
+                        pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
+                        self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off,
+                        self.ratios, self.start_seconds, self.max_offset_samples, want_all=want_all,
+                        memspace=_native.B2_HOST)
                 res = r[:5] + (r[5],)
             except _native.NativeError as e:
                 if not _is_unsupported(e):
@@ -238,11 +285,15 @@ class BatchSynchronizer:
         B, K = len(pcm_off) - 1, len(self.ratios)
         dev = pcm.device
         mine = distributed.shard_candidates(K, rank, world)
-        fpw = h.frames_per_window(self.frame_rate, self.sample_rate)
-        ref_off = np.concatenate([[0], np.cumsum((np.diff(pcm_off) + fpw - 1) // fpw)]).astype(np.int64)
-        ref = torch.empty(int(ref_off[-1]), dtype=torch.float32, device=dev)
-        h.vad_energy_zcr(pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
-                         self.energy_threshold, self.z_lo, self.z_hi, out=ref.data_ptr(), memspace=_native.B2_DEVICE)
+        if self.auditok:   # b2_vad_auditok's float64 signal, rounded once to float32
+            ref, ref_off = self._vad_auditok_device(pcm, pcm_off)
+        else:
+            fpw = h.frames_per_window(self.frame_rate, self.sample_rate)
+            ref_off = np.concatenate([[0], np.cumsum((np.diff(pcm_off) + fpw - 1) // fpw)]).astype(np.int64)
+            ref = torch.empty(int(ref_off[-1]), dtype=torch.float32, device=dev)
+            h.vad_energy_zcr(pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                             self.energy_threshold, self.z_lo, self.z_hi, out=ref.data_ptr(),
+                             memspace=_native.B2_DEVICE)
         k_loc = len(mine)
         local = torch.zeros((B, max(k_loc, 1), 3), dtype=torch.float64, device=dev)
         if k_loc:
@@ -277,7 +328,7 @@ class BatchSynchronizer:
         """pcm: int16 numpy array (ideally backed by pinned memory).  Blocks until results are on
         the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]), and gss_ratio last
         with the golden-section search."""
-        if self.gss:
+        if self.gss or self.auditok:
             return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
                                          cue_end, cue_off, cue_keep, want_all=want_all)
         res = self.handle.sync_batch(
@@ -288,9 +339,10 @@ class BatchSynchronizer:
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False):
         """The golden-section search outside the envelope of b2_sync_tracks_gss, composed of the public steps:
-        the VAD (b2_vad_energy_zcr), the grid (b2_sync_tracks), gss_align_batch on each track's reference
-        signal and the reference's combine.  pcm: int16 numpy array or CUDA tensor.  Returns numpy arrays
-        (best_score, best_offset, best_k, gss_ratio, all_score, all_offset) (all_* None unless want_all)."""
+        the VAD (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32), the grid (b2_sync_tracks or
+        b2_sync_tracks_auditok), gss_align_batch on each track's reference signal and the reference's combine.
+        pcm: int16 numpy array or CUDA tensor.  Returns numpy arrays (best_score, best_offset, best_k, gss_ratio,
+        all_score, all_offset) (all_* None unless want_all)."""
         import torch
         from .gss_batch import combine_gss, gss_align_batch
         h = self.handle
@@ -304,12 +356,18 @@ class BatchSynchronizer:
             pcm_host = pcm.cpu().numpy()
         else:
             pcm_host = pcm
-        grid = h.sync_tracks(pcm_host, pcm_off, track_video, self.frame_rate, self.sample_rate,
-                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end,
-                             cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples,
-                             want_all=True, memspace=_native.B2_HOST)
-        ref, ref_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
-                                        self.energy_threshold, self.z_lo, self.z_hi)
+        if self.auditok:
+            grid = self._auditok_tracks(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
+                                        want_all=True, memspace=_native.B2_HOST)
+            ref, ref_off = h.vad_auditok(pcm_host, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                                         chunk_samples=self.chunk_samples)
+        else:
+            grid = h.sync_tracks(pcm_host, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                 self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi, cue_start,
+                                 cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples,
+                                 want_all=True, memspace=_native.B2_HOST)
+            ref, ref_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
+                                            self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
@@ -319,3 +377,22 @@ class BatchSynchronizer:
         bs, bo, bk, ratio, a_s, a_o = combine_gss(grid[0], grid[1], grid[2], g, K, self.max_offset_samples,
                                                   grid[3], grid[4])
         return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))
+
+    def _vad_auditok_device(self, pcm, pcm_off):
+        """b2_vad_auditok over the videos of the CUDA tensor pcm (chunked as the batched calls chunk them), rounded
+        once to float32.  Returns (float32 CUDA tensor, ref_off int64[V+1])."""
+        import torch
+        h = self.handle
+        pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+        fpw = int(h.lib.b2_auditok_block_size(self.frame_rate, self.sample_rate))
+        if fpw <= 0:
+            raise ValueError("auditok detector: unsupported frame_rate=%r / sample_rate=%r"
+                             % (self.frame_rate, self.sample_rate))
+        n = np.diff(pcm_off)
+        c = self.chunk_samples
+        nwin = n // c * ((c + fpw - 1) // fpw) + (n % c + fpw - 1) // fpw
+        ref_off = np.concatenate([[0], np.cumsum(nwin)]).astype(np.int64)
+        ref64 = torch.empty(int(ref_off[-1]), dtype=torch.float64, device=pcm.device)
+        h.vad_auditok(pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                      chunk_samples=c, out=ref64.data_ptr(), memspace=_native.B2_DEVICE)
+        return ref64.to(torch.float32), ref_off

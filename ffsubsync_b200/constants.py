@@ -11,10 +11,20 @@ DEFAULT_START_SECONDS: int = 0
 DEFAULT_SCALE_FACTOR: float = 1
 DEFAULT_MAX_OFFSET_SECONDS: int = 60        # constants.py:18
 DEFAULT_VAD: str = "energy_zcr"             # the detector this package implements
+BATCH_VADS = ("energy_zcr", "auditok")      # detectors the batched sync calls run
 
 # energy / zero-crossing detector defaults (DESIGN.md): auditok's energy_threshold=50 dB
 # (speech_transformers.py:125) is mean(x^2) >= 1e5
 DEFAULT_ENERGY_THRESHOLD: int = 100000
+
+# the reference's chunk loop reads 10 000 windows of ``2 * frame_rate // sample_rate`` bytes per detector
+# call (speech_transformers.py:710-711,741)
+CHUNK_WINDOWS: int = 10000
+
+
+def detector_chunk_bytes(frame_rate: int, sample_rate: int, windows: int = CHUNK_WINDOWS) -> int:
+    """Bytes of s16le PCM per detector call of the reference's chunk loop (half as many samples)."""
+    return (2 * frame_rate // sample_rate) * windows
 
 
 def framerate_ratios_to_try(no_fix_framerate: bool = False, gss: bool = False) -> list:

@@ -980,6 +980,13 @@ extern "C" int b2_reduce_ratios(b2_handle h, const double* score, const int32_t*
 // subtitle tracks: track t is synced against video track_video[t] (non-decreasing; NULL: V == T, track t
 // against video t - b2_sync_batch).  Each video's PCM goes through the VAD once; its reference spectra
 // serve the K ratio jobs t*K + k of every one of its tracks.
+// The detector is this package's energy / zero-crossing VAD, or with `aud` the reference's auditok detector
+// (b2_vad_auditok's arguments; its float64 signal rounded once to float32 is the reference signal).
+struct AuditokArgs {
+  double non_speech_label, energy_threshold_db, min_length, max_continuous_silence;
+  int64_t max_length, chunk_samples;
+};
+
 static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm, const int64_t* pcm_off, int V,
                             const int32_t* track_video, int T, int frame_rate, int sample_rate,
                             float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
@@ -987,10 +994,16 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
                             const int64_t* cue_off, const double* ratios, int K, double start_seconds,
                             int64_t max_offset_samples, double* best_score, int32_t* best_offset,
                             int32_t* best_k, double* all_score, int32_t* all_offset, int memspace,
-                            bool gss = false, double* gss_ratio = nullptr, double* gss_evals = nullptr) {
+                            bool gss = false, double* gss_ratio = nullptr, double* gss_evals = nullptr,
+                            const AuditokArgs* aud = nullptr) {
   const bool resident = memspace == B2_DEVICE_RESIDENT;
   if (resident) memspace = B2_DEVICE;
-  const char* who = gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
+  const char* who = aud ? (gss ? "sync_tracks_auditok (search)" : "sync_tracks_auditok")
+                        : gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
+  // the run path and the GSS rounds need a reference of the two levels 1.0 and the label: auditok's clipped
+  // cumsum has them only at label 0 (starts and ends alternate and an overwrite only turns an end into a
+  // start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3)
+  const bool two_level = !aud || aud->non_speech_label == 0.0;
   if (V < 0 || T < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
     B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad arguments", who);
   if (track_video) {
@@ -1010,6 +1023,9 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
               "2 max_offset_samples <= %d offsets, one CTA of the run path)", kRunMaxWindow / 2, kRunMaxWindow);
     if (!std::isfinite(non_speech_label))
       B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: non_speech_label must be finite (the run path's two-level reference)");
+    if (!two_level)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: non_speech_label = %g gives the auditok signal more than two levels; the "
+              "search runs on the run path, which needs label 0", who, aud->non_speech_label);
     for (int t = 0; t < T; ++t)
       if (cue_off[t + 1] - cue_off[t] > kRunMaxCues)
         B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: track %d has %lld cues, more than %d", t,
@@ -1018,7 +1034,15 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   if (T == 0) return B2_OK;
   if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null output", who);
   if (gss && !gss_ratio) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null gss_ratio", who);
-  const int fpw = b2_vad_frames_per_window(frame_rate, sample_rate);
+  const int fpw = aud ? b2_auditok_block_size(frame_rate, sample_rate) : b2_vad_frames_per_window(frame_rate, sample_rate);
+  if (aud) {   // b2_vad_auditok's checks
+    if (fpw <= 0)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: int(frame_rate/sample_rate) block size and frame_rate//sample_rate window "
+              "size differ (or are 0) for %d / %d", who, frame_rate, sample_rate);
+    if (aud->max_length <= 0 || !(aud->min_length > 0) || aud->min_length > (double)aud->max_length ||
+        !(aud->max_continuous_silence < (double)aud->max_length) || aud->chunk_samples < 0)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad tokenizer parameters", who);
+  }
   if (fpw <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
   if (z_lo < 0) z_lo = 0;
   if (z_hi < 0) z_hi = (3 * fpw) / 8;
@@ -1037,8 +1061,44 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   for (int v = 0; v < V; ++v) {
     const int64_t n = pcm_off[v + 1] - pcm_off[v];
     if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
-    ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
+    if (!aud) ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
   }
+  // auditok: the reference's chunk loop.  Video v is cut into detector calls of chunk_samples samples (0: one
+  // call), chunks ch_first[v] .. ch_first[v+1]-1; chunk c spans samples ch_pcm[c] .. ch_pcm[c+1] of the PCM
+  // buffer and blocks ch_out[c] .. ch_out[c+1] of the reference signal, ceil(len/fpw) of them, so a video's
+  // signal is the sum over its chunks of ceil(len/fpw) long.  ch_tail[c]: the energy floor of the chunk's
+  // short last block (0: none).  Chunk starts are multiples of chunk_samples from the video's start
+  // ((2 fr // sr) * 5000 samples in the Python layer: a multiple of 8, so aligned videos stay eligible for
+  // the lane-per-window energy kernel).
+  std::vector<int64_t> ch_pcm, ch_out, ch_tail;
+  std::vector<int> ch_first;
+  if (aud) {
+    ch_first.assign(V + 1, 0);
+    ch_pcm.push_back(V ? pcm_off[0] : 0);
+    ch_out.push_back(0);
+    int tail_rem = -1;
+    int64_t tail_floor = 0;
+    for (int v = 0; v < V; ++v) {
+      const int64_t n = pcm_off[v + 1] - pcm_off[v];
+      const int64_t step = aud->chunk_samples > 0 ? aud->chunk_samples : (n > 0 ? n : 1);
+      for (int64_t s = 0; s < n; s += step) {
+        const int64_t len = std::min(step, n - s);
+        ch_pcm.push_back(pcm_off[v] + s + len);
+        ch_out.push_back(ch_out.back() + (len + fpw - 1) / fpw);
+        const int rem = (int)(len % fpw);
+        if (rem && rem != tail_rem) {
+          tail_rem = rem;
+          tail_floor = b2_auditok_energy_floor(rem, aud->energy_threshold_db);
+        }
+        ch_tail.push_back(rem ? tail_floor : 0);
+      }
+      ch_first[v + 1] = (int)ch_tail.size();
+      ref_off[v + 1] = ch_out.back();
+    }
+  }
+  const int64_t auditok_e_min = aud ? b2_auditok_energy_floor(fpw, aud->energy_threshold_db) : 0;
+  const B2TokenizerParams tok{aud ? aud->min_length : 0.0, aud ? aud->max_continuous_silence : 0.0,
+                              aud ? aud->non_speech_label : 0.0, aud ? (long long)aud->max_length : 0};
   // the lengths pass checks the cue times and ratios too; the offending input is looked for on failure
   if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
       rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, ratios, K, 0, sample_rate, lengths.data()) != B2_OK) {
@@ -1147,7 +1207,7 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
       B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + t0, nt, ratios, K, 0, nullptr,
                                sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
     const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds,
-                          non_speech_label};
+                          non_speech_label, two_level};
     B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
                             (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
                             o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
@@ -1179,8 +1239,28 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   // Cuts that would leave a sub-batch without tracks are dropped; a video without tracks has its VAD run in
   // the sub-batch of the next video that has tracks (trailing ones: of the last).  Where the cuts fall
   // changes no result.
+  // The detector step of the videos [v0, v1), on whichever stream the handle launches on: the energy / ZCR VAD
+  // into the reference-signal buffer, or for auditok the energy pass over the videos' chunks (label 0, every
+  // crossing count accepted, a short last block judged on its own samples) writing its 0/1 flags there, then
+  // the tokenizer turning each chunk's flags into its float32 signal in place.  Both auditok launches take a
+  // metadata arena from the ring of the stream they run on; on the pipeline's internal stream that ring is its
+  // own, so the GSS invariant (no later arena of a chain recycles the chain's arena, runcorr.cu b2i_gss_launch)
+  // holds as before: the chains' arenas come from the caller-facing ring, and with one sub-batch the detector's
+  // arenas there precede the chain's.
+  auto detect = [&](int v0, int v1) -> int {
+    if (!aud)
+      return b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label, (int64_t)fpw * energy_threshold,
+                            z_lo, z_hi, (float*)d_refsig, ref_off.data() + v0);
+    const int c0 = ch_first[v0], nc = ch_first[v1] - c0;
+    B2_TRY(b2i_vad_launch(h, d_pcm, ch_pcm.data() + c0, nc, fpw, 0.0f, auditok_e_min, 0, fpw, (float*)d_refsig,
+                          ch_out.data() + c0, ch_tail.data() + c0));
+    return b2i_tokenize_inplace_launch(h, (float*)d_refsig, ch_out.data() + c0, nc, tok);
+  };
   int n_sub = 1, vad_sms = 0;
-  if (T >= 96 && b2i_vad_lane_eligible(pcm_off, V, fpw)) {
+  // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks
+  const bool lane_ok = aud ? b2i_vad_lane_eligible(ch_pcm.data(), (int)ch_tail.size(), fpw)
+                           : b2i_vad_lane_eligible(pcm_off, V, fpw);
+  if (T >= 96 && lane_ok) {
     n_sub = 3;
     vad_sms = (h->sm_count * 54 + 50) / 100;
   }
@@ -1196,8 +1276,7 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   cut.push_back(V);
   n_sub = (int)cut.size() - 1;
   if (n_sub == 1) {
-    B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off, V, fpw, non_speech_label, (int64_t)fpw * energy_threshold, z_lo,
-                          z_hi, (float*)d_refsig, ref_off.data()));
+    B2_TRY(detect(0, V));
     B2_TRY(enqueue_chain(0, V));
   } else {
     std::vector<cudaEvent_t> vad_done(n_sub);
@@ -1233,9 +1312,7 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
         const int v0 = cut[i], v1 = cut[i + 1];
         h->vad_partition_sms = (i > 0 || prev_busy) ? vad_sms : 0;
         if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
-        const int st = b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label,
-                                      (int64_t)fpw * energy_threshold, z_lo, z_hi, (float*)d_refsig,
-                                      ref_off.data() + v0);
+        const int st = detect(v0, v1);
         h->vad_partition_sms = 0;
         if (st != B2_OK) return st;
         vad_done[i] = next_event(h);
@@ -1337,4 +1414,26 @@ extern "C" int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t
                           non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
                           ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
                           all_offset, memspace, /*gss=*/true, gss_ratio, gss_evals);
+}
+
+extern "C" int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                      const int32_t* track_video, int T, int frame_rate, int sample_rate,
+                                      double non_speech_label, double energy_threshold_db, double min_length,
+                                      int64_t max_length, double max_continuous_silence, int64_t chunk_samples,
+                                      const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                      const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                      int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                      int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                      double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_auditok");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_auditok: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_auditok: gss_evals without gss_ratio");
+  const AuditokArgs aud{non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
+                        chunk_samples};
+  // the energy / ZCR arguments are unused: z_lo / z_hi < 0 select defaults, the threshold is never read
+  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                          (float)non_speech_label, 0, -1, -1, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K,
+                          start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score, all_offset,
+                          memspace, /*gss=*/gss_ratio != nullptr, gss_ratio, gss_evals, &aud);
 }

@@ -171,6 +171,10 @@ struct B2TokenizerParams {
 // flags / out share the offset table off_host[n_chunks + 1] (one detector call per chunk)
 int b2i_tokenize_launch(b2_ctx* h, const float* d_flags, const int64_t* off_host, int n_chunks,
                         const B2TokenizerParams& tp, double* d_out);
+// The same scan writing float32 over its own flags (the energy pass's label-0 output): the reference
+// signal of b2_sync_tracks_auditok, built in place in the reference-signal buffer.
+int b2i_tokenize_inplace_launch(b2_ctx* h, float* d_flags_sig, const int64_t* off_host, int n_chunks,
+                                const B2TokenizerParams& tp);
 int b2i_synth_launch(b2_ctx* h, const uint8_t* d_cls, int64_t n_windows, int fpw, uint32_t seed,
                      int16_t* d_out);
 int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
@@ -192,7 +196,9 @@ struct B2CueSource {
   const double* ratios;      // [K]
   int sample_rate;
   double start_seconds;
-  float ref_label;           // the reference is this call's VAD output: every value is 1.0f or ref_label
+  float ref_label;           // the reference is this call's VAD output: every value is 1.0f or ref_label ...
+  bool ref_two_level;        // ... when this is set (the run path and the GSS rounds rely on it); the auditok
+                             // signal is a clipped cumsum with other levels unless its label is 0
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);

@@ -752,8 +752,9 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   // (runcorr.cu) scores every offset of the window from the cue runs, exactly up to a float64 margin, when
   // its work (cues x window) is below the FFT blocks it replaces for every live job.  A capture of the
   // nominations (b2_capture_nominations) probes the FFT paths and keeps them, unless B2_ALIGN_PATH=runs asks
-  // for the run path (then its float64 scores are captured).
-  if (cue_mode && (!capture || force_runs) && !use_big && std::isfinite(cue_src->ref_label) &&
+  // for the run path (then its float64 scores are captured).  A reference with further levels (auditok at a
+  // non-zero label) stays on the FFT paths, which read its values as they are, even under B2_ALIGN_PATH=runs.
+  if (cue_mode && (!capture || force_runs) && !use_big && cue_src->ref_two_level && std::isfinite(cue_src->ref_label) &&
       !(path_env && !strcmp(path_env, "tiled"))) {
     bool fits = true, pays = true;
     int max_runs = 1;

@@ -31,10 +31,12 @@ import numpy as np
 
 from . import _native
 from .constants import (
+    CHUNK_WINDOWS,
     DEFAULT_ENERGY_THRESHOLD,
     DEFAULT_SCALE_FACTOR,
     DEFAULT_START_SECONDS,
     SAMPLE_RATE,
+    detector_chunk_bytes,
 )
 from .sklearn_shim import Pipeline, TransformerMixin
 from .subtitle_transformers import SubtitleScaler
@@ -350,12 +352,12 @@ class VideoSpeechTransformer(TransformerMixin):
         return proc.stdout, None, proc.wait
 
     # -- chunk loop (speech_transformers.py:680-753) -------------------------------------------------
-    CHUNK_WINDOWS: int = 10000   # 100 s per detector call at the 100 Hz sample rate (:711,741)
+    CHUNK_WINDOWS: int = CHUNK_WINDOWS   # 100 s per detector call at the 100 Hz sample rate (:711,741)
 
     def _chunks(self, readable):
         """PCM in the reference's read granularity: 10 000 windows of ``2 * frame_rate // sample_rate``
         bytes each (:710-711,741)."""
-        n = (2 * self.frame_rate // self.sample_rate) * self.CHUNK_WINDOWS
+        n = detector_chunk_bytes(self.frame_rate, self.sample_rate, self.CHUNK_WINDOWS)
         while True:
             data = readable.read(n)
             if not data:

@@ -242,6 +242,31 @@ int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /
                        double* all_score /* [T*(K+1)] or NULL */, int32_t* all_offset /* [T*(K+1)] or NULL */,
                        double* gss_ratio /* [T] */, double* gss_evals /* [T*17] or NULL */, int memspace);
 
+/* ---- the whole hot path with the reference's auditok detector (--vad auditok) ----------------------------
+ * `ffs movie.mkv -i a.srt ... --vad auditok [--gss]` for V videos and T tracks.  Track t gets exactly what this
+ * composition of public calls returns: b2_vad_auditok on the PCM of video track_video[t] with these detector
+ * arguments and chunk_samples, rounded once to float32, then b2_sync_tracks (b2_sync_tracks_gss when gss_ratio is
+ * not NULL) with that signal in place of the energy / ZCR VAD output.  Detector arguments as for b2_vad_auditok
+ * (B2_ERR_UNSUPPORTED for a block-size mismatch, B2_ERR_BAD_ARG for bad tokenizer parameters); each video is cut
+ * into detector calls of chunk_samples samples and the tokenizer restarts in every call, so a video's reference
+ * signal holds the sum over its chunks of ceil(len/fpw) blocks.  Every other argument as for b2_sync_tracks /
+ * b2_sync_tracks_gss: gss_ratio NULL = the grid only, all_* [T*K]; else gss_ratio [T], gss_evals [T*17] or NULL,
+ * all_* [T*(K+1)].  The search needs non_speech_label == 0 (only then is the signal two-level, 1.0 and 0.0; the
+ * rounds run on the run path): any other label is B2_ERR_UNSUPPORTED with gss_ratio.  Grid calls with another
+ * label align on the FFT paths.  memspace: B2_HOST, B2_DEVICE or B2_DEVICE_RESIDENT; resident calls chain with
+ * b2_sync_batch, b2_sync_tracks and b2_sync_tracks_gss in any order.  The pair form (b2_sync_batch) is the
+ * identity track map. */
+int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_off /* [V+1] */, int V,
+                           const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                           double non_speech_label, double energy_threshold_db, double min_length, int64_t max_length,
+                           double max_continuous_silence, int64_t chunk_samples,
+                           const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                           const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                           int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                           double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                           double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                           int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before

@@ -8,7 +8,7 @@ kernels (lane-group: vector path, generic path, ragged tails; lane-per-window: m
 one CTA reusing its ring many times); the auditok energy + tokenizer scan; both rasterisers;
 boundaries; blend; the correlation kernels (float and bit-mask subtitle signals, a multi-block job,
 the split-block small batch path), the run path (reference bits, run correlation), candidate selection, exact re-score, pick and the ratio
-reduction; b2_sync_batch with and without the sub-batch pipeline.  Results are checked against the
+reduction; b2_sync_batch with and without the sub-batch pipeline; b2_sync_tracks_auditok (grid and search).  Results are checked against the
 oracle so that a run under the sanitizer is also a parity run.
 """
 import os
@@ -106,6 +106,20 @@ def main():
                          np.tile(ends, 2), None, cue_off, BENCH_RATIOS, 0.0, 6000, want_all=True)
     os.environ.pop("B2_ALIGN_PATH")
     assert all(np.array_equal(a, b) for a, b in zip(j_all, j_fft))
+    # ---- the auditok detector inside the batched sync (energy pass + in-place tokenizer), grid and search, against
+    # the per-stage composition (the reference signal is two-level at label 0, so the run path may read it)
+    chunk = 160 * 7000
+    ba = BatchSynchronizer(BENCH_RATIOS, 16000, 100, 0.0, max_offset_seconds=60, device=0, vad="auditok")
+    got = h.sync_tracks_auditok(pcm, args[1], [0, 1], 16000, 100, 0.0, args[2], args[3], None, cue_off, BENCH_RATIOS,
+                                0.0, 6000, chunk, want_all=True)
+    ref64, ref_off = h.vad_auditok(pcm, args[1], 16000, 100, 0.0, chunk_samples=chunk)
+    sub, sub_off = h.rasterize(args[2], args[3], None, cue_off, BENCH_RATIOS, 5, False, 100, 0.0)
+    sc, of, stt = h.align_batch(ref64.astype(np.float32), ref_off, sub, sub_off, 2, 5, 6000)
+    assert np.array_equal(got[3], sc) and np.array_equal(got[4], of)
+    g = h.sync_tracks_auditok(pcm, args[1], [0, 1], 16000, 100, 0.0, args[2], args[3], None, cue_off, BENCH_RATIOS,
+                              0.0, 6000, chunk, gss=True)
+    assert np.isfinite(g[5]).all()
+    ba.sync_host(*args)
     h.synchronize()
     print("sanitize_smoke ok")
 

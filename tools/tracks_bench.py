@@ -40,8 +40,10 @@ def gpu_info():
     return out
 
 
-def make_tracks(handle, V, T, duration_s, ratios, seed0):
-    """V videos; track i of video v is the video's master cue list at its own ratio and delay (planted)."""
+def make_tracks(handle, V, T, duration_s, ratios, seed0, flip=0.10, hiss_fraction=0.05):
+    """V videos; track i of video v is the video's master cue list at its own ratio and delay (planted).  A video's
+    windows are voiced where its master list has speech, a fraction `flip` of them flipped, and `hiss_fraction` of
+    the rest loud hiss (the random draws do not depend on the fractions, so the cue lists do not either)."""
     from ffsubsync_b200.synth import synthetic_cues
     n = int(duration_s * SAMPLE_RATE)
     cls = np.zeros(V * n, dtype=np.uint8)
@@ -54,8 +56,8 @@ def make_tracks(handle, V, T, duration_s, ratios, seed0):
         rng = np.random.RandomState(seed + 100003)
         ref = np.zeros(n, dtype=bool)
         ref[: len(mask)] = mask
-        ref ^= rng.rand(n) < 0.10
-        hiss = rng.rand(n) < 0.05
+        ref ^= rng.rand(n) < flip
+        hiss = rng.rand(n) < hiss_fraction
         cls[v * n:(v + 1) * n] = np.where(ref, 1, np.where(hiss, 2, 0))
         for _ in range(T):
             k, delta = int(rng.randint(len(ratios))), int(rng.randint(-3000, 3001))
