@@ -29,8 +29,9 @@ EXPORTS = [
     "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
-    "b2_sync_tracks_auditok",
+    "b2_sync_tracks_auditok", "b2_sync_tracks_subs",
 ]
+B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
 
 
@@ -97,6 +98,10 @@ def load() -> ctypes.CDLL:
                                                ctypes.c_int, _f64, _f64, _f64, _i64, _f64, _i64, _vp, _vp, _vp,
                                                _vp, _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp,
                                                _vp, ctypes.c_int]
+        lib.b2_sync_tracks_subs.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                            ctypes.c_int, _f64, _i64, ctypes.c_int, ctypes.c_int, _f64, _f64, _i64,
+                                            _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int,
+                                            _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -516,6 +521,70 @@ class Handle:
             _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
             _ptr(gss_evals) if gss else None, memspace)
         self._check(st, "b2_sync_tracks_auditok")
+        res = (best_score, best_offset, best_k, all_score, all_offset)
+        return res + (gss_ratio, gss_evals) if gss else res
+
+    def sync_tracks_subs(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
+                         ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, ref_cue_off, cue_start_s,
+                         cue_end_s, cue_keep, cue_off, ratios, start_seconds: float,
+                         max_offset_samples: Optional[int], detector: int = B2_DETECTOR_ENERGY_ZCR,
+                         energy_threshold: int = 0, z_lo: int = -1, z_hi: int = -1, chunk_samples: int = 0,
+                         energy_threshold_db: float = 50.0, min_length: Optional[float] = None,
+                         max_length: Optional[int] = None, max_continuous_silence: Optional[float] = None,
+                         gss: bool = False, best_score=None, best_offset=None, best_k=None, all_score=None,
+                         all_offset=None, gss_ratio=None, gss_evals=None, want_all: bool = False,
+                         want_evals: bool = False, memspace: int = B2_HOST):
+        """sync_tracks / sync_tracks_auditok where the videos with ref_is_subs[v] != 0 take their subtitle stream
+        (reference cues ref_cue_off[v] .. ref_cue_off[v+1], host arrays) as reference signal instead of the
+        detector's output (b2_sync_tracks_subs).  pcm may be None when no video has samples.  detector:
+        B2_DETECTOR_ENERGY_ZCR (energy_threshold, z_lo, z_hi) or B2_DETECTOR_AUDITOK (chunk_samples and the
+        tokenizer arguments, defaults as for vad_auditok).  Returns (best_score, best_offset, best_k, all_score,
+        all_offset), plus (gss_ratio, gss_evals) with gss=True (all_* then [T*(K+1)])."""
+        pcm_off, cue_off, ref_cue_off = _i64a(pcm_off), _i64a(cue_off), _i64a(ref_cue_off)
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        V, T = len(pcm_off) - 1, len(track_video)
+        if len(cue_off) != T + 1 or len(ref_cue_off) != V + 1:
+            raise NativeError(-1, "b2_sync_tracks_subs", "cue_off / ref_cue_off have %d / %d entries for %d tracks / "
+                              "%d videos" % (len(cue_off), len(ref_cue_off), T, V))
+        ref_is_subs = None if ref_is_subs is None else np.ascontiguousarray(ref_is_subs, dtype=np.uint8)
+        if ref_is_subs is not None and len(ref_is_subs) != V:
+            raise NativeError(-1, "b2_sync_tracks_subs", "ref_is_subs has %d entries for %d videos"
+                              % (len(ref_is_subs), V))
+        ref_cue_start_s = np.ascontiguousarray(ref_cue_start_s, dtype=np.float64)
+        ref_cue_end_s = np.ascontiguousarray(ref_cue_end_s, dtype=np.float64)
+        ref_cue_keep = None if ref_cue_keep is None else np.ascontiguousarray(ref_cue_keep, dtype=np.uint8)
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        K = len(ratios)
+        min_length = 0.2 * sample_rate if min_length is None else min_length
+        max_length = int(5 * sample_rate) if max_length is None else max_length
+        max_continuous_silence = 0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
+        mos = _mask_width(max_offset_samples)
+        cols = K + 1 if gss else K
+        if memspace == B2_HOST:
+            pcm = None if pcm is None else np.ascontiguousarray(pcm, dtype=np.int16)
+            best_score = np.empty(T, dtype=np.float64)
+            best_offset = np.empty(T, dtype=np.int32)
+            best_k = np.empty(T, dtype=np.int32)
+            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
+            if want_all:
+                all_score = np.empty(T * cols, dtype=np.float64)
+                all_offset = np.empty(T * cols, dtype=np.int32)
+            if gss and want_evals:
+                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
+        elif gss and gss_ratio is None:
+            raise ValueError("sync_tracks_subs(gss=True) on device memory needs gss_ratio")
+        st = self.lib.b2_sync_tracks_subs(
+            self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate, sample_rate, int(detector),
+            float(non_speech_label), int(energy_threshold), int(z_lo), int(z_hi), float(energy_threshold_db),
+            float(min_length), int(max_length), float(max_continuous_silence), int(chunk_samples), _ptr(ref_is_subs),
+            _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep), _ptr(ref_cue_off), _ptr(cue_start_s),
+            _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos,
+            _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset),
+            _ptr(gss_ratio) if gss else None, _ptr(gss_evals) if gss else None, memspace)
+        self._check(st, "b2_sync_tracks_subs")
         res = (best_score, best_offset, best_k, all_score, all_offset)
         return res + (gss_ratio, gss_evals) if gss else res
 

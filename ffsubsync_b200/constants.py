@@ -12,6 +12,8 @@ DEFAULT_SCALE_FACTOR: float = 1
 DEFAULT_MAX_OFFSET_SECONDS: int = 60        # constants.py:18
 DEFAULT_VAD: str = "energy_zcr"             # the detector this package implements
 BATCH_VADS = ("energy_zcr", "auditok")      # detectors the batched sync calls run
+# ... and with a video's embedded subtitle stream as its reference where the caller hands one over
+BATCH_VADS += ("subs_then_energy_zcr", "subs_then_auditok")
 
 # energy / zero-crossing detector defaults (DESIGN.md): auditok's energy_threshold=50 dB
 # (speech_transformers.py:125) is mean(x^2) >= 1e5

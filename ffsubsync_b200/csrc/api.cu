@@ -986,6 +986,15 @@ struct AuditokArgs {
   double non_speech_label, energy_threshold_db, min_length, max_continuous_silence;
   int64_t max_length, chunk_samples;
 };
+// b2_sync_tracks_subs: videos with is_subs[v] != 0 take their cue list ref_off[v] .. ref_off[v+1] (host arrays,
+// absolute indices), rasterised at ratio 1.0 and level 1.0, as reference signal instead of the detector's output.
+struct SubsRefArgs {
+  const uint8_t* is_subs;
+  const double* cue_start_s;
+  const double* cue_end_s;
+  const uint8_t* cue_keep;   // may be null
+  const int64_t* cue_off;    // [V+1]
+};
 
 static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm, const int64_t* pcm_off, int V,
                             const int32_t* track_video, int T, int frame_rate, int sample_rate,
@@ -995,17 +1004,46 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
                             int64_t max_offset_samples, double* best_score, int32_t* best_offset,
                             int32_t* best_k, double* all_score, int32_t* all_offset, int memspace,
                             bool gss = false, double* gss_ratio = nullptr, double* gss_evals = nullptr,
-                            const AuditokArgs* aud = nullptr) {
+                            const AuditokArgs* aud = nullptr, const SubsRefArgs* subs = nullptr) {
   const bool resident = memspace == B2_DEVICE_RESIDENT;
   if (resident) memspace = B2_DEVICE;
-  const char* who = aud ? (gss ? "sync_tracks_auditok (search)" : "sync_tracks_auditok")
-                        : gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
-  // the run path and the GSS rounds need a reference of the two levels 1.0 and the label: auditok's clipped
-  // cumsum has them only at label 0 (starts and ends alternate and an overwrite only turns an end into a
-  // start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3)
-  const bool two_level = !aud || aud->non_speech_label == 0.0;
+  const char* who = subs ? (gss ? "sync_tracks_subs (search)" : "sync_tracks_subs")
+                    : aud ? (gss ? "sync_tracks_auditok (search)" : "sync_tracks_auditok")
+                          : gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
   if (V < 0 || T < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
     B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad arguments", who);
+  // b2_sync_tracks_subs: which videos take a subtitle reference, checked before anything reads their tables
+  bool any_subs = false, any_audio = !subs;
+  int64_t audio_samples = 0;
+  if (subs) {
+    for (int v = 0; v < V; ++v) {
+      const bool is_subs = subs->is_subs && subs->is_subs[v];
+      if (subs->cue_off[v + 1] < subs->cue_off[v])
+        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: ref_cue_off not monotone at %d", who, v);
+      if (!is_subs && subs->cue_off[v + 1] != subs->cue_off[v])
+        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: video %d has reference cues but no subtitle reference (ref_is_subs[%d] = 0)",
+                who, v, v);
+      if (is_subs && pcm_off[v + 1] != pcm_off[v])
+        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: video %d has a subtitle reference and a non-empty PCM range (%lld samples); "
+                "its audio is never read", who, v, (long long)(pcm_off[v + 1] - pcm_off[v]));
+      any_subs = any_subs || is_subs;
+      any_audio = any_audio || !is_subs;
+      if (pcm_off[v + 1] > pcm_off[v]) audio_samples += pcm_off[v + 1] - pcm_off[v];
+    }
+    if (V > 0 && subs->cue_off[V] > subs->cue_off[0] && (!subs->cue_start_s || !subs->cue_end_s))
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null reference cue arrays", who);
+    if (audio_samples > 0 && !pcm) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null pcm with %lld samples of audio", who,
+                                           (long long)audio_samples);
+  }
+  // The run path and the GSS rounds need a reference of the two levels 1.0 and ref_label.  The detector's signal
+  // has the levels 1.0 and the label, a subtitle reference 1.0 and 0.0, so ref_label is the label unless every
+  // reference is a subtitle stream; a call that mixes the two at a non-zero label has three levels.  auditok's
+  // clipped cumsum has two levels only at label 0 (starts and ends alternate and an overwrite only turns an end
+  // into a start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3).
+  const float ref_label = any_audio ? non_speech_label : 0.0f;
+  const bool auditok_two_level = !aud || aud->non_speech_label == 0.0;
+  const bool mix_two_level = !any_subs || non_speech_label == 0.0f;
+  const bool two_level = !any_audio || (auditok_two_level && mix_two_level);
   if (track_video) {
     for (int t = 0; t < T; ++t)
       if (track_video[t] < 0 || track_video[t] >= V || (t > 0 && track_video[t] < track_video[t - 1]))
@@ -1021,11 +1059,15 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
         max_offset_samples > (int64_t)(kRunMaxWindow / 2))
       B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: max_offset_samples must lie in [0, %d] (a window of at most "
               "2 max_offset_samples <= %d offsets, one CTA of the run path)", kRunMaxWindow / 2, kRunMaxWindow);
-    if (!std::isfinite(non_speech_label))
+    if (!std::isfinite(ref_label))
       B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: non_speech_label must be finite (the run path's two-level reference)");
-    if (!two_level)
+    if (!two_level && !auditok_two_level)
       B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: non_speech_label = %g gives the auditok signal more than two levels; the "
               "search runs on the run path, which needs label 0", who, aud->non_speech_label);
+    if (!two_level)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: subtitle references (levels 1 and 0) and audio references (levels 1 and "
+              "non_speech_label = %g) in one call give three levels; the search runs on the run path, which needs "
+              "label 0 or references of one kind", who, (double)non_speech_label);
     for (int t = 0; t < T; ++t)
       if (cue_off[t + 1] - cue_off[t] > kRunMaxCues)
         B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: track %d has %lld cues, more than %d", t,
@@ -1058,10 +1100,33 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   const size_t J = (size_t)T * K;
   std::vector<int64_t> ref_off(V + 1), sub_off(J + 1), lengths(J);
   ref_off[0] = 0;
+  // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
+  // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
+  // the tracks' cues).  sub_video: the videos with a subtitle reference, ascending.
+  std::vector<int64_t> subs_len;
+  std::vector<int> sub_video;
+  if (any_subs) {
+    const double one = 1.0;
+    subs_len.resize(V);
+    if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
+        rasterize_lengths(subs->cue_start_s, subs->cue_end_s, subs->cue_off, V, &one, 1, 0, sample_rate,
+                          subs_len.data()) != B2_OK) {
+      int64_t bad_at;
+      double bad_val;
+      const char* why = bad_cue_input(subs->cue_start_s, subs->cue_end_s, subs->cue_off, V, &one, 1, 0, start_seconds,
+                                      &bad_at, &bad_val);
+      if (!why) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad reference cue list", who);
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: reference %s (index %lld: %g)", who, why, (long long)bad_at, bad_val);
+    }
+    for (int v = 0; v < V; ++v)
+      if (subs->is_subs[v]) sub_video.push_back(v);
+  }
+  auto is_subs = [&](int v) { return any_subs && subs->is_subs[v] != 0; };
   for (int v = 0; v < V; ++v) {
     const int64_t n = pcm_off[v + 1] - pcm_off[v];
     if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
-    if (!aud) ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
+    if (is_subs(v)) ref_off[v + 1] = ref_off[v] + subs_len[v];
+    else if (!aud) ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
   }
   // auditok: the reference's chunk loop.  Video v is cut into detector calls of chunk_samples samples (0: one
   // call), chunks ch_first[v] .. ch_first[v+1]-1; chunk c spans samples ch_pcm[c] .. ch_pcm[c+1] of the PCM
@@ -1070,16 +1135,28 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   // short last block (0: none).  Chunk starts are multiples of chunk_samples from the video's start
   // ((2 fr // sr) * 5000 samples in the Python layer: a multiple of 8, so aligned videos stay eligible for
   // the lane-per-window energy kernel).
-  std::vector<int64_t> ch_pcm, ch_out, ch_tail;
-  std::vector<int> ch_first;
+  // A video with a subtitle reference (no PCM) is one empty chunk spanning its reference's frames: the energy
+  // pass has no tiles there and the tokenizer's table (tok_*) leaves it out, so only the rasteriser writes it.
+  std::vector<int64_t> ch_pcm, ch_out, ch_tail, tok_off, tok_end;
+  std::vector<int> ch_first, tok_first;
   if (aud) {
     ch_first.assign(V + 1, 0);
     ch_pcm.push_back(V ? pcm_off[0] : 0);
     ch_out.push_back(0);
+    if (any_subs) tok_first.assign(V + 1, 0);
     int tail_rem = -1;
     int64_t tail_floor = 0;
     for (int v = 0; v < V; ++v) {
       const int64_t n = pcm_off[v + 1] - pcm_off[v];
+      if (is_subs(v)) {
+        ch_pcm.push_back(pcm_off[v + 1]);
+        ch_out.push_back(ch_out.back() + subs_len[v]);
+        ch_tail.push_back(0);
+        ch_first[v + 1] = (int)ch_tail.size();
+        tok_first[v + 1] = (int)tok_off.size();
+        ref_off[v + 1] = ch_out.back();
+        continue;
+      }
       const int64_t step = aud->chunk_samples > 0 ? aud->chunk_samples : (n > 0 ? n : 1);
       for (int64_t s = 0; s < n; s += step) {
         const int64_t len = std::min(step, n - s);
@@ -1091,8 +1168,13 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
           tail_floor = b2_auditok_energy_floor(rem, aud->energy_threshold_db);
         }
         ch_tail.push_back(rem ? tail_floor : 0);
+        if (any_subs) {
+          tok_off.push_back(ch_out[ch_out.size() - 2]);
+          tok_end.push_back(ch_out.back());
+        }
       }
       ch_first[v + 1] = (int)ch_tail.size();
+      if (any_subs) tok_first[v + 1] = (int)tok_off.size();
       ref_off[v + 1] = ch_out.back();
     }
   }
@@ -1182,7 +1264,7 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
     }
   }
   const int16_t* d_pcm = pcm;
-  if (memspace == B2_HOST) {
+  if (memspace == B2_HOST && !(subs && !pcm)) {   // (without any audio b2_sync_tracks_subs may take no pcm)
     void* dp;
     B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, pcm, (size_t)pcm_off[V] * 2, &dp));
     d_pcm = (const int16_t*)dp;
@@ -1207,7 +1289,7 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
       B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + t0, nt, ratios, K, 0, nullptr,
                                sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
     const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds,
-                          non_speech_label, two_level};
+                          ref_label, two_level};
     B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
                             (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
                             o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
@@ -1247,14 +1329,31 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   // own, so the GSS invariant (no later arena of a chain recycles the chain's arena, runcorr.cu b2i_gss_launch)
   // holds as before: the chains' arenas come from the caller-facing ring, and with one sub-batch the detector's
   // arenas there precede the chain's.
+  // With subtitle references (b2_sync_tracks_subs) the step also rasterises those of the videos [v0, v1) into
+  // their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
+  // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
   auto detect = [&](int v0, int v1) -> int {
-    if (!aud)
-      return b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label, (int64_t)fpw * energy_threshold,
-                            z_lo, z_hi, (float*)d_refsig, ref_off.data() + v0);
-    const int c0 = ch_first[v0], nc = ch_first[v1] - c0;
-    B2_TRY(b2i_vad_launch(h, d_pcm, ch_pcm.data() + c0, nc, fpw, 0.0f, auditok_e_min, 0, fpw, (float*)d_refsig,
-                          ch_out.data() + c0, ch_tail.data() + c0));
-    return b2i_tokenize_inplace_launch(h, (float*)d_refsig, ch_out.data() + c0, nc, tok);
+    if (!aud) {
+      B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label, (int64_t)fpw * energy_threshold,
+                            z_lo, z_hi, (float*)d_refsig, ref_off.data() + v0));
+    } else {
+      const int c0 = ch_first[v0], nc = ch_first[v1] - c0;
+      B2_TRY(b2i_vad_launch(h, d_pcm, ch_pcm.data() + c0, nc, fpw, 0.0f, auditok_e_min, 0, fpw, (float*)d_refsig,
+                            ch_out.data() + c0, ch_tail.data() + c0));
+      if (!any_subs) return b2i_tokenize_inplace_launch(h, (float*)d_refsig, ch_out.data() + c0, nc, tok);
+      const int k0 = tok_first[v0];
+      B2_TRY(b2i_tokenize_inplace_launch(h, (float*)d_refsig, tok_off.data() + k0, tok_first[v1] - k0, tok,
+                                         tok_end.data() + k0));
+    }
+    if (!any_subs) return B2_OK;
+    const int s0 = (int)(std::lower_bound(sub_video.begin(), sub_video.end(), v0) - sub_video.begin());
+    const int s1 = (int)(std::lower_bound(sub_video.begin(), sub_video.end(), v1) - sub_video.begin());
+    if (s1 == s0) return B2_OK;
+    std::vector<int> rel(sub_video.begin() + s0, sub_video.begin() + s1);
+    for (int& v : rel) v -= v0;
+    return b2i_raster_ref_launch(h, subs->cue_start_s, subs->cue_end_s, subs->cue_keep, subs->cue_off + v0,
+                                 ref_off.data() + v0, v1 - v0, rel.data(), (int)rel.size(), sample_rate, start_seconds,
+                                 (float*)d_refsig);
   };
   int n_sub = 1, vad_sms = 0;
   // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks
@@ -1436,4 +1535,40 @@ extern "C" int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int
                           (float)non_speech_label, 0, -1, -1, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K,
                           start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score, all_offset,
                           memspace, /*gss=*/gss_ratio != nullptr, gss_ratio, gss_evals, &aud);
+}
+
+extern "C" int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                   const int32_t* track_video, int T, int frame_rate, int sample_rate, int detector,
+                                   double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                                   double energy_threshold_db, double min_length, int64_t max_length,
+                                   double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs,
+                                   const double* ref_cue_start_s, const double* ref_cue_end_s,
+                                   const uint8_t* ref_cue_keep, const int64_t* ref_cue_off,
+                                   const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                   const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                   int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                   int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                   double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_subs");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_subs: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_subs: gss_evals without gss_ratio");
+  if (V > 0 && (!pcm_off || !ref_cue_off)) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_subs: null pcm_off / ref_cue_off");
+  if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_subs: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, "
+            "not %d", detector);
+  const int64_t no_cues[1] = {0};
+  const SubsRefArgs subs{ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : no_cues};
+  const bool gss = gss_ratio != nullptr;
+  if (detector == B2_DETECTOR_ENERGY_ZCR)
+    return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                            (float)non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep,
+                            cue_off, ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k,
+                            all_score, all_offset, memspace, gss, gss_ratio, gss_evals, nullptr, &subs);
+  const AuditokArgs aud{non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
+                        chunk_samples};
+  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                          (float)non_speech_label, 0, -1, -1, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K,
+                          start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score, all_offset,
+                          memspace, gss, gss_ratio, gss_evals, &aud, &subs);
 }

@@ -172,15 +172,23 @@ struct B2TokenizerParams {
 int b2i_tokenize_launch(b2_ctx* h, const float* d_flags, const int64_t* off_host, int n_chunks,
                         const B2TokenizerParams& tp, double* d_out);
 // The same scan writing float32 over its own flags (the energy pass's label-0 output): the reference
-// signal of b2_sync_tracks_auditok, built in place in the reference-signal buffer.
+// signal of b2_sync_tracks_auditok, built in place in the reference-signal buffer.  end_host (nullable,
+// [n_chunks]): chunk c spans off_host[c] .. end_host[c] (chunks need not abut: b2_sync_tracks_subs leaves
+// the subtitle references' ranges out); null = off_host[c + 1].
 int b2i_tokenize_inplace_launch(b2_ctx* h, float* d_flags_sig, const int64_t* off_host, int n_chunks,
-                                const B2TokenizerParams& tp);
+                                const B2TokenizerParams& tp, const int64_t* end_host = nullptr);
 int b2i_synth_launch(b2_ctx* h, const uint8_t* d_cls, int64_t n_windows, int fpw, uint32_t seed,
                      int16_t* d_out);
 int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
                       const uint8_t* cue_keep, const int64_t* cue_off, int B, const double* ratios,
                       int K, int per_pair_ratios, const double* levels, int sample_rate,
                       double start_seconds, float* d_out, const int64_t* out_off_host);
+// Subtitle references of b2_sync_tracks_subs: for each of the n_subs videos videos[i] (indices into the host
+// tables cue_off / out_off [n_videos + 1], absolute), zero d_out[out_off[v] .. out_off[v+1]) and write 1.0 over
+// its kept cues at ratio 1.0 - b2_rasterize at ratio 1.0 and level 1.0, at per-video bases.
+int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_end, const uint8_t* cue_keep,
+                          const int64_t* cue_off, const int64_t* out_off, int n_videos, const int* videos, int n_subs,
+                          int sample_rate, double start_seconds, float* d_out);
 int b2i_bounds_launch(b2_ctx* h, const float* d_sig, const int64_t* off_host, int n,
                       int64_t* d_first, int64_t* d_last);
 int b2i_blend_launch(b2_ctx* h, const float* d_a, const float* d_b, int64_t n, int mode, double wa,
@@ -196,9 +204,10 @@ struct B2CueSource {
   const double* ratios;      // [K]
   int sample_rate;
   double start_seconds;
-  float ref_label;           // the reference is this call's VAD output: every value is 1.0f or ref_label ...
-  bool ref_two_level;        // ... when this is set (the run path and the GSS rounds rely on it); the auditok
-                             // signal is a clipped cumsum with other levels unless its label is 0
+  float ref_label;           // the reference is this call's detector output (or subtitle references, 1.0 / 0.0):
+  bool ref_two_level;        // every value is 1.0f or ref_label when this is set (the run path and the GSS rounds
+                             // rely on it); the auditok signal is a clipped cumsum with other levels unless its label
+                             // is 0, and subtitle and audio references mixed at a non-zero label have three levels
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);

@@ -101,6 +101,39 @@ __global__ void __launch_bounds__(256) raster_bits_kernel(RasterBitsParams p) {
   }
 }
 
+// K2r: embedded-subtitle references (b2_sync_tracks_subs): the reference signal of a video with a subtitle
+// stream is its cue list rasterised at ratio 1.0 and level 1.0 (SubtitleScaler(1.0) +
+// SubtitleSpeechTransformer, speech_transformers.py:479-523), written into the reference-signal buffer at
+// the video's own base between the detector's outputs.  One CTA per such video: zero the signal, then one
+// warp per cue with the same cue arithmetic as raster_cues_kernel.
+struct RasterRefParams {
+  const double* start_s;
+  const double* end_s;
+  const uint8_t* keep;        // may be null
+  const long long* cue_off;   // [n_videos+1] absolute
+  const long long* out_off;   // [n_videos+1] the reference-signal buffer's offsets
+  const int* video;           // [grid.x] the videos (indices into cue_off / out_off) with a subtitle reference
+  float* out;
+  int sample_rate;
+  double start_seconds;
+};
+
+__global__ void __launch_bounds__(256) raster_ref_kernel(RasterRefParams p) {
+  const int v = p.video[blockIdx.x];
+  const long long c0 = p.cue_off[v], c1 = p.cue_off[v + 1];
+  const long long n = p.out_off[v + 1] - p.out_off[v];
+  float* out = p.out + p.out_off[v];
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) out[i] = 0.0f;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  for (long long c = c0 + (threadIdx.x >> 5); c < c1; c += blockDim.x >> 5) {
+    if (p.keep && !p.keep[c]) continue;
+    long long first, last;
+    b2_cue_bounds(p.start_s[c], p.end_s[c], 1.0, p.start_seconds, p.sample_rate, n, first, last);
+    for (long long i = first + lane; i < last; i += 32) out[i] = 1.0f;
+  }
+}
+
 // ---- K7 -------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) bounds_kernel(const float* __restrict__ sig,
                                                       const long long* __restrict__ off, int n_sig,
@@ -230,6 +263,33 @@ int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
     raster_cues_kernel<<<grid, 256, 0, h->stream>>>(p);
     B2_CHECK_LAUNCH(h, "raster_cues_kernel");
   }
+  return B2_OK;
+}
+
+int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_end, const uint8_t* cue_keep,
+                          const int64_t* cue_off, const int64_t* out_off, int n_videos, const int* videos, int n_subs,
+                          int sample_rate, double start_seconds, float* d_out) {
+  if (n_subs <= 0) return B2_OK;
+  B2Range range("b2:raster_ref");
+  // cue_off / out_off are slices of the call's tables (a sub-batch): entries are absolute, only
+  // [cue_off[0], cue_off[n_videos]) is uploaded (pointers rebased)
+  const size_t c0 = (size_t)cue_off[0], nc = (size_t)cue_off[n_videos] - c0;
+  const size_t tbl = (size_t)(n_videos + 1) * 8;
+  MetaArena a;
+  B2_TRY(b2i_meta_begin(h, &a, nc * 17 + 2 * tbl + (size_t)n_subs * 4 + 1024));
+  RasterRefParams p;
+  p.start_s = (const double*)b2i_meta_put(&a, cue_start + c0, nc * 8) - c0;
+  p.end_s = (const double*)b2i_meta_put(&a, cue_end + c0, nc * 8) - c0;
+  p.keep = cue_keep ? (const uint8_t*)b2i_meta_put(&a, cue_keep + c0, nc) - c0 : nullptr;
+  p.cue_off = (const long long*)b2i_meta_put(&a, cue_off, tbl);
+  p.out_off = (const long long*)b2i_meta_put(&a, out_off, tbl);
+  p.video = (const int*)b2i_meta_put(&a, videos, (size_t)n_subs * 4);
+  B2_TRY(b2i_meta_commit(&a));
+  p.out = d_out;
+  p.sample_rate = sample_rate;
+  p.start_seconds = start_seconds;
+  raster_ref_kernel<<<n_subs, 256, 0, h->stream>>>(p);
+  B2_CHECK_LAUNCH(h, "raster_ref_kernel");
   return B2_OK;
 }
 

@@ -32,7 +32,8 @@ template <typename Out>
 struct TokParams {
   const float* flags;      // K1 output with label 0: non-zero = the block passed the energy test
   Out* out;                // may alias flags
-  const long long* off;    // [n_chunks + 1] windows
+  const long long* off;    // [n_chunks] first window of each chunk
+  const long long* end;    // [n_chunks] one past its last window (off + 1 for abutting chunks)
   int n_chunks;
   double min_length, max_sil, down;  // down = non_speech_label - 1.0
   long long max_length;
@@ -68,7 +69,7 @@ __global__ void __launch_bounds__(128) auditok_tokenize_kernel(TokParams<Out> p)
   const int lane = threadIdx.x & 31;
   if (chunk >= p.n_chunks) return;
   const long long base = p.off[chunk];
-  const int n = (int)(p.off[chunk + 1] - base);
+  const int n = (int)(p.end[chunk] - base);
   const float* f = p.flags + base;
   Out* out = p.out + base;
 
@@ -163,14 +164,15 @@ __global__ void __launch_bounds__(128) auditok_tokenize_kernel(TokParams<Out> p)
 
 template <typename Out>
 int tokenize_launch(b2_ctx* h, const float* d_flags, const int64_t* off_host, int n_chunks,
-                    const B2TokenizerParams& tp, Out* d_out) {
+                    const B2TokenizerParams& tp, Out* d_out, const int64_t* end_host = nullptr) {
   if (n_chunks <= 0) return B2_OK;
   B2Range range("b2:auditok_tokenize");
   MetaArena a;
   const size_t tbl = (size_t)(n_chunks + 1) * 8;
-  B2_TRY(b2i_meta_begin(h, &a, tbl + 256));
+  B2_TRY(b2i_meta_begin(h, &a, 2 * tbl + 256));
   TokParams<Out> p;
-  p.off = (const long long*)b2i_meta_put(&a, off_host, tbl);
+  p.off = (const long long*)b2i_meta_put(&a, off_host, end_host ? tbl - 8 : tbl);
+  p.end = end_host ? (const long long*)b2i_meta_put(&a, end_host, tbl - 8) : p.off + 1;
   B2_TRY(b2i_meta_commit(&a));
   p.flags = d_flags;
   p.out = d_out;
@@ -193,6 +195,6 @@ int b2i_tokenize_launch(b2_ctx* h, const float* d_flags, const int64_t* off_host
 }
 
 int b2i_tokenize_inplace_launch(b2_ctx* h, float* d_flags_sig, const int64_t* off_host, int n_chunks,
-                                const B2TokenizerParams& tp) {
-  return tokenize_launch(h, (const float*)d_flags_sig, off_host, n_chunks, tp, d_flags_sig);
+                                const B2TokenizerParams& tp, const int64_t* end_host) {
+  return tokenize_launch(h, (const float*)d_flags_sig, off_host, n_chunks, tp, d_flags_sig, end_host);
 }

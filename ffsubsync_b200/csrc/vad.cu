@@ -576,13 +576,14 @@ int b2i_synth_launch(b2_ctx* h, const uint8_t* d_cls, int64_t n_windows, int fpw
 }
 
 // Would b2i_vad_launch take the lane-per-window kernel for these signals?  (b2_sync_batch pipelines
-// sub-batches over an SM partition only then.)
+// sub-batches over an SM partition only then.)  An empty signal has no tiles, so where it starts does not
+// matter (b2_sync_tracks_subs: a video with a subtitle reference has an empty PCM range).
 bool b2i_vad_lane_eligible(const int64_t* pcm_off, int B, int fpw) {
   if (fpw != 80 && fpw != 160) return false;
   if (const char* e = getenv("B2_VAD_LAYOUT"))
     if (strcmp(e, "group") == 0) return false;
   for (int b = 0; b < B; ++b)
-    if (pcm_off[b] % 8 != 0) return false;
+    if (pcm_off[b + 1] > pcm_off[b] && pcm_off[b] % 8 != 0) return false;
   return true;
 }
 
@@ -644,7 +645,7 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
     long long n = pcm_off[b + 1] - pcm_off[b];
     long long nwin = (n + fpw - 1) / fpw;
     tile_off[b + 1] = tile_off[b] + (nwin + p.tw - 1) / p.tw;
-    if (pcm_off[b] % 8 != 0) aligned = false;
+    if (n > 0 && pcm_off[b] % 8 != 0) aligned = false;   // an empty signal has no tiles
   }
   if (!aligned) p.fast = 0;  // window starts are not 16-byte aligned in the staged span
   // lane-per-window kernel: 16-byte aligned signals and an instantiated chunk count (8 / 16 / 32 / 48 kHz

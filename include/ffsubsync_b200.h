@@ -267,6 +267,49 @@ int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_o
                            double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                            int memspace);
 
+/* ---- embedded subtitle streams as references (--vad subs_then_webrtc / subs_then_auditok) -----------------
+ * `ffs movie.mkv -i a.srt ...` with a subs_then_ detector for V videos and T tracks: a video with a text subtitle
+ * stream is synced against that stream rasterised (VideoSpeechTransformer.fit -> try_fit_using_embedded_subs,
+ * ffsubsync/speech_transformers.py:479-523,609-619), any other video against the detector's output.  Choosing the
+ * stream (the reference takes the one with the largest max_end - start_seconds, the first on a tie), parsing it
+ * and the metadata flags are the caller's; so is extracting streams from containers.
+ * Arguments as for b2_sync_tracks_auditok, plus:
+ *   detector             B2_DETECTOR_ENERGY_ZCR (energy_threshold, z_lo, z_hi as for b2_sync_tracks; the label is
+ *                        rounded to float) or B2_DETECTOR_AUDITOK (energy_threshold_db ... chunk_samples as for
+ *                        b2_sync_tracks_auditok); the other detector's arguments are not read.
+ *   ref_is_subs [V]      non-zero: video v has a subtitle reference.  NULL = none (every video is audio).
+ *   ref_cue_start_s, ref_cue_end_s, ref_cue_keep, ref_cue_off [V+1]
+ *                        host arrays: video v's reference cues are ref_cue_off[v] .. ref_cue_off[v+1] (seconds,
+ *                        unscaled, keep as for b2_rasterize; ref_cue_keep may be NULL = keep all).  A video without a
+ *                        subtitle reference has an empty list; a subtitle reference may be empty (a 2-frame signal).
+ * Track t gets exactly what this composition of public calls returns: the reference of video track_video[t] -
+ * b2_rasterize of its cue list at ratio 1.0 with level 1.0 (int(max_end * sample_rate) + 2 frames, max_end over
+ * all its cues, metadata ones included, 0 without cues) for a subtitle video, the detector's output as in
+ * b2_sync_tracks / b2_sync_tracks_auditok otherwise - then b2_align_batch and b2_reduce_ratios over the ratios,
+ * plus the golden-section search's candidate as in b2_sync_tracks_gss when gss_ratio is not NULL.
+ * A subtitle video's PCM range must be empty (B2_ERR_BAD_ARG otherwise): its audio is never read, and pcm may be
+ * NULL when no video has samples.  Reference cue times get the checks of b2_rasterize (B2_ERR_BAD_ARG, the message
+ * names the index); so does a non-monotone ref_cue_off, or cues given for a video without a subtitle reference.
+ * Levels: a subtitle reference holds 1.0 and 0.0, the detector's 1.0 and non_speech_label.  A call that mixes the
+ * two at a non-zero label, or runs auditok at a non-zero label on any video, aligns on the FFT paths; with
+ * gss_ratio it is B2_ERR_UNSUPPORTED (the search runs on the run path).  Without subtitle videos the call returns
+ * what b2_sync_tracks / b2_sync_tracks_gss / b2_sync_tracks_auditok return.  memspace: B2_HOST, B2_DEVICE or
+ * B2_DEVICE_RESIDENT; resident calls chain with the other sync calls in any order. */
+enum { B2_DETECTOR_ENERGY_ZCR = 0, B2_DETECTOR_AUDITOK = 1 };
+int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm /* or NULL without audio */, const int64_t* pcm_off /* [V+1] */,
+                        int V, const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                        int detector, double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                        double energy_threshold_db, double min_length, int64_t max_length,
+                        double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs /* [V] */,
+                        const double* ref_cue_start_s, const double* ref_cue_end_s, const uint8_t* ref_cue_keep,
+                        const int64_t* ref_cue_off /* [V+1] */, const double* cue_start_s, const double* cue_end_s,
+                        const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */, const double* ratios, int K,
+                        double start_seconds, int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                        int32_t* best_k /* [T] */,
+                        double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                        double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                        int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
