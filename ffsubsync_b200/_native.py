@@ -138,6 +138,14 @@ def _mask_width(max_offset_samples) -> int:
     return max(-lim, min(lim, int(max_offset_samples)))
 
 
+def _auditok_tokenizer(sample_rate: int, min_length=None, max_length=None, max_continuous_silence=None):
+    """(min_length, max_length, max_continuous_silence) of the auditok tokenizer in blocks, None taking the
+    reference's defaults (speech_transformers.py:126-131): 0.2 s, 5 s, 0.25 s."""
+    return (float(0.2 * sample_rate if min_length is None else min_length),
+            int(int(5 * sample_rate) if max_length is None else max_length),
+            float(0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence))
+
+
 def _i64a(x) -> np.ndarray:
     return np.ascontiguousarray(x, dtype=np.int64)
 
@@ -217,19 +225,9 @@ class Handle:
         (speech_transformers.py:126-131).  Returns (float64 per block, out_off[B+1])."""
         pcm_off = _i64a(pcm_off)
         B = len(pcm_off) - 1
-        fpw = int(self.lib.b2_auditok_block_size(frame_rate, sample_rate))
-        if fpw <= 0:
-            raise ValueError("auditok detector: unsupported frame_rate=%r / sample_rate=%r" % (frame_rate, sample_rate))
-        min_length = 0.2 * sample_rate if min_length is None else min_length
-        max_length = int(5 * sample_rate) if max_length is None else max_length
-        max_continuous_silence = 0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence
-        n = np.diff(pcm_off)
-        if chunk_samples > 0:
-            full, rem = n // chunk_samples, n % chunk_samples
-            nwin = full * ((chunk_samples + fpw - 1) // fpw) + (rem + fpw - 1) // fpw
-        else:
-            nwin = (n + fpw - 1) // fpw
-        out_off = np.concatenate([[0], np.cumsum(nwin)]).astype(np.int64)
+        min_length, max_length, max_continuous_silence = _auditok_tokenizer(sample_rate, min_length, max_length,
+                                                                            max_continuous_silence)
+        out_off = self.auditok_out_off(pcm_off, frame_rate, sample_rate, chunk_samples)
         if memspace == B2_HOST:
             pcm = np.ascontiguousarray(pcm, dtype=np.int16)
             out = np.empty(int(out_off[-1]), dtype=np.float64)
@@ -239,6 +237,19 @@ class Handle:
                                      _ptr(out), _ptr(out_off), memspace)
         self._check(st, "b2_vad_auditok")
         return out, out_off
+
+    def auditok_out_off(self, pcm_off, frame_rate: int, sample_rate: int, chunk_samples: int) -> np.ndarray:
+        """out_off [B+1] of the auditok detector over B signals cut into detector calls of chunk_samples samples
+        (0: one call each): a signal has the sum over its chunks of ceil(chunk / block) blocks."""
+        fpw = int(self.lib.b2_auditok_block_size(frame_rate, sample_rate))
+        if fpw <= 0:
+            raise ValueError("auditok detector: unsupported frame_rate=%r / sample_rate=%r" % (frame_rate, sample_rate))
+        n = np.diff(_i64a(pcm_off))
+        if chunk_samples > 0:
+            nwin = n // chunk_samples * ((chunk_samples + fpw - 1) // fpw) + (n % chunk_samples + fpw - 1) // fpw
+        else:
+            nwin = (n + fpw - 1) // fpw
+        return np.concatenate([[0], np.cumsum(nwin)]).astype(np.int64)
 
     # streaming detector (b2_vad_stream_*): push() returns before the chunk is processed
     def vad_stream_begin(self, frame_rate: int, sample_rate: int, non_speech_label: float,
@@ -367,35 +378,63 @@ class Handle:
         self._check(st, "b2_reduce_ratios")
         return best_score, best_offset, best_k
 
-    def sync_batch(self, pcm, pcm_off, frame_rate: int, sample_rate: int, non_speech_label: float,
-                   energy_threshold: int, z_lo: int, z_hi: int, cue_start_s, cue_end_s, cue_keep,
-                   cue_off, ratios, start_seconds: float, max_offset_samples: Optional[int],
-                   best_score=None, best_offset=None, best_k=None, all_score=None, all_offset=None,
-                   want_all: bool = False, memspace: int = B2_HOST):
+    def _sync(self, entry, pcm, pcm_off, track_video, detector_args, cue_start_s, cue_end_s, cue_keep, cue_off,
+              ratios, start_seconds, max_offset_samples, outs, want_all, memspace, gss=None, want_evals=False):
+        """The call of one b2_sync_* entry point: coerces the arrays, checks cue_off's length, allocates the host
+        outputs (all_* with K + 1 columns with the search) and passes the arguments in the ABI's order.
+        track_video None: b2_sync_batch (video b against track b).  detector_args: the entry point's arguments
+        between sample_rate and the track cues.  outs: (best_score, best_offset, best_k, all_score, all_offset,
+        gss_ratio, gss_evals).  gss: None for the entry points without the search's arguments, else whether it runs.
+        Returns (best_score, best_offset, best_k, all_score, all_offset), plus (gss_ratio, gss_evals) with gss."""
         pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
-        B = len(pcm_off) - 1
+        V = len(pcm_off) - 1
+        videos = [V]
+        if track_video is not None:
+            track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+            T = len(track_video)
+            if len(cue_off) != T + 1:
+                raise NativeError(-1, entry, "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+            videos += [_ptr(track_video), T]
+        else:
+            T = V
         ratios = np.ascontiguousarray(ratios, dtype=np.float64)
         K = len(ratios)
         cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
         cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
         cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
-        mos = _mask_width(max_offset_samples)
+        best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals = outs
         if memspace == B2_HOST:
-            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
-            best_score = np.empty(B, dtype=np.float64)
-            best_offset = np.empty(B, dtype=np.int32)
-            best_k = np.empty(B, dtype=np.int32)
+            pcm = None if pcm is None else np.ascontiguousarray(pcm, dtype=np.int16)
+            best_score = np.empty(T, dtype=np.float64)
+            best_offset = np.empty(T, dtype=np.int32)
+            best_k = np.empty(T, dtype=np.int32)
+            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
             if want_all:
-                all_score = np.empty(B * K, dtype=np.float64)
-                all_offset = np.empty(B * K, dtype=np.int32)
-        st = self.lib.b2_sync_batch(self.h, _ptr(pcm), _ptr(pcm_off), B, frame_rate, sample_rate,
-                                    float(non_speech_label), int(energy_threshold), int(z_lo), int(z_hi),
-                                    _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off),
-                                    _ptr(ratios), K, float(start_seconds), mos, _ptr(best_score),
-                                    _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset),
-                                    memspace)
-        self._check(st, "b2_sync_batch")
-        return best_score, best_offset, best_k, all_score, all_offset
+                cols = K + 1 if gss else K
+                all_score = np.empty(T * cols, dtype=np.float64)
+                all_offset = np.empty(T * cols, dtype=np.int32)
+            gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64) if gss and want_evals else None
+        elif gss and gss_ratio is None:
+            raise ValueError("%s with the search on device memory needs gss_ratio" % entry)
+        search = [] if gss is None else [_ptr(gss_ratio) if gss else None, _ptr(gss_evals) if gss else None]
+        st = getattr(self.lib, entry)(
+            self.h, _ptr(pcm), _ptr(pcm_off), *videos, *detector_args, _ptr(cue_start_s), _ptr(cue_end_s),
+            _ptr(cue_keep), _ptr(cue_off), _ptr(ratios), K, float(start_seconds), _mask_width(max_offset_samples),
+            _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset), *search, memspace)
+        self._check(st, entry)
+        res = (best_score, best_offset, best_k, all_score, all_offset)
+        return res + (gss_ratio, gss_evals) if gss else res
+
+    def sync_batch(self, pcm, pcm_off, frame_rate: int, sample_rate: int, non_speech_label: float,
+                   energy_threshold: int, z_lo: int, z_hi: int, cue_start_s, cue_end_s, cue_keep,
+                   cue_off, ratios, start_seconds: float, max_offset_samples: Optional[int],
+                   best_score=None, best_offset=None, best_k=None, all_score=None, all_offset=None,
+                   want_all: bool = False, memspace: int = B2_HOST):
+        return self._sync("b2_sync_batch", pcm, pcm_off, None,
+                          (frame_rate, sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
+                           int(z_hi)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds,
+                          max_offset_samples, (best_score, best_offset, best_k, all_score, all_offset, None, None),
+                          want_all, memspace)
 
     def sync_tracks(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
                     energy_threshold: int, z_lo: int, z_hi: int, cue_start_s, cue_end_s, cue_keep,
@@ -405,32 +444,11 @@ class Handle:
         """sync_batch for T subtitle tracks over V videos (b2_sync_tracks): pcm_off [V+1] sample offsets,
         track_video [T] (non-decreasing video index of each track), cue_off [T+1].  Outputs per track:
         best_* [T], all_* [T*K]."""
-        pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
-        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
-        V, T = len(pcm_off) - 1, len(track_video)
-        if len(cue_off) != T + 1:
-            raise NativeError(-1, "b2_sync_tracks", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
-        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
-        K = len(ratios)
-        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
-        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
-        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
-        mos = _mask_width(max_offset_samples)
-        if memspace == B2_HOST:
-            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
-            best_score = np.empty(T, dtype=np.float64)
-            best_offset = np.empty(T, dtype=np.int32)
-            best_k = np.empty(T, dtype=np.int32)
-            if want_all:
-                all_score = np.empty(T * K, dtype=np.float64)
-                all_offset = np.empty(T * K, dtype=np.int32)
-        st = self.lib.b2_sync_tracks(self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate,
-                                     sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
-                                     int(z_hi), _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off),
-                                     _ptr(ratios), K, float(start_seconds), mos, _ptr(best_score),
-                                     _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset), memspace)
-        self._check(st, "b2_sync_tracks")
-        return best_score, best_offset, best_k, all_score, all_offset
+        return self._sync("b2_sync_tracks", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
+                           int(z_hi)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds,
+                          max_offset_samples, (best_score, best_offset, best_k, all_score, all_offset, None, None),
+                          want_all, memspace)
 
     def sync_tracks_gss(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
                         energy_threshold: int, z_lo: int, z_hi: int, cue_start_s, cue_end_s, cue_keep,
@@ -442,36 +460,11 @@ class Handle:
         best_* [T] (best_k == K: the search won), all_* [T*(K+1)] (column K: the search's candidate),
         gss_ratio [T] (NaN for an empty reference), gss_evals [T*17].  Raises NativeError with status
         B2_ERR_UNSUPPORTED (-6) outside the envelope of the device-driven rounds."""
-        pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
-        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
-        V, T = len(pcm_off) - 1, len(track_video)
-        if len(cue_off) != T + 1:
-            raise NativeError(-1, "b2_sync_tracks_gss", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
-        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
-        K = len(ratios)
-        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
-        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
-        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
-        mos = _mask_width(max_offset_samples)
-        if memspace == B2_HOST:
-            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
-            best_score = np.empty(T, dtype=np.float64)
-            best_offset = np.empty(T, dtype=np.int32)
-            best_k = np.empty(T, dtype=np.int32)
-            gss_ratio = np.empty(T, dtype=np.float64)
-            if want_all:
-                all_score = np.empty(T * (K + 1), dtype=np.float64)
-                all_offset = np.empty(T * (K + 1), dtype=np.int32)
-            if want_evals:
-                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
-        st = self.lib.b2_sync_tracks_gss(self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate,
-                                         sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
-                                         int(z_hi), _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep),
-                                         _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos,
-                                         _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(all_score),
-                                         _ptr(all_offset), _ptr(gss_ratio), _ptr(gss_evals), memspace)
-        self._check(st, "b2_sync_tracks_gss")
-        return best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals
+        return self._sync("b2_sync_tracks_gss", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, float(non_speech_label), int(energy_threshold), int(z_lo),
+                           int(z_hi)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds,
+                          max_offset_samples, (best_score, best_offset, best_k, all_score, all_offset, gss_ratio,
+                                               gss_evals), want_all, memspace, gss=True, want_evals=want_evals)
 
     def sync_tracks_auditok(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int,
                             non_speech_label: float, cue_start_s, cue_end_s, cue_keep, cue_off, ratios,
@@ -485,44 +478,13 @@ class Handle:
         is cut into detector calls of chunk_samples samples (0: one call).  Detector defaults as for vad_auditok.
         Returns (best_score, best_offset, best_k, all_score, all_offset), plus (gss_ratio, gss_evals) with
         gss=True (all_* then [T*(K+1)])."""
-        pcm_off, cue_off = _i64a(pcm_off), _i64a(cue_off)
-        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
-        V, T = len(pcm_off) - 1, len(track_video)
-        if len(cue_off) != T + 1:
-            raise NativeError(-1, "b2_sync_tracks_auditok", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
-        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
-        K = len(ratios)
-        min_length = 0.2 * sample_rate if min_length is None else min_length
-        max_length = int(5 * sample_rate) if max_length is None else max_length
-        max_continuous_silence = 0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence
-        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
-        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
-        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
-        mos = _mask_width(max_offset_samples)
-        cols = K + 1 if gss else K
-        if memspace == B2_HOST:
-            pcm = np.ascontiguousarray(pcm, dtype=np.int16)
-            best_score = np.empty(T, dtype=np.float64)
-            best_offset = np.empty(T, dtype=np.int32)
-            best_k = np.empty(T, dtype=np.int32)
-            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
-            if want_all:
-                all_score = np.empty(T * cols, dtype=np.float64)
-                all_offset = np.empty(T * cols, dtype=np.int32)
-            if gss and want_evals:
-                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
-        elif gss and gss_ratio is None:
-            raise ValueError("sync_tracks_auditok(gss=True) on device memory needs gss_ratio")
-        st = self.lib.b2_sync_tracks_auditok(
-            self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate, sample_rate,
-            float(non_speech_label), float(energy_threshold_db), float(min_length), int(max_length),
-            float(max_continuous_silence), int(chunk_samples), _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep),
-            _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos, _ptr(best_score), _ptr(best_offset),
-            _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
-            _ptr(gss_evals) if gss else None, memspace)
-        self._check(st, "b2_sync_tracks_auditok")
-        res = (best_score, best_offset, best_k, all_score, all_offset)
-        return res + (gss_ratio, gss_evals) if gss else res
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        return self._sync("b2_sync_tracks_auditok", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, float(non_speech_label), float(energy_threshold_db), tok[0],
+                           tok[1], tok[2], int(chunk_samples)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios,
+                          start_seconds, max_offset_samples,
+                          (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
+                          memspace, gss=bool(gss), want_evals=want_evals)
 
     def sync_tracks_subs(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
                          ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, ref_cue_off, cue_start_s,
@@ -540,9 +502,8 @@ class Handle:
         B2_DETECTOR_ENERGY_ZCR (energy_threshold, z_lo, z_hi) or B2_DETECTOR_AUDITOK (chunk_samples and the
         tokenizer arguments, defaults as for vad_auditok).  Returns (best_score, best_offset, best_k, all_score,
         all_offset), plus (gss_ratio, gss_evals) with gss=True (all_* then [T*(K+1)])."""
-        pcm_off, cue_off, ref_cue_off = _i64a(pcm_off), _i64a(cue_off), _i64a(ref_cue_off)
-        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
         V, T = len(pcm_off) - 1, len(track_video)
+        ref_cue_off = _i64a(ref_cue_off)
         if len(cue_off) != T + 1 or len(ref_cue_off) != V + 1:
             raise NativeError(-1, "b2_sync_tracks_subs", "cue_off / ref_cue_off have %d / %d entries for %d tracks / "
                               "%d videos" % (len(cue_off), len(ref_cue_off), T, V))
@@ -553,40 +514,15 @@ class Handle:
         ref_cue_start_s = np.ascontiguousarray(ref_cue_start_s, dtype=np.float64)
         ref_cue_end_s = np.ascontiguousarray(ref_cue_end_s, dtype=np.float64)
         ref_cue_keep = None if ref_cue_keep is None else np.ascontiguousarray(ref_cue_keep, dtype=np.uint8)
-        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
-        K = len(ratios)
-        min_length = 0.2 * sample_rate if min_length is None else min_length
-        max_length = int(5 * sample_rate) if max_length is None else max_length
-        max_continuous_silence = 0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence
-        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
-        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
-        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
-        mos = _mask_width(max_offset_samples)
-        cols = K + 1 if gss else K
-        if memspace == B2_HOST:
-            pcm = None if pcm is None else np.ascontiguousarray(pcm, dtype=np.int16)
-            best_score = np.empty(T, dtype=np.float64)
-            best_offset = np.empty(T, dtype=np.int32)
-            best_k = np.empty(T, dtype=np.int32)
-            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
-            if want_all:
-                all_score = np.empty(T * cols, dtype=np.float64)
-                all_offset = np.empty(T * cols, dtype=np.int32)
-            if gss and want_evals:
-                gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64)
-        elif gss and gss_ratio is None:
-            raise ValueError("sync_tracks_subs(gss=True) on device memory needs gss_ratio")
-        st = self.lib.b2_sync_tracks_subs(
-            self.h, _ptr(pcm), _ptr(pcm_off), V, _ptr(track_video), T, frame_rate, sample_rate, int(detector),
-            float(non_speech_label), int(energy_threshold), int(z_lo), int(z_hi), float(energy_threshold_db),
-            float(min_length), int(max_length), float(max_continuous_silence), int(chunk_samples), _ptr(ref_is_subs),
-            _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep), _ptr(ref_cue_off), _ptr(cue_start_s),
-            _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off), _ptr(ratios), K, float(start_seconds), mos,
-            _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset),
-            _ptr(gss_ratio) if gss else None, _ptr(gss_evals) if gss else None, memspace)
-        self._check(st, "b2_sync_tracks_subs")
-        res = (best_score, best_offset, best_k, all_score, all_offset)
-        return res + (gss_ratio, gss_evals) if gss else res
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        return self._sync("b2_sync_tracks_subs", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, int(detector), float(non_speech_label), int(energy_threshold),
+                           int(z_lo), int(z_hi), float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
+                           _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
+                           _ptr(ref_cue_off)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds,
+                          max_offset_samples,
+                          (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
+                          memspace, gss=bool(gss), want_evals=want_evals)
 
     # -- diagnostics (tests) --------------------------------------------------------------------
     @contextlib.contextmanager

@@ -119,22 +119,42 @@ class BatchSynchronizer:
                                         streams["ref_stream_video"], self.start_seconds,
                                         content=streams.get("ref_cue_content"), keep=streams.get("ref_cue_keep"))
 
-    def _subs_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, **kw):
-        """b2_sync_tracks_subs with this synchroniser's settings (grid, or grid + search with gss)."""
-        det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
-        is_subs, rs, re_, rk, roff = refs
-        return self.handle.sync_tracks_subs(
-            pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label, is_subs, rs, re_,
-            rk, roff, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples,
-            detector=det, energy_threshold=self.energy_threshold, z_lo=self.z_lo, z_hi=self.z_hi,
-            chunk_samples=self.chunk_samples, gss=gss, **kw)
+    def _dispatch(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, **kw):
+        """The batched call of this synchroniser's detector with the search on or off: b2_sync_tracks_subs with
+        subtitle references (refs, from _subs_refs), else b2_sync_tracks_auditok for auditok, else
+        b2_sync_tracks_gss / b2_sync_tracks.  pcm: int16 numpy array, CUDA tensor or None; kw: the outputs (device
+        pointers) or want_all, and memspace.  Returns (best_score, best_offset, best_k, all_score, all_offset), plus
+        (gss_ratio, gss_evals) with gss."""
+        h = self.handle
+        p = pcm if pcm is None or isinstance(pcm, np.ndarray) else pcm.data_ptr()
+        cues = (cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples)
+        if refs is not None:
+            det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
+            return h.sync_tracks_subs(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                      self.non_speech_label, *refs, *cues, detector=det,
+                                      energy_threshold=self.energy_threshold, z_lo=self.z_lo, z_hi=self.z_hi,
+                                      chunk_samples=self.chunk_samples, gss=gss, **kw)
+        if self.auditok:
+            return h.sync_tracks_auditok(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                         self.non_speech_label, *cues, self.chunk_samples, gss=gss, **kw)
+        energy = (self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+        return (h.sync_tracks_gss if gss else h.sync_tracks)(p, pcm_off, track_video, *energy, *cues, **kw)
 
-    def _auditok_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, gss: bool, **kw):
-        """b2_sync_tracks_auditok with this synchroniser's settings (grid, or grid + search with gss)."""
-        return self.handle.sync_tracks_auditok(
-            pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label, cue_start, cue_end,
-            cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples, self.chunk_samples, gss=gss,
-            **kw)
+    def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, **kw):
+        """_dispatch with this synchroniser's search.  Outside the envelope of the device-driven search
+        (B2_ERR_UNSUPPORTED) the search is composed of public steps instead (_gss_compose).  Returns
+        (best_score, best_offset, best_k, all_score, all_offset), plus gss_ratio with the search; composed results
+        are numpy arrays (all_* None unless want_all or device outputs were given)."""
+        try:
+            return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
+                                  **kw)[:6]
+        except _native.NativeError as e:
+            if not (self.gss and _is_unsupported(e)):
+                raise
+        want_all = kw.get("want_all", False) or kw.get("all_score") is not None
+        bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off,
+                                                        cue_keep, want_all=want_all, refs=refs)
+        return bs, bo, bk, a_s, a_o, ratio
 
     def use_torch_stream(self) -> None:
         """Launch on torch's current stream (so torch events / NCCL ops order against our kernels)."""
@@ -197,63 +217,19 @@ class BatchSynchronizer:
                    "best_k": torch.empty(T, dtype=torch.int32, device=dev)}
         if self.gss and "gss_ratio" not in out:
             out["gss_ratio"] = torch.empty(T, dtype=torch.float64, device=dev)
-        a_s = all_out["score"].data_ptr() if all_out else None
-        a_o = all_out["offset"].data_ptr() if all_out else None
         memspace = _native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE
-        if refs is not None:
-            try:
-                self._subs_tracks(pcm.data_ptr() if pcm is not None else None, pcm_off, track_video, cue_start,
-                                  cue_end, cue_off, cue_keep, refs, self.gss, best_score=out["best_score"].data_ptr(),
-                                  best_offset=out["best_offset"].data_ptr(), best_k=out["best_k"].data_ptr(),
-                                  all_score=a_s, all_offset=a_o,
-                                  gss_ratio=out["gss_ratio"].data_ptr() if self.gss else None, memspace=memspace)
-            except _native.NativeError as e:
-                if not (self.gss and _is_unsupported(e)):
-                    raise
-                res = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep,
-                                        want_all=all_out is not None, refs=refs)
-                for key, v in zip(("best_score", "best_offset", "best_k", "gss_ratio"), res[:4]):
-                    out[key].copy_(torch.from_numpy(v))
-                if all_out:
-                    all_out["score"].copy_(torch.from_numpy(res[4]))
-                    all_out["offset"].copy_(torch.from_numpy(res[5]))
-            return out
-        if self.auditok and not self.gss:
-            self._auditok_tracks(pcm.data_ptr(), pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
-                                 best_score=out["best_score"].data_ptr(), best_offset=out["best_offset"].data_ptr(),
-                                 best_k=out["best_k"].data_ptr(), all_score=a_s, all_offset=a_o, memspace=memspace)
-            return out
-        if self.gss:
-            try:
-                if self.auditok:
-                    self._auditok_tracks(pcm.data_ptr(), pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep,
-                                         True, best_score=out["best_score"].data_ptr(),
-                                         best_offset=out["best_offset"].data_ptr(), best_k=out["best_k"].data_ptr(),
-                                         all_score=a_s, all_offset=a_o, gss_ratio=out["gss_ratio"].data_ptr(),
-                                         memspace=memspace)
-                    return out
-                self.handle.sync_tracks_gss(
-                    pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
-                    self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
-                    self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
-                    out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o, out["gss_ratio"].data_ptr(),
-                    memspace=memspace)
-            except _native.NativeError as e:
-                if not _is_unsupported(e):
-                    raise
-                res = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep,
-                                        want_all=all_out is not None)
-                for key, v in zip(("best_score", "best_offset", "best_k", "gss_ratio"), res[:4]):
-                    out[key].copy_(torch.from_numpy(v))
-                if all_out:
-                    all_out["score"].copy_(torch.from_numpy(res[4]))
-                    all_out["offset"].copy_(torch.from_numpy(res[5]))
-            return out
-        self.handle.sync_tracks(
-            pcm.data_ptr(), pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
-            self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
-            self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
-            out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o, memspace=memspace)
+        keys = ("best_score", "best_offset", "best_k") + (("gss_ratio",) if self.gss else ())
+        ptrs = {k: out[k].data_ptr() for k in keys}
+        if all_out:
+            ptrs.update(all_score=all_out["score"].data_ptr(), all_offset=all_out["offset"].data_ptr())
+        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs,
+                                    memspace=memspace, **ptrs)
+        if isinstance(res[0], np.ndarray):   # composed on the host
+            for k, v in zip(keys, res[:3] + res[5:]):
+                out[k].copy_(torch.from_numpy(v))
+            if all_out:
+                all_out["score"].copy_(torch.from_numpy(res[3]))
+                all_out["offset"].copy_(torch.from_numpy(res[4]))
         return out
 
     def sync_host_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None,
@@ -262,46 +238,9 @@ class BatchSynchronizer:
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
         track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks."""
         refs = self._subs_refs(len(pcm_off) - 1, streams)
-        if refs is not None:
-            try:
-                r = self._subs_tracks(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
-                                      want_all=want_all, memspace=_native.B2_HOST)
-                res = r[:5] + ((r[5],) if self.gss else ())
-            except _native.NativeError as e:
-                if not (self.gss and _is_unsupported(e)):
-                    raise
-                bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end,
-                                                                cue_off, cue_keep, want_all=want_all, refs=refs)
-                res = (bs, bo, bk, a_s, a_o, ratio)
-            return res if want_all else res[:3] + res[5:]
-        if self.auditok and not self.gss:
-            res = self._auditok_tracks(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
-                                       want_all=want_all, memspace=_native.B2_HOST)
-            return res if want_all else res[:3]
-        if self.gss:
-            try:
-                if self.auditok:
-                    r = self._auditok_tracks(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, True,
-                                             want_all=want_all, memspace=_native.B2_HOST)
-                else:
-                    r = self.handle.sync_tracks_gss(
-                        pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
-                        self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off,
-                        self.ratios, self.start_seconds, self.max_offset_samples, want_all=want_all,
-                        memspace=_native.B2_HOST)
-                res = r[:5] + (r[5],)
-            except _native.NativeError as e:
-                if not _is_unsupported(e):
-                    raise
-                bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end,
-                                                                cue_off, cue_keep, want_all=want_all)
-                res = (bs, bo, bk, a_s, a_o, ratio)
-            return res if want_all else res[:3] + res[5:]
-        res = self.handle.sync_tracks(
-            pcm, pcm_off, track_video, self.frame_rate, self.sample_rate, self.non_speech_label,
-            self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
-            self.start_seconds, self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
-        return res if want_all else res[:3]
+        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs,
+                                    want_all=want_all, memspace=_native.B2_HOST)
+        return res if want_all else res[:3] + res[5:]
 
     def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None):
         """Same as sync_device but starting from reference speech SIGNALS (100 Hz float32, all pairs
@@ -427,11 +366,9 @@ class BatchSynchronizer:
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
                      refs=None):
-        """The golden-section search outside the envelope of b2_sync_tracks_gss, composed of the public steps:
-        the VAD (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32), the grid (b2_sync_tracks or
-        b2_sync_tracks_auditok), gss_align_batch on each track's reference signal and the reference's combine.
-        With subtitle references (refs, from _subs_refs) the grid is b2_sync_tracks_subs and a subtitle video's
-        signal is b2_rasterize of its stream at ratio 1.0 and level 1.0.
+        """The golden-section search outside the envelope of the device-driven search, composed of public steps:
+        the grid (this synchroniser's batched call with the search off), gss_align_batch on each track's reference
+        signal (_reference_signals, with subtitle references refs from _subs_refs) and the reference's combine.
         pcm: int16 numpy array or CUDA tensor (or None without audio).  Returns numpy arrays (best_score,
         best_offset, best_k, gss_ratio, all_score, all_offset) (all_* None unless want_all)."""
         import torch
@@ -447,22 +384,9 @@ class BatchSynchronizer:
             pcm_host = pcm.cpu().numpy()
         else:
             pcm_host = pcm
-        if refs is not None:
-            grid = self._subs_tracks(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs,
-                                     False, want_all=True, memspace=_native.B2_HOST)
-            ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs)
-        elif self.auditok:
-            grid = self._auditok_tracks(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, False,
-                                        want_all=True, memspace=_native.B2_HOST)
-            ref, ref_off = h.vad_auditok(pcm_host, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
-                                         chunk_samples=self.chunk_samples)
-        else:
-            grid = h.sync_tracks(pcm_host, pcm_off, track_video, self.frame_rate, self.sample_rate,
-                                 self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi, cue_start,
-                                 cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples,
-                                 want_all=True, memspace=_native.B2_HOST)
-            ref, ref_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
-                                            self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+        grid = self._dispatch(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, False,
+                              want_all=True, memspace=_native.B2_HOST)
+        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs)
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
@@ -473,13 +397,12 @@ class BatchSynchronizer:
                                                   grid[3], grid[4])
         return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))
 
-    def _reference_signals(self, pcm_host, pcm_off, refs):
-        """The per-video reference signals b2_sync_tracks_subs syncs against, composed of public calls: the detector
-        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, and for a video with a
-        subtitle reference b2_rasterize of its stream at ratio 1.0 and level 1.0.  Returns (float32 signals back
-        to back, ref_off int64[V+1])."""
+    def _reference_signals(self, pcm_host, pcm_off, refs=None):
+        """The per-video reference signals the batched calls sync against, composed of public calls: the detector
+        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, and with subtitle references
+        (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0.
+        Returns (float32 signals back to back, ref_off int64[V+1])."""
         h = self.handle
-        is_subs, rs, re_, rk, roff = refs
         V = len(pcm_off) - 1
         if pcm_host is None:   # no video has samples: every detector signal is empty
             det, det_off = np.zeros(0, np.float32), np.zeros(V + 1, np.int64)
@@ -489,6 +412,9 @@ class BatchSynchronizer:
         else:
             det, det_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
                                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+        if refs is None:
+            return det.astype(np.float32), det_off
+        is_subs, rs, re_, rk, roff = refs
         sub, sub_off = h.rasterize(rs, re_, rk, roff, [1.0], 1, False, self.sample_rate, self.start_seconds,
                                    levels=[1.0])
         parts = [sub[sub_off[v]: sub_off[v + 1]] if is_subs[v] else det[det_off[v]: det_off[v + 1]].astype(np.float32)
@@ -502,17 +428,10 @@ class BatchSynchronizer:
         import torch
         h = self.handle
         pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
-        fpw = int(h.lib.b2_auditok_block_size(self.frame_rate, self.sample_rate))
-        if fpw <= 0:
-            raise ValueError("auditok detector: unsupported frame_rate=%r / sample_rate=%r"
-                             % (self.frame_rate, self.sample_rate))
-        n = np.diff(pcm_off)
-        c = self.chunk_samples
-        nwin = n // c * ((c + fpw - 1) // fpw) + (n % c + fpw - 1) // fpw
-        ref_off = np.concatenate([[0], np.cumsum(nwin)]).astype(np.int64)
+        ref_off = h.auditok_out_off(pcm_off, self.frame_rate, self.sample_rate, self.chunk_samples)
         ref64 = torch.empty(int(ref_off[-1]), dtype=torch.float64, device=pcm.device)
         h.vad_auditok(pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
-                      chunk_samples=c, out=ref64.data_ptr(), memspace=_native.B2_DEVICE)
+                      chunk_samples=self.chunk_samples, out=ref64.data_ptr(), memspace=_native.B2_DEVICE)
         return ref64.to(torch.float32), ref_off
 
 

@@ -1,7 +1,8 @@
 // C-ABI entry points (include/ffsubsync_b200.h): handle lifecycle, workspace management and
 // the host<->device staging that turns B2_HOST calls into the device path.  All arithmetic
 // lives in the kernels (vad.cu, tokenizer.cu, raster.cu, corr.cu, bigfft.cu); nothing here computes
-// results on the CPU.
+// results on the CPU.  The batched sync calls are planned on the host by sync_plan.h (argument checks,
+// tables, sub-batch cuts) and run by the pipeline at the end of this file.
 #include <math.h>
 
 #include <chrono>
@@ -11,9 +12,7 @@
 #include <thread>
 
 #include "common.cuh"
-#include "corr_jobs.cuh"
-#include "job_plan.cuh"
-#include "raster_math.cuh"
+#include "sync_plan.h"
 
 // Entry guard: the handle's device is current for the duration of the call and the caller
 // thread's previous device is restored on every return path.
@@ -411,9 +410,7 @@ static int check_device_ptr(b2_ctx* h, const void* p, const char* what) {
 
 // ---- VAD -----------------------------------------------------------------------------------
 extern "C" int b2_vad_frames_per_window(int frame_rate, int sample_rate) {
-  if (frame_rate <= 0 || sample_rate <= 0) return 0;
-  // speech_transformers.py:163-164: int(window_duration * frame_rate + 0.5)
-  return (int)((1.0 / (double)sample_rate) * (double)frame_rate + 0.5);
+  return vad_frames_per_window(frame_rate, sample_rate);
 }
 
 extern "C" int64_t b2_vad_num_windows(int64_t n_samples, int frame_rate, int sample_rate) {
@@ -464,39 +461,11 @@ extern "C" int b2_vad_energy_zcr(b2_handle h, const int16_t* pcm, const int64_t*
 
 // ---- auditok detector (speech_transformers.py:101-152) ---------------------------------------
 extern "C" int b2_auditok_block_size(int frame_rate, int sample_rate) {
-  if (frame_rate <= 0 || sample_rate <= 0) return 0;
-  // ADSFactory.ads(block_dur=1.0/sample_rate): int(sampling_rate * block_dur), speech_transformers.py:140;
-  // the output length formula uses frame_rate // sample_rate (:122,143-145): the two must agree
-  volatile double dur = 1.0 / (double)sample_rate;
-  volatile double prod = (double)frame_rate * dur;
-  const int block = (int)prod;
-  return block == frame_rate / sample_rate ? block : 0;
+  return auditok_block_size(frame_rate, sample_rate);
 }
 
 extern "C" int64_t b2_auditok_energy_floor(int n_samples, double energy_threshold_db) {
-  // smallest integer sum of squares E with 10*log10(E/n) >= threshold, evaluated with the same
-  // float64 expression auditok's AudioEnergyValidator uses (log energy -200 for E = 0)
-  if (n_samples <= 0) return INT64_MAX;
-  if (-200.0 >= energy_threshold_db) return 0;
-  auto valid = [&](int64_t e) {
-    volatile double energy = (double)e / (double)n_samples;
-    volatile double le = 10.0 * log10(energy);
-    return le >= energy_threshold_db;
-  };
-  const double guess = (double)n_samples * pow(10.0, energy_threshold_db / 10.0);
-  const double e_max = (double)n_samples * 32768.0 * 32768.0;   // int16 blocks cannot exceed this
-  if (!(guess <= 2.0 * e_max)) return INT64_MAX;
-  int64_t lo = 0, hi = (int64_t)guess + 1;                       // !valid(0) holds: log energy -200
-  while (!valid(hi)) {
-    if ((double)hi > 4.0 * e_max) return INT64_MAX;
-    hi *= 2;
-  }
-  while (hi - lo > 1) {
-    const int64_t mid = lo + (hi - lo) / 2;
-    if (valid(mid)) hi = mid;
-    else lo = mid;
-  }
-  return hi;
+  return auditok_energy_floor(n_samples, energy_threshold_db);
 }
 
 extern "C" int b2_vad_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
@@ -506,38 +475,23 @@ extern "C" int b2_vad_auditok(b2_handle h, const int16_t* pcm, const int64_t* pc
                               const int64_t* out_off, int memspace) {
   B2_ENTER(h);
   if (B < 0 || !pcm_off || !out_off) B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: null offset table / B<0");
-  const int fpw = b2_auditok_block_size(frame_rate, sample_rate);
+  const int fpw = auditok_block_size(frame_rate, sample_rate);
   if (fpw <= 0)
     B2_FAIL(h, B2_ERR_UNSUPPORTED, "auditok: int(frame_rate/sample_rate) block size and frame_rate//sample_rate "
                                    "window size differ (or are 0) for %d / %d", frame_rate, sample_rate);
-  // StreamTokenizer.__init__ argument checks
-  if (max_length <= 0 || !(min_length > 0) || min_length > (double)max_length ||
-      !(max_continuous_silence < (double)max_length) || chunk_samples < 0)
+  if (!tokenizer_params_ok(min_length, max_length, max_continuous_silence, chunk_samples))
     B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: bad tokenizer parameters");
   // one detector call per chunk: chunk c of signal b becomes "signal" n of the batched energy kernel
-  std::vector<int64_t> c_pcm(1, 0), c_out(1, 0), tail;
+  ChunkTable ct;
+  build_chunk_table(pcm_off, B, B ? pcm_off[0] : 0, fpw, chunk_samples, energy_threshold_db, nullptr, &ct);
   for (int b = 0; b < B; ++b) {
-    const int64_t n = pcm_off[b + 1] - pcm_off[b];
-    if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: pcm_off not monotone at %d", b);
-    if (c_pcm.back() != pcm_off[b] - pcm_off[0])
-      B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: internal chunk table mismatch");
-    int64_t nwin = 0;
-    const int64_t step = chunk_samples > 0 ? chunk_samples : (n > 0 ? n : 1);
-    for (int64_t s = 0; s < n; s += step) {
-      const int64_t len = std::min(step, n - s);
-      const int64_t w = (len + fpw - 1) / fpw;
-      c_pcm.push_back(c_pcm.back() + len);
-      c_out.push_back(c_out.back() + w);
-      const int rem = (int)(len % fpw);
-      tail.push_back(rem ? b2_auditok_energy_floor(rem, energy_threshold_db) : 0);
-      nwin += w;
-    }
-    if (out_off[b + 1] - out_off[b] != nwin)
+    if (pcm_off[b + 1] < pcm_off[b]) B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: pcm_off not monotone at %d", b);
+    if (out_off[b + 1] - out_off[b] != ct.out[ct.first[b + 1]] - ct.out[ct.first[b]])
       B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: out_off[%d] span must be the sum of ceil(chunk/fpw)", b);
   }
-  const int n_chunks = (int)tail.size();
+  const int n_chunks = (int)ct.tail.size();
   if (n_chunks == 0) return B2_OK;
-  const int64_t n_total = pcm_off[B] - pcm_off[0], w_total = c_out.back();
+  const int64_t n_total = pcm_off[B] - pcm_off[0], w_total = ct.out.back();
   if ((n_total && !pcm) || (w_total && !out)) B2_FAIL(h, B2_ERR_BAD_ARG, "auditok: null data pointer");
   B2_CHECK_DEV(h, memspace, pcm, "auditok: pcm");
   B2_CHECK_DEV(h, memspace, out, "auditok: out");
@@ -551,11 +505,10 @@ extern "C" int b2_vad_auditok(b2_handle h, const int16_t* pcm, const int64_t* pc
     d_out = (double*)dq;
   }
   B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_REF, (size_t)w_total * 4 + 64, &d_flags));
-  B2_TRY(b2i_vad_launch(h, d_pcm, c_pcm.data(), n_chunks, fpw, 0.0f,
-                        b2_auditok_energy_floor(fpw, energy_threshold_db), 0, fpw, (float*)d_flags,
-                        c_out.data(), tail.data()));
+  B2_TRY(b2i_vad_launch(h, d_pcm, ct.pcm.data(), n_chunks, fpw, 0.0f, auditok_energy_floor(fpw, energy_threshold_db),
+                        0, fpw, (float*)d_flags, ct.out.data(), ct.tail.data()));
   B2TokenizerParams tp{min_length, max_continuous_silence, non_speech_label, (long long)max_length};
-  B2_TRY(b2i_tokenize_launch(h, (const float*)d_flags, c_out.data(), n_chunks, tp, d_out));
+  B2_TRY(b2i_tokenize_launch(h, (const float*)d_flags, ct.out.data(), n_chunks, tp, d_out));
   if (memspace == B2_HOST) {
     B2_TRY(copy_out(h, out + out_off[0], d_out, (size_t)w_total * 8));
     B2_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -686,110 +639,6 @@ extern "C" int b2_synth_pcm(b2_handle h, const uint8_t* window_class, int64_t n_
 }
 
 // ---- rasteriser ----------------------------------------------------------------------------
-// Bits of |x| as an integer: ordered like |x| for every double, with inf above every finite value and
-// NaN above inf, so one integer maximum over a cue array finds its largest or non-finite time.
-static inline uint64_t magnitude_bits(double x) {
-  uint64_t u;
-  memcpy(&u, &x, 8);
-  return u & 0x7fffffffffffffffull;
-}
-
-static inline double from_bits(uint64_t u) {
-  double x;
-  memcpy(&x, &u, 8);
-  return x;
-}
-
-// The cue arithmetic (raster_math.cuh) reproduces the reference for finite times with
-// |t| * ratio < B2_MAX_CUE_SECONDS; fl(|t| * r) is monotone in |t| and r, so the largest magnitude and
-// the largest ratio of a pair decide.  NaN and inf fail the comparison.
-static inline bool cue_magnitude_ok(uint64_t max_bits, double r_max) {
-  return from_bits(max_bits) * r_max < B2_MAX_CUE_SECONDS;
-}
-
-static inline bool ratio_ok(double r) { return r > 0.0 && r < INFINITY; }
-
-// Why the cues of pairs [0, B) cannot be rasterised exactly, or nullptr: start_seconds, a ratio that is
-// not finite and positive, or a cue time (start or end; either array may be null = not checked) beyond
-// the limit above.  For non-finite times the reference raises in timedelta.  Metadata cues count: the
-// reference scales them too.  *at: the offending ratio or cue index, *val its value.
-static const char* bad_cue_input(const double* cue_start_s, const double* cue_end_s, const int64_t* cue_off,
-                                 int B, const double* ratios, int K, int per_pair_ratios, double start_seconds,
-                                 int64_t* at, double* val) {
-  *at = -1;
-  *val = start_seconds;
-  if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS)) return "start_seconds is not finite or too large";
-  for (int b = 0; b < B; ++b) {
-    double r_max = 0.0;
-    for (int k = 0; k < K; ++k) {
-      const size_t i = per_pair_ratios ? (size_t)b * K + k : (size_t)k;
-      *at = (int64_t)i;
-      *val = ratios[i];
-      if (!ratio_ok(ratios[i])) return "ratio is not a finite positive number";
-      r_max = std::max(r_max, ratios[i]);
-    }
-    const int64_t c0 = cue_off[b], c1 = cue_off[b + 1];
-    for (const double* t : {cue_start_s, cue_end_s}) {
-      if (!t) continue;
-      // one branch-free pass (four independent chains); the offending cue is looked for only on failure
-      uint64_t m4[4] = {0, 0, 0, 0};
-      int64_t c = c0;
-      for (; c + 4 <= c1; c += 4)
-        for (int i = 0; i < 4; ++i) m4[i] = std::max(m4[i], magnitude_bits(t[c + i]));
-      for (; c < c1; ++c) m4[0] = std::max(m4[0], magnitude_bits(t[c]));
-      if (cue_magnitude_ok(std::max(std::max(m4[0], m4[1]), std::max(m4[2], m4[3])), r_max)) continue;
-      for (int64_t c = c0; c < c1; ++c)
-        if (!cue_magnitude_ok(magnitude_bits(t[c]), r_max)) {
-          *at = c;
-          *val = t[c];
-          return t == cue_start_s ? "cue start time times ratio is not finite or too large"
-                                  : "cue end time times ratio is not finite or too large";
-        }
-    }
-  }
-  return nullptr;
-}
-
-// b2_rasterize_lengths, also checking the start times when cue_start_s is not null (b2_sync_batch: one
-// pass over the cues for both)
-static int rasterize_lengths(const double* cue_start_s, const double* cue_end_s, const int64_t* cue_off, int B,
-                             const double* ratios, int K, int per_pair_ratios, int sample_rate, int64_t* lengths) {
-  if (B < 0 || K < 0 || !cue_off || (!ratios && K) || !lengths || sample_rate <= 0)
-    return B2_ERR_BAD_ARG;
-  for (int b = 0; b < B; ++b) {
-    // max over cues of scaled(end) == scaled(max end) for ratio > 0: the product, the microsecond
-    // rounding and the division are all monotone non-decreasing (speech_transformers.py:958-960).
-    // The same pass finds the largest magnitude for the input check (see bad_cue_input).
-    // (four independent chains: this runs over every cue of every b2_sync_batch call).  A NaN end
-    // fails the check, so max_end may ignore it.
-    const int64_t c0 = cue_off[b], c1 = cue_off[b + 1];
-    const bool any = c1 > c0;
-    double e4[4];
-    uint64_t m4[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 4; ++i) e4[i] = any ? cue_end_s[c0] : 0.0;
-    int64_t c = c0;
-    for (; c + 4 <= c1; c += 4)
-      for (int i = 0; i < 4; ++i) {
-        e4[i] = std::max(e4[i], cue_end_s[c + i]);
-        m4[i] = std::max(m4[i], magnitude_bits(cue_end_s[c + i]));
-        if (cue_start_s) m4[i] = std::max(m4[i], magnitude_bits(cue_start_s[c + i]));
-      }
-    for (; c < c1; ++c) {
-      e4[0] = std::max(e4[0], cue_end_s[c]);
-      m4[0] = std::max(m4[0], magnitude_bits(cue_end_s[c]));
-      if (cue_start_s) m4[0] = std::max(m4[0], magnitude_bits(cue_start_s[c]));
-    }
-    const double max_end = std::max(std::max(e4[0], e4[1]), std::max(e4[2], e4[3]));
-    const uint64_t m = std::max(std::max(m4[0], m4[1]), std::max(m4[2], m4[3]));
-    for (int k = 0; k < K; ++k) {
-      double r = per_pair_ratios ? ratios[(size_t)b * K + k] : ratios[k];
-      if (!ratio_ok(r) || !cue_magnitude_ok(m, r)) return B2_ERR_BAD_ARG;
-      lengths[(size_t)b * K + k] = b2_signal_length(any ? max_end : 0.0, r, sample_rate);
-    }
-  }
-  return B2_OK;
-}
-
 extern "C" int b2_rasterize_lengths(const double* cue_end_s, const int64_t* cue_off, int B,
                                     const double* ratios, int K, int per_pair_ratios,
                                     int sample_rate, int64_t* lengths) {
@@ -980,250 +829,219 @@ extern "C" int b2_reduce_ratios(b2_handle h, const double* score, const int32_t*
 // subtitle tracks: track t is synced against video track_video[t] (non-decreasing; NULL: V == T, track t
 // against video t - b2_sync_batch).  Each video's PCM goes through the VAD once; its reference spectra
 // serve the K ratio jobs t*K + k of every one of its tracks.
-// The detector is this package's energy / zero-crossing VAD, or with `aud` the reference's auditok detector
-// (b2_vad_auditok's arguments; its float64 signal rounded once to float32 is the reference signal).
-struct AuditokArgs {
-  double non_speech_label, energy_threshold_db, min_length, max_continuous_silence;
-  int64_t max_length, chunk_samples;
-};
-// b2_sync_tracks_subs: videos with is_subs[v] != 0 take their cue list ref_off[v] .. ref_off[v+1] (host arrays,
-// absolute indices), rasterised at ratio 1.0 and level 1.0, as reference signal instead of the detector's output.
-struct SubsRefArgs {
-  const uint8_t* is_subs;
-  const double* cue_start_s;
-  const double* cue_end_s;
-  const uint8_t* cue_keep;   // may be null
-  const int64_t* cue_off;    // [V+1]
+// The detector is this package's energy / zero-crossing VAD, or the reference's auditok detector
+// (b2_vad_auditok's arguments; its float64 signal rounded once to float32 is the reference signal).  With
+// subtitle references (b2_sync_tracks_subs) the videos that have one take it instead.  Each entry point fills
+// one SyncRequest; plan_sync (sync_plan.h) checks it and builds the host tables, and sync_run below runs the
+// plan.
+
+// The device buffers one call reads and writes
+struct SyncBufs {
+  const int16_t* pcm;
+  float* refsig;
+  float* subsig;           // float subtitle signals (unfused raster only)
+  double* score;           // [T*K] per-ratio results: the caller's all_* on B2_DEVICE without the search
+  int32_t* offset;
+  int32_t* status;
+  double* bs;              // [T] reduced results: the caller's on B2_DEVICE
+  int32_t* bo;
+  int32_t* bk;
+  double* g_all_score;     // GSS outputs: the caller's on B2_DEVICE, staged otherwise
+  int32_t* g_all_offset;
+  double* g_ratio;
+  double* g_evals;
+  bool fused;
+  int winner_only;
 };
 
-static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm, const int64_t* pcm_off, int V,
-                            const int32_t* track_video, int T, int frame_rate, int sample_rate,
-                            float non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
-                            const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
-                            const int64_t* cue_off, const double* ratios, int K, double start_seconds,
-                            int64_t max_offset_samples, double* best_score, int32_t* best_offset,
-                            int32_t* best_k, double* all_score, int32_t* all_offset, int memspace,
-                            bool gss = false, double* gss_ratio = nullptr, double* gss_evals = nullptr,
-                            const AuditokArgs* aud = nullptr, const SubsRefArgs* subs = nullptr) {
-  const bool resident = memspace == B2_DEVICE_RESIDENT;
-  if (resident) memspace = B2_DEVICE;
-  const char* who = subs ? (gss ? "sync_tracks_subs (search)" : "sync_tracks_subs")
-                    : aud ? (gss ? "sync_tracks_auditok (search)" : "sync_tracks_auditok")
-                          : gss ? "sync_tracks_gss" : track_video ? "sync_tracks" : "sync_batch";
-  if (V < 0 || T < 0 || K <= 0 || !pcm_off || !cue_off || !ratios)
-    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad arguments", who);
-  // b2_sync_tracks_subs: which videos take a subtitle reference, checked before anything reads their tables
-  bool any_subs = false, any_audio = !subs;
-  int64_t audio_samples = 0;
-  if (subs) {
-    for (int v = 0; v < V; ++v) {
-      const bool is_subs = subs->is_subs && subs->is_subs[v];
-      if (subs->cue_off[v + 1] < subs->cue_off[v])
-        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: ref_cue_off not monotone at %d", who, v);
-      if (!is_subs && subs->cue_off[v + 1] != subs->cue_off[v])
-        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: video %d has reference cues but no subtitle reference (ref_is_subs[%d] = 0)",
-                who, v, v);
-      if (is_subs && pcm_off[v + 1] != pcm_off[v])
-        B2_FAIL(h, B2_ERR_BAD_ARG, "%s: video %d has a subtitle reference and a non-empty PCM range (%lld samples); "
-                "its audio is never read", who, v, (long long)(pcm_off[v + 1] - pcm_off[v]));
-      any_subs = any_subs || is_subs;
-      any_audio = any_audio || !is_subs;
-      if (pcm_off[v + 1] > pcm_off[v]) audio_samples += pcm_off[v + 1] - pcm_off[v];
+// rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
+// caller's stream, then the GSS rounds with the search
+static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1) {
+  const int K = r.K, t0 = p.trk_off[v0], nt = p.trk_off[v1] - t0;
+  const size_t j0 = (size_t)t0 * K;
+  std::vector<int> chain_trk(v1 - v0 + 1);
+  for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = p.trk_off[v] - t0;
+  if (!b.fused)
+    B2_TRY(b2i_raster_launch(h, r.cue_start_s, r.cue_end_s, r.cue_keep, r.cue_off + t0, nt, r.ratios, K, 0, nullptr,
+                             r.sample_rate, r.start_seconds, b.subsig, p.sub_off.data() + j0));
+  const B2CueSource src{r.cue_start_s, r.cue_end_s, r.cue_keep, r.cue_off + t0, r.ratios, r.sample_rate,
+                        r.start_seconds, p.ref_label, p.two_level};
+  B2_TRY(b2i_align_launch(h, b.refsig, p.ref_off.data() + v0, v1 - v0, chain_trk.data(), b.subsig,
+                          p.sub_off.data() + j0, nt, K, r.max_offset_samples, b.score + j0, b.offset + j0,
+                          b.status + j0, b.winner_only, b.fused ? &src : nullptr, (long long)j0));
+  B2_TRY(b2i_reduce_launch(h, b.score + j0, b.offset + j0, b.status + j0, nt, K, r.max_offset_samples, b.bs + t0,
+                           b.bo + t0, b.bk + t0));
+  if (!p.gss || nt == 0) return B2_OK;
+  const size_t a0 = (size_t)t0 * (K + 1);
+  const B2GssOut go{b.bs + t0, b.bo + t0, b.bk + t0, b.score + j0, b.offset + j0,
+                    b.g_all_score ? b.g_all_score + a0 : nullptr, b.g_all_offset ? b.g_all_offset + a0 : nullptr,
+                    b.g_ratio + t0, b.g_evals ? b.g_evals + (size_t)t0 * kGssEvals : nullptr};
+  return b2i_gss_launch(h, b.refsig, p.ref_off.data() + v0, v1 - v0, chain_trk.data(), K, src,
+                        p.max_end.data() + t0, r.max_offset_samples, go);
+}
+
+// The detector step of the videos [v0, v1), on whichever stream the handle launches on: the energy / ZCR VAD
+// into the reference-signal buffer, or for auditok the energy pass over the videos' chunks (label 0, every
+// crossing count accepted, a short last block judged on its own samples) writing its 0/1 flags there, then
+// the tokenizer turning each chunk's flags into its float32 signal in place.  Both auditok launches take a
+// metadata arena from the ring of the stream they run on; on the pipeline's internal stream that ring is its
+// own, so the GSS invariant (no later arena of a chain recycles the chain's arena, runcorr.cu b2i_gss_launch)
+// holds as before: the chains' arenas come from the caller-facing ring, and with one sub-batch the detector's
+// arenas there precede the chain's.
+// With subtitle references (b2_sync_tracks_subs) the step also rasterises those of the videos [v0, v1) into
+// their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
+// the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
+static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1) {
+  if (!p.auditok) {
+    B2_TRY(b2i_vad_launch(h, b.pcm, r.pcm_off + v0, v1 - v0, p.fpw, r.energy.non_speech_label,
+                          (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, p.ref_off.data() + v0));
+  } else {
+    const ChunkTable& ch = p.ch;
+    const int c0 = ch.first[v0], nc = ch.first[v1] - c0;
+    B2_TRY(b2i_vad_launch(h, b.pcm, ch.pcm.data() + c0, nc, p.fpw, 0.0f, p.auditok_e_min, 0, p.fpw, b.refsig,
+                          ch.out.data() + c0, ch.tail.data() + c0));
+    if (!p.any_subs) return b2i_tokenize_inplace_launch(h, b.refsig, ch.out.data() + c0, nc, p.tok);
+    const int k0 = ch.tok_first[v0];
+    B2_TRY(b2i_tokenize_inplace_launch(h, b.refsig, ch.tok_off.data() + k0, ch.tok_first[v1] - k0, p.tok,
+                                       ch.tok_end.data() + k0));
+  }
+  if (!p.any_subs) return B2_OK;
+  const auto& sv = p.sub_video;
+  const int s0 = (int)(std::lower_bound(sv.begin(), sv.end(), v0) - sv.begin());
+  const int s1 = (int)(std::lower_bound(sv.begin(), sv.end(), v1) - sv.begin());
+  if (s1 == s0) return B2_OK;
+  std::vector<int> rel(sv.begin() + s0, sv.begin() + s1);
+  for (int& v : rel) v -= v0;
+  return b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
+                               p.ref_off.data() + v0, v1 - v0, rel.data(), (int)rel.size(), r.sample_rate,
+                               r.start_seconds, b.refsig);
+}
+
+// Software pipeline over the plan's sub-batches of videos (sync_plan.h plan_cuts).  The VAD (HBM-bound) of every
+// sub-batch is queued on the internal high-priority stream: sub-batch 0 on the whole GPU, the later ones on
+// `vad_sms` SMs only (one lane-per-window CTA per SM, csrc/vad.cu); the rasterisation / correlation / reduction
+// of the tracks of sub-batch i (FP32- and shared-memory bound) follows on the caller's stream as soon as its VAD
+// is done and runs on the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler
+// keeps the two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); the
+// lane-group kernel needs every SM's issue slots to reach the HBM roofline, so partitioning never paid with it.
+// B2_DEVICE_RESIDENT, previous entry point on this handle = a pipelined resident b2_sync_batch or b2_sync_tracks
+// (`chained`): the VAD starts behind that call's fence (everything on the caller's stream up to, not including,
+// its last correlation chain) and overlaps that chain like a further sub-batch - on vad_sms SMs if it is still
+// running.  It writes the other reference-signal buffer (the chain still reads the previous one); the chains of
+// the call before that, which read this buffer, precede the fence.
+static int run_pipeline(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, bool resident,
+                        bool chained, int refsig_slot) {
+  const int n_sub = p.n_sub;
+  const std::vector<int>& cut = p.cut;
+  if (n_sub == 1) {
+    B2_TRY(detect(h, r, p, b, 0, r.V));
+    return enqueue_chain(h, r, p, b, 0, r.V);
+  }
+  std::vector<cudaEvent_t> vad_done(n_sub);
+  cudaEvent_t inputs_ready = next_event(h);
+  B2_CUDA(h, cudaEventRecord(inputs_ready, h->stream));
+  // B2_PIPE_TRACE=1 (diagnostic; synchronises): device timeline of the sub-batches and host enqueue times
+  const bool trace = getenv("B2_PIPE_TRACE") != nullptr;
+  std::vector<cudaEvent_t> tev;   // t0, then per sub-batch: VAD start, VAD end, chain start, chain end
+  std::vector<double> host_ms(n_sub + 1, 0.0);
+  const auto host_t0 = std::chrono::steady_clock::now();
+  auto host_now = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count(); };
+  if (trace) {
+    tev.resize(1 + 4 * (size_t)n_sub);
+    for (auto& e : tev) B2_CUDA(h, cudaEventCreate(&e));
+    B2_CUDA(h, cudaEventRecord(tev[0], h->stream));
+  }
+  bool prev_busy = false;
+  if (chained) {
+    prev_busy = cudaEventQuery(h->resident_done) == cudaErrorNotReady;
+    cudaGetLastError();
+  }
+  {
+    Stream2Scope on2(h);
+    B2_CUDA(h, cudaStreamWaitEvent(h->stream, chained ? h->resident_fence : inputs_ready, 0));
+    for (int i = 0; i < n_sub; ++i) {
+      h->vad_partition_sms = (i > 0 || prev_busy) ? p.vad_sms : 0;
+      if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
+      const int st = detect(h, r, p, b, cut[i], cut[i + 1]);
+      h->vad_partition_sms = 0;
+      if (st != B2_OK) return st;
+      vad_done[i] = next_event(h);
+      B2_CUDA(h, cudaEventRecord(vad_done[i], h->stream));
+      if (trace) B2_CUDA(h, cudaEventRecord(tev[2 + 4 * i], h->stream));
     }
-    if (V > 0 && subs->cue_off[V] > subs->cue_off[0] && (!subs->cue_start_s || !subs->cue_end_s))
-      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null reference cue arrays", who);
-    if (audio_samples > 0 && !pcm) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null pcm with %lld samples of audio", who,
-                                           (long long)audio_samples);
   }
-  // The run path and the GSS rounds need a reference of the two levels 1.0 and ref_label.  The detector's signal
-  // has the levels 1.0 and the label, a subtitle reference 1.0 and 0.0, so ref_label is the label unless every
-  // reference is a subtitle stream; a call that mixes the two at a non-zero label has three levels.  auditok's
-  // clipped cumsum has two levels only at label 0 (starts and ends alternate and an overwrite only turns an end
-  // into a start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3).
-  const float ref_label = any_audio ? non_speech_label : 0.0f;
-  const bool auditok_two_level = !aud || aud->non_speech_label == 0.0;
-  const bool mix_two_level = !any_subs || non_speech_label == 0.0f;
-  const bool two_level = !any_audio || (auditok_two_level && mix_two_level);
-  if (track_video) {
-    for (int t = 0; t < T; ++t)
-      if (track_video[t] < 0 || track_video[t] >= V || (t > 0 && track_video[t] < track_video[t - 1]))
-        B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: track_video[%d] = %d is out of [0, %d) or decreases", t,
-                (int)track_video[t], V);
-    for (int t = 0; t < T; ++t)
-      if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: cue_off not monotone at %d", t);
+  host_ms[0] = host_now();
+  for (int i = 0; i < n_sub; ++i) {
+    if (resident && i == n_sub - 1) B2_CUDA(h, cudaEventRecord(h->resident_fence, h->stream));
+    B2_CUDA(h, cudaStreamWaitEvent(h->stream, vad_done[i], 0));
+    if (trace) B2_CUDA(h, cudaEventRecord(tev[3 + 4 * i], h->stream));
+    B2_TRY(enqueue_chain(h, r, p, b, cut[i], cut[i + 1]));
+    if (trace) B2_CUDA(h, cudaEventRecord(tev[4 + 4 * i], h->stream));
+    host_ms[i + 1] = host_now();
   }
-  if (gss) {
-    // the envelope of the device-driven rounds (DESIGN.md section 4 "K8g"): every round runs on the run path
-    // (compared with half the window bound: 2 * max_offset_samples overflows for widths from 2^62 on)
-    if (max_offset_samples == B2_MAX_OFFSET_NONE || max_offset_samples < 0 ||
-        max_offset_samples > (int64_t)(kRunMaxWindow / 2))
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: max_offset_samples must lie in [0, %d] (a window of at most "
-              "2 max_offset_samples <= %d offsets, one CTA of the run path)", kRunMaxWindow / 2, kRunMaxWindow);
-    if (!std::isfinite(ref_label))
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: non_speech_label must be finite (the run path's two-level reference)");
-    if (!two_level && !auditok_two_level)
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: non_speech_label = %g gives the auditok signal more than two levels; the "
-              "search runs on the run path, which needs label 0", who, aud->non_speech_label);
-    if (!two_level)
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: subtitle references (levels 1 and 0) and audio references (levels 1 and "
-              "non_speech_label = %g) in one call give three levels; the search runs on the run path, which needs "
-              "label 0 or references of one kind", who, (double)non_speech_label);
-    for (int t = 0; t < T; ++t)
-      if (cue_off[t + 1] - cue_off[t] > kRunMaxCues)
-        B2_FAIL(h, B2_ERR_UNSUPPORTED, "sync_tracks_gss: track %d has %lld cues, more than %d", t,
-                (long long)(cue_off[t + 1] - cue_off[t]), kRunMaxCues);
+  if (resident) {
+    B2_CUDA(h, cudaEventRecord(h->resident_done, h->stream));
+    h->refsig_parity = refsig_slot == b2_ctx::WS_SIG_REF2 ? 1 : 0;
+    h->resident_fence_valid = true;
   }
+  if (trace) {
+    B2_CUDA(h, cudaStreamSynchronize(h->stream2));
+    B2_CUDA(h, cudaStreamSynchronize(h->stream));
+    auto at = [&](size_t k) {
+      float ms = 0.f;
+      cudaEventElapsedTime(&ms, tev[0], tev[k]);
+      return ms;
+    };
+    fprintf(stderr, "[b2 pipe] V=%d T=%d n_sub=%d vad_sms=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
+            r.V, r.T, n_sub, p.vad_sms, (int)chained, (int)prev_busy, host_ms[0]);
+    for (int i = 0; i < n_sub; ++i)
+      fprintf(stderr, "[b2 pipe]  sub %d videos %4d..%4d  VAD %7.3f -> %7.3f ms   chain %7.3f -> %7.3f ms   host enqueued chain at %.3f ms\n",
+              i, cut[i], cut[i + 1], at(1 + 4 * i), at(2 + 4 * i), at(3 + 4 * i), at(4 + 4 * i), host_ms[i + 1]);
+    for (auto& e : tev) cudaEventDestroy(e);
+  }
+  return B2_OK;
+}
+
+static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
+  SyncPlan p;
+  const SyncPipeEnv env{h->sm_count, b2_ctx::kEvents - 2, getenv("B2_SUBBATCHES"), getenv("B2_VAD_SMS"),
+                        b2i_vad_lane_eligible};
+  if (const int st = plan_sync(r, env, &p)) {
+    h->err = p.err;
+    return st;
+  }
+  const int T = r.T, K = r.K;
   if (T == 0) return B2_OK;
-  if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null output", who);
-  if (gss && !gss_ratio) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null gss_ratio", who);
-  const int fpw = aud ? b2_auditok_block_size(frame_rate, sample_rate) : b2_vad_frames_per_window(frame_rate, sample_rate);
-  if (aud) {   // b2_vad_auditok's checks
-    if (fpw <= 0)
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "%s: int(frame_rate/sample_rate) block size and frame_rate//sample_rate window "
-              "size differ (or are 0) for %d / %d", who, frame_rate, sample_rate);
-    if (aud->max_length <= 0 || !(aud->min_length > 0) || aud->min_length > (double)aud->max_length ||
-        !(aud->max_continuous_silence < (double)aud->max_length) || aud->chunk_samples < 0)
-      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad tokenizer parameters", who);
+  const bool resident = r.memspace == B2_DEVICE_RESIDENT;
+  const int memspace = resident ? B2_DEVICE : r.memspace;
+  // every bulk pointer of a B2_DEVICE call, before anything is launched
+  const char* prefix = r.track_video ? "sync_tracks" : "sync_batch";
+  const std::pair<const void*, const char*> bulk[] = {{r.pcm, "pcm"}, {r.best_score, "best_score"},
+                                                      {r.best_offset, "best_offset"}, {r.best_k, "best_k"},
+                                                      {r.all_score, "all_score"}, {r.all_offset, "all_offset"}};
+  for (const auto& [ptr, name] : bulk) {
+    char what[64];
+    snprintf(what, sizeof(what), "%s: %s", prefix, name);
+    B2_CHECK_DEV(h, memspace, ptr, what);
   }
-  if (fpw <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
-  if (z_lo < 0) z_lo = 0;
-  if (z_hi < 0) z_hi = (3 * fpw) / 8;
-  // trk_off[v]: first track of video v
-  std::vector<int> trk_off(V + 1);
-  for (int v = 0, t = 0; v <= V; ++v) {
-    if (track_video)
-      while (t < T && track_video[t] < v) ++t;
-    else
-      t = v;
-    trk_off[v] = t;
+  if (p.gss) {
+    B2_CHECK_DEV(h, memspace, r.gss_ratio, "sync_tracks_gss: gss_ratio");
+    B2_CHECK_DEV(h, memspace, r.gss_evals, "sync_tracks_gss: gss_evals");
   }
-  const size_t J = (size_t)T * K;
-  std::vector<int64_t> ref_off(V + 1), sub_off(J + 1), lengths(J);
-  ref_off[0] = 0;
-  // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
-  // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
-  // the tracks' cues).  sub_video: the videos with a subtitle reference, ascending.
-  std::vector<int64_t> subs_len;
-  std::vector<int> sub_video;
-  if (any_subs) {
-    const double one = 1.0;
-    subs_len.resize(V);
-    if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
-        rasterize_lengths(subs->cue_start_s, subs->cue_end_s, subs->cue_off, V, &one, 1, 0, sample_rate,
-                          subs_len.data()) != B2_OK) {
-      int64_t bad_at;
-      double bad_val;
-      const char* why = bad_cue_input(subs->cue_start_s, subs->cue_end_s, subs->cue_off, V, &one, 1, 0, start_seconds,
-                                      &bad_at, &bad_val);
-      if (!why) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad reference cue list", who);
-      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: reference %s (index %lld: %g)", who, why, (long long)bad_at, bad_val);
-    }
-    for (int v = 0; v < V; ++v)
-      if (subs->is_subs[v]) sub_video.push_back(v);
-  }
-  auto is_subs = [&](int v) { return any_subs && subs->is_subs[v] != 0; };
-  for (int v = 0; v < V; ++v) {
-    const int64_t n = pcm_off[v + 1] - pcm_off[v];
-    if (n < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
-    if (is_subs(v)) ref_off[v + 1] = ref_off[v] + subs_len[v];
-    else if (!aud) ref_off[v + 1] = ref_off[v] + (n + fpw - 1) / fpw;
-  }
-  // auditok: the reference's chunk loop.  Video v is cut into detector calls of chunk_samples samples (0: one
-  // call), chunks ch_first[v] .. ch_first[v+1]-1; chunk c spans samples ch_pcm[c] .. ch_pcm[c+1] of the PCM
-  // buffer and blocks ch_out[c] .. ch_out[c+1] of the reference signal, ceil(len/fpw) of them, so a video's
-  // signal is the sum over its chunks of ceil(len/fpw) long.  ch_tail[c]: the energy floor of the chunk's
-  // short last block (0: none).  Chunk starts are multiples of chunk_samples from the video's start
-  // ((2 fr // sr) * 5000 samples in the Python layer: a multiple of 8, so aligned videos stay eligible for
-  // the lane-per-window energy kernel).
-  // A video with a subtitle reference (no PCM) is one empty chunk spanning its reference's frames: the energy
-  // pass has no tiles there and the tokenizer's table (tok_*) leaves it out, so only the rasteriser writes it.
-  std::vector<int64_t> ch_pcm, ch_out, ch_tail, tok_off, tok_end;
-  std::vector<int> ch_first, tok_first;
-  if (aud) {
-    ch_first.assign(V + 1, 0);
-    ch_pcm.push_back(V ? pcm_off[0] : 0);
-    ch_out.push_back(0);
-    if (any_subs) tok_first.assign(V + 1, 0);
-    int tail_rem = -1;
-    int64_t tail_floor = 0;
-    for (int v = 0; v < V; ++v) {
-      const int64_t n = pcm_off[v + 1] - pcm_off[v];
-      if (is_subs(v)) {
-        ch_pcm.push_back(pcm_off[v + 1]);
-        ch_out.push_back(ch_out.back() + subs_len[v]);
-        ch_tail.push_back(0);
-        ch_first[v + 1] = (int)ch_tail.size();
-        tok_first[v + 1] = (int)tok_off.size();
-        ref_off[v + 1] = ch_out.back();
-        continue;
-      }
-      const int64_t step = aud->chunk_samples > 0 ? aud->chunk_samples : (n > 0 ? n : 1);
-      for (int64_t s = 0; s < n; s += step) {
-        const int64_t len = std::min(step, n - s);
-        ch_pcm.push_back(pcm_off[v] + s + len);
-        ch_out.push_back(ch_out.back() + (len + fpw - 1) / fpw);
-        const int rem = (int)(len % fpw);
-        if (rem && rem != tail_rem) {
-          tail_rem = rem;
-          tail_floor = b2_auditok_energy_floor(rem, aud->energy_threshold_db);
-        }
-        ch_tail.push_back(rem ? tail_floor : 0);
-        if (any_subs) {
-          tok_off.push_back(ch_out[ch_out.size() - 2]);
-          tok_end.push_back(ch_out.back());
-        }
-      }
-      ch_first[v + 1] = (int)ch_tail.size();
-      if (any_subs) tok_first[v + 1] = (int)tok_off.size();
-      ref_off[v + 1] = ch_out.back();
-    }
-  }
-  const int64_t auditok_e_min = aud ? b2_auditok_energy_floor(fpw, aud->energy_threshold_db) : 0;
-  const B2TokenizerParams tok{aud ? aud->min_length : 0.0, aud ? aud->max_continuous_silence : 0.0,
-                              aud ? aud->non_speech_label : 0.0, aud ? (long long)aud->max_length : 0};
-  // the lengths pass checks the cue times and ratios too; the offending input is looked for on failure
-  if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
-      rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, ratios, K, 0, sample_rate, lengths.data()) != B2_OK) {
-    int64_t bad_at;
-    double bad_val;
-    const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, T, ratios, K, 0, start_seconds, &bad_at, &bad_val);
-    if (!why) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad cue list / ratios", who);
-    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: %s (index %lld: %g)", who, why, (long long)bad_at, bad_val);
-  }
-  sub_off[0] = 0;
-  for (size_t j = 0; j < J; ++j) sub_off[j + 1] = sub_off[j] + lengths[j];
-  // GSS: each track's largest cue end (its signal length at any ratio), the cue times checked at the
-  // interval's upper end as well
-  std::vector<double> max_end;
-  if (gss) {
-    const double r_hi = B2_GSS_HI;
-    std::vector<int64_t> len_hi(T);
-    if (rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, &r_hi, 1, 0, sample_rate, len_hi.data()) != B2_OK) {
-      int64_t bad_at;
-      double bad_val;
-      const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, T, &r_hi, 1, 0, start_seconds, &bad_at, &bad_val);
-      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: at ratio %g: %s (index %lld: %g)", who, r_hi, why ? why : "bad cue list",
-              (long long)bad_at, bad_val);
-    }
-    max_end.assign(T, 0.0);
-    for (int t = 0; t < T; ++t)
-      for (int64_t c = cue_off[t]; c < cue_off[t + 1]; ++c)
-        max_end[t] = c == cue_off[t] ? cue_end_s[c] : std::max(max_end[t], cue_end_s[c]);
-  }
-
   // Default: the K subtitle signals of a track are never materialised as floats - the cue list is
   // rasterised into bit masks (1 bit per frame) that the correlation kernel and the exact re-score
   // read.  B2_FUSED_RASTER=0 (A/B and test knob): raster_cues_kernel writes float signals to HBM and
   // the generic aligner (the b2_align_batch path) reads them back.
-  bool fused = true;
-  if (const char* e = getenv("B2_FUSED_RASTER")) fused = atoi(e) != 0;
-
+  SyncBufs b{};
+  b.fused = true;
+  if (const char* e = getenv("B2_FUSED_RASTER")) b.fused = atoi(e) != 0;
+  const size_t J = (size_t)T * K, JG = (size_t)T * (K + 1);
   void *d_refsig, *d_subsig = nullptr, *d_res;
-  // a chained resident call (see below) writes the buffer the previous call is not reading any more
-  const bool chained_candidate = resident && fence_was_valid;
-  const int refsig_slot = chained_candidate && h->refsig_parity == 0 ? b2_ctx::WS_SIG_REF2 : b2_ctx::WS_SIG_REF;
-  B2_TRY(b2i_ws(h, refsig_slot, (size_t)ref_off[V] * 4 + 64, &d_refsig));
-  if (!fused) B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_SUB, (size_t)sub_off[J] * 4 + 64, &d_subsig));
+  // a chained resident call writes the buffer the previous call is not reading any more
+  const bool chained = resident && fence_was_valid;
+  const int refsig_slot = chained && h->refsig_parity == 0 ? b2_ctx::WS_SIG_REF2 : b2_ctx::WS_SIG_REF;
+  B2_TRY(b2i_ws(h, refsig_slot, (size_t)p.ref_off[r.V] * 4 + 64, &d_refsig));
+  if (!b.fused) B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_SUB, (size_t)p.sub_off[J] * 4 + 64, &d_subsig));
   B2_TRY(b2i_ws(h, b2_ctx::WS_MISC, J * 16 + (size_t)T * 16 + 256, &d_res));
   double* d_score = (double*)d_res;
   double* d_bs = d_score + J;
@@ -1231,236 +1049,55 @@ static int sync_tracks_body(b2_ctx* h, bool fence_was_valid, const int16_t* pcm,
   int32_t* d_status = d_offset + J;
   int32_t* d_bo = d_status + J;
   int32_t* d_bk = d_bo + T;
-
-  B2_CHECK_DEV(h, memspace, pcm, track_video ? "sync_tracks: pcm" : "sync_batch: pcm");
-  B2_CHECK_DEV(h, memspace, best_score, track_video ? "sync_tracks: best_score" : "sync_batch: best_score");
-  if (track_video) {   // b2_sync_batch has always checked the two above only
-    B2_CHECK_DEV(h, memspace, best_offset, "sync_tracks: best_offset");
-    B2_CHECK_DEV(h, memspace, best_k, "sync_tracks: best_k");
-    B2_CHECK_DEV(h, memspace, all_score, "sync_tracks: all_score");
-    B2_CHECK_DEV(h, memspace, all_offset, "sync_tracks: all_offset");
-  }
-  if (gss) {
-    B2_CHECK_DEV(h, memspace, gss_ratio, "sync_tracks_gss: gss_ratio");
-    B2_CHECK_DEV(h, memspace, gss_evals, "sync_tracks_gss: gss_evals");
-  }
+  b.refsig = (float*)d_refsig;
+  b.subsig = (float*)d_subsig;
+  b.status = d_status;
   // GSS: the grid's per-ratio results stay in the workspace (all_* then hold K + 1 columns, written by the
   // combine); host calls stage the GSS outputs in a second workspace
-  const size_t JG = (size_t)T * (K + 1);
-  double *g_all_score = nullptr, *g_ratio = gss_ratio, *g_evals = gss_evals;
-  int32_t* g_all_offset = nullptr;
-  if (gss) {
+  b.g_ratio = r.gss_ratio;
+  b.g_evals = r.gss_evals;
+  if (p.gss) {
     void* d_go;
     B2_TRY(b2i_ws(h, b2_ctx::WS_GSS_OUT, JG * 12 + (size_t)T * 8 * (1 + kGssEvals) + 256, &d_go));
     double* hs = (double*)d_go;
     double* hr = hs + JG;
     double* he = hr + T;
     int32_t* ho = (int32_t*)(he + (size_t)T * kGssEvals);
-    g_all_score = all_score ? (memspace == B2_DEVICE ? all_score : hs) : nullptr;
-    g_all_offset = all_offset ? (memspace == B2_DEVICE ? all_offset : ho) : nullptr;
+    b.g_all_score = r.all_score ? (memspace == B2_DEVICE ? r.all_score : hs) : nullptr;
+    b.g_all_offset = r.all_offset ? (memspace == B2_DEVICE ? r.all_offset : ho) : nullptr;
     if (memspace != B2_DEVICE) {
-      g_ratio = hr;
-      g_evals = gss_evals ? he : nullptr;
+      b.g_ratio = hr;
+      b.g_evals = r.gss_evals ? he : nullptr;
     }
   }
-  const int16_t* d_pcm = pcm;
-  if (memspace == B2_HOST && !(subs && !pcm)) {   // (without any audio b2_sync_tracks_subs may take no pcm)
-    void* dp;
-    B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, pcm, (size_t)pcm_off[V] * 2, &dp));
-    d_pcm = (const int16_t*)dp;
+  b.pcm = r.pcm;
+  if (memspace == B2_HOST) {   // a call without audio samples reads no PCM (b2_sync_tracks_subs may pass none)
+    void* dp = nullptr;
+    if (p.audio_samples > 0) B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, &dp));
+    b.pcm = (const int16_t*)dp;
   }
-  double* o_score = (memspace == B2_DEVICE && all_score && !gss) ? all_score : d_score;
-  int32_t* o_offset = (memspace == B2_DEVICE && all_offset && !gss) ? all_offset : d_offset;
-  double* o_bs = memspace == B2_DEVICE ? best_score : d_bs;
-  int32_t* o_bo = memspace == B2_DEVICE ? best_offset : d_bo;
-  int32_t* o_bk = memspace == B2_DEVICE ? best_k : d_bk;
+  const bool dev = memspace == B2_DEVICE;
+  b.score = (dev && r.all_score && !p.gss) ? r.all_score : d_score;
+  b.offset = (dev && r.all_offset && !p.gss) ? r.all_offset : d_offset;
+  b.bs = dev ? r.best_score : d_bs;
+  b.bo = dev ? r.best_offset : d_bo;
+  b.bk = dev ? r.best_k : d_bk;
   // only the best ratio of each track is reported unless the per-ratio arrays are requested:
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
-  const int winner_only = (!all_score && !all_offset) ? 1 : 0;
-  // rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
-  // caller's stream
-  std::vector<int> chain_trk;
-  auto enqueue_chain = [&](int v0, int v1) -> int {
-    const int t0 = trk_off[v0], nt = trk_off[v1] - t0;
-    const size_t j0 = (size_t)t0 * K;
-    chain_trk.resize(v1 - v0 + 1);
-    for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = trk_off[v] - t0;
-    if (!fused)
-      B2_TRY(b2i_raster_launch(h, cue_start_s, cue_end_s, cue_keep, cue_off + t0, nt, ratios, K, 0, nullptr,
-                               sample_rate, start_seconds, (float*)d_subsig, sub_off.data() + j0));
-    const B2CueSource src{cue_start_s, cue_end_s, cue_keep, cue_off + t0, ratios, sample_rate, start_seconds,
-                          ref_label, two_level};
-    B2_TRY(b2i_align_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(),
-                            (const float*)d_subsig, sub_off.data() + j0, nt, K, max_offset_samples, o_score + j0,
-                            o_offset + j0, d_status + j0, winner_only, fused ? &src : nullptr, (long long)j0));
-    B2_TRY(b2i_reduce_launch(h, o_score + j0, o_offset + j0, d_status + j0, nt, K, max_offset_samples,
-                             o_bs + t0, o_bo + t0, o_bk + t0));
-    if (!gss || nt == 0) return B2_OK;
-    const size_t a0 = (size_t)t0 * (K + 1);
-    const B2GssOut go{o_bs + t0, o_bo + t0, o_bk + t0, o_score + j0, o_offset + j0,
-                      g_all_score ? g_all_score + a0 : nullptr, g_all_offset ? g_all_offset + a0 : nullptr,
-                      g_ratio + t0, g_evals ? g_evals + (size_t)t0 * kGssEvals : nullptr};
-    return b2i_gss_launch(h, (const float*)d_refsig, ref_off.data() + v0, v1 - v0, chain_trk.data(), K, src,
-                          max_end.data() + t0, max_offset_samples, go);
-  };
-
-  // Software pipeline over sub-batches of videos.  The VAD (HBM-bound) of every sub-batch is queued on the
-  // internal high-priority stream: sub-batch 0 on the whole GPU, the later ones on `vad_sms` SMs only (one
-  // lane-per-window CTA per SM, csrc/vad.cu); the rasterisation / correlation / reduction of the tracks of
-  // sub-batch i (FP32- and shared-memory bound) follows on the caller's stream as soon as its VAD is done and
-  // runs on the SMs the VAD leaves free - a VAD CTA owns its SM's shared memory, so the block scheduler keeps
-  // the two apart.  Needs the lane-per-window kernel (1.3 instructions per byte: ~80 GB/s per SM); the
-  // lane-group kernel needs every SM's issue slots to reach the HBM roofline, so partitioning never paid
-  // with it.  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
-  // Defaults: 3 sub-batches, the later VADs on 54 % of the SMs (71 of an H100's 132;
-  // tools/pipeline_probe.py sweeps both); small batches stay unpipelined (the alignment of a third of a small
-  // batch is launch- and tail-bound).
-  // Sub-batches are cut at video boundaries (a video's tracks run in the chain behind its own VAD) and
-  // balanced by track count, since the chain's work scales with tracks: cut i is the first video whose
-  // tracks start at or after track T*i/n_sub.  With one track per video these are T*i/n_sub exactly.
-  // Cuts that would leave a sub-batch without tracks are dropped; a video without tracks has its VAD run in
-  // the sub-batch of the next video that has tracks (trailing ones: of the last).  Where the cuts fall
-  // changes no result.
-  // The detector step of the videos [v0, v1), on whichever stream the handle launches on: the energy / ZCR VAD
-  // into the reference-signal buffer, or for auditok the energy pass over the videos' chunks (label 0, every
-  // crossing count accepted, a short last block judged on its own samples) writing its 0/1 flags there, then
-  // the tokenizer turning each chunk's flags into its float32 signal in place.  Both auditok launches take a
-  // metadata arena from the ring of the stream they run on; on the pipeline's internal stream that ring is its
-  // own, so the GSS invariant (no later arena of a chain recycles the chain's arena, runcorr.cu b2i_gss_launch)
-  // holds as before: the chains' arenas come from the caller-facing ring, and with one sub-batch the detector's
-  // arenas there precede the chain's.
-  // With subtitle references (b2_sync_tracks_subs) the step also rasterises those of the videos [v0, v1) into
-  // their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
-  // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
-  auto detect = [&](int v0, int v1) -> int {
-    if (!aud) {
-      B2_TRY(b2i_vad_launch(h, d_pcm, pcm_off + v0, v1 - v0, fpw, non_speech_label, (int64_t)fpw * energy_threshold,
-                            z_lo, z_hi, (float*)d_refsig, ref_off.data() + v0));
-    } else {
-      const int c0 = ch_first[v0], nc = ch_first[v1] - c0;
-      B2_TRY(b2i_vad_launch(h, d_pcm, ch_pcm.data() + c0, nc, fpw, 0.0f, auditok_e_min, 0, fpw, (float*)d_refsig,
-                            ch_out.data() + c0, ch_tail.data() + c0));
-      if (!any_subs) return b2i_tokenize_inplace_launch(h, (float*)d_refsig, ch_out.data() + c0, nc, tok);
-      const int k0 = tok_first[v0];
-      B2_TRY(b2i_tokenize_inplace_launch(h, (float*)d_refsig, tok_off.data() + k0, tok_first[v1] - k0, tok,
-                                         tok_end.data() + k0));
-    }
-    if (!any_subs) return B2_OK;
-    const int s0 = (int)(std::lower_bound(sub_video.begin(), sub_video.end(), v0) - sub_video.begin());
-    const int s1 = (int)(std::lower_bound(sub_video.begin(), sub_video.end(), v1) - sub_video.begin());
-    if (s1 == s0) return B2_OK;
-    std::vector<int> rel(sub_video.begin() + s0, sub_video.begin() + s1);
-    for (int& v : rel) v -= v0;
-    return b2i_raster_ref_launch(h, subs->cue_start_s, subs->cue_end_s, subs->cue_keep, subs->cue_off + v0,
-                                 ref_off.data() + v0, v1 - v0, rel.data(), (int)rel.size(), sample_rate, start_seconds,
-                                 (float*)d_refsig);
-  };
-  int n_sub = 1, vad_sms = 0;
-  // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks
-  const bool lane_ok = aud ? b2i_vad_lane_eligible(ch_pcm.data(), (int)ch_tail.size(), fpw)
-                           : b2i_vad_lane_eligible(pcm_off, V, fpw);
-  if (T >= 96 && lane_ok) {
-    n_sub = 3;
-    vad_sms = (h->sm_count * 54 + 50) / 100;
-  }
-  if (const char* e = getenv("B2_SUBBATCHES")) n_sub = std::max(1, std::min(T, atoi(e)));
-  if (const char* e = getenv("B2_VAD_SMS")) vad_sms = std::max(0, std::min(h->sm_count, atoi(e)));
-  n_sub = std::min(n_sub, b2_ctx::kEvents - 2);
-  std::vector<int> cut(1, 0);   // video cuts; every sub-batch holds at least one track
-  for (int i = 1; i < n_sub; ++i) {
-    const int target = (int)((int64_t)T * i / n_sub);
-    const int v = (int)(std::lower_bound(trk_off.begin(), trk_off.end(), target) - trk_off.begin());
-    if (trk_off[v] > trk_off[cut.back()] && trk_off[v] < T) cut.push_back(v);
-  }
-  cut.push_back(V);
-  n_sub = (int)cut.size() - 1;
-  if (n_sub == 1) {
-    B2_TRY(detect(0, V));
-    B2_TRY(enqueue_chain(0, V));
+  b.winner_only = (!r.all_score && !r.all_offset) ? 1 : 0;
+  B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
+  if (dev) return B2_OK;
+  B2_TRY(copy_out(h, r.best_score, d_bs, (size_t)T * 8));
+  B2_TRY(copy_out(h, r.best_offset, d_bo, (size_t)T * 4));
+  B2_TRY(copy_out(h, r.best_k, d_bk, (size_t)T * 4));
+  if (p.gss) {
+    if (r.all_score) B2_TRY(copy_out(h, r.all_score, b.g_all_score, JG * 8));
+    if (r.all_offset) B2_TRY(copy_out(h, r.all_offset, b.g_all_offset, JG * 4));
+    B2_TRY(copy_out(h, r.gss_ratio, b.g_ratio, (size_t)T * 8));
+    if (r.gss_evals) B2_TRY(copy_out(h, r.gss_evals, b.g_evals, (size_t)T * kGssEvals * 8));
   } else {
-    std::vector<cudaEvent_t> vad_done(n_sub);
-    cudaEvent_t inputs_ready = next_event(h);
-    B2_CUDA(h, cudaEventRecord(inputs_ready, h->stream));
-    // B2_PIPE_TRACE=1 (diagnostic; synchronises): device timeline of the sub-batches and host enqueue times
-  const bool trace = getenv("B2_PIPE_TRACE") != nullptr;
-    std::vector<cudaEvent_t> tev;   // t0, then per sub-batch: VAD start, VAD end, chain start, chain end
-    std::vector<double> host_ms(n_sub + 1, 0.0);
-    const auto host_t0 = std::chrono::steady_clock::now();
-    auto host_now = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count(); };
-    if (trace) {
-      tev.resize(1 + 4 * (size_t)n_sub);
-      for (auto& e : tev) B2_CUDA(h, cudaEventCreate(&e));
-      B2_CUDA(h, cudaEventRecord(tev[0], h->stream));
-    }
-    // B2_DEVICE_RESIDENT, previous entry point on this handle = a pipelined resident b2_sync_batch or
-    // b2_sync_tracks: the VAD starts behind that call's fence (everything on the caller's stream up to, not
-    // including, its last correlation chain) and overlaps that chain like a further sub-batch - on vad_sms
-    // SMs if it is still running.
-    // It writes the other reference-signal buffer (the chain still reads the previous one); the chains of the
-    // call before that, which read this buffer, precede the fence.
-    const bool chained = chained_candidate;
-    bool prev_busy = false;
-    if (chained) {
-      prev_busy = cudaEventQuery(h->resident_done) == cudaErrorNotReady;
-      cudaGetLastError();
-    }
-    {
-      Stream2Scope on2(h);
-      B2_CUDA(h, cudaStreamWaitEvent(h->stream, chained ? h->resident_fence : inputs_ready, 0));
-      for (int i = 0; i < n_sub; ++i) {
-        const int v0 = cut[i], v1 = cut[i + 1];
-        h->vad_partition_sms = (i > 0 || prev_busy) ? vad_sms : 0;
-        if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
-        const int st = detect(v0, v1);
-        h->vad_partition_sms = 0;
-        if (st != B2_OK) return st;
-        vad_done[i] = next_event(h);
-        B2_CUDA(h, cudaEventRecord(vad_done[i], h->stream));
-        if (trace) B2_CUDA(h, cudaEventRecord(tev[2 + 4 * i], h->stream));
-      }
-    }
-    host_ms[0] = host_now();
-    for (int i = 0; i < n_sub; ++i) {
-      if (resident && i == n_sub - 1) B2_CUDA(h, cudaEventRecord(h->resident_fence, h->stream));
-      B2_CUDA(h, cudaStreamWaitEvent(h->stream, vad_done[i], 0));
-      if (trace) B2_CUDA(h, cudaEventRecord(tev[3 + 4 * i], h->stream));
-      B2_TRY(enqueue_chain(cut[i], cut[i + 1]));
-      if (trace) B2_CUDA(h, cudaEventRecord(tev[4 + 4 * i], h->stream));
-      host_ms[i + 1] = host_now();
-    }
-    if (resident) {
-      B2_CUDA(h, cudaEventRecord(h->resident_done, h->stream));
-      h->refsig_parity = refsig_slot == b2_ctx::WS_SIG_REF2 ? 1 : 0;
-      h->resident_fence_valid = true;
-    }
-    if (trace) {
-      B2_CUDA(h, cudaStreamSynchronize(h->stream2));
-      B2_CUDA(h, cudaStreamSynchronize(h->stream));
-      auto at = [&](size_t k) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, tev[0], tev[k]);
-        return ms;
-      };
-      fprintf(stderr, "[b2 pipe] V=%d T=%d n_sub=%d vad_sms=%d chained=%d prev_busy=%d; host: VADs enqueued at %.3f ms\n",
-              V, T, n_sub, vad_sms, (int)chained, (int)prev_busy, host_ms[0]);
-      for (int i = 0; i < n_sub; ++i)
-        fprintf(stderr, "[b2 pipe]  sub %d videos %4d..%4d  VAD %7.3f -> %7.3f ms   chain %7.3f -> %7.3f ms   host enqueued chain at %.3f ms\n",
-                i, cut[i], cut[i + 1], at(1 + 4 * i), at(2 + 4 * i), at(3 + 4 * i), at(4 + 4 * i), host_ms[i + 1]);
-      for (auto& e : tev) cudaEventDestroy(e);
-    }
-  }
-  if (memspace == B2_DEVICE) return B2_OK;
-  B2_TRY(copy_out(h, best_score, d_bs, (size_t)T * 8));
-  B2_TRY(copy_out(h, best_offset, d_bo, (size_t)T * 4));
-  B2_TRY(copy_out(h, best_k, d_bk, (size_t)T * 4));
-  if (gss) {
-    if (all_score) B2_TRY(copy_out(h, all_score, g_all_score, JG * 8));
-    if (all_offset) B2_TRY(copy_out(h, all_offset, g_all_offset, JG * 4));
-    B2_TRY(copy_out(h, gss_ratio, g_ratio, (size_t)T * 8));
-    if (gss_evals) B2_TRY(copy_out(h, gss_evals, g_evals, (size_t)T * kGssEvals * 8));
-  } else {
-    if (all_score) B2_TRY(copy_out(h, all_score, d_score, J * 8));
-    if (all_offset) B2_TRY(copy_out(h, all_offset, d_offset, J * 4));
+    if (r.all_score) B2_TRY(copy_out(h, r.all_score, d_score, J * 8));
+    if (r.all_offset) B2_TRY(copy_out(h, r.all_offset, d_offset, J * 4));
   }
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
@@ -1476,10 +1113,11 @@ extern "C" int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm
                              double* all_score, int32_t* all_offset, int memspace) {
   B2_ENTER(h);
   B2Range range("b2_sync_batch");
-  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, B, nullptr, B, frame_rate, sample_rate,
-                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
-                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
-                          all_offset, memspace);
+  const SyncRequest r{"sync_batch", pcm, pcm_off, B, nullptr, B, frame_rate, sample_rate, B2_DETECTOR_ENERGY_ZCR,
+                      {non_speech_label, energy_threshold, z_lo, z_hi}, {}, {},
+                      cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                      best_score, best_offset, best_k, all_score, all_offset, false, nullptr, nullptr, memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
 }
 
 extern "C" int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
@@ -1492,10 +1130,11 @@ extern "C" int b2_sync_tracks(b2_handle h, const int16_t* pcm, const int64_t* pc
   B2_ENTER(h);
   B2Range range("b2_sync_tracks");
   if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks: null track_video");
-  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
-                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
-                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
-                          all_offset, memspace);
+  const SyncRequest r{"sync_tracks", pcm, pcm_off, V, track_video, T, frame_rate, sample_rate, B2_DETECTOR_ENERGY_ZCR,
+                      {non_speech_label, energy_threshold, z_lo, z_hi}, {}, {},
+                      cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                      best_score, best_offset, best_k, all_score, all_offset, false, nullptr, nullptr, memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
 }
 
 extern "C" int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
@@ -1509,10 +1148,11 @@ extern "C" int b2_sync_tracks_gss(b2_handle h, const int16_t* pcm, const int64_t
   B2_ENTER(h);
   B2Range range("b2_sync_tracks_gss");
   if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_gss: null track_video");
-  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
-                          non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep, cue_off,
-                          ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
-                          all_offset, memspace, /*gss=*/true, gss_ratio, gss_evals);
+  const SyncRequest r{"sync_tracks_gss", pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
+                      B2_DETECTOR_ENERGY_ZCR, {non_speech_label, energy_threshold, z_lo, z_hi}, {}, {},
+                      cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                      best_score, best_offset, best_k, all_score, all_offset, true, gss_ratio, gss_evals, memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
 }
 
 extern "C" int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
@@ -1528,13 +1168,14 @@ extern "C" int b2_sync_tracks_auditok(b2_handle h, const int16_t* pcm, const int
   B2Range range("b2_sync_tracks_auditok");
   if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_auditok: null track_video");
   if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_auditok: gss_evals without gss_ratio");
-  const AuditokArgs aud{non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
-                        chunk_samples};
-  // the energy / ZCR arguments are unused: z_lo / z_hi < 0 select defaults, the threshold is never read
-  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
-                          (float)non_speech_label, 0, -1, -1, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K,
-                          start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score, all_offset,
-                          memspace, /*gss=*/gss_ratio != nullptr, gss_ratio, gss_evals, &aud);
+  const SyncRequest r{gss_ratio ? "sync_tracks_auditok (search)" : "sync_tracks_auditok", pcm, pcm_off, V, track_video,
+                      T, frame_rate, sample_rate, B2_DETECTOR_AUDITOK, {},
+                      {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
+                       chunk_samples},
+                      {}, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                      best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
+                      memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
 }
 
 extern "C" int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
@@ -1557,18 +1198,14 @@ extern "C" int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm, const int64_
   if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
     B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_subs: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, "
             "not %d", detector);
-  const int64_t no_cues[1] = {0};
-  const SubsRefArgs subs{ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : no_cues};
-  const bool gss = gss_ratio != nullptr;
-  if (detector == B2_DETECTOR_ENERGY_ZCR)
-    return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
-                            (float)non_speech_label, energy_threshold, z_lo, z_hi, cue_start_s, cue_end_s, cue_keep,
-                            cue_off, ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k,
-                            all_score, all_offset, memspace, gss, gss_ratio, gss_evals, nullptr, &subs);
-  const AuditokArgs aud{non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
-                        chunk_samples};
-  return sync_tracks_body(h, _b2_fence_was_valid, pcm, pcm_off, V, track_video, T, frame_rate, sample_rate,
-                          (float)non_speech_label, 0, -1, -1, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K,
-                          start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score, all_offset,
-                          memspace, gss, gss_ratio, gss_evals, &aud, &subs);
+  static const int64_t no_cues[1] = {0};
+  const SyncRequest r{gss_ratio ? "sync_tracks_subs (search)" : "sync_tracks_subs", pcm, pcm_off, V, track_video, T,
+                      frame_rate, sample_rate, detector, {(float)non_speech_label, energy_threshold, z_lo, z_hi},
+                      {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length,
+                       chunk_samples},
+                      {ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : no_cues},
+                      cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                      best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
+                      memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
 }

@@ -1,8 +1,8 @@
 """CPU suite for the auditok detector inside the batched sync (b2_sync_tracks_auditok).
 
 Checks what can be checked without a GPU: the symbol and its ctypes signature against the header, the
-front end's argument checks, the chunk table / reference-length arithmetic the C side uses (recomputed here
-against the lengths the oracle's chunk loop produces), and the two-level property of the auditok signal at
+front end's argument checks, the chunk table / reference-length arithmetic of the C planner (against the lengths
+the oracle's chunk loop produces), and the two-level property of the auditok signal at
 label 0 that lets the run path and the golden-section search read it."""
 import ctypes
 import os
@@ -14,6 +14,7 @@ import pytest
 
 from conftest import ROOT
 from oracle import auditok_oracle as au
+from sync_plan import plan
 
 
 @pytest.fixture(scope="module")
@@ -94,22 +95,14 @@ def test_chunk_samples_is_the_chunk_loop_read_size():
 
 # ---------------------------------------------------------------- chunk table
 
-def _chunk_table(pcm_off, fpw, chunk_samples):
-    """The C side's table (api.cu, sync_tracks_body): per video, chunks of chunk_samples samples (0: one);
-    returns (chunk pcm offsets, chunk block offsets, first chunk of each video, ref_off)."""
-    ch_pcm, ch_out, first, ref_off = [pcm_off[0] if len(pcm_off) > 1 else 0], [0], [0], [0]
-    for v in range(len(pcm_off) - 1):
-        n = pcm_off[v + 1] - pcm_off[v]
-        step = chunk_samples if chunk_samples > 0 else max(n, 1)
-        s = 0
-        while s < n:
-            ln = min(step, n - s)
-            ch_pcm.append(pcm_off[v] + s + ln)
-            ch_out.append(ch_out[-1] + (ln + fpw - 1) // fpw)
-            s += step
-        first.append(len(ch_pcm) - 1)
-        ref_off.append(ch_out[-1])
-    return ch_pcm, ch_out, first, ref_off
+def _chunk_table(pcm_off, fr, chunk_samples):
+    """The planner's table (csrc/sync_plan.h, build_chunk_table, as b2_sync_tracks_auditok plans it with one track
+    per video): returns (chunk pcm offsets, chunk block offsets, first chunk of each video, ref_off)."""
+    V = len(pcm_off) - 1
+    p = plan(who="sync_tracks_auditok", detector=1, frame_rate=fr, sample_rate=100, chunk_samples=chunk_samples,
+             pcm_off=pcm_off, cue_start=[], cue_end=[], cue_off=[0] * (V + 1), ratios=[1.0])
+    assert p["status"] == 0, p["err"]
+    return p["ch_pcm"].tolist(), p["ch_out"].tolist(), p["ch_first"].tolist(), p["ref_off"].tolist()
 
 
 @pytest.mark.parametrize("fr", [8000, 16000, 22050, 44100, 48000])
@@ -119,7 +112,7 @@ def test_reference_length_is_the_oracle_chunk_loop_length(fr):
     chunk = (2 * fr // sr) * 5000
     lengths = [0, 1, fpw - 1, fpw, chunk - 1, chunk, chunk + 1, 2 * chunk, 3 * chunk + 7, 2 * chunk - fpw + 1]
     pcm_off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
-    ch_pcm, ch_out, first, ref_off = _chunk_table(list(pcm_off), fpw, chunk)
+    ch_pcm, ch_out, first, ref_off = _chunk_table(list(pcm_off), fr, chunk)
     silent = np.zeros(max(lengths), np.int16)
     for v, n in enumerate(lengths):
         # the reference's chunk loop: one detector call per chunk, outputs concatenated
@@ -141,7 +134,7 @@ def test_reference_length_is_the_oracle_chunk_loop_length(fr):
 
 def test_chunk_samples_zero_is_one_call_per_video():
     pcm_off = [0, 0, 1, 161, 16000 * 300 + 5]
-    _, _, first, ref_off = _chunk_table(pcm_off, 160, 0)
+    _, _, first, ref_off = _chunk_table(pcm_off, 16000, 0)
     assert np.diff(first).tolist() == [0, 1, 1, 1]
     assert np.diff(ref_off).tolist() == [0, 1, 1, (16000 * 300 + 5 - 161 + 159) // 160]
 

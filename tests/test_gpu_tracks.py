@@ -310,3 +310,30 @@ def test_tracks_bad_arguments(handle, corpus):
     assert st == -1
     # nothing to sync: legal
     assert _run_tracks(handle, dict(c, track_video=np.zeros(0, np.int32), cue_off=c["cue_off"][:1]))[0].shape == (0,)
+
+
+def test_sync_batch_rejects_a_host_output_under_b2_device(handle, corpus):
+    """b2_sync_batch checks every device output the way the track calls do, before it launches anything."""
+    import torch
+    from ffsubsync_b200 import _native
+    c = corpus
+    B = len(c["pcm_off"]) - 1
+    cue_off = c["cue_off"][: B + 1]                  # the first B tracks, track b against video b
+    pcm_d = torch.from_numpy(c["pcm"]).cuda()
+    dev = dict(best_score=torch.empty(B, dtype=torch.float64, device="cuda"),
+               best_offset=torch.empty(B, dtype=torch.int32, device="cuda"),
+               best_k=torch.empty(B, dtype=torch.int32, device="cuda"),
+               all_score=torch.empty(B * len(GRID), dtype=torch.float64, device="cuda"),
+               all_offset=torch.empty(B * len(GRID), dtype=torch.int32, device="cuda"))
+    args = (c["pcm_off"], 16000, 100, 0.0, 100000, -1, -1, c["cue_start"], c["cue_end"], None, cue_off, GRID, 0.0, MOS)
+    handle.sync_batch(pcm_d.data_ptr(), *args, **{k: v.data_ptr() for k, v in dev.items()},
+                      memspace=_native.B2_DEVICE)
+    handle.synchronize()
+    for host in dev:
+        host_buf = np.empty(dev[host].numel(), dtype=dev[host].cpu().numpy().dtype)
+        ptrs = {k: (host_buf.ctypes.data if k == host else v.data_ptr()) for k, v in dev.items()}
+        n0 = handle.launch_count
+        with pytest.raises(_native.NativeError) as ei:
+            handle.sync_batch(pcm_d.data_ptr(), *args, **ptrs, memspace=_native.B2_DEVICE)
+        assert ei.value.status == -1 and "sync_batch: %s" % host in str(ei.value), host
+        assert handle.launch_count == n0, host

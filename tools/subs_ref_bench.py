@@ -134,9 +134,9 @@ def main():
         c_out = [torch.empty(V, dtype=dt, device=dev) for dt in (torch.float64, torch.int32, torch.int32)]
         c_as = torch.empty(V * K, dtype=torch.float64, device=dev)
         c_ao = torch.empty(V * K, dtype=torch.int32, device=dev)
-        ss._subs_tracks(pcm.data_ptr(), pcm_off, tv, cs, ce, cue_off, None, refs, False,
-                        best_score=c_out[0].data_ptr(), best_offset=c_out[1].data_ptr(), best_k=c_out[2].data_ptr(),
-                        all_score=c_as.data_ptr(), all_offset=c_ao.data_ptr(), memspace=_native.B2_DEVICE)
+        ss._dispatch(pcm, pcm_off, tv, cs, ce, cue_off, None, refs, False,
+                     best_score=c_out[0].data_ptr(), best_offset=c_out[1].data_ptr(), best_k=c_out[2].data_ptr(),
+                     all_score=c_as.data_ptr(), all_offset=c_ao.data_ptr(), memspace=_native.B2_DEVICE)
         # the composition: detector / raster reference per video, then the public aligner steps
         fpw = h.frames_per_window(FRAME_RATE, SAMPLE_RATE)
         det_off = np.concatenate([[0], np.cumsum((np.diff(pcm_off) + fpw - 1) // fpw)]).astype(np.int64)
