@@ -856,7 +856,8 @@ struct SyncBufs {
 
 // rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
 // caller's stream, then the GSS rounds with the search
-static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1) {
+static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
+                         bool ref_packed) {
   const int K = r.K, t0 = p.trk_off[v0], nt = p.trk_off[v1] - t0;
   const size_t j0 = (size_t)t0 * K;
   std::vector<int> chain_trk(v1 - v0 + 1);
@@ -865,7 +866,7 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
     B2_TRY(b2i_raster_launch(h, r.cue_start_s, r.cue_end_s, r.cue_keep, r.cue_off + t0, nt, r.ratios, K, 0, nullptr,
                              r.sample_rate, r.start_seconds, b.subsig, p.sub_off.data() + j0));
   const B2CueSource src{r.cue_start_s, r.cue_end_s, r.cue_keep, r.cue_off + t0, r.ratios, r.sample_rate,
-                        r.start_seconds, p.ref_label, p.two_level};
+                        r.start_seconds, p.ref_label, p.two_level, ref_packed};
   B2_TRY(b2i_align_launch(h, b.refsig, p.ref_off.data() + v0, v1 - v0, chain_trk.data(), b.subsig,
                           p.sub_off.data() + j0, nt, K, r.max_offset_samples, b.score + j0, b.offset + j0,
                           b.status + j0, b.winner_only, b.fused ? &src : nullptr, (long long)j0));
@@ -891,10 +892,12 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // With subtitle references (b2_sync_tracks_subs) the step also rasterises those of the videos [v0, v1) into
 // their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
 // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
-static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1) {
+static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
+                  bool ref_packed) {
   if (!p.auditok) {
     B2_TRY(b2i_vad_launch(h, b.pcm, r.pcm_off + v0, v1 - v0, p.fpw, r.energy.non_speech_label,
-                          (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, p.ref_off.data() + v0));
+                          (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, p.ref_off.data() + v0,
+                          nullptr, ref_packed));
   } else {
     const ChunkTable& ch = p.ch;
     const int c0 = ch.first[v0], nc = ch.first[v1] - c0;
@@ -934,8 +937,8 @@ static int run_pipeline(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, cons
   const int n_sub = p.n_sub;
   const std::vector<int>& cut = p.cut;
   if (n_sub == 1) {
-    B2_TRY(detect(h, r, p, b, 0, r.V));
-    return enqueue_chain(h, r, p, b, 0, r.V);
+    B2_TRY(detect(h, r, p, b, 0, r.V, p.ref_packed[0]));
+    return enqueue_chain(h, r, p, b, 0, r.V, p.ref_packed[0]);
   }
   std::vector<cudaEvent_t> vad_done(n_sub);
   cudaEvent_t inputs_ready = next_event(h);
@@ -962,7 +965,7 @@ static int run_pipeline(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, cons
     for (int i = 0; i < n_sub; ++i) {
       h->vad_partition_sms = (i > 0 || prev_busy) ? p.vad_sms : 0;
       if (trace) B2_CUDA(h, cudaEventRecord(tev[1 + 4 * i], h->stream));
-      const int st = detect(h, r, p, b, cut[i], cut[i + 1]);
+      const int st = detect(h, r, p, b, cut[i], cut[i + 1], p.ref_packed[i]);
       h->vad_partition_sms = 0;
       if (st != B2_OK) return st;
       vad_done[i] = next_event(h);
@@ -975,7 +978,7 @@ static int run_pipeline(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, cons
     if (resident && i == n_sub - 1) B2_CUDA(h, cudaEventRecord(h->resident_fence, h->stream));
     B2_CUDA(h, cudaStreamWaitEvent(h->stream, vad_done[i], 0));
     if (trace) B2_CUDA(h, cudaEventRecord(tev[3 + 4 * i], h->stream));
-    B2_TRY(enqueue_chain(h, r, p, b, cut[i], cut[i + 1]));
+    B2_TRY(enqueue_chain(h, r, p, b, cut[i], cut[i + 1], p.ref_packed[i]));
     if (trace) B2_CUDA(h, cudaEventRecord(tev[4 + 4 * i], h->stream));
     host_ms[i + 1] = host_now();
   }
@@ -1004,8 +1007,14 @@ static int run_pipeline(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, cons
 
 static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   SyncPlan p;
-  const SyncPipeEnv env{h->sm_count, b2_ctx::kEvents - 2, getenv("B2_SUBBATCHES"), getenv("B2_VAD_SMS"),
-                        b2i_vad_lane_eligible};
+  SyncPipeEnv env{h->sm_count, b2_ctx::kEvents - 2, getenv("B2_SUBBATCHES"), getenv("B2_VAD_SMS"),
+                  b2i_vad_lane_eligible};
+  env.quirk_mask = h->log2_quirk_mask;
+  env.capture = h->capture.scores != nullptr;
+  env.align_path = getenv("B2_ALIGN_PATH");
+  env.fused = true;
+  if (const char* e = getenv("B2_FUSED_RASTER")) env.fused = atoi(e) != 0;
+  env.ref_packed = getenv("B2_REF_PACKED");
   if (const int st = plan_sync(r, env, &p)) {
     h->err = p.err;
     return st;
@@ -1033,8 +1042,7 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // read.  B2_FUSED_RASTER=0 (A/B and test knob): raster_cues_kernel writes float signals to HBM and
   // the generic aligner (the b2_align_batch path) reads them back.
   SyncBufs b{};
-  b.fused = true;
-  if (const char* e = getenv("B2_FUSED_RASTER")) b.fused = atoi(e) != 0;
+  b.fused = env.fused;
   const size_t J = (size_t)T * K, JG = (size_t)T * (K + 1);
   void *d_refsig, *d_subsig = nullptr, *d_res;
   // a chained resident call writes the buffer the previous call is not reading any more

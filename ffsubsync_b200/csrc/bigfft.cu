@@ -23,8 +23,8 @@
 #include "bigfft.cuh"
 #include "corr_jobs.cuh"
 
-int bigfft_min_log2n() { return bigfft::kMinQ1 + 11; }
-int bigfft_max_log2n() { return bigfft::kMaxQ1 + 11; }
+static_assert(kBigMinLog2n == bigfft::kMinQ1 + 11 && kBigMaxLog2n == bigfft::kMaxQ1 + 11,
+              "padded lengths of the large-window path");
 
 namespace {
 

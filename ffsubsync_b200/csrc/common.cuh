@@ -160,10 +160,14 @@ static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b;
 // e_min_full: smallest sum of squares of a full window that is speech.  tail_emin_host (nullable,
 // [B]): evaluate each signal's trailing partial window against its own floor (auditok contract);
 // null = partial windows are non-speech (webrtc contract).
+// packed (lane-per-window kernel only, B2_ERR_UNSUPPORTED otherwise): instead of the floats, the bits
+// m = (r == 1.0f) of every window, 32 to a word; signal b's words start at d_out + out_off_host[b] (read as
+// uint32), ceil(windows / 32) of them, with zero bits past its last window.
 bool b2i_vad_lane_eligible(const int64_t* pcm_off_host, int B, int fpw);
 int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off_host, int B, int fpw,
                    float non_speech_label, int64_t e_min_full, int z_lo, int z_hi,
-                   float* d_out, const int64_t* out_off_host, const int64_t* tail_emin_host = nullptr);
+                   float* d_out, const int64_t* out_off_host, const int64_t* tail_emin_host = nullptr,
+                   bool packed = false);
 struct B2TokenizerParams {
   double min_length, max_continuous_silence, non_speech_label;
   long long max_length;
@@ -208,6 +212,8 @@ struct B2CueSource {
   bool ref_two_level;        // every value is 1.0f or ref_label when this is set (the run path and the GSS rounds
                              // rely on it); the auditok signal is a clipped cumsum with other levels unless its label
                              // is 0, and subtitle and audio references mixed at a non-zero label have three levels
+  bool ref_packed = false;   // the detector wrote the reference as packed bits m = (r == 1.0f), one 32-bit word per
+                             // 32 frames from each video's ref_off on, and no floats (run-path chains only)
 };
 int b2i_raster_bits_launch(b2_ctx* h, const B2CueSource* src, int B, int K, const int64_t* sig_off,
                            const long long* bits_off, uint32_t* d_bits);

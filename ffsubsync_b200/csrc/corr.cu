@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <cmath>
 
+#include "align_path.h"
 #include "common.cuh"
 #include "corr.cuh"
 #include "corr_jobs.cuh"
@@ -29,6 +30,7 @@
 namespace {
 
 using namespace corr;
+static_assert(kP == kAlignBlock, "overlap-save block of the host planner");
 
 struct SpecItem {      // one reference block to transform
   long long ref_off;   // element offset of the pair's reference signal
@@ -444,6 +446,11 @@ __global__ void __launch_bounds__(256) nominate_select_kernel(const SelJob* __re
 // overlap is cut into kRescoreSeg segments handled by different CTAs (persistent grid over the
 // work list); every partial sum has a fixed summation order and pick_kernel adds the partials in
 // segment order, so the result is deterministic.
+// PACKED_REF (run-path chains whose detector wrote packed bits): `ref` holds, from job.ref_off on, the words of
+// the reference's bits m = (r == 1.0f); frame value r = m ? 1.0f : ref_label is rebuilt as a float, so every
+// product and the summation order are those of the float reference, and the sums are bit-identical.  The float
+// variant (every other chain) reads the float signal and never its last argument.
+template <bool PACKED_REF>
 __global__ void __launch_bounds__(256) rescore_kernel(const SelJob* __restrict__ jobs,
                                                        const float* __restrict__ ref,
                                                        const float* __restrict__ sub,
@@ -451,7 +458,7 @@ __global__ void __launch_bounds__(256) rescore_kernel(const SelJob* __restrict__
                                                        const int* __restrict__ work_list,
                                                        const int* __restrict__ work_count,
                                                        const uint32_t* __restrict__ sub_bits,
-                                                       double* __restrict__ cand_partial) {
+                                                       double* __restrict__ cand_partial, float ref_label) {
   __shared__ double sh[256];
   const int total = *work_count * kRescoreSeg;
   for (int w = blockIdx.x; w < total; w += gridDim.x) {
@@ -467,7 +474,31 @@ __global__ void __launch_bounds__(256) rescore_kernel(const SelJob* __restrict__
     const int a0 = j_lo + seg * per, a1 = min(j_hi, a0 + per);
     double acc = 0.0;
     int i = a0 + threadIdx.x;
-    if (job.bits_off >= 0) {
+    if (PACKED_REF) {
+      // both signals as bits (cue mode): reference frame i + o >= 0 is bit (i + o) & 31 of its word, the same
+      // bit position for all u as for the mask
+      const uint32_t* bits = sub_bits + job.bits_off;
+      const uint32_t* rbits = reinterpret_cast<const uint32_t*>(ref) + job.ref_off;
+      const double hi = 2.0 * (double)job.sub_level - 1.0;
+      const int rsh = (i + o) & 31;
+      for (; i + 7 * 256 < a1; i += 8 * 256) {  // 16 independent loads in flight per thread
+        uint32_t bw[8];
+        float rv[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          bw[u] = __ldg(bits + ((i + u * 256) >> 5));
+          rv[u] = ((__ldg(rbits + ((i + u * 256 + o) >> 5)) >> rsh) & 1u) ? 1.0f : ref_label;
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u)
+          acc = fma(((bw[u] >> (i & 31)) & 1u) ? hi : -1.0, 2.0 * (double)rv[u] - 1.0, acc);
+      }
+      for (; i < a1; i += 256) {
+        const double a = ((__ldg(bits + (i >> 5)) >> (i & 31)) & 1u) ? hi : -1.0;
+        const float rv = ((__ldg(rbits + ((i + o) >> 5)) >> rsh) & 1u) ? 1.0f : ref_label;
+        acc = fma(a, 2.0 * (double)rv - 1.0, acc);
+      }
+    } else if (job.bits_off >= 0) {
       // bit-mask mode: subtitle frame i is bit i of the mask written by raster_bits_kernel;
       // its value after x -> 2x-1 is (2*level - 1) inside a cue and -1 outside
       const uint32_t* bits = sub_bits + job.bits_off;
@@ -642,81 +673,24 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   // cue mode (b2_sync_batch): the subtitle signals exist only as bit masks, rasterised from the cue
   // list by raster_bits_kernel below (sub_off then only carries the signal lengths)
   const bool cue_mode = cue_src != nullptr;
-  std::vector<long long> bits_off(cue_mode ? J + 1 : 1, 0);
-  if (cue_mode)
-    for (size_t j = 0; j < J; ++j)
-      bits_off[j + 1] = bits_off[j] + ((sub_off[j + 1] - sub_off[j]) + kP) / 32 + 1;
-  std::vector<SelJob> sel(J);
-  std::vector<long long> idx_lo(J, 0), idx_hi(J, 0), n_pad(J, 0);
-  // one plan per reference (video): its window covers the live jobs of all its tracks, whose K ratio jobs
-  // are [trk_off[v] * K, trk_off[v + 1] * K)
-  struct PairPlan { long long o_min, o_max; int n_tiles; bool any; };
-  std::vector<PairPlan> pp(V);
-  long long max_w = 1;
-  bool big_ok = true;   // every live job's padded length suits the large-window path
-  const long long mo_clamped =
-      std::max<long long>(-(1LL << 40), std::min<long long>(1LL << 40, max_offset_samples));
-  for (int v = 0; v < V; ++v) {
-    const long long R = ref_off[v + 1] - ref_off[v];
-    if (R < 0 || R > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad reference length at %d", v);
-    PairPlan& p = pp[v];
-    p.any = false;
-    p.o_min = 0;
-    p.o_max = -1;
-    for (int b = trk_off[v]; b < trk_off[v + 1]; ++b) {
-      long long t_min = 0, t_max = -1;   // window of this track's K jobs (winner-only pruning is per track)
-      bool t_any = false;
-      for (int k = 0; k < K; ++k) {
-        const size_t j = (size_t)b * K + k;
-        const long long S = sub_off[j + 1] - sub_off[j];
-        if (S < 0 || S > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "align: bad subtitle length at %zu", j);
-        SelJob& s = sel[j];
-        memset(&s, 0, sizeof(s));
-        s.ref_off = ref_off[v];
-        s.sub_off = sub_off[j];
-        s.R = (int)R;
-        s.S = (int)S;
-        s.out_index = (int)j;
-        s.bits_off = cue_mode ? bits_off[j] : -1;
-        s.sub_level = cue_mode ? (float)std::min(1.0 / cue_src->ratios[k], 1.0) : 0.f;  // speech_transformers.py:977
-        // aligners.py:31-66: empty input, padded length, surviving index range (job_plan.cuh)
-        const B2JobPlan jp = b2_plan_job(R, S, max_offset_samples, h->log2_quirk_mask);
-        if (jp.kind != 0) {
-          s.kind = jp.kind;
-          s.masked_offset = jp.masked_offset;
-          continue;
-        }
-        const long long N = jp.N, o_lo = jp.o_lo, o_hi = jp.o_hi;
-        idx_lo[j] = jp.lo;
-        idx_hi[j] = jp.hi;
-        n_pad[j] = N;
-        if (N < (1LL << (bigfft_min_log2n())) || N > (1LL << bigfft_max_log2n())) big_ok = false;
-        s.kind = 0;
-        s.m_lo = (int)o_lo;  // temporarily absolute offsets; rebased below
-        s.m_hi = (int)o_hi;
-        t_min = t_any ? std::min(t_min, o_lo) : o_lo;
-        t_max = t_any ? std::max(t_max, o_hi) : o_hi;
-        t_any = true;
-      }
-      if (!t_any) continue;
-      p.o_min = p.any ? std::min(p.o_min, t_min) : t_min;
-      p.o_max = p.any ? std::max(p.o_max, t_max) : t_max;
-      p.any = true;
-      if (max_offset_samples != B2_MAX_OFFSET_NONE && std::max(llabs(t_min), llabs(t_max)) > mo_clamped)
-        for (int k = 0; k < K; ++k) sel[(size_t)b * K + k].no_prune = 1;
-    }
-    if (p.any) max_w = std::max(max_w, p.o_max - p.o_min + 1);
+  // the jobs, windows and tiling (align_path.h: the sync calls' planner runs the same code)
+  B2AlignJobs aj;
+  if (const int st = b2_plan_align_jobs(ref_off, V, trk_off, sub_off, B, K, max_offset_samples, h->log2_quirk_mask,
+                                        cue_mode ? cue_src->ratios : nullptr, &aj)) {
+    h->err = aj.err;
+    return st;
   }
+  std::vector<SelJob>& sel = aj.sel;
+  const std::vector<long long>& bits_off = aj.bits_off;
+  std::vector<B2AlignPairPlan>& pp = aj.pp;
+  const long long max_w = aj.max_w;
   const bool capture = h->capture.scores != nullptr;
   if (capture)
     for (size_t j = 0; j < J; ++j)
       if (sel[j].kind == 0 && (long long)sel[j].m_hi - sel[j].m_lo + 1 > h->capture.stride)
         B2_FAIL(h, B2_ERR_BAD_ARG, "capture: job %lld has %lld surviving offsets, stride %lld",
                 capture_j0 + (long long)j, (long long)sel[j].m_hi - sel[j].m_lo + 1, h->capture.stride);
-  // offsets per tile: Wt = 1 (mod 32) so that L = P - Wt + 1 is a multiple of 32 (vector loads,
-  // whole words of the speech bit mask per block), at most P/2 + 1
-  const int Wt = (int)(max_w <= kP / 2 + 1 ? 32 * ((max_w + 30) / 32) + 1 : (kP / 2 + 1));
-  const int L = kP - Wt + 1;
+  const int Wt = aj.Wt, L = aj.L;
   uint32_t* d_bits = nullptr;
   if (cue_mode) {
     void* db;
@@ -737,55 +711,26 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   cb.work_count = cb.work_list + J * kCandMax;
   if (J >= (1u << 26)) B2_FAIL(h, B2_ERR_UNSUPPORTED, "align: B*K too large for one call");
 
-  // Large windows (FFTAligner's default max_offset_samples=None, or a mask wider than a few tiles):
-  // the overlap-save path would recompute every block for every 16 385-offset tile; one padded-length
-  // FFT per signal (four-step, bigfft.cu) is cheaper from kBigMinTiles tiles on.
-  // B2_ALIGN_PATH=tiled|big|runs: test / A-B knob.
-  bool use_big = big_ok && max_w > (long long)kBigMinTiles * (kP / 2 + 1);
-  const char* path_env = getenv("B2_ALIGN_PATH");
-  const bool force_runs = path_env && !strcmp(path_env, "runs");
-  if (path_env) {
-    if (!strcmp(path_env, "tiled") || force_runs) use_big = false;
-    if (!strcmp(path_env, "big") && big_ok) use_big = true;
+  // the path (align_path.h); B2_ALIGN_PATH=tiled|big|runs: test / A-B knob
+  const B2AlignPathChoice path =
+      b2_align_path(aj, trk_off, V, K, cue_mode ? cue_src->cue_off : nullptr, cue_mode && cue_src->ref_two_level,
+                    cue_mode ? cue_src->ref_label : 0.0f, getenv("B2_ALIGN_PATH"), capture);
+  // a packed reference (the detector wrote bits, no floats) is planned for run-path chains only
+  const bool ref_packed = cue_mode && cue_src->ref_packed;
+  if (ref_packed && path.path != B2_PATH_RUNS)
+    B2_FAIL(h, B2_ERR_UNSUPPORTED, "align: internal error: packed reference on a chain that takes the %s path",
+            path.path == B2_PATH_BIG ? "large-window" : "tiled");
+  if (path.path == B2_PATH_RUNS) {
+    const SelJob* d_sel_runs = nullptr;
+    B2_TRY(b2i_align_runs(h, d_ref, ref_off, V, trk_off, K, sel, d_bits, path.max_runs, cue_src->ref_label,
+                          winner_only, ref_packed, cb, &d_sel_runs, capture_j0));
+    return b2i_rescore_pick(h, d_sel_runs, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status, ref_packed,
+                            cue_src->ref_label);
   }
-  // Cue mode with the reference from this call's VAD (two levels, 1.0f and the label): the run path
-  // (runcorr.cu) scores every offset of the window from the cue runs, exactly up to a float64 margin, when
-  // its work (cues x window) is below the FFT blocks it replaces for every live job.  A capture of the
-  // nominations (b2_capture_nominations) probes the FFT paths and keeps them, unless B2_ALIGN_PATH=runs asks
-  // for the run path (then its float64 scores are captured).  A reference with further levels (auditok at a
-  // non-zero label) stays on the FFT paths, which read its values as they are, even under B2_ALIGN_PATH=runs.
-  if (cue_mode && (!capture || force_runs) && !use_big && cue_src->ref_two_level && std::isfinite(cue_src->ref_label) &&
-      !(path_env && !strcmp(path_env, "tiled"))) {
-    bool fits = true, pays = true;
-    int max_runs = 1;
-    for (int v = 0; v < V && fits; ++v) {
-      const long long n_tiles_v = pp[v].any ? ceil_div64(pp[v].o_max - pp[v].o_min + 1, Wt) : 0;
-      for (int b = trk_off[v]; b < trk_off[v + 1]; ++b) {
-        const long long cues = cue_src->cue_off[b + 1] - cue_src->cue_off[b];  // runs of a mask <= its cues
-        for (int k = 0; k < K; ++k) {
-          const SelJob& s = sel[(size_t)b * K + k];
-          if (s.kind != 0) continue;
-          const long long w = (long long)s.m_hi - s.m_lo + 1;
-          if (w > kRunMaxWindow || cues > kRunMaxCues || llabs((long long)s.m_lo) > (1LL << 30) ||
-              llabs((long long)s.m_hi) > (1LL << 30))
-            fits = false;
-          if ((double)cues * (double)w > kRunCostPerBlock * (double)(n_tiles_v * (ceil_div64(s.S, L) + 1)))
-            pays = false;
-          max_runs = std::max<int>(max_runs, (int)std::min<long long>(cues, kRunMaxCues));
-        }
-      }
-    }
-    if (fits && (pays || force_runs)) {
-      const SelJob* d_sel_runs = nullptr;
-      B2_TRY(b2i_align_runs(h, d_ref, ref_off, V, trk_off, K, sel, d_bits, max_runs, cue_src->ref_label, winner_only,
-                            cb, &d_sel_runs, capture_j0));
-      return b2i_rescore_pick(h, d_sel_runs, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
-    }
-  }
-  if (use_big) {
+  if (path.path == B2_PATH_BIG) {
     const SelJob* d_sel_big = nullptr;
-    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, V, trk_off, K, sel, idx_lo, idx_hi, n_pad, winner_only, cb,
-                         &d_sel_big, capture_j0));
+    B2_TRY(b2i_align_big(h, d_ref, d_sub, d_bits, V, trk_off, K, sel, aj.idx_lo, aj.idx_hi, aj.n_pad, winner_only,
+                         cb, &d_sel_big, capture_j0));
     return b2i_rescore_pick(h, d_sel_big, J, d_ref, d_sub, d_bits, cb, d_score, d_offset, d_status);
   }
 
@@ -797,7 +742,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   // fixed order.  Costs one extra inverse transform per chunk, so chunks keep >= 4 blocks.
   long long n_jobs_total = 0, max_blocks = 1;
   for (int v = 0; v < V; ++v) {
-    PairPlan& p = pp[v];
+    B2AlignPairPlan& p = pp[v];
     p.n_tiles = p.any ? (int)ceil_div64(p.o_max - p.o_min + 1, Wt) : 0;
     for (size_t j = (size_t)trk_off[v] * K; j < (size_t)trk_off[v + 1] * K; ++j) {
       const SelJob& s = sel[j];
@@ -813,7 +758,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
   if (const char* e = getenv("B2_ALIGN_SPLIT")) n_split = std::max(1, atoi(e));  // test / tuning knob
   long long score_total = 0, energy_total = 0, max_score_len = 0;
   for (int v = 0; v < V; ++v) {
-    PairPlan& p = pp[v];
+    B2AlignPairPlan& p = pp[v];
     for (size_t j = (size_t)trk_off[v] * K; j < (size_t)trk_off[v + 1] * K; ++j) {
       SelJob& s = sel[j];
       if (s.kind != 0) continue;
@@ -883,7 +828,7 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
 
   // the reference blocks of a (video, tile) are transformed once and read by every track and ratio of the video
   for (int v = 0; v < V; ++v) {
-    const PairPlan& p = pp[v];
+    const B2AlignPairPlan& p = pp[v];
     if (!p.any) continue;
     const long long R = ref_off[v + 1] - ref_off[v];
     const size_t j_lo = (size_t)trk_off[v] * K, j_hi = (size_t)trk_off[v + 1] * K;
@@ -951,9 +896,10 @@ int b2i_align_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int 
 
 int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_ref, const float* d_sub,
                      const uint32_t* d_bits, const B2CandBuffers& cb, double* d_score, int32_t* d_offset,
-                     int32_t* d_status) {
-  rescore_kernel<<<(unsigned)(h->sm_count * 8), 256, 0, h->stream>>>(
-      d_sel, d_ref, d_sub, cb.cand_off, cb.work_list, cb.work_count, d_bits, cb.cand_partial);
+                     int32_t* d_status, bool ref_packed, float ref_label) {
+  auto rescore = ref_packed ? rescore_kernel<true> : rescore_kernel<false>;
+  rescore<<<(unsigned)(h->sm_count * 8), 256, 0, h->stream>>>(
+      d_sel, d_ref, d_sub, cb.cand_off, cb.work_list, cb.work_count, d_bits, cb.cand_partial, ref_label);
   B2_CHECK_LAUNCH(h, "rescore_kernel");
   pick_kernel<<<(unsigned)((J + 127) / 128), 128, 0, h->stream>>>(d_sel, (int)J, cb.cand_off, cb.cand_cnt,
                                                                    cb.cand_partial, cb.job_stat, d_score,

@@ -60,8 +60,7 @@ struct SelJob {        // one (pair, ratio)
 
 // The large-window path takes over from kBigMinTiles overlap-save tiles on; padded lengths it handles.
 constexpr int kBigMinTiles = 4;
-int bigfft_min_log2n();
-int bigfft_max_log2n();
+constexpr int kBigMinLog2n = 17, kBigMaxLog2n = 23;
 
 // Common tail (corr.cu): candidate selection, exact float64 re-score of the nominated candidates and
 // the argmax.  job_stat is filled by either path (window_max_kernel, big_stat_kernel); cand_off /
@@ -80,9 +79,11 @@ struct B2CandBuffers {
 // winner_only: a ratio that cannot be its pair's best keeps only its fp32 argmax (B2_ALIGN_APPROX).
 int b2i_select_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n, const float* scores,
                       int n_chunks, int K, int winner_only, int* chunk_cnt, const B2CandBuffers& cb);
+// ref_packed: d_ref holds each reference's bits m = (r == 1.0f) as words from its ref_off on (the detector's
+// packed output, run-path chains only); the re-score reads r = m ? 1.0f : ref_label.
 int b2i_rescore_pick(b2_ctx* h, const SelJob* d_sel, size_t J, const float* d_ref, const float* d_sub,
                      const uint32_t* d_bits, const B2CandBuffers& cb, double* d_score, int32_t* d_offset,
-                     int32_t* d_status);
+                     int32_t* d_status, bool ref_packed = false, float ref_label = 0.0f);
 // b2_capture_nominations (corr.cu): copies the window scores, job_stat and cand_cnt of n jobs into
 // h->capture at global index j0 + j, after the selection kernels.  Jobs d_jlist[0..n) (NULL: 0..n-1);
 // with scores == NULL only the jobs without a live window are written, unless scores_written (the run
@@ -94,9 +95,11 @@ int b2i_capture_launch(b2_ctx* h, const SelJob* d_sel, const int* d_jlist, int n
 // subtitle bit masks in d_bits, at most max_runs cue runs per job.  Fills cand_off / cand_cnt / job_stat /
 // work_list / work_count like the selection; the caller then runs b2i_rescore_pick on *d_sel_out.  Under a
 // capture the float64 scores (rounded to float32), job_stat and cand_cnt go to it at global index capture_j0 + j.
+// ref_packed: d_ref holds packed reference bits (see b2i_rescore_pick), which a scan turns into the run path's
+// reference table; otherwise ref_bits_kernel packs the float reference.
 int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
                    std::vector<SelJob>& sel, const uint32_t* d_bits, int max_runs, float ref_label, int winner_only,
-                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0);
+                   bool ref_packed, const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0);
 // The run path is chosen per call when every live job has cues x window <= kRunCostPerBlock x (its FFT block
 // transforms): the break-even measured in the bench step on an H100 (DESIGN.md section 4, "K4r").
 // kRunMaxCues bounds the shared memory of a job's run table (3 ints per run).

@@ -18,7 +18,7 @@ using namespace runcorr;
 static_assert(kMaxWindow == kRunMaxWindow, "run path window bound");
 
 struct RunRef {        // one video's reference
-  long long ref_off;   // element offset of its float signal
+  long long ref_off;   // element offset of its float signal (packed: word offset of its bits)
   long long q_off;     // entry offset of its packed bits (rc_ref_entries(R) entries)
   int R;
 };
@@ -93,6 +93,43 @@ __global__ void __launch_bounds__(1024) ref_bits_kernel(const float* __restrict_
     if (w < n_words) q[w + 1] = make_uint2(mine, (uint32_t)(carry + ex));
     carry += tot;
   }
+}
+
+// The same table from a reference the detector wrote as packed bits (words 0 .. (R + 31) / 32 - 1 from
+// v.ref_off on, zero past frame R - 1): one coalesced word per thread and a scan of their counts.
+__global__ void __launch_bounds__(1024) ref_words_scan_kernel(const uint32_t* __restrict__ ref_words,
+                                                              const RunRef* __restrict__ vids,
+                                                              uint2* __restrict__ q_all) {
+  __shared__ int sh[33];
+  const RunRef v = vids[blockIdx.x];
+  const uint32_t* r = ref_words + v.ref_off;
+  uint2* q = q_all + v.q_off;
+  const int n_in = (v.R + 31) >> 5;    // words the detector wrote
+  const int n_words = (v.R >> 5) + 2;  // words 0 .. (R >> 5) + 1
+  if (threadIdx.x == 0) q[0] = make_uint2(0u, 0u);
+  int carry = 0;
+  for (int w0 = 0; w0 < n_words; w0 += blockDim.x) {
+    const int w = w0 + threadIdx.x;
+    const uint32_t mine = w < n_in ? __ldg(r + w) : 0u;
+    int tot;
+    const int ex = block_excl_scan(__popc(mine), sh, &tot);
+    if (w < n_words) q[w + 1] = make_uint2(mine, (uint32_t)(carry + ex));
+    carry += tot;
+  }
+}
+
+// The run path's reference table of every video in vids: from the float reference, or the packed bits
+int launch_ref_table(b2_ctx* h, const float* d_ref, bool ref_packed, const RunRef* d_vids, size_t n_vids, uint2* q) {
+  if (n_vids == 0) return B2_OK;
+  if (ref_packed) {
+    ref_words_scan_kernel<<<(unsigned)n_vids, 1024, 0, h->stream>>>(reinterpret_cast<const uint32_t*>(d_ref), d_vids,
+                                                                    q);
+    B2_CHECK_LAUNCH(h, "ref_words_scan_kernel");
+  } else {
+    ref_bits_kernel<<<(unsigned)n_vids, 1024, 0, h->stream>>>(d_ref, d_vids, q);
+    B2_CHECK_LAUNCH(h, "ref_bits_kernel");
+  }
+  return B2_OK;
 }
 
 // One CTA per (track, ratio) job: blockDim.x / 32 >= ceil(window / 32) threads, thread t owning the offsets
@@ -273,8 +310,8 @@ __global__ void __launch_bounds__(128) run_finalize_kernel(const SelJob* __restr
 
 int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V, const int* trk_off, int K,
                    std::vector<SelJob>& sel, const uint32_t* d_bits, int max_runs, float ref_label, int winner_only,
-                   const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0) {
-  B2Range range("b2:align runs (ref_bits, run_corr, finalize)");
+                   bool ref_packed, const B2CandBuffers& cb, const SelJob** d_sel_out, long long capture_j0) {
+  B2Range range("b2:align runs (ref_bits or ref_words_scan, run_corr, finalize)");
   const size_t J = sel.size();
   std::vector<RunRef> vids;
   std::vector<long long> job_q(J, 0);
@@ -312,10 +349,7 @@ int b2i_align_runs(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
   const RunRef* d_vids = vids.empty() ? nullptr : (const RunRef*)b2i_meta_put(&a, vids.data(), vids.size() * sizeof(RunRef));
   B2_TRY(b2i_meta_commit(&a));
   *d_sel_out = d_sel;
-  if (!vids.empty()) {
-    ref_bits_kernel<<<(unsigned)vids.size(), 1024, 0, h->stream>>>(d_ref, d_vids, q);
-    B2_CHECK_LAUNCH(h, "ref_bits_kernel");
-  }
+  B2_TRY(launch_ref_table(h, d_ref, ref_packed, d_vids, vids.size(), q));
   max_runs = std::max(1, max_runs);
   const size_t smem = (size_t)3 * max_runs * sizeof(int);
   const bool capture = h->capture.scores != nullptr;
@@ -427,8 +461,7 @@ int b2i_gss_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
   const RunRef* d_vids = (const RunRef*)b2i_meta_put(&a, vids.data(), vids.size() * sizeof(RunRef));
   B2_TRY(b2i_meta_commit(&a));
 
-  ref_bits_kernel<<<(unsigned)vids.size(), 1024, 0, h->stream>>>(d_ref, d_vids, q);
-  B2_CHECK_LAUNCH(h, "ref_bits_kernel");
+  B2_TRY(launch_ref_table(h, d_ref, src.ref_packed, d_vids, vids.size(), q));
   const size_t smem = (size_t)3 * max_runs * sizeof(int);
   B2_CUDA(h, cudaFuncSetAttribute(run_corr_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   for (int r = 0; r < kGssEvals; ++r) {
@@ -441,7 +474,8 @@ int b2i_gss_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off, int V,
     B2_CUDA(h, cudaMemsetAsync(cb.work_count, 0, sizeof(int), h->stream));
     run_finalize_kernel<<<(unsigned)((T + 127) / 128), 128, 0, h->stream>>>(d_sel, T, 1, /*winner_only=*/0, stat, cb);
     B2_CHECK_LAUNCH(h, "run_finalize_kernel");
-    B2_TRY(b2i_rescore_pick(h, d_sel, (size_t)T, d_ref, nullptr, d_bits, cb, r_score, r_offset, r_status));
+    B2_TRY(b2i_rescore_pick(h, d_sel, (size_t)T, d_ref, nullptr, d_bits, cb, r_score, r_offset, r_status,
+                            src.ref_packed, src.ref_label));
   }
   return b2i_gss_combine_launch(h, T, K, d_trk, d_x, r_score, r_offset, max_offset_samples, out);
 }

@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "align_path.h"    // b2_plan_align_jobs, b2_align_path
 #include "common.cuh"      // B2_FAIL, B2TokenizerParams
 #include "corr_jobs.cuh"   // kRunMaxCues, kRunMaxWindow
 #include "job_plan.cuh"    // B2_GSS_HI, b2_signal_length, B2_MAX_CUE_SECONDS
@@ -297,11 +298,19 @@ struct SyncRequest {
 // What plan_sync reads from the handle and the environment: the SM count, the most sub-batches the handle's
 // event pool orders, B2_SUBBATCHES / B2_VAD_SMS (null: unset) and the energy kernel's lane-per-window
 // eligibility test (b2i_vad_lane_eligible).
+// For the reference format (plan_ref_format) also what the aligner's path choice reads (align_path.h): the
+// handle's log2 quirk mask and capture state, B2_ALIGN_PATH, whether the subtitle signals are bit masks
+// (B2_FUSED_RASTER), and B2_REF_PACKED ("0": every reference as floats).
 struct SyncPipeEnv {
   int sm_count, max_sub;
   const char* subbatches;
   const char* vad_sms;
   bool (*lane_eligible)(const int64_t* pcm_off, int n, int fpw);
+  uint64_t quirk_mask = 0;
+  bool capture = false;
+  const char* align_path = nullptr;
+  bool fused = true;
+  const char* ref_packed = nullptr;
 };
 
 struct SyncPlan {
@@ -323,6 +332,8 @@ struct SyncPlan {
   // Sub-batches of the pipeline: videos cut[i] .. cut[i+1]-1; the later ones' detector runs on vad_sms SMs
   int n_sub = 1, vad_sms = 0;
   std::vector<int> cut;
+  // per sub-batch: its detector writes the reference as packed bits instead of floats (plan_ref_format)
+  std::vector<uint8_t> ref_packed;
 };
 
 // Sub-batches are cut at video boundaries (a video's tracks run in the chain behind its own VAD) and balanced by
@@ -356,6 +367,34 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
   }
   p->cut.push_back(V);
   p->n_sub = (int)p->cut.size() - 1;
+}
+
+// The reference format of each sub-batch.  The run path reads a reference only as its bits m = (r == 1.0f) (and
+// r = m ? 1.0f : ref_label in the exact re-score), so a sub-batch whose detector is the lane-per-window energy
+// kernel, with no subtitle reference, whose chain takes the run path has its VAD write those bits, 32 to a word,
+// instead of the floats: 1/32 of the bytes written, and the chain reads bits instead of floats.  The chain's path
+// is decided here by the aligner's own functions on the chain's own inputs (align_path.h, as enqueue_chain passes
+// them), so the launcher reaches the same choice.  auditok, subtitle references, the lane-group kernel and the
+// FFT paths keep the float reference.  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
+static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
+  p->ref_packed.assign(p->n_sub, 0);
+  if (p->auditok || !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0)) return;
+  for (int i = 0; i < p->n_sub; ++i) {
+    const int v0 = p->cut[i], v1 = p->cut[i + 1];
+    const auto& sv = p->sub_video;
+    if (std::lower_bound(sv.begin(), sv.end(), v0) != std::lower_bound(sv.begin(), sv.end(), v1)) continue;
+    if (!env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw)) continue;
+    const int t0 = p->trk_off[v0], nt = p->trk_off[v1] - t0;
+    std::vector<int> chain_trk(v1 - v0 + 1);
+    for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = p->trk_off[v] - t0;
+    B2AlignJobs aj;   // a chain the aligner rejects keeps the floats (and fails there with its message)
+    if (b2_plan_align_jobs(p->ref_off.data() + v0, v1 - v0, chain_trk.data(), p->sub_off.data() + (size_t)t0 * r.K,
+                           nt, r.K, r.max_offset_samples, env.quirk_mask, r.ratios, &aj) != B2_OK)
+      continue;
+    const B2AlignPathChoice c = b2_align_path(aj, chain_trk.data(), v1 - v0, r.K, r.cue_off + t0, p->two_level,
+                                              p->ref_label, env.align_path, env.capture);
+    p->ref_packed[i] = c.path == B2_PATH_RUNS;
+  }
 }
 
 // Checks of the subtitle references, before anything reads their tables.
@@ -518,5 +557,6 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
         p->max_end[t] = c == r.cue_off[t] ? r.cue_end_s[c] : std::max(p->max_end[t], r.cue_end_s[c]);
   }
   plan_cuts(r, env, p);
+  plan_ref_format(r, env, p);
   return B2_OK;
 }

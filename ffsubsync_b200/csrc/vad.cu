@@ -58,6 +58,9 @@ struct VadParams {
   // samples it has, speech <=> sum x^2 >= tail_emin[b] (no zero-crossing band).  nullptr: the
   // webrtc contract - a partial window is non-speech.
   const long long* tail_emin;
+  // lane-per-window kernel, packed output (b2i_vad_launch): the window bits m = (r == 1.0f) as words, signal b's
+  // from bits + out_off[b] on; tiles then carry word offsets in out_base.  nullptr: float output to out.
+  uint32_t* bits;
   int B, fpw, G, tw, z_lo, z_hi, fast, stage_bytes, cpl, stages, consumers, batch, evict_first;
   float label;
 };
@@ -350,7 +353,7 @@ __device__ __forceinline__ TileDesc make_tile_cached(const VadParams& p, long lo
   const long long w0 = (t - c.tile_lo) * p.tw;
   const long long s0 = c.sig0 + w0 * p.fpw;
   d.sig = c.b;
-  d.out_base = c.out0 + w0;
+  d.out_base = c.out0 + (p.bits ? w0 >> 5 : w0);   // tiles start at multiples of 32 windows
   d.n_left = c.sig1 - s0;
   d.seq = 0;
   if (t + 1 < c.tile_hi) {
@@ -520,7 +523,14 @@ __global__ void __launch_bounds__(kLaneConsumers + 32 * kLanePipes) vad_lane_ker
         for (int i = 0; i < (int)avail; ++i) e += (long long)xs[i] * xs[i];
         speech = e >= p.tail_emin[d.sig];
       }
-      if (active) p.out[d.out_base + wl] = speech ? 1.0f : p.label;
+      if (p.bits) {
+        // packed: iteration k is word k of the tile (32 consecutive windows); m = (r == 1.0f) of the float below,
+        // 0 past the last window.  A word wholly past it is not the signal's.
+        const uint32_t m = __ballot_sync(0xffffffffu, active && (speech || p.label == 1.0f));
+        if (lane == 0 && 32 * k < d.n_windows) p.bits[d.out_base + k] = m;
+      } else if (active) {
+        p.out[d.out_base + wl] = speech ? 1.0f : p.label;
+      }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[stage]);
@@ -589,7 +599,7 @@ bool b2i_vad_lane_eligible(const int64_t* pcm_off, int B, int fpw) {
 
 int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int B, int fpw,
                    float non_speech_label, int64_t e_min_full, int z_lo, int z_hi,
-                   float* d_out, const int64_t* out_off, const int64_t* tail_emin) {
+                   float* d_out, const int64_t* out_off, const int64_t* tail_emin, bool packed) {
   B2Range range("b2:vad_energy_zcr");
   if (((uintptr_t)d_pcm & 15) != 0)
     B2_FAIL(h, B2_ERR_BAD_ARG, "vad: device PCM pointer must be 16-byte aligned");
@@ -678,6 +688,9 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
       tile_off[b + 1] = tile_off[b] + ((n + fpw - 1) / fpw + p.tw - 1) / p.tw;
     }
   }
+  if (packed && !lane_layout)
+    B2_FAIL(h, B2_ERR_UNSUPPORTED, "vad: internal error: packed output asked of the lane-group kernel");
+  p.bits = packed ? reinterpret_cast<uint32_t*>(d_out) : nullptr;
   p.total_tiles = tile_off[B];
   if (p.total_tiles == 0) return B2_OK;
 
