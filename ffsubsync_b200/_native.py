@@ -29,7 +29,8 @@ EXPORTS = [
     "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
-    "b2_sync_tracks_auditok", "b2_sync_tracks_subs",
+    "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
+    "b2_sync_tracks_pgs",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
@@ -102,6 +103,13 @@ def load() -> ctypes.CDLL:
                                             ctypes.c_int, _f64, _i64, ctypes.c_int, ctypes.c_int, _f64, _f64, _i64,
                                             _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int,
                                             _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_rasterize_pgs_lengths.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
+        lib.b2_rasterize_pgs.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _f64, _vp, _vp, ctypes.c_int]
+        lib.b2_sync_tracks_pgs.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_int, _f64, _i64, ctypes.c_int, ctypes.c_int, _f64, _f64, _i64,
+                                           _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                           _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                           ctypes.c_int]
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -322,6 +330,35 @@ class Handle:
         self._check(st, "b2_rasterize")
         return out, out_off
 
+    def rasterize_pgs_lengths(self, end_s, off, sample_rate: int) -> np.ndarray:
+        """Signal lengths int(max_end * sample_rate) + 2 of B PGS interval lists (b2_rasterize_pgs_lengths)."""
+        end_s = np.ascontiguousarray(end_s, dtype=np.float64)
+        off = _i64a(off)
+        B = len(off) - 1
+        lengths = np.empty(B, dtype=np.int64)
+        st = self.lib.b2_rasterize_pgs_lengths(_ptr(end_s), _ptr(off), B, int(sample_rate), _ptr(lengths))
+        if st != 0:
+            raise NativeError(st, "b2_rasterize_pgs_lengths")
+        return lengths
+
+    def rasterize_pgs(self, start_s, end_s, off, sample_rate: int, start_seconds: float, out=None, out_off=None,
+                      memspace: int = B2_HOST):
+        """PGSSpeechTransformer.fit's signal of B interval lists (b2_rasterize_pgs): list b is
+        start_s / end_s[off[b] .. off[b+1]].  Returns (float32 signals back to back, out_off int64[B+1])."""
+        start_s = np.ascontiguousarray(start_s, dtype=np.float64)
+        end_s = np.ascontiguousarray(end_s, dtype=np.float64)
+        off = _i64a(off)
+        B = len(off) - 1
+        if out_off is None:
+            out_off = np.concatenate([[0], np.cumsum(self.rasterize_pgs_lengths(end_s, off, sample_rate))])
+        out_off = _i64a(out_off)
+        if memspace == B2_HOST:
+            out = np.empty(int(out_off[-1]), dtype=np.float32)
+        st = self.lib.b2_rasterize_pgs(self.h, _ptr(start_s), _ptr(end_s), _ptr(off), B, int(sample_rate),
+                                       float(start_seconds), _ptr(out), _ptr(out_off), memspace)
+        self._check(st, "b2_rasterize_pgs")
+        return out, out_off
+
     def blend_signals(self, a, b, mode: int, wa: float = 0.6, wb: float = 0.4, out=None, n=None,
                       memspace: int = B2_HOST):
         """mode 0 = min, 1 = max, 2 = wa*a + wb*b; host arrays are clipped to their common length."""
@@ -521,6 +558,49 @@ class Handle:
                            _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
                            _ptr(ref_cue_off)), cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds,
                           max_offset_samples,
+                          (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
+                          memspace, gss=bool(gss), want_evals=want_evals)
+
+    def sync_tracks_pgs(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
+                        ref_is_pgs, pgs_start_s, pgs_end_s, pgs_off, cue_start_s, cue_end_s, cue_keep, cue_off, ratios,
+                        start_seconds: float, max_offset_samples: Optional[int], ref_is_subs=None,
+                        ref_cue_start_s=None, ref_cue_end_s=None, ref_cue_keep=None, ref_cue_off=None,
+                        detector: int = B2_DETECTOR_ENERGY_ZCR, energy_threshold: int = 0, z_lo: int = -1,
+                        z_hi: int = -1, chunk_samples: int = 0, energy_threshold_db: float = 50.0,
+                        min_length: Optional[float] = None, max_length: Optional[int] = None,
+                        max_continuous_silence: Optional[float] = None, gss: bool = False, best_score=None,
+                        best_offset=None, best_k=None, all_score=None, all_offset=None, gss_ratio=None, gss_evals=None,
+                        want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST):
+        """sync_tracks_subs where the videos with ref_is_pgs[v] != 0 take their PGS display intervals (pgs_off[v] ..
+        pgs_off[v+1], host arrays) rasterised by PGSSpeechTransformer's rule as reference signal
+        (b2_sync_tracks_pgs).  The text references (ref_is_subs, ref_cue_*) are optional.  Returns as
+        sync_tracks_subs."""
+        V, T = len(pcm_off) - 1, len(track_video)
+        pgs_off = _i64a(pgs_off)
+        if len(cue_off) != T + 1 or len(pgs_off) != V + 1:
+            raise NativeError(-1, "b2_sync_tracks_pgs", "cue_off / pgs_off have %d / %d entries for %d tracks / "
+                              "%d videos" % (len(cue_off), len(pgs_off), T, V))
+        ref_is_pgs = None if ref_is_pgs is None else np.ascontiguousarray(ref_is_pgs, dtype=np.uint8)
+        ref_is_subs = None if ref_is_subs is None else np.ascontiguousarray(ref_is_subs, dtype=np.uint8)
+        for name, a in (("ref_is_pgs", ref_is_pgs), ("ref_is_subs", ref_is_subs)):
+            if a is not None and len(a) != V:
+                raise NativeError(-1, "b2_sync_tracks_pgs", "%s has %d entries for %d videos" % (name, len(a), V))
+        if ref_cue_off is not None:
+            ref_cue_off = _i64a(ref_cue_off)
+            if len(ref_cue_off) != V + 1:
+                raise NativeError(-1, "b2_sync_tracks_pgs", "ref_cue_off has %d entries for %d videos"
+                                  % (len(ref_cue_off), V))
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)   # noqa: E731
+        pgs_start_s, pgs_end_s = f64(pgs_start_s), f64(pgs_end_s)
+        ref_cue_start_s, ref_cue_end_s = f64(ref_cue_start_s), f64(ref_cue_end_s)
+        ref_cue_keep = None if ref_cue_keep is None else np.ascontiguousarray(ref_cue_keep, dtype=np.uint8)
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        return self._sync("b2_sync_tracks_pgs", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, int(detector), float(non_speech_label), int(energy_threshold),
+                           int(z_lo), int(z_hi), float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
+                           _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
+                           _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off)),
+                          cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
                           (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
                           memspace, gss=bool(gss), want_evals=want_evals)
 

@@ -33,6 +33,8 @@ def load_serialized_speech(paths, non_speech_label: float = 0.0):
 
 # keyword arguments of the sync methods that describe the embedded subtitle streams of a subs_then_ detector
 _STREAM_ARGS = ("ref_cue_start", "ref_cue_end", "ref_cue_off", "ref_stream_video", "ref_cue_content", "ref_cue_keep")
+# keyword arguments of the sync methods that describe the videos' PGS (bitmap subtitle) display intervals
+_PGS_ARGS = ("pgs_start", "pgs_end", "pgs_off", "pgs_video")
 
 
 def _is_unsupported(e: Exception) -> bool:
@@ -60,9 +62,17 @@ class BatchSynchronizer:
     ``ref_cue_content`` (the cue texts: keep flags by the reference's metadata filter) or ``ref_cue_keep``.  Each
     video uses its stream with the largest ``max_end - start_seconds`` (the first on a tie), rasterised at
     ``sample_rate`` with level 1.0; a video with a stream must have an empty PCM range (its audio is never read;
-    ``pcm`` may be None when no video has any).  Extracting the streams from containers (ffprobe / ffmpeg), bitmap
-    (PGS) streams and ``--reference-stream`` remain the caller's job.  Without streams the results are those of the
-    detector alone."""
+    ``pcm`` may be None when no video has any).  Extracting the streams from containers (ffprobe / ffmpeg) and
+    ``--reference-stream`` remain the caller's job; bitmap (PGS) streams come as their own arguments (below).  Without streams the results are those of the
+    detector alone.
+
+    PGS references (``--pgs-ref-stream``, with every ``vad``): the sync methods also take the display intervals of
+    P videos' PGS (Blu-ray bitmap) subtitle streams as keyword arguments ``pgs_start`` / ``pgs_end`` (seconds:
+    ffprobe's ``pts_time`` and ``pts_time + duration_time``, e.g. from ``speech_transformers.pgs_timings_from_packets``),
+    ``pgs_off`` [P+1] and ``pgs_video`` [P] (increasing: at most one interval list per video).  Such a video is synced
+    against its intervals rasterised by PGSSpeechTransformer's rule (b2_rasterize_pgs) instead of its audio or text
+    stream - the reference tries ``--pgs-ref-stream`` first - and must have an empty PCM range.  Running ffprobe
+    stays the caller's job."""
 
     def __init__(self, ratios: Sequence[Optional[float]], frame_rate: int = 16000, sample_rate: int = SAMPLE_RATE,
                  non_speech_label: float = 0.0, energy_threshold: int = DEFAULT_ENERGY_THRESHOLD,
@@ -101,6 +111,48 @@ class BatchSynchronizer:
     def auditok(self) -> bool:
         return self.detector == "auditok"
 
+    def _references(self, V: int, streams: dict):
+        """(refs, pgs) of the keyword arguments: refs from _subs_refs, pgs from _pgs_refs.  A video with both a PGS
+        reference and text streams keeps the PGS one (make_reference_pipe's order), so its text stream is dropped."""
+        pgs = self._pgs_refs(V, {k: streams.pop(k) for k in _PGS_ARGS if k in streams})
+        refs = self._subs_refs(V, streams)
+        if refs is None or pgs is None or not np.any(refs[0] & pgs[0]):
+            return refs, pgs
+        is_subs, rs, re_, rk, roff = refs
+        keep_v = (is_subs != 0) & (pgs[0] == 0)
+        pick = np.concatenate([np.arange(roff[v], roff[v + 1]) for v in range(V) if keep_v[v]]
+                              + [np.zeros(0, np.int64)]).astype(np.int64)
+        lens = np.where(keep_v, np.diff(roff), 0)
+        return ((keep_v.astype(np.uint8), rs[pick], re_[pick], None if rk is None else rk[pick],
+                 np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)), pgs)
+
+    def _pgs_refs(self, V: int, args: dict):
+        """Each video's PGS interval list, or None when none is given: returns (ref_is_pgs u8[V], pgs_start,
+        pgs_end, pgs_off [V+1]) for b2_sync_tracks_pgs."""
+        if all(args.get(k) is None for k in _PGS_ARGS):
+            return None
+        missing = [k for k in _PGS_ARGS if args.get(k) is None]
+        if missing:
+            raise ValueError("PGS references need %s" % ", ".join(_PGS_ARGS))
+        start = np.ascontiguousarray(args["pgs_start"], dtype=np.float64)
+        end = np.ascontiguousarray(args["pgs_end"], dtype=np.float64)
+        off = np.ascontiguousarray(args["pgs_off"], dtype=np.int64)
+        video = np.ascontiguousarray(args["pgs_video"], dtype=np.int64)
+        P = len(off) - 1
+        if len(video) != P:
+            raise ValueError("pgs_video has %d entries for %d interval lists" % (len(video), P))
+        if P and (np.any(np.diff(video) <= 0) or video[0] < 0 or video[-1] >= V):
+            raise ValueError("pgs_video must be increasing video indices in [0, %d) (one interval list per video)" % V)
+        if np.any(np.diff(off) < 0) or (P and (off[0] < 0 or off[-1] > min(len(start), len(end)))):
+            raise ValueError("pgs_off must be non-decreasing and within the interval arrays")
+        is_pgs = np.zeros(V, dtype=np.uint8)
+        is_pgs[video] = 1
+        lens = np.zeros(V, dtype=np.int64)
+        lens[video] = np.diff(off)
+        pick = np.concatenate([np.arange(off[i], off[i + 1]) for i in range(P)] + [np.zeros(0, np.int64)])
+        pick = pick.astype(np.int64)
+        return is_pgs, start[pick], end[pick], np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+
     def _subs_refs(self, V: int, streams: dict):
         """Each video's reference stream by the reference's rule, or None when no stream is given: returns
         (ref_is_subs u8[V], ref_cue_start, ref_cue_end, ref_cue_keep, ref_cue_off [V+1]) for b2_sync_tracks_subs."""
@@ -119,15 +171,24 @@ class BatchSynchronizer:
                                         streams["ref_stream_video"], self.start_seconds,
                                         content=streams.get("ref_cue_content"), keep=streams.get("ref_cue_keep"))
 
-    def _dispatch(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, **kw):
-        """The batched call of this synchroniser's detector with the search on or off: b2_sync_tracks_subs with
-        subtitle references (refs, from _subs_refs), else b2_sync_tracks_auditok for auditok, else
+    def _dispatch(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, pgs=None,
+                  **kw):
+        """The batched call of this synchroniser's detector with the search on or off: b2_sync_tracks_pgs with PGS
+        references (pgs, from _pgs_refs), else b2_sync_tracks_subs with subtitle references (refs, from _subs_refs), else b2_sync_tracks_auditok for auditok, else
         b2_sync_tracks_gss / b2_sync_tracks.  pcm: int16 numpy array, CUDA tensor or None; kw: the outputs (device
         pointers) or want_all, and memspace.  Returns (best_score, best_offset, best_k, all_score, all_offset), plus
         (gss_ratio, gss_evals) with gss."""
         h = self.handle
         p = pcm if pcm is None or isinstance(pcm, np.ndarray) else pcm.data_ptr()
         cues = (cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples)
+        if pgs is not None:
+            det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
+            text = {} if refs is None else dict(zip(("ref_is_subs", "ref_cue_start_s", "ref_cue_end_s", "ref_cue_keep",
+                                                     "ref_cue_off"), refs))
+            return h.sync_tracks_pgs(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                     self.non_speech_label, *pgs, *cues, detector=det,
+                                     energy_threshold=self.energy_threshold, z_lo=self.z_lo, z_hi=self.z_hi,
+                                     chunk_samples=self.chunk_samples, gss=gss, **text, **kw)
         if refs is not None:
             det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
             return h.sync_tracks_subs(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
@@ -140,20 +201,21 @@ class BatchSynchronizer:
         energy = (self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
         return (h.sync_tracks_gss if gss else h.sync_tracks)(p, pcm_off, track_video, *energy, *cues, **kw)
 
-    def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, **kw):
+    def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=None,
+                         **kw):
         """_dispatch with this synchroniser's search.  Outside the envelope of the device-driven search
         (B2_ERR_UNSUPPORTED) the search is composed of public steps instead (_gss_compose).  Returns
         (best_score, best_offset, best_k, all_score, all_offset), plus gss_ratio with the search; composed results
         are numpy arrays (all_* None unless want_all or device outputs were given)."""
         try:
             return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
-                                  **kw)[:6]
+                                  pgs=pgs, **kw)[:6]
         except _native.NativeError as e:
             if not (self.gss and _is_unsupported(e)):
                 raise
         want_all = kw.get("want_all", False) or kw.get("all_score") is not None
         bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off,
-                                                        cue_keep, want_all=want_all, refs=refs)
+                                                        cue_keep, want_all=want_all, refs=refs, pgs=pgs)
         return bs, bo, bk, a_s, a_o, ratio
 
     def use_torch_stream(self) -> None:
@@ -170,15 +232,16 @@ class BatchSynchronizer:
         stream before this call still writes ``pcm`` (a corpus that sits in HBM).  Back-to-back calls then
         overlap: the VAD of this batch starts while the last correlation chain of the previous batch is
         still running.  Results are identical; outputs stay ordered on the stream.
-        With a ``subs_then_`` detector the embedded subtitle streams come as keyword arguments (see the class)."""
+        With a ``subs_then_`` detector the embedded subtitle streams come as keyword arguments, and with any detector
+        the PGS references (see the class)."""
         import torch
         B = len(pcm_off) - 1
         K = len(self.ratios)
-        if self.gss or self.auditok or self.subs_then:   # the identity track map: pair b is track b of video b
+        if self.gss or self.auditok or self.subs_then or any(streams.get(k) is not None for k in _PGS_ARGS):   # the identity track map: pair b is track b of video b
             return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
                                            cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident,
                                            **streams)
-        self._subs_refs(B, streams)   # rejects streams and unknown keywords
+        self._references(B, streams)   # rejects streams and unknown keywords
         dev = pcm.device
         if out is None:
             out = {"best_score": torch.empty(B, dtype=torch.float64, device=dev),
@@ -206,10 +269,11 @@ class BatchSynchronizer:
         as for sync_device (resident calls of both methods chain with each other).
         With the golden-section search (a trailing None in ratios) out also holds gss_ratio f64[T] and all_out
         is {"score": f64[T*(K+1)], "offset": i32[T*(K+1)]} with column K the search's candidate.
-        streams: the embedded subtitle streams of a ``subs_then_`` detector (ref_cue_start, ... - see the class)."""
+        streams: the embedded subtitle streams of a ``subs_then_`` detector (ref_cue_start, ... - see the class) and
+        the PGS references (pgs_start, pgs_end, pgs_off, pgs_video)."""
         import torch
         T = len(track_video)
-        refs = self._subs_refs(len(pcm_off) - 1, streams)
+        refs, pgs = self._references(len(pcm_off) - 1, streams)
         dev = pcm.device if pcm is not None else torch.device("cuda", self.handle.device)
         if out is None:
             out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
@@ -222,7 +286,7 @@ class BatchSynchronizer:
         ptrs = {k: out[k].data_ptr() for k in keys}
         if all_out:
             ptrs.update(all_score=all_out["score"].data_ptr(), all_offset=all_out["offset"].data_ptr())
-        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs,
+        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
                                     memspace=memspace, **ptrs)
         if isinstance(res[0], np.ndarray):   # composed on the host
             for k, v in zip(keys, res[:3] + res[5:]):
@@ -237,8 +301,8 @@ class BatchSynchronizer:
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
         track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks."""
-        refs = self._subs_refs(len(pcm_off) - 1, streams)
-        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs,
+        refs, pgs = self._references(len(pcm_off) - 1, streams)
+        res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
                                     want_all=want_all, memspace=_native.B2_HOST)
         return res if want_all else res[:3] + res[5:]
 
@@ -285,7 +349,7 @@ class BatchSynchronizer:
         return bs, bo, bk, ratio
 
     def sync_device_candidate_sharded(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None,
-                                      rank: int = 0, world: int = 1, group=None):
+                                      rank: int = 0, world: int = 1, group=None, **pgs_args):
         """Secondary multi-GPU mode (SURVEY.md section 8e, "B < G": a few pairs on many GPUs): the K
         ratio candidates of every pair are dealt round-robin over the ranks.  Every rank runs the
         VAD of the (replicated) reference PCM - 33 us per 2 h signal, cheaper than shipping the
@@ -304,6 +368,12 @@ class BatchSynchronizer:
         if self.subs_then:
             raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
                              "embedded subtitle references (vad=%r)" % self.vad)
+        unknown = set(pgs_args) - set(_PGS_ARGS)
+        if unknown:
+            raise TypeError("unexpected keyword arguments %s" % ", ".join(sorted(unknown)))
+        if any(v is not None for v in pgs_args.values()):
+            raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
+                             "PGS references (%s)" % ", ".join(sorted(pgs_args)))
         h = self.handle
         self.use_torch_stream()   # torch ops and NCCL below are ordered against our kernels by the stream
         pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
@@ -353,11 +423,11 @@ class BatchSynchronizer:
         """pcm: int16 numpy array (ideally backed by pinned memory).  Blocks until results are on
         the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]), and gss_ratio last
         with the golden-section search.  With a ``subs_then_`` detector the embedded subtitle streams come as
-        keyword arguments (see the class)."""
-        if self.gss or self.auditok or self.subs_then:
+        keyword arguments, and with any detector the PGS references (see the class)."""
+        if self.gss or self.auditok or self.subs_then or any(streams.get(k) is not None for k in _PGS_ARGS):
             return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
                                          cue_end, cue_off, cue_keep, want_all=want_all, **streams)
-        self._subs_refs(len(pcm_off) - 1, streams)   # rejects streams and unknown keywords
+        self._references(len(pcm_off) - 1, streams)   # rejects streams and unknown keywords
         res = self.handle.sync_batch(
             pcm, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold,
             self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds,
@@ -365,7 +435,7 @@ class BatchSynchronizer:
         return res if want_all else res[:3]
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
-                     refs=None):
+                     refs=None, pgs=None):
         """The golden-section search outside the envelope of the device-driven search, composed of public steps:
         the grid (this synchroniser's batched call with the search off), gss_align_batch on each track's reference
         signal (_reference_signals, with subtitle references refs from _subs_refs) and the reference's combine.
@@ -385,8 +455,8 @@ class BatchSynchronizer:
         else:
             pcm_host = pcm
         grid = self._dispatch(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, False,
-                              want_all=True, memspace=_native.B2_HOST)
-        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs)
+                              pgs=pgs, want_all=True, memspace=_native.B2_HOST)
+        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs)
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
@@ -397,10 +467,11 @@ class BatchSynchronizer:
                                                   grid[3], grid[4])
         return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))
 
-    def _reference_signals(self, pcm_host, pcm_off, refs=None):
+    def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None):
         """The per-video reference signals the batched calls sync against, composed of public calls: the detector
-        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, and with subtitle references
-        (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0.
+        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, with subtitle references
+        (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0, and
+        with PGS references (pgs, from _pgs_refs) for a video that has one b2_rasterize_pgs of its intervals.
         Returns (float32 signals back to back, ref_off int64[V+1])."""
         h = self.handle
         V = len(pcm_off) - 1
@@ -412,13 +483,22 @@ class BatchSynchronizer:
         else:
             det, det_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
                                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
-        if refs is None:
+        if refs is None and pgs is None:
             return det.astype(np.float32), det_off
-        is_subs, rs, re_, rk, roff = refs
-        sub, sub_off = h.rasterize(rs, re_, rk, roff, [1.0], 1, False, self.sample_rate, self.start_seconds,
-                                   levels=[1.0])
-        parts = [sub[sub_off[v]: sub_off[v + 1]] if is_subs[v] else det[det_off[v]: det_off[v + 1]].astype(np.float32)
-                 for v in range(V)]
+        parts = [det[det_off[v]: det_off[v + 1]].astype(np.float32) for v in range(V)]
+        if refs is not None:
+            is_subs, rs, re_, rk, roff = refs
+            sub, sub_off = h.rasterize(rs, re_, rk, roff, [1.0], 1, False, self.sample_rate, self.start_seconds,
+                                       levels=[1.0])
+            for v in np.flatnonzero(is_subs):
+                parts[v] = sub[sub_off[v]: sub_off[v + 1]]
+        if pgs is not None:
+            is_pgs, ps, pe, poff = pgs
+            vids = np.flatnonzero(is_pgs)
+            sig, sig_off = h.rasterize_pgs(ps, pe, np.concatenate([[0], np.cumsum(np.diff(poff)[vids])]),
+                                           self.sample_rate, self.start_seconds)
+            for i, v in enumerate(vids):
+                parts[v] = sig[sig_off[i]: sig_off[i + 1]]
         off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
         return (np.concatenate(parts) if parts else np.zeros(0, np.float32)), off
 

@@ -678,6 +678,53 @@ extern "C" int b2_rasterize(b2_handle h, const double* cue_start_s, const double
   return B2_OK;
 }
 
+// ---- PGS rasteriser (PGSSpeechTransformer.fit) ------------------------------------------------
+extern "C" int b2_rasterize_pgs_lengths(const double* end_s, const int64_t* off, int B, int sample_rate,
+                                        int64_t* lengths) {
+  if (B < 0 || !off || !lengths) return B2_ERR_BAD_ARG;
+  std::string err;
+  return pgs_lengths(&err, "rasterize_pgs_lengths", "", nullptr, end_s, off, B, sample_rate, false, 0.0, nullptr,
+                     lengths);
+}
+
+extern "C" int b2_rasterize_pgs(b2_handle h, const double* start_s, const double* end_s, const int64_t* off, int B,
+                                int sample_rate, double start_seconds, float* out, const int64_t* out_off,
+                                int memspace) {
+  B2_ENTER(h);
+  if (B < 0 || !off || !out_off) B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize_pgs: bad arguments");
+  if (B == 0) return B2_OK;
+  std::vector<int64_t> lengths(B);
+  if (const int st = pgs_lengths(&h->err, "rasterize_pgs", "", start_s, end_s, off, B, sample_rate, true,
+                                 start_seconds, nullptr, lengths.data()))
+    return st;
+  for (int b = 0; b < B; ++b)
+    if (out_off[b + 1] < out_off[b]) B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize_pgs: out_off not monotone at %d", b);
+  const int64_t base = out_off[0], total = out_off[B] - base;
+  if (total && !out) B2_FAIL(h, B2_ERR_BAD_ARG, "rasterize_pgs: null output");
+  if (total) B2_CHECK_DEV(h, memspace, out, "rasterize_pgs: out");
+  // signal b goes to out + out_off[b]; a host call stages the signals from offset 0
+  float* d_out = out;
+  std::vector<int64_t> staged_off;
+  const int64_t* d_off = out_off;
+  if (memspace == B2_HOST) {
+    void* dq;
+    B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_OUT, (size_t)total * 4 + 16, &dq));
+    d_out = (float*)dq;
+    staged_off.resize(B + 1);
+    for (int b = 0; b <= B; ++b) staged_off[b] = out_off[b] - base;
+    d_off = staged_off.data();
+  }
+  std::vector<int> all(B);
+  for (int b = 0; b < B; ++b) all[b] = b;
+  B2_TRY(b2i_raster_ref_launch(h, start_s, end_s, nullptr, off, d_off, B, all.data(), B, sample_rate, start_seconds,
+                               d_out, true));
+  if (memspace == B2_HOST) {
+    B2_TRY(copy_out(h, out + base, d_out, (size_t)total * 4));
+    B2_CUDA(h, cudaStreamSynchronize(h->stream));
+  }
+  return B2_OK;
+}
+
 // ---- fused-VAD blend -------------------------------------------------------------------------
 extern "C" int b2_blend_signals(b2_handle h, const float* a, const float* b, int64_t n, int mode,
                                 double wa, double wb, float* out, int memspace) {
@@ -889,7 +936,8 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // own, so the GSS invariant (no later arena of a chain recycles the chain's arena, runcorr.cu b2i_gss_launch)
 // holds as before: the chains' arenas come from the caller-facing ring, and with one sub-batch the detector's
 // arenas there precede the chain's.
-// With subtitle references (b2_sync_tracks_subs) the step also rasterises those of the videos [v0, v1) into
+// With subtitle references (b2_sync_tracks_subs; text and PGS ones with b2_sync_tracks_pgs) the step also
+// rasterises those of the videos [v0, v1) into
 // their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
 // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
@@ -909,15 +957,22 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
                                        ch.tok_end.data() + k0));
   }
   if (!p.any_subs) return B2_OK;
-  const auto& sv = p.sub_video;
-  const int s0 = (int)(std::lower_bound(sv.begin(), sv.end(), v0) - sv.begin());
-  const int s1 = (int)(std::lower_bound(sv.begin(), sv.end(), v1) - sv.begin());
-  if (s1 == s0) return B2_OK;
-  std::vector<int> rel(sv.begin() + s0, sv.begin() + s1);
-  for (int& v : rel) v -= v0;
-  return b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
-                               p.ref_off.data() + v0, v1 - v0, rel.data(), (int)rel.size(), r.sample_rate,
-                               r.start_seconds, b.refsig);
+  // the videos of `list` in [v0, v1), relative to v0
+  auto in_range = [&](const std::vector<int>& list) {
+    std::vector<int> rel(std::lower_bound(list.begin(), list.end(), v0), std::lower_bound(list.begin(), list.end(), v1));
+    for (int& v : rel) v -= v0;
+    return rel;
+  };
+  const std::vector<int> subs = in_range(p.sub_video), pgs = in_range(p.pgs_video);
+  if (!subs.empty())
+    B2_TRY(b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
+                                 p.ref_off.data() + v0, v1 - v0, subs.data(), (int)subs.size(), r.sample_rate,
+                                 r.start_seconds, b.refsig));
+  if (!pgs.empty())
+    B2_TRY(b2i_raster_ref_launch(h, r.pgs.start_s, r.pgs.end_s, nullptr, r.pgs.off + v0, p.ref_off.data() + v0,
+                                 v1 - v0, pgs.data(), (int)pgs.size(), r.sample_rate, r.start_seconds, b.refsig,
+                                 true));
+  return B2_OK;
 }
 
 // Software pipeline over the plan's sub-batches of videos (sync_plan.h plan_cuts).  The VAD (HBM-bound) of every
@@ -1215,5 +1270,39 @@ extern "C" int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm, const int64_
                       cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
                       best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
                       memspace};
+  return sync_run(h, _b2_fence_was_valid, r);
+}
+
+extern "C" int b2_sync_tracks_pgs(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                  const int32_t* track_video, int T, int frame_rate, int sample_rate, int detector,
+                                  double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                                  double energy_threshold_db, double min_length, int64_t max_length,
+                                  double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs,
+                                  const double* ref_cue_start_s, const double* ref_cue_end_s,
+                                  const uint8_t* ref_cue_keep, const int64_t* ref_cue_off, const uint8_t* ref_is_pgs,
+                                  const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off,
+                                  const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                  const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                  int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                  int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                  double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_pgs");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_pgs: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_pgs: gss_evals without gss_ratio");
+  if (V > 0 && (!pcm_off || !pgs_off)) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_pgs: null pcm_off / pgs_off");
+  if (ref_is_subs && !ref_cue_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_pgs: ref_is_subs without ref_cue_off");
+  if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_pgs: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, "
+            "not %d", detector);
+  static const int64_t no_intervals[1] = {0};
+  SyncRequest r{gss_ratio ? "sync_tracks_pgs (search)" : "sync_tracks_pgs", pcm, pcm_off, V, track_video, T,
+                frame_rate, sample_rate, detector, {(float)non_speech_label, energy_threshold, z_lo, z_hi},
+                {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length, chunk_samples},
+                {ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : nullptr},
+                cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
+                memspace};
+  r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : no_intervals};
   return sync_run(h, _b2_fence_was_valid, r);
 }

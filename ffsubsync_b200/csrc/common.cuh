@@ -189,10 +189,11 @@ int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
                       double start_seconds, float* d_out, const int64_t* out_off_host);
 // Subtitle references of b2_sync_tracks_subs: for each of the n_subs videos videos[i] (indices into the host
 // tables cue_off / out_off [n_videos + 1], absolute), zero d_out[out_off[v] .. out_off[v+1]) and write 1.0 over
-// its kept cues at ratio 1.0 - b2_rasterize at ratio 1.0 and level 1.0, at per-video bases.
+// its kept cues at ratio 1.0 - b2_rasterize at ratio 1.0 and level 1.0, at per-video bases.  pgs: the lists are
+// PGS intervals (b2_sync_tracks_pgs, b2_rasterize_pgs), written by b2_pgs_bounds; cue_keep is not read.
 int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_end, const uint8_t* cue_keep,
                           const int64_t* cue_off, const int64_t* out_off, int n_videos, const int* videos, int n_subs,
-                          int sample_rate, double start_seconds, float* d_out);
+                          int sample_rate, double start_seconds, float* d_out, bool pgs = false);
 int b2i_bounds_launch(b2_ctx* h, const float* d_sig, const int64_t* off_host, int n,
                       int64_t* d_first, int64_t* d_last);
 int b2i_blend_launch(b2_ctx* h, const float* d_a, const float* d_b, int64_t n, int mode, double wa,

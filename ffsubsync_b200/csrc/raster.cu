@@ -106,10 +106,14 @@ __global__ void __launch_bounds__(256) raster_bits_kernel(RasterBitsParams p) {
 // SubtitleSpeechTransformer, speech_transformers.py:479-523), written into the reference-signal buffer at
 // the video's own base between the detector's outputs.  One CTA per such video: zero the signal, then one
 // warp per cue with the same cue arithmetic as raster_cues_kernel.
+// K2p: PGS references (b2_sync_tracks_pgs, b2_rasterize_pgs) have the same structure with PGSSpeechTransformer's
+// interval arithmetic (b2_pgs_bounds: every write lies in [0, n) of the video's own range) and no keep flags.
+enum RefRule { kRefCues = 0, kRefPgs = 1 };
+
 struct RasterRefParams {
   const double* start_s;
   const double* end_s;
-  const uint8_t* keep;        // may be null
+  const uint8_t* keep;        // may be null (kRefPgs: not read)
   const long long* cue_off;   // [n_videos+1] absolute
   const long long* out_off;   // [n_videos+1] the reference-signal buffer's offsets
   const int* video;           // [grid.x] the videos (indices into cue_off / out_off) with a subtitle reference
@@ -118,6 +122,7 @@ struct RasterRefParams {
   double start_seconds;
 };
 
+template <int kRule>
 __global__ void __launch_bounds__(256) raster_ref_kernel(RasterRefParams p) {
   const int v = p.video[blockIdx.x];
   const long long c0 = p.cue_off[v], c1 = p.cue_off[v + 1];
@@ -127,9 +132,13 @@ __global__ void __launch_bounds__(256) raster_ref_kernel(RasterRefParams p) {
   __syncthreads();
   const int lane = threadIdx.x & 31;
   for (long long c = c0 + (threadIdx.x >> 5); c < c1; c += blockDim.x >> 5) {
-    if (p.keep && !p.keep[c]) continue;
     long long first, last;
-    b2_cue_bounds(p.start_s[c], p.end_s[c], 1.0, p.start_seconds, p.sample_rate, n, first, last);
+    if (kRule == kRefPgs) {
+      b2_pgs_bounds(p.start_s[c], p.end_s[c], p.start_seconds, p.sample_rate, n, first, last);
+    } else {
+      if (p.keep && !p.keep[c]) continue;
+      b2_cue_bounds(p.start_s[c], p.end_s[c], 1.0, p.start_seconds, p.sample_rate, n, first, last);
+    }
     for (long long i = first + lane; i < last; i += 32) out[i] = 1.0f;
   }
 }
@@ -268,9 +277,9 @@ int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
 
 int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_end, const uint8_t* cue_keep,
                           const int64_t* cue_off, const int64_t* out_off, int n_videos, const int* videos, int n_subs,
-                          int sample_rate, double start_seconds, float* d_out) {
+                          int sample_rate, double start_seconds, float* d_out, bool pgs) {
   if (n_subs <= 0) return B2_OK;
-  B2Range range("b2:raster_ref");
+  B2Range range(pgs ? "b2:raster_pgs" : "b2:raster_ref");
   // cue_off / out_off are slices of the call's tables (a sub-batch): entries are absolute, only
   // [cue_off[0], cue_off[n_videos]) is uploaded (pointers rebased)
   const size_t c0 = (size_t)cue_off[0], nc = (size_t)cue_off[n_videos] - c0;
@@ -288,8 +297,13 @@ int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_
   p.out = d_out;
   p.sample_rate = sample_rate;
   p.start_seconds = start_seconds;
-  raster_ref_kernel<<<n_subs, 256, 0, h->stream>>>(p);
-  B2_CHECK_LAUNCH(h, "raster_ref_kernel");
+  if (pgs) {
+    raster_ref_kernel<kRefPgs><<<n_subs, 256, 0, h->stream>>>(p);
+    B2_CHECK_LAUNCH(h, "raster_ref_kernel<pgs>");
+  } else {
+    raster_ref_kernel<kRefCues><<<n_subs, 256, 0, h->stream>>>(p);
+    B2_CHECK_LAUNCH(h, "raster_ref_kernel");
+  }
   return B2_OK;
 }
 

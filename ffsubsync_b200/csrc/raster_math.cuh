@@ -1,4 +1,5 @@
-// Bit-exact restatement of the reference's cue arithmetic, shared by both rasterisers (raster.cu:
+// Bit-exact restatement of the reference's cue arithmetic (and, at the end, of its PGS interval arithmetic),
+// shared by both rasterisers (raster.cu:
 // raster_cues_kernel, raster_bits_kernel), by b2_rasterize_lengths on the host (api.cu) and by the
 // CPU emulator tests/host_emul/raster_emul.cu.  Reference: SubtitleScaler.fit
 // (ffsubsync/subtitle_transformers.py:35-47) + SubtitleSpeechTransformer.fit
@@ -86,4 +87,27 @@ RASTER_HD void b2_cue_bounds(double start_s, double end_s, double ratio, double 
   last = first + b2_rm_rint(b2_rm_mul(b2_rm_sub(en, st), (double)sample_rate));
   if (first < 0) { first += n; if (first < 0) first = 0; } else if (first > n) first = n;
   if (last < 0) { last += n; if (last < 0) last = 0; } else if (last > n) last = n;
+}
+
+// ---- PGS references (PGSSpeechTransformer.fit, ffsubsync/speech_transformers.py:1186-1198) ----------------------
+// The bitmap-subtitle rule differs from the text one above: raw float64 times (no microsecond rounding), each end
+// rounded on its own, and a length that is truncated toward zero with no max(0, .).  Valid for finite times and
+// start_seconds with magnitude below B2_MAX_CUE_SECONDS and sample_rate <= B2_PGS_MAX_SAMPLE_RATE: every frame index
+// then fits an int64 (2 * 2^33 s * 2^28 Hz < 2^62).  Callers reject everything else (sync_plan.h pgs_list_check).
+#define B2_PGS_MAX_SAMPLE_RATE (1 << 28)
+
+// int(max_end * sample_rate) + 2: may be 1, 0 or negative for max_end < 0 (np.zeros raises on negative)
+RASTER_HD long long b2_pgs_length(double max_end, int sample_rate) {
+  return (long long)b2_rm_mul(max_end, (double)sample_rate) + 2;
+}
+
+// The interval's frames [first, last) in a length-n signal: int(round((t - start_seconds) * sample_rate)) per end
+// (Python round: half to even), then first = max(first, 0), last = min(last, n).  Empty when first >= last
+// (intervals may overlap, be unsorted or have a negative duration).
+RASTER_HD void b2_pgs_bounds(double start_s, double end_s, double start_seconds, int sample_rate, long long n,
+                             long long& first, long long& last) {
+  first = b2_rm_rint(b2_rm_mul(b2_rm_sub(start_s, start_seconds), (double)sample_rate));
+  last = b2_rm_rint(b2_rm_mul(b2_rm_sub(end_s, start_seconds), (double)sample_rate));
+  if (first < 0) first = 0;
+  if (last > n) last = n;
 }

@@ -1,5 +1,5 @@
 // Host-side plan of one batched sync call (b2_sync_batch, b2_sync_tracks, b2_sync_tracks_gss,
-// b2_sync_tracks_auditok, b2_sync_tracks_subs): every argument check and every host table the pipeline in
+// b2_sync_tracks_auditok, b2_sync_tracks_subs, b2_sync_tracks_pgs): every argument check and every host table the pipeline in
 // api.cu reads.  No CUDA call happens here, so tests/host_emul/plan_emul.cu runs the same code on the CPU.
 #pragma once
 
@@ -143,6 +143,80 @@ static int cue_lengths(std::string* err, const char* who, const char* what, cons
   return B2_ERR_BAD_ARG;
 }
 
+// ---- PGS interval lists ------------------------------------------------------------------------
+// Why interval list [i0, i1) cannot be rasterised by PGSSpeechTransformer.fit's rule (raster_math.cuh b2_pgs_bounds),
+// or nullptr; else *len = its signal length int(max_end * sample_rate) + 2.  The reference raises for an empty list
+// (ValueError), a non-finite time (round / int) and a negative length (np.zeros); times of magnitude
+// B2_MAX_CUE_SECONDS and more are rejected too, so that every frame index fits an int64.  start_s may be null (not
+// checked: b2_rasterize_pgs_lengths).  *at: the offending interval (-1: the list), *val its value.
+static const char* pgs_list_check(const double* start_s, const double* end_s, int64_t i0, int64_t i1, int sample_rate,
+                                  int64_t* len, int64_t* at, double* val) {
+  *at = -1;
+  *val = (double)(i1 - i0);
+  if (i1 <= i0) return "empty interval list";
+  double max_end = end_s[i0];
+  for (int64_t i = i0; i < i1; ++i) {
+    for (const double* t : {start_s, end_s}) {
+      if (!t || fabs(t[i]) < B2_MAX_CUE_SECONDS) continue;
+      *at = i;
+      *val = t[i];
+      return t == start_s ? "interval start time is not finite or too large" : "interval end time is not finite or too large";
+    }
+    max_end = std::max(max_end, end_s[i]);
+  }
+  *len = b2_pgs_length(max_end, sample_rate);
+  if (*len < 0) {
+    *val = max_end;
+    return "negative signal length int(max_end * sample_rate) + 2";
+  }
+  return nullptr;
+}
+
+// The signal lengths of the interval lists [0, B) (off [B+1], absolute), with sample_rate, the offset table, null
+// arrays, start_seconds and the start times (when check_start) and every time checked; lists with only && !only[b] are skipped (length -1).  Messages
+// "<who>: <what><why> (index i: value)"; the index is the interval's, or "list b" for a list-level error.
+static int pgs_lengths(std::string* err, const char* who, const char* what, const double* start_s, const double* end_s,
+                       const int64_t* off, int B, int sample_rate, bool check_start, double start_seconds,
+                       const uint8_t* only, int64_t* lengths) {
+  char b[512];
+  if (sample_rate <= 0 || sample_rate > B2_PGS_MAX_SAMPLE_RATE) {
+    snprintf(b, sizeof(b), "%s: sample_rate %d is out of (0, %d]", who, sample_rate, B2_PGS_MAX_SAMPLE_RATE);
+    *err = b;
+    return B2_ERR_BAD_ARG;
+  }
+  if (check_start && !(fabs(start_seconds) < B2_MAX_CUE_SECONDS)) {
+    snprintf(b, sizeof(b), "%s: start_seconds is not finite or too large (%g)", who, start_seconds);
+    *err = b;
+    return B2_ERR_BAD_ARG;
+  }
+  // the whole table first: only a monotone one bounds every list by [off[0], off[B]), so that a null array is
+  // read by no list exactly when that range is empty
+  for (int v = 0; v < B; ++v)
+    if (off[v + 1] < off[v]) {
+      snprintf(b, sizeof(b), "%s: %soff not monotone at %d", who, what, v);
+      *err = b;
+      return B2_ERR_BAD_ARG;
+    }
+  if (B > 0 && off[B] > off[0] && (!end_s || (check_start && !start_s))) {
+    snprintf(b, sizeof(b), "%s: null %sinterval arrays", who, what);
+    *err = b;
+    return B2_ERR_BAD_ARG;
+  }
+  for (int v = 0; v < B; ++v) {
+    lengths[v] = -1;
+    if (only && !only[v]) continue;
+    int64_t at;
+    double val;
+    if (const char* why = pgs_list_check(start_s, end_s, off[v], off[v + 1], sample_rate, &lengths[v], &at, &val)) {
+      if (at < 0) snprintf(b, sizeof(b), "%s: %s%s (list %d: %g)", who, what, why, v, val);
+      else snprintf(b, sizeof(b), "%s: %s%s (index %lld: %g)", who, what, why, (long long)at, val);
+      *err = b;
+      return B2_ERR_BAD_ARG;
+    }
+  }
+  return B2_OK;
+}
+
 // ---- detectors --------------------------------------------------------------------------------
 static inline int vad_frames_per_window(int frame_rate, int sample_rate) {
   if (frame_rate <= 0 || sample_rate <= 0) return 0;
@@ -199,7 +273,7 @@ static inline bool tokenizer_params_ok(double min_length, int64_t max_length, do
 // chunks of ceil(len/fpw) long.  tail[c]: the energy floor of the chunk's short last block (0: none).  Chunk
 // starts are multiples of chunk_samples from the video's start ((2 fr // sr) * 5000 samples in the Python layer:
 // a multiple of 8, so aligned videos stay eligible for the lane-per-window energy kernel).
-// With subs_len (b2_sync_tracks_subs), a video with subs_len[v] >= 0 has a subtitle reference and no PCM: it is
+// With subs_len (b2_sync_tracks_subs / _pgs), a video with subs_len[v] >= 0 has a subtitle reference (text or PGS) and no PCM: it is
 // one empty chunk spanning its reference's subs_len[v] frames, so the energy pass has no tiles there, and the
 // tokenizer's table tok_* (chunks tok_first[v] .. tok_first[v+1]-1, frames tok_off[k] .. tok_end[k]) leaves it
 // out, so only the rasteriser writes it.  Without subs_len the tok_* tables stay empty (the tokenizer reads out).
@@ -293,6 +367,15 @@ struct SyncRequest {
   double* gss_ratio;               // [T]: the search's ratio
   double* gss_evals;               // may be null
   int memspace;
+  // PGS references (b2_sync_tracks_pgs; off null: none): videos with is_pgs[v] != 0 take their intervals
+  // off[v] .. off[v+1] (host arrays, absolute indices), rasterised by PGSSpeechTransformer's rule, as reference
+  // signal.  The value-initialised state is "no PGS video", so the other entry points leave it out.
+  struct {
+    const uint8_t* is_pgs;         // may be null: no video
+    const double* start_s;
+    const double* end_s;
+    const int64_t* off;            // [V+1]
+  } pgs;
 };
 
 // What plan_sync reads from the handle and the environment: the SM count, the most sub-batches the handle's
@@ -315,7 +398,8 @@ struct SyncPipeEnv {
 
 struct SyncPlan {
   std::string err;
-  bool gss = false, auditok = false, any_subs = false;
+  bool gss = false, auditok = false;
+  bool any_subs = false;           // a video has a subtitle reference, text or PGS (levels 1 and 0, no PCM)
   int fpw = 0, z_lo = 0, z_hi = 0;
   // the reference's levels (B2CueSource::ref_label / ref_two_level)
   float label = 0.0f, ref_label = 0.0f;
@@ -324,7 +408,8 @@ struct SyncPlan {
   std::vector<int> trk_off;        // [V+1]: first track of video v
   std::vector<int64_t> ref_off;    // [V+1]: reference signal of video v
   std::vector<int64_t> sub_off;    // [T*K+1]: float subtitle signal of job j (unfused raster)
-  std::vector<int> sub_video;      // the videos with a subtitle reference, ascending
+  std::vector<int> sub_video;      // the videos with a text subtitle reference, ascending
+  std::vector<int> pgs_video;      // the videos with a PGS reference, ascending
   ChunkTable ch;                   // auditok
   int64_t auditok_e_min = 0;
   B2TokenizerParams tok{0.0, 0.0, 0.0, 0};
@@ -375,14 +460,16 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // instead of the floats: 1/32 of the bytes written, and the chain reads bits instead of floats.  The chain's path
 // is decided here by the aligner's own functions on the chain's own inputs (align_path.h, as enqueue_chain passes
 // them), so the launcher reaches the same choice.  auditok, subtitle references, the lane-group kernel and the
-// FFT paths keep the float reference.  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
+// FFT paths keep the float reference (text and PGS references alike).  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
   if (p->auditok || !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0)) return;
   for (int i = 0; i < p->n_sub; ++i) {
     const int v0 = p->cut[i], v1 = p->cut[i + 1];
     const auto& sv = p->sub_video;
+    const auto& pv = p->pgs_video;
     if (std::lower_bound(sv.begin(), sv.end(), v0) != std::lower_bound(sv.begin(), sv.end(), v1)) continue;
+    if (std::lower_bound(pv.begin(), pv.end(), v0) != std::lower_bound(pv.begin(), pv.end(), v1)) continue;
     if (!env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw)) continue;
     const int t0 = p->trk_off[v0], nt = p->trk_off[v1] - t0;
     std::vector<int> chain_trk(v1 - v0 + 1);
@@ -397,24 +484,41 @@ static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPl
   }
 }
 
-// Checks of the subtitle references, before anything reads their tables.
+// Checks of the subtitle references (text and PGS), before anything reads their tables.
 static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio) {
   const char* who = r.who;
   const auto& s = r.refs;
+  const auto& g = r.pgs;
   for (int v = 0; v < r.V; ++v) {
-    const bool is_subs = s.is_subs && s.is_subs[v];
-    if (s.cue_off[v + 1] < s.cue_off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: ref_cue_off not monotone at %d", who, v);
-    if (!is_subs && s.cue_off[v + 1] != s.cue_off[v])
-      B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has reference cues but no subtitle reference (ref_is_subs[%d] = 0)",
-              who, v, v);
-    if (is_subs && r.pcm_off[v + 1] != r.pcm_off[v])
-      B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has a subtitle reference and a non-empty PCM range (%lld samples); "
-              "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
-    p->any_subs = p->any_subs || is_subs;
-    *any_audio = *any_audio || !is_subs;
+    const bool is_subs = s.cue_off && s.is_subs && s.is_subs[v];
+    const bool is_pgs = g.off && g.is_pgs && g.is_pgs[v];
+    if (s.cue_off) {
+      if (s.cue_off[v + 1] < s.cue_off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: ref_cue_off not monotone at %d", who, v);
+      if (!is_subs && s.cue_off[v + 1] != s.cue_off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has reference cues but no subtitle reference (ref_is_subs[%d] = 0)",
+                who, v, v);
+      if (is_subs && r.pcm_off[v + 1] != r.pcm_off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has a subtitle reference and a non-empty PCM range (%lld samples); "
+                "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
+    }
+    if (g.off) {
+      if (g.off[v + 1] < g.off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: pgs_off not monotone at %d", who, v);
+      if (!is_pgs && g.off[v + 1] != g.off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has PGS intervals but no PGS reference (ref_is_pgs[%d] = 0)", who,
+                v, v);
+      if (is_pgs && is_subs)
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d is marked both as a PGS and as a text subtitle reference", who, v);
+      if (is_pgs && r.pcm_off[v + 1] != r.pcm_off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has a PGS reference and a non-empty PCM range (%lld samples); "
+                "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
+    }
+    p->any_subs = p->any_subs || is_subs || is_pgs;
+    *any_audio = *any_audio || (!is_subs && !is_pgs);
   }
-  if (r.V > 0 && s.cue_off[r.V] > s.cue_off[0] && (!s.cue_start_s || !s.cue_end_s))
+  if (s.cue_off && r.V > 0 && s.cue_off[r.V] > s.cue_off[0] && (!s.cue_start_s || !s.cue_end_s))
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null reference cue arrays", who);
+  if (g.off && r.V > 0 && g.off[r.V] > g.off[0] && (!g.start_s || !g.end_s))
+    B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null PGS interval arrays", who);
   if (p->audio_samples > 0 && !r.pcm)
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null pcm with %lld samples of audio", who, (long long)p->audio_samples);
   return B2_OK;
@@ -468,15 +572,30 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
   // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
   // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
   // the tracks' cues).  subs_len[v] = -1: the video's reference is the detector's.
+  // PGS references: int(max_end * sample_rate) + 2 frames, the length b2_rasterize_pgs_lengths gives.
   std::vector<int64_t> subs_len;
   if (p->any_subs) {
-    const double one = 1.0;
-    subs_len.resize(V);
-    B2_TRY(cue_lengths(&p->err, who, "reference ", "bad reference cue list", r.refs.cue_start_s, r.refs.cue_end_s,
-                       r.refs.cue_off, V, &one, 1, r.start_seconds, r.sample_rate, subs_len.data()));
-    for (int v = 0; v < V; ++v) {
-      if (r.refs.is_subs[v]) p->sub_video.push_back(v);
-      else subs_len[v] = -1;
+    subs_len.assign(V, -1);
+    const uint8_t* is_subs = r.refs.cue_off ? r.refs.is_subs : nullptr;
+    const uint8_t* is_pgs = r.pgs.off ? r.pgs.is_pgs : nullptr;
+    if (is_subs && std::any_of(is_subs, is_subs + V, [](uint8_t x) { return x != 0; })) {
+      const double one = 1.0;
+      B2_TRY(cue_lengths(&p->err, who, "reference ", "bad reference cue list", r.refs.cue_start_s, r.refs.cue_end_s,
+                         r.refs.cue_off, V, &one, 1, r.start_seconds, r.sample_rate, subs_len.data()));
+      for (int v = 0; v < V; ++v) {
+        if (is_subs[v]) p->sub_video.push_back(v);
+        else subs_len[v] = -1;
+      }
+    }
+    if (is_pgs) {
+      std::vector<int64_t> pgs_len(V);
+      B2_TRY(pgs_lengths(&p->err, who, "PGS ", r.pgs.start_s, r.pgs.end_s, r.pgs.off, V, r.sample_rate, true,
+                         r.start_seconds, is_pgs, pgs_len.data()));
+      for (int v = 0; v < V; ++v)
+        if (is_pgs[v]) {
+          p->pgs_video.push_back(v);
+          subs_len[v] = pgs_len[v];
+        }
     }
   }
   p->ref_off.assign(V + 1, 0);
@@ -503,10 +622,10 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
   p->auditok = r.detector == B2_DETECTOR_AUDITOK;
   if (V < 0 || T < 0 || K <= 0 || !r.pcm_off || !r.cue_off || !r.ratios)
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad arguments", who);
-  bool any_audio = !r.refs.cue_off;
+  bool any_audio = !r.refs.cue_off && !r.pgs.off;
   for (int v = 0; v < V; ++v)
     if (r.pcm_off[v + 1] > r.pcm_off[v]) p->audio_samples += r.pcm_off[v + 1] - r.pcm_off[v];
-  if (r.refs.cue_off) B2_TRY(plan_refs_check(r, p, &any_audio));
+  if (r.refs.cue_off || r.pgs.off) B2_TRY(plan_refs_check(r, p, &any_audio));
   // The run path and the GSS rounds need a reference of the two levels 1.0 and ref_label.  The detector's signal
   // has the levels 1.0 and the label, a subtitle reference 1.0 and 0.0, so ref_label is the label unless every
   // reference is a subtitle stream; a call that mixes the two at a non-zero label has three levels.  auditok's

@@ -637,6 +637,131 @@ class SubtitleSpeechTransformer(TransformerMixin, ComputeSpeechFrameBoundariesMi
         return self.subtitle_speech_results_
 
 
+# ----------------------------------------------------------------------------- PGS (bitmap subtitle) references
+
+
+def _ffprobe_json(fname: str, ffmpeg_path: Optional[str], *args: str) -> dict:
+    """``ffprobe -of json <args> fname`` as a dict, the way ffmpeg.probe runs it (raises on failure)."""
+    import json
+    exe = os.path.join(ffmpeg_path, "ffprobe") if ffmpeg_path else "ffprobe"
+    if shutil.which(exe) is None:
+        raise RuntimeError("no ffprobe binary found")
+    out = subprocess.check_output([exe, "-v", "error", "-of", "json", *args, fname], stderr=subprocess.DEVNULL)
+    return json.loads(out.decode("utf-8", "replace"))
+
+
+_PGS_CODEC = "hdmv_pgs_subtitle"
+# PGS "clear" packets (the end of a caption) carry no image and are about 30 bytes; show packets are larger
+_PGS_CLEAR_PACKET_BYTES = 50
+
+
+def find_pgs_stream(probe: dict) -> Optional[str]:
+    """The ffmpeg stream specifier ("0:s:N") of the first PGS stream in an ffprobe ``streams`` dict, N counting
+    subtitle streams only, or None (the reference's find_pgs_stream after its ffprobe call)."""
+    subtitles = [s for s in probe.get("streams", []) if s.get("codec_type") == "subtitle"]
+    n = next((i for i, s in enumerate(subtitles) if s.get("codec_name") == _PGS_CODEC), None)
+    if n is None:
+        return None
+    logger.info("PGS stream 0:s:%d is ffprobe stream %s", n, subtitles[n].get("index"))
+    return "0:s:%d" % n
+
+
+def _show_interval(packet: dict) -> Optional[Tuple[float, float]]:
+    """(pts, pts + duration) of a PGS show packet; None for a clear packet, an "N/A" duration, a missing field or a
+    value that does not parse."""
+    pts, duration, size = (packet.get(k) for k in ("pts_time", "duration_time", "size"))
+    if pts is None or duration is None or size is None or duration == "N/A":
+        return None
+    try:
+        t0, dt, n_bytes = float(pts), float(duration), int(size)
+    except ValueError:
+        return None
+    return (t0, t0 + dt) if n_bytes > _PGS_CLEAR_PACKET_BYTES else None
+
+
+def pgs_timings_from_packets(probe: dict) -> Optional[List[Tuple[float, float]]]:
+    """The display intervals of the show packets of an ffprobe ``packets`` dict, in packet order, or None when there
+    are none (the reference's _get_pgs_timings_via_ffprobe after its ffprobe call)."""
+    shown = [iv for iv in map(_show_interval, probe.get("packets", [])) if iv is not None]
+    return shown or None
+
+
+class PGSSpeechTransformer(TransformerMixin, ComputeSpeechFrameBoundariesMixin):
+    """``--pgs-ref-stream``: a video's PGS (Blu-ray bitmap) subtitle display intervals as its reference signal
+    (the reference's PGSSpeechTransformer): 1.0 while a caption is shown, 0.0 otherwise, at ``sample_rate``,
+    rasterised by b2_rasterize_pgs.  ``fit`` takes a file name (the stream is ``ref_stream``, with or without its
+    "0:" prefix, or the first PGS stream; its packet timings are read with ffprobe) or a list of (start, end) pairs
+    in seconds.  ``num_frames`` is None: PGS times are in the video's timebase, so no framerate ratio is inferred."""
+
+    @property
+    def num_frames(self) -> None:
+        return None
+
+    def __init__(self, sample_rate: int, start_seconds: int = 0, ffmpeg_path: Optional[str] = None,
+                 ref_stream: Optional[str] = None, gui_mode: bool = False) -> None:
+        ComputeSpeechFrameBoundariesMixin.__init__(self)
+        self.sample_rate, self.start_seconds = sample_rate, start_seconds
+        self.ffmpeg_path, self.ref_stream, self.gui_mode = ffmpeg_path, ref_stream, gui_mode
+        self.pgs_speech_results_: Optional[np.ndarray] = None
+
+    def _given_stream(self) -> Optional[str]:
+        """ref_stream as an input-0 specifier ("s:1" -> "0:s:1"), or None."""
+        s = self.ref_stream
+        return None if s is None else (s if s.startswith("0:") else "0:" + s)
+
+    def _probe_stream(self, fname: str) -> str:
+        stream = self._given_stream()
+        if stream is not None:
+            return stream
+        try:
+            stream = find_pgs_stream(_ffprobe_json(fname, self.ffmpeg_path, "-show_format", "-show_streams"))
+        except Exception as e:   # as the reference: a failed probe is "no PGS stream"
+            logger.warning("ffprobe could not list the streams of %s: %s", fname, e)
+        if stream is None:
+            raise ValueError("No hdmv_pgs_subtitle stream found in {}. "
+                             "Specify one explicitly with --pgs-ref-stream.".format(fname))
+        return stream
+
+    def _probe_intervals(self, fname: str) -> List[Tuple[float, float]]:
+        stream = self._probe_stream(fname)
+        # -select_streams names a stream of the (only) input without the "0:" prefix
+        entries = ("-show_format", "-show_streams", "-show_packets", "-select_streams", stream[2:], "-show_entries",
+                   "packet=pts_time,duration_time,size")
+        try:
+            intervals = pgs_timings_from_packets(_ffprobe_json(fname, self.ffmpeg_path, *entries))
+        except Exception:
+            intervals = None
+        if intervals is None:
+            raise ValueError("Failed to get PGS timings via ffprobe for stream {} from {}. "
+                             "Make sure the stream exists and is an hdmv_pgs_subtitle track "
+                             "(check with: ffprobe -show_streams {}).".format(stream, fname, fname))
+        return intervals
+
+    def fit(self, fname, *_) -> "PGSSpeechTransformer":
+        from_file = isinstance(fname, (str, os.PathLike))
+        intervals = self._probe_intervals(fname) if from_file else list(fname)
+        if not intervals:
+            given = self._given_stream()
+            raise ValueError("No subtitle timings found in PGS stream {}.".format(given) if given is not None
+                             else "No subtitle timings found in the PGS intervals given.")
+        t = np.asarray(intervals, dtype=np.float64).reshape(-1, 2)
+        try:
+            out, _ = _native.get_handle().rasterize_pgs(t[:, 0], t[:, 1], [0, len(t)], self.sample_rate,
+                                                         float(self.start_seconds))
+        except _native.NativeError as e:
+            if e.status != -1:   # B2_ERR_BAD_ARG: times the reference's round / int / np.zeros raise ValueError for
+                raise
+            raise ValueError(str(e)) from None
+        self.pgs_speech_results_ = out.astype(np.float64)
+        self.fit_boundaries(self.pgs_speech_results_)
+        logger.info("PGS reference: %d intervals, %d frames on screen", len(t), int(np.sum(out)))
+        return self
+
+    def transform(self, *_) -> np.ndarray:
+        assert self.pgs_speech_results_ is not None
+        return self.pgs_speech_results_
+
+
 class DeserializeSpeechTransformer(TransformerMixin):
     def __init__(self, non_speech_label: float) -> None:
         self._non_speech_label: float = non_speech_label

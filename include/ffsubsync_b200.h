@@ -152,6 +152,23 @@ int b2_rasterize(b2_handle h, const double* cue_start_s, const double* cue_end_s
                  const double* levels /* or NULL */, int sample_rate, double start_seconds,
                  float* out, const int64_t* out_off /* [B*K+1] */, int memspace);
 
+/* ---- PGSSpeechTransformer.fit: bitmap-subtitle (PGS) display intervals -> 100 Hz speech signal ---------------
+ * ffsubsync/speech_transformers.py:1186-1198, for B interval lists (list b: off[b] .. off[b+1], seconds as ffprobe's
+ * pts_time and pts_time + duration_time).  Not the text rule of b2_rasterize: raw float64 times, each end rounded on
+ * its own, s = int(round((t - start_seconds) * sample_rate)) (half to even), signal length
+ * int(max_end * sample_rate) + 2 (truncation toward zero, no max(0, .)), and an interval fills [max(s0, 0),
+ * min(s1, n)) with 1.0 when that is not empty (intervals may overlap, be unsorted or have a negative duration).
+ * b2_rasterize_pgs_lengths (host) gives the lengths; b2_rasterize_pgs writes signal b at out + out_off[b] (out_off
+ * [B+1], normally the cumulative lengths; the n of the clamp is out_off[b+1] - out_off[b]), out following memspace.
+ * B2_ERR_BAD_ARG (the message names the list or interval) for an empty list (the reference raises ValueError), a
+ * non-finite time, |t| >= B2_MAX_CUE_SECONDS, a negative length (np.zeros raises), a non-monotone off, sample_rate
+ * outside (0, 2^28] or |start_seconds| >= B2_MAX_CUE_SECONDS.  b2_rasterize_pgs_lengths reads only end times. */
+int b2_rasterize_pgs_lengths(const double* end_s, const int64_t* off /* [B+1] */, int B, int sample_rate,
+                             int64_t* lengths /* [B] */);
+int b2_rasterize_pgs(b2_handle h, const double* start_s, const double* end_s, const int64_t* off /* [B+1] */, int B,
+                     int sample_rate, double start_seconds, float* out, const int64_t* out_off /* [B+1] */,
+                     int memspace);
+
 /* ---- fused-VAD blend ------------------------------------------------------------------------
  * ffsubsync/speech_transformers.py:281-294 (_make_fused_detector._detect): two detector outputs
  * clipped to their common length n and combined element-wise.
@@ -309,6 +326,40 @@ int b2_sync_tracks_subs(b2_handle h, const int16_t* pcm /* or NULL without audio
                         double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
                         double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                         int memspace);
+
+/* ---- PGS subtitle timings as references (--pgs-ref-stream) ------------------------------------------------
+ * `ffs movie.mkv -i a.srt ... --pgs-ref-stream [S]` for V videos and T tracks: a video with a PGS (hdmv_pgs_subtitle)
+ * stream is synced against that stream's display intervals rasterised (PGSSpeechTransformer, ffsubsync/ffsubsync.py:
+ * 307-327), any other video as in b2_sync_tracks_subs.  Running ffprobe and choosing the stream are the caller's.
+ * Arguments as for b2_sync_tracks_subs (ref_is_subs and ref_cue_* may be NULL: no text references), plus:
+ *   ref_is_pgs [V]       non-zero: video v has a PGS reference.  NULL = none.
+ *   pgs_start_s, pgs_end_s, pgs_off [V+1]
+ *                        host arrays: video v's intervals are pgs_off[v] .. pgs_off[v+1] (seconds: pts_time and
+ *                        pts_time + duration_time).  A video without a PGS reference has an empty list.
+ * Track t gets exactly what this composition of public calls returns: the reference of video track_video[t] -
+ * b2_rasterize_pgs of its intervals for a PGS video, what b2_sync_tracks_subs uses otherwise - then b2_align_batch
+ * and b2_reduce_ratios over the ratios, plus the golden-section search's candidate as in b2_sync_tracks_gss when
+ * gss_ratio is not NULL.  The PGS reference has no inferred framerate ratio: the grid is the caller's.
+ * A PGS reference counts as a subtitle reference for the rules of b2_sync_tracks_subs: levels 1.0 and 0.0, an empty
+ * PCM range, and the same label / path / B2_ERR_UNSUPPORTED rules.  B2_ERR_BAD_ARG also for the errors of
+ * b2_rasterize_pgs, a PGS video with a non-empty PCM range, a video marked both PGS and text, intervals given for a
+ * video without ref_is_pgs and a non-monotone pgs_off.  Without PGS videos the call returns what b2_sync_tracks_subs
+ * returns.  memspace: B2_HOST, B2_DEVICE or B2_DEVICE_RESIDENT; resident calls chain with the other sync calls in any
+ * order. */
+int b2_sync_tracks_pgs(b2_handle h, const int16_t* pcm /* or NULL without audio */, const int64_t* pcm_off /* [V+1] */,
+                       int V, const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                       int detector, double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                       double energy_threshold_db, double min_length, int64_t max_length,
+                       double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs /* [V] */,
+                       const double* ref_cue_start_s, const double* ref_cue_end_s, const uint8_t* ref_cue_keep,
+                       const int64_t* ref_cue_off /* [V+1] or NULL */, const uint8_t* ref_is_pgs /* [V] */,
+                       const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off /* [V+1] */,
+                       const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                       const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                       int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                       double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                       double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                       int memspace);
 
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
