@@ -30,7 +30,7 @@ EXPORTS = [
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
-    "b2_sync_tracks_pgs",
+    "b2_sync_tracks_pgs", "b2_capture_reference",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
@@ -123,6 +123,7 @@ def load() -> ctypes.CDLL:
         lib.b2_vad_auditok.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _f64, _f64,
                                        _f64, _i64, _f64, _i64, _vp, _vp, ctypes.c_int]
         lib.b2_capture_nominations.argtypes = [_vp, _vp, _i64, _vp, _vp, _vp]
+        lib.b2_capture_reference.argtypes = [_vp, _vp, _i64, _vp, _vp, _i64]
         _lib = lib
         return lib
 
@@ -629,6 +630,29 @@ class Handle:
             self._check(self.lib.b2_capture_nominations(self.h, None, 0, None, None, None), "b2_capture_nominations")
             self.synchronize()
             out.update({k: v.cpu().numpy() for k, v in t.items()})
+
+    @contextlib.contextmanager
+    def capture_reference(self, capacity: int, max_videos: int):
+        """While the block runs, every batched sync call on this handle copies its reference signals into a
+        NaN-filled device array of `capacity` floats (b2_capture_reference); the last call's copy is kept.  Yields a
+        dict that holds numpy arrays once the block has exited: ref float32[capacity], ref_off int64[max_videos + 1]
+        and packed uint8[max_videos] (1: the video's range starts with ceil(R/32) words of packed bits; read
+        ref[...].view(np.uint32)).  ref_off is -1 and packed 255 where no call wrote."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        ref = torch.full((max(int(capacity), 1),), float("nan"), dtype=torch.float32, device=dev)
+        ref_off = np.full(int(max_videos) + 1, -1, dtype=np.int64)
+        packed = np.full(max(int(max_videos), 1), 255, dtype=np.uint8)
+        torch.cuda.synchronize(dev)   # the fill runs on torch's stream, the copies on the handle's
+        self._check(self.lib.b2_capture_reference(self.h, ref.data_ptr(), int(capacity), _ptr(ref_off), _ptr(packed),
+                                                  int(max_videos)), "b2_capture_reference")
+        out = {}
+        try:
+            yield out
+        finally:
+            self._check(self.lib.b2_capture_reference(self.h, None, 0, None, None, 0), "b2_capture_reference")
+            self.synchronize()
+            out.update(ref=ref.cpu().numpy()[: int(capacity)], ref_off=ref_off, packed=packed[: int(max_videos)])
 
 
 def _default_device() -> int:

@@ -828,6 +828,18 @@ extern "C" int b2_capture_nominations(b2_handle h, float* scores, int64_t stride
   return B2_OK;
 }
 
+extern "C" int b2_capture_reference(b2_handle h, float* ref, int64_t capacity, int64_t* ref_off, uint8_t* packed,
+                                    int64_t max_videos) {
+  B2_ENTER(h);
+  h->ref_capture = B2RefCapture{};
+  if (!ref) return B2_OK;
+  if (capacity < 0 || max_videos < 0 || !ref_off || !packed)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "capture_reference: bad arguments");
+  B2_TRY(check_device_ptr(h, ref, "capture_reference: ref"));
+  h->ref_capture = B2RefCapture{ref, (long long)capacity, ref_off, packed, (long long)max_videos};
+  return B2_OK;
+}
+
 extern "C" int b2_reduce_ratios(b2_handle h, const double* score, const int32_t* offset,
                                 const int32_t* status, int B, int K, int64_t max_offset_samples,
                                 double* best_score, int32_t* best_offset, int32_t* best_k,
@@ -1076,6 +1088,10 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   }
   const int T = r.T, K = r.K;
   if (T == 0) return B2_OK;
+  const B2RefCapture rc = h->ref_capture;
+  if (rc.ref && (p.ref_off[r.V] > rc.capacity || r.V > rc.max_videos))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: the reference capture holds %lld frames of %lld videos, the call has %lld of %d",
+            r.who, rc.capacity, rc.max_videos, (long long)p.ref_off[r.V], r.V);
   const bool resident = r.memspace == B2_DEVICE_RESIDENT;
   const int memspace = resident ? B2_DEVICE : r.memspace;
   // every bulk pointer of a B2_DEVICE call, before anything is launched
@@ -1149,6 +1165,17 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   b.winner_only = (!r.all_score && !r.all_offset) ? 1 : 0;
   B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
+  // The reference capture: one copy behind every chain on the caller's stream, when every detector step is done.
+  // The buffer stays valid until then: no chain kernel writes it (they read it as const), the next chained
+  // resident call writes the other buffer, and the call after that starts its detector behind a fence recorded
+  // on this stream after the copy.
+  if (rc.ref) {
+    for (int v = 0; v <= r.V; ++v) rc.ref_off[v] = p.ref_off[v];
+    for (int i = 0; i < p.n_sub; ++i)
+      for (int v = p.cut[i]; v < p.cut[i + 1]; ++v) rc.packed[v] = p.ref_packed[i];
+    if (p.ref_off[r.V] > 0)
+      B2_CUDA(h, cudaMemcpyAsync(rc.ref, b.refsig, (size_t)p.ref_off[r.V] * 4, cudaMemcpyDeviceToDevice, h->stream));
+  }
   if (dev) return B2_OK;
   B2_TRY(copy_out(h, r.best_score, d_bs, (size_t)T * 8));
   B2_TRY(copy_out(h, r.best_offset, d_bo, (size_t)T * 4));

@@ -40,6 +40,16 @@ struct B2Capture {
   int* cand = nullptr;
 };
 
+// b2_capture_reference: where the batched sync calls copy their reference-signal buffer.  Unlike B2Capture it
+// is read only after the call's plan is made and its launches are enqueued, so it changes neither.
+struct B2RefCapture {
+  float* ref = nullptr;       // device, `capacity` floats; nullptr: capture off
+  long long capacity = 0;
+  int64_t* ref_off = nullptr; // host, max_videos + 1 entries
+  uint8_t* packed = nullptr;  // host, max_videos entries
+  long long max_videos = 0;
+};
+
 struct b2_ctx {
   int device = 0;
   int sm_count = 132;
@@ -50,6 +60,7 @@ struct b2_ctx {
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
   int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
   B2Capture capture;             // set by b2_capture_nominations (tests)
+  B2RefCapture ref_capture;      // set by b2_capture_reference (tests)
   // B2_DEVICE_RESIDENT chaining of b2_sync_batch calls (api.cu): `resident_fence` is recorded on the caller's
   // stream before the LAST sub-batch's correlation chain of a pipelined call, `resident_done` after it; the
   // next resident call (if no other entry point ran in between: `resident_fence_valid`) starts its VAD behind

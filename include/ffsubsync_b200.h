@@ -382,6 +382,23 @@ int b2_sync_tracks_pgs(b2_handle h, const int16_t* pcm /* or NULL without audio 
 int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* win, float* stat,
                            int32_t* cand);
 
+/* ---- diagnostics for tests: the batched sync calls' reference signals ------------------------
+ * Exposes the per-video reference signal a batched sync call (b2_sync_batch, b2_sync_tracks, _gss, _auditok,
+ * _subs, _pgs) builds in its detector step - the detector's output, the tokenised auditok signal or a rasterised
+ * subtitle / PGS reference, ffsubsync/speech_transformers.py's VideoSpeechTransformer.fit output.  While set, every
+ * such call with at least one track writes, overwriting the previous call's:
+ *   ref[0 .. ref_off[V])  its reference buffer (DEVICE array; one device-to-device copy on the handle's stream after
+ *                         the call's last kernel).  Video v's signal is ref[ref_off[v] .. ref_off[v+1]) as float32,
+ *                         or, when packed[v] is set, ceil(R/32) uint32 words of bits m = (r == 1.0f) from ref_off[v]
+ *                         on (R = ref_off[v+1] - ref_off[v]; zero bits past R; the rest of the range is not the
+ *                         signal's).
+ *   ref_off[0 .. V]       HOST array: the call's per-video offsets.
+ *   packed[0 .. V-1]      HOST array: 1 where the video's sub-batch got packed words, else 0.
+ * A call needing more than `capacity` floats or `max_videos` videos fails with B2_ERR_BAD_ARG before anything is
+ * enqueued.  The capture changes nothing the call plans, launches or returns.  ref == NULL clears the capture. */
+int b2_capture_reference(b2_handle h, float* ref, int64_t capacity, int64_t* ref_off, uint8_t* packed,
+                         int64_t max_videos);
+
 /* ---- synthetic PCM (bench / tests): counter-hash generator replayable in numpy -------------
  * oracle/vad_oracle.py:synth_pcm.  window_class: uint8 per 10 ms window (0 silence, 1 voiced,
  * 2 loud hiss), device or host per memspace; writes n_windows*fpw int16 samples. */

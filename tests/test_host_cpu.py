@@ -81,8 +81,12 @@ def test_no_cpu_fallback_without_gpu(built):
     with pytest.raises(_native.NativeError):
         with _native.get_handle().capture_nominations(1, 16):
             pass
+    with pytest.raises(_native.NativeError):
+        with _native.get_handle().capture_reference(16, 1):
+            pass
     # the entry point itself refuses a handle-less call instead of recording anything
     assert _native.load().b2_capture_nominations(None, None, 0, None, None, None) == -1
+    assert _native.load().b2_capture_reference(None, None, 0, None, None, 0) == -1
     src = open(os.path.join(ROOT, "ffsubsync_b200", "aligners.py")).read() + \
         open(os.path.join(ROOT, "ffsubsync_b200", "speech_transformers.py")).read() + \
         open(os.path.join(ROOT, "ffsubsync_b200", "_native.py")).read()
