@@ -30,9 +30,10 @@ EXPORTS = [
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
-    "b2_sync_tracks_pgs", "b2_capture_reference",
+    "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
+B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
 
 
@@ -110,6 +111,11 @@ def load() -> ctypes.CDLL:
                                            _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                            _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                            ctypes.c_int]
+        lib.b2_sync_tracks_sig.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_int, _f64, _i64, ctypes.c_int, ctypes.c_int, _f64, _f64, _i64,
+                                           _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                           _vp, _vp, _vp, _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp,
+                                           _vp, _vp, ctypes.c_int]
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -601,6 +607,53 @@ class Handle:
                            int(z_lo), int(z_hi), float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
                            _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
                            _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off)),
+                          cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
+                          (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
+                          memspace, gss=bool(gss), want_evals=want_evals)
+
+    def sync_tracks_sig(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
+                        ref_is_sig, x, sig_off, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds: float,
+                        max_offset_samples: Optional[int], ref_is_subs=None, ref_cue_start_s=None, ref_cue_end_s=None,
+                        ref_cue_keep=None, ref_cue_off=None, ref_is_pgs=None, pgs_start_s=None, pgs_end_s=None,
+                        pgs_off=None, detector: int = B2_DETECTOR_ENERGY_ZCR, energy_threshold: int = 0,
+                        z_lo: int = -1, z_hi: int = -1, chunk_samples: int = 0, energy_threshold_db: float = 50.0,
+                        min_length: Optional[float] = None, max_length: Optional[int] = None,
+                        max_continuous_silence: Optional[float] = None, gss: bool = False, best_score=None,
+                        best_offset=None, best_k=None, all_score=None, all_offset=None, gss_ratio=None, gss_evals=None,
+                        want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST):
+        """sync_tracks_pgs where the videos with ref_is_sig[v] != 0 take their serialized speech signal (the float64
+        values x[sig_off[v] .. sig_off[v+1]), frame (float)(x < 1.0 ? non_speech_label : x)) as reference signal
+        (b2_sync_tracks_sig).  x: a float64 numpy array under B2_HOST, a device pointer otherwise; sig_off: host.
+        The text and PGS references are optional.  A video whose signal holds a value > 1.0 or NaN gets best_k =
+        B2_BEST_K_BAD_SIGNAL on every track.  Returns as sync_tracks_subs."""
+        V, T = len(pcm_off) - 1, len(track_video)
+        sig_off = _i64a(sig_off)
+        if len(cue_off) != T + 1 or len(sig_off) != V + 1:
+            raise NativeError(-1, "b2_sync_tracks_sig", "cue_off / sig_off have %d / %d entries for %d tracks / "
+                              "%d videos" % (len(cue_off), len(sig_off), T, V))
+        u8 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.uint8)   # noqa: E731
+        ref_is_sig, ref_is_pgs, ref_is_subs = u8(ref_is_sig), u8(ref_is_pgs), u8(ref_is_subs)
+        for name, a in (("ref_is_sig", ref_is_sig), ("ref_is_pgs", ref_is_pgs), ("ref_is_subs", ref_is_subs)):
+            if a is not None and len(a) != V:
+                raise NativeError(-1, "b2_sync_tracks_sig", "%s has %d entries for %d videos" % (name, len(a), V))
+        for name, off in (("ref_cue_off", ref_cue_off), ("pgs_off", pgs_off)):
+            if off is not None and len(off) != V + 1:
+                raise NativeError(-1, "b2_sync_tracks_sig", "%s has %d entries for %d videos" % (name, len(off), V))
+        ref_cue_off = None if ref_cue_off is None else _i64a(ref_cue_off)
+        pgs_off = None if pgs_off is None else _i64a(pgs_off)
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)   # noqa: E731
+        if x is not None and not isinstance(x, int):
+            x = f64(x)
+        pgs_start_s, pgs_end_s = f64(pgs_start_s), f64(pgs_end_s)
+        ref_cue_start_s, ref_cue_end_s = f64(ref_cue_start_s), f64(ref_cue_end_s)
+        ref_cue_keep = u8(ref_cue_keep)
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        return self._sync("b2_sync_tracks_sig", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, int(detector), float(non_speech_label), int(energy_threshold),
+                           int(z_lo), int(z_hi), float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
+                           _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
+                           _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off),
+                           _ptr(ref_is_sig), _ptr(x), _ptr(sig_off)),
                           cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
                           (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
                           memspace, gss=bool(gss), want_evals=want_evals)

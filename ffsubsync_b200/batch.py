@@ -19,12 +19,19 @@ from .constants import (BATCH_VADS, DEFAULT_ENERGY_THRESHOLD, DEFAULT_MAX_OFFSET
                         detector_chunk_bytes)
 
 
-def load_serialized_speech(paths, non_speech_label: float = 0.0):
+def load_serialized_speech(paths, non_speech_label: float = 0.0, stored: bool = False):
     """Batch ingest of ``--serialize-speech`` / ``--make-test-case`` artefacts (``.npz`` with key
     "speech", or ``.npy``): each file goes through DeserializeSpeechTransformer
     (ffsubsync/speech_transformers.py:987-1009: values < 1 become ``non_speech_label``).
-    Returns (signals float32 back to back, offsets int64[B+1]) ready for ``sync_signals``."""
-    from .speech_transformers import DeserializeSpeechTransformer
+    Returns (signals float32 back to back, offsets int64[B+1]) ready for ``sync_signals``.
+    stored=True: the stored values themselves as float64, back to back, without the rule (non_speech_label is not
+    read), ready for the ``sig`` / ``sig_off`` arguments of the sync methods, which apply the rule at their own
+    label."""
+    from .speech_transformers import DeserializeSpeechTransformer, load_stored_speech
+    if stored:
+        sigs = [np.asarray(load_stored_speech(p), dtype=np.float64).ravel() for p in paths]
+        off = np.concatenate([[0], np.cumsum([len(s) for s in sigs])]).astype(np.int64)
+        return (np.concatenate(sigs) if sigs else np.zeros(0, np.float64)), off
     sigs = [np.asarray(DeserializeSpeechTransformer(non_speech_label).fit(p).transform(), dtype=np.float32)
             for p in paths]
     off = np.concatenate([[0], np.cumsum([len(s) for s in sigs])]).astype(np.int64)
@@ -35,6 +42,8 @@ def load_serialized_speech(paths, non_speech_label: float = 0.0):
 _STREAM_ARGS = ("ref_cue_start", "ref_cue_end", "ref_cue_off", "ref_stream_video", "ref_cue_content", "ref_cue_keep")
 # keyword arguments of the sync methods that describe the videos' PGS (bitmap subtitle) display intervals
 _PGS_ARGS = ("pgs_start", "pgs_end", "pgs_off", "pgs_video")
+# keyword arguments of the sync methods that give videos a serialized speech signal as reference
+_SIG_ARGS = ("sig", "sig_off", "sig_video")
 
 
 def _is_unsupported(e: Exception) -> bool:
@@ -72,7 +81,18 @@ class BatchSynchronizer:
     ``pgs_off`` [P+1] and ``pgs_video`` [P] (increasing: at most one interval list per video).  Such a video is synced
     against its intervals rasterised by PGSSpeechTransformer's rule (b2_rasterize_pgs) instead of its audio or text
     stream - the reference tries ``--pgs-ref-stream`` first - and must have an empty PCM range.  Running ffprobe
-    stays the caller's job."""
+    stays the caller's job.
+
+    Serialized speech signals (``ffs ref.npz -i in.srt``, with every ``vad``): the sync methods also take the stored
+    values of P videos' ``--serialize-speech`` / ``--make-test-case`` signals as keyword arguments ``sig`` (the values
+    back to back, e.g. ``load_serialized_speech(paths, stored=True)``: a numpy array for the host methods, a CUDA
+    tensor for the device ones; other dtypes are converted to float64), ``sig_off`` [P+1] and ``sig_video`` [P]
+    (increasing: one signal per video).  Such a video is synced against its signal by DeserializeSpeechTransformer's
+    rule at this synchroniser's ``non_speech_label``, frame ``(float)(x < 1.0 ? non_speech_label : x)`` - no detector
+    runs for it - and must have an empty PCM range and no text or PGS reference.  Every stored value must be < 1.0 or
+    exactly 1.0: a video with a value > 1.0 or NaN gets ``best_k == -2`` (``_native.B2_BEST_K_BAD_SIGNAL``), NaN
+    scores and offsets 0 on all its tracks from the device methods, and the host methods raise ValueError naming the
+    video and its first such frame."""
 
     def __init__(self, ratios: Sequence[Optional[float]], frame_rate: int = 16000, sample_rate: int = SAMPLE_RATE,
                  non_speech_label: float = 0.0, energy_threshold: int = DEFAULT_ENERGY_THRESHOLD,
@@ -126,6 +146,83 @@ class BatchSynchronizer:
         return ((keep_v.astype(np.uint8), rs[pick], re_[pick], None if rk is None else rk[pick],
                  np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)), pgs)
 
+    def _all_refs(self, V: int, streams: dict, on_device: bool):
+        """(refs, pgs, sig) of the keyword arguments: refs and pgs from _references, sig from _sig_refs.  A video with
+        a signal and a text or PGS reference is refused: the reference tool's reference is a single file."""
+        sig = self._sig_refs(V, {k: streams.pop(k) for k in _SIG_ARGS if k in streams}, on_device)
+        refs, pgs = self._references(V, streams)
+        if sig is not None:
+            other = np.zeros(V, dtype=bool)
+            for r in (refs, pgs):
+                if r is not None:
+                    other |= r[0] != 0
+            both = np.flatnonzero(other & (sig[0] != 0))
+            if len(both):
+                raise ValueError("video %d has a serialized signal and a text / PGS reference; a video has one "
+                                 "reference" % int(both[0]))
+        return refs, pgs, sig
+
+    def _sig_refs(self, V: int, args: dict, on_device: bool):
+        """Each video's stored signal, or None when none is given: returns (ref_is_sig u8[V], x float64, sig_off
+        int64[V+1]) for b2_sync_tracks_sig, x a numpy array (on_device False) or a CUDA tensor on the handle's device,
+        sig_off absolute into x."""
+        if all(args.get(k) is None for k in _SIG_ARGS):
+            return None
+        missing = [k for k in _SIG_ARGS if args.get(k) is None]
+        if missing:
+            raise ValueError("signal references need %s" % ", ".join(_SIG_ARGS))
+        off = np.ascontiguousarray(args["sig_off"], dtype=np.int64)
+        video = np.ascontiguousarray(args["sig_video"], dtype=np.int64)
+        P = len(off) - 1
+        if len(video) != P:
+            raise ValueError("sig_video has %d entries for %d signals" % (len(video), P))
+        if P and (np.any(np.diff(video) <= 0) or video[0] < 0 or video[-1] >= V):
+            raise ValueError("sig_video must be increasing video indices in [0, %d) (one signal per video)" % V)
+        x = args["sig"]
+        if on_device:
+            import torch
+            dev = torch.device("cuda", self.handle.device)
+            x = torch.as_tensor(x).to(device=dev, dtype=torch.float64).contiguous()
+        else:
+            x = np.ascontiguousarray(x.cpu().numpy() if hasattr(x, "cpu") else x, dtype=np.float64)
+        if x.ndim != 1:
+            raise ValueError("sig must be one-dimensional (the signals back to back)")
+        if np.any(np.diff(off) < 0) or (P and (off[0] < 0 or off[-1] > len(x))):
+            raise ValueError("sig_off must be non-decreasing and within sig")
+        is_sig = np.zeros(V, dtype=np.uint8)
+        is_sig[video] = 1
+        # video v's range in x: its signal's, or an empty one where the previous range ended
+        voff = np.empty(V + 1, dtype=np.int64)
+        pos, i = (int(off[0]) if P else 0), 0
+        for v in range(V):
+            voff[v] = pos
+            if i < P and video[i] == v:
+                voff[v], pos = off[i], off[i + 1]
+                i += 1
+        voff[V] = pos
+        return is_sig, x, voff
+
+    @staticmethod
+    def _bad_signals(sig):
+        """{video: first frame} of the signal videos with a stored value > 1.0 or NaN (sig from _sig_refs)."""
+        is_sig, x, voff = sig
+        x = x.cpu().numpy() if hasattr(x, "cpu") else x
+        bad = {}
+        for v in np.flatnonzero(is_sig):
+            out = np.flatnonzero(~(x[voff[v]: voff[v + 1]] <= 1.0))
+            if len(out):
+                bad[int(v)] = int(out[0])
+        return bad
+
+    def _raise_bad_signals(self, sig, best_k) -> None:
+        """The host methods' error for the sentinel best_k == B2_BEST_K_BAD_SIGNAL."""
+        if sig is None or not np.any(np.asarray(best_k) == _native.B2_BEST_K_BAD_SIGNAL):
+            return
+        v, f = sorted(self._bad_signals(sig).items())[0]
+        x = sig[1]
+        raise ValueError("video %d: its serialized signal holds %r at frame %d; stored values must be < 1.0 or "
+                         "exactly 1.0" % (v, float(x[int(sig[2][v]) + f]), f))
+
     def _pgs_refs(self, V: int, args: dict):
         """Each video's PGS interval list, or None when none is given: returns (ref_is_pgs u8[V], pgs_start,
         pgs_end, pgs_off [V+1]) for b2_sync_tracks_pgs."""
@@ -172,15 +269,28 @@ class BatchSynchronizer:
                                         content=streams.get("ref_cue_content"), keep=streams.get("ref_cue_keep"))
 
     def _dispatch(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, pgs=None,
-                  **kw):
+                  sig=None, **kw):
         """The batched call of this synchroniser's detector with the search on or off: b2_sync_tracks_pgs with PGS
         references (pgs, from _pgs_refs), else b2_sync_tracks_subs with subtitle references (refs, from _subs_refs), else b2_sync_tracks_auditok for auditok, else
-        b2_sync_tracks_gss / b2_sync_tracks.  pcm: int16 numpy array, CUDA tensor or None; kw: the outputs (device
+        b2_sync_tracks_gss / b2_sync_tracks; b2_sync_tracks_sig with signal references (sig, from _sig_refs, with
+        any of the others).  pcm: int16 numpy array, CUDA tensor or None; kw: the outputs (device
         pointers) or want_all, and memspace.  Returns (best_score, best_offset, best_k, all_score, all_offset), plus
         (gss_ratio, gss_evals) with gss."""
         h = self.handle
         p = pcm if pcm is None or isinstance(pcm, np.ndarray) else pcm.data_ptr()
         cues = (cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples)
+        if sig is not None:
+            det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
+            is_sig, x, voff = sig
+            other = {} if refs is None else dict(zip(("ref_is_subs", "ref_cue_start_s", "ref_cue_end_s",
+                                                      "ref_cue_keep", "ref_cue_off"), refs))
+            if pgs is not None:
+                other.update(zip(("ref_is_pgs", "pgs_start_s", "pgs_end_s", "pgs_off"), pgs))
+            xp = x if isinstance(x, np.ndarray) else (x.data_ptr() if x.numel() else None)
+            return h.sync_tracks_sig(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                     self.non_speech_label, is_sig, xp, voff, *cues, detector=det,
+                                     energy_threshold=self.energy_threshold, z_lo=self.z_lo, z_hi=self.z_hi,
+                                     chunk_samples=self.chunk_samples, gss=gss, **other, **kw)
         if pgs is not None:
             det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
             text = {} if refs is None else dict(zip(("ref_is_subs", "ref_cue_start_s", "ref_cue_end_s", "ref_cue_keep",
@@ -202,20 +312,20 @@ class BatchSynchronizer:
         return (h.sync_tracks_gss if gss else h.sync_tracks)(p, pcm_off, track_video, *energy, *cues, **kw)
 
     def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=None,
-                         **kw):
+                         sig=None, **kw):
         """_dispatch with this synchroniser's search.  Outside the envelope of the device-driven search
         (B2_ERR_UNSUPPORTED) the search is composed of public steps instead (_gss_compose).  Returns
         (best_score, best_offset, best_k, all_score, all_offset), plus gss_ratio with the search; composed results
         are numpy arrays (all_* None unless want_all or device outputs were given)."""
         try:
             return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
-                                  pgs=pgs, **kw)[:6]
+                                  pgs=pgs, sig=sig, **kw)[:6]
         except _native.NativeError as e:
             if not (self.gss and _is_unsupported(e)):
                 raise
         want_all = kw.get("want_all", False) or kw.get("all_score") is not None
         bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off,
-                                                        cue_keep, want_all=want_all, refs=refs, pgs=pgs)
+                                                        cue_keep, want_all=want_all, refs=refs, pgs=pgs, sig=sig)
         return bs, bo, bk, a_s, a_o, ratio
 
     def use_torch_stream(self) -> None:
@@ -233,11 +343,13 @@ class BatchSynchronizer:
         overlap: the VAD of this batch starts while the last correlation chain of the previous batch is
         still running.  Results are identical; outputs stay ordered on the stream.
         With a ``subs_then_`` detector the embedded subtitle streams come as keyword arguments, and with any detector
-        the PGS references (see the class)."""
+        the PGS references and the serialized signals (see the class); with inputs_resident the promise covers
+        ``sig`` too."""
         import torch
         B = len(pcm_off) - 1
         K = len(self.ratios)
-        if self.gss or self.auditok or self.subs_then or any(streams.get(k) is not None for k in _PGS_ARGS):   # the identity track map: pair b is track b of video b
+        if (self.gss or self.auditok or self.subs_then
+                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS)):   # the identity track map: pair b is track b of video b
             return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
                                            cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident,
                                            **streams)
@@ -270,10 +382,12 @@ class BatchSynchronizer:
         With the golden-section search (a trailing None in ratios) out also holds gss_ratio f64[T] and all_out
         is {"score": f64[T*(K+1)], "offset": i32[T*(K+1)]} with column K the search's candidate.
         streams: the embedded subtitle streams of a ``subs_then_`` detector (ref_cue_start, ... - see the class) and
-        the PGS references (pgs_start, pgs_end, pgs_off, pgs_video)."""
+        the PGS references (pgs_start, pgs_end, pgs_off, pgs_video) and the serialized signals (sig, sig_off,
+        sig_video; a float64 CUDA tensor keeps the call asynchronous, other inputs are converted first)."""
         import torch
         T = len(track_video)
-        refs, pgs = self._references(len(pcm_off) - 1, streams)
+        sig_in = streams.get("sig")
+        refs, pgs, sig = self._all_refs(len(pcm_off) - 1, streams, on_device=True)
         dev = pcm.device if pcm is not None else torch.device("cuda", self.handle.device)
         if out is None:
             out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
@@ -286,8 +400,13 @@ class BatchSynchronizer:
         ptrs = {k: out[k].data_ptr() for k in keys}
         if all_out:
             ptrs.update(all_score=all_out["score"].data_ptr(), all_offset=all_out["offset"].data_ptr())
+        if sig is not None and sig[1] is not sig_in:
+            # a converted copy: ready before the handle's stream reads it, and kept until the call is done
+            torch.cuda.current_stream(sig[1].device).synchronize()
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    memspace=memspace, **ptrs)
+                                    sig=sig, memspace=memspace, **ptrs)
+        if sig is not None and sig[1] is not sig_in:
+            self.handle.synchronize()
         if isinstance(res[0], np.ndarray):   # composed on the host
             for k, v in zip(keys, res[:3] + res[5:]):
                 out[k].copy_(torch.from_numpy(v))
@@ -301,9 +420,10 @@ class BatchSynchronizer:
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
         track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks."""
-        refs, pgs = self._references(len(pcm_off) - 1, streams)
+        refs, pgs, sig = self._all_refs(len(pcm_off) - 1, streams, on_device=False)
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    want_all=want_all, memspace=_native.B2_HOST)
+                                    sig=sig, want_all=want_all, memspace=_native.B2_HOST)
+        self._raise_bad_signals(sig, res[2])
         return res if want_all else res[:3] + res[5:]
 
     def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None):
@@ -368,9 +488,13 @@ class BatchSynchronizer:
         if self.subs_then:
             raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
                              "embedded subtitle references (vad=%r)" % self.vad)
-        unknown = set(pgs_args) - set(_PGS_ARGS)
+        unknown = set(pgs_args) - set(_PGS_ARGS + _SIG_ARGS)
         if unknown:
             raise TypeError("unexpected keyword arguments %s" % ", ".join(sorted(unknown)))
+        given_sig = sorted(k for k in _SIG_ARGS if pgs_args.get(k) is not None)
+        if given_sig:
+            raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
+                             "serialized signal references (%s)" % ", ".join(given_sig))
         if any(v is not None for v in pgs_args.values()):
             raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
                              "PGS references (%s)" % ", ".join(sorted(pgs_args)))
@@ -423,8 +547,9 @@ class BatchSynchronizer:
         """pcm: int16 numpy array (ideally backed by pinned memory).  Blocks until results are on
         the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]), and gss_ratio last
         with the golden-section search.  With a ``subs_then_`` detector the embedded subtitle streams come as
-        keyword arguments, and with any detector the PGS references (see the class)."""
-        if self.gss or self.auditok or self.subs_then or any(streams.get(k) is not None for k in _PGS_ARGS):
+        keyword arguments, and with any detector the PGS references and the serialized signals (see the class)."""
+        if (self.gss or self.auditok or self.subs_then
+                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS)):
             return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
                                          cue_end, cue_off, cue_keep, want_all=want_all, **streams)
         self._references(len(pcm_off) - 1, streams)   # rejects streams and unknown keywords
@@ -435,12 +560,13 @@ class BatchSynchronizer:
         return res if want_all else res[:3]
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
-                     refs=None, pgs=None):
+                     refs=None, pgs=None, sig=None):
         """The golden-section search outside the envelope of the device-driven search, composed of public steps:
         the grid (this synchroniser's batched call with the search off), gss_align_batch on each track's reference
         signal (_reference_signals, with subtitle references refs from _subs_refs) and the reference's combine.
         pcm: int16 numpy array or CUDA tensor (or None without audio).  Returns numpy arrays (best_score,
-        best_offset, best_k, gss_ratio, all_score, all_offset) (all_* None unless want_all)."""
+        best_offset, best_k, gss_ratio, all_score, all_offset) (all_* None unless want_all).  With signal references
+        (sig, from _sig_refs) the tracks of a video with an out-of-domain value get the batched calls' sentinel."""
         import torch
         from .gss_batch import combine_gss, gss_align_batch
         h = self.handle
@@ -454,9 +580,13 @@ class BatchSynchronizer:
             pcm_host = pcm.cpu().numpy()
         else:
             pcm_host = pcm
+        if sig is not None and not isinstance(sig[1], np.ndarray):
+            h.synchronize()
+            torch.cuda.synchronize(sig[1].device)
+            sig = (sig[0], sig[1].cpu().numpy(), sig[2])
         grid = self._dispatch(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, False,
-                              pgs=pgs, want_all=True, memspace=_native.B2_HOST)
-        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs)
+                              pgs=pgs, sig=sig, want_all=True, memspace=_native.B2_HOST)
+        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs, sig)
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
@@ -465,13 +595,20 @@ class BatchSynchronizer:
                             self.sample_rate, self.start_seconds, handle=h)
         bs, bo, bk, ratio, a_s, a_o = combine_gss(grid[0], grid[1], grid[2], g, K, self.max_offset_samples,
                                                   grid[3], grid[4])
+        if sig is not None:
+            for t in np.flatnonzero(np.isin(track_video, list(self._bad_signals(sig)))):
+                bs[t], bo[t], bk[t], ratio[t] = np.nan, 0, _native.B2_BEST_K_BAD_SIGNAL, np.nan
+                a_s[t * (K + 1): (t + 1) * (K + 1)] = np.nan
+                a_o[t * (K + 1): (t + 1) * (K + 1)] = 0
         return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))
 
-    def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None):
+    def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None, sig=None):
         """The per-video reference signals the batched calls sync against, composed of public calls: the detector
         (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, with subtitle references
         (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0, and
-        with PGS references (pgs, from _pgs_refs) for a video that has one b2_rasterize_pgs of its intervals.
+        with PGS references (pgs, from _pgs_refs) for a video that has one b2_rasterize_pgs of its intervals, and with
+        signal references (sig, from _sig_refs, on the host) for a video that has one DeserializeSpeechTransformer's
+        rule at this synchroniser's label, in float64, rounded once to float32.
         Returns (float32 signals back to back, ref_off int64[V+1])."""
         h = self.handle
         V = len(pcm_off) - 1
@@ -483,7 +620,7 @@ class BatchSynchronizer:
         else:
             det, det_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
                                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
-        if refs is None and pgs is None:
+        if refs is None and pgs is None and sig is None:
             return det.astype(np.float32), det_off
         parts = [det[det_off[v]: det_off[v + 1]].astype(np.float32) for v in range(V)]
         if refs is not None:
@@ -492,6 +629,7 @@ class BatchSynchronizer:
                                        levels=[1.0])
             for v in np.flatnonzero(is_subs):
                 parts[v] = sub[sub_off[v]: sub_off[v + 1]]
+        stored = sig
         if pgs is not None:
             is_pgs, ps, pe, poff = pgs
             vids = np.flatnonzero(is_pgs)
@@ -499,6 +637,11 @@ class BatchSynchronizer:
                                            self.sample_rate, self.start_seconds)
             for i, v in enumerate(vids):
                 parts[v] = sig[sig_off[i]: sig_off[i + 1]]
+        if stored is not None:
+            is_sig, x, voff = stored
+            for v in np.flatnonzero(is_sig):
+                xv = x[voff[v]: voff[v + 1]]
+                parts[v] = np.where(xv < 1.0, np.float64(self.non_speech_label), xv).astype(np.float32)
         off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
         return (np.concatenate(parts) if parts else np.zeros(0, np.float32)), off
 

@@ -911,6 +911,8 @@ struct SyncBufs {
   double* g_evals;
   bool fused;
   int winner_only;
+  const double* sigx;                 // signal references' stored values (absolute sig_off indices), on the device
+  unsigned long long* first_bad;      // [V]: per video, its first out-of-domain frame (sig_ref_kernel)
 };
 
 // rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
@@ -952,29 +954,38 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // rasterises those of the videos [v0, v1) into
 // their ranges, on the same stream: the detector never writes there (no PCM: no tiles, no tokenizer chunk), and
 // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
+// With signal references (b2_sync_tracks_sig) sig_ref_kernel writes those of the videos [v0, v1) the same way, as
+// floats or, in a packed sub-batch, as the bits the VAD would write; it also resets and sets their flags.
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
                   bool ref_packed) {
   if (!p.auditok) {
+    // a packed sub-batch of signal videos alone has no audio: the VAD has no tiles and is not asked for bits
     B2_TRY(b2i_vad_launch(h, b.pcm, r.pcm_off + v0, v1 - v0, p.fpw, r.energy.non_speech_label,
                           (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, p.ref_off.data() + v0,
-                          nullptr, ref_packed));
+                          nullptr, ref_packed && r.pcm_off[v1] > r.pcm_off[v0]));
   } else {
     const ChunkTable& ch = p.ch;
     const int c0 = ch.first[v0], nc = ch.first[v1] - c0;
     B2_TRY(b2i_vad_launch(h, b.pcm, ch.pcm.data() + c0, nc, p.fpw, 0.0f, p.auditok_e_min, 0, p.fpw, b.refsig,
                           ch.out.data() + c0, ch.tail.data() + c0));
-    if (!p.any_subs) return b2i_tokenize_inplace_launch(h, b.refsig, ch.out.data() + c0, nc, p.tok);
+    if (!p.any_ref) return b2i_tokenize_inplace_launch(h, b.refsig, ch.out.data() + c0, nc, p.tok);
     const int k0 = ch.tok_first[v0];
     B2_TRY(b2i_tokenize_inplace_launch(h, b.refsig, ch.tok_off.data() + k0, ch.tok_first[v1] - k0, p.tok,
                                        ch.tok_end.data() + k0));
   }
-  if (!p.any_subs) return B2_OK;
+  if (!p.any_ref) return B2_OK;
   // the videos of `list` in [v0, v1), relative to v0
   auto in_range = [&](const std::vector<int>& list) {
     std::vector<int> rel(std::lower_bound(list.begin(), list.end(), v0), std::lower_bound(list.begin(), list.end(), v1));
     for (int& v : rel) v -= v0;
     return rel;
   };
+  const std::vector<int> sig(std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v0),
+                             std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v1));
+  if (!sig.empty())
+    B2_TRY(b2i_sig_ref_launch(h, b.sigx, r.sig.off, p.ref_off.data(), r.V, sig.data(), (int)sig.size(), p.label,
+                              ref_packed, b.refsig, b.first_bad));
+  if (!p.any_subs) return B2_OK;
   const std::vector<int> subs = in_range(p.sub_video), pgs = in_range(p.pgs_video);
   if (!subs.empty())
     B2_TRY(b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
@@ -1108,6 +1119,13 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
     B2_CHECK_DEV(h, memspace, r.gss_ratio, "sync_tracks_gss: gss_ratio");
     B2_CHECK_DEV(h, memspace, r.gss_evals, "sync_tracks_gss: gss_evals");
   }
+  const bool any_sig = !p.sig_video.empty();
+  const int64_t sig0 = any_sig ? r.sig.off[0] : 0, n_sig_values = any_sig ? r.sig.off[r.V] - sig0 : 0;
+  if (n_sig_values > 0) {
+    char what[64];
+    snprintf(what, sizeof(what), "%s: x", r.who);
+    B2_CHECK_DEV(h, memspace, r.sig.x, what);
+  }
   // Default: the K subtitle signals of a track are never materialised as floats - the cue list is
   // rasterised into bit masks (1 bit per frame) that the correlation kernel and the exact re-score
   // read.  B2_FUSED_RASTER=0 (A/B and test knob): raster_cues_kernel writes float signals to HBM and
@@ -1119,7 +1137,12 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // a chained resident call writes the buffer the previous call is not reading any more
   const bool chained = resident && fence_was_valid;
   const int refsig_slot = chained && h->refsig_parity == 0 ? b2_ctx::WS_SIG_REF2 : b2_ctx::WS_SIG_REF;
-  B2_TRY(b2i_ws(h, refsig_slot, (size_t)p.ref_off[r.V] * 4 + 64, &d_refsig));
+  // signal references: the per-video flags of sig_ref_kernel follow the reference in the same buffer, so a chained
+  // resident call's flags alternate with its reference and live exactly as long
+  const size_t ref_bytes = any_sig ? (((size_t)p.ref_off[r.V] * 4 + 64 + 7) & ~(size_t)7)
+                                   : (size_t)p.ref_off[r.V] * 4 + 64;
+  B2_TRY(b2i_ws(h, refsig_slot, ref_bytes + (any_sig ? (size_t)r.V * 8 : 0), &d_refsig));
+  b.first_bad = any_sig ? (unsigned long long*)((char*)d_refsig + ref_bytes) : nullptr;
   if (!b.fused) B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_SUB, (size_t)p.sub_off[J] * 4 + 64, &d_subsig));
   B2_TRY(b2i_ws(h, b2_ctx::WS_MISC, J * 16 + (size_t)T * 16 + 256, &d_res));
   double* d_score = (double*)d_res;
@@ -1155,6 +1178,12 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
     if (p.audio_samples > 0) B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, &dp));
     b.pcm = (const int16_t*)dp;
   }
+  b.sigx = r.sig.x;
+  if (memspace == B2_HOST && n_sig_values > 0) {   // the values [sig_off[0], sig_off[V]), read with their indices
+    void* dx;
+    B2_TRY(stage_in(h, b2_ctx::WS_STAGE_SIG, r.sig.x + sig0, (size_t)n_sig_values * 8, &dx));
+    b.sigx = (const double*)dx - sig0;
+  }
   const bool dev = memspace == B2_DEVICE;
   b.score = (dev && r.all_score && !p.gss) ? r.all_score : d_score;
   b.offset = (dev && r.all_offset && !p.gss) ? r.all_offset : d_offset;
@@ -1165,6 +1194,22 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   b.winner_only = (!r.all_score && !r.all_offset) ? 1 : 0;
   B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
+  // Signal videos with out-of-domain values: their tracks' outputs are overwritten behind every chain, on the
+  // caller's stream, before the host copies (the flags stay valid as the reference buffer does, below)
+  if (any_sig) {
+    B2SigBadOut so{b.bs, b.bo, b.bk, nullptr, nullptr, K, nullptr, nullptr, kGssEvals};
+    if (p.gss) {
+      so.a_score = b.g_all_score;
+      so.a_offset = b.g_all_offset;
+      so.cols = K + 1;
+      so.ratio = b.g_ratio;
+      so.evals = b.g_evals;
+    } else {
+      so.a_score = r.all_score ? b.score : nullptr;
+      so.a_offset = r.all_offset ? b.offset : nullptr;
+    }
+    B2_TRY(b2i_sig_bad_launch(h, b.first_bad, p.sig_video.data(), (int)p.sig_video.size(), p.trk_off.data(), so));
+  }
   // The reference capture: one copy behind every chain on the caller's stream, when every detector step is done.
   // The buffer stays valid until then: no chain kernel writes it (they read it as const), the next chained
   // resident call writes the other buffer, and the call after that starts its detector behind a fence recorded
@@ -1331,5 +1376,42 @@ extern "C" int b2_sync_tracks_pgs(b2_handle h, const int16_t* pcm, const int64_t
                 best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
                 memspace};
   r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : no_intervals};
+  return sync_run(h, _b2_fence_was_valid, r);
+}
+
+extern "C" int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                  const int32_t* track_video, int T, int frame_rate, int sample_rate, int detector,
+                                  double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                                  double energy_threshold_db, double min_length, int64_t max_length,
+                                  double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs,
+                                  const double* ref_cue_start_s, const double* ref_cue_end_s,
+                                  const uint8_t* ref_cue_keep, const int64_t* ref_cue_off, const uint8_t* ref_is_pgs,
+                                  const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off,
+                                  const uint8_t* ref_is_sig, const double* x, const int64_t* sig_off,
+                                  const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                  const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                  int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                  int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                  double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_sig");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: gss_evals without gss_ratio");
+  if (V > 0 && (!pcm_off || !sig_off)) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: null pcm_off / sig_off");
+  if (ref_is_subs && !ref_cue_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: ref_is_subs without ref_cue_off");
+  if (ref_is_pgs && !pgs_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: ref_is_pgs without pgs_off");
+  if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_sig: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, "
+            "not %d", detector);
+  static const int64_t no_values[1] = {0};
+  SyncRequest r{gss_ratio ? "sync_tracks_sig (search)" : "sync_tracks_sig", pcm, pcm_off, V, track_video, T,
+                frame_rate, sample_rate, detector, {(float)non_speech_label, energy_threshold, z_lo, z_hi},
+                {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length, chunk_samples},
+                {ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : nullptr},
+                cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
+                memspace};
+  r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
+  r.sig = {ref_is_sig, x, V > 0 ? sig_off : no_values};
   return sync_run(h, _b2_fence_was_valid, r);
 }

@@ -70,7 +70,8 @@ struct b2_ctx {
   int refsig_parity = 0;
   // named grow-only workspaces
   enum { WS_STAGE_IN0, WS_STAGE_IN1, WS_STAGE_OUT, WS_META, WS_SPEC, WS_SCORES, WS_CAND,
-         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_GSS, WS_GSS_OUT, WS_COUNT };
+         WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_GSS, WS_GSS_OUT, WS_STAGE_SIG,
+         WS_COUNT };
   DeviceBuf ws[WS_COUNT];
   HostBuf pinned[4];
   cudaEvent_t pinned_ev[4] = {};   // recorded after the last async copy out of pinned[i]
@@ -205,6 +206,31 @@ int b2i_raster_launch(b2_ctx* h, const double* cue_start, const double* cue_end,
 int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_end, const uint8_t* cue_keep,
                           const int64_t* cue_off, const int64_t* out_off, int n_videos, const int* videos, int n_subs,
                           int sample_rate, double start_seconds, float* d_out, bool pgs = false);
+// Signal references of b2_sync_tracks_sig (K1s, sig_ref.cu): for each of the n_sig videos videos[i] (ascending
+// indices into the host tables x_off / out_off [n_videos + 1], absolute), write the frames of the stored values
+// d_x[x_off[v] ..] (sig_ref.cuh), out_off[v+1] - out_off[v] of them, to d_out + out_off[v]: floats, or with packed
+// ceil(R/32) words of the bits m = (r == 1.0f) with zero bits past R.  d_first_bad[v] is reset first and ends as the
+// first out-of-domain frame (kSigNoBadFrame: none).  The grid keeps to h->vad_partition_sms SMs when it is set.
+int b2i_sig_ref_launch(b2_ctx* h, const double* d_x, const int64_t* x_off, const int64_t* out_off, int n_videos,
+                       const int* videos, int n_sig, float label, bool packed, float* d_out,
+                       unsigned long long* d_first_bad);
+// The outputs of one batched sync call that sig_bad_kernel overwrites for the tracks of a flagged signal video
+// (device arrays; a_* [T * cols], evals [T * n_evals] and ratio may be null)
+struct B2SigBadOut {
+  double* bs;
+  int32_t* bo;
+  int32_t* bk;
+  double* a_score;
+  int32_t* a_offset;
+  int cols;
+  double* ratio;
+  double* evals;
+  int n_evals;
+};
+// For each signal video videos[i] whose d_first_bad entry is set: best_k = B2_BEST_K_BAD_SIGNAL, best_score,
+// all_score, gss_ratio and gss_evals NaN, best_offset and all_offset 0, on every track trk_off[v] .. trk_off[v+1]-1.
+int b2i_sig_bad_launch(b2_ctx* h, const unsigned long long* d_first_bad, const int* videos, int n_sig,
+                       const int* trk_off, const B2SigBadOut& out);
 int b2i_bounds_launch(b2_ctx* h, const float* d_sig, const int64_t* off_host, int n,
                       int64_t* d_first, int64_t* d_last);
 int b2i_blend_launch(b2_ctx* h, const float* d_a, const float* d_b, int64_t n, int mode, double wa,

@@ -1,6 +1,6 @@
 // Host-side plan of one batched sync call (b2_sync_batch, b2_sync_tracks, b2_sync_tracks_gss,
-// b2_sync_tracks_auditok, b2_sync_tracks_subs, b2_sync_tracks_pgs): every argument check and every host table the pipeline in
-// api.cu reads.  No CUDA call happens here, so tests/host_emul/plan_emul.cu runs the same code on the CPU.
+// b2_sync_tracks_auditok, b2_sync_tracks_subs, b2_sync_tracks_pgs, b2_sync_tracks_sig): every argument check and every
+// host table the pipeline in api.cu reads.  No CUDA call happens here, so tests/host_emul/plan_emul.cu runs the same code on the CPU.
 #pragma once
 
 #include <math.h>
@@ -376,6 +376,15 @@ struct SyncRequest {
     const double* end_s;
     const int64_t* off;            // [V+1]
   } pgs;
+  // Serialized speech signals (b2_sync_tracks_sig; off null: none): videos with is_sig[v] != 0 take the stored
+  // float64 values x[off[v] .. off[v+1]) (x follows memspace, off is a host array of absolute indices), each
+  // frame (float)(x < 1.0 ? label : x) (DeserializeSpeechTransformer), as reference signal.  The
+  // value-initialised state is "no signal video", so the other entry points leave it out.
+  struct {
+    const uint8_t* is_sig;         // may be null: no video
+    const double* x;
+    const int64_t* off;            // [V+1]
+  } sig;
 };
 
 // What plan_sync reads from the handle and the environment: the SM count, the most sub-batches the handle's
@@ -410,6 +419,10 @@ struct SyncPlan {
   std::vector<int64_t> sub_off;    // [T*K+1]: float subtitle signal of job j (unfused raster)
   std::vector<int> sub_video;      // the videos with a text subtitle reference, ascending
   std::vector<int> pgs_video;      // the videos with a PGS reference, ascending
+  std::vector<int> sig_video;      // the videos with a serialized signal reference, ascending
+  // a video's reference is not the detector's (text, PGS or signal): it has no PCM, its length comes from its
+  // reference, and the tokenizer's table leaves it out.  Without signal videos this is any_subs.
+  bool any_ref = false;
   ChunkTable ch;                   // auditok
   int64_t auditok_e_min = 0;
   B2TokenizerParams tok{0.0, 0.0, 0.0, 0};
@@ -461,16 +474,21 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // is decided here by the aligner's own functions on the chain's own inputs (align_path.h, as enqueue_chain passes
 // them), so the launcher reaches the same choice.  auditok, subtitle references, the lane-group kernel and the
 // FFT paths keep the float reference (text and PGS references alike).  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
+// Serialized signal references (b2_sync_tracks_sig) have the bits too: sig_ref_kernel writes them, so a sub-batch
+// whose videos are all signal videos or lane-eligible energy audio is packed like an audio one, with either
+// detector (auditok sub-batches qualify only when every video is a signal video).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
-  if (p->auditok || !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0)) return;
+  if ((p->auditok && p->sig_video.empty()) || !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0)) return;
+  // how many videos of `list` lie in [v0, v1)
+  auto count = [](const std::vector<int>& list, int v0, int v1) {
+    return (int)(std::lower_bound(list.begin(), list.end(), v1) - std::lower_bound(list.begin(), list.end(), v0));
+  };
   for (int i = 0; i < p->n_sub; ++i) {
     const int v0 = p->cut[i], v1 = p->cut[i + 1];
-    const auto& sv = p->sub_video;
-    const auto& pv = p->pgs_video;
-    if (std::lower_bound(sv.begin(), sv.end(), v0) != std::lower_bound(sv.begin(), sv.end(), v1)) continue;
-    if (std::lower_bound(pv.begin(), pv.end(), v0) != std::lower_bound(pv.begin(), pv.end(), v1)) continue;
-    if (!env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw)) continue;
+    if (count(p->sub_video, v0, v1) || count(p->pgs_video, v0, v1)) continue;
+    const bool all_sig = count(p->sig_video, v0, v1) == v1 - v0;
+    if (!all_sig && (p->auditok || !env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw))) continue;
     const int t0 = p->trk_off[v0], nt = p->trk_off[v1] - t0;
     std::vector<int> chain_trk(v1 - v0 + 1);
     for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = p->trk_off[v] - t0;
@@ -484,14 +502,30 @@ static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPl
   }
 }
 
-// Checks of the subtitle references (text and PGS), before anything reads their tables.
-static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio) {
+// Checks of the subtitle references (text and PGS) and of the signal references, before anything reads their
+// tables.  *any_audio: a video's reference is the detector's; *any_sig: a video has a signal reference.
+static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio, bool* any_sig) {
   const char* who = r.who;
   const auto& s = r.refs;
   const auto& g = r.pgs;
+  const auto& q = r.sig;
   for (int v = 0; v < r.V; ++v) {
     const bool is_subs = s.cue_off && s.is_subs && s.is_subs[v];
     const bool is_pgs = g.off && g.is_pgs && g.is_pgs[v];
+    const bool is_sig = q.off && q.is_sig && q.is_sig[v];
+    if (q.off) {
+      if (q.off[v + 1] < q.off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: sig_off not monotone at %d", who, v);
+      if (!is_sig && q.off[v + 1] != q.off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has signal values but no signal reference (ref_is_sig[%d] = 0)",
+                who, v, v);
+      if (is_sig && is_subs)
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d is marked both as a signal and as a text subtitle reference", who, v);
+      if (is_sig && is_pgs)
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d is marked both as a signal and as a PGS reference", who, v);
+      if (is_sig && r.pcm_off[v + 1] != r.pcm_off[v])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has a signal reference and a non-empty PCM range (%lld samples); "
+                "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
+    }
     if (s.cue_off) {
       if (s.cue_off[v + 1] < s.cue_off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: ref_cue_off not monotone at %d", who, v);
       if (!is_subs && s.cue_off[v + 1] != s.cue_off[v])
@@ -513,12 +547,15 @@ static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio) {
                 "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
     }
     p->any_subs = p->any_subs || is_subs || is_pgs;
-    *any_audio = *any_audio || (!is_subs && !is_pgs);
+    *any_audio = *any_audio || (!is_subs && !is_pgs && !is_sig);
+    *any_sig = *any_sig || is_sig;
   }
   if (s.cue_off && r.V > 0 && s.cue_off[r.V] > s.cue_off[0] && (!s.cue_start_s || !s.cue_end_s))
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null reference cue arrays", who);
   if (g.off && r.V > 0 && g.off[r.V] > g.off[0] && (!g.start_s || !g.end_s))
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null PGS interval arrays", who);
+  if (q.off && r.V > 0 && q.off[r.V] > q.off[0] && !q.x)
+    B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null signal values x with %lld values", who, (long long)(q.off[r.V] - q.off[0]));
   if (p->audio_samples > 0 && !r.pcm)
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null pcm with %lld samples of audio", who, (long long)p->audio_samples);
   return B2_OK;
@@ -573,8 +610,9 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
   // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
   // the tracks' cues).  subs_len[v] = -1: the video's reference is the detector's.
   // PGS references: int(max_end * sample_rate) + 2 frames, the length b2_rasterize_pgs_lengths gives.
+  // Signal references: one frame per stored value, sig_off[v+1] - sig_off[v].
   std::vector<int64_t> subs_len;
-  if (p->any_subs) {
+  if (p->any_ref) {
     subs_len.assign(V, -1);
     const uint8_t* is_subs = r.refs.cue_off ? r.refs.is_subs : nullptr;
     const uint8_t* is_pgs = r.pgs.off ? r.pgs.is_pgs : nullptr;
@@ -597,17 +635,23 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
           subs_len[v] = pgs_len[v];
         }
     }
+    if (r.sig.off && r.sig.is_sig)
+      for (int v = 0; v < V; ++v)
+        if (r.sig.is_sig[v]) {
+          p->sig_video.push_back(v);
+          subs_len[v] = r.sig.off[v + 1] - r.sig.off[v];
+        }
   }
   p->ref_off.assign(V + 1, 0);
   for (int v = 0; v < V; ++v) {
     const int64_t n = r.pcm_off[v + 1] - r.pcm_off[v];
     if (n < 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
-    if (p->any_subs && subs_len[v] >= 0) p->ref_off[v + 1] = p->ref_off[v] + subs_len[v];
+    if (p->any_ref && subs_len[v] >= 0) p->ref_off[v + 1] = p->ref_off[v] + subs_len[v];
     else if (!p->auditok) p->ref_off[v + 1] = p->ref_off[v] + (n + fpw - 1) / fpw;
   }
   if (p->auditok) {
     build_chunk_table(r.pcm_off, V, 0, fpw, r.auditok.chunk_samples, r.auditok.energy_threshold_db,
-                      p->any_subs ? subs_len.data() : nullptr, &p->ch);
+                      p->any_ref ? subs_len.data() : nullptr, &p->ch);
     for (int v = 0; v < V; ++v) p->ref_off[v + 1] = p->ch.out[p->ch.first[v + 1]];
   }
   return B2_OK;
@@ -622,20 +666,23 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
   p->auditok = r.detector == B2_DETECTOR_AUDITOK;
   if (V < 0 || T < 0 || K <= 0 || !r.pcm_off || !r.cue_off || !r.ratios)
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad arguments", who);
-  bool any_audio = !r.refs.cue_off && !r.pgs.off;
+  bool any_audio = !r.refs.cue_off && !r.pgs.off && !r.sig.off, any_sig = false;
   for (int v = 0; v < V; ++v)
     if (r.pcm_off[v + 1] > r.pcm_off[v]) p->audio_samples += r.pcm_off[v + 1] - r.pcm_off[v];
-  if (r.refs.cue_off || r.pgs.off) B2_TRY(plan_refs_check(r, p, &any_audio));
+  if (r.refs.cue_off || r.pgs.off || r.sig.off) B2_TRY(plan_refs_check(r, p, &any_audio, &any_sig));
+  p->any_ref = p->any_subs || any_sig;
   // The run path and the GSS rounds need a reference of the two levels 1.0 and ref_label.  The detector's signal
   // has the levels 1.0 and the label, a subtitle reference 1.0 and 0.0, so ref_label is the label unless every
   // reference is a subtitle stream; a call that mixes the two at a non-zero label has three levels.  auditok's
   // clipped cumsum has two levels only at label 0 (starts and ends alternate and an overwrite only turns an end
   // into a start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3).
+  // A signal reference has the levels 1.0 and the label whichever the detector (its stored values are < 1.0 or
+  // exactly 1.0), so it counts like energy audio: a call of signals alone is two-level.
   p->label = p->auditok ? (float)r.auditok.non_speech_label : r.energy.non_speech_label;
-  p->ref_label = any_audio ? p->label : 0.0f;
-  const bool auditok_two_level = !p->auditok || r.auditok.non_speech_label == 0.0;
+  p->ref_label = any_audio || any_sig ? p->label : 0.0f;
+  const bool auditok_two_level = !p->auditok || r.auditok.non_speech_label == 0.0 || !any_audio;
   const bool mix_two_level = !p->any_subs || p->label == 0.0f;
-  p->two_level = !any_audio || (auditok_two_level && mix_two_level);
+  p->two_level = (!any_audio && !any_sig) || (auditok_two_level && mix_two_level);
   if (r.track_video) {
     for (int t = 0; t < T; ++t)
       if (r.track_video[t] < 0 || r.track_video[t] >= V || (t > 0 && r.track_video[t] < r.track_video[t - 1]))

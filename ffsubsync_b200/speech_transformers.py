@@ -762,18 +762,25 @@ class PGSSpeechTransformer(TransformerMixin, ComputeSpeechFrameBoundariesMixin):
         return self.pgs_speech_results_
 
 
+def load_stored_speech(fname) -> np.ndarray:
+    """The array a ``--serialize-speech`` / ``--make-test-case`` artefact stores (``.npz`` with key "speech", or
+    ``.npy``), as np.load returns it: DeserializeSpeechTransformer.fit before its rule."""
+    speech = np.load(fname)
+    if hasattr(speech, "files"):
+        if "speech" not in speech.files:
+            raise ValueError('could not find "speech" array in serialized file; only contains: %s'
+                             % speech.files)
+        speech = speech["speech"]
+    return speech
+
+
 class DeserializeSpeechTransformer(TransformerMixin):
     def __init__(self, non_speech_label: float) -> None:
         self._non_speech_label: float = non_speech_label
         self.deserialized_speech_results_: Optional[np.ndarray] = None
 
     def fit(self, fname, *_) -> "DeserializeSpeechTransformer":
-        speech = np.load(fname)
-        if hasattr(speech, "files"):
-            if "speech" not in speech.files:
-                raise ValueError('could not find "speech" array in serialized file; only contains: %s'
-                                 % speech.files)
-            speech = speech["speech"]
+        speech = load_stored_speech(fname)
         speech[speech < 1.0] = self._non_speech_label
         self.deserialized_speech_results_ = speech
         return self

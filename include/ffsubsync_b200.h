@@ -71,6 +71,10 @@ enum {
  * everything (score -inf, offset N-1-S), widths beyond the padded length mask nothing. */
 #define B2_MAX_OFFSET_NONE INT64_MIN
 
+/* best_k of a track whose video's serialized signal reference holds a value outside its domain (> 1.0 or NaN;
+ * b2_sync_tracks_sig).  best_k = -1 stays the reference's FailedToFindAlignment (an empty signal). */
+#define B2_BEST_K_BAD_SIGNAL (-2)
+
 /* ---- lifecycle ----------------------------------------------------------------------- */
 int b2_version(void);
 int b2_create(int device, b2_handle* out);
@@ -361,6 +365,47 @@ int b2_sync_tracks_pgs(b2_handle h, const int16_t* pcm /* or NULL without audio 
                        double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                        int memspace);
 
+/* ---- serialized speech signals as references (`ffs ref.npz -i in.srt`) -------------------------------------
+ * The signals that --serialize-speech / --make-test-case store (DeserializeSpeechTransformer, ffsubsync/
+ * speech_transformers.py:987-1009) as references of V videos and T tracks.  Arguments as for b2_sync_tracks_pgs,
+ * plus:
+ *   ref_is_sig [V]       host; non-zero: video v's reference is its stored signal.  NULL = none.
+ *   x                    the stored values as float64 (np.load's dtype), in memspace: video v's are
+ *                        x[sig_off[v] .. sig_off[v+1]).  B2_DEVICE_RESIDENT: the resident promise (nothing queued
+ *                        on the handle's stream before the call writes pcm) covers x too.
+ *   sig_off [V+1]        host; a video without a signal reference has an empty range.
+ * Frame i of a signal video is (float)(x < 1.0 ? non_speech_label : x) - the rule in float64, rounded once (so
+ * values in (1 - 2^-25, 1) stay non-speech) - with the call's own label; start_seconds does not apply.  Every
+ * stored value must be < 1.0 or exactly 1.0 (what the reference's detectors and rasterisers write), so a signal
+ * reference has the levels 1.0 and the label like the energy detector's output, and counts like a detector video
+ * for the label / path / B2_ERR_UNSUPPORTED rules of b2_sync_tracks_subs: signals alone are two-level with either
+ * detector; mixed with text / PGS references or auditok audio at a non-zero label they make three levels.
+ * A value > 1.0 or NaN is outside the domain: every track of that video gets best_k = B2_BEST_K_BAD_SIGNAL,
+ * best_score NaN, best_offset 0, all_score NaN / all_offset 0 in every column, gss_ratio and gss_evals NaN, without
+ * a host synchronisation; the other tracks are unaffected.  An empty signal gives best_k = -1.
+ * Track t gets exactly what this composition of public calls returns: the rule applied to its video's signal (what
+ * b2_sync_tracks_pgs uses for other videos), then b2_align_batch and b2_reduce_ratios over the ratios, plus the
+ * golden-section search's candidate as in b2_sync_tracks_gss when gss_ratio is not NULL.  No inferred framerate
+ * ratio: the grid is the caller's.  B2_ERR_BAD_ARG also for a non-monotone sig_off, values given for a video without
+ * ref_is_sig, a signal video with a non-empty PCM range, a video marked signal and text or signal and PGS, a null x
+ * under non-empty ranges and a host x under B2_DEVICE.  memspace: B2_HOST, B2_DEVICE or B2_DEVICE_RESIDENT;
+ * resident calls chain with the other sync calls in any order. */
+int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm /* or NULL without audio */, const int64_t* pcm_off /* [V+1] */,
+                       int V, const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                       int detector, double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                       double energy_threshold_db, double min_length, int64_t max_length,
+                       double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs /* [V] */,
+                       const double* ref_cue_start_s, const double* ref_cue_end_s, const uint8_t* ref_cue_keep,
+                       const int64_t* ref_cue_off /* [V+1] or NULL */, const uint8_t* ref_is_pgs /* [V] */,
+                       const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off /* [V+1] or NULL */,
+                       const uint8_t* ref_is_sig /* [V] */, const double* x, const int64_t* sig_off /* [V+1] */,
+                       const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                       const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                       int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                       double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                       double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                       int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
@@ -384,8 +429,9 @@ int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* 
 
 /* ---- diagnostics for tests: the batched sync calls' reference signals ------------------------
  * Exposes the per-video reference signal a batched sync call (b2_sync_batch, b2_sync_tracks, _gss, _auditok,
- * _subs, _pgs) builds in its detector step - the detector's output, the tokenised auditok signal or a rasterised
- * subtitle / PGS reference, ffsubsync/speech_transformers.py's VideoSpeechTransformer.fit output.  While set, every
+ * _subs, _pgs, _sig) builds in its detector step - the detector's output, the tokenised auditok signal, a rasterised
+ * subtitle / PGS reference or a serialized signal's frames, ffsubsync/speech_transformers.py's
+ * VideoSpeechTransformer.fit / DeserializeSpeechTransformer.fit output.  While set, every
  * such call with at least one track writes, overwriting the previous call's:
  *   ref[0 .. ref_off[V])  its reference buffer (DEVICE array; one device-to-device copy on the handle's stream after
  *                         the call's last kernel).  Video v's signal is ref[ref_off[v] .. ref_off[v+1]) as float32,
