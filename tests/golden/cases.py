@@ -112,6 +112,15 @@ def multi_segment_case(true_scale: float, true_shift: float, sr: int = 100):
 # Signal families that stress the round-off bound tau of the nomination stage: large means (the
 # ||c||_2 term of tau dominates), flat or periodic correlation landscapes, exact ties, wide dynamic range.
 SIGNAL_FAMILIES = ["random", "ones", "zeros", "period2", "period_block", "sparse", "wide", "ramp"]
+# Families aimed at the large-window path's four-step layout: its [M1][1024] work array holds
+# z[n] = x[2n] + i x[2n+1] row by row, so one row is 2048 real samples.  A period of 2048 makes every column
+# constant (all energy in column bin 0); the impulse train is the extreme broad, flat correlation.
+LAYOUT_FAMILIES = ["square_2048", "impulse_2048"]
+# (reference, subtitle) family pairings run at the largest transform sizes (2^22, 2^23 and their CPU emulation),
+# where every pairing would cost too much: the large-mean and block-periodic references against random subtitles,
+# and the layout families on either side.
+BIG_TRANSFORM_PAIRS = [(f, "random") for f in ("random", "period_block", "ones", "sparse", "ramp", "wide")] + \
+    [(f, g) for f in LAYOUT_FAMILIES for g in ("random", f)] + [("random", f) for f in LAYOUT_FAMILIES]
 
 
 def signal_family(name, n, rng, level=1.0):
@@ -135,6 +144,10 @@ def signal_family(name, n, rng, level=1.0):
         return (10.0 ** rng.uniform(-3, 3, n) * rng.choice([0.0, 1.0], n)).astype(np.float32)
     if name == "ramp":
         return np.linspace(0.0, level, n).astype(np.float32)
+    if name == "square_2048":
+        return ((np.arange(n) // 1024) % 2).astype(np.float32) * np.float32(level)
+    if name == "impulse_2048":
+        return (np.arange(n) % 2048 == 0).astype(np.float32) * np.float32(level)
     raise ValueError(name)
 
 

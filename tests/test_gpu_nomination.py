@@ -6,7 +6,8 @@ offset within tau of the maximum exactly (DESIGN.md section 4, "Round-off bound"
 needs |fp32 score - exact score| <= tau at every offset; the final (score, offset) alone hides any
 fp32 error smaller than the winner's margin.  b2_capture_nominations exposes the fp32 window,
 (maximum, tau) and the candidate count of every (pair, ratio), and these tests check them against
-oracle/aligner_oracle.correlation (complex128) on the signals the kernels were given:
+the float64 correlation of oracle/aligner_oracle.correlation (nomination_check.Exact) on the signals the kernels
+were given:
   * the surviving window equals the oracle's;
   * the captured maximum is the maximum of the captured scores;
   * max |fp32 - exact| <= tau (tau is the kernels' own bound, never loosened here);
@@ -24,10 +25,11 @@ import cases
 from oracle import aligner_oracle as ao
 from oracle import raster_oracle as ro
 from oracle import vad_oracle as vo
+from nomination_check import Exact as _Exact
+from nomination_check import check_jobs
 
 pytestmark = pytest.mark.gpu
 
-K_CAND = 32
 WORST = {}   # (path, subtitle encoding) -> worst max |fp32 - exact| / tau
 
 
@@ -44,96 +46,8 @@ def report_worst():
         print("nomination error / tau, worst [%s, %s]: %.3g" % (key + WORST[key][:1]), *WORST[key][1:])
 
 
-# ------------------------------------------------------------------------------------------ oracle
-
-class _Exact:
-    """float64 correlation of a (ref, sub) pair, computed once per pair of signals."""
-
-    def __init__(self):
-        self.memo = {}
-
-    def window(self, ref, sub, w0, n):
-        key = (id(ref), id(sub))
-        if key not in self.memo:
-            conv = ao.correlation(ref, sub)
-            if _binary(ref) and _binary(sub):
-                conv = np.round(conv)          # +-1 products: the exact scores are integers
-            self.memo[key] = (conv, ref, sub)  # keep the arrays alive: their ids are the key
-        conv = self.memo[key][0]
-        N, S = len(conv), len(sub)
-        o = w0 + np.arange(n)
-        # aligners.py:47; offsets where the signals do not overlap score exactly 0 (no FFT round-off)
-        return np.where((o > -S) & (o < len(ref)), conv[N - 1 - S - o], 0.0)
-
-
-def _binary(x):
-    return bool(np.all((x == 0) | (x == 1)))
-
-
-def _norm(x):
-    return float(np.sqrt(np.sum((2.0 * np.asarray(x, np.float64) - 1.0) ** 2)))
-
-
-def _check_jobs(cap, sigs, mos, exact, key, out=None, winner_only=False, K=1):
-    """sigs[j] = (ref, sub) float64 arrays of global job j as the kernels saw them; out = (score, offset,
-    status) per job (None in winner-only calls).  Returns the per-job fp32 maxima / taus."""
-    stats = []
-    for j, (ref, sub) in enumerate(sigs):
-        w0, n = (int(v) for v in cap["win"][j])
-        mx, tau = (np.float32(v) for v in cap["stat"][j])
-        cand = int(cap["cand"][j])
-        o_lo, o_hi = ao.offset_range(len(ref), len(sub), mos)
-        where = (key, j, len(ref), len(sub), mos)
-        if o_lo > o_hi:
-            assert n == 0 and cand == 0 and mx == -np.inf, where
-            stats.append((mx, tau, None))
-            continue
-        assert (w0, n) == (o_lo, o_hi - o_lo + 1), where
-        f = cap["scores"][j, :n]
-        assert mx == f.max(), where
-        ex = exact.window(ref, sub, w0, n)
-        err = float(np.abs(f.astype(np.float64) - ex).max())
-        assert err <= float(tau), (where, err, float(tau))
-        WORST[key] = max(WORST.get(key, (0.0,)), (err / float(tau), "N=%d" % ao.padded_length(len(ref), len(sub)),
-                                                   "R=%d S=%d" % (len(ref), len(sub)), "mos=%s" % mos))
-        cut = np.float32(mx - tau)           # float32 subtraction, as the selection kernels do
-        hits = np.flatnonzero(f >= cut)
-        if cand != -1:
-            assert cand == len(hits), (where, cand, len(hits))
-        if out is not None:
-            score, offset, status = (None if a is None else a[j] for a in out)
-            assert cand != -1, where
-            if status is not None:           # b2_sync_batch does not return the per-ratio status
-                assert bool(status & 4) == (cand > K_CAND), (where, status, cand)
-            top = hits[::-1][:K_CAND]        # largest offsets first
-            best = ex[top].max()
-            m = int(offset) - w0
-            assert m in set(top.tolist()), (where, int(offset))
-            tol = 1e-9 * (_norm(ref) * _norm(sub) + 1.0)
-            assert ex[m] >= best - tol and abs(float(score) - ex[m]) <= tol, (where, float(score), ex[m], best)
-            if _binary(ref) and _binary(sub):   # integer scores: the tie rule is checkable exactly
-                assert m == int(top[np.flatnonzero(ex[top] == best)[0]]), where
-        stats.append((mx, tau, (w0, n, f)))
-    if winner_only:
-        _check_approx(cap, stats, mos, K, key)
-    return stats
-
-
-def _check_approx(cap, stats, mos, K, key):
-    """Winner-only pruning: cand == -1 exactly when max + tau < max_k (max_k - tau_k) and no surviving
-    offset of the pair exceeds the mask width (no_prune)."""
-    for b in range(len(stats) // K):
-        js = range(b * K, b * K + K)
-        floor = max(np.float32(stats[j][0] - stats[j][1]) for j in js)
-        no_prune = mos is not None and any(
-            stats[j][2] is not None and max(abs(stats[j][2][0]), abs(stats[j][2][0] + stats[j][2][1] - 1)) > mos
-            for j in js)
-        for j in js:
-            mx, tau, w = stats[j]
-            if w is None:
-                continue
-            want = (not no_prune) and np.float32(mx + tau) < floor
-            assert (int(cap["cand"][j]) == -1) == want, (key, b, j, float(mx), float(tau), float(floor))
+def _check_jobs(*args, **kw):
+    return check_jobs(*args, worst=WORST, **kw)
 
 
 # ------------------------------------------------------------------------------- b2_align_batch

@@ -7,6 +7,8 @@ import re
 import struct
 import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 from datetime import timedelta
 
 import numpy as np
@@ -404,23 +406,22 @@ def test_pipeline_maker_keeps_the_reference_signature():
 # ---- large-window path: the four-step FFT kernels emulated on the CPU (bigfft.cuh) --------------------
 
 def _emulate_big(ref, sub, q1, mode=0):
-    tmp = os.path.join(ROOT, "tests", "host_emul")
-    fin, fout = os.path.join(tmp, "_bin.bin"), os.path.join(tmp, "_bout.bin")
-    with open(fin, "wb") as f:
-        f.write(struct.pack("4i", len(ref), len(sub), q1, mode))
-        f.write(np.asarray(ref, np.float32).tobytes())
-        f.write(np.asarray(sub, np.float32).tobytes())
-    subprocess.check_call([os.path.join(tmp, "bigfft_emul"), fin, fout])
-    out = np.fromfile(fout, dtype=np.float32)
-    os.remove(fin)
-    os.remove(fout)
+    with tempfile.TemporaryDirectory() as tmp:   # one directory per run: runs may go in parallel
+        fin, fout = os.path.join(tmp, "in.bin"), os.path.join(tmp, "out.bin")
+        with open(fin, "wb") as f:
+            f.write(struct.pack("4i", len(ref), len(sub), q1, mode))
+            f.write(np.asarray(ref, np.float32).tobytes())
+            f.write(np.asarray(sub, np.float32).tobytes())
+        subprocess.check_call([os.path.join(ROOT, "tests", "host_emul", "bigfft_emul"), fin, fout])
+        out = np.fromfile(fout, dtype=np.float32)
     n = 1 << (q1 + 11)
     return out[:n].astype(np.float64), float(out[n]), float(out[n + 1]), float(out[n + 2])
 
 
 def _direct_big(ref, sub, n):
+    import scipy.fft
     r, s = 2 * np.asarray(ref, np.float64) - 1, 2 * np.asarray(sub, np.float64) - 1
-    full = np.fft.irfft(np.conj(np.fft.rfft(s, n)) * np.fft.rfft(r, n), n)   # full[o mod n] = score(o)
+    full = scipy.fft.irfft(np.conj(scipy.fft.rfft(s, n)) * scipy.fft.rfft(r, n), n)   # full[o mod n] = score(o)
     return full[(np.arange(n) - len(s)) % n]                                 # scores[m], offset o = m - S
 
 
@@ -464,6 +465,65 @@ def test_bigfft_roundoff_adversarial(built):
         got, es, er, cn = _emulate_big(ref, sub, 7, 0)
         want = _direct_big(ref, sub, 1 << 18)
         assert np.abs(got - want).max() <= _tau(es, er, cn) / 4, (fam_r, fam_s)
+
+
+def test_nomination_oracle_is_the_reference_correlation():
+    """tests/nomination_check.Exact (real transforms, reference spectra shared) reads the same scores as
+    oracle/aligner_oracle.correlation at every offset of the window, and 0 where the signals do not overlap."""
+    from nomination_check import Exact
+    rng = np.random.RandomState(7)
+    for R, S, level in ((1, 1, 1.0), (1000, 700, 1.0), (5000, 3001, 0.96), (300, 4000, 0.5)):
+        ref, sub = (rng.rand(R) > 0.5).astype(float), (rng.rand(S) > 0.4) * level
+        N, conv = ao.padded_length(R, S), ao.correlation(ref, sub)
+        o = np.arange(-S - 3, N - S)
+        want = np.where((o > -S) & (o < R), conv[(N - 1 - S - o) % N], 0.0)
+        assert np.abs(Exact().window(ref, sub, int(o[0]), len(o)) - want).max() <= 1e-9 * N
+
+
+_BIG_FAMILIES = cases.SIGNAL_FAMILIES + cases.LAYOUT_FAMILIES
+
+
+def _bigfft_family_case(q1, fam_r, fam_s, mode):
+    """One emulated large-window correlation: reference of family fam_r, subtitles of family fam_s as float32
+    at level 0.96 (mode 0) or as a bit mask (mode 1).  The lengths alternate between balanced and lopsided
+    shapes.  Returns (err / tau, err / (u sqrt(Es Er)))."""
+    n = 1 << (q1 + 11)
+    i, k = _BIG_FAMILIES.index(fam_r), _BIG_FAMILIES.index(fam_s)
+    rng = np.random.RandomState(1000 * q1 + 20 * i + 2 * k + mode)
+    R, S = [(int(0.45 * n), n // 2 - 3), (n // 8 + 1, int(0.8 * n) + 5), (int(0.7 * n) - 7, n // 4)][(i + k) % 3]
+    ref = _family(fam_r, R, rng)
+    sub = _family(fam_s, S, rng, level=0.96 if mode == 0 else 1.0)
+    if mode == 1:
+        sub = (sub != 0).astype(np.float32)
+    got, es, er, cn = _emulate_big(ref, sub, q1, mode)
+    err = float(np.abs(got - _direct_big(ref, sub, n)).max())
+    tau = _tau(es, er, cn)
+    assert err <= tau / 4, (q1, fam_r, fam_s, mode, err, tau)
+    return err / tau, err / (2.0 ** -24 * np.sqrt(es * er))
+
+
+def _bigfft_family_cases(cases_):
+    with ThreadPoolExecutor(max_workers=os.cpu_count() or 1) as ex:   # each emulation is its own process
+        res = list(ex.map(lambda c: _bigfft_family_case(*c), cases_))
+    worst = max(zip(res, cases_))
+    print("worst %.3g tau (%.1f u sqrt(Es Er)) at q1=%d %s x %s mode %d" % (worst[0] + worst[1]))
+
+
+@pytest.mark.parametrize("fam_r", _BIG_FAMILIES)
+@pytest.mark.parametrize("q1", [6, 7, 8, 9])
+def test_bigfft_roundoff_every_family_pairing(built, q1, fam_r):
+    """The four-step chain on every (reference, subtitle) pairing of the signal families and the layout
+    families, float and bit-mask subtitle signals (bit masks for the two-level families): error <= tau / 4."""
+    _bigfft_family_cases([(q1, fam_r, fam_s, mode) for fam_s in _BIG_FAMILIES
+                          for mode in ((0, 1) if fam_s not in ("wide", "ramp") else (0,))])
+
+
+@pytest.mark.parametrize("fam_r,fam_s", cases.BIG_TRANSFORM_PAIRS)
+@pytest.mark.parametrize("q1", [10, 11, 12])
+def test_bigfft_roundoff_largest_transforms(built, q1, fam_r, fam_s):
+    """The pairings the GPU runs at 2^22 and 2^23, at M1 = 2^10 .. 2^12, where the column passes and the
+    four-step twiddle grow longest: error <= tau / 4."""
+    _bigfft_family_cases([(q1, fam_r, fam_s, mode) for mode in ((0, 1) if fam_s not in ("wide", "ramp") else (0,))])
 
 
 # --------------------------------------------------------- CPU emulation of the lane-per-window VAD
