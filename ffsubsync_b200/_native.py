@@ -30,7 +30,7 @@ EXPORTS = [
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
-    "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig",
+    "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -130,6 +130,9 @@ def load() -> ctypes.CDLL:
                                        _f64, _i64, _f64, _i64, _vp, _vp, ctypes.c_int]
         lib.b2_capture_nominations.argtypes = [_vp, _vp, _i64, _vp, _vp, _vp]
         lib.b2_capture_reference.argtypes = [_vp, _vp, _i64, _vp, _vp, _i64]
+        lib.b2_apply_sync.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int,
+                                      ctypes.c_int, _f64, ctypes.c_int, _f64, _f64, _f64, ctypes.c_int, _f64,
+                                      _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
         _lib = lib
         return lib
 
@@ -659,6 +662,38 @@ class Handle:
                           memspace, gss=bool(gss), want_evals=want_evals)
 
     # -- diagnostics (tests) --------------------------------------------------------------------
+    def apply_sync(self, best_score, best_offset, best_k, gss_ratio, cue_start_s, cue_end_s, cue_off, ratios,
+                   sample_rate: int, apply_offset_seconds: float = 0.0, gate: bool = False, min_score: float = 0.0,
+                   quality_max_offset_seconds: float = 30.0, max_framerate_deviation: float = 0.1,
+                   suppress: Optional[float] = None, outs=None, memspace: int = B2_HOST):
+        """b2_apply_sync over the T = len(cue_off) - 1 tracks of a finished sync call.  best_* / gss_ratio (None: no
+        search) are that call's outputs in memspace; cue times, cue_off and ratios are host arrays.  B2_HOST: returns
+        numpy (synced_start_us, synced_end_us, offset_seconds, scale, status).  B2_DEVICE: outs holds those five
+        device pointers in that order; enqueued on the handle's stream, returns outs."""
+        cue_off = _i64a(cue_off)
+        T = len(cue_off) - 1
+        if T < 0:
+            raise NativeError(-1, "b2_apply_sync", "cue_off needs at least one entry")
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        if memspace == B2_HOST:
+            best_score = np.ascontiguousarray(best_score, dtype=np.float64)
+            best_offset = np.ascontiguousarray(best_offset, dtype=np.int32)
+            best_k = np.ascontiguousarray(best_k, dtype=np.int32)
+            gss_ratio = None if gss_ratio is None else np.ascontiguousarray(gss_ratio, dtype=np.float64)
+            n = int(cue_off[-1]) if T else 0
+            outs = (np.zeros(n, np.int64), np.zeros(n, np.int64), np.empty(T, np.float64), np.empty(T, np.float64),
+                    np.empty(T, np.int32))
+        st = self.lib.b2_apply_sync(
+            self.h, _ptr(best_score), _ptr(best_offset), _ptr(best_k), _ptr(gss_ratio), T, _ptr(cue_start_s),
+            _ptr(cue_end_s), _ptr(cue_off), _ptr(ratios), len(ratios), int(sample_rate), float(apply_offset_seconds),
+            int(bool(gate)), float(min_score), float(quality_max_offset_seconds), float(max_framerate_deviation),
+            int(suppress is not None), 0.0 if suppress is None else float(suppress), *[_ptr(o) for o in outs],
+            memspace)
+        self._check(st, "b2_apply_sync")
+        return outs
+
     @contextlib.contextmanager
     def capture_nominations(self, n_jobs: int, stride: int):
         """While the block runs, the aligner calls on this handle copy their nomination stage (fp32

@@ -15,8 +15,9 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _native
-from .constants import (BATCH_VADS, DEFAULT_ENERGY_THRESHOLD, DEFAULT_MAX_OFFSET_SECONDS, SAMPLE_RATE,
-                        detector_chunk_bytes)
+from .constants import (BATCH_VADS, DEFAULT_APPLY_OFFSET_SECONDS, DEFAULT_ENERGY_THRESHOLD,
+                        DEFAULT_MAX_FRAMERATE_DEVIATION, DEFAULT_MAX_OFFSET_SECONDS, DEFAULT_MIN_SCORE,
+                        DEFAULT_QUALITY_MAX_OFFSET_SECONDS, SAMPLE_RATE, detector_chunk_bytes)
 
 
 def load_serialized_speech(paths, non_speech_label: float = 0.0, stored: bool = False):
@@ -558,6 +559,61 @@ class BatchSynchronizer:
             self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds,
             self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
         return res if want_all else res[:3]
+
+    def _apply_sync_args(self, apply_offset_seconds, skip_sync_on_low_quality, min_score, quality_max_offset_seconds,
+                         max_framerate_deviation, suppress_output_if_offset_less_than) -> dict:
+        return dict(sample_rate=self.sample_rate, apply_offset_seconds=apply_offset_seconds,
+                    gate=skip_sync_on_low_quality, min_score=min_score,
+                    quality_max_offset_seconds=quality_max_offset_seconds,
+                    max_framerate_deviation=max_framerate_deviation, suppress=suppress_output_if_offset_less_than)
+
+    def apply_sync(self, out, cue_start, cue_end, cue_off, *, apply_offset_seconds: float = DEFAULT_APPLY_OFFSET_SECONDS,
+                   skip_sync_on_low_quality: bool = False, min_score: float = DEFAULT_MIN_SCORE,
+                   quality_max_offset_seconds: float = DEFAULT_QUALITY_MAX_OFFSET_SECONDS,
+                   max_framerate_deviation: float = DEFAULT_MAX_FRAMERATE_DEVIATION,
+                   suppress_output_if_offset_less_than: Optional[float] = None) -> dict:
+        """try_sync's output step (ffsubsync/ffsubsync.py:236-299) over the results of a device sync call: ``out`` is
+        the dict sync_device / sync_device_tracks returned (gss_ratio included with the search), cue_start /
+        cue_end / cue_off the same host cue lists that call took.  Enqueues one kernel on the handle's stream behind
+        that call, without synchronising, and keeps a chain of resident calls intact.  Returns CUDA tensors:
+        ``synced_start_us`` / ``synced_end_us`` int64 per cue (microseconds, as the reference writes them:
+        scaled and shifted, or the originals for a gated or failed track), ``offset_seconds`` / ``scale`` f64 per
+        track (NaN when the alignment failed) and ``status`` i32 per track (sync_output's bits).  The keywords are
+        the reference's options of the same names (``--apply-offset-seconds``, ``--skip-sync-on-low-quality``, ...)."""
+        import torch
+        dev = out["best_score"].device
+        n, T = int(np.asarray(cue_off)[-1]), len(cue_off) - 1
+        res = {"synced_start_us": torch.empty(n, dtype=torch.int64, device=dev),
+               "synced_end_us": torch.empty(n, dtype=torch.int64, device=dev),
+               "offset_seconds": torch.empty(T, dtype=torch.float64, device=dev),
+               "scale": torch.empty(T, dtype=torch.float64, device=dev),
+               "status": torch.empty(T, dtype=torch.int32, device=dev)}
+        gss = out["gss_ratio"].data_ptr() if self.gss else None
+        self.handle.apply_sync(
+            out["best_score"].data_ptr(), out["best_offset"].data_ptr(), out["best_k"].data_ptr(), gss, cue_start,
+            cue_end, cue_off, self.ratios,
+            outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE,
+            **self._apply_sync_args(apply_offset_seconds, skip_sync_on_low_quality, min_score,
+                                    quality_max_offset_seconds, max_framerate_deviation,
+                                    suppress_output_if_offset_less_than))
+        return res
+
+    def apply_sync_host(self, res, cue_start, cue_end, cue_off, *,
+                        apply_offset_seconds: float = DEFAULT_APPLY_OFFSET_SECONDS,
+                        skip_sync_on_low_quality: bool = False, min_score: float = DEFAULT_MIN_SCORE,
+                        quality_max_offset_seconds: float = DEFAULT_QUALITY_MAX_OFFSET_SECONDS,
+                        max_framerate_deviation: float = DEFAULT_MAX_FRAMERATE_DEVIATION,
+                        suppress_output_if_offset_less_than: Optional[float] = None) -> dict:
+        """apply_sync over the numpy results of a host sync call: ``res`` is the tuple sync_host /
+        sync_host_tracks returned (best_score, best_offset, best_k first, gss_ratio last with the search).  Blocks;
+        returns the same keys as apply_sync as numpy arrays."""
+        gss = res[-1] if self.gss else None
+        outs = self.handle.apply_sync(
+            res[0], res[1], res[2], gss, cue_start, cue_end, cue_off, self.ratios, memspace=_native.B2_HOST,
+            **self._apply_sync_args(apply_offset_seconds, skip_sync_on_low_quality, min_score,
+                                    quality_max_offset_seconds, max_framerate_deviation,
+                                    suppress_output_if_offset_less_than))
+        return dict(zip(("synced_start_us", "synced_end_us", "offset_seconds", "scale", "status"), outs))
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
                      refs=None, pgs=None, sig=None):

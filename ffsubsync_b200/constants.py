@@ -39,3 +39,9 @@ def framerate_ratios_to_try(no_fix_framerate: bool = False, gss: bool = False) -
     if gss:
         out.append(None)
     return out
+
+# try_sync's output step (constants.py:19-28): --apply-offset-seconds and the --skip-sync-on-low-quality gate
+DEFAULT_APPLY_OFFSET_SECONDS: int = 0
+DEFAULT_MIN_SCORE: float = 0.0
+DEFAULT_QUALITY_MAX_OFFSET_SECONDS: float = 30.0
+DEFAULT_MAX_FRAMERATE_DEVIATION: float = 0.1

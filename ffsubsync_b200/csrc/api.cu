@@ -13,6 +13,7 @@
 
 #include "common.cuh"
 #include "sync_plan.h"
+#include "sync_output.cuh"
 
 // Entry guard: the handle's device is current for the duration of the call and the caller
 // thread's previous device is restored on every return path.
@@ -1414,4 +1415,87 @@ extern "C" int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm, const int64_t
   r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
   r.sig = {ref_is_sig, x, V > 0 ? sig_off : no_values};
   return sync_run(h, _b2_fence_was_valid, r);
+}
+
+// ---- try_sync's epilogue (sync_output.cu) ----------------------------------------------------------------------
+extern "C" int b2_apply_sync(b2_handle h, const double* best_score, const int32_t* best_offset, const int32_t* best_k,
+                             const double* gss_ratio, int T, const double* cue_start_s, const double* cue_end_s,
+                             const int64_t* cue_off, const double* ratios, int K, int sample_rate,
+                             double apply_offset_seconds, int gate_enabled, double min_score,
+                             double quality_max_offset_seconds, double max_framerate_deviation, int has_suppress,
+                             double suppress_output_if_offset_less_than, int64_t* synced_start_us,
+                             int64_t* synced_end_us, double* offset_seconds, double* scale, int32_t* status,
+                             int memspace) {
+  // Not B2_ENTER: this call only reads outputs already ordered on the handle's stream and writes none of the
+  // buffers a sync call keeps between calls, so a chain of resident sync calls stays valid across it.
+  if (!h) return B2_ERR_BAD_ARG;
+  h->err.clear();
+  DeviceScope scope(h->device);
+  if (!scope.ok) return B2_ERR_CUDA;
+  if (T < 0 || K < 0 || !cue_off) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: bad arguments (T %d, K %d)", T, K);
+  if (sample_rate <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: sample_rate %d <= 0", sample_rate);
+  if (!std::isfinite(apply_offset_seconds))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: apply_offset_seconds %g is not finite", apply_offset_seconds);
+  if (T == 0) return B2_OK;
+  if (!best_score || !best_offset || !best_k) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: null best_score / offset / k");
+  if (!offset_seconds || !scale || !status) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: null offset_seconds / scale / status");
+  if (K && !ratios) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: null ratios");
+  if (cue_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: cue_off[0] %lld < 0", (long long)cue_off[0]);
+  for (int t = 0; t < T; ++t)
+    if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: cue_off not monotone at track %d", t);
+  const int64_t c0 = cue_off[0], n = cue_off[T] - c0;
+  if (n && (!cue_start_s || !cue_end_s)) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: null cue times");
+  if (n && (!synced_start_us || !synced_end_us)) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: null synced_start_us / end_us");
+  double smax = gss_ratio ? 1.1 : 1.0;
+  for (int k = 0; k < K; ++k) {
+    if (!std::isfinite(ratios[k])) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_sync: ratio %d (%g) is not finite", k, ratios[k]);
+    smax = std::max(smax, fabs(ratios[k]));
+  }
+  // every output time is at most |t| * smax + |shift| in magnitude, |shift| <= 2^31 / sample_rate + |apply|: cue
+  // times below this bound stay where the microsecond arithmetic is exact (checked while they are uploaded)
+  const double t_max = (B2_MAX_CUE_SECONDS - 2147483648.0 / sample_rate - fabs(apply_offset_seconds)) / smax;
+  B2_CHECK_DEV(h, memspace, best_score, "apply_sync: best_score");
+  B2_CHECK_DEV(h, memspace, best_offset, "apply_sync: best_offset");
+  B2_CHECK_DEV(h, memspace, best_k, "apply_sync: best_k");
+  B2_CHECK_DEV(h, memspace, gss_ratio, "apply_sync: gss_ratio");
+  B2_CHECK_DEV(h, memspace, offset_seconds, "apply_sync: offset_seconds");
+  B2_CHECK_DEV(h, memspace, scale, "apply_sync: scale");
+  B2_CHECK_DEV(h, memspace, status, "apply_sync: status");
+  if (n) {
+    B2_CHECK_DEV(h, memspace, synced_start_us, "apply_sync: synced_start_us");
+    B2_CHECK_DEV(h, memspace, synced_end_us, "apply_sync: synced_end_us");
+  }
+  const B2SyncRule rule = b2_sync_rule(sample_rate, apply_offset_seconds, gate_enabled, min_score,
+                                       quality_max_offset_seconds, max_framerate_deviation, has_suppress,
+                                       suppress_output_if_offset_less_than);
+  if (memspace == B2_DEVICE)
+    return b2i_apply_sync_launch(h, best_score, best_offset, best_k, gss_ratio, T, cue_start_s, cue_end_s, cue_off,
+                                 t_max, ratios, K, rule, synced_start_us, synced_end_us, offset_seconds, scale, status);
+  // B2_HOST: inputs and outputs staged through the workspaces; cue outputs at their absolute indices
+  void *din, *dout;
+  const size_t Ts = (size_t)T;
+  B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_IN0, Ts * 24 + 64, &din));
+  B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_OUT, (size_t)n * 16 + Ts * 20 + 64, &dout));
+  double* d_bs = (double*)din;
+  double* d_gss = gss_ratio ? d_bs + Ts : nullptr;
+  int32_t* d_bo = (int32_t*)(d_bs + 2 * Ts);
+  int32_t* d_bk = d_bo + Ts;
+  B2_CUDA(h, cudaMemcpyAsync(d_bs, best_score, Ts * 8, cudaMemcpyHostToDevice, h->stream));
+  if (gss_ratio) B2_CUDA(h, cudaMemcpyAsync(d_gss, gss_ratio, Ts * 8, cudaMemcpyHostToDevice, h->stream));
+  B2_CUDA(h, cudaMemcpyAsync(d_bo, best_offset, Ts * 4, cudaMemcpyHostToDevice, h->stream));
+  B2_CUDA(h, cudaMemcpyAsync(d_bk, best_k, Ts * 4, cudaMemcpyHostToDevice, h->stream));
+  int64_t* d_su = (int64_t*)dout;
+  int64_t* d_eu = d_su + n;
+  double* d_off = (double*)(d_eu + n);
+  double* d_sc = d_off + Ts;
+  int32_t* d_st = (int32_t*)(d_sc + Ts);
+  B2_TRY(b2i_apply_sync_launch(h, d_bs, d_bo, d_bk, d_gss, T, cue_start_s, cue_end_s, cue_off, t_max, ratios, K, rule,
+                               d_su - c0, d_eu - c0, d_off, d_sc, d_st));
+  B2_TRY(copy_out(h, synced_start_us + c0, d_su, (size_t)n * 8));
+  B2_TRY(copy_out(h, synced_end_us + c0, d_eu, (size_t)n * 8));
+  B2_TRY(copy_out(h, offset_seconds, d_off, Ts * 8));
+  B2_TRY(copy_out(h, scale, d_sc, Ts * 8));
+  B2_TRY(copy_out(h, status, d_st, Ts * 4));
+  B2_CUDA(h, cudaStreamSynchronize(h->stream));
+  return B2_OK;
 }

@@ -301,3 +301,12 @@ struct B2GssOut {
 };
 int b2i_gss_launch(b2_ctx* h, const float* d_ref, const int64_t* ref_off_host, int V, const int* trk_off, int K,
                    const B2CueSource& src, const double* max_end, int64_t max_offset_samples, const B2GssOut& out);
+// b2_apply_sync's kernel (sync_output.cu): best_* / gss (nullable) / the outputs are DEVICE arrays, cue_start /
+// cue_end / cue_off [T+1] (absolute cue indices, also those of d_start_us / d_end_us) and ratios [K] HOST arrays.
+// Fails with B2_ERR_BAD_ARG before the launch, naming the cue, when a cue time is not finite or |t| >= t_max.
+struct B2SyncRule;
+int b2i_apply_sync_launch(b2_ctx* h, const double* d_bs, const int32_t* d_bo, const int32_t* d_bk,
+                          const double* d_gss, int T, const double* cue_start, const double* cue_end,
+                          const int64_t* cue_off, double t_max, const double* ratios, int K, const B2SyncRule& rule,
+                          int64_t* d_start_us, int64_t* d_end_us, double* d_offset_seconds, double* d_scale,
+                          int32_t* d_status);

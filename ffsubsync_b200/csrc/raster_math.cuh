@@ -57,15 +57,20 @@ RASTER_HD long long b2_rm_rint(double x) {  // half-to-even (the host's default 
 #endif
 }
 
-// timedelta(seconds=t*ratio).total_seconds(): whole seconds exact, fractional part * 1e6 rounded
-// half-to-even to integer microseconds, then one correctly rounded division (no FMA contraction).
-RASTER_HD double b2_scaled_seconds(double t, double ratio) {
-  const double x = b2_rm_mul(t, ratio);
+// timedelta(seconds=x) in integer microseconds: whole seconds exact, fractional part * 1e6 rounded
+// half-to-even (CPython's delta_new; the whole part is a multiple of 1e6, so its parity is even).
+RASTER_HD long long b2_timedelta_us(double x) {
   double whole;
   const double frac = modf(x, &whole);
-  const long long us = (long long)whole * 1000000LL + b2_rm_rint(b2_rm_mul(frac, 1e6));
-  return b2_rm_div((double)us, 1e6);
+  return (long long)whole * 1000000LL + b2_rm_rint(b2_rm_mul(frac, 1e6));
 }
+
+// timedelta(seconds=t*ratio) in microseconds (SubtitleScaler.fit, one correctly rounded product)
+RASTER_HD long long b2_scaled_us(double t, double ratio) { return b2_timedelta_us(b2_rm_mul(t, ratio)); }
+
+// timedelta(seconds=t*ratio).total_seconds(): the microseconds above, then one correctly rounded
+// division (no FMA contraction).
+RASTER_HD double b2_scaled_seconds(double t, double ratio) { return b2_rm_div((double)b2_scaled_us(t, ratio), 1e6); }
 
 // Signal length int(max_time * sample_rate) + 2 (speech_transformers.py:958-962), max_time the largest
 // scaled cue end and at least 0.  max_end: the largest unscaled cue end (0 for a track without cues).

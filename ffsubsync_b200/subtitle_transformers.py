@@ -69,3 +69,23 @@ class SubtitleScaler(TransformerMixin):
 
     def transform(self, *_):
         return self.subs_
+
+
+class SubtitleShifter(TransformerMixin):
+    """The reference's SubtitleShifter (ffsubsync/subtitle_transformers.py:13-26): every cue moved by
+    ``timedelta(seconds=td_seconds)`` (or the timedelta given), for the single-pair Pipeline.  The batched calls'
+    output step is b2_apply_sync (sync_output.py), which reproduces this rounding on the GPU."""
+
+    def __init__(self, td_seconds) -> None:
+        self.td_seconds = td_seconds if isinstance(td_seconds, timedelta) else timedelta(seconds=td_seconds)
+        self.subs_ = None
+
+    def fit(self, subs, *_) -> "SubtitleShifter":
+        if hasattr(subs, "offset"):   # the reference's GenericSubtitlesFile
+            self.subs_ = subs.offset(self.td_seconds)
+        else:
+            self.subs_ = [type(s)(s.start + self.td_seconds, s.end + self.td_seconds, s.inner) for s in subs]
+        return self
+
+    def transform(self, *_):
+        return self.subs_

@@ -406,6 +406,50 @@ int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm /* or NULL without audio 
                        double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                        int memspace);
 
+/* ---- try_sync's epilogue: synced cue times and the low-quality gate ----------------------------------------
+ * What ffsubsync/ffsubsync.py:236-299 does with the aligner's answer, for the T tracks of a finished batched sync
+ * call (any of the calls above, or b2_reduce_ratios): best_score, best_offset, best_k [T] and, when the call ran
+ * the golden-section search, gss_ratio [T] (NULL otherwise) are that call's outputs, in memspace.  Per track t:
+ *   scale          ratios[best_k] for 0 <= best_k < K; gss_ratio[t] for best_k == K with gss_ratio (a value outside
+ *                  [0.9, 1.1] - the search's interval - fails the track); otherwise the track FAILED (the reference's
+ *                  FailedToFindAlignmentException): nothing is written, scale and offset_seconds are NaN.
+ *   offset_seconds best_offset / (double)sample_rate + apply_offset_seconds (two correctly rounded operations).
+ *   status         B2_SYNC_* bits below, in the reference's order: failure, negative score (SUCCESSFUL cleared, the
+ *                  output still written), the gate when gate_enabled (assess_alignment_quality: best_score < min_score,
+ *                  |offset_seconds| > quality_max_offset_seconds, |scale - 1| > max_framerate_deviation, plain IEEE
+ *                  comparisons - a gated track gets its original cues WRITTEN, is not SUCCESSFUL, and the reference
+ *                  leaves its result["offset_seconds"] / ["framerate_scale_factor"] unset), then suppression when
+ *                  has_suppress and suppress_output_if_offset_less_than is not 0.0 (`thresh or -inf`): an
+ *                  offset_seconds below it (or a NaN threshold) is SUPPRESSED instead of WRITTEN.
+ * Per cue i of track t (cue_off[t] <= i < cue_off[t+1]; metadata cues too - the reference writes them), into
+ * synced_start_us[i] / synced_end_us[i] (int64 microseconds): for an APPLIED track
+ * timedelta(seconds=t_i * scale) + timedelta(seconds=offset_seconds) - each rounded half-to-even to the microsecond
+ * on its own (SubtitleScaler, SubtitleShifter) - and timedelta(seconds=t_i) (the parsed original) otherwise.
+ * cue_start_s, cue_end_s, cue_off [T+1] and ratios [K] are host metadata; the outputs follow memspace (B2_HOST copies
+ * back and synchronises; B2_DEVICE enqueues one kernel on the handle's stream behind the call that wrote the inputs
+ * and returns).  Unlike every other entry point it does not break a chain of B2_DEVICE_RESIDENT sync calls.
+ * B2_ERR_BAD_ARG (the message names the item) for a non-monotone cue_off, a non-finite cue time, ratio or
+ * apply_offset_seconds, sample_rate <= 0, a cue time with |t| >= (B2_MAX_CUE_SECONDS - 2^31 / sample_rate -
+ * |apply_offset_seconds|) / smax (smax: the largest of 1, |ratios[k]| and 1.1 with gss_ratio - a bound on every output
+ * time that does not need the device results), a null input or output, and a host pointer under B2_DEVICE. */
+enum {
+  B2_SYNC_WRITTEN = 1,        /* the reference writes this track's output file */
+  B2_SYNC_APPLIED = 2,        /* synced_* hold the scaled and shifted times (else the originals) */
+  B2_SYNC_SUCCESSFUL = 4,     /* the track leaves try_sync's sync_was_successful true */
+  B2_SYNC_FAILED = 8,         /* no alignment (best_k < 0 or out of range) */
+  B2_SYNC_SUPPRESSED = 16,    /* --suppress-output-if-offset-less-than held the output back */
+  B2_SYNC_LOW_SCORE = 32,     /* gate: best_score < min_score */
+  B2_SYNC_LOW_OFFSET = 64,    /* gate: |offset_seconds| > quality_max_offset_seconds */
+  B2_SYNC_LOW_FRAMERATE = 128 /* gate: |scale - 1| > max_framerate_deviation */
+};
+int b2_apply_sync(b2_handle h, const double* best_score, const int32_t* best_offset, const int32_t* best_k,
+                  const double* gss_ratio /* [T] or NULL */, int T, const double* cue_start_s, const double* cue_end_s,
+                  const int64_t* cue_off /* [T+1] */, const double* ratios, int K, int sample_rate,
+                  double apply_offset_seconds, int gate_enabled, double min_score, double quality_max_offset_seconds,
+                  double max_framerate_deviation, int has_suppress, double suppress_output_if_offset_less_than,
+                  int64_t* synced_start_us, int64_t* synced_end_us, double* offset_seconds /* [T] */,
+                  double* scale /* [T] */, int32_t* status /* [T] */, int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before
