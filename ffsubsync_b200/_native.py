@@ -31,9 +31,11 @@ EXPORTS = [
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
+    "b2_sync_tracks_seg",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
+B2_BEST_K_NO_SPEECH = -3    # best_k of the tracks of a video whose sampled segments hold no speech (b2_sync_tracks_seg)
 GSS_EVALS = 17   # evaluations of the golden-section search over [0.9, 1.1] with tolerance 1e-4
 
 
@@ -116,6 +118,8 @@ def load() -> ctypes.CDLL:
                                            _f64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                            _vp, _vp, _vp, _vp, ctypes.c_int, _f64, _i64, _vp, _vp, _vp, _vp, _vp,
                                            _vp, _vp, ctypes.c_int]
+        lib.b2_sync_tracks_seg.argtypes = (lib.b2_sync_tracks_sig.argtypes[:30] + [ctypes.c_int] + [_vp] * 6
+                                           + lib.b2_sync_tracks_sig.argtypes[30:])
         lib.b2_synth_pcm.argtypes = [_vp, _vp, _i64, ctypes.c_int, ctypes.c_uint32, _vp, ctypes.c_int]
         lib.b2_vad_stream_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _f32, _i64, ctypes.c_int,
                                             ctypes.c_int]
@@ -657,6 +661,62 @@ class Handle:
                            _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
                            _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off),
                            _ptr(ref_is_sig), _ptr(x), _ptr(sig_off)),
+                          cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
+                          (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
+                          memspace, gss=bool(gss), want_evals=want_evals)
+
+    def sync_tracks_seg(self, pcm, pcm_off, track_video, frame_rate: int, sample_rate: int, non_speech_label: float,
+                        seg_video, seg_total, seg_off, seg_start, seg_lo, seg_hi, cue_start_s, cue_end_s, cue_keep,
+                        cue_off, ratios, start_seconds: float, max_offset_samples: Optional[int], ref_is_sig=None, x=None,
+                        sig_off=None, ref_is_subs=None, ref_cue_start_s=None, ref_cue_end_s=None, ref_cue_keep=None,
+                        ref_cue_off=None, ref_is_pgs=None, pgs_start_s=None, pgs_end_s=None, pgs_off=None,
+                        detector: int = B2_DETECTOR_ENERGY_ZCR, energy_threshold: int = 0, z_lo: int = -1,
+                        z_hi: int = -1, chunk_samples: int = 0, energy_threshold_db: float = 50.0,
+                        min_length: Optional[float] = None, max_length: Optional[int] = None,
+                        max_continuous_silence: Optional[float] = None, gss: bool = False, best_score=None,
+                        best_offset=None, best_k=None, all_score=None, all_offset=None, gss_ratio=None, gss_evals=None,
+                        want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST):
+        """sync_tracks_sig where the P videos seg_video [P] (increasing) take MultiSegmentVideoSpeechTransformer.fit's
+        sparse reference of their sampled segments (b2_sync_tracks_seg): video seg_video[i] has the probed duration
+        seg_total[i] seconds and the segments seg_off[i] .. seg_off[i+1]-1, segment j starting at seg_start[j] whole
+        seconds with the samples pcm_off[v] + seg_lo[j] .. pcm_off[v] + seg_hi[j] (host arrays).  The signal, text and
+        PGS references are optional.  A video without speech in its segments gets best_k = B2_BEST_K_NO_SPEECH on
+        every track.  Returns as sync_tracks_subs."""
+        V, T = len(pcm_off) - 1, len(track_video)
+        seg_video = np.ascontiguousarray(seg_video, dtype=np.int32)
+        seg_total = np.ascontiguousarray(seg_total, dtype=np.float64)
+        seg_off = _i64a(seg_off)
+        P = len(seg_video)
+        if len(cue_off) != T + 1 or len(seg_off) != P + 1 or len(seg_total) != P:
+            raise NativeError(-1, "b2_sync_tracks_seg", "cue_off / seg_off / seg_total have %d / %d / %d entries for "
+                              "%d tracks / %d segment videos" % (len(cue_off), len(seg_off), len(seg_total), T, P))
+        seg_start, seg_lo, seg_hi = (_i64a(a) for a in (seg_start, seg_lo, seg_hi))
+        if not (len(seg_start) == len(seg_lo) == len(seg_hi) >= (seg_off[-1] if P else 0)):
+            raise NativeError(-1, "b2_sync_tracks_seg", "seg_start / seg_lo / seg_hi have %d / %d / %d entries for %d "
+                              "segments" % (len(seg_start), len(seg_lo), len(seg_hi), int(seg_off[-1]) if P else 0))
+        u8 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.uint8)   # noqa: E731
+        ref_is_sig, ref_is_pgs, ref_is_subs = u8(ref_is_sig), u8(ref_is_pgs), u8(ref_is_subs)
+        for name, a in (("ref_is_sig", ref_is_sig), ("ref_is_pgs", ref_is_pgs), ("ref_is_subs", ref_is_subs)):
+            if a is not None and len(a) != V:
+                raise NativeError(-1, "b2_sync_tracks_seg", "%s has %d entries for %d videos" % (name, len(a), V))
+        for name, off in (("ref_cue_off", ref_cue_off), ("pgs_off", pgs_off), ("sig_off", sig_off)):
+            if off is not None and len(off) != V + 1:
+                raise NativeError(-1, "b2_sync_tracks_seg", "%s has %d entries for %d videos" % (name, len(off), V))
+        ref_cue_off, pgs_off, sig_off = (None if a is None else _i64a(a) for a in (ref_cue_off, pgs_off, sig_off))
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)   # noqa: E731
+        if x is not None and not isinstance(x, int):
+            x = f64(x)
+        pgs_start_s, pgs_end_s = f64(pgs_start_s), f64(pgs_end_s)
+        ref_cue_start_s, ref_cue_end_s = f64(ref_cue_start_s), f64(ref_cue_end_s)
+        ref_cue_keep = u8(ref_cue_keep)
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        return self._sync("b2_sync_tracks_seg", pcm, pcm_off, track_video,
+                          (frame_rate, sample_rate, int(detector), float(non_speech_label), int(energy_threshold),
+                           int(z_lo), int(z_hi), float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
+                           _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
+                           _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off),
+                           _ptr(ref_is_sig), _ptr(x), _ptr(sig_off), P, _ptr(seg_video), _ptr(seg_total),
+                           _ptr(seg_off), _ptr(seg_start), _ptr(seg_lo), _ptr(seg_hi)),
                           cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
                           (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
                           memspace, gss=bool(gss), want_evals=want_evals)

@@ -45,6 +45,57 @@ _STREAM_ARGS = ("ref_cue_start", "ref_cue_end", "ref_cue_off", "ref_stream_video
 _PGS_ARGS = ("pgs_start", "pgs_end", "pgs_off", "pgs_video")
 # keyword arguments of the sync methods that give videos a serialized speech signal as reference
 _SIG_ARGS = ("sig", "sig_off", "sig_video")
+# keyword arguments of the sync methods that give videos sampled segments as reference (--multi-segment-sync)
+_SEG_ARGS = ("seg_video", "seg_total", "seg_off", "seg_start", "seg_lo", "seg_hi")
+_NO_SPEECH_MESSAGE = ("Unable to detect speech in any sampled segment. "
+                      "Perhaps try specifying a different stream / track, or a different vad.")
+
+
+def segment_table(pcm_off, frame_rate: int, videos=None, totals=None, segment_count: int = 8,
+                  segment_duration: int = 60, skip_intro_outro: bool = False, piece_samples=None) -> dict:
+    """The segment keyword arguments of the sync methods (``--multi-segment-sync``) for the videos ``videos`` (default:
+    every video of pcm_off [V+1]), with the reference's knobs ``segment_count``, ``segment_duration`` and
+    ``skip_intro_outro``.  Each video's starts are MultiSegmentVideoSpeechTransformer._segment_starts of its duration
+    ``totals[i]`` (seconds, e.g. ffprobe's; default: its samples / frame_rate, as the transformer probes raw PCM).
+    Two layouts of a video's PCM range:
+    - ``piece_samples`` None: the range holds the video's whole decode; segment s is the slice lo = min(n, round(s *
+      frame_rate)), hi = min(n, lo + round(segment_duration * frame_rate)).
+    - ``piece_samples[i]``: the range holds only the sampled windows (``ffmpeg -ss s -t segment_duration``) back to
+      back in start order, with these sample counts (one per start; a short last piece is fine).
+    Returns dict(seg_video, seg_total, seg_off, seg_start, seg_lo, seg_hi)."""
+    from .speech_transformers import MultiSegmentVideoSpeechTransformer
+    pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+    V = len(pcm_off) - 1
+    videos = np.arange(V) if videos is None else np.ascontiguousarray(videos, dtype=np.int64)
+    t = MultiSegmentVideoSpeechTransformer(vad="energy", sample_rate=SAMPLE_RATE, frame_rate=frame_rate,
+                                           non_speech_label=0.0, segment_count=segment_count,
+                                           segment_duration=segment_duration, skip_intro_outro=skip_intro_outro)
+    total_out, off, start, lo, hi = [], [0], [], [], []
+    for i, v in enumerate(videos):
+        n = int(pcm_off[v + 1] - pcm_off[v])
+        total = float(totals[i]) if totals is not None else n / float(frame_rate)
+        starts = t._segment_starts(total)
+        if piece_samples is None:
+            for s in starts:
+                a = min(n, int(round(s * frame_rate)))
+                lo.append(a)
+                hi.append(min(n, a + int(round(segment_duration * frame_rate))))
+        else:
+            pieces = [int(x) for x in piece_samples[i]]
+            if len(pieces) != len(starts) or sum(pieces) != n:
+                raise ValueError("video %d: %d decoded pieces of %d samples for %d starts in a range of %d samples"
+                                 % (int(v), len(pieces), sum(pieces), len(starts), n))
+            at = 0
+            for m in pieces:
+                lo.append(at)
+                hi.append(at + m)
+                at += m
+        start += [int(s) for s in starts]
+        total_out.append(total)
+        off.append(len(start))
+    return dict(seg_video=np.asarray(videos, dtype=np.int32), seg_total=np.asarray(total_out, dtype=np.float64),
+                seg_off=np.asarray(off, dtype=np.int64), seg_start=np.asarray(start, dtype=np.int64),
+                seg_lo=np.asarray(lo, dtype=np.int64), seg_hi=np.asarray(hi, dtype=np.int64))
 
 
 def _is_unsupported(e: Exception) -> bool:
@@ -139,19 +190,26 @@ class BatchSynchronizer:
         refs = self._subs_refs(V, streams)
         if refs is None or pgs is None or not np.any(refs[0] & pgs[0]):
             return refs, pgs
-        is_subs, rs, re_, rk, roff = refs
-        keep_v = (is_subs != 0) & (pgs[0] == 0)
-        pick = np.concatenate([np.arange(roff[v], roff[v + 1]) for v in range(V) if keep_v[v]]
-                              + [np.zeros(0, np.int64)]).astype(np.int64)
-        lens = np.where(keep_v, np.diff(roff), 0)
-        return ((keep_v.astype(np.uint8), rs[pick], re_[pick], None if rk is None else rk[pick],
-                 np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)), pgs)
+        return self._drop_text(V, refs, pgs[0] != 0), pgs
 
     def _all_refs(self, V: int, streams: dict, on_device: bool):
-        """(refs, pgs, sig) of the keyword arguments: refs and pgs from _references, sig from _sig_refs.  A video with
-        a signal and a text or PGS reference is refused: the reference tool's reference is a single file."""
+        """(refs, pgs, sig, seg) of the keyword arguments: refs and pgs from _references, sig from _sig_refs, seg from
+        _seg_refs.  A video with a signal and a text or PGS reference is refused: the reference tool's reference is a
+        single file.  So is a video with segments and a PGS or signal reference; its text streams are dropped, since
+        sampling is audio-only (the reference drops a ``subs_then_`` prefix)."""
+        seg = self._seg_refs(V, {k: streams.pop(k) for k in _SEG_ARGS if k in streams})
         sig = self._sig_refs(V, {k: streams.pop(k) for k in _SIG_ARGS if k in streams}, on_device)
         refs, pgs = self._references(V, streams)
+        if seg is not None:
+            is_seg = np.zeros(V, dtype=bool)
+            is_seg[seg[0]] = True
+            for r, what in ((pgs, "a PGS reference"), (sig, "a serialized signal")):
+                both = np.flatnonzero(is_seg & (r[0] != 0)) if r is not None else []
+                if len(both):
+                    raise ValueError("video %d has sampled segments and %s; a video has one reference"
+                                     % (int(both[0]), what))
+            if refs is not None and np.any(is_seg & (refs[0] != 0)):
+                refs = self._drop_text(V, refs, is_seg)
         if sig is not None:
             other = np.zeros(V, dtype=bool)
             for r in (refs, pgs):
@@ -161,7 +219,47 @@ class BatchSynchronizer:
             if len(both):
                 raise ValueError("video %d has a serialized signal and a text / PGS reference; a video has one "
                                  "reference" % int(both[0]))
-        return refs, pgs, sig
+        return refs, pgs, sig, seg
+
+    @staticmethod
+    def _drop_text(V: int, refs, drop):
+        """refs (from _subs_refs) without the text streams of the videos where drop[v] is set."""
+        is_subs, rs, re_, rk, roff = refs
+        keep_v = (is_subs != 0) & ~drop
+        pick = np.concatenate([np.arange(roff[v], roff[v + 1]) for v in range(V) if keep_v[v]]
+                              + [np.zeros(0, np.int64)]).astype(np.int64)
+        lens = np.where(keep_v, np.diff(roff), 0)
+        return (keep_v.astype(np.uint8), rs[pick], re_[pick], None if rk is None else rk[pick],
+                np.concatenate([[0], np.cumsum(lens)]).astype(np.int64))
+
+    @staticmethod
+    def _seg_refs(V: int, args: dict):
+        """The segment table, or None when none is given: (seg_video i32, seg_total f64, seg_off, seg_start, seg_lo,
+        seg_hi int64) for b2_sync_tracks_seg (e.g. from segment_table)."""
+        if all(args.get(k) is None for k in _SEG_ARGS):
+            return None
+        missing = [k for k in _SEG_ARGS if args.get(k) is None]
+        if missing:
+            raise ValueError("segment references need %s" % ", ".join(_SEG_ARGS))
+        video = np.ascontiguousarray(args["seg_video"], dtype=np.int32)
+        if len(video) and (np.any(np.diff(video) <= 0) or video[0] < 0 or video[-1] >= V):
+            raise ValueError("seg_video must be increasing video indices in [0, %d) (one segment table per video)" % V)
+        return (video, np.ascontiguousarray(args["seg_total"], dtype=np.float64)) + tuple(
+            np.ascontiguousarray(args[k], dtype=np.int64) for k in ("seg_off", "seg_start", "seg_lo", "seg_hi"))
+
+    @staticmethod
+    def _no_speech_videos(seg, best_k, track_video):
+        """The segment videos whose tracks got B2_BEST_K_NO_SPEECH, ascending."""
+        if seg is None:
+            return []
+        bk = np.asarray(best_k)
+        return sorted({int(track_video[t]) for t in np.flatnonzero(bk == _native.B2_BEST_K_NO_SPEECH)})
+
+    def _raise_no_speech(self, seg, best_k, track_video) -> None:
+        """The host methods' error for the sentinel best_k == B2_BEST_K_NO_SPEECH."""
+        vids = self._no_speech_videos(seg, best_k, track_video)
+        if vids:
+            raise ValueError("video %d: %s" % (vids[0], _NO_SPEECH_MESSAGE))
 
     def _sig_refs(self, V: int, args: dict, on_device: bool):
         """Each video's stored signal, or None when none is given: returns (ref_is_sig u8[V], x float64, sig_off
@@ -270,7 +368,7 @@ class BatchSynchronizer:
                                         content=streams.get("ref_cue_content"), keep=streams.get("ref_cue_keep"))
 
     def _dispatch(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, gss: bool, pgs=None,
-                  sig=None, **kw):
+                  sig=None, seg=None, **kw):
         """The batched call of this synchroniser's detector with the search on or off: b2_sync_tracks_pgs with PGS
         references (pgs, from _pgs_refs), else b2_sync_tracks_subs with subtitle references (refs, from _subs_refs), else b2_sync_tracks_auditok for auditok, else
         b2_sync_tracks_gss / b2_sync_tracks; b2_sync_tracks_sig with signal references (sig, from _sig_refs, with
@@ -280,6 +378,20 @@ class BatchSynchronizer:
         h = self.handle
         p = pcm if pcm is None or isinstance(pcm, np.ndarray) else pcm.data_ptr()
         cues = (cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds, self.max_offset_samples)
+        if seg is not None:   # b2_sync_tracks_seg, with any of the other references
+            det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
+            other = {} if refs is None else dict(zip(("ref_is_subs", "ref_cue_start_s", "ref_cue_end_s",
+                                                      "ref_cue_keep", "ref_cue_off"), refs))
+            if pgs is not None:
+                other.update(zip(("ref_is_pgs", "pgs_start_s", "pgs_end_s", "pgs_off"), pgs))
+            if sig is not None:
+                is_sig, x, voff = sig
+                other.update(ref_is_sig=is_sig, x=x if isinstance(x, np.ndarray) else (x.data_ptr() if x.numel()
+                                                                                       else None), sig_off=voff)
+            return h.sync_tracks_seg(p, pcm_off, track_video, self.frame_rate, self.sample_rate,
+                                     self.non_speech_label, *seg, *cues, detector=det,
+                                     energy_threshold=self.energy_threshold, z_lo=self.z_lo, z_hi=self.z_hi,
+                                     chunk_samples=self.chunk_samples, gss=gss, **other, **kw)
         if sig is not None:
             det = _native.B2_DETECTOR_AUDITOK if self.auditok else _native.B2_DETECTOR_ENERGY_ZCR
             is_sig, x, voff = sig
@@ -313,20 +425,21 @@ class BatchSynchronizer:
         return (h.sync_tracks_gss if gss else h.sync_tracks)(p, pcm_off, track_video, *energy, *cues, **kw)
 
     def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=None,
-                         sig=None, **kw):
+                         sig=None, seg=None, **kw):
         """_dispatch with this synchroniser's search.  Outside the envelope of the device-driven search
         (B2_ERR_UNSUPPORTED) the search is composed of public steps instead (_gss_compose).  Returns
         (best_score, best_offset, best_k, all_score, all_offset), plus gss_ratio with the search; composed results
         are numpy arrays (all_* None unless want_all or device outputs were given)."""
         try:
             return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
-                                  pgs=pgs, sig=sig, **kw)[:6]
+                                  pgs=pgs, sig=sig, seg=seg, **kw)[:6]
         except _native.NativeError as e:
             if not (self.gss and _is_unsupported(e)):
                 raise
         want_all = kw.get("want_all", False) or kw.get("all_score") is not None
         bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off,
-                                                        cue_keep, want_all=want_all, refs=refs, pgs=pgs, sig=sig)
+                                                        cue_keep, want_all=want_all, refs=refs, pgs=pgs, sig=sig,
+                                                        seg=seg)
         return bs, bo, bk, a_s, a_o, ratio
 
     def use_torch_stream(self) -> None:
@@ -350,7 +463,7 @@ class BatchSynchronizer:
         B = len(pcm_off) - 1
         K = len(self.ratios)
         if (self.gss or self.auditok or self.subs_then
-                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS)):   # the identity track map: pair b is track b of video b
+                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS + _SEG_ARGS)):   # the identity track map: pair b is track b of video b
             return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
                                            cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident,
                                            **streams)
@@ -388,7 +501,7 @@ class BatchSynchronizer:
         import torch
         T = len(track_video)
         sig_in = streams.get("sig")
-        refs, pgs, sig = self._all_refs(len(pcm_off) - 1, streams, on_device=True)
+        refs, pgs, sig, seg = self._all_refs(len(pcm_off) - 1, streams, on_device=True)
         dev = pcm.device if pcm is not None else torch.device("cuda", self.handle.device)
         if out is None:
             out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
@@ -405,7 +518,7 @@ class BatchSynchronizer:
             # a converted copy: ready before the handle's stream reads it, and kept until the call is done
             torch.cuda.current_stream(sig[1].device).synchronize()
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    sig=sig, memspace=memspace, **ptrs)
+                                    sig=sig, seg=seg, memspace=memspace, **ptrs)
         if sig is not None and sig[1] is not sig_in:
             self.handle.synchronize()
         if isinstance(res[0], np.ndarray):   # composed on the host
@@ -421,10 +534,11 @@ class BatchSynchronizer:
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
         track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks."""
-        refs, pgs, sig = self._all_refs(len(pcm_off) - 1, streams, on_device=False)
+        refs, pgs, sig, seg = self._all_refs(len(pcm_off) - 1, streams, on_device=False)
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    sig=sig, want_all=want_all, memspace=_native.B2_HOST)
+                                    sig=sig, seg=seg, want_all=want_all, memspace=_native.B2_HOST)
         self._raise_bad_signals(sig, res[2])
+        self._raise_no_speech(seg, res[2], track_video)
         return res if want_all else res[:3] + res[5:]
 
     def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None):
@@ -489,9 +603,13 @@ class BatchSynchronizer:
         if self.subs_then:
             raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
                              "embedded subtitle references (vad=%r)" % self.vad)
-        unknown = set(pgs_args) - set(_PGS_ARGS + _SIG_ARGS)
+        unknown = set(pgs_args) - set(_PGS_ARGS + _SIG_ARGS + _SEG_ARGS)
         if unknown:
             raise TypeError("unexpected keyword arguments %s" % ", ".join(sorted(unknown)))
+        given_seg = sorted(k for k in _SEG_ARGS if pgs_args.pop(k, None) is not None)
+        if given_seg:
+            raise ValueError("sync_device_candidate_sharded runs the detector on every video's whole audio; it does "
+                             "not take sampled segment references (%s)" % ", ".join(given_seg))
         given_sig = sorted(k for k in _SIG_ARGS if pgs_args.get(k) is not None)
         if given_sig:
             raise ValueError("sync_device_candidate_sharded runs the detector on every video; it does not take "
@@ -550,7 +668,7 @@ class BatchSynchronizer:
         with the golden-section search.  With a ``subs_then_`` detector the embedded subtitle streams come as
         keyword arguments, and with any detector the PGS references and the serialized signals (see the class)."""
         if (self.gss or self.auditok or self.subs_then
-                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS)):
+                or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS + _SEG_ARGS)):
             return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
                                          cue_end, cue_off, cue_keep, want_all=want_all, **streams)
         self._references(len(pcm_off) - 1, streams)   # rejects streams and unknown keywords
@@ -616,7 +734,7 @@ class BatchSynchronizer:
         return dict(zip(("synced_start_us", "synced_end_us", "offset_seconds", "scale", "status"), outs))
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
-                     refs=None, pgs=None, sig=None):
+                     refs=None, pgs=None, sig=None, seg=None):
         """The golden-section search outside the envelope of the device-driven search, composed of public steps:
         the grid (this synchroniser's batched call with the search off), gss_align_batch on each track's reference
         signal (_reference_signals, with subtitle references refs from _subs_refs) and the reference's combine.
@@ -641,8 +759,8 @@ class BatchSynchronizer:
             torch.cuda.synchronize(sig[1].device)
             sig = (sig[0], sig[1].cpu().numpy(), sig[2])
         grid = self._dispatch(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, False,
-                              pgs=pgs, sig=sig, want_all=True, memspace=_native.B2_HOST)
-        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs, sig)
+                              pgs=pgs, sig=sig, seg=seg, want_all=True, memspace=_native.B2_HOST)
+        ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs, sig, seg)
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
@@ -651,20 +769,28 @@ class BatchSynchronizer:
                             self.sample_rate, self.start_seconds, handle=h)
         bs, bo, bk, ratio, a_s, a_o = combine_gss(grid[0], grid[1], grid[2], g, K, self.max_offset_samples,
                                                   grid[3], grid[4])
+        marked = []
         if sig is not None:
-            for t in np.flatnonzero(np.isin(track_video, list(self._bad_signals(sig)))):
-                bs[t], bo[t], bk[t], ratio[t] = np.nan, 0, _native.B2_BEST_K_BAD_SIGNAL, np.nan
+            marked.append((list(self._bad_signals(sig)), _native.B2_BEST_K_BAD_SIGNAL))
+        if seg is not None:
+            marked.append((self._no_speech_videos(seg, grid[2], track_video), _native.B2_BEST_K_NO_SPEECH))
+        for vids, sentinel in marked:
+            for t in np.flatnonzero(np.isin(track_video, vids)):
+                bs[t], bo[t], bk[t], ratio[t] = np.nan, 0, sentinel, np.nan
                 a_s[t * (K + 1): (t + 1) * (K + 1)] = np.nan
                 a_o[t * (K + 1): (t + 1) * (K + 1)] = 0
         return (bs, bo, bk, ratio) + ((a_s, a_o) if want_all else (None, None))
 
-    def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None, sig=None):
+    def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None, sig=None, seg=None):
         """The per-video reference signals the batched calls sync against, composed of public calls: the detector
         (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, with subtitle references
         (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0, and
         with PGS references (pgs, from _pgs_refs) for a video that has one b2_rasterize_pgs of its intervals, and with
         signal references (sig, from _sig_refs, on the host) for a video that has one DeserializeSpeechTransformer's
-        rule at this synchroniser's label, in float64, rounded once to float32.
+        rule at this synchroniser's label, in float64, rounded once to float32, and with segment references (seg, from
+        _seg_refs) for a video that has them the detector over each segment's samples as one signal (b2_vad_energy_zcr,
+        or b2_vad_auditok with the chunk loop rounded to float32), placed by MultiSegmentVideoSpeechTransformer.fit's
+        rule (segment_oracle.assemble's, in start order) into int(total * sample_rate) + 2 frames of 0.0.
         Returns (float32 signals back to back, ref_off int64[V+1])."""
         h = self.handle
         V = len(pcm_off) - 1
@@ -676,7 +802,7 @@ class BatchSynchronizer:
         else:
             det, det_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
                                             self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
-        if refs is None and pgs is None and sig is None:
+        if refs is None and pgs is None and sig is None and seg is None:
             return det.astype(np.float32), det_off
         parts = [det[det_off[v]: det_off[v + 1]].astype(np.float32) for v in range(V)]
         if refs is not None:
@@ -698,6 +824,27 @@ class BatchSynchronizer:
             for v in np.flatnonzero(is_sig):
                 xv = x[voff[v]: voff[v + 1]]
                 parts[v] = np.where(xv < 1.0, np.float64(self.non_speech_label), xv).astype(np.float32)
+        if seg is not None:
+            video, total, s_off, s_start, s_lo, s_hi = seg
+            for i, v in enumerate(video):
+                js = range(int(s_off[i]), int(s_off[i + 1]))
+                pieces = [pcm_host[pcm_off[v] + s_lo[j]: pcm_off[v] + s_hi[j]] for j in js]
+                p_off = np.concatenate([[0], np.cumsum([len(q) for q in pieces])]).astype(np.int64)
+                flat = np.concatenate(pieces + [np.zeros(0, np.int16)]).astype(np.int16)
+                if self.auditok:
+                    d, d_off = h.vad_auditok(flat, p_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                                             chunk_samples=self.chunk_samples)
+                else:
+                    d, d_off = h.vad_energy_zcr(flat, p_off, self.frame_rate, self.sample_rate,
+                                                self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+                L = int(float(total[i]) * self.sample_rate) + 2
+                x = np.zeros(L, dtype=np.float32)
+                for k, j in enumerate(js):
+                    b = int(s_start[j]) * self.sample_rate
+                    e = min(b + int(d_off[k + 1] - d_off[k]), L)
+                    if e > b:
+                        x[b:e] = d[d_off[k]: d_off[k] + (e - b)].astype(np.float32)
+                parts[v] = x
         off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
         return (np.concatenate(parts) if parts else np.zeros(0, np.float32)), off
 

@@ -305,13 +305,38 @@ struct CopyCrew {
   std::atomic<bool> abort{false};
 };
 
-static void copy_slice(char* dst, const char* src, size_t n, int t, int nthreads) {
-  const size_t per = ((n / nthreads) + 4095) & ~(size_t)4095;
-  const size_t lo = std::min(n, per * (size_t)t), hi = t == nthreads - 1 ? n : std::min(n, per * (size_t)(t + 1));
-  if (hi > lo) memcpy(dst + lo, src + lo, hi - lo);
+// The bytes [at[i], at[i] + len[i]) of host and device buffers, ascending and disjoint, read as one stream: stream byte
+// s lies in range i where sum(len[0 .. i-1]) <= s < sum(len[0 .. i]) (pre[i] = that sum).
+struct ByteRanges {
+  std::vector<size_t> at, len, pre;
+  void add(size_t a, size_t n) {
+    if (!n) return;
+    pre.push_back(pre.empty() ? 0 : pre.back() + len.back());
+    at.push_back(a);
+    len.push_back(n);
+  }
+  size_t total() const { return pre.empty() ? 0 : pre.back() + len.back(); }
+  size_t find(size_t s) const { return (size_t)(std::upper_bound(pre.begin(), pre.end(), s) - pre.begin()) - 1; }
+};
+
+// Copy stream bytes [s0, s0 + n) of `host` (ranges rg) to dst
+static void gather(char* dst, const char* host, const ByteRanges& rg, size_t s0, size_t n) {
+  for (size_t i = n ? rg.find(s0) : 0, done = 0; done < n; ++i) {
+    const size_t off = s0 + done - rg.pre[i], m = std::min(n - done, rg.len[i] - off);
+    memcpy(dst + done, host + rg.at[i] + off, m);
+    done += m;
+  }
 }
 
-static int staged_h2d(b2_ctx* h, void* dev, const void* host, size_t bytes) {
+static void copy_slice(char* dst, const char* host, const ByteRanges& rg, size_t s0, size_t n, int t, int nthreads) {
+  const size_t per = ((n / nthreads) + 4095) & ~(size_t)4095;
+  const size_t lo = std::min(n, per * (size_t)t), hi = t == nthreads - 1 ? n : std::min(n, per * (size_t)(t + 1));
+  if (hi > lo) gather(dst + lo, host, rg, s0 + lo, hi - lo);
+}
+
+// The ranges rg of host to the same positions of dev (one range [0, bytes): the whole buffer)
+static int staged_h2d(b2_ctx* h, void* dev, const void* host, const ByteRanges& rg) {
+  const size_t bytes = rg.total();
   for (auto& b : h->bounce)
     if (!b.p) {
       B2_CUDA(h, cudaMallocHost(&b.p, kBounceBytes));
@@ -328,7 +353,7 @@ static int staged_h2d(b2_ctx* h, void* dev, const void* host, size_t bytes) {
         std::this_thread::yield();
       }
       const size_t off = (size_t)c * kBounceBytes, n = std::min(kBounceBytes, bytes - off);
-      copy_slice((char*)h->bounce[c & 1].p, (const char*)host + off, n, t, nthreads);
+      copy_slice((char*)h->bounce[c & 1].p, (const char*)host, rg, off, n, t, nthreads);
       crew.done.fetch_add(1, std::memory_order_release);
     }
   };
@@ -350,11 +375,16 @@ static int staged_h2d(b2_ctx* h, void* dev, const void* host, size_t bytes) {
       break;
     }
     crew.ready.store(c, std::memory_order_release);
-    copy_slice((char*)b.p, (const char*)host + off, n, 0, nthreads);
+    copy_slice((char*)b.p, (const char*)host, rg, off, n, 0, nthreads);
     while (crew.done.load(std::memory_order_acquire) < (c + 1) * (nthreads - 1)) std::this_thread::yield();
-    if (cudaMemcpyAsync((char*)dev + off, b.p, n, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaEventRecord(b.ev, h->stream) != cudaSuccess)
-      status = B2_ERR_CUDA;
+    for (size_t i = rg.find(off), done = 0; done < n && status == B2_OK; ++i) {   // one copy per range piece
+      const size_t o = off + done - rg.pre[i], m = std::min(n - done, rg.len[i] - o);
+      if (cudaMemcpyAsync((char*)dev + rg.at[i] + o, (char*)b.p + done, m, cudaMemcpyHostToDevice, h->stream) !=
+          cudaSuccess)
+        status = B2_ERR_CUDA;
+      done += m;
+    }
+    if (status == B2_OK && cudaEventRecord(b.ev, h->stream) != cudaSuccess) status = B2_ERR_CUDA;
   }
   if (status != B2_OK) crew.abort.store(true);
   crew.ready.store(n_chunks, std::memory_order_release);
@@ -366,8 +396,27 @@ static int staged_h2d(b2_ctx* h, void* dev, const void* host, size_t bytes) {
 static int stage_in(b2_ctx* h, int which, const void* host, size_t bytes, void** dev) {
   B2_TRY(b2i_ws(h, which, bytes ? bytes : 16, dev));
   if (!bytes) return B2_OK;
-  if (bytes >= kBounceBytes / 2 && is_pageable(host)) return staged_h2d(h, *dev, host, bytes);
+  if (bytes >= kBounceBytes / 2 && is_pageable(host)) {
+    ByteRanges rg;
+    rg.add(0, bytes);
+    return staged_h2d(h, *dev, host, rg);
+  }
   B2_CUDA(h, cudaMemcpyAsync(*dev, host, bytes, cudaMemcpyHostToDevice, h->stream));
+  return B2_OK;
+}
+
+// stage_in of the int16 sample ranges [lo[i], hi[i]) (ascending, disjoint) of a buffer of `bytes` bytes: the device
+// workspace spans the whole buffer, and only those ranges are copied, to their own positions (b2_sync_tracks_seg: the
+// sampled segments and the audio videos, not the samples between segments).
+static int stage_ranges(b2_ctx* h, int which, const void* host, size_t bytes, const std::vector<int64_t>& lo,
+                        const std::vector<int64_t>& hi, void** dev) {
+  B2_TRY(b2i_ws(h, which, bytes ? bytes : 16, dev));
+  ByteRanges rg;
+  for (size_t i = 0; i < lo.size(); ++i) rg.add((size_t)lo[i] * 2, (size_t)(hi[i] - lo[i]) * 2);
+  if (rg.total() >= kBounceBytes / 2 && is_pageable(host)) return staged_h2d(h, *dev, host, rg);
+  for (size_t i = 0; i < rg.at.size(); ++i)
+    B2_CUDA(h, cudaMemcpyAsync((char*)*dev + rg.at[i], (const char*)host + rg.at[i], rg.len[i], cudaMemcpyHostToDevice,
+                               h->stream));
   return B2_OK;
 }
 
@@ -914,6 +963,8 @@ struct SyncBufs {
   int winner_only;
   const double* sigx;                 // signal references' stored values (absolute sig_off indices), on the device
   unsigned long long* first_bad;      // [V]: per video, its first out-of-domain frame (sig_ref_kernel)
+  float* seg_scratch;                 // the sampled segments' detector output (plan: seg_frames floats)
+  unsigned long long* speech;         // [V]: per segment video, its first frame > 0 (seg_ref_kernel)
 };
 
 // rasterise (float signals only if !fused) -> align -> reduce the tracks of the videos [v0, v1) on the
@@ -957,18 +1008,28 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // the step stays the buffer's only writer, so the pipeline and resident chaining need nothing new.
 // With signal references (b2_sync_tracks_sig) sig_ref_kernel writes those of the videos [v0, v1) the same way, as
 // floats or, in a packed sub-batch, as the bits the VAD would write; it also resets and sets their flags.
+// With sampled segments (b2_sync_tracks_seg) a segment video is empty in the main launch (plan det_end); a second
+// detector launch reads only its segments' samples into the scratch (floats), and seg_ref_kernel writes its reference
+// from there, floats or bits, and resets and sets its speech flag.
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
                   bool ref_packed) {
+  const bool seg = !p.det_end.empty();
   if (!p.auditok) {
-    // a packed sub-batch of signal videos alone has no audio: the VAD has no tiles and is not asked for bits
+    // a packed sub-batch of signal (or segment) videos alone has no audio: the VAD has no tiles and is not asked
+    // for bits
+    bool audio = r.pcm_off[v1] > r.pcm_off[v0];
+    if (seg) {
+      audio = false;
+      for (int v = v0; v < v1; ++v) audio = audio || p.det_end[v] > r.pcm_off[v];
+    }
     B2_TRY(b2i_vad_launch(h, b.pcm, r.pcm_off + v0, v1 - v0, p.fpw, r.energy.non_speech_label,
                           (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, p.ref_off.data() + v0,
-                          nullptr, ref_packed && r.pcm_off[v1] > r.pcm_off[v0]));
+                          nullptr, ref_packed && audio, seg ? p.det_end.data() + v0 : nullptr));
   } else {
     const ChunkTable& ch = p.ch;
     const int c0 = ch.first[v0], nc = ch.first[v1] - c0;
     B2_TRY(b2i_vad_launch(h, b.pcm, ch.pcm.data() + c0, nc, p.fpw, 0.0f, p.auditok_e_min, 0, p.fpw, b.refsig,
-                          ch.out.data() + c0, ch.tail.data() + c0));
+                          ch.out.data() + c0, ch.tail.data() + c0, false, seg ? p.det_end.data() + c0 : nullptr));
     if (!p.any_ref) return b2i_tokenize_inplace_launch(h, b.refsig, ch.out.data() + c0, nc, p.tok);
     const int k0 = ch.tok_first[v0];
     B2_TRY(b2i_tokenize_inplace_launch(h, b.refsig, ch.tok_off.data() + k0, ch.tok_first[v1] - k0, p.tok,
@@ -986,6 +1047,24 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
   if (!sig.empty())
     B2_TRY(b2i_sig_ref_launch(h, b.sigx, r.sig.off, p.ref_off.data(), r.V, sig.data(), (int)sig.size(), p.label,
                               ref_packed, b.refsig, b.first_bad));
+  const int s0 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v0) - p.seg_video.begin());
+  const int s1 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v1) - p.seg_video.begin());
+  if (s1 > s0) {
+    const int k0 = p.item_first[v0], nk = p.item_first[v1] - k0;
+    if (nk > 0 && !p.auditok) {
+      B2_TRY(b2i_vad_launch(h, b.pcm, p.item_start.data() + k0, nk, p.fpw, r.energy.non_speech_label,
+                            (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.seg_scratch,
+                            p.item_out.data() + k0, nullptr, false, p.item_end.data() + k0));
+    } else if (nk > 0) {   // auditok: the energy pass, then the tokenizer restarting in every item
+      B2_TRY(b2i_vad_launch(h, b.pcm, p.item_start.data() + k0, nk, p.fpw, 0.0f, p.auditok_e_min, 0, p.fpw,
+                            b.seg_scratch, p.item_out.data() + k0, p.item_tail.data() + k0, false,
+                            p.item_end.data() + k0));
+      B2_TRY(b2i_tokenize_inplace_launch(h, b.seg_scratch, p.item_out.data() + k0, nk, p.tok));
+    }
+    B2_TRY(b2i_seg_ref_launch(h, b.seg_scratch, p.ref_off.data(), p.seg_video.data() + s0, s1 - s0,
+                              p.run_first.data() + s0, p.run_lo.data(), p.run_src.data(), ref_packed, b.refsig,
+                              b.speech));
+  }
   if (!p.any_subs) return B2_OK;
   const std::vector<int> subs = in_range(p.sub_video), pgs = in_range(p.pgs_video);
   if (!subs.empty())
@@ -1140,10 +1219,17 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   const int refsig_slot = chained && h->refsig_parity == 0 ? b2_ctx::WS_SIG_REF2 : b2_ctx::WS_SIG_REF;
   // signal references: the per-video flags of sig_ref_kernel follow the reference in the same buffer, so a chained
   // resident call's flags alternate with its reference and live exactly as long
-  const size_t ref_bytes = any_sig ? (((size_t)p.ref_off[r.V] * 4 + 64 + 7) & ~(size_t)7)
-                                   : (size_t)p.ref_off[r.V] * 4 + 64;
-  B2_TRY(b2i_ws(h, refsig_slot, ref_bytes + (any_sig ? (size_t)r.V * 8 : 0), &d_refsig));
+  // (and so do the speech flags of seg_ref_kernel, then the segments' detector scratch)
+  const bool any_seg = !p.seg_video.empty();
+  const size_t ref_bytes = any_sig || any_seg ? (((size_t)p.ref_off[r.V] * 4 + 64 + 7) & ~(size_t)7)
+                                              : (size_t)p.ref_off[r.V] * 4 + 64;
+  const size_t flag_bytes = (any_sig ? (size_t)r.V * 8 : 0) + (any_seg ? (size_t)r.V * 8 : 0);
+  const size_t scr_at = (ref_bytes + flag_bytes + 15) & ~(size_t)15;
+  B2_TRY(b2i_ws(h, refsig_slot, any_seg ? scr_at + (size_t)p.seg_frames * 4 + 64 : ref_bytes + flag_bytes,
+                &d_refsig));
   b.first_bad = any_sig ? (unsigned long long*)((char*)d_refsig + ref_bytes) : nullptr;
+  b.speech = any_seg ? (unsigned long long*)((char*)d_refsig + ref_bytes + (any_sig ? (size_t)r.V * 8 : 0)) : nullptr;
+  b.seg_scratch = any_seg ? (float*)((char*)d_refsig + scr_at) : nullptr;
   if (!b.fused) B2_TRY(b2i_ws(h, b2_ctx::WS_SIG_SUB, (size_t)p.sub_off[J] * 4 + 64, &d_subsig));
   B2_TRY(b2i_ws(h, b2_ctx::WS_MISC, J * 16 + (size_t)T * 16 + 256, &d_res));
   double* d_score = (double*)d_res;
@@ -1176,7 +1262,10 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   b.pcm = r.pcm;
   if (memspace == B2_HOST) {   // a call without audio samples reads no PCM (b2_sync_tracks_subs may pass none)
     void* dp = nullptr;
-    if (p.audio_samples > 0) B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, &dp));
+    if (p.audio_samples > 0 && any_seg)   // the ranges the detector reads, at their own positions
+      B2_TRY(stage_ranges(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, p.stage_lo, p.stage_hi, &dp));
+    else if (p.audio_samples > 0)
+      B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, &dp));
     b.pcm = (const int16_t*)dp;
   }
   b.sigx = r.sig.x;
@@ -1195,9 +1284,10 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   b.winner_only = (!r.all_score && !r.all_offset) ? 1 : 0;
   B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
-  // Signal videos with out-of-domain values: their tracks' outputs are overwritten behind every chain, on the
-  // caller's stream, before the host copies (the flags stay valid as the reference buffer does, below)
-  if (any_sig) {
+  // Signal videos with out-of-domain values and segment videos without speech: their tracks' outputs are overwritten
+  // behind every chain, on the caller's stream, before the host copies (the flags stay valid as the reference buffer
+  // does, below)
+  if (any_sig || any_seg) {
     B2SigBadOut so{b.bs, b.bo, b.bk, nullptr, nullptr, K, nullptr, nullptr, kGssEvals};
     if (p.gss) {
       so.a_score = b.g_all_score;
@@ -1209,7 +1299,11 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
       so.a_score = r.all_score ? b.score : nullptr;
       so.a_offset = r.all_offset ? b.offset : nullptr;
     }
-    B2_TRY(b2i_sig_bad_launch(h, b.first_bad, p.sig_video.data(), (int)p.sig_video.size(), p.trk_off.data(), so));
+    B2_TRY(b2i_sentinel_launch(h, b.first_bad, p.sig_video.data(), (int)p.sig_video.size(), p.trk_off.data(), so,
+                               B2_BEST_K_BAD_SIGNAL, true));
+    // segment videos without a frame > 0
+    B2_TRY(b2i_sentinel_launch(h, b.speech, p.seg_video.data(), (int)p.seg_video.size(), p.trk_off.data(), so,
+                               B2_BEST_K_NO_SPEECH, false));
   }
   // The reference capture: one copy behind every chain on the caller's stream, when every detector step is done.
   // The buffer stays valid until then: no chain kernel writes it (they read it as const), the next chained
@@ -1414,6 +1508,49 @@ extern "C" int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm, const int64_t
                 memspace};
   r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
   r.sig = {ref_is_sig, x, V > 0 ? sig_off : no_values};
+  return sync_run(h, _b2_fence_was_valid, r);
+}
+
+extern "C" int b2_sync_tracks_seg(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int V,
+                                  const int32_t* track_video, int T, int frame_rate, int sample_rate, int detector,
+                                  double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                                  double energy_threshold_db, double min_length, int64_t max_length,
+                                  double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs,
+                                  const double* ref_cue_start_s, const double* ref_cue_end_s,
+                                  const uint8_t* ref_cue_keep, const int64_t* ref_cue_off, const uint8_t* ref_is_pgs,
+                                  const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off,
+                                  const uint8_t* ref_is_sig, const double* x, const int64_t* sig_off, int n_seg_videos,
+                                  const int32_t* seg_video, const double* seg_total, const int64_t* seg_off,
+                                  const int64_t* seg_start, const int64_t* seg_lo, const int64_t* seg_hi,
+                                  const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                                  const int64_t* cue_off, const double* ratios, int K, double start_seconds,
+                                  int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                                  int32_t* best_k, double* all_score, int32_t* all_offset, double* gss_ratio,
+                                  double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_sync_tracks_seg");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: gss_evals without gss_ratio");
+  if (V > 0 && !pcm_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: null pcm_off");
+  if (n_seg_videos < 0 || (n_seg_videos > 0 && !seg_off))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: %d segment videos without seg_off", n_seg_videos);
+  if (ref_is_subs && !ref_cue_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: ref_is_subs without ref_cue_off");
+  if (ref_is_pgs && !pgs_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: ref_is_pgs without pgs_off");
+  if (ref_is_sig && !sig_off) B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: ref_is_sig without sig_off");
+  if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "sync_tracks_seg: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, "
+            "not %d", detector);
+  static const int64_t no_segments[1] = {0};
+  SyncRequest r{gss_ratio ? "sync_tracks_seg (search)" : "sync_tracks_seg", pcm, pcm_off, V, track_video, T,
+                frame_rate, sample_rate, detector, {(float)non_speech_label, energy_threshold, z_lo, z_hi},
+                {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length, chunk_samples},
+                {ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : nullptr},
+                cue_start_s, cue_end_s, cue_keep, cue_off, ratios, K, start_seconds, max_offset_samples,
+                best_score, best_offset, best_k, all_score, all_offset, gss_ratio != nullptr, gss_ratio, gss_evals,
+                memspace};
+  r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
+  r.sig = {ref_is_sig, x, V > 0 ? sig_off : nullptr};
+  r.seg = {n_seg_videos, seg_video, seg_total, n_seg_videos > 0 ? seg_off : no_segments, seg_start, seg_lo, seg_hi};
   return sync_run(h, _b2_fence_was_valid, r);
 }
 

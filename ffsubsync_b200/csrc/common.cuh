@@ -175,11 +175,14 @@ static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b;
 // packed (lane-per-window kernel only, B2_ERR_UNSUPPORTED otherwise): instead of the floats, the bits
 // m = (r == 1.0f) of every window, 32 to a word; signal b's words start at d_out + out_off_host[b] (read as
 // uint32), ceil(windows / 32) of them, with zero bits past its last window.
+// pcm_end_host (nullable, [B]): signal b spans pcm_off_host[b] .. pcm_end_host[b] (signals with gaps between them, or
+// overlapping: the sampled segments of b2_sync_tracks_seg); null = pcm_off_host[b + 1].  Lane eligibility (8-sample
+// aligned starts) is decided per non-empty signal either way.
 bool b2i_vad_lane_eligible(const int64_t* pcm_off_host, int B, int fpw);
 int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off_host, int B, int fpw,
                    float non_speech_label, int64_t e_min_full, int z_lo, int z_hi,
                    float* d_out, const int64_t* out_off_host, const int64_t* tail_emin_host = nullptr,
-                   bool packed = false);
+                   bool packed = false, const int64_t* pcm_end_host = nullptr);
 struct B2TokenizerParams {
   double min_length, max_continuous_silence, non_speech_label;
   long long max_length;
@@ -214,7 +217,16 @@ int b2i_raster_ref_launch(b2_ctx* h, const double* cue_start, const double* cue_
 int b2i_sig_ref_launch(b2_ctx* h, const double* d_x, const int64_t* x_off, const int64_t* out_off, int n_videos,
                        const int* videos, int n_sig, float label, bool packed, float* d_out,
                        unsigned long long* d_first_bad);
-// The outputs of one batched sync call that sig_bad_kernel overwrites for the tracks of a flagged signal video
+// Sampled-segment references of b2_sync_tracks_seg (K1m, seg_ref.cu): for each of the n_seg videos videos[i]
+// (ascending indices into the host table out_off [n_videos + 1]), write every frame of d_out + out_off[v], L =
+// out_off[v+1] - out_off[v] of them, from the segments' detector output d_scratch by the owned-frame runs
+// run_first[i] .. run_first[i+1]-1 (run_lo / run_src, sync_plan.h), 0.0 where no segment owns the frame: floats, or
+// with packed ceil(L/32) words of the bits m = (r == 1.0f) with zero bits past L.  d_speech[v] is reset first and ends
+// as the video's first frame > 0 (kSigNoBadFrame: none).  The grid keeps to h->vad_partition_sms SMs when it is set.
+int b2i_seg_ref_launch(b2_ctx* h, const float* d_scratch, const int64_t* out_off, const int* videos, int n_seg,
+                       const int* run_first, const int64_t* run_lo, const int64_t* run_src, bool packed,
+                       float* d_out, unsigned long long* d_speech);
+// The outputs of one batched sync call that sentinel_kernel overwrites for the tracks of a flagged video
 // (device arrays; a_* [T * cols], evals [T * n_evals] and ratio may be null)
 struct B2SigBadOut {
   double* bs;
@@ -227,10 +239,12 @@ struct B2SigBadOut {
   double* evals;
   int n_evals;
 };
-// For each signal video videos[i] whose d_first_bad entry is set: best_k = B2_BEST_K_BAD_SIGNAL, best_score,
-// all_score, gss_ratio and gss_evals NaN, best_offset and all_offset 0, on every track trk_off[v] .. trk_off[v+1]-1.
-int b2i_sig_bad_launch(b2_ctx* h, const unsigned long long* d_first_bad, const int* videos, int n_sig,
-                       const int* trk_off, const B2SigBadOut& out);
+// For each video videos[i] whose flag d_flag[v] is set (!= kSigNoBadFrame) when bad_if_set, or unset when not:
+// best_k = sentinel, best_score, all_score, gss_ratio and gss_evals NaN, best_offset and all_offset 0, on every track
+// trk_off[v] .. trk_off[v+1]-1.  Signal videos: their first out-of-domain frame, set = B2_BEST_K_BAD_SIGNAL; segment
+// videos: their first frame > 0, unset = B2_BEST_K_NO_SPEECH.
+int b2i_sentinel_launch(b2_ctx* h, const unsigned long long* d_flag, const int* videos, int n, const int* trk_off,
+                        const B2SigBadOut& out, int sentinel, bool bad_if_set);
 int b2i_bounds_launch(b2_ctx* h, const float* d_sig, const int64_t* off_host, int n,
                       int64_t* d_first, int64_t* d_last);
 int b2i_blend_launch(b2_ctx* h, const float* d_a, const float* d_b, int64_t n, int mode, double wa,

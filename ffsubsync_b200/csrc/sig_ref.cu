@@ -1,7 +1,8 @@
 // K1s: serialized speech signals as references of the batched sync calls (b2_sync_tracks_sig, DESIGN.md section 4).
 // sig_ref_kernel turns each signal video's stored float64 values into its reference frames (sig_ref.cuh) in the
 // reference-signal buffer - floats, or the run path's packed bits - and flags a video with out-of-domain values;
-// sig_bad_kernel then overwrites every output of a flagged video's tracks with the B2_BEST_K_BAD_SIGNAL sentinel.
+// sentinel_kernel then overwrites every output of a flagged video's tracks with the B2_BEST_K_BAD_SIGNAL sentinel
+// (and of a segment video without speech with B2_BEST_K_NO_SPEECH: seg_ref.cu sets those flags).
 #include <algorithm>
 
 #include "common.cuh"
@@ -67,9 +68,9 @@ __global__ void __launch_bounds__(kSigThreads, 1) sig_ref_kernel(SigRefParams p)
   }
 }
 
-struct SigBadParams {
-  const unsigned long long* first_bad;   // [call's V]
-  const int* vid;                        // [n]: the signal videos
+struct SentinelParams {
+  const unsigned long long* flag;        // [call's V]: kSigNoBadFrame = unset
+  const int* vid;                        // [n]: the flagged kind's videos
   const int* trk;                        // [2n]: their tracks trk[2i] .. trk[2i+1]-1
   double* bs;
   int32_t* bo;
@@ -80,18 +81,20 @@ struct SigBadParams {
   double* ratio;                         // may be null: [T]
   double* evals;                         // may be null: [T * kGssEvals]
   int n_evals;
+  int sentinel;
+  int bad_if_set;                        // 1: a set flag marks the video, 0: an unset one
 };
 
-// One CTA per signal video; a video none of whose values is out of the domain leaves everything as it is.
-__global__ void __launch_bounds__(128) sig_bad_kernel(SigBadParams p) {
+// One CTA per listed video; a video that is not marked leaves everything as it is.
+__global__ void __launch_bounds__(128) sentinel_kernel(SentinelParams p) {
   const int i = blockIdx.x;
-  if (p.first_bad[p.vid[i]] == kSigNoBadFrame) return;
+  if ((p.flag[p.vid[i]] != kSigNoBadFrame) != (p.bad_if_set != 0)) return;
   const long long t0 = p.trk[2 * i], t1 = p.trk[2 * i + 1];
   const double nan = __longlong_as_double(0x7ff8000000000000ll);
   for (long long t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
     p.bs[t] = nan;
     p.bo[t] = 0;
-    p.bk[t] = B2_BEST_K_BAD_SIGNAL;
+    p.bk[t] = p.sentinel;
     if (p.ratio) p.ratio[t] = nan;
   }
   for (long long j = t0 * p.cols + threadIdx.x; j < t1 * p.cols; j += blockDim.x) {
@@ -148,10 +151,10 @@ int b2i_sig_ref_launch(b2_ctx* h, const double* d_x, const int64_t* x_off, const
   return B2_OK;
 }
 
-int b2i_sig_bad_launch(b2_ctx* h, const unsigned long long* d_first_bad, const int* videos, int n_sig,
-                       const int* trk_off, const B2SigBadOut& out) {
+int b2i_sentinel_launch(b2_ctx* h, const unsigned long long* d_flag, const int* videos, int n_sig, const int* trk_off,
+                        const B2SigBadOut& out, int sentinel, bool bad_if_set) {
   if (n_sig <= 0) return B2_OK;
-  B2Range range("b2:sig_bad");
+  B2Range range("b2:sentinel");
   std::vector<int> trk(2 * (size_t)n_sig);
   for (int i = 0; i < n_sig; ++i) {
     trk[2 * i] = trk_off[videos[i]];
@@ -159,11 +162,11 @@ int b2i_sig_bad_launch(b2_ctx* h, const unsigned long long* d_first_bad, const i
   }
   MetaArena a;
   B2_TRY(b2i_meta_begin(h, &a, (size_t)n_sig * 12 + 512));
-  SigBadParams p;
+  SentinelParams p;
   p.vid = (const int*)b2i_meta_put(&a, videos, (size_t)n_sig * 4);
   p.trk = (const int*)b2i_meta_put(&a, trk.data(), (size_t)n_sig * 8);
   B2_TRY(b2i_meta_commit(&a));
-  p.first_bad = d_first_bad;
+  p.flag = d_flag;
   p.bs = out.bs;
   p.bo = out.bo;
   p.bk = out.bk;
@@ -173,7 +176,9 @@ int b2i_sig_bad_launch(b2_ctx* h, const unsigned long long* d_first_bad, const i
   p.ratio = out.ratio;
   p.evals = out.evals;
   p.n_evals = out.n_evals;
-  sig_bad_kernel<<<(unsigned)n_sig, 128, 0, h->stream>>>(p);
-  B2_CHECK_LAUNCH(h, "sig_bad_kernel");
+  p.sentinel = sentinel;
+  p.bad_if_set = bad_if_set ? 1 : 0;
+  sentinel_kernel<<<(unsigned)n_sig, 128, 0, h->stream>>>(p);
+  B2_CHECK_LAUNCH(h, "sentinel_kernel");
   return B2_OK;
 }

@@ -1,5 +1,5 @@
 // Host-side plan of one batched sync call (b2_sync_batch, b2_sync_tracks, b2_sync_tracks_gss,
-// b2_sync_tracks_auditok, b2_sync_tracks_subs, b2_sync_tracks_pgs, b2_sync_tracks_sig): every argument check and every
+// b2_sync_tracks_auditok, b2_sync_tracks_subs, b2_sync_tracks_pgs, b2_sync_tracks_sig, b2_sync_tracks_seg): every argument check and every
 // host table the pipeline in api.cu reads.  No CUDA call happens here, so tests/host_emul/plan_emul.cu runs the same code on the CPU.
 #pragma once
 
@@ -385,6 +385,20 @@ struct SyncRequest {
     const double* x;
     const int64_t* off;            // [V+1]
   } sig;
+  // Sampled segments (b2_sync_tracks_seg, --multi-segment-sync; off null: none): video video[i] (increasing) has the
+  // probed duration total[i] seconds and the segments off[i] .. off[i+1]-1, segment j starting at start[j] whole
+  // seconds (strictly increasing within a video) with the samples pcm_off[v] + lo[j] .. pcm_off[v] + hi[j].  Its
+  // reference is MultiSegmentVideoSpeechTransformer.fit's sparse signal.  All host arrays; the value-initialised state
+  // is "no segment video", so the other entry points leave it out.
+  struct {
+    int n;                         // P: videos with segments
+    const int32_t* video;          // [P]
+    const double* total;           // [P]
+    const int64_t* off;            // [P+1]
+    const int64_t* start;          // per segment
+    const int64_t* lo;
+    const int64_t* hi;
+  } seg;
 };
 
 // What plan_sync reads from the handle and the environment: the SM count, the most sub-batches the handle's
@@ -432,6 +446,30 @@ struct SyncPlan {
   std::vector<int> cut;
   // per sub-batch: its detector writes the reference as packed bits instead of floats (plan_ref_format)
   std::vector<uint8_t> ref_packed;
+  // Sampled segments (plan_segments).  seg_video: the segment videos, ascending; seg_of[v]: v's index into the
+  // request's seg arrays, -1 for other videos.
+  std::vector<int> seg_video, seg_of;
+  // det_end: with segment videos, the end of every entry of the main detector launch (videos, or auditok's chunks),
+  // which then starts at r.pcm_off / ch.pcm as before; a segment video's entry is empty (its PCM is read only through
+  // the segment items below).  Empty without segment videos.
+  std::vector<int64_t> det_end;
+  // The detector launch over the sampled segments: item k reads the samples item_start[k] .. item_end[k] (absolute
+  // in the call's pcm) and writes the scratch frames item_out[k] .. item_out[k+1]; item_tail[k] is auditok's energy
+  // floor of its short last block (0: none).  One item per segment for energy / ZCR, one per chunk of chunk_samples
+  // from the segment's first sample for auditok (the tokenizer restarts in every item).  item_first[v] .. item_first
+  // [v+1]-1: the items of video v (none for other videos).  item_start has one spare entry (the vad launch's table
+  // has n + 1 entries).  seg_frames: the scratch's size.
+  std::vector<int64_t> item_start, item_end, item_out, item_tail;
+  std::vector<int> item_first;
+  int64_t seg_frames = 0;
+  // Owned frames of segment video seg_video[i]: runs run_first[i] .. run_first[i+1]-1 cover its reference [0, L) in
+  // order; run r starts at frame run_lo[r] and ends where the next starts (or at L), and takes scratch frames from
+  // run_src[r] on (-1: 0.0, no segment covers it).  Segments write in increasing start order, the later one wins.
+  std::vector<int> run_first;
+  std::vector<int64_t> run_lo, run_src;
+  // B2_HOST with segment videos: the sample ranges [stage_lo[i], stage_hi[i]) (ascending, disjoint) that the
+  // detector reads - the audio videos' and the segments' - copied to the device at their own positions.
+  std::vector<int64_t> stage_lo, stage_hi;
 };
 
 // Sub-batches are cut at video boundaries (a video's tracks run in the chain behind its own VAD) and balanced by
@@ -442,11 +480,35 @@ struct SyncPlan {
 // Defaults: 3 sub-batches, the later VADs on 54 % of the SMs (71 of an H100's 132; tools/pipeline_probe.py sweeps
 // both), on the lane-per-window kernel only; small batches stay unpipelined (the alignment of a third of a small
 // batch is launch- and tail-bound).  B2_SUBBATCHES / B2_VAD_SMS override the defaults; 1 / 0 = off.
+// Lane eligibility of ranges [start[i], end[i]) that need not abut (the tables of a call with segment videos): each
+// non-empty range on its own, and the window size through an empty table.
+static bool ranges_lane_ok(const SyncPipeEnv& env, const int64_t* start, const int64_t* end, int n, int fpw) {
+  bool ok = env.lane_eligible(start, 0, fpw);
+  for (int i = 0; i < n && ok; ++i) {
+    const int64_t t[2] = {start[i], end[i]};
+    if (end[i] > start[i]) ok = env.lane_eligible(t, 1, fpw);
+  }
+  return ok;
+}
+
+// The audio videos [v0, v1) of the main detector launch (segment videos are empty there)
+static bool audio_lane_ok(const SyncRequest& r, const SyncPipeEnv& env, const SyncPlan* p, int v0, int v1) {
+  if (p->det_end.empty()) return env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw);
+  return ranges_lane_ok(env, r.pcm_off + v0, p->det_end.data() + v0, v1 - v0, p->fpw);
+}
+
 static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   const int V = r.V, T = r.T;
-  // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks
-  const bool lane_ok = p->auditok ? env.lane_eligible(p->ch.pcm.data(), (int)p->ch.tail.size(), p->fpw)
-                                  : env.lane_eligible(r.pcm_off, V, p->fpw);
+  // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks, and the
+  // sampled segments' items
+  bool lane_ok;
+  if (p->det_end.empty())
+    lane_ok = p->auditok ? env.lane_eligible(p->ch.pcm.data(), (int)p->ch.tail.size(), p->fpw)
+                         : env.lane_eligible(r.pcm_off, V, p->fpw);
+  else
+    lane_ok = (p->auditok ? ranges_lane_ok(env, p->ch.pcm.data(), p->det_end.data(), (int)p->ch.tail.size(), p->fpw)
+                          : audio_lane_ok(r, env, p, 0, V)) &&
+              ranges_lane_ok(env, p->item_start.data(), p->item_end.data(), (int)p->item_end.size(), p->fpw);
   p->n_sub = 1;
   p->vad_sms = 0;
   if (T >= 96 && lane_ok) {
@@ -477,9 +539,13 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // Serialized signal references (b2_sync_tracks_sig) have the bits too: sig_ref_kernel writes them, so a sub-batch
 // whose videos are all signal videos or lane-eligible energy audio is packed like an audio one, with either
 // detector (auditok sub-batches qualify only when every video is a signal video).
+// Sampled-segment references (b2_sync_tracks_seg) likewise: seg_ref_kernel writes their bits, so they count like
+// signal videos (their chains take the run path only at label 0, where the reference has the levels 1.0 and 0.0).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
-  if ((p->auditok && p->sig_video.empty()) || !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0)) return;
+  if ((p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
+      (env.ref_packed && atoi(env.ref_packed) == 0))
+    return;
   // how many videos of `list` lie in [v0, v1)
   auto count = [](const std::vector<int>& list, int v0, int v1) {
     return (int)(std::lower_bound(list.begin(), list.end(), v1) - std::lower_bound(list.begin(), list.end(), v0));
@@ -487,8 +553,8 @@ static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPl
   for (int i = 0; i < p->n_sub; ++i) {
     const int v0 = p->cut[i], v1 = p->cut[i + 1];
     if (count(p->sub_video, v0, v1) || count(p->pgs_video, v0, v1)) continue;
-    const bool all_sig = count(p->sig_video, v0, v1) == v1 - v0;
-    if (!all_sig && (p->auditok || !env.lane_eligible(r.pcm_off + v0, v1 - v0, p->fpw))) continue;
+    const bool all_sig = count(p->sig_video, v0, v1) + count(p->seg_video, v0, v1) == v1 - v0;
+    if (!all_sig && (p->auditok || !audio_lane_ok(r, env, p, v0, v1))) continue;
     const int t0 = p->trk_off[v0], nt = p->trk_off[v1] - t0;
     std::vector<int> chain_trk(v1 - v0 + 1);
     for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = p->trk_off[v] - t0;
@@ -513,6 +579,10 @@ static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio, b
     const bool is_subs = s.cue_off && s.is_subs && s.is_subs[v];
     const bool is_pgs = g.off && g.is_pgs && g.is_pgs[v];
     const bool is_sig = q.off && q.is_sig && q.is_sig[v];
+    const bool is_seg = !p->seg_of.empty() && p->seg_of[v] >= 0;
+    if (is_seg && (is_subs || is_pgs || is_sig))
+      B2_FAIL(p, B2_ERR_BAD_ARG, "%s: video %d has sampled segments and a %s reference; a video has one reference",
+              who, v, is_sig ? "serialized signal" : is_pgs ? "PGS" : "text subtitle");
     if (q.off) {
       if (q.off[v + 1] < q.off[v]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: sig_off not monotone at %d", who, v);
       if (!is_sig && q.off[v + 1] != q.off[v])
@@ -547,7 +617,7 @@ static int plan_refs_check(const SyncRequest& r, SyncPlan* p, bool* any_audio, b
                 "its audio is never read", who, v, (long long)(r.pcm_off[v + 1] - r.pcm_off[v]));
     }
     p->any_subs = p->any_subs || is_subs || is_pgs;
-    *any_audio = *any_audio || (!is_subs && !is_pgs && !is_sig);
+    *any_audio = *any_audio || (!is_subs && !is_pgs && !is_sig && !is_seg);
     *any_sig = *any_sig || is_sig;
   }
   if (s.cue_off && r.V > 0 && s.cue_off[r.V] > s.cue_off[0] && (!s.cue_start_s || !s.cue_end_s))
@@ -571,6 +641,9 @@ static int plan_gss_check(const SyncRequest& r, SyncPlan* p, bool auditok_two_le
             "2 max_offset_samples <= %d offsets, one CTA of the run path)", kRunMaxWindow / 2, kRunMaxWindow);
   if (!std::isfinite(p->ref_label))
     B2_FAIL(p, B2_ERR_UNSUPPORTED, "sync_tracks_gss: non_speech_label must be finite (the run path's two-level reference)");
+  if (!p->seg_video.empty() && p->label != 0.0f)
+    B2_FAIL(p, B2_ERR_UNSUPPORTED, "%s: sampled segments (0.0 outside them) at non_speech_label = %g give three "
+            "levels; the search runs on the run path, which needs label 0", who, (double)p->label);
   if (!p->two_level && !auditok_two_level)
     B2_FAIL(p, B2_ERR_UNSUPPORTED, "%s: non_speech_label = %g gives the auditok signal more than two levels; the "
             "search runs on the run path, which needs label 0", who, r.auditok.non_speech_label);
@@ -583,6 +656,156 @@ static int plan_gss_check(const SyncRequest& r, SyncPlan* p, bool auditok_two_le
       B2_FAIL(p, B2_ERR_UNSUPPORTED, "sync_tracks_gss: track %d has %lld cues, more than %d", t,
               (long long)(r.cue_off[t + 1] - r.cue_off[t]), kRunMaxCues);
   return B2_OK;
+}
+
+// MultiSegmentVideoSpeechTransformer.fit's reference length int(total * sample_rate) + 2 (float64 product,
+// truncated), or -1 when total is not finite, too large, or gives a negative length
+static inline int64_t seg_ref_length(double total, int sample_rate) {
+  if (!(fabs(total) < B2_MAX_CUE_SECONDS) || sample_rate <= 0) return -1;
+  const int64_t len = (int64_t)(total * (double)sample_rate) + 2;
+  return len >= 0 ? len : -1;
+}
+
+// Checks of the segment table, before anything reads it; fills seg_video / seg_of and counts the segments' samples
+// (and no other sample of a segment video) in audio_samples.
+static int plan_seg_check(const SyncRequest& r, SyncPlan* p) {
+  const char* who = r.who;
+  const auto& s = r.seg;
+  const int P = s.n;
+  if (P < 0 || (P > 0 && (!s.video || !s.total))) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad segment videos (%d)", who, P);
+  for (int i = 0; i < P; ++i)
+    if (s.off[i + 1] < s.off[i]) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: seg_off not monotone at %d", who, i);
+  if (P > 0 && s.off[P] > s.off[0] && (!s.start || !s.lo || !s.hi))
+    B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null segment arrays with %lld segments", who, (long long)(s.off[P] - s.off[0]));
+  p->seg_of.assign(r.V, -1);
+  for (int i = 0; i < P; ++i) {
+    const int v = s.video[i];
+    if (v < 0 || v >= r.V || (i > 0 && v <= s.video[i - 1]))
+      B2_FAIL(p, B2_ERR_BAD_ARG, "%s: seg_video[%d] = %d is out of [0, %d) or not increasing", who, i, v, r.V);
+    p->seg_of[v] = i;
+    p->seg_video.push_back(v);
+    if (seg_ref_length(s.total[i], r.sample_rate > 0 ? r.sample_rate : 1) < 0)
+      B2_FAIL(p, B2_ERR_BAD_ARG, "%s: seg_total[%d] = %g (video %d) is not finite, too large, or gives a negative "
+              "signal length int(total * sample_rate) + 2", who, i, s.total[i], v);
+    const int64_t n = r.pcm_off[v + 1] - r.pcm_off[v];
+    if (n < 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
+    p->audio_samples -= n;
+    for (int64_t j = s.off[i]; j < s.off[i + 1]; ++j) {
+      if (s.start[j] < 0 || (double)s.start[j] >= B2_MAX_CUE_SECONDS)
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: segment %lld of video %d starts at %lld s, outside [0, %.0f)", who,
+                (long long)j, v, (long long)s.start[j], B2_MAX_CUE_SECONDS);
+      if (j > s.off[i] && s.start[j] <= s.start[j - 1])
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: segment %lld of video %d starts at %lld s, not after the previous one (%lld s)",
+                who, (long long)j, v, (long long)s.start[j], (long long)s.start[j - 1]);
+      if (s.lo[j] < 0 || s.hi[j] < s.lo[j] || s.hi[j] > n)
+        B2_FAIL(p, B2_ERR_BAD_ARG, "%s: segment %lld of video %d has the sample range [%lld, %lld), not inside the "
+                "video's PCM range [0, %lld)", who, (long long)j, v, (long long)s.lo[j], (long long)s.hi[j],
+                (long long)n);
+      p->audio_samples += s.hi[j] - s.lo[j];
+    }
+  }
+  return B2_OK;
+}
+
+// The segment videos' tables (SyncPlan: det_end, item_*, run_*, stage_*), after ref_off and the chunk table.
+static void plan_segments(const SyncRequest& r, SyncPlan* p) {
+  const auto& s = r.seg;
+  const int V = r.V, fpw = p->fpw;
+  // the main launch: every entry as before, a segment video's empty
+  if (p->auditok) {
+    const int nc = (int)p->ch.tail.size();
+    p->det_end.assign(p->ch.pcm.begin() + 1, p->ch.pcm.begin() + 1 + nc);
+    for (int v : p->seg_video) p->det_end[p->ch.first[v]] = p->ch.pcm[p->ch.first[v]];
+  } else {
+    p->det_end.assign(r.pcm_off + 1, r.pcm_off + V + 1);
+    for (int v : p->seg_video) p->det_end[v] = r.pcm_off[v];
+  }
+  // the segments' items: energy one per segment, auditok one per chunk
+  p->item_first.assign(V + 1, 0);
+  p->item_out.assign(1, 0);
+  p->item_start.clear();
+  p->item_end.clear();
+  p->item_tail.clear();
+  std::vector<int64_t> seg_scr(s.n > 0 ? (size_t)(s.off[s.n] - s.off[0]) : 0), seg_len(seg_scr.size());
+  int tail_rem = -1;
+  int64_t tail_floor = 0;
+  for (int v = 0; v < V; ++v) {
+    const int i = p->seg_of[v];
+    for (int64_t j = i < 0 ? 0 : s.off[i]; i >= 0 && j < s.off[i + 1]; ++j) {
+      const int64_t a = r.pcm_off[v] + s.lo[j], n = s.hi[j] - s.lo[j];
+      seg_scr[j - s.off[0]] = p->item_out.back();
+      const int64_t step = !p->auditok || r.auditok.chunk_samples <= 0 ? (n > 0 ? n : 1) : r.auditok.chunk_samples;
+      for (int64_t c = 0; c < n; c += step) {
+        const int64_t len = std::min(step, n - c);
+        p->item_start.push_back(a + c);
+        p->item_end.push_back(a + c + len);
+        p->item_out.push_back(p->item_out.back() + (len + fpw - 1) / fpw);
+        const int rem = (int)(len % fpw);
+        if (p->auditok && rem && rem != tail_rem) {
+          tail_rem = rem;
+          tail_floor = auditok_energy_floor(rem, r.auditok.energy_threshold_db);
+        }
+        p->item_tail.push_back(p->auditok && rem ? tail_floor : 0);
+      }
+      seg_len[j - s.off[0]] = p->item_out.back() - seg_scr[j - s.off[0]];
+    }
+    p->item_first[v + 1] = (int)p->item_end.size();
+  }
+  p->item_start.push_back(p->item_start.empty() ? 0 : p->item_start.back());
+  p->seg_frames = p->item_out.back();
+  // owned frames: a sweep in start order, each segment overwriting [begin, min(begin + len, L)) of the runs so far
+  p->run_first.assign(1, 0);
+  p->run_lo.clear();
+  p->run_src.clear();
+  for (int v : p->seg_video) {
+    const int i = p->seg_of[v];
+    const int64_t L = p->ref_off[v + 1] - p->ref_off[v];
+    struct Piece { int64_t lo, hi, src; };
+    std::vector<Piece> owned, next;
+    for (int64_t j = s.off[i]; j < s.off[i + 1]; ++j) {
+      const int64_t b = s.start[j] * (int64_t)r.sample_rate, e = std::min(b + seg_len[j - s.off[0]], L);
+      if (e <= b) continue;
+      next.clear();
+      for (const Piece& q : owned) {
+        if (q.lo < b) next.push_back({q.lo, std::min(q.hi, b), q.src});
+        if (q.hi > e) next.push_back({std::max(q.lo, e), q.hi, q.src + (std::max(q.lo, e) - q.lo)});
+      }
+      next.push_back({b, e, seg_scr[j - s.off[0]]});
+      std::sort(next.begin(), next.end(), [](const Piece& x, const Piece& y) { return x.lo < y.lo; });
+      owned.swap(next);
+    }
+    int64_t at = 0;
+    for (const Piece& q : owned) {
+      if (q.lo > at) {
+        p->run_lo.push_back(at);
+        p->run_src.push_back(-1);
+      }
+      p->run_lo.push_back(q.lo);
+      p->run_src.push_back(q.src);
+      at = q.hi;
+    }
+    if (at < L) {
+      p->run_lo.push_back(at);
+      p->run_src.push_back(-1);
+    }
+    p->run_first.push_back((int)p->run_lo.size());
+  }
+  // B2_HOST: the ranges the detector reads, merged
+  std::vector<std::pair<int64_t, int64_t>> rg;
+  for (int v = 0; v < V; ++v)
+    if (p->seg_of[v] < 0 && r.pcm_off[v + 1] > r.pcm_off[v])
+      rg.push_back({r.pcm_off[v], r.pcm_off[v + 1]});
+  for (size_t k = 0; k < p->item_end.size(); ++k) rg.push_back({p->item_start[k], p->item_end[k]});
+  std::sort(rg.begin(), rg.end());
+  p->stage_lo.clear();
+  p->stage_hi.clear();
+  for (const auto& [a, b] : rg) {
+    if (!p->stage_hi.empty() && a <= p->stage_hi.back()) p->stage_hi.back() = std::max(p->stage_hi.back(), b);
+    else {
+      p->stage_lo.push_back(a);
+      p->stage_hi.push_back(b);
+    }
+  }
 }
 
 // The detector's window size and arguments, and each video's reference length.
@@ -641,6 +864,8 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
           p->sig_video.push_back(v);
           subs_len[v] = r.sig.off[v + 1] - r.sig.off[v];
         }
+    // Segment references: int(total * sample_rate) + 2 frames (speech_transformers.py:871)
+    for (int v : p->seg_video) subs_len[v] = seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate);
   }
   p->ref_off.assign(V + 1, 0);
   for (int v = 0; v < V; ++v) {
@@ -654,6 +879,7 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
                       p->any_ref ? subs_len.data() : nullptr, &p->ch);
     for (int v = 0; v < V; ++v) p->ref_off[v + 1] = p->ch.out[p->ch.first[v + 1]];
   }
+  if (!p->seg_video.empty()) plan_segments(r, p);
   return B2_OK;
 }
 
@@ -666,11 +892,13 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
   p->auditok = r.detector == B2_DETECTOR_AUDITOK;
   if (V < 0 || T < 0 || K <= 0 || !r.pcm_off || !r.cue_off || !r.ratios)
     B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad arguments", who);
-  bool any_audio = !r.refs.cue_off && !r.pgs.off && !r.sig.off, any_sig = false;
+  bool any_audio = !r.refs.cue_off && !r.pgs.off && !r.sig.off && !r.seg.off, any_sig = false;
   for (int v = 0; v < V; ++v)
     if (r.pcm_off[v + 1] > r.pcm_off[v]) p->audio_samples += r.pcm_off[v + 1] - r.pcm_off[v];
-  if (r.refs.cue_off || r.pgs.off || r.sig.off) B2_TRY(plan_refs_check(r, p, &any_audio, &any_sig));
-  p->any_ref = p->any_subs || any_sig;
+  if (r.seg.off) B2_TRY(plan_seg_check(r, p));
+  if (r.refs.cue_off || r.pgs.off || r.sig.off || r.seg.off) B2_TRY(plan_refs_check(r, p, &any_audio, &any_sig));
+  const bool any_seg = !p->seg_video.empty();
+  p->any_ref = p->any_subs || any_sig || any_seg;
   // The run path and the GSS rounds need a reference of the two levels 1.0 and ref_label.  The detector's signal
   // has the levels 1.0 and the label, a subtitle reference 1.0 and 0.0, so ref_label is the label unless every
   // reference is a subtitle stream; a call that mixes the two at a non-zero label has three levels.  auditok's
@@ -678,11 +906,14 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
   // into a start, so the integer sum stays in {0, 1}); other labels give further levels (0.3, 0.6, ... for 0.3).
   // A signal reference has the levels 1.0 and the label whichever the detector (its stored values are < 1.0 or
   // exactly 1.0), so it counts like energy audio: a call of signals alone is two-level.
+  // A sampled-segment reference has 0.0 outside its segments and the detector's levels inside: {0, 1, label} for
+  // energy / ZCR, {0, 1} for auditok at label 0.  It is two-level only at label 0, where it has the levels of a
+  // subtitle reference and mixes with text / PGS references and with audio as those do.
   p->label = p->auditok ? (float)r.auditok.non_speech_label : r.energy.non_speech_label;
   p->ref_label = any_audio || any_sig ? p->label : 0.0f;
   const bool auditok_two_level = !p->auditok || r.auditok.non_speech_label == 0.0 || !any_audio;
-  const bool mix_two_level = !p->any_subs || p->label == 0.0f;
-  p->two_level = (!any_audio && !any_sig) || (auditok_two_level && mix_two_level);
+  const bool mix_two_level = !(p->any_subs || any_seg) || p->label == 0.0f;
+  p->two_level = (!any_audio && !any_sig && !any_seg) || (auditok_two_level && mix_two_level);
   if (r.track_video) {
     for (int t = 0; t < T; ++t)
       if (r.track_video[t] < 0 || r.track_video[t] >= V || (t > 0 && r.track_video[t] < r.track_video[t - 1]))

@@ -48,6 +48,9 @@ struct VadParams {
   const unsigned char* pcm_bytes;
   float* out;
   const long long* pcm_off;   // [B+1] samples
+  // [B] samples: signal b spans pcm_off[b] .. pcm_end[b] (signals need not abut: the sampled segments of
+  // b2_sync_tracks_seg leave gaps and may overlap).  nullptr: pcm_off[b + 1].
+  const long long* pcm_end;
   const long long* out_off;   // [B+1] windows
   const long long* tile_off;  // [B+1] tiles
   unsigned long long* tile_counter;  // zeroed before the launch
@@ -155,7 +158,7 @@ __device__ __forceinline__ TileDesc make_tile(const VadParams& p, long long t, i
   TileDesc d;
   while (t >= p.tile_off[cur_b + 1]) ++cur_b;
   const long long w0 = (t - p.tile_off[cur_b]) * p.tw;
-  const long long sig0 = p.pcm_off[cur_b], sig1 = p.pcm_off[cur_b + 1];
+  const long long sig0 = p.pcm_off[cur_b], sig1 = p.pcm_end ? p.pcm_end[cur_b] : p.pcm_off[cur_b + 1];
   const long long nwin = p.out_off[cur_b + 1] - p.out_off[cur_b];
   const int nw = (int)min((long long)p.tw, nwin - w0);
   const long long s0 = sig0 + w0 * p.fpw;
@@ -345,7 +348,7 @@ __device__ __forceinline__ TileDesc make_tile_cached(const VadParams& p, long lo
     c.tile_lo = p.tile_off[b];
     c.tile_hi = p.tile_off[b + 1];
     c.sig0 = p.pcm_off[b];
-    c.sig1 = p.pcm_off[b + 1];
+    c.sig1 = p.pcm_end ? p.pcm_end[b] : p.pcm_off[b + 1];
     c.out0 = p.out_off[b];
     c.nwin = p.out_off[b + 1] - c.out0;
   }
@@ -599,8 +602,10 @@ bool b2i_vad_lane_eligible(const int64_t* pcm_off, int B, int fpw) {
 
 int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int B, int fpw,
                    float non_speech_label, int64_t e_min_full, int z_lo, int z_hi,
-                   float* d_out, const int64_t* out_off, const int64_t* tail_emin, bool packed) {
+                   float* d_out, const int64_t* out_off, const int64_t* tail_emin, bool packed,
+                   const int64_t* pcm_end) {
   B2Range range("b2:vad_energy_zcr");
+  auto sig_end = [&](int b) { return pcm_end ? pcm_end[b] : pcm_off[b + 1]; };
   if (((uintptr_t)d_pcm & 15) != 0)
     B2_FAIL(h, B2_ERR_BAD_ARG, "vad: device PCM pointer must be 16-byte aligned");
   VadParams p;
@@ -652,10 +657,10 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   tile_off[0] = 0;
   bool aligned = true;
   for (int b = 0; b < B; ++b) {
-    long long n = pcm_off[b + 1] - pcm_off[b];
+    long long n = sig_end(b) - pcm_off[b];
     long long nwin = (n + fpw - 1) / fpw;
     tile_off[b + 1] = tile_off[b] + (nwin + p.tw - 1) / p.tw;
-    if (n > 0 && pcm_off[b] % 8 != 0) aligned = false;   // an empty signal has no tiles
+    if (n > 0 && pcm_off[b] % 8 != 0) aligned = false;   // an empty signal has no tiles (eligibility per signal)
   }
   if (!aligned) p.fast = 0;  // window starts are not 16-byte aligned in the staged span
   // lane-per-window kernel: 16-byte aligned signals and an instantiated chunk count (8 / 16 / 32 / 48 kHz
@@ -684,7 +689,7 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
     smem = (size_t)kLanePipes * stages * p.stage_bytes + 2 * kLaneMaxStages * sizeof(uint64_t) +
            kLaneMaxStages * sizeof(TileDesc) + 64;
     for (int b = 0; b < B; ++b) {
-      const long long n = pcm_off[b + 1] - pcm_off[b];
+      const long long n = sig_end(b) - pcm_off[b];
       tile_off[b + 1] = tile_off[b] + ((n + fpw - 1) / fpw + p.tw - 1) / p.tw;
     }
   }
@@ -696,8 +701,9 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
 
   MetaArena a;
   size_t tbl = (size_t)(B + 1) * 8;
-  B2_TRY(b2i_meta_begin(h, &a, 4 * tbl + 256));
+  B2_TRY(b2i_meta_begin(h, &a, (pcm_end ? 5 : 4) * tbl + 256));
   p.pcm_off = (const long long*)b2i_meta_put(&a, pcm_off, tbl);
+  p.pcm_end = pcm_end ? (const long long*)b2i_meta_put(&a, pcm_end, (size_t)B * 8) : nullptr;
   p.out_off = (const long long*)b2i_meta_put(&a, out_off, tbl);
   p.tile_off = (const long long*)b2i_meta_put(&a, tile_off.data(), tbl);
   p.tail_emin = tail_emin ? (const long long*)b2i_meta_put(&a, tail_emin, (size_t)B * 8) : nullptr;
@@ -706,7 +712,15 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
   p.pcm_bytes = (const unsigned char*)d_pcm;
   p.out = d_out;
   p.B = B;
-  p.pcm_total_bytes = 2 * (long long)pcm_off[B];
+  // bulk copies stay below the last sample any signal reads (with pcm_end: the largest end; the caller's buffer
+  // holds at least that much)
+  long long pcm_total = pcm_off[B];
+  if (pcm_end) {
+    pcm_total = 0;
+    for (int b = 0; b < B; ++b)
+      if (pcm_end[b] > pcm_off[b]) pcm_total = std::max<long long>(pcm_total, pcm_end[b]);
+  }
+  p.pcm_total_bytes = 2 * pcm_total;
   p.e_min = (long long)e_min_full;
   p.z_lo = z_lo;
   p.z_hi = z_hi;

@@ -75,6 +75,10 @@ enum {
  * b2_sync_tracks_sig).  best_k = -1 stays the reference's FailedToFindAlignment (an empty signal). */
 #define B2_BEST_K_BAD_SIGNAL (-2)
 
+/* best_k of a track whose video's sampled segments hold no frame > 0 (b2_sync_tracks_seg): the reference's
+ * "Unable to detect speech in any sampled segment" (MultiSegmentVideoSpeechTransformer.fit). */
+#define B2_BEST_K_NO_SPEECH (-3)
+
 /* ---- lifecycle ----------------------------------------------------------------------- */
 int b2_version(void);
 int b2_create(int device, b2_handle* out);
@@ -402,6 +406,64 @@ int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm /* or NULL without audio 
                        const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
                        const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
                        int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                       double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                       double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                       int memspace);
+
+/* ---- sampled segments as references (`ffs movie.mkv -i in.srt --multi-segment-sync`) -----------------------
+ * MultiSegmentVideoSpeechTransformer.fit (ffsubsync/speech_transformers.py:811-900) as the reference of some of V
+ * videos: the detector runs only on a few sampled windows of the video, and the reference is 0.0 elsewhere.
+ * Arguments as for b2_sync_tracks_sig (ref_is_subs, ref_is_pgs, ref_is_sig and their tables may be NULL), plus
+ * these host arrays:
+ *   n_seg_videos = P     videos with segments.  0 = none.
+ *   seg_video [P]        their indices, increasing.
+ *   seg_total [P]        the probed duration in seconds (ffprobe's format duration; samples / frame_rate for raw PCM).
+ *   seg_off [P+1]        video i's segments are seg_off[i] .. seg_off[i+1]-1 of the arrays below.
+ *   seg_start            per segment: its start in whole seconds (MultiSegmentVideoSpeechTransformer._segment_starts),
+ *                        strictly increasing within a video.
+ *   seg_lo, seg_hi       per segment: its samples pcm[pcm_off[v] + seg_lo .. pcm_off[v] + seg_hi), inside the video's
+ *                        PCM range.  Ranges may overlap and leave gaps: the video's range may hold its whole decode
+ *                        (segments are slices of it) or only the decoded windows back to back.  Samples outside the
+ *                        segments are never read, and B2_HOST copies only the segments (and the audio videos) to the
+ *                        device.
+ * Segment j writes what the call's detector returns for its samples taken as one signal - energy / ZCR:
+ * ceil(n / fpw) frames, a trailing partial window non-speech; auditok: the chunk loop of chunk_samples from the
+ * segment's first sample, the tokenizer restarting in every chunk - to the frames [seg_start * sample_rate,
+ * min(seg_start * sample_rate + len, L)) of a reference of L = int(seg_total * sample_rate) + 2 frames (float64
+ * product, truncated), in increasing start order, so that a later segment overwrites an earlier one where they
+ * overlap.  Frames no segment covers are 0.0.  start_seconds does not apply to a segment reference (the reference's
+ * transformer has no such argument); it still applies to the subtitle tracks.
+ * A segment reference has the levels 0.0, 1.0 and the label: it is two-level only at label 0, where it counts like a
+ * subtitle reference for the label / path / B2_ERR_UNSUPPORTED rules of b2_sync_tracks_subs (the search needs label 0
+ * in a call with segment videos).
+ * A video none of whose reference frames is > 0 has no speech (the reference raises "Unable to detect speech in any
+ * sampled segment"): every track of that video gets best_k = B2_BEST_K_NO_SPEECH, best_score NaN, best_offset 0,
+ * all_score NaN / all_offset 0 in every column, gss_ratio and gss_evals NaN, without a host synchronisation; the
+ * other tracks are unaffected.
+ * Track t gets exactly what this composition of public calls returns: for a segment video the reference above, built
+ * from b2_vad_energy_zcr (or b2_vad_auditok rounded to float32) over its segments, for the others what
+ * b2_sync_tracks_sig uses, then b2_align_batch and b2_reduce_ratios over the ratios, plus the golden-section search's
+ * candidate as in b2_sync_tracks_gss when gss_ratio is not NULL.
+ * B2_ERR_BAD_ARG also for a non-monotone seg_off, seg_video not increasing or out of [0, V), a seg_total that is not
+ * finite or gives a negative length, a negative start or one not after the previous one, a range outside the video's
+ * PCM range, null segment arrays under segments, and a segment video that also has a text, PGS or signal reference
+ * (a video has one reference).  Without segment videos the call returns what b2_sync_tracks_sig returns.
+ * memspace: B2_HOST, B2_DEVICE or B2_DEVICE_RESIDENT; resident calls chain with the other sync calls in any order. */
+int b2_sync_tracks_seg(b2_handle h, const int16_t* pcm /* or NULL without audio */, const int64_t* pcm_off /* [V+1] */,
+                       int V, const int32_t* track_video /* [T] */, int T, int frame_rate, int sample_rate,
+                       int detector, double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                       double energy_threshold_db, double min_length, int64_t max_length,
+                       double max_continuous_silence, int64_t chunk_samples, const uint8_t* ref_is_subs /* [V] */,
+                       const double* ref_cue_start_s, const double* ref_cue_end_s, const uint8_t* ref_cue_keep,
+                       const int64_t* ref_cue_off /* [V+1] or NULL */, const uint8_t* ref_is_pgs /* [V] */,
+                       const double* pgs_start_s, const double* pgs_end_s, const int64_t* pgs_off /* [V+1] or NULL */,
+                       const uint8_t* ref_is_sig /* [V] */, const double* x, const int64_t* sig_off /* [V+1] or NULL */,
+                       int n_seg_videos, const int32_t* seg_video /* [P] */, const double* seg_total /* [P] */,
+                       const int64_t* seg_off /* [P+1] */, const int64_t* seg_start, const int64_t* seg_lo,
+                       const int64_t* seg_hi, const double* cue_start_s, const double* cue_end_s,
+                       const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */, const double* ratios, int K,
+                       double start_seconds, int64_t max_offset_samples, double* best_score, int32_t* best_offset,
+                       int32_t* best_k /* [T] */,
                        double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
                        double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                        int memspace);

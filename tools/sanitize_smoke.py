@@ -8,7 +8,9 @@ kernels (lane-group: vector path, generic path, ragged tails; lane-per-window: m
 one CTA reusing its ring many times); the auditok energy + tokenizer scan; both rasterisers;
 boundaries; blend; the correlation kernels (float and bit-mask subtitle signals, a multi-block job,
 the split-block small batch path), the run path (reference bits, run correlation), candidate selection, exact re-score, pick and the ratio
-reduction; b2_sync_batch with and without the sub-batch pipeline; b2_sync_tracks_auditok (grid and search).  Results are checked against the
+reduction; b2_sync_batch with and without the sub-batch pipeline; b2_sync_tracks_auditok (grid and search);
+b2_sync_tracks_seg (overlapping and misaligned segments, both detectors, packed and float references, a video
+without speech).  Results are checked against the
 oracle so that a run under the sanitizer is also a parity run.
 """
 import os
@@ -120,6 +122,29 @@ def main():
                               0.0, 6000, chunk, gss=True)
     assert np.isfinite(g[5]).all()
     ba.sync_host(*args)
+    # ---- sampled segments (b2_sync_tracks_seg): overlapping 20 s segments of both videos' full decodes, one set off a
+    # multiple of 8 samples (the lane-group kernel), against the composition of public calls; a silent third video
+    from ffsubsync_b200.batch import segment_table
+    n_pcm = int(args[1][2])
+    pcm3 = np.concatenate([pcm, np.zeros(30 * 16000, np.int16)])
+    off3 = np.array([0, int(args[1][1]), n_pcm, n_pcm + 30 * 16000], np.int64)
+    tab = segment_table(off3, 16000, segment_count=3, segment_duration=20)
+    cue3 = np.concatenate([cue_off, [cue_off[-1] + (cue_off[1] - cue_off[0])]])
+    starts3, ends3 = np.concatenate([args[2], args[2][: cue_off[1]]]), np.concatenate([args[3], args[3][: cue_off[1]]])
+    for det, shift in (("energy_zcr", 0), ("auditok", 0), ("energy_zcr", 3)):
+        t = dict(tab, seg_lo=np.minimum(tab["seg_lo"] + shift, tab["seg_hi"]))
+        bseg = BatchSynchronizer(BENCH_RATIOS, 16000, 100, 0.0, max_offset_seconds=60, device=0, vad=det)
+        for env in ({}, {"B2_REF_PACKED": "0"}):
+            os.environ.update(env)
+            got = bseg._dispatch(pcm3, off3, np.arange(3, dtype=np.int32), starts3, ends3, cue3, None, None, False,
+                                 seg=bseg._seg_refs(3, t), want_all=True, memspace=_native.B2_HOST)
+            for k in env:
+                os.environ.pop(k)
+            assert got[2][2] == _native.B2_BEST_K_NO_SPEECH, got[2]
+            ref, ref_off = bseg._reference_signals(pcm3, off3, seg=bseg._seg_refs(3, t))
+            sub, sub_off = h.rasterize(starts3, ends3, None, cue3, BENCH_RATIOS, 5, False, 100, 0.0)
+            sc, of, stt = h.align_batch(ref, ref_off, sub, sub_off, 3, 5, 6000)
+            assert np.array_equal(got[3][:10], sc[:10]) and np.array_equal(got[4][:10], of[:10]), (det, shift, env)
     h.synchronize()
     print("sanitize_smoke ok")
 

@@ -157,7 +157,7 @@ def main():
                               sig_ref_kernel_us=round(us, 1), bytes=int(moved),
                               gb_per_s=round(moved / (us * 1e-6) / 1e9, 1) if us > 0 else None)), flush=True)
         # the call with per-ratio outputs, and its composition of public entry points
-        refs, pgs, sg = ss._all_refs(V, dict(kw), on_device=True)
+        refs, pgs, sg, _ = ss._all_refs(V, dict(kw), on_device=True)
         tv = np.arange(V, dtype=np.int32)
         c_out = [torch.empty(V, dtype=dt, device=dev) for dt in (torch.float64, torch.int32, torch.int32)]
         c_as = torch.empty(V * K, dtype=torch.float64, device=dev)
