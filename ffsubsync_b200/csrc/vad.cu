@@ -16,6 +16,7 @@
 // "empty" mbarrier - no CTA-wide barrier on the steady-state path.
 #include "common.cuh"
 #include "vad_group.cuh"
+#include "vad_layout.h"
 #include "vad_lane.cuh"
 
 namespace {
@@ -592,12 +593,7 @@ int b2i_synth_launch(b2_ctx* h, const uint8_t* d_cls, int64_t n_windows, int fpw
 // sub-batches over an SM partition only then.)  An empty signal has no tiles, so where it starts does not
 // matter (b2_sync_tracks_subs: a video with a subtitle reference has an empty PCM range).
 bool b2i_vad_lane_eligible(const int64_t* pcm_off, int B, int fpw) {
-  if (fpw != 80 && fpw != 160) return false;
-  if (const char* e = getenv("B2_VAD_LAYOUT"))
-    if (strcmp(e, "group") == 0) return false;
-  for (int b = 0; b < B; ++b)
-    if (pcm_off[b + 1] > pcm_off[b] && pcm_off[b] % 8 != 0) return false;
-  return true;
+  return vad_layout(pcm_off, nullptr, B, fpw, getenv("B2_VAD_LAYOUT")).kernel == kVadLane;
 }
 
 int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int B, int fpw,
@@ -610,25 +606,11 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
     B2_FAIL(h, B2_ERR_BAD_ARG, "vad: device PCM pointer must be 16-byte aligned");
   VadParams p;
   p.consumers = kConsumerThreads;
-  // lanes per window G: the vector path needs the window's C 16-byte chunks to split evenly over
-  // the lanes; prefer an odd chunks-per-lane count (conflict-free LDS.128) and tiles <= 64 KB
+  // which kernel, and its lanes per window (vad_layout.h)
   const int C = fpw / 8;
-  p.fast = (fpw % 8 == 0) ? 1 : 0;
-  int G = 0, best_score = -1;
-  for (int g = 32; g >= 2 && p.fast; g >>= 1) {
-    if (C % g != 0) continue;
-    const int cpl = C / g;
-    const long long tile = (long long)(kConsumerThreads / g) * fpw * 2;
-    const int score = ((cpl & 1) ? 4 : 0) + (tile <= 65536 ? 2 : 0) + (cpl >= 3 ? 1 : 0);
-    if (score > best_score) { best_score = score; G = g; }
-  }
-  if (G == 0) {  // generic 16-bit path: any window size
-    p.fast = 0;
-    G = 4;
-    if (C > 32) G = 8;
-    if (C > 64) G = 16;
-    if (C > 128) G = 32;
-  }
+  const VadLayout lay = vad_layout(pcm_off, pcm_end, B, fpw, getenv("B2_VAD_LAYOUT"));
+  p.fast = lay.kernel != kVadGeneric ? 1 : 0;
+  const int G = lay.G;
   p.G = G;
   p.cpl = p.fast ? C / G : 0;
   // tile = wpt rounds of (256 / G) windows: per-tile costs (mbarrier wait, descriptor, release)
@@ -655,18 +637,14 @@ int b2i_vad_launch(b2_ctx* h, const int16_t* d_pcm, const int64_t* pcm_off, int 
 
   std::vector<long long> tile_off(B + 1);
   tile_off[0] = 0;
-  bool aligned = true;
   for (int b = 0; b < B; ++b) {
     long long n = sig_end(b) - pcm_off[b];
     long long nwin = (n + fpw - 1) / fpw;
     tile_off[b + 1] = tile_off[b] + (nwin + p.tw - 1) / p.tw;
-    if (n > 0 && pcm_off[b] % 8 != 0) aligned = false;   // an empty signal has no tiles (eligibility per signal)
   }
-  if (!aligned) p.fast = 0;  // window starts are not 16-byte aligned in the staged span
-  // lane-per-window kernel: 16-byte aligned signals and an instantiated chunk count (8 / 16 / 32 / 48 kHz
-  // at 100 windows per second).  B2_VAD_LAYOUT=group keeps the lane-group kernel (A/B and test knob).
-  bool lane_layout = p.fast && (C == 10 || C == 20);
-  if (const char* e = getenv("B2_VAD_LAYOUT")) lane_layout = lane_layout && strcmp(e, "group") != 0;
+  // lane-per-window kernel: 16-byte aligned signals and an instantiated chunk count (8 / 16 kHz at 100 windows
+  // per second).  B2_VAD_LAYOUT=group keeps the lane-group kernel (A/B and test knob).
+  const bool lane_layout = lay.kernel == kVadLane;
   // windows per lane and tile: stages of 10 KB
   int wpl = C == 10 ? 2 : 1;
   if (const char* e = getenv("B2_VAD_WPL")) wpl = (C == 10 ? 2 : 1) * (atoi(e) >= 2 ? 2 : 1);   // tuning knob

@@ -214,9 +214,11 @@ def auditok_detect(asegment, sample_rate: int = 100, frame_rate: int = 16000, no
 
 
 def auditok_detect_fast(asegment, sample_rate: int = 100, frame_rate: int = 16000, non_speech_label: float = 0.0,
-                        energy_threshold: float = 50) -> np.ndarray:
+                        energy_threshold: float = 50, min_length=None, max_length=None,
+                        max_continuous_silence=None) -> np.ndarray:
     """Same result as ``auditok_detect`` with the per-block validity vectorised through the integer
-    energy floor (tests check the two agree); used for the long (250 s ... 2 h) parity inputs."""
+    energy floor (tests check the two agree); used for the long (250 s ... 2 h) parity inputs.  The
+    tokenizer parameters (in blocks) default to the reference's 0.2 s, 5 s and 0.25 s."""
     raw = np.frombuffer(asegment, dtype=np.uint8) if isinstance(asegment, (bytes, bytearray, memoryview)) \
         else np.ascontiguousarray(asegment).view(np.uint8)
     if len(raw) % 2 != 0:
@@ -230,7 +232,9 @@ def auditok_detect_fast(asegment, sample_rate: int = 100, frame_rate: int = 1600
     tail = pcm[n_full * block_size:]
     if len(tail):
         valid.append(bool((tail * tail).sum() >= energy_floor(len(tail), energy_threshold)))
-    tokens = tokenize(valid, 0.2 * sample_rate, int(5 * sample_rate), 0.25 * sample_rate)
+    tokens = tokenize(valid, 0.2 * sample_rate if min_length is None else min_length,
+                      int(5 * sample_rate) if max_length is None else int(max_length),
+                      0.25 * sample_rate if max_continuous_silence is None else max_continuous_silence)
     length = (len(raw) // 2 + frames_per_window - 1) // frames_per_window
     media_bstring = np.zeros(length + 1)
     for start, end in tokens:

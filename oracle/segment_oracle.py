@@ -37,14 +37,15 @@ def has_speech(x) -> bool:
 
 
 def detect(pcm, detector: str = "energy_zcr", sample_rate: int = 100, frame_rate: int = 16000,
-           non_speech_label: float = 0.0, chunk_samples: int = 0, **energy) -> np.ndarray:
-    """The call's detector on one segment's int16 samples taken as one signal: energy / ZCR (vad_oracle), or auditok
-    over the chunk loop of chunk_samples samples from the segment's first sample (0: one call)."""
+           non_speech_label: float = 0.0, chunk_samples: int = 0, **params) -> np.ndarray:
+    """The call's detector on one segment's int16 samples taken as one signal: energy / ZCR (vad_oracle; params:
+    energy_threshold, z_lo, z_hi), or auditok over the chunk loop of chunk_samples samples from the segment's first
+    sample (0: one call; params: energy_threshold in dB, min_length, max_length, max_continuous_silence)."""
     pcm = np.asarray(pcm, dtype=np.int16)
     if detector == "energy_zcr":
-        return vo.energy_zcr_detect(pcm, sample_rate, frame_rate, non_speech_label, **energy)
+        return vo.energy_zcr_detect(pcm, sample_rate, frame_rate, non_speech_label, **params)
     step = chunk_samples if chunk_samples > 0 else max(len(pcm), 1)
-    parts = [au.auditok_detect_fast(pcm[i:i + step].tobytes(), sample_rate, frame_rate, non_speech_label)
+    parts = [au.auditok_detect_fast(pcm[i:i + step].tobytes(), sample_rate, frame_rate, non_speech_label, **params)
              for i in range(0, len(pcm), step)]
     return np.concatenate(parts) if parts else np.zeros(0)
 

@@ -10,8 +10,10 @@
 //   lane's run found by bisection and then advanced, every ballot built from the lanes' predicates.
 // usage: seg_ref_emul plan in.txt out.txt
 //   in : "name n v0 .. v(n-1)" per line as for sig_ref_emul, plus seg_video seg_total seg_off seg_start seg_lo seg_hi
-//        and the scalars frame_rate chunk_samples
-//   out: "status s", "err <message>", then the plan's reference and segment tables
+//        and the scalars frame_rate chunk_samples; "lane 3" takes the library's own lane test (vad_layout.h, reading
+//        B2_VAD_LAYOUT from the environment as the library does)
+//   out: "status s", "err <message>", then the plan's reference and segment tables, and "seg_kernel k G cpl": the
+//        energy kernel (vad_layout.h VadKernel) the segments' detector launch takes, with its lanes per window
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -23,10 +25,13 @@
 #include "../../ffsubsync_b200/csrc/seg_ref.cuh"
 #include "../../ffsubsync_b200/csrc/sig_ref.cuh"
 #include "../../ffsubsync_b200/csrc/sync_plan.h"
+#include "../../ffsubsync_b200/csrc/vad_layout.h"
 
 static int g_lane = 0;
-static bool lane_eligible(const int64_t* off, int n, int) {
-  // "lane" 1: every table eligible; 2: eligible when every non-empty range starts at a multiple of 8 (the real test)
+static bool lane_eligible(const int64_t* off, int n, int fpw) {
+  // "lane" 1: every table eligible; 2: eligible when every non-empty range starts at a multiple of 8; 3: the
+  // library's test (b2i_vad_lane_eligible)
+  if (g_lane == 3) return vad_layout(off, nullptr, n, fpw, getenv("B2_VAD_LAYOUT")).kernel == kVadLane;
   if (!g_lane) return false;
   for (int b = 0; b < n; ++b)
     if (off[b + 1] > off[b] && off[b] % 8 != 0 && g_lane > 1) return false;
@@ -221,6 +226,11 @@ static int run_plan(const char* in_path, const char* out_path) {
   put("stage_hi", p.stage_hi);
   put("n_sub", std::vector<int>{p.n_sub});
   fprintf(o, "two_level %d %.9g\n", (int)p.two_level, (double)p.ref_label);
+  if (st == 0 && p.fpw > 0) {   // the segments' detector launch: b2i_vad_launch over item_start / item_end
+    const VadLayout lay = vad_layout(p.item_start.data(), p.item_end.data(), (int)p.item_end.size(), p.fpw,
+                                     getenv("B2_VAD_LAYOUT"));
+    fprintf(o, "seg_kernel %d %d %d\n", lay.kernel, lay.G, lay.cpl);
+  }
   fclose(o);
   return 0;
 }

@@ -116,7 +116,7 @@ def test_export_and_header_signature(built):
 
 # ---------------------------------------------------------------- the planner
 
-def _plan(**req):
+def _plan(env=None, **req):
     with tempfile.TemporaryDirectory() as d:
         src, dst = os.path.join(d, "in.txt"), os.path.join(d, "out.txt")
         with open(src, "w") as f:
@@ -125,7 +125,7 @@ def _plan(**req):
                 f.write("%s %d %s\n" % (k, len(vals), " ".join(
                     x if isinstance(x, str) else repr(float(x)) if isinstance(x, (float, np.floating)) else str(int(x))
                     for x in vals)))
-        subprocess.check_call([EMUL, "plan", src, dst])
+        subprocess.check_call([EMUL, "plan", src, dst], env=None if env is None else dict(os.environ, **env))
         out = {}
         for line in open(dst).read().splitlines():
             k, _, rest = line.partition(" ")
@@ -314,6 +314,51 @@ def test_lane_eligibility_is_per_segment(built):
     # the segment videos' whole ranges do not count: misaligned video starts between segments do not matter
     req = _mixed(120, ("seg",), lane=2, pcm_off=np.arange(121) * (30 * FR + 8))
     assert _plan(**req)["n_sub"] == [3]
+
+
+def _variant_tables():
+    from test_gpu_vad_exact import VARIANTS
+    if not _TABLES:
+        from test_gpu_seg_exact import auditok_layout, energy_layout
+        for fr, geo, _, cpl in VARIANTS.values():
+            if (fr, geo, cpl) not in _TABLES:
+                _TABLES[(fr, geo, cpl)] = (energy_layout(fr, geo, cpl), auditok_layout(fr, geo))
+    return _TABLES
+
+
+_TABLES = {}
+
+
+def test_segment_launch_kernel_per_variant(built):
+    """Each row of tests/test_gpu_seg_exact.py's kernel table reaches that kernel: the planner, with the library's own
+    lane test, on that module's tables (energy and auditok), names the segment launch's kernel (vad_layout.h)."""
+    from test_gpu_seg_exact import KERNEL
+    from test_gpu_vad_exact import VARIANTS
+    tables = _variant_tables()
+    seen = set()
+    for variant, (fr, geo, env, cpl) in VARIANTS.items():
+        for det, c in enumerate(tables[(fr, geo, cpl)]):
+            req = dict(pcm_off=c["pcm_off"], track_video=c["track_video"], cue_start=c["cue_start"],
+                       cue_end=c["cue_end"], cue_off=c["cue_off"], ratios=[1.0], frame_rate=fr, detector=det,
+                       chunk_samples=c.get("chunk", 0), lane=3, **c["seg"])
+            layout = {"B2_VAD_LAYOUT": env["B2_VAD_LAYOUT"]} if "B2_VAD_LAYOUT" in env else {"B2_VAD_LAYOUT": ""}
+            p = _plan(env=layout, **req)
+            assert p["status"] == 0, (variant, p["err"])
+            kernel, g, got_cpl = p["seg_kernel"]
+            assert kernel == KERNEL[variant], (variant, det, p["seg_kernel"])
+            if kernel == 1:   # the lane-group vector path at the chunks per lane of test_gpu_vad_exact's table
+                assert got_cpl == cpl and c["fpw"] // 8 == g * cpl, (variant, det, p["seg_kernel"])
+            seen.add(kernel)
+    assert seen == {0, 1, 2}
+    # the decision looks at starts only: a lane table stays lane-eligible with ragged ends, and one start off a
+    # multiple of 8 moves it to the 16-bit path
+    c = tables[(16000, "aligned", 5)][0]
+    assert any(int(h) % 8 for h in c["seg"]["seg_hi"])
+    req = dict(pcm_off=c["pcm_off"], track_video=c["track_video"], cue_start=c["cue_start"], cue_end=c["cue_end"],
+               cue_off=c["cue_off"], ratios=[1.0], frame_rate=16000, lane=3, **dict(c["seg"]))
+    req["seg_lo"] = np.array(req["seg_lo"])
+    req["seg_lo"][3] += 1
+    assert _plan(env={"B2_VAD_LAYOUT": ""}, **req)["seg_kernel"][0] == 2
 
 
 # ---------------------------------------------------------------- seg_ref_kernel on the CPU

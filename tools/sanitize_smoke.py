@@ -10,7 +10,8 @@ boundaries; blend; the correlation kernels (float and bit-mask subtitle signals,
 the split-block small batch path), the run path (reference bits, run correlation), candidate selection, exact re-score, pick and the ratio
 reduction; b2_sync_batch with and without the sub-batch pipeline; b2_sync_tracks_auditok (grid and search);
 b2_sync_tracks_seg (overlapping and misaligned segments, both detectors, packed and float references, a video
-without speech).  Results are checked against the
+without speech; ranges ending mid-buffer off a 16-byte boundary on the lane-per-window kernel, empty and sub-window
+items, a range ending at the last sample of a buffer whose length is no multiple of 8).  Results are checked against the
 oracle so that a run under the sanitizer is also a parity run.
 """
 import os
@@ -145,6 +146,29 @@ def main():
             sub, sub_off = h.rasterize(starts3, ends3, None, cue3, BENCH_RATIOS, 5, False, 100, 0.0)
             sc, of, stt = h.align_batch(ref, ref_off, sub, sub_off, 3, 5, 6000)
             assert np.array_equal(got[3][:10], sc[:10]) and np.array_equal(got[4][:10], of[:10]), (det, shift, env)
+    # segments on the lane-per-window kernel that end mid-buffer off a 16-byte boundary, an empty and sub-window
+    # items, and a range ending at the last sample of a buffer of 16 s + 13 samples, against the segment oracle
+    from oracle import segment_oracle as so
+    x = rng.randint(-32768, 32768, 16000 * 16 + 13).astype(np.int16)
+    lo = [0, 8008, 16000, 16800, 17600, 32000, len(x) - 4005]
+    hi = [3205, 8008, 16100, 16959, 17761, 33607, len(x)]
+    starts = [0, 2, 3, 4, 5, 6, 8]
+    tok = dict(min_length=1, max_length=10 ** 6, max_continuous_silence=0)
+    for det, kw in (("energy_zcr", dict(energy_threshold=0, z_lo=0, z_hi=160)), ("auditok", dict(chunk_samples=1000,
+                                                                                                **tok))):
+        with h.capture_reference(2000, 1) as cap:
+            h.sync_tracks_seg(x, [0, len(x)], [0], 16000, 100, 0.0 if det == "auditok" else 0.5, [0], [10.0], [0, 7],
+                              starts, lo, hi, starts3[:5], ends3[:5], None, [0, 5], [1.0], 0.0, 200,
+                              detector=_native.B2_DETECTOR_AUDITOK if det == "auditok" else 0, **kw)
+        want = so.segment_reference(x, 10.0, starts, lo, hi, 100, detector=det, frame_rate=16000,
+                                    non_speech_label=0.0 if det == "auditok" else 0.5, **kw).astype(np.float32)
+        assert cap["ref_off"][1] == len(want), det
+        if cap["packed"][0]:   # auditok at label 0: two-level, the run path's bits
+            from oracle import sig_oracle
+            got = cap["ref"][: (len(want) + 31) // 32].view(np.uint32)
+            assert np.array_equal(got, sig_oracle.packed_words(want)), det
+        else:
+            assert np.array_equal(cap["ref"][: len(want)], want), det
     h.synchronize()
     print("sanitize_smoke ok")
 
