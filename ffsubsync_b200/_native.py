@@ -31,7 +31,7 @@ EXPORTS = [
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
-    "b2_sync_tracks_seg",
+    "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -134,6 +134,9 @@ def load() -> ctypes.CDLL:
                                        _f64, _i64, _f64, _i64, _vp, _vp, ctypes.c_int]
         lib.b2_capture_nominations.argtypes = [_vp, _vp, _i64, _vp, _vp, _vp]
         lib.b2_capture_reference.argtypes = [_vp, _vp, _i64, _vp, _vp, _i64]
+        lib.b2_speech_output.argtypes = [_vp, _vp, _i64, _vp, ctypes.c_int, _vp, ctypes.c_int]
+        lib.b2_segment_length.argtypes = [_f64, ctypes.c_int]
+        lib.b2_segment_length.restype = _i64
         lib.b2_apply_sync.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int,
                                       ctypes.c_int, _f64, ctypes.c_int, _f64, _f64, _f64, ctypes.c_int, _f64,
                                       _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
@@ -720,6 +723,27 @@ class Handle:
                           cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
                           (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
                           memspace, gss=bool(gss), want_evals=want_evals)
+
+    def segment_length(self, total_seconds: float, sample_rate: int) -> int:
+        """The reference length int(total_seconds * sample_rate) + 2 of a segment video (b2_segment_length); raises
+        ValueError where the batched calls refuse the duration."""
+        n = int(self.lib.b2_segment_length(float(total_seconds), int(sample_rate)))
+        if n < 0:
+            raise ValueError("seg_total %r is not finite, too large, or gives a negative signal length" % total_seconds)
+        return n
+
+    def speech_output(self, speech, capacity: int, videos, speech_off, memspace: int = B2_DEVICE) -> None:
+        """Set (speech: a device pointer under B2_DEVICE, a float64 numpy array under B2_HOST) or clear (speech None)
+        the speech output of the batched sync calls (b2_speech_output): each later call writes the reference signal
+        of every video of ``videos`` (increasing) as float64 into speech and fills ``speech_off`` (int64 numpy array,
+        len(videos) + 1, kept alive by the caller).  Enqueues nothing."""
+        if speech is None:
+            self._check(self.lib.b2_speech_output(self.h, None, 0, None, 0, None, 0), "b2_speech_output")
+            return
+        self._speech_videos = np.ascontiguousarray(videos, dtype=np.int32)
+        self._check(self.lib.b2_speech_output(self.h, _ptr(speech), int(capacity), _ptr(self._speech_videos),
+                                              len(self._speech_videos), _ptr(speech_off), int(memspace)),
+                    "b2_speech_output")
 
     # -- diagnostics (tests) --------------------------------------------------------------------
     def apply_sync(self, best_score, best_offset, best_k, gss_ratio, cue_start_s, cue_end_s, cue_off, ratios,

@@ -10,6 +10,7 @@ This is what ``ffs ref.mkv -i in.srt`` does per pair in the reference - VideoSpe
 (ffsubsync/ffsubsync.py:637) followed by MaxScoreAligner over the ratio grid (:196-235) - for a
 batch, with the subtitle scaling + rasterisation fused into one kernel.
 """
+import contextlib
 from typing import Optional, Sequence
 
 import numpy as np
@@ -37,6 +38,39 @@ def load_serialized_speech(paths, non_speech_label: float = 0.0, stored: bool = 
             for p in paths]
     off = np.concatenate([[0], np.cumsum([len(s) for s in sigs])]).astype(np.int64)
     return (np.concatenate(sigs) if sigs else np.zeros(0, np.float32)), off
+
+
+def save_serialized_speech(paths, speech, speech_off, speech_video=None, seg_video=None) -> None:
+    """Write what ``--serialize-speech`` writes (ffsubsync/ffsubsync.py:639-644): ``np.savez_compressed(paths[i],
+    speech=...)`` of listed video i's signal ``speech[speech_off[i]: speech_off[i+1]]`` (the ``speech`` /
+    ``speech_off`` results of a sync method called with ``speech_video``), readable by ``load_stored_speech`` and
+    ``load_serialized_speech``.  Choosing the names (the reference's ``_npy_savename``) is the caller's job.
+    A CUDA ``speech`` is copied to the host after a synchronisation of its whole device, so the signals a device sync
+    method enqueued on its handle's own stream are complete before they are read.
+    ``seg_video``: the call's segment videos (``--multi-segment-sync``); ``speech_video``, the call's listed videos, is
+    then required.  A listed segment video whose signal has no frame > 0 is refused with the reference's ValueError
+    before anything is written, as MultiSegmentVideoSpeechTransformer.fit raises before the reference serializes.
+    This is the rule behind the tracks' ``best_k == B2_BEST_K_NO_SPEECH``, so it also covers a call without tracks."""
+    if hasattr(speech, "cpu"):
+        import torch
+        if speech.is_cuda:
+            torch.cuda.synchronize(speech.device)
+        speech = speech.cpu().numpy()
+    speech = np.asarray(speech)
+    speech_off = np.asarray(speech_off, dtype=np.int64)
+    if len(paths) != len(speech_off) - 1:
+        raise ValueError("%d paths for %d signals" % (len(paths), len(speech_off) - 1))
+    if seg_video is not None:
+        if speech_video is None:
+            raise ValueError("seg_video needs speech_video, the videos the signals belong to")
+        if len(speech_video) != len(paths):
+            raise ValueError("speech_video has %d entries for %d paths" % (len(speech_video), len(paths)))
+        seg = {int(v) for v in np.asarray(seg_video).ravel()}
+        for i, v in enumerate(np.asarray(speech_video).ravel()):
+            if int(v) in seg and not np.any(speech[speech_off[i]: speech_off[i + 1]] > 0):
+                raise ValueError("video %d: %s" % (int(v), _NO_SPEECH_MESSAGE))
+    for i, path in enumerate(paths):
+        np.savez_compressed(path, speech=np.asarray(speech[speech_off[i]: speech_off[i + 1]], dtype=np.float64))
 
 
 # keyword arguments of the sync methods that describe the embedded subtitle streams of a subs_then_ detector
@@ -425,21 +459,24 @@ class BatchSynchronizer:
         return (h.sync_tracks_gss if gss else h.sync_tracks)(p, pcm_off, track_video, *energy, *cues, **kw)
 
     def _sync_or_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=None,
-                         sig=None, seg=None, **kw):
+                         sig=None, seg=None, speech=None, **kw):
         """_dispatch with this synchroniser's search.  Outside the envelope of the device-driven search
         (B2_ERR_UNSUPPORTED) the search is composed of public steps instead (_gss_compose).  Returns
         (best_score, best_offset, best_k, all_score, all_offset), plus gss_ratio with the search; composed results
-        are numpy arrays (all_* None unless want_all or device outputs were given)."""
+        are numpy arrays (all_* None unless want_all or device outputs were given).  speech (from _speech_request):
+        the call writes the listed videos' reference signals into it; the composed search fills it from the
+        reference signals it builds."""
         try:
-            return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
-                                  pgs=pgs, sig=sig, seg=seg, **kw)[:6]
+            with self._speech_output(speech):
+                return self._dispatch(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, self.gss,
+                                      pgs=pgs, sig=sig, seg=seg, **kw)[:6]
         except _native.NativeError as e:
             if not (self.gss and _is_unsupported(e)):
                 raise
         want_all = kw.get("want_all", False) or kw.get("all_score") is not None
         bs, bo, bk, ratio, a_s, a_o = self._gss_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off,
                                                         cue_keep, want_all=want_all, refs=refs, pgs=pgs, sig=sig,
-                                                        seg=seg)
+                                                        seg=seg, speech=speech)
         return bs, bo, bk, a_s, a_o, ratio
 
     def use_torch_stream(self) -> None:
@@ -447,8 +484,77 @@ class BatchSynchronizer:
         import torch
         self.handle.set_stream(torch.cuda.current_stream().cuda_stream)
 
+    def _reference_lengths(self, pcm_off, refs=None, pgs=None, sig=None, seg=None) -> np.ndarray:
+        """Each video's reference length [V] in the batched calls, from the library's length helpers: the detector's
+        windows (b2_vad_num_windows, or auditok_out_off's chunk loop), a text stream's b2_rasterize_lengths at ratio
+        1.0, a PGS list's b2_rasterize_pgs_lengths, a signal's stored length and a segment video's b2_segment_length."""
+        h = self.handle
+        pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+        if self.auditok:
+            lens = np.diff(h.auditok_out_off(pcm_off, self.frame_rate, self.sample_rate, self.chunk_samples))
+        else:
+            lens = np.array([h.lib.b2_vad_num_windows(int(n), self.frame_rate, self.sample_rate)
+                             for n in np.diff(pcm_off)], dtype=np.int64)
+        if refs is not None:
+            is_subs, _, re_, _, roff = refs
+            sub = h.rasterize_lengths(re_, roff, [1.0], 1, False, self.sample_rate)
+            lens = np.where(is_subs != 0, sub, lens)
+        if pgs is not None:
+            is_pgs, _, pe, poff = pgs
+            vids = np.flatnonzero(is_pgs)
+            lens[vids] = h.rasterize_pgs_lengths(pe, np.concatenate([[0], np.cumsum(np.diff(poff)[vids])]),
+                                                 self.sample_rate)
+        if sig is not None:
+            is_sig, _, voff = sig
+            lens = np.where(is_sig != 0, np.diff(voff), lens)
+        if seg is not None:
+            for v, total in zip(seg[0], seg[1]):
+                lens[v] = h.segment_length(total, self.sample_rate)
+        return lens.astype(np.int64)
+
+    def _speech_request(self, speech_video, pcm_off, refs=None, pgs=None, sig=None, seg=None, on_device=True,
+                        device=None):
+        """The speech output of a sync call with speech_video (None: no output): dict(video, off (the call writes
+        it), buf (float64, CUDA tensor or numpy array, sized from _reference_lengths), total, memspace)."""
+        if speech_video is None:
+            return None
+        V = len(pcm_off) - 1
+        video = np.ascontiguousarray(speech_video, dtype=np.int64)
+        if video.ndim != 1 or (len(video) and (np.any(np.diff(video) <= 0) or video[0] < 0 or video[-1] >= V)):
+            raise ValueError("speech_video must be increasing video indices in [0, %d)" % V)
+        lens = self._reference_lengths(pcm_off, refs, pgs, sig, seg)[video]
+        off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+        total = int(off[-1])
+        if on_device:
+            import torch
+            buf = torch.empty(max(total, 1), dtype=torch.float64,
+                              device=device if device is not None else torch.device("cuda", self.handle.device))
+        else:
+            buf = np.empty(max(total, 1), dtype=np.float64)
+        return dict(video=video, off=np.empty(len(video) + 1, dtype=np.int64), want_off=off, buf=buf, total=total,
+                    memspace=_native.B2_DEVICE if on_device else _native.B2_HOST)
+
+    @contextlib.contextmanager
+    def _speech_output(self, speech):
+        """The handle's speech output set to the request `speech` (from _speech_request) while the block runs."""
+        if speech is None:
+            yield
+            return
+        buf = speech["buf"]
+        self.handle.speech_output(buf.data_ptr() if hasattr(buf, "data_ptr") else buf, speech["total"],
+                                  speech["video"], speech["off"], speech["memspace"])
+        try:
+            yield
+        finally:
+            self.handle.speech_output(None, 0, None, None)
+
+    @staticmethod
+    def _speech_result(speech):
+        """(speech, speech_off) of a finished request: the written frames and offsets."""
+        return speech["buf"][: speech["total"]], speech["off"]
+
     def sync_device(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None, out=None, all_out=None,
-                    inputs_resident: bool = False, **streams):
+                    inputs_resident: bool = False, speech_video=None, **streams):
         """pcm: int16 CUDA tensor with all pairs back to back; pcm_off: [B+1] sample offsets (host).
         out: optional dict of preallocated CUDA tensors best_score f64[B], best_offset i32[B],
         best_k i32[B].  Returns that dict; nothing is synchronised.
@@ -458,7 +564,10 @@ class BatchSynchronizer:
         still running.  Results are identical; outputs stay ordered on the stream.
         With a ``subs_then_`` detector the embedded subtitle streams come as keyword arguments, and with any detector
         the PGS references and the serialized signals (see the class); with inputs_resident the promise covers
-        ``sig`` too."""
+        ``sig`` too.
+        speech_video: increasing video indices whose reference signals the call also writes (``--serialize-speech``):
+        out then gains ``speech`` (float64 CUDA tensor, the signals back to back) and ``speech_off`` (int64 numpy
+        array [P+1]); see b2_speech_output."""
         import torch
         B = len(pcm_off) - 1
         K = len(self.ratios)
@@ -466,7 +575,7 @@ class BatchSynchronizer:
                 or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS + _SEG_ARGS)):   # the identity track map: pair b is track b of video b
             return self.sync_device_tracks(pcm, pcm_off, np.arange(B, dtype=np.int32), cue_start, cue_end, cue_off,
                                            cue_keep, out=out, all_out=all_out, inputs_resident=inputs_resident,
-                                           **streams)
+                                           speech_video=speech_video, **streams)
         self._references(B, streams)   # rejects streams and unknown keywords
         dev = pcm.device
         if out is None:
@@ -475,17 +584,21 @@ class BatchSynchronizer:
                    "best_k": torch.empty(B, dtype=torch.int32, device=dev)}
         a_s = all_out["score"].data_ptr() if all_out else None
         a_o = all_out["offset"].data_ptr() if all_out else None
-        self.handle.sync_batch(
-            pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
-            self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
-            self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
-            out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o,
-            memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+        speech = self._speech_request(speech_video, pcm_off, device=dev)
+        with self._speech_output(speech):
+            self.handle.sync_batch(
+                pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+                self.energy_threshold, self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios,
+                self.start_seconds, self.max_offset_samples, out["best_score"].data_ptr(),
+                out["best_offset"].data_ptr(), out["best_k"].data_ptr(), a_s, a_o,
+                memspace=_native.B2_DEVICE_RESIDENT if inputs_resident else _native.B2_DEVICE)
+        if speech is not None:
+            out["speech"], out["speech_off"] = self._speech_result(speech)
         assert K == len(self.ratios)
         return out
 
     def sync_device_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, out=None,
-                           all_out=None, inputs_resident: bool = False, **streams):
+                           all_out=None, inputs_resident: bool = False, speech_video=None, **streams):
         """sync_device for several subtitle tracks per video (``ffs movie.mkv -i en.srt de.srt ...``):
         pcm holds the V videos back to back, pcm_off: [V+1] sample offsets (host); track t (cue list
         cue_off[t] .. cue_off[t+1]) is synced against video track_video[t] (host, non-decreasing).  Each
@@ -497,12 +610,15 @@ class BatchSynchronizer:
         is {"score": f64[T*(K+1)], "offset": i32[T*(K+1)]} with column K the search's candidate.
         streams: the embedded subtitle streams of a ``subs_then_`` detector (ref_cue_start, ... - see the class) and
         the PGS references (pgs_start, pgs_end, pgs_off, pgs_video) and the serialized signals (sig, sig_off,
-        sig_video; a float64 CUDA tensor keeps the call asynchronous, other inputs are converted first)."""
+        sig_video; a float64 CUDA tensor keeps the call asynchronous, other inputs are converted first).
+        speech_video as for sync_device (out gains speech and speech_off); with no tracks the call runs only the
+        detector step of those videos (the reference's serialize-only run)."""
         import torch
         T = len(track_video)
         sig_in = streams.get("sig")
         refs, pgs, sig, seg = self._all_refs(len(pcm_off) - 1, streams, on_device=True)
         dev = pcm.device if pcm is not None else torch.device("cuda", self.handle.device)
+        speech = self._speech_request(speech_video, pcm_off, refs, pgs, sig, seg, device=dev)
         if out is None:
             out = {"best_score": torch.empty(T, dtype=torch.float64, device=dev),
                    "best_offset": torch.empty(T, dtype=torch.int32, device=dev),
@@ -518,7 +634,7 @@ class BatchSynchronizer:
             # a converted copy: ready before the handle's stream reads it, and kept until the call is done
             torch.cuda.current_stream(sig[1].device).synchronize()
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    sig=sig, seg=seg, memspace=memspace, **ptrs)
+                                    sig=sig, seg=seg, speech=speech, memspace=memspace, **ptrs)
         if sig is not None and sig[1] is not sig_in:
             self.handle.synchronize()
         if isinstance(res[0], np.ndarray):   # composed on the host
@@ -527,29 +643,36 @@ class BatchSynchronizer:
             if all_out:
                 all_out["score"].copy_(torch.from_numpy(res[3]))
                 all_out["offset"].copy_(torch.from_numpy(res[4]))
+        if speech is not None:
+            out["speech"], out["speech_off"] = self._speech_result(speech)
         return out
 
     def sync_host_tracks(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None,
-                         want_all=False, **streams):
+                         want_all=False, speech_video=None, **streams):
         """sync_device_tracks with host buffers (pcm: int16 numpy array of the V videos).  Blocks until
         results are on the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]) per
-        track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks."""
+        track, and gss_ratio last with the golden-section search.  streams as for sync_device_tracks.
+        speech_video as for sync_device_tracks: the tuple then ends with (speech float64 numpy array, speech_off)."""
         refs, pgs, sig, seg = self._all_refs(len(pcm_off) - 1, streams, on_device=False)
+        speech = self._speech_request(speech_video, pcm_off, refs, pgs, sig, seg, on_device=False)
         res = self._sync_or_compose(pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, pgs=pgs,
-                                    sig=sig, seg=seg, want_all=want_all, memspace=_native.B2_HOST)
+                                    sig=sig, seg=seg, speech=speech, want_all=want_all, memspace=_native.B2_HOST)
         self._raise_bad_signals(sig, res[2])
         self._raise_no_speech(seg, res[2], track_video)
-        return res if want_all else res[:3] + res[5:]
+        res = res if want_all else res[:3] + res[5:]
+        return res if speech is None else res + self._speech_result(speech)
 
-    def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None):
+    def sync_signals(self, ref, ref_off, cue_start, cue_end, cue_off, cue_keep=None, speech_video=None):
         """Same as sync_device but starting from reference speech SIGNALS (100 Hz float32, all pairs
         back to back; numpy array or CUDA tensor) instead of PCM - the replay path of the
         reference's test-case bundles: ``ref.npz{"speech"}`` + ``in.srt``
         (ffsubsync/ffsubsync.py:338-343,639-644; DeserializeSpeechTransformer).
         Returns (best_score f64[B], best_offset i32[B], best_k i32[B]) as numpy arrays, and gss_ratio f64[B]
         last with the golden-section search (gss_batch.gss_align_batch on the same signals, merged as
-        candidate K by gss_batch.combine_gss)."""
+        candidate K by gss_batch.combine_gss).  speech_video is refused: the signals are the caller's already."""
         import torch
+        if speech_video is not None:
+            raise ValueError("sync_signals starts from the reference signals; it does not write them (speech_video)")
         h = self.handle
         ref_off = np.ascontiguousarray(ref_off, dtype=np.int64)
         B, K = len(ref_off) - 1, len(self.ratios)
@@ -584,7 +707,7 @@ class BatchSynchronizer:
         return bs, bo, bk, ratio
 
     def sync_device_candidate_sharded(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None,
-                                      rank: int = 0, world: int = 1, group=None, **pgs_args):
+                                      rank: int = 0, world: int = 1, group=None, speech_video=None, **pgs_args):
         """Secondary multi-GPU mode (SURVEY.md section 8e, "B < G": a few pairs on many GPUs): the K
         ratio candidates of every pair are dealt round-robin over the ranks.  Every rank runs the
         VAD of the (replicated) reference PCM - 33 us per 2 h signal, cheaper than shipping the
@@ -597,6 +720,9 @@ class BatchSynchronizer:
         its 17 evaluations are sequential per pair, so they cannot be dealt over ranks like grid candidates."""
         import torch
         from . import distributed
+        if speech_video is not None:
+            raise ValueError("sync_device_candidate_sharded does not write reference signals (speech_video); a "
+                             "multi-GPU run writes each rank's own videos with sync_device")
         if self.gss:
             raise ValueError("sync_device_candidate_sharded shards the ratio grid; it does not run the "
                              "golden-section search (None in ratios)")
@@ -662,21 +788,27 @@ class BatchSynchronizer:
                         best_k=bk.data_ptr(), memspace=_native.B2_DEVICE)
         return bs, bo, bk
 
-    def sync_host(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None, want_all=False, **streams):
+    def sync_host(self, pcm, pcm_off, cue_start, cue_end, cue_off, cue_keep=None, want_all=False, speech_video=None,
+                  **streams):
         """pcm: int16 numpy array (ideally backed by pinned memory).  Blocks until results are on
         the host.  Returns (best_score, best_offset, best_k[, all_score, all_offset]), and gss_ratio last
         with the golden-section search.  With a ``subs_then_`` detector the embedded subtitle streams come as
-        keyword arguments, and with any detector the PGS references and the serialized signals (see the class)."""
+        keyword arguments, and with any detector the PGS references and the serialized signals (see the class).
+        speech_video as for sync_host_tracks."""
         if (self.gss or self.auditok or self.subs_then
                 or any(streams.get(k) is not None for k in _PGS_ARGS + _SIG_ARGS + _SEG_ARGS)):
             return self.sync_host_tracks(pcm, pcm_off, np.arange(len(pcm_off) - 1, dtype=np.int32), cue_start,
-                                         cue_end, cue_off, cue_keep, want_all=want_all, **streams)
+                                         cue_end, cue_off, cue_keep, want_all=want_all, speech_video=speech_video,
+                                         **streams)
         self._references(len(pcm_off) - 1, streams)   # rejects streams and unknown keywords
-        res = self.handle.sync_batch(
-            pcm, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold,
-            self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds,
-            self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
-        return res if want_all else res[:3]
+        speech = self._speech_request(speech_video, pcm_off, on_device=False)
+        with self._speech_output(speech):
+            res = self.handle.sync_batch(
+                pcm, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label, self.energy_threshold,
+                self.z_lo, self.z_hi, cue_start, cue_end, cue_keep, cue_off, self.ratios, self.start_seconds,
+                self.max_offset_samples, want_all=want_all, memspace=_native.B2_HOST)
+        res = res if want_all else res[:3]
+        return res if speech is None else res + self._speech_result(speech)
 
     def _apply_sync_args(self, apply_offset_seconds, skip_sync_on_low_quality, min_score, quality_max_offset_seconds,
                          max_framerate_deviation, suppress_output_if_offset_less_than) -> dict:
@@ -734,7 +866,7 @@ class BatchSynchronizer:
         return dict(zip(("synced_start_us", "synced_end_us", "offset_seconds", "scale", "status"), outs))
 
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
-                     refs=None, pgs=None, sig=None, seg=None):
+                     refs=None, pgs=None, sig=None, seg=None, speech=None):
         """The golden-section search outside the envelope of the device-driven search, composed of public steps:
         the grid (this synchroniser's batched call with the search off), gss_align_batch on each track's reference
         signal (_reference_signals, with subtitle references refs from _subs_refs) and the reference's combine.
@@ -761,6 +893,15 @@ class BatchSynchronizer:
         grid = self._dispatch(pcm_host, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep, refs, False,
                               pgs=pgs, sig=sig, seg=seg, want_all=True, memspace=_native.B2_HOST)
         ref, ref_off = self._reference_signals(pcm_host, pcm_off, refs, pgs, sig, seg)
+        if speech is not None:   # the listed videos' reference signals, widened
+            parts = [ref[ref_off[v]: ref_off[v + 1]] for v in speech["video"]]
+            x = np.concatenate(parts + [np.zeros(0, np.float32)]).astype(np.float64)
+            speech["off"][:] = np.concatenate([[0], np.cumsum([len(p) for p in parts])])
+            if isinstance(speech["buf"], np.ndarray):
+                speech["buf"][: len(x)] = x
+            else:
+                import torch
+                speech["buf"][: len(x)].copy_(torch.from_numpy(x))
         # one copy of its video's reference signal per track
         parts = [ref[ref_off[v]: ref_off[v + 1]] for v in track_video]
         t_off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)

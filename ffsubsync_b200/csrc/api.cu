@@ -14,6 +14,7 @@
 #include "common.cuh"
 #include "sync_plan.h"
 #include "sync_output.cuh"
+#include "speech_out.cuh"
 
 // Entry guard: the handle's device is current for the duration of the call and the caller
 // thread's previous device is restored on every return path.
@@ -890,6 +891,39 @@ extern "C" int b2_capture_reference(b2_handle h, float* ref, int64_t capacity, i
   return B2_OK;
 }
 
+extern "C" int b2_speech_output(b2_handle h, double* speech, int64_t capacity, const int32_t* videos, int n_videos,
+                                int64_t* speech_off, int memspace) {
+  // Not B2_ENTER: this call enqueues nothing and is read only after a sync call's plan, so a chain of resident sync
+  // calls stays valid across it (as across b2_apply_sync).
+  if (!h) return B2_ERR_BAD_ARG;
+  h->err.clear();
+  DeviceScope scope(h->device);
+  if (!scope.ok) return B2_ERR_CUDA;
+  h->speech_out = B2SpeechOut{};
+  if (!speech) return B2_OK;
+  if (capacity < 0 || n_videos < 0 || !speech_off || (n_videos > 0 && !videos))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "speech_output: bad arguments (capacity %lld, %d videos)", (long long)capacity,
+            n_videos);
+  if (memspace != B2_HOST && memspace != B2_DEVICE)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "speech_output: memspace must be B2_HOST or B2_DEVICE");
+  for (int i = 0; i < n_videos; ++i)
+    if (videos[i] < 0 || (i > 0 && videos[i] <= videos[i - 1]))
+      B2_FAIL(h, B2_ERR_BAD_ARG, "speech_output: videos[%d] = %d is negative or not increasing", i, (int)videos[i]);
+  if (memspace == B2_DEVICE) B2_TRY(check_device_ptr(h, speech, "speech_output: speech"));
+  B2SpeechOut sout;
+  sout.speech = speech;
+  sout.capacity = capacity;
+  sout.videos.assign(videos, videos + n_videos);
+  sout.speech_off = speech_off;
+  sout.memspace = memspace;
+  h->speech_out = std::move(sout);
+  return B2_OK;
+}
+
+extern "C" int64_t b2_segment_length(double total_seconds, int sample_rate) {
+  return seg_ref_length(total_seconds, sample_rate);
+}
+
 extern "C" int b2_reduce_ratios(b2_handle h, const double* score, const int32_t* offset,
                                 const int32_t* status, int B, int K, int64_t max_offset_samples,
                                 double* best_score, int32_t* best_offset, int32_t* best_k,
@@ -1173,18 +1207,38 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   env.fused = true;
   if (const char* e = getenv("B2_FUSED_RASTER")) env.fused = atoi(e) != 0;
   env.ref_packed = getenv("B2_REF_PACKED");
+  const B2SpeechOut& sout = h->speech_out;
+  env.speech_out = sout.speech != nullptr;
   if (const int st = plan_sync(r, env, &p)) {
     h->err = p.err;
     return st;
   }
   const int T = r.T, K = r.K;
-  if (T == 0) return B2_OK;
+  if (T == 0 && !sout.speech) return B2_OK;
   const B2RefCapture rc = h->ref_capture;
   if (rc.ref && (p.ref_off[r.V] > rc.capacity || r.V > rc.max_videos))
     B2_FAIL(h, B2_ERR_BAD_ARG, "%s: the reference capture holds %lld frames of %lld videos, the call has %lld of %d",
             r.who, rc.capacity, rc.max_videos, (long long)p.ref_off[r.V], r.V);
   const bool resident = r.memspace == B2_DEVICE_RESIDENT;
   const int memspace = resident ? B2_DEVICE : r.memspace;
+  // The speech output: its offsets and its checks, before anything is enqueued
+  const int n_speech = (int)sout.videos.size();
+  std::vector<int64_t> speech_off;
+  if (sout.speech) {
+    if ((sout.memspace == B2_HOST) != (memspace == B2_HOST))
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: the speech output was set for %s memory, the call is a %s call", r.who,
+              sout.memspace == B2_HOST ? "host" : "device", memspace == B2_HOST ? "B2_HOST" : "B2_DEVICE");
+    if (n_speech > 0 && sout.videos.back() >= r.V)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: the speech output lists video %d, the call has %d videos", r.who,
+              sout.videos.back(), r.V);
+    speech_off.assign(n_speech + 1, 0);
+    for (int i = 0; i < n_speech; ++i)
+      speech_off[i + 1] = speech_off[i] + p.ref_off[sout.videos[i] + 1] - p.ref_off[sout.videos[i]];
+    if (speech_off[n_speech] > sout.capacity)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: the speech output holds %lld frames, the listed videos need %lld", r.who,
+              sout.capacity, (long long)speech_off[n_speech]);
+    std::copy(speech_off.begin(), speech_off.end(), sout.speech_off);
+  }
   // every bulk pointer of a B2_DEVICE call, before anything is launched
   const char* prefix = r.track_video ? "sync_tracks" : "sync_batch";
   const std::pair<const void*, const char*> bulk[] = {{r.pcm, "pcm"}, {r.best_score, "best_score"},
@@ -1262,7 +1316,26 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   b.pcm = r.pcm;
   if (memspace == B2_HOST) {   // a call without audio samples reads no PCM (b2_sync_tracks_subs may pass none)
     void* dp = nullptr;
-    if (p.audio_samples > 0 && any_seg)   // the ranges the detector reads, at their own positions
+    if (T == 0) {   // serialize-only: the samples the listed videos' detector step reads, at their own positions
+      std::vector<std::pair<int64_t, int64_t>> rg;
+      for (int v : sout.videos) {
+        if (any_seg && p.seg_of[v] >= 0) {
+          for (int k = p.item_first[v]; k < p.item_first[v + 1]; ++k) rg.push_back({p.item_start[k], p.item_end[k]});
+        } else if (r.pcm_off[v + 1] > r.pcm_off[v]) {
+          rg.push_back({r.pcm_off[v], r.pcm_off[v + 1]});
+        }
+      }
+      std::sort(rg.begin(), rg.end());
+      std::vector<int64_t> lo, hi;
+      for (const auto& [a0, b0] : rg) {
+        if (!hi.empty() && a0 <= hi.back()) hi.back() = std::max(hi.back(), b0);
+        else {
+          lo.push_back(a0);
+          hi.push_back(b0);
+        }
+      }
+      if (!lo.empty()) B2_TRY(stage_ranges(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, lo, hi, &dp));
+    } else if (p.audio_samples > 0 && any_seg)   // the ranges the detector reads, at their own positions
       B2_TRY(stage_ranges(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, p.stage_lo, p.stage_hi, &dp));
     else if (p.audio_samples > 0)
       B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, r.pcm, (size_t)r.pcm_off[r.V] * 2, &dp));
@@ -1283,11 +1356,22 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   // only the best ratio of each track is reported unless the per-ratio arrays are requested:
   // ratios that cannot win even after the round-off bound tau are then not re-scored exactly (B2_ALIGN_APPROX)
   b.winner_only = (!r.all_score && !r.all_offset) ? 1 : 0;
-  B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
+  if (T > 0) {
+    B2_TRY(run_pipeline(h, r, p, b, resident, chained, refsig_slot));
+  } else {
+    // no tracks, speech output set (the reference's serialize-only run): the detector step of the listed videos,
+    // one launch sequence per run of consecutive indices, on the caller's stream
+    for (int i = 0; i < n_speech;) {
+      int j = i + 1;
+      while (j < n_speech && sout.videos[j] == sout.videos[j - 1] + 1) ++j;
+      B2_TRY(detect(h, r, p, b, sout.videos[i], sout.videos[j - 1] + 1, false));
+      i = j;
+    }
+  }
   // Signal videos with out-of-domain values and segment videos without speech: their tracks' outputs are overwritten
   // behind every chain, on the caller's stream, before the host copies (the flags stay valid as the reference buffer
   // does, below)
-  if (any_sig || any_seg) {
+  if (T > 0 && (any_sig || any_seg)) {
     B2SigBadOut so{b.bs, b.bo, b.bk, nullptr, nullptr, K, nullptr, nullptr, kGssEvals};
     if (p.gss) {
       so.a_score = b.g_all_score;
@@ -1316,7 +1400,30 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
     if (p.ref_off[r.V] > 0)
       B2_CUDA(h, cudaMemcpyAsync(rc.ref, b.refsig, (size_t)p.ref_off[r.V] * 4, cudaMemcpyDeviceToDevice, h->stream));
   }
+  // The speech output (K1o): one kernel at the capture's spot, behind every chain on the caller's stream, so the same
+  // argument keeps the buffer valid.  There it reads a buffer no kernel writes any more and adds no ordering beyond
+  // the stream's; beside the later sub-batches' detector it would take HBM bandwidth from that bandwidth-bound step.
+  // B2_HOST: written to a workspace and copied out with the results below.
+  double* d_speech = sout.speech;
+  if (sout.speech && speech_off[n_speech] > 0) {
+    std::vector<B2SpeechVideo> sv(n_speech);
+    for (int i = 0; i < n_speech; ++i) {
+      const int v = sout.videos[i];
+      const int sb = (int)(std::upper_bound(p.cut.begin(), p.cut.end(), v) - p.cut.begin()) - 1;
+      auto has = [v](const std::vector<int>& list) { return std::binary_search(list.begin(), list.end(), v); };
+      // a clear bit is the label for detector and signal videos, 0.0 for text, PGS and segment videos
+      const bool zero_low = has(p.sub_video) || has(p.pgs_video) || has(p.seg_video);
+      sv[i] = B2SpeechVideo{(long long)p.ref_off[v], zero_low ? 0.0f : p.label, p.ref_packed[sb] ? 1 : 0};
+    }
+    if (!dev) {
+      void* ds;
+      B2_TRY(b2i_ws(h, b2_ctx::WS_SPEECH, (size_t)speech_off[n_speech] * 8 + 64, &ds));
+      d_speech = (double*)ds;
+    }
+    B2_TRY(b2i_speech_out_launch(h, b.refsig, speech_off.data(), sv.data(), n_speech, d_speech));
+  }
   if (dev) return B2_OK;
+  if (sout.speech) B2_TRY(copy_out(h, sout.speech, d_speech, (size_t)speech_off[n_speech] * 8));
   B2_TRY(copy_out(h, r.best_score, d_bs, (size_t)T * 8));
   B2_TRY(copy_out(h, r.best_offset, d_bo, (size_t)T * 4));
   B2_TRY(copy_out(h, r.best_k, d_bk, (size_t)T * 4));

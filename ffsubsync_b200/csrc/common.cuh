@@ -50,6 +50,16 @@ struct B2RefCapture {
   long long max_videos = 0;
 };
 
+// b2_speech_output: where the batched sync calls write the listed videos' reference signals as float64.  Like
+// B2RefCapture it is read after the call's plan is made; setting or clearing it enqueues nothing.
+struct B2SpeechOut {
+  double* speech = nullptr;      // `capacity` doubles in `memspace`; nullptr: output off
+  long long capacity = 0;
+  std::vector<int> videos;       // increasing
+  int64_t* speech_off = nullptr; // host, videos.size() + 1 entries, written by each call
+  int memspace = 0;
+};
+
 struct b2_ctx {
   int device = 0;
   int sm_count = 132;
@@ -61,6 +71,7 @@ struct b2_ctx {
   int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
   B2Capture capture;             // set by b2_capture_nominations (tests)
   B2RefCapture ref_capture;      // set by b2_capture_reference (tests)
+  B2SpeechOut speech_out;        // set by b2_speech_output
   // B2_DEVICE_RESIDENT chaining of b2_sync_batch calls (api.cu): `resident_fence` is recorded on the caller's
   // stream before the LAST sub-batch's correlation chain of a pipelined call, `resident_done` after it; the
   // next resident call (if no other entry point ran in between: `resident_fence_valid`) starts its VAD behind
@@ -71,7 +82,7 @@ struct b2_ctx {
   // named grow-only workspaces
   enum { WS_STAGE_IN0, WS_STAGE_IN1, WS_STAGE_OUT, WS_META, WS_SPEC, WS_SCORES, WS_CAND,
          WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_GSS, WS_GSS_OUT, WS_STAGE_SIG,
-         WS_COUNT };
+         WS_SPEECH, WS_COUNT };
   DeviceBuf ws[WS_COUNT];
   HostBuf pinned[4];
   cudaEvent_t pinned_ev[4] = {};   // recorded after the last async copy out of pinned[i]
@@ -226,6 +237,11 @@ int b2i_sig_ref_launch(b2_ctx* h, const double* d_x, const int64_t* x_off, const
 int b2i_seg_ref_launch(b2_ctx* h, const float* d_scratch, const int64_t* out_off, const int* videos, int n_seg,
                        const int* run_first, const int64_t* run_lo, const int64_t* run_src, bool packed,
                        float* d_out, unsigned long long* d_speech);
+// The speech output (K1o, speech_out.cu): frames off[i] .. off[i+1] of d_out (host table off [n+1]) are listed video i's
+// reference signal, read from the reference buffer d_ref at vids[i] (speech_out.cuh), widened to float64.
+struct B2SpeechVideo;
+int b2i_speech_out_launch(b2_ctx* h, const float* d_ref, const int64_t* off, const B2SpeechVideo* vids, int n,
+                          double* d_out);
 // The outputs of one batched sync call that sentinel_kernel overwrites for the tracks of a flagged video
 // (device arrays; a_* [T * cols], evals [T * n_evals] and ratio may be null)
 struct B2SigBadOut {

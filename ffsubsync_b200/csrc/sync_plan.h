@@ -417,6 +417,7 @@ struct SyncPipeEnv {
   const char* align_path = nullptr;
   bool fused = true;
   const char* ref_packed = nullptr;
+  bool speech_out = false;         // b2_speech_output is set: a call without tracks still plans its references
 };
 
 struct SyncPlan {
@@ -884,7 +885,8 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
 }
 
 // Every argument check and every host table of one batched sync call.  Errors go to p->err with the status.
-// T == 0 returns B2_OK after the checks that do not need tracks, with no tables.
+// T == 0 returns B2_OK after the checks that do not need tracks, with no tables; with env.speech_out it also plans
+// the references (ref_off and the detector's tables) as one sub-batch of floats, for the detector step alone.
 static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   const char* who = r.who;
   const int V = r.V, T = r.T, K = r.K;
@@ -923,7 +925,15 @@ static int plan_sync(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) 
       if (r.cue_off[t + 1] < r.cue_off[t]) B2_FAIL(p, B2_ERR_BAD_ARG, "sync_tracks: cue_off not monotone at %d", t);
   }
   if (p->gss) B2_TRY(plan_gss_check(r, p, auditok_two_level));
-  if (T == 0) return B2_OK;
+  if (T == 0 && !env.speech_out) return B2_OK;
+  if (T == 0) {
+    B2_TRY(plan_references(r, p));
+    p->trk_off.assign(V + 1, 0);
+    p->sub_off.assign(1, 0);
+    p->cut = {0, V};
+    p->ref_packed.assign(1, 0);
+    return B2_OK;
+  }
   if (!r.best_score || !r.best_offset || !r.best_k) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null output", who);
   if (p->gss && !r.gss_ratio) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: null gss_ratio", who);
   B2_TRY(plan_references(r, p));

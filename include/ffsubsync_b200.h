@@ -551,6 +551,34 @@ int b2_capture_nominations(b2_handle h, float* scores, int64_t stride, int64_t* 
 int b2_capture_reference(b2_handle h, float* ref, int64_t capacity, int64_t* ref_off, uint8_t* packed,
                          int64_t max_videos);
 
+/* ---- speech output of the batched sync calls (--serialize-speech) ----------------------------
+ * While set on a handle, every batched sync call (b2_sync_batch, b2_sync_tracks, _gss, _auditok, _subs, _pgs, _sig,
+ * _seg) writes the reference signal of each listed video as float64: listed video i = videos[i] lands at
+ * speech[speech_off[i] .. speech_off[i+1]), its length the call's own reference length (ceil(n/fpw) frames for
+ * energy / ZCR, the chunk loop's blocks for auditok, int(max_end*sr) + 2 for a text stream or PGS, int(seg_total*sr)
+ * + 2 for segments, the stored length for a signal).  Each frame is the float32 frame the call aligned against,
+ * widened: VideoSpeechTransformer's output rounded to float32 for detector videos, the rasterised stream for text,
+ * PGSSpeechTransformer for PGS, the sparse MultiSegmentVideoSpeechTransformer signal for segments and
+ * DeserializeSpeechTransformer(label) for signal videos.  Videos the call flags (best_k -2 or -3) are written too, as
+ * the call built them (a stored value > 1.0 or NaN as the label).  A call with T == 0 has no tracks to carry those
+ * flags: a segment video's signal without a frame > 0 is written as it is, and the caller applies the reference's
+ * no-speech rule to it (batch.save_serialized_speech does).
+ * speech_off is a HOST array of n_videos + 1 entries that each call fills when it is planned.  The call fails with
+ * B2_ERR_BAD_ARG before anything is enqueued when the listed videos need more than `capacity` frames, when a listed
+ * video is >= V, or when the call's memspace is not the output's (B2_DEVICE_RESIDENT counts as B2_DEVICE).
+ * memspace B2_DEVICE: speech is device memory of the handle's device, written by one kernel behind the call's last
+ * chain with no host synchronisation.  B2_HOST: speech is host memory, copied back with the call's results.
+ * A call with T == 0 and the output set runs the detector step of the listed videos and writes them, and nothing
+ * else (the reference's serialize-only run); without the output T == 0 returns at once, as before.
+ * videos must be increasing and >= 0; a host speech pointer under B2_DEVICE is refused.  Setting or clearing the
+ * output enqueues nothing and leaves a chain of resident calls intact; with it cleared every call plans, launches
+ * and returns what it does without it.  speech == NULL clears it. */
+int b2_speech_output(b2_handle h, double* speech, int64_t capacity, const int32_t* videos /* [n], increasing */,
+                     int n_videos, int64_t* speech_off /* host [n+1], written by each call */, int memspace);
+/* MultiSegmentVideoSpeechTransformer.fit's reference length int(total_seconds * sample_rate) + 2, or -1 when total is
+ * not finite, too large, or gives a negative length (the length b2_sync_tracks_seg gives a segment video) */
+int64_t b2_segment_length(double total_seconds, int sample_rate);
+
 /* ---- synthetic PCM (bench / tests): counter-hash generator replayable in numpy -------------
  * oracle/vad_oracle.py:synth_pcm.  window_class: uint8 per 10 ms window (0 silence, 1 voiced,
  * 2 loud hiss), device or host per memspace; writes n_windows*fpw int16 samples. */
