@@ -31,7 +31,8 @@ EXPORTS = [
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
-    "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length",
+    "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
+    "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -140,6 +141,13 @@ def load() -> ctypes.CDLL:
         lib.b2_apply_sync.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int,
                                       ctypes.c_int, _f64, ctypes.c_int, _f64, _f64, _f64, ctypes.c_int, _f64,
                                       _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_ingest_begin.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _f64, _i64,
+                                        ctypes.c_int, ctypes.c_int, _f64, _f64, _i64, _f64, _i64, _vp]
+        lib.b2_ingest_push.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp]
+        lib.b2_ingest_windows.argtypes = [_vp, _vp]
+        lib.b2_ingest_sync_tracks.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _f64, _i64,
+                                              _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_ingest_abort.argtypes = [_vp]
         _lib = lib
         return lib
 
@@ -723,6 +731,89 @@ class Handle:
                           cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds, max_offset_samples,
                           (best_score, best_offset, best_k, all_score, all_offset, gss_ratio, gss_evals), want_all,
                           memspace, gss=bool(gss), want_evals=want_evals)
+
+    # batched ingest session (b2_ingest_*): push() returns before the chunks are processed
+    def ingest_begin(self, V: int, frame_rate: int, sample_rate: int, non_speech_label: float,
+                     detector: int = B2_DETECTOR_ENERGY_ZCR, energy_threshold: int = 0, z_lo: int = -1, z_hi: int = -1,
+                     chunk_samples: int = 0, energy_threshold_db: float = 50.0, min_length: Optional[float] = None,
+                     max_length: Optional[int] = None, max_continuous_silence: Optional[float] = None,
+                     expect_samples=None) -> None:
+        """Open a session for V videos (b2_ingest_begin); detector arguments as for sync_tracks_subs, expect_samples
+        [V] a sizing hint (or None)."""
+        tok = _auditok_tokenizer(sample_rate, min_length, max_length, max_continuous_silence)
+        expect = None if expect_samples is None else _i64a(expect_samples)
+        if expect is not None and len(expect) != V:
+            raise NativeError(-1, "b2_ingest_begin", "expect_samples has %d entries for %d videos" % (len(expect), V))
+        self._check(self.lib.b2_ingest_begin(self.h, int(V), frame_rate, sample_rate, int(detector),
+                                             float(non_speech_label), int(energy_threshold), int(z_lo), int(z_hi),
+                                             float(energy_threshold_db), tok[0], tok[1], tok[2], int(chunk_samples),
+                                             _ptr(expect)), "b2_ingest_begin")
+        self._ingest_V = int(V)
+
+    def ingest_push(self, videos, chunks) -> None:
+        """Append chunks[i] (bytes-like, uint8 or int16 array) to video videos[i], in order (b2_ingest_push).  The
+        library has copied them when this returns."""
+        bufs = []
+        for c in chunks:
+            if isinstance(c, np.ndarray):
+                bufs.append(np.ascontiguousarray(c).view(np.uint8).reshape(-1))
+            else:
+                bufs.append(np.frombuffer(c, dtype=np.uint8))
+        n = len(bufs)
+        video = np.ascontiguousarray(videos, dtype=np.int32)
+        if len(video) != n:
+            raise NativeError(-1, "b2_ingest_push", "%d videos for %d chunks" % (len(video), n))
+        ptrs = (ctypes.c_void_p * max(n, 1))(*[b.ctypes.data if len(b) else None for b in bufs])
+        sizes = np.array([len(b) for b in bufs], dtype=np.int64)
+        self._check(self.lib.b2_ingest_push(self.h, n, _ptr(video), ptrs, _ptr(sizes)), "b2_ingest_push")
+
+    def ingest_windows(self) -> np.ndarray:
+        out = np.zeros(max(getattr(self, "_ingest_V", 0), 1), dtype=np.int64)
+        self._check(self.lib.b2_ingest_windows(self.h, _ptr(out)), "b2_ingest_windows")
+        return out[: getattr(self, "_ingest_V", 0)]
+
+    def ingest_abort(self) -> None:
+        self._check(self.lib.b2_ingest_abort(self.h), "b2_ingest_abort")
+
+    def ingest_sync_tracks(self, track_video, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds: float,
+                           max_offset_samples: Optional[int], gss: bool = False, best_score=None, best_offset=None,
+                           best_k=None, all_score=None, all_offset=None, gss_ratio=None, gss_evals=None,
+                           want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST):
+        """Flush, sync the tracks against the session's references and close it (b2_ingest_sync_tracks).  Outputs as
+        for sync_tracks / sync_tracks_gss (memspace B2_HOST allocates them; B2_DEVICE takes device pointers).
+        Returns (best_score, best_offset, best_k, all_score, all_offset), plus (gss_ratio, gss_evals) with gss."""
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        cue_off = _i64a(cue_off)
+        T = len(track_video)
+        if len(cue_off) != T + 1:
+            self.ingest_abort()
+            raise NativeError(-1, "b2_ingest_sync_tracks", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        K = len(ratios)
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        cue_keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
+        if memspace == B2_HOST:
+            best_score = np.empty(T, dtype=np.float64)
+            best_offset = np.empty(T, dtype=np.int32)
+            best_k = np.empty(T, dtype=np.int32)
+            gss_ratio = np.empty(T, dtype=np.float64) if gss else None
+            if want_all:
+                cols = K + 1 if gss else K
+                all_score = np.empty(T * cols, dtype=np.float64)
+                all_offset = np.empty(T * cols, dtype=np.int32)
+            gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64) if gss and want_evals else None
+        elif gss and gss_ratio is None:
+            self.ingest_abort()
+            raise ValueError("b2_ingest_sync_tracks with the search on device memory needs gss_ratio")
+        st = self.lib.b2_ingest_sync_tracks(
+            self.h, _ptr(track_video), T, _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off),
+            _ptr(ratios), K, float(start_seconds), _mask_width(max_offset_samples), _ptr(best_score),
+            _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
+            _ptr(gss_evals) if gss else None, memspace)
+        self._check(st, "b2_ingest_sync_tracks")
+        res = (best_score, best_offset, best_k, all_score, all_offset)
+        return res + (gss_ratio, gss_evals) if gss else res
 
     def segment_length(self, total_seconds: float, sample_rate: int) -> int:
         """The reference length int(total_seconds * sample_rate) + 2 of a segment video (b2_segment_length); raises

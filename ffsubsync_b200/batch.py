@@ -1001,6 +1001,170 @@ class BatchSynchronizer:
                       chunk_samples=self.chunk_samples, out=ref64.data_ptr(), memspace=_native.B2_DEVICE)
         return ref64.to(torch.float32), ref_off
 
+    def ingest(self, V: int, expect_samples=None) -> "IngestSession":
+        """A batched ingest session for V videos (b2_ingest_*): their PCM arrives in pushes of any size and the
+        detector runs on the device as it comes, so only the reference signals are ever held - not the videos'
+        whole decodes.  The results equal the whole-PCM sync methods' over the same bytes.  expect_samples [V]: a
+        sizing hint (e.g. ffprobe's duration times frame_rate); a longer video still fits.  The audio detector is
+        this synchroniser's (the one after ``subs_then_``); a session has no subtitle, PGS, signal or segment
+        references."""
+        return IngestSession(self, V, expect_samples)
+
+
+class IngestSession:
+    """A batched ingest session (``BatchSynchronizer.ingest``).  ``push`` / ``push_many`` append s16le mono PCM to
+    videos in any sizes and interleaving (bytes, uint8 or int16 arrays; copied before they return, detected on the
+    device without a host synchronisation), ``windows`` reports the reference frames fixed so far, and
+    ``sync_tracks`` runs the sync chain over the references and closes the session.  The handle is shared with the
+    synchroniser and is not thread-safe: push from one thread."""
+
+    def __init__(self, sync: BatchSynchronizer, V: int, expect_samples=None) -> None:
+        self.sync = sync
+        self.V = int(V)
+        self._bytes = np.zeros(self.V, dtype=np.int64)
+        det = _native.B2_DETECTOR_AUDITOK if sync.auditok else _native.B2_DETECTOR_ENERGY_ZCR
+        sync.handle.ingest_begin(self.V, sync.frame_rate, sync.sample_rate, sync.non_speech_label, detector=det,
+                                 energy_threshold=sync.energy_threshold, z_lo=sync.z_lo, z_hi=sync.z_hi,
+                                 chunk_samples=sync.chunk_samples, expect_samples=expect_samples)
+
+    def push(self, video: int, chunk) -> None:
+        self.push_many([video], [chunk])
+
+    def push_many(self, videos, chunks) -> None:
+        """chunks[i] to video videos[i], in order (one b2_ingest_push)."""
+        self.sync.handle.ingest_push(videos, chunks)
+        for v, c in zip(videos, chunks):
+            self._bytes[int(v)] += memoryview(c).nbytes
+
+    def windows(self) -> np.ndarray:
+        return self.sync.handle.ingest_windows()
+
+    def abort(self) -> None:
+        self.sync.handle.ingest_abort()
+
+    def sync_tracks(self, track_video, cue_start, cue_end, cue_off, cue_keep=None, speech_video=None, out=None,
+                    all_out=None, want_all: bool = False):
+        """Sync track t (cue list cue_off[t] .. cue_off[t+1]) against video track_video[t] (non-decreasing) and close
+        the session.  Without ``out``: what ``sync_host_tracks`` returns over the videos' PCM back to back.  With
+        ``out`` (CUDA tensors best_score f64[T], best_offset i32[T], best_k i32[T], gss_ratio f64[T] with the search;
+        ``all_out`` as for sync_device_tracks): what ``sync_device_tracks`` returns, with nothing synchronised.
+        ``speech_video`` as there.  The golden-section search runs on the device only: outside its envelope the call
+        raises (there is no PCM left to compose it from)."""
+        s = self.sync
+        h = s.handle
+        pcm_off = np.concatenate([[0], np.cumsum(self._bytes // 2)]).astype(np.int64)
+        on_device = out is not None
+        try:
+            speech = s._speech_request(speech_video, pcm_off, on_device=on_device)
+        except Exception:
+            self.abort()
+            raise
+        cues = (track_video, cue_start, cue_end, cue_keep, cue_off, s.ratios, s.start_seconds, s.max_offset_samples)
+        with s._speech_output(speech):
+            if on_device:
+                ptrs = {k: out[k].data_ptr() for k in ("best_score", "best_offset", "best_k")}
+                if s.gss:
+                    ptrs["gss_ratio"] = out["gss_ratio"].data_ptr()
+                if all_out:
+                    ptrs.update(all_score=all_out["score"].data_ptr(), all_offset=all_out["offset"].data_ptr())
+                h.ingest_sync_tracks(*cues, gss=s.gss, memspace=_native.B2_DEVICE, **ptrs)
+            else:
+                res = h.ingest_sync_tracks(*cues, gss=s.gss, want_all=want_all, memspace=_native.B2_HOST)
+        if on_device:
+            if speech is not None:
+                out["speech"], out["speech_off"] = s._speech_result(speech)
+            return out
+        res = res[:6] if want_all else res[:3] + res[5:6]
+        return res if speech is None else res + s._speech_result(speech)
+
+
+def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, cue_off, cue_keep=None,
+               max_decoders: int = 4, ffmpeg_path: Optional[str] = None, max_duration_seconds: Optional[float] = None,
+               ref_stream: Optional[str] = None, expect_samples=None, speech_video=None, want_all: bool = False):
+    """``ffs movie.mkv -i a.srt ...`` for a library: decodes paths[v] with up to ``max_decoders`` ffmpeg processes at
+    a time (VideoSpeechTransformer._build_ffmpeg_args: ``-ss`` from the synchroniser's start_seconds, ``-t`` from
+    max_duration_seconds, ffmpeg_path, ref_stream), reads each pipe in the reference's 100 s ``read()`` calls on a
+    thread per decoder, pushes the chunks into one ingest session from this thread, and syncs the tracks as
+    ``IngestSession.sync_tracks`` does on the host.  No video's whole decode is ever held."""
+    import queue
+    import shutil
+    import subprocess
+    import threading
+
+    from .constants import detector_chunk_bytes
+    from .speech_transformers import VideoSpeechTransformer
+    vst = VideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate, frame_rate=sync.frame_rate,
+                                 non_speech_label=sync.non_speech_label, start_seconds=sync.start_seconds,
+                                 ffmpeg_path=ffmpeg_path, ref_stream=ref_stream,
+                                 max_duration_seconds=max_duration_seconds)
+    args = [vst._build_ffmpeg_args(p) for p in paths]
+    if args and shutil.which(args[0][0]) is None:
+        raise ValueError("cannot decode media: no ffmpeg binary found at %r" % args[0][0])
+    n_read = detector_chunk_bytes(sync.frame_rate, sync.sample_rate)
+    n_workers = max(1, min(int(max_decoders), len(paths)))
+    chunks: "queue.Queue" = queue.Queue(maxsize=2 * n_workers)
+    todo: "queue.Queue" = queue.Queue()
+    for v in range(len(paths)):
+        todo.put(v)
+    stop = threading.Event()
+
+    def decode(v: int):
+        """Pushes video v's 100 s reads to `chunks`; returns why it failed (None: it did not)."""
+        proc = subprocess.Popen(args[v], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL)
+        try:
+            while not stop.is_set():
+                data = proc.stdout.read(n_read)
+                if not data:
+                    break
+                chunks.put((v, data, None))
+        finally:
+            if stop.is_set():
+                proc.kill()
+            proc.stdout.close()
+            status = proc.wait()
+        return "ffmpeg exited with status %d" % status if status and not stop.is_set() else None
+
+    def worker() -> None:
+        # every video taken ends with exactly one (v, None, error) sentinel, whatever happens while decoding it
+        while not stop.is_set():
+            try:
+                v = todo.get_nowait()
+            except queue.Empty:
+                return
+            try:
+                err = decode(v)
+            except Exception as e:   # Popen or the pipe failed (missing binary, EMFILE, ...)
+                err = "%s: %s" % (type(e).__name__, e)
+            chunks.put((v, None, err))
+
+    session = sync.ingest(len(paths), expect_samples)
+    threads = [threading.Thread(target=worker, daemon=True) for _ in range(n_workers)]
+    for t in threads:
+        t.start()
+    try:
+        left = len(paths)
+        while left:
+            v, data, err = chunks.get()
+            if data is not None:
+                session.push(v, data)
+                continue
+            left -= 1
+            if err:
+                raise RuntimeError("decoding %r failed: %s" % (paths[v], err))
+    except BaseException:
+        stop.set()
+        session.abort()
+        while any(t.is_alive() for t in threads):   # drain so that no decoder blocks on a full queue
+            try:
+                chunks.get(timeout=0.05)
+            except queue.Empty:
+                pass
+        raise
+    for t in threads:
+        t.join()
+    return session.sync_tracks(track_video, cue_start, cue_end, cue_off, cue_keep, speech_video=speech_video,
+                               want_all=want_all)
+
 
 def select_reference_streams(V: int, cue_start, cue_end, cue_off, stream_video, start_seconds: float = 0.0,
                              content=None, keep=None):

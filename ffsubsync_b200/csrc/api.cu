@@ -12,6 +12,7 @@
 #include <thread>
 
 #include "common.cuh"
+#include "ingest_plan.h"
 #include "sync_plan.h"
 #include "sync_output.cuh"
 #include "speech_out.cuh"
@@ -88,11 +89,14 @@ extern "C" int b2_create(int device, b2_handle* out) {
   return B2_OK;
 }
 
+static void ingest_free(b2_ctx* h);
+
 extern "C" int b2_destroy(b2_handle h) {
   if (!h) return B2_OK;
   DeviceScope scope(h->device);
   if (h->stream2) cudaStreamSynchronize(h->stream2);
   cudaStreamSynchronize(h->stream);
+  ingest_free(h);
   for (auto& w : h->ws)
     if (w.p) cudaFree(w.p);
   for (auto& p : h->pinned)
@@ -1045,8 +1049,22 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // With sampled segments (b2_sync_tracks_seg) a segment video is empty in the main launch (plan det_end); a second
 // detector launch reads only its segments' samples into the scratch (floats), and seg_ref_kernel writes its reference
 // from there, floats or bits, and resets and sets its speech flag.
+// With ingested references (b2_ingest_sync_tracks) the detector already ran as the PCM arrived: the step copies the
+// videos' references from the session's buffer to their ranges, one copy per run of videos stored back to back.
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
                   bool ref_packed) {
+  if (r.ready.len) {
+    for (int v = v0; v < v1;) {
+      int w = v + 1;
+      while (w < v1 && r.ready.at[w] == r.ready.at[w - 1] + r.ready.len[w - 1]) ++w;
+      const int64_t n = p.ref_off[w] - p.ref_off[v];
+      if (n > 0)
+        B2_CUDA(h, cudaMemcpyAsync(b.refsig + p.ref_off[v], r.ready.ref + r.ready.at[v], (size_t)n * 4,
+                                   cudaMemcpyDeviceToDevice, h->stream));
+      v = w;
+    }
+    return B2_OK;
+  }
   const bool seg = !p.det_end.empty();
   if (!p.auditok) {
     // a packed sub-batch of signal (or segment) videos alone has no audio: the VAD has no tiles and is not asked
@@ -1658,6 +1676,354 @@ extern "C" int b2_sync_tracks_seg(b2_handle h, const int16_t* pcm, const int64_t
   r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
   r.sig = {ref_is_sig, x, V > 0 ? sig_off : nullptr};
   r.seg = {n_seg_videos, seg_video, seg_total, n_seg_videos > 0 ? seg_off : no_segments, seg_start, seg_lo, seg_hi};
+  return sync_run(h, _b2_fence_was_valid, r);
+}
+
+// ---- batched ingest session (b2_ingest_*, DESIGN.md section 4 "K1i") ---------------------------------------------
+// The reference's chunk loop (speech_transformers.py:680-753) for V videos at once: each push is cut by the span
+// planner (ingest_plan.h), its spans staged in a ring slot of pinned host and device memory, copied to the device
+// and run through the detector in one b2i_vad_launch over a table of (staging offset, samples, destination frame);
+// for auditok the tokenizer then runs over every detector call the push completed.  Only the references stay on
+// the device, video v's at frames [at[v], at[v] + cap[v]) of one buffer; b2_ingest_sync_tracks hands them to the
+// batched sync calls' chain as ingested references (SyncRequest::ready).
+struct IngestSession {
+  static const int kSlots = 3;
+  struct Slot {
+    void* hp = nullptr;   // pinned staging
+    void* dp = nullptr;   // device staging
+    size_t cap = 0;
+    cudaEvent_t ev = nullptr;
+    bool busy = false;
+  } slot[kSlots];
+  uint64_t seq = 0;
+  bool active = false;
+  SyncRequest req{};                  // the detector arguments, as the sync call passes them
+  SyncPlan det;                       // fpw, z_lo, z_hi, auditok_e_min, tok of those arguments
+  IngestPlanner plan;
+  std::vector<std::vector<uint8_t>> held;   // video v's stream bytes [2 * plan.base[v], plan.bytes[v])
+  float* ref = nullptr;               // cudaMallocAsync on the handle's stream
+  std::vector<int64_t> at, cap;
+};
+
+static void ingest_release_ref(b2_ctx* h, IngestSession* s) {
+  if (s->ref) cudaFreeAsync(s->ref, h->stream);   // behind every kernel and copy that reads or writes it
+  s->ref = nullptr;
+  s->active = false;
+  s->held.clear();
+}
+
+static void ingest_free(b2_ctx* h) {
+  IngestSession* s = h->ingest;
+  if (!s) return;
+  ingest_release_ref(h, s);
+  cudaStreamSynchronize(h->stream);
+  for (auto& sl : s->slot) {
+    if (sl.hp) cudaFreeHost(sl.hp);
+    if (sl.dp) cudaFree(sl.dp);
+    if (sl.ev) cudaEventDestroy(sl.ev);
+  }
+  delete s;
+  h->ingest = nullptr;
+}
+
+// Room for frames [at[v], at[v] + need[v]) of every video.  On overflow every region grows to at least twice what its
+// video needs and to what the longest video needs (videos decoded side by side grow alike), the written frames are
+// copied over on the stream, and the old buffer is freed behind them.
+static int ingest_reserve(b2_ctx* h, IngestSession* s, const std::vector<int64_t>& need) {
+  const int V = (int)need.size();
+  bool grow = false;
+  int64_t longest = 0;
+  for (int v = 0; v < V; ++v) {
+    grow = grow || need[v] > s->cap[v];
+    longest = std::max(longest, need[v]);
+  }
+  if (!grow) return B2_OK;
+  std::vector<int64_t> at(V), cap(V);
+  int64_t total = 0;
+  for (int v = 0; v < V; ++v) {
+    cap[v] = std::max(s->cap[v], std::max(2 * need[v], longest));
+    at[v] = total;
+    total += cap[v];
+  }
+  float* ref = nullptr;
+  const cudaError_t e = cudaMallocAsync((void**)&ref, (size_t)total * 4 + 16, h->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    B2_FAIL(h, B2_ERR_NOMEM, "ingest: cudaMallocAsync(%lld frames) for the references failed: %s", (long long)total,
+            cudaGetErrorString(e));
+  }
+  for (int v = 0; v < V; ++v) {   // every frame written so far lies in the old region
+    const int64_t m = std::min(s->cap[v], need[v]);
+    if (m > 0)
+      B2_CUDA(h, cudaMemcpyAsync(ref + at[v], s->ref + s->at[v], (size_t)m * 4, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  if (s->ref) B2_CUDA(h, cudaFreeAsync(s->ref, h->stream));
+  s->ref = ref;
+  s->at.swap(at);
+  s->cap.swap(cap);
+  return B2_OK;
+}
+
+// Appends the bytes [b0, b1) of the concatenation a ++ b (lengths na, nb) to dst
+static void concat_bytes(uint8_t* dst, const uint8_t* a, int64_t na, const uint8_t* b, int64_t b0, int64_t b1) {
+  if (b0 < na) {
+    const int64_t m = std::min(b1, na) - b0;
+    memcpy(dst, a + b0, (size_t)m);
+    dst += m;
+    b0 += m;
+  }
+  if (b1 > b0) memcpy(dst, b + (b0 - na), (size_t)(b1 - b0));
+}
+
+// Videos' streams grew by the chunks (video[i], bytes[i], n_bytes[i]) (n = 0 and final: every video's end): plans the
+// spans, stages them in the next ring slot, and enqueues the copy, the detector launch and the tokenizer launch.
+static int ingest_enqueue(b2_ctx* h, IngestSession* s, int n, const int32_t* video, const void* const* bytes,
+                          const int64_t* n_bytes, bool final) {
+  IngestPlanner& pl = s->plan;
+  const int V = (int)pl.bytes.size(), fpw = pl.fpw;
+  // staging bound: every chunk with a held-back window and an odd byte in front, 16 bytes of alignment per span
+  size_t bound = 0;
+  auto spans_bound = [&](int64_t nb) { return 2 + (pl.chunk > 0 ? (nb / 2 + fpw) / pl.chunk : 0); };
+  for (int i = 0; i < n; ++i) bound += (size_t)n_bytes[i] + 2 * fpw + 2 + 16 * spans_bound(n_bytes[i] + 2 * fpw);
+  if (final)
+    for (int v = 0; v < V; ++v) bound += s->held[v].size() + 16 * 2;
+  IngestSession::Slot& sl = s->slot[s->seq % IngestSession::kSlots];
+  if (sl.busy) B2_CUDA(h, cudaEventSynchronize(sl.ev));   // the push kSlots ago has read this slot
+  sl.busy = false;
+  if (bound > sl.cap) {
+    if (sl.hp) B2_CUDA(h, cudaFreeHost(sl.hp));
+    if (sl.dp) B2_CUDA(h, cudaFree(sl.dp));
+    sl.hp = sl.dp = nullptr;
+    sl.cap = 0;
+    const size_t want = bound + bound / 4 + 4096;
+    B2_CUDA(h, cudaMallocHost(&sl.hp, want));
+    B2_CUDA(h, cudaMalloc(&sl.dp, want));
+    sl.cap = want;
+  }
+  if (!sl.ev) B2_CUDA(h, cudaEventCreateWithFlags(&sl.ev, cudaEventDisableTiming));
+  std::vector<IngestSpan> spans;
+  std::vector<IngestChunk> chunks;
+  std::vector<int64_t> stage;   // per span: its first sample in the slot (a multiple of 8)
+  int64_t used = 0;             // samples
+  auto add = [&](int v, const uint8_t* src, int64_t nsrc, int64_t base0, size_t from) {
+    // the spans from index `from` on read video v's bytes [2 * base0, ...) = held ++ src
+    const std::vector<uint8_t>& hv = s->held[v];
+    for (size_t j = from; j < spans.size(); ++j) {
+      const IngestSpan& sp = spans[j];
+      stage.push_back(used);
+      concat_bytes((uint8_t*)sl.hp + used * 2, hv.data(), (int64_t)hv.size(), src, 2 * (sp.s0 - base0),
+                   2 * (sp.s1 - base0));
+      used += (sp.s1 - sp.s0 + 7) & ~(int64_t)7;
+    }
+    // the new held-back bytes
+    const int64_t keep0 = 2 * (pl.base[v] - base0), total = (int64_t)hv.size() + nsrc;
+    std::vector<uint8_t> rest((size_t)(total - keep0));
+    concat_bytes(rest.data(), hv.data(), (int64_t)hv.size(), src, keep0, total);
+    s->held[v].swap(rest);
+  };
+  for (int i = 0; i < n; ++i) {
+    const int v = video[i];
+    const int64_t base0 = pl.base[v];
+    const size_t from = spans.size();
+    pl.push(v, n_bytes[i], &spans, &chunks);
+    add(v, (const uint8_t*)bytes[i], n_bytes[i], base0, from);
+  }
+  if (final)
+    for (int v = 0; v < V; ++v) {
+      const int64_t base0 = pl.base[v];
+      const size_t from = spans.size();
+      pl.finish(v, &spans, &chunks);
+      add(v, nullptr, 0, base0, from);
+    }
+  ++s->seq;
+  const SyncPlan& dp = s->det;
+  if (!spans.empty()) {
+    B2_TRY(ingest_reserve(h, s, pl.frames));
+    B2_CUDA(h, cudaMemcpyAsync(sl.dp, sl.hp, (size_t)used * 2, cudaMemcpyHostToDevice, h->stream));
+    // the launch table: span j is entry 2j; entry 2j + 1 is an empty gap up to span j + 1's first frame, so that
+    // out_off[2j + 1] - out_off[2j] is span j's window count while destinations need not be ordered
+    const int S = (int)spans.size(), B = 2 * S - 1;
+    std::vector<int64_t> off(B + 1), end(B), out(B + 1), tail(B, 0);
+    for (int j = 0; j < S; ++j) {
+      const IngestSpan& sp = spans[j];
+      const int64_t d = s->at[sp.video] + sp.frame;
+      off[2 * j] = stage[j];
+      end[2 * j] = stage[j] + (sp.s1 - sp.s0);
+      out[2 * j] = d;
+      out[2 * j + 1] = d + (sp.s1 - sp.s0 + fpw - 1) / fpw;
+      tail[2 * j] = sp.tail;
+      if (j + 1 < S) off[2 * j + 1] = end[2 * j + 1] = end[2 * j];
+    }
+    off[B] = end[B - 1];
+    if (!pl.auditok)
+      B2_TRY(b2i_vad_launch(h, (const int16_t*)sl.dp, off.data(), B, fpw, s->req.energy.non_speech_label,
+                            (int64_t)fpw * s->req.energy.energy_threshold, dp.z_lo, dp.z_hi, s->ref, out.data(),
+                            nullptr, false, end.data()));
+    else   // the energy pass (label 0, every crossing count, a closed call's short last block on its own samples)
+      B2_TRY(b2i_vad_launch(h, (const int16_t*)sl.dp, off.data(), B, fpw, 0.0f, dp.auditok_e_min, 0, fpw, s->ref,
+                            out.data(), tail.data(), false, end.data()));
+    B2_CUDA(h, cudaEventRecord(sl.ev, h->stream));
+    sl.busy = true;
+  }
+  // auditok: the tokenizer over every detector call this step completed.  A call can complete without a span of its
+  // own here: the flush closes a video's last call even when its length ends on a window boundary (nothing held back).
+  if (!chunks.empty()) {
+    std::vector<int64_t> c0(chunks.size() + 1), c1(chunks.size());
+    for (size_t k = 0; k < chunks.size(); ++k) {
+      c0[k] = s->at[chunks[k].video] + chunks[k].f0;
+      c1[k] = s->at[chunks[k].video] + chunks[k].f1;
+    }
+    c0.back() = c1.back();
+    B2_TRY(b2i_tokenize_inplace_launch(h, s->ref, c0.data(), (int)chunks.size(), dp.tok, c1.data()));
+  }
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_begin(b2_handle h, int V, int frame_rate, int sample_rate, int detector,
+                               double non_speech_label, int64_t energy_threshold, int z_lo, int z_hi,
+                               double energy_threshold_db, double min_length, int64_t max_length,
+                               double max_continuous_silence, int64_t chunk_samples, const int64_t* expect_samples) {
+  B2_ENTER(h);
+  if (h->ingest && h->ingest->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_begin: a session is already open on this handle");
+  if (V < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_begin: V = %d < 0", V);
+  if (detector != B2_DETECTOR_ENERGY_ZCR && detector != B2_DETECTOR_AUDITOK)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_begin: detector must be B2_DETECTOR_ENERGY_ZCR or B2_DETECTOR_AUDITOK, not %d",
+            detector);
+  for (int v = 0; expect_samples && v < V; ++v)
+    if (expect_samples[v] < 0)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_begin: expect_samples[%d] = %lld < 0", v, (long long)expect_samples[v]);
+  // the detector arguments and their checks: the sync calls' own (plan_references), on a call without videos
+  static const int64_t no_pcm[1] = {0};
+  SyncRequest r{};
+  r.who = "ingest_begin";
+  r.pcm_off = no_pcm;
+  r.frame_rate = frame_rate;
+  r.sample_rate = sample_rate;
+  r.detector = detector;
+  r.energy = {(float)non_speech_label, energy_threshold, z_lo, z_hi};
+  r.auditok = {non_speech_label, energy_threshold_db, min_length, max_continuous_silence, max_length, chunk_samples};
+  SyncPlan det;
+  det.auditok = detector == B2_DETECTOR_AUDITOK;
+  if (const int st = plan_references(r, &det)) {
+    h->err = det.err;
+    return st;
+  }
+  if (!h->ingest) h->ingest = new IngestSession();
+  IngestSession* s = h->ingest;
+  s->req = r;
+  s->det = det;
+  s->plan.begin(V, det.fpw, det.auditok, chunk_samples, energy_threshold_db);
+  s->held.assign(V, {});
+  s->at.assign(V, 0);
+  s->cap.assign(V, 0);
+  std::vector<int64_t> need(V, 0);
+  for (int v = 0; expect_samples && v < V; ++v) need[v] = s->plan.length(expect_samples[v]);
+  // sized to the hint exactly (regions back to back: the sync step then copies them in one piece)
+  int64_t total = 0;
+  for (int v = 0; v < V; ++v) {
+    s->at[v] = total;
+    s->cap[v] = need[v];
+    total += need[v];
+  }
+  if (total > 0) {
+    const cudaError_t e = cudaMallocAsync((void**)&s->ref, (size_t)total * 4 + 16, h->stream);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      s->ref = nullptr;
+      B2_FAIL(h, B2_ERR_NOMEM, "ingest_begin: cudaMallocAsync(%lld frames) for the references failed: %s",
+              (long long)total, cudaGetErrorString(e));
+    }
+  }
+  s->active = true;
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_push(b2_handle h, int n, const int32_t* video, const void* const* bytes,
+                              const int64_t* n_bytes) {
+  B2_ENTER(h);
+  IngestSession* s = h->ingest;
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: no open session on this handle");
+  if (n < 0 || (n > 0 && (!video || !bytes || !n_bytes)))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: bad chunk table (n = %d)", n);
+  const int V = (int)s->held.size();
+  for (int i = 0; i < n; ++i) {
+    if (video[i] < 0 || video[i] >= V)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: video %d is out of [0, %d)", i, (int)video[i], V);
+    if (n_bytes[i] < 0)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: n_bytes = %lld < 0", i, (long long)n_bytes[i]);
+    if (n_bytes[i] > 0 && !bytes[i])
+      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: null bytes with n_bytes = %lld", i, (long long)n_bytes[i]);
+  }
+  B2Range range("b2_ingest_push");
+  if (const int st = ingest_enqueue(h, s, n, video, bytes, n_bytes, false)) {
+    ingest_release_ref(h, s);   // the planner ran ahead of what reached the device: the session cannot go on
+    return st;
+  }
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_windows(b2_handle h, int64_t* windows) {
+  B2_ENTER(h);
+  IngestSession* s = h->ingest;
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_windows: no open session on this handle");
+  if (!windows && !s->held.empty()) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_windows: null windows");
+  for (size_t v = 0; v < s->held.size(); ++v) windows[v] = s->plan.frames[v];
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_abort(b2_handle h) {
+  B2_ENTER(h);
+  if (h->ingest) ingest_release_ref(h, h->ingest);
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, int T, const double* cue_start_s,
+                                     const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                     const double* ratios, int K, double start_seconds, int64_t max_offset_samples,
+                                     double* best_score, int32_t* best_offset, int32_t* best_k, double* all_score,
+                                     int32_t* all_offset, double* gss_ratio, double* gss_evals, int memspace) {
+  B2_ENTER(h);
+  B2Range range("b2_ingest_sync_tracks");
+  IngestSession* s = h->ingest;
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: no open session on this handle");
+  // the session closes whatever the outcome
+  struct Close {
+    b2_ctx* h;
+    IngestSession* s;
+    ~Close() { ingest_release_ref(h, s); }
+  } close{h, s};
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: null track_video");
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: gss_evals without gss_ratio");
+  if (memspace != B2_HOST && memspace != B2_DEVICE)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: memspace must be B2_HOST or B2_DEVICE");
+  B2_TRY(ingest_enqueue(h, s, 0, nullptr, nullptr, nullptr, true));
+  const int V = (int)s->held.size();
+  std::vector<int64_t> pcm_off(V + 1, 0);
+  SyncRequest r = s->req;
+  r.who = gss_ratio ? "ingest_sync_tracks (search)" : "ingest_sync_tracks";
+  r.pcm = nullptr;
+  r.pcm_off = pcm_off.data();
+  r.V = V;
+  r.track_video = track_video;
+  r.T = T;
+  r.cue_start_s = cue_start_s;
+  r.cue_end_s = cue_end_s;
+  r.cue_keep = cue_keep;
+  r.cue_off = cue_off;
+  r.ratios = ratios;
+  r.K = K;
+  r.start_seconds = start_seconds;
+  r.max_offset_samples = max_offset_samples;
+  r.best_score = best_score;
+  r.best_offset = best_offset;
+  r.best_k = best_k;
+  r.all_score = all_score;
+  r.all_offset = all_offset;
+  r.search = gss_ratio != nullptr;
+  r.gss_ratio = gss_ratio;
+  r.gss_evals = gss_evals;
+  r.memspace = memspace;
+  r.ready = {s->ref, s->at.data(), s->plan.frames.data()};
   return sync_run(h, _b2_fence_was_valid, r);
 }
 

@@ -121,6 +121,8 @@ struct b2_ctx {
     uint64_t seq = 0;
     std::vector<float> results;
   } vs;
+  // b2_ingest_*: the batched ingest session (api.cu), null until the first b2_ingest_begin
+  struct IngestSession* ingest = nullptr;
   // pageable B2_HOST inputs: two pinned bounce buffers filled by a few host threads (see stage_in)
   struct Bounce {
     void* p = nullptr;

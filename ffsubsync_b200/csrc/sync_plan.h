@@ -399,6 +399,16 @@ struct SyncRequest {
     const int64_t* lo;
     const int64_t* hi;
   } seg;
+  // Ingested references (b2_ingest_sync_tracks; len null: none): every video's reference is already on the device,
+  // the detector's output over its PCM as the ingest session's pushes wrote it - video v's len[v] frames at
+  // ref + at[v] (at, len: host arrays [V]).  The call has no PCM (pcm_off all equal); its detector step copies the
+  // references into the reference buffer, and the videos count as detector videos for every level and path rule.
+  // The value-initialised state is "no ingested references", so the other entry points leave it out.
+  struct {
+    const float* ref;
+    const int64_t* at;
+    const int64_t* len;
+  } ready;
 };
 
 // What plan_sync reads from the handle and the environment: the SM count, the most sub-batches the handle's
@@ -500,6 +510,12 @@ static bool audio_lane_ok(const SyncRequest& r, const SyncPipeEnv& env, const Sy
 
 static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   const int V = r.V, T = r.T;
+  if (r.ready.len) {   // ingested references: no detector step for the chains to overlap
+    p->n_sub = 1;
+    p->vad_sms = 0;
+    p->cut = {0, V};
+    return;
+  }
   // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks, and the
   // sampled segments' items
   bool lane_ok;
@@ -544,7 +560,8 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // signal videos (their chains take the run path only at label 0, where the reference has the levels 1.0 and 0.0).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
-  if ((p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
+  // ingested references are floats; the run path packs them itself (ref_bits_kernel)
+  if (r.ready.len || (p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
       (env.ref_packed && atoi(env.ref_packed) == 0))
     return;
   // how many videos of `list` lie in [v0, v1)
@@ -830,6 +847,11 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
   if (fpw <= 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
   p->z_lo = r.energy.z_lo < 0 ? 0 : r.energy.z_lo;
   p->z_hi = r.energy.z_hi < 0 ? (3 * fpw) / 8 : r.energy.z_hi;
+  p->ref_off.assign(V + 1, 0);
+  if (r.ready.len) {   // ingested references: their lengths are the pushes' (no chunk table, nothing to detect)
+    for (int v = 0; v < V; ++v) p->ref_off[v + 1] = p->ref_off[v] + r.ready.len[v];
+    return B2_OK;
+  }
   // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
   // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
   // the tracks' cues).  subs_len[v] = -1: the video's reference is the detector's.
@@ -868,7 +890,6 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
     // Segment references: int(total * sample_rate) + 2 frames (speech_transformers.py:871)
     for (int v : p->seg_video) subs_len[v] = seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate);
   }
-  p->ref_off.assign(V + 1, 0);
   for (int v = 0; v < V; ++v) {
     const int64_t n = r.pcm_off[v + 1] - r.pcm_off[v];
     if (n < 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);

@@ -579,6 +579,55 @@ int b2_speech_output(b2_handle h, double* speech, int64_t capacity, const int32_
  * not finite, too large, or gives a negative length (the length b2_sync_tracks_seg gives a segment video) */
 int64_t b2_segment_length(double total_seconds, int sample_rate);
 
+/* ---- batched ingest session: the chunk loop for a batch of decoders --------------------------------------------
+ * The reference reads ffmpeg's pipe 100 s at a time and runs the detector on each chunk as it arrives
+ * (ffsubsync/speech_transformers.py:680-753).  A session does that for V videos at once: their PCM arrives as host
+ * chunks of any size in any interleaving across videos, the detector runs on the device as they come, and only each
+ * video's reference signal stays on the device - never its PCM.  A final call runs the batched sync chain over them.
+ * Let P_v be all bytes pushed for video v, in push order, with a trailing odd byte dropped.  Whatever the cut of P_v
+ * into pushes (1-byte and odd pushes, pushes that split a window or a detector call) and the interleaving:
+ *   energy / ZCR   video v's reference is b2_vad_energy_zcr over P_v (ceil(n/fpw) windows, a partial last window
+ *                  non-speech);
+ *   auditok        it is b2_vad_auditok over P_v with chunk_samples, rounded once to float32: the tokenizer restarts
+ *                  at every chunk_samples boundary of P_v wherever the pushes fell (read(n) on a pipe returns n bytes
+ *                  until EOF, so the stream fixes the boundaries, not the caller);
+ *   the sync call  returns exactly what b2_sync_tracks (b2_sync_tracks_gss with gss_ratio) for energy / ZCR, or
+ *                  b2_sync_tracks_auditok for auditok, returns for the same tracks and arguments over the PCM
+ *                  P_0 ... P_{V-1} back to back, b2_speech_output included.
+ * b2_ingest_begin     opens the session: the detector arguments and their checks are b2_sync_tracks_subs's (detector,
+ *                     label, energy_threshold, z_lo, z_hi for energy / ZCR; energy_threshold_db ... chunk_samples for
+ *                     auditok).  expect_samples [V] (or NULL) is a sizing hint, e.g. ffprobe's duration: a video that
+ *                     outgrows it grows its buffer, it never fails.  B2_ERR_BAD_ARG for a second begin.
+ * b2_ingest_push      appends n host chunks: chunk i (bytes[i], n_bytes[i] bytes) to video video[i]; within a video
+ *                     in push order.  The library copies the chunks before it returns (the caller may reuse its buffers
+ *                     at once), enqueues the copy to the device and the detector on the handle's stream and returns
+ *                     without a host synchronisation (it waits only for the push three calls earlier to have left its
+ *                     staging slot).  B2_ERR_BAD_ARG (the message names the chunk) for a video out of range, a negative
+ *                     n_bytes or a null chunk with n_bytes > 0; such a call pushes nothing.
+ * b2_ingest_windows   windows [V]: the reference frames the pushes so far fix (an unfinished window is held back).
+ * b2_ingest_sync_tracks  flushes every video's held-back samples, then runs the chain of b2_sync_tracks (with the
+ *                     search when gss_ratio is not NULL) over the references: arguments and outputs as there, memspace
+ *                     (B2_HOST or B2_DEVICE) for the outputs only.  T == 0 with b2_speech_output set writes only the
+ *                     signals (the reference's serialize-only run).  The session closes, whatever the outcome.
+ * b2_ingest_abort     closes the session without a sync (no session: nothing to do).
+ * A push, windows or sync call without an open session is B2_ERR_BAD_ARG.  A failed call leaves the handle usable.
+ * The handle stays single-threaded: decoder threads hand their chunks to the one thread that pushes. */
+int b2_ingest_begin(b2_handle h, int V, int frame_rate, int sample_rate, int detector, double non_speech_label,
+                    int64_t energy_threshold, int z_lo, int z_hi, double energy_threshold_db, double min_length,
+                    int64_t max_length, double max_continuous_silence, int64_t chunk_samples,
+                    const int64_t* expect_samples /* [V] or NULL */);
+int b2_ingest_push(b2_handle h, int n, const int32_t* video /* [n] */, const void* const* bytes /* [n] */,
+                   const int64_t* n_bytes /* [n] */);
+int b2_ingest_windows(b2_handle h, int64_t* windows /* [V] */);
+int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video /* [T] */, int T, const double* cue_start_s,
+                          const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */,
+                          const double* ratios, int K, double start_seconds, int64_t max_offset_samples,
+                          double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                          double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
+                          double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
+                          int memspace);
+int b2_ingest_abort(b2_handle h);
+
 /* ---- synthetic PCM (bench / tests): counter-hash generator replayable in numpy -------------
  * oracle/vad_oracle.py:synth_pcm.  window_class: uint8 per 10 ms window (0 silence, 1 voiced,
  * 2 loud hiss), device or host per memspace; writes n_windows*fpw int16 samples. */
