@@ -32,7 +32,8 @@ EXPORTS = [
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
     "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
-    "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort",
+    "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort", "b2_ingest_segments", "b2_ingest_push_segments",
+    "b2_ingest_drop_segment",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -148,6 +149,9 @@ def load() -> ctypes.CDLL:
         lib.b2_ingest_sync_tracks.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _f64, _i64,
                                               _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
         lib.b2_ingest_abort.argtypes = [_vp]
+        lib.b2_ingest_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
+        lib.b2_ingest_push_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
+        lib.b2_ingest_drop_segment.argtypes = [_vp, ctypes.c_int, _i64]
         _lib = lib
         return lib
 
@@ -750,9 +754,25 @@ class Handle:
                                              _ptr(expect)), "b2_ingest_begin")
         self._ingest_V = int(V)
 
-    def ingest_push(self, videos, chunks) -> None:
-        """Append chunks[i] (bytes-like, uint8 or int16 array) to video videos[i], in order (b2_ingest_push).  The
-        library has copied them when this returns."""
+    def ingest_segments(self, seg_video, seg_total, seg_off, seg_start) -> None:
+        """Declare the session's segment videos (b2_ingest_segments): segment_table's arrays without seg_lo / seg_hi."""
+        video = np.ascontiguousarray(seg_video, dtype=np.int32)
+        total = np.ascontiguousarray(seg_total, dtype=np.float64)
+        off = _i64a(seg_off)
+        start = _i64a(seg_start)
+        if len(total) != len(video) or len(off) != len(video) + 1:
+            raise NativeError(-1, "b2_ingest_segments", "%d totals and %d offsets for %d segment videos"
+                              % (len(total), len(off), len(video)))
+        self._check(self.lib.b2_ingest_segments(self.h, len(video), _ptr(video), _ptr(total), _ptr(off), _ptr(start)),
+                    "b2_ingest_segments")
+
+    def ingest_drop_segment(self, video: int, segment: int) -> None:
+        self._check(self.lib.b2_ingest_drop_segment(self.h, int(video), int(segment)), "b2_ingest_drop_segment")
+
+    def ingest_push(self, videos, chunks, segments=None) -> None:
+        """Append chunks[i] (bytes-like, uint8 or int16 array) to video videos[i], in order (b2_ingest_push), or with
+        ``segments`` to its segment segments[i] (b2_ingest_push_segments).  The library has copied them when this
+        returns."""
         bufs = []
         for c in chunks:
             if isinstance(c, np.ndarray):
@@ -765,7 +785,14 @@ class Handle:
             raise NativeError(-1, "b2_ingest_push", "%d videos for %d chunks" % (len(video), n))
         ptrs = (ctypes.c_void_p * max(n, 1))(*[b.ctypes.data if len(b) else None for b in bufs])
         sizes = np.array([len(b) for b in bufs], dtype=np.int64)
-        self._check(self.lib.b2_ingest_push(self.h, n, _ptr(video), ptrs, _ptr(sizes)), "b2_ingest_push")
+        if segments is None:
+            self._check(self.lib.b2_ingest_push(self.h, n, _ptr(video), ptrs, _ptr(sizes)), "b2_ingest_push")
+            return
+        seg = _i64a(segments)
+        if len(seg) != n:
+            raise NativeError(-1, "b2_ingest_push_segments", "%d segments for %d chunks" % (len(seg), n))
+        self._check(self.lib.b2_ingest_push_segments(self.h, n, _ptr(video), _ptr(seg), ptrs, _ptr(sizes)),
+                    "b2_ingest_push_segments")
 
     def ingest_windows(self) -> np.ndarray:
         out = np.zeros(max(getattr(self, "_ingest_V", 0), 1), dtype=np.int64)

@@ -1001,14 +1001,17 @@ class BatchSynchronizer:
                       chunk_samples=self.chunk_samples, out=ref64.data_ptr(), memspace=_native.B2_DEVICE)
         return ref64.to(torch.float32), ref_off
 
-    def ingest(self, V: int, expect_samples=None) -> "IngestSession":
+    def ingest(self, V: int, expect_samples=None, segments=None) -> "IngestSession":
         """A batched ingest session for V videos (b2_ingest_*): their PCM arrives in pushes of any size and the
         detector runs on the device as it comes, so only the reference signals are ever held - not the videos'
         whole decodes.  The results equal the whole-PCM sync methods' over the same bytes.  expect_samples [V]: a
         sizing hint (e.g. ffprobe's duration times frame_rate); a longer video still fits.  The audio detector is
-        this synchroniser's (the one after ``subs_then_``); a session has no subtitle, PGS, signal or segment
-        references."""
-        return IngestSession(self, V, expect_samples)
+        this synchroniser's (the one after ``subs_then_``); a session has no subtitle, PGS or signal references.
+        segments (``--multi-segment-sync``): dict(seg_video, seg_total, seg_off, seg_start), e.g. from
+        ``ingest_segment_table``; those videos take their sampled segments' PCM (``push_segment``) and are synced
+        against the sparse reference, as the sync methods with ``segment_table(..., piece_samples=...)`` over the
+        pieces pushed.  A segment video's expect_samples entry is the hint for each of its segments."""
+        return IngestSession(self, V, expect_samples, segments)
 
 
 class IngestSession:
@@ -1018,23 +1021,44 @@ class IngestSession:
     ``sync_tracks`` runs the sync chain over the references and closes the session.  The handle is shared with the
     synchroniser and is not thread-safe: push from one thread."""
 
-    def __init__(self, sync: BatchSynchronizer, V: int, expect_samples=None) -> None:
+    def __init__(self, sync: BatchSynchronizer, V: int, expect_samples=None, segments=None) -> None:
         self.sync = sync
         self.V = int(V)
         self._bytes = np.zeros(self.V, dtype=np.int64)
+        self._seg = None
         det = _native.B2_DETECTOR_AUDITOK if sync.auditok else _native.B2_DETECTOR_ENERGY_ZCR
         sync.handle.ingest_begin(self.V, sync.frame_rate, sync.sample_rate, sync.non_speech_label, detector=det,
                                  energy_threshold=sync.energy_threshold, z_lo=sync.z_lo, z_hi=sync.z_hi,
                                  chunk_samples=sync.chunk_samples, expect_samples=expect_samples)
+        if segments is not None:
+            try:
+                sync.handle.ingest_segments(*(segments[k] for k in ("seg_video", "seg_total", "seg_off", "seg_start")))
+            except BaseException:
+                self.abort()
+                raise
+            # (seg_video, seg_total): what _reference_lengths and the no-speech rule read of a segment table
+            self._seg = (np.asarray(segments["seg_video"], dtype=np.int32),
+                         np.asarray(segments["seg_total"], dtype=np.float64))
 
     def push(self, video: int, chunk) -> None:
         self.push_many([video], [chunk])
 
-    def push_many(self, videos, chunks) -> None:
-        """chunks[i] to video videos[i], in order (one b2_ingest_push)."""
-        self.sync.handle.ingest_push(videos, chunks)
-        for v, c in zip(videos, chunks):
-            self._bytes[int(v)] += memoryview(c).nbytes
+    def push_segment(self, video: int, segment: int, chunk) -> None:
+        """chunk to segment ``segment`` (counted within the video's segments) of segment video ``video``."""
+        self.push_many([video], [chunk], segments=[segment])
+
+    def push_many(self, videos, chunks, segments=None) -> None:
+        """chunks[i] to video videos[i], in order (one b2_ingest_push), or with ``segments`` to its segment segments[i]
+        (one b2_ingest_push_segments)."""
+        self.sync.handle.ingest_push(videos, chunks, segments)
+        if segments is None:
+            for v, c in zip(videos, chunks):
+                self._bytes[int(v)] += memoryview(c).nbytes
+
+    def drop_segment(self, video: int, segment: int) -> None:
+        """Discard a segment (the reference's "failed to extract segment"): what was pushed to it takes no part in the
+        reference, and a later push to it is refused."""
+        self.sync.handle.ingest_drop_segment(video, segment)
 
     def windows(self) -> np.ndarray:
         return self.sync.handle.ingest_windows()
@@ -1049,13 +1073,14 @@ class IngestSession:
         ``out`` (CUDA tensors best_score f64[T], best_offset i32[T], best_k i32[T], gss_ratio f64[T] with the search;
         ``all_out`` as for sync_device_tracks): what ``sync_device_tracks`` returns, with nothing synchronised.
         ``speech_video`` as there.  The golden-section search runs on the device only: outside its envelope the call
-        raises (there is no PCM left to compose it from)."""
+        raises (there is no PCM left to compose it from).  A segment video without a frame > 0 raises the reference's
+        ValueError on the host and gets ``best_k == B2_BEST_K_NO_SPEECH`` on the device, as the sync methods do."""
         s = self.sync
         h = s.handle
         pcm_off = np.concatenate([[0], np.cumsum(self._bytes // 2)]).astype(np.int64)
         on_device = out is not None
         try:
-            speech = s._speech_request(speech_video, pcm_off, on_device=on_device)
+            speech = s._speech_request(speech_video, pcm_off, seg=self._seg, on_device=on_device)
         except Exception:
             self.abort()
             raise
@@ -1074,49 +1099,104 @@ class IngestSession:
             if speech is not None:
                 out["speech"], out["speech_off"] = s._speech_result(speech)
             return out
+        s._raise_no_speech(self._seg, res[2], track_video)
         res = res[:6] if want_all else res[:3] + res[5:6]
         return res if speech is None else res + s._speech_result(speech)
 
 
+def ingest_segment_table(totals, videos, segment_count: int = 8, segment_duration: int = 60,
+                         skip_intro_outro: bool = False) -> dict:
+    """The ``segments`` of ``BatchSynchronizer.ingest`` for the videos ``videos`` (increasing) of probed durations
+    ``totals`` (seconds): MultiSegmentVideoSpeechTransformer._segment_starts with the reference's knobs, as
+    ``segment_table`` without seg_lo / seg_hi (a session's pushes supply the samples)."""
+    videos = np.ascontiguousarray(videos, dtype=np.int64)
+    pcm_off = np.zeros(int(videos.max()) + 2 if len(videos) else 1, dtype=np.int64)
+    t = segment_table(pcm_off, SAMPLE_RATE, videos, totals, segment_count, segment_duration, skip_intro_outro)
+    return {k: t[k] for k in ("seg_video", "seg_total", "seg_off", "seg_start")}
+
+
 def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, cue_off, cue_keep=None,
                max_decoders: int = 4, ffmpeg_path: Optional[str] = None, max_duration_seconds: Optional[float] = None,
-               ref_stream: Optional[str] = None, expect_samples=None, speech_video=None, want_all: bool = False):
+               ref_stream: Optional[str] = None, expect_samples=None, speech_video=None, want_all: bool = False,
+               multi_segment=False, segment_count: int = 8, segment_duration: int = 60,
+               skip_intro_outro: bool = False):
     """``ffs movie.mkv -i a.srt ...`` for a library: decodes paths[v] with up to ``max_decoders`` ffmpeg processes at
     a time (VideoSpeechTransformer._build_ffmpeg_args: ``-ss`` from the synchroniser's start_seconds, ``-t`` from
     max_duration_seconds, ffmpeg_path, ref_stream), reads each pipe in the reference's 100 s ``read()`` calls on a
     thread per decoder, pushes the chunks into one ingest session from this thread, and syncs the tracks as
-    ``IngestSession.sync_tracks`` does on the host.  No video's whole decode is ever held."""
+    ``IngestSession.sync_tracks`` does on the host.  No video's whole decode is ever held.
+    ``multi_segment`` (``--multi-segment-sync``): True for every video, or a list of video indices.  Such a video's
+    duration is probed with ffprobe (MultiSegmentVideoSpeechTransformer._probe_duration; a failure raises its
+    ValueError), and only its ``segment_count`` windows of ``segment_duration`` seconds (``_segment_starts``, with
+    ``skip_intro_outro``) are decoded, each by its own ``ffmpeg -ss start -t segment_duration`` in the same pool.  A
+    segment decoder that fails or cannot start is logged as the reference's "failed to extract segment" warning and
+    the segment is dropped; a failing full-audio decoder aborts, as without segments.  The synchroniser's
+    start_seconds applies to the subtitle tracks only there."""
     import queue
     import shutil
     import subprocess
     import threading
 
     from .constants import detector_chunk_bytes
-    from .speech_transformers import VideoSpeechTransformer
-    vst = VideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate, frame_rate=sync.frame_rate,
-                                 non_speech_label=sync.non_speech_label, start_seconds=sync.start_seconds,
-                                 ffmpeg_path=ffmpeg_path, ref_stream=ref_stream,
-                                 max_duration_seconds=max_duration_seconds)
-    args = [vst._build_ffmpeg_args(p) for p in paths]
-    if args and shutil.which(args[0][0]) is None:
-        raise ValueError("cannot decode media: no ffmpeg binary found at %r" % args[0][0])
+    from .speech_transformers import MultiSegmentVideoSpeechTransformer, VideoSpeechTransformer, logger
+    V = len(paths)
+    if multi_segment is True:
+        seg_videos = list(range(V))
+    elif multi_segment is False or multi_segment is None:
+        seg_videos = []
+    else:
+        seg_videos = sorted({int(v) for v in multi_segment})
+        if seg_videos and (seg_videos[0] < 0 or seg_videos[-1] >= V):
+            raise ValueError("multi_segment lists video indices in [0, %d), not %r" % (V, list(multi_segment)))
+    if seg_videos and max_duration_seconds is not None:
+        raise ValueError("max_duration_seconds limits a full decode; multi_segment decodes sampled segments of "
+                         "segment_duration seconds instead")
+
+    def ffmpeg_args(path, start_seconds, duration):
+        return VideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate, frame_rate=sync.frame_rate,
+                                      non_speech_label=sync.non_speech_label, start_seconds=start_seconds,
+                                      ffmpeg_path=ffmpeg_path, ref_stream=ref_stream,
+                                      max_duration_seconds=duration)._build_ffmpeg_args(path)
+
+    # the decoder jobs: (video, segment or None, ffmpeg arguments); a segment video has one job per segment
+    is_seg = set(seg_videos)
+    jobs = [(v, None, ffmpeg_args(paths[v], sync.start_seconds, max_duration_seconds)) for v in range(V)
+            if v not in is_seg]
+    segments = None
+    if seg_videos:
+        mst = MultiSegmentVideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate,
+                                                 frame_rate=sync.frame_rate, non_speech_label=sync.non_speech_label,
+                                                 segment_count=segment_count, segment_duration=segment_duration,
+                                                 skip_intro_outro=skip_intro_outro, ffmpeg_path=ffmpeg_path,
+                                                 ref_stream=ref_stream)
+        segments = ingest_segment_table([mst._probe_duration(paths[v]) for v in seg_videos], seg_videos,
+                                        segment_count, segment_duration, skip_intro_outro)
+        for i, v in enumerate(seg_videos):
+            for j in range(int(segments["seg_off"][i]), int(segments["seg_off"][i + 1])):
+                start = int(segments["seg_start"][j])
+                jobs.append((v, j - int(segments["seg_off"][i]), ffmpeg_args(paths[v], start, segment_duration)))
+        expect = np.zeros(V, dtype=np.int64) if expect_samples is None else np.array(expect_samples, dtype=np.int64)
+        expect[seg_videos] = int(round(segment_duration * sync.frame_rate))   # the hint of each segment
+        expect_samples = expect
+    if jobs and shutil.which(jobs[0][2][0]) is None:
+        raise ValueError("cannot decode media: no ffmpeg binary found at %r" % jobs[0][2][0])
     n_read = detector_chunk_bytes(sync.frame_rate, sync.sample_rate)
-    n_workers = max(1, min(int(max_decoders), len(paths)))
+    n_workers = max(1, min(int(max_decoders), len(jobs)))
     chunks: "queue.Queue" = queue.Queue(maxsize=2 * n_workers)
     todo: "queue.Queue" = queue.Queue()
-    for v in range(len(paths)):
-        todo.put(v)
+    for job in range(len(jobs)):
+        todo.put(job)
     stop = threading.Event()
 
-    def decode(v: int):
-        """Pushes video v's 100 s reads to `chunks`; returns why it failed (None: it did not)."""
-        proc = subprocess.Popen(args[v], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL)
+    def decode(job: int):
+        """Pushes job's 100 s reads to `chunks`; returns why it failed (None: it did not)."""
+        proc = subprocess.Popen(jobs[job][2], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL)
         try:
             while not stop.is_set():
                 data = proc.stdout.read(n_read)
                 if not data:
                     break
-                chunks.put((v, data, None))
+                chunks.put((job, data, None))
         finally:
             if stop.is_set():
                 proc.kill()
@@ -1125,31 +1205,39 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
         return "ffmpeg exited with status %d" % status if status and not stop.is_set() else None
 
     def worker() -> None:
-        # every video taken ends with exactly one (v, None, error) sentinel, whatever happens while decoding it
+        # every job taken ends with exactly one (job, None, error) sentinel, whatever happens while decoding it
         while not stop.is_set():
             try:
-                v = todo.get_nowait()
+                job = todo.get_nowait()
             except queue.Empty:
                 return
             try:
-                err = decode(v)
+                err = decode(job)
             except Exception as e:   # Popen or the pipe failed (missing binary, EMFILE, ...)
                 err = "%s: %s" % (type(e).__name__, e)
-            chunks.put((v, None, err))
+            chunks.put((job, None, err))
 
-    session = sync.ingest(len(paths), expect_samples)
+    session = sync.ingest(V, expect_samples, segments)
     threads = [threading.Thread(target=worker, daemon=True) for _ in range(n_workers)]
     for t in threads:
         t.start()
     try:
-        left = len(paths)
+        left = len(jobs)
         while left:
-            v, data, err = chunks.get()
+            job, data, err = chunks.get()
+            v, seg, _ = jobs[job]
             if data is not None:
-                session.push(v, data)
+                if seg is None:
+                    session.push(v, data)
+                else:
+                    session.push_segment(v, seg, data)
                 continue
             left -= 1
-            if err:
+            if err and seg is not None:   # one bad window must not sink the sync (speech_transformers.py:878-882)
+                start = int(segments["seg_start"][int(segments["seg_off"][seg_videos.index(v)]) + seg])
+                logger.warning("failed to extract segment at %ds: %s", start, err)
+                session.drop_segment(v, seg)
+            elif err:
                 raise RuntimeError("decoding %r failed: %s" % (paths[v], err))
     except BaseException:
         stop.set()

@@ -1050,19 +1050,33 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // detector launch reads only its segments' samples into the scratch (floats), and seg_ref_kernel writes its reference
 // from there, floats or bits, and resets and sets its speech flag.
 // With ingested references (b2_ingest_sync_tracks) the detector already ran as the PCM arrived: the step copies the
-// videos' references from the session's buffer to their ranges, one copy per run of videos stored back to back.
+// audio videos' references from the session's buffer to their ranges, one copy per run of videos stored back to back,
+// and seg_ref_kernel assembles the segment videos' ones from their segments' frames there.
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
                   bool ref_packed) {
+  // the segment videos [s0, s1) of p.seg_video lie in [v0, v1)
+  const int s0 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v0) - p.seg_video.begin());
+  const int s1 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v1) - p.seg_video.begin());
   if (r.ready.len) {
+    auto is_seg = [&](int v) { return !p.seg_of.empty() && p.seg_of[v] >= 0; };
     for (int v = v0; v < v1;) {
+      if (is_seg(v)) {
+        ++v;
+        continue;
+      }
       int w = v + 1;
-      while (w < v1 && r.ready.at[w] == r.ready.at[w - 1] + r.ready.len[w - 1]) ++w;
+      while (w < v1 && !is_seg(w) && r.ready.at[w] == r.ready.at[w - 1] + r.ready.len[w - 1]) ++w;
       const int64_t n = p.ref_off[w] - p.ref_off[v];
       if (n > 0)
         B2_CUDA(h, cudaMemcpyAsync(b.refsig + p.ref_off[v], r.ready.ref + r.ready.at[v], (size_t)n * 4,
                                    cudaMemcpyDeviceToDevice, h->stream));
       v = w;
     }
+    // segment videos: their sparse references from the segments' frames in the session's buffer (run_src points there)
+    if (s1 > s0)
+      B2_TRY(b2i_seg_ref_launch(h, r.ready.ref, p.ref_off.data(), p.seg_video.data() + s0, s1 - s0,
+                                p.run_first.data() + s0, p.run_lo.data(), p.run_src.data(), ref_packed, b.refsig,
+                                b.speech));
     return B2_OK;
   }
   const bool seg = !p.det_end.empty();
@@ -1099,8 +1113,6 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
   if (!sig.empty())
     B2_TRY(b2i_sig_ref_launch(h, b.sigx, r.sig.off, p.ref_off.data(), r.V, sig.data(), (int)sig.size(), p.label,
                               ref_packed, b.refsig, b.first_bad));
-  const int s0 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v0) - p.seg_video.begin());
-  const int s1 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v1) - p.seg_video.begin());
   if (s1 > s0) {
     const int k0 = p.item_first[v0], nk = p.item_first[v1] - k0;
     if (nk > 0 && !p.auditok) {
@@ -1334,7 +1346,7 @@ static int sync_run(b2_ctx* h, bool fence_was_valid, const SyncRequest& r) {
   b.pcm = r.pcm;
   if (memspace == B2_HOST) {   // a call without audio samples reads no PCM (b2_sync_tracks_subs may pass none)
     void* dp = nullptr;
-    if (T == 0) {   // serialize-only: the samples the listed videos' detector step reads, at their own positions
+    if (T == 0 && !r.ready.len) {   // serialize-only: the samples the listed videos' detector step reads
       std::vector<std::pair<int64_t, int64_t>> rg;
       for (int v : sout.videos) {
         if (any_seg && p.seg_of[v] >= 0) {
@@ -1683,9 +1695,10 @@ extern "C" int b2_sync_tracks_seg(b2_handle h, const int16_t* pcm, const int64_t
 // The reference's chunk loop (speech_transformers.py:680-753) for V videos at once: each push is cut by the span
 // planner (ingest_plan.h), its spans staged in a ring slot of pinned host and device memory, copied to the device
 // and run through the detector in one b2i_vad_launch over a table of (staging offset, samples, destination frame);
-// for auditok the tokenizer then runs over every detector call the push completed.  Only the references stay on
-// the device, video v's at frames [at[v], at[v] + cap[v]) of one buffer; b2_ingest_sync_tracks hands them to the
-// batched sync calls' chain as ingested references (SyncRequest::ready).
+// for auditok the tokenizer then runs over every detector call the push completed.  Only the detector's output stays
+// on the device, stream k's (an audio video's, or a sampled segment's: IngestStreams) at frames [at[k], at[k] + cap[k])
+// of one buffer; b2_ingest_sync_tracks hands them to the batched sync calls' chain as ingested references
+// (SyncRequest::ready), the segments' ones to be assembled into their videos' sparse references there.
 struct IngestSession {
   static const int kSlots = 3;
   struct Slot {
@@ -1699,10 +1712,13 @@ struct IngestSession {
   bool active = false;
   SyncRequest req{};                  // the detector arguments, as the sync call passes them
   SyncPlan det;                       // fpw, z_lo, z_hi, auditok_e_min, tok of those arguments
-  IngestPlanner plan;
-  std::vector<std::vector<uint8_t>> held;   // video v's stream bytes [2 * plan.base[v], plan.bytes[v])
+  int V = 0;
+  IngestStreams streams;              // which stream each push feeds
+  IngestPlanner plan;                 // per stream
+  std::vector<std::vector<uint8_t>> held;   // stream k's bytes [2 * plan.base[k], plan.bytes[k])
+  std::vector<int64_t> hint;          // [V] frames expected per stream of video v (expect_samples), 0: none
   float* ref = nullptr;               // cudaMallocAsync on the handle's stream
-  std::vector<int64_t> at, cap;
+  std::vector<int64_t> at, cap;       // per stream
 };
 
 static void ingest_release_ref(b2_ctx* h, IngestSession* s) {
@@ -1726,24 +1742,16 @@ static void ingest_free(b2_ctx* h) {
   h->ingest = nullptr;
 }
 
-// Room for frames [at[v], at[v] + need[v]) of every video.  On overflow every region grows to at least twice what its
-// video needs and to what the longest video needs (videos decoded side by side grow alike), the written frames are
-// copied over on the stream, and the old buffer is freed behind them.
-static int ingest_reserve(b2_ctx* h, IngestSession* s, const std::vector<int64_t>& need) {
-  const int V = (int)need.size();
-  bool grow = false;
-  int64_t longest = 0;
-  for (int v = 0; v < V; ++v) {
-    grow = grow || need[v] > s->cap[v];
-    longest = std::max(longest, need[v]);
-  }
-  if (!grow) return B2_OK;
-  std::vector<int64_t> at(V), cap(V);
+// The streams' regions become cap[k] frames each, back to back in a new buffer: the frames written so far (at most
+// written[k]) are copied over on the stream, and the old buffer is freed behind them.
+static int ingest_relayout(b2_ctx* h, IngestSession* s, const std::vector<int64_t>& cap,
+                           const std::vector<int64_t>& written) {
+  const int n = (int)cap.size();
+  std::vector<int64_t> at(n);
   int64_t total = 0;
-  for (int v = 0; v < V; ++v) {
-    cap[v] = std::max(s->cap[v], std::max(2 * need[v], longest));
-    at[v] = total;
-    total += cap[v];
+  for (int k = 0; k < n; ++k) {
+    at[k] = total;
+    total += cap[k];
   }
   float* ref = nullptr;
   const cudaError_t e = cudaMallocAsync((void**)&ref, (size_t)total * 4 + 16, h->stream);
@@ -1752,16 +1760,35 @@ static int ingest_reserve(b2_ctx* h, IngestSession* s, const std::vector<int64_t
     B2_FAIL(h, B2_ERR_NOMEM, "ingest: cudaMallocAsync(%lld frames) for the references failed: %s", (long long)total,
             cudaGetErrorString(e));
   }
-  for (int v = 0; v < V; ++v) {   // every frame written so far lies in the old region
-    const int64_t m = std::min(s->cap[v], need[v]);
+  for (int k = 0; k < n; ++k) {   // every frame written so far lies in the old region
+    const int64_t m = k < (int)s->cap.size() ? std::min(std::min(s->cap[k], written[k]), cap[k]) : 0;
     if (m > 0)
-      B2_CUDA(h, cudaMemcpyAsync(ref + at[v], s->ref + s->at[v], (size_t)m * 4, cudaMemcpyDeviceToDevice, h->stream));
+      B2_CUDA(h, cudaMemcpyAsync(ref + at[k], s->ref + s->at[k], (size_t)m * 4, cudaMemcpyDeviceToDevice, h->stream));
   }
   if (s->ref) B2_CUDA(h, cudaFreeAsync(s->ref, h->stream));
   s->ref = ref;
   s->at.swap(at);
-  s->cap.swap(cap);
+  s->cap = cap;
   return B2_OK;
+}
+
+// Room for frames [at[k], at[k] + need[k]) of every stream.  On overflow every live region grows to at least twice
+// what its stream needs and to what the longest stream of its kind needs (videos decoded side by side grow alike, and
+// so do their segments; a segment never grows to a whole video's length because a video did).  Streams that take no
+// pushes (a segment video's own, a dropped segment's) keep their regions.
+static int ingest_reserve(b2_ctx* h, IngestSession* s, const std::vector<int64_t>& need) {
+  const int n = (int)need.size();
+  bool grow = false;
+  int64_t longest[2] = {0, 0};
+  for (int k = 0; k < n; ++k) {
+    grow = grow || need[k] > s->cap[k];
+    longest[k >= s->V] = std::max(longest[k >= s->V], need[k]);
+  }
+  if (!grow) return B2_OK;
+  std::vector<int64_t> cap(n);
+  for (int k = 0; k < n; ++k)
+    cap[k] = s->streams.live(k) ? std::max(s->cap[k], std::max(2 * need[k], longest[k >= s->V])) : s->cap[k];
+  return ingest_relayout(h, s, cap, need);
 }
 
 // Appends the bytes [b0, b1) of the concatenation a ++ b (lengths na, nb) to dst
@@ -1775,18 +1802,18 @@ static void concat_bytes(uint8_t* dst, const uint8_t* a, int64_t na, const uint8
   if (b1 > b0) memcpy(dst, b + (b0 - na), (size_t)(b1 - b0));
 }
 
-// Videos' streams grew by the chunks (video[i], bytes[i], n_bytes[i]) (n = 0 and final: every video's end): plans the
+// Streams grew by the chunks (stream[i], bytes[i], n_bytes[i]) (n = 0 and final: every live stream's end): plans the
 // spans, stages them in the next ring slot, and enqueues the copy, the detector launch and the tokenizer launch.
 static int ingest_enqueue(b2_ctx* h, IngestSession* s, int n, const int32_t* video, const void* const* bytes,
                           const int64_t* n_bytes, bool final) {
   IngestPlanner& pl = s->plan;
-  const int V = (int)pl.bytes.size(), fpw = pl.fpw;
+  const int NS = (int)pl.bytes.size(), fpw = pl.fpw;
   // staging bound: every chunk with a held-back window and an odd byte in front, 16 bytes of alignment per span
   size_t bound = 0;
   auto spans_bound = [&](int64_t nb) { return 2 + (pl.chunk > 0 ? (nb / 2 + fpw) / pl.chunk : 0); };
   for (int i = 0; i < n; ++i) bound += (size_t)n_bytes[i] + 2 * fpw + 2 + 16 * spans_bound(n_bytes[i] + 2 * fpw);
   if (final)
-    for (int v = 0; v < V; ++v) bound += s->held[v].size() + 16 * 2;
+    for (int k = 0; k < NS; ++k) bound += s->held[k].size() + 16 * 2;
   IngestSession::Slot& sl = s->slot[s->seq % IngestSession::kSlots];
   if (sl.busy) B2_CUDA(h, cudaEventSynchronize(sl.ev));   // the push kSlots ago has read this slot
   sl.busy = false;
@@ -1829,7 +1856,8 @@ static int ingest_enqueue(b2_ctx* h, IngestSession* s, int n, const int32_t* vid
     add(v, (const uint8_t*)bytes[i], n_bytes[i], base0, from);
   }
   if (final)
-    for (int v = 0; v < V; ++v) {
+    for (int v = 0; v < NS; ++v) {
+      if (!s->streams.live(v)) continue;   // a segment video's own stream, a dropped segment
       const int64_t base0 = pl.base[v];
       const size_t from = spans.size();
       pl.finish(v, &spans, &chunks);
@@ -1912,12 +1940,15 @@ extern "C" int b2_ingest_begin(b2_handle h, int V, int frame_rate, int sample_ra
   IngestSession* s = h->ingest;
   s->req = r;
   s->det = det;
+  s->V = V;
+  s->streams.begin(V);
   s->plan.begin(V, det.fpw, det.auditok, chunk_samples, energy_threshold_db);
   s->held.assign(V, {});
   s->at.assign(V, 0);
   s->cap.assign(V, 0);
   std::vector<int64_t> need(V, 0);
   for (int v = 0; expect_samples && v < V; ++v) need[v] = s->plan.length(expect_samples[v]);
+  s->hint = need;
   // sized to the hint exactly (regions back to back: the sync step then copies them in one piece)
   int64_t total = 0;
   for (int v = 0; v < V; ++v) {
@@ -1938,27 +1969,80 @@ extern "C" int b2_ingest_begin(b2_handle h, int V, int frame_rate, int sample_ra
   return B2_OK;
 }
 
-extern "C" int b2_ingest_push(b2_handle h, int n, const int32_t* video, const void* const* bytes,
-                              const int64_t* n_bytes) {
-  B2_ENTER(h);
+// Routes chunk i to its stream: video[i]'s own, or with `segmented` its segment segment[i].  A refused chunk refuses
+// the whole call before anything is pushed.  The chunks' videos then count as pushed to.
+static int ingest_push_any(b2_ctx* h, const char* who, int n, const int32_t* video, bool segmented,
+                           const int64_t* segment, const void* const* bytes, const int64_t* n_bytes) {
   IngestSession* s = h->ingest;
-  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: no open session on this handle");
-  if (n < 0 || (n > 0 && (!video || !bytes || !n_bytes)))
-    B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: bad chunk table (n = %d)", n);
-  const int V = (int)s->held.size();
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: no open session on this handle", who);
+  if (n < 0 || (n > 0 && (!video || !bytes || !n_bytes || (segmented && !segment))))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: bad chunk table (n = %d)", who, n);
+  std::vector<int32_t> stream(n);
   for (int i = 0; i < n; ++i) {
-    if (video[i] < 0 || video[i] >= V)
-      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: video %d is out of [0, %d)", i, (int)video[i], V);
+    const int k = s->streams.route(who, i, video[i], segmented, segmented ? segment[i] : 0);
+    if (k < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s", s->streams.err.c_str());
+    stream[i] = k;
     if (n_bytes[i] < 0)
-      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: n_bytes = %lld < 0", i, (long long)n_bytes[i]);
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: chunk %d: n_bytes = %lld < 0", who, i, (long long)n_bytes[i]);
     if (n_bytes[i] > 0 && !bytes[i])
-      B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_push: chunk %d: null bytes with n_bytes = %lld", i, (long long)n_bytes[i]);
+      B2_FAIL(h, B2_ERR_BAD_ARG, "%s: chunk %d: null bytes with n_bytes = %lld", who, i, (long long)n_bytes[i]);
   }
-  B2Range range("b2_ingest_push");
-  if (const int st = ingest_enqueue(h, s, n, video, bytes, n_bytes, false)) {
+  for (int i = 0; i < n; ++i) s->streams.touched[video[i]] = 1;
+  if (const int st = ingest_enqueue(h, s, n, stream.data(), bytes, n_bytes, false)) {
     ingest_release_ref(h, s);   // the planner ran ahead of what reached the device: the session cannot go on
     return st;
   }
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_push(b2_handle h, int n, const int32_t* video, const void* const* bytes,
+                              const int64_t* n_bytes) {
+  B2_ENTER(h);
+  B2Range range("b2_ingest_push");
+  return ingest_push_any(h, "ingest_push", n, video, false, nullptr, bytes, n_bytes);
+}
+
+extern "C" int b2_ingest_push_segments(b2_handle h, int n, const int32_t* video, const int64_t* segment,
+                                       const void* const* bytes, const int64_t* n_bytes) {
+  B2_ENTER(h);
+  B2Range range("b2_ingest_push_segments");
+  return ingest_push_any(h, "ingest_push_segments", n, video, true, segment, bytes, n_bytes);
+}
+
+extern "C" int b2_ingest_segments(b2_handle h, int P, const int32_t* seg_video, const double* seg_total,
+                                  const int64_t* seg_off, const int64_t* seg_start) {
+  B2_ENTER(h);
+  IngestSession* s = h->ingest;
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_segments: no open session on this handle");
+  if (const int st = s->streams.declare(s->req, P, seg_video, seg_total, seg_off, seg_start))
+    B2_FAIL(h, st, "%s", s->streams.err.c_str());
+  // one stream per segment, its region sized from its video's hint; a segment video's own region is released
+  const int V = s->V, NS = s->streams.streams();
+  s->plan.add_streams(NS - V);
+  s->held.resize(NS);
+  std::vector<int64_t> cap(s->cap), written(s->plan.frames);
+  cap.resize(NS, 0);
+  for (int i = 0; i < P; ++i) {
+    const int v = seg_video[i];
+    cap[v] = 0;
+    for (int64_t k = V + s->streams.first[i]; k < V + s->streams.first[i + 1]; ++k) cap[k] = s->hint[v];
+  }
+  if (const int st = ingest_relayout(h, s, cap, written)) {
+    ingest_release_ref(h, s);
+    return st;
+  }
+  return B2_OK;
+}
+
+extern "C" int b2_ingest_drop_segment(b2_handle h, int video, int64_t segment) {
+  B2_ENTER(h);
+  IngestSession* s = h->ingest;
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_drop_segment: no open session on this handle");
+  const int k = s->streams.segment("ingest_drop_segment", -1, video, segment);
+  if (k < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "%s", s->streams.err.c_str());
+  s->streams.dropped[k - s->V] = 1;   // its frames stay where they are; the sync reads none of them
+  s->held[k].clear();
+  s->held[k].shrink_to_fit();
   return B2_OK;
 }
 
@@ -1966,8 +2050,8 @@ extern "C" int b2_ingest_windows(b2_handle h, int64_t* windows) {
   B2_ENTER(h);
   IngestSession* s = h->ingest;
   if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_windows: no open session on this handle");
-  if (!windows && !s->held.empty()) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_windows: null windows");
-  for (size_t v = 0; v < s->held.size(); ++v) windows[v] = s->plan.frames[v];
+  if (!windows && s->V > 0) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_windows: null windows");
+  for (int v = 0; v < s->V; ++v) windows[v] = s->streams.windows(s->plan, v);
   return B2_OK;
 }
 
@@ -1997,8 +2081,23 @@ extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, in
   if (memspace != B2_HOST && memspace != B2_DEVICE)
     B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: memspace must be B2_HOST or B2_DEVICE");
   B2_TRY(ingest_enqueue(h, s, 0, nullptr, nullptr, nullptr, true));
-  const int V = (int)s->held.size();
+  const int V = s->V;
   std::vector<int64_t> pcm_off(V + 1, 0);
+  // the live segments' table: b2_sync_tracks_seg's, its sample ranges empty (the detector's output is on the
+  // device), each segment's frames in the session's buffer
+  const IngestStreams& ss = s->streams;
+  const int P = (int)ss.video.size();
+  std::vector<int64_t> seg_off(1, 0), seg_start, seg_at, seg_len;
+  for (int i = 0; i < P; ++i) {
+    for (int64_t j = ss.first[i]; j < ss.first[i + 1]; ++j)
+      if (!ss.dropped[j]) {
+        seg_start.push_back(ss.start[j]);
+        seg_at.push_back(s->at[V + j]);
+        seg_len.push_back(s->plan.frames[V + j]);
+      }
+    seg_off.push_back((int64_t)seg_start.size());
+  }
+  const std::vector<int64_t> no_range(seg_start.size() + 1, 0);
   SyncRequest r = s->req;
   r.who = gss_ratio ? "ingest_sync_tracks (search)" : "ingest_sync_tracks";
   r.pcm = nullptr;
@@ -2023,7 +2122,9 @@ extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, in
   r.gss_ratio = gss_ratio;
   r.gss_evals = gss_evals;
   r.memspace = memspace;
-  r.ready = {s->ref, s->at.data(), s->plan.frames.data()};
+  r.ready = {s->ref, s->at.data(), s->plan.frames.data(), seg_at.data(), seg_len.data()};
+  if (ss.declared)
+    r.seg = {P, ss.video.data(), ss.total.data(), seg_off.data(), seg_start.data(), no_range.data(), no_range.data()};
   return sync_run(h, _b2_fence_was_valid, r);
 }
 

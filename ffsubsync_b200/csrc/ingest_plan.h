@@ -1,14 +1,16 @@
-// Host-side span planner of the batched ingest session (b2_ingest_*, DESIGN.md section 4 "K1i").  Video v's PCM
-// arrives as pushes of any byte count; the planner cuts its stream into spans the detector can run on as they come:
+// Host-side span planner of the batched ingest session (b2_ingest_*, DESIGN.md section 4 "K1i").  A stream's PCM (an
+// audio video's, or one sampled segment's; IngestStreams below numbers them, and the planner's `video` index is that
+// stream number) arrives as pushes of any byte count; the planner cuts it into spans the detector can run on as they come:
 // every span starts on a window boundary and ends on one, or at the end of a detector call (auditok's chunk of
 // chunk_samples), so the windows of a span are exactly the windows the one-shot detector has over the same samples.
-// The samples of an unfinished window (and an odd trailing byte) are held back until the next push of that video or
+// The samples of an unfinished window (and an odd trailing byte) are held back until the next push of that stream or
 // until finish().  No CUDA call happens here, so tests/host_emul/ingest_emul.cu runs the same code on the CPU.
 #pragma once
 
 #include <stdint.h>
 
 #include <algorithm>
+#include <string>
 #include <vector>
 
 #include "sync_plan.h"   // auditok_energy_floor
@@ -47,6 +49,14 @@ struct IngestPlanner {
     base.assign(V, 0);
     frames.assign(V, 0);
     done.assign(V, 0);
+  }
+
+  // n more streams, empty, numbered after the existing ones
+  void add_streams(int n) {
+    bytes.resize(bytes.size() + n, 0);
+    base.resize(base.size() + n, 0);
+    frames.resize(frames.size() + n, 0);
+    done.resize(done.size() + n, 0);
   }
 
   // frames of one detector call of n samples, and the calls' geometry
@@ -97,4 +107,128 @@ struct IngestPlanner {
     const int64_t k0 = chunk > 0 ? n / chunk * per_chunk() : 0;   // the call in progress (chunk: empty when n ends one)
     if (frames[v] > k0) chunks->push_back(IngestChunk{v, k0, frames[v]});
   }
+};
+
+// The streams of a session and where each push goes.  Stream v < V is video v's own; b2_ingest_segments gives each
+// sampled segment a stream of its own: segment j (counted within its video) of the i-th segment video is stream
+// V + first[i] + j, so that energy / ZCR restarts its windows and auditok its chunk loop at each segment's first
+// sample, as the whole-call segment path's detector items do.  A segment video's own stream takes no pushes, an audio
+// video has no segment streams, and a dropped segment's stream takes none from the drop on.  The refusals leave
+// everything as it was.
+struct IngestStreams {
+  std::string err;
+  int V = 0;
+  bool declared = false;
+  std::vector<uint8_t> touched;   // [V]: a push named video v
+  std::vector<int> seg_of;        // [V]: v's index among the segment videos, -1: an audio video
+  std::vector<int32_t> video;     // [P] the segment videos, increasing
+  std::vector<double> total;      // [P] their probed durations (seconds)
+  std::vector<int64_t> first;     // [P+1] their segments
+  std::vector<int64_t> start;     // per segment: its whole-second start
+  std::vector<uint8_t> dropped;   // per segment
+
+  void begin(int V_) {
+    V = V_;
+    declared = false;
+    touched.assign(V, 0);
+    seg_of.assign(V, -1);
+    video.clear();
+    total.clear();
+    first.assign(1, 0);
+    start.clear();
+    dropped.clear();
+  }
+
+  int streams() const { return V + (int)start.size(); }
+  // the stream takes pushes (an audio video, or a segment not dropped)
+  bool live(int k) const { return k < V ? seg_of[k] < 0 : !dropped[k - V]; }
+
+  // b2_ingest_segments: the table's checks are b2_sync_tracks_seg's (plan_seg_check on `det`, the session's detector
+  // arguments, with empty PCM ranges and empty sample ranges), then those of the session.
+  int declare(const SyncRequest& det, int P, const int32_t* vid, const double* tot, const int64_t* off,
+              const int64_t* st) {
+    const char* who = "ingest_segments";
+    if (declared) B2_FAIL(this, B2_ERR_BAD_ARG, "%s: the session's segments are already declared", who);
+    if (P < 0 || (P > 0 && (!vid || !tot || !off))) B2_FAIL(this, B2_ERR_BAD_ARG, "%s: bad segment videos (%d)", who, P);
+    const int64_t S = P > 0 ? off[P] - off[0] : 0;
+    std::vector<int64_t> pcm_off(V + 1, 0), no_range(S > 0 ? S : 1, 0);
+    SyncRequest r = det;
+    r.who = who;
+    r.V = V;
+    r.pcm_off = pcm_off.data();
+    const int64_t* st_rel = P > 0 && st ? st + off[0] : st;
+    r.seg = {P, vid, tot, off, P > 0 && st ? st : nullptr, no_range.data() - (P > 0 ? off[0] : 0),
+             no_range.data() - (P > 0 ? off[0] : 0)};
+    SyncPlan p;
+    if (const int e = plan_seg_check(r, &p)) {
+      err = p.err;
+      return e;
+    }
+    for (int i = 0; i < P; ++i)
+      if (touched[vid[i]])
+        B2_FAIL(this, B2_ERR_BAD_ARG, "%s: video %d already has pushes; declare its segments before its first push",
+                who, (int)vid[i]);
+    declared = true;
+    for (int i = 0; i < P; ++i) {
+      seg_of[vid[i]] = i;
+      video.push_back(vid[i]);
+      total.push_back(tot[i]);
+      first.push_back(off[i + 1] - off[0]);
+    }
+    start.assign(st_rel, st_rel + S);
+    dropped.assign(S, 0);
+    return B2_OK;
+  }
+
+  // The frames video v's stream fixed so far, or for a segment video its live segments' streams together
+  int64_t windows(const IngestPlanner& pl, int v) const {
+    int64_t n = pl.frames[v];
+    const int q = seg_of[v];
+    for (int64_t j = q < 0 ? 0 : first[q]; q >= 0 && j < first[q + 1]; ++j)
+      if (!dropped[j]) n += pl.frames[V + j];
+    return n;
+  }
+
+  // The stream of chunk i: video v's own (b2_ingest_push), or with `segmented` its segment seg
+  // (b2_ingest_push_segments); -1 with err set when the chunk is refused.
+  int route(const char* who, int i, int v, bool segmented, int64_t seg) {
+    if (segmented) return segment(who, i, v, seg);
+    if (v < 0 || v >= V) {
+      snprintf(buf_, sizeof(buf_), "%s: chunk %d: video %d is out of [0, %d)", who, i, v, V);
+    } else if (seg_of[v] >= 0) {
+      snprintf(buf_, sizeof(buf_), "%s: chunk %d: video %d has sampled segments; push them with "
+               "b2_ingest_push_segments", who, i, v);
+    } else {
+      return v;
+    }
+    err = buf_;
+    return -1;
+  }
+
+  // The stream of segment seg of video v (i >= 0: names chunk i; b2_ingest_drop_segment passes -1), -1 with err set
+  int segment(const char* who, int i, int v, int64_t seg) {
+    char at[32] = "";
+    if (i >= 0) snprintf(at, sizeof(at), " chunk %d:", i);
+    if (v < 0 || v >= V) {
+      snprintf(buf_, sizeof(buf_), "%s:%s video %d is out of [0, %d)", who, at, v, V);
+    } else if (seg_of[v] < 0) {
+      snprintf(buf_, sizeof(buf_), "%s:%s video %d has no sampled segments", who, at, v);
+    } else {
+      const int q = seg_of[v];
+      const int64_t n = first[q + 1] - first[q];
+      if (seg < 0 || seg >= n) {
+        snprintf(buf_, sizeof(buf_), "%s:%s segment %lld of video %d is out of [0, %lld)", who, at, (long long)seg, v,
+                 (long long)n);
+      } else if (i >= 0 && dropped[first[q] + seg]) {
+        snprintf(buf_, sizeof(buf_), "%s:%s segment %lld of video %d was dropped", who, at, (long long)seg, v);
+      } else {
+        return V + (int)(first[q] + seg);
+      }
+    }
+    err = buf_;
+    return -1;
+  }
+
+ private:
+  char buf_[256];
 };

@@ -404,10 +404,15 @@ struct SyncRequest {
   // ref + at[v] (at, len: host arrays [V]).  The call has no PCM (pcm_off all equal); its detector step copies the
   // references into the reference buffer, and the videos count as detector videos for every level and path rule.
   // The value-initialised state is "no ingested references", so the other entry points leave it out.
+  // With sampled segments (seg.off set; their sample ranges lo / hi all empty) a segment video's reference is
+  // assembled from its segments' detector output, segment j's seg_len[j] frames at ref + seg_at[j] (indexed as
+  // seg.start), and its own len is not read.
   struct {
     const float* ref;
     const int64_t* at;
     const int64_t* len;
+    const int64_t* seg_at;
+    const int64_t* seg_len;
   } ready;
 };
 
@@ -560,8 +565,9 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // signal videos (their chains take the run path only at label 0, where the reference has the levels 1.0 and 0.0).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
-  // ingested references are floats; the run path packs them itself (ref_bits_kernel)
-  if (r.ready.len || (p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
+  // ingested audio references are floats; the run path packs them itself (ref_bits_kernel).  Segment videos' ones
+  // are assembled at sync by seg_ref_kernel, which writes bits as it does for b2_sync_tracks_seg.
+  if ((r.ready.len && p->seg_video.size() < (size_t)r.V) || (p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
       (env.ref_packed && atoi(env.ref_packed) == 0))
     return;
   // how many videos of `list` lie in [v0, v1)
@@ -725,6 +731,49 @@ static int plan_seg_check(const SyncRequest& r, SyncPlan* p) {
   return B2_OK;
 }
 
+// The owned-frame runs of every segment video (SyncPlan run_*): segment j's detector output is len[j] frames from
+// src[j] on (indexed as r.seg.start); a sweep in start order, each segment overwriting [begin, min(begin + len, L))
+// of the runs so far.
+static void plan_seg_runs(const SyncRequest& r, SyncPlan* p, const int64_t* src, const int64_t* len) {
+  const auto& s = r.seg;
+  p->run_first.assign(1, 0);
+  p->run_lo.clear();
+  p->run_src.clear();
+  for (int v : p->seg_video) {
+    const int i = p->seg_of[v];
+    const int64_t L = p->ref_off[v + 1] - p->ref_off[v];
+    struct Piece { int64_t lo, hi, src; };
+    std::vector<Piece> owned, next;
+    for (int64_t j = s.off[i]; j < s.off[i + 1]; ++j) {
+      const int64_t b = s.start[j] * (int64_t)r.sample_rate, e = std::min(b + len[j], L);
+      if (e <= b) continue;
+      next.clear();
+      for (const Piece& q : owned) {
+        if (q.lo < b) next.push_back({q.lo, std::min(q.hi, b), q.src});
+        if (q.hi > e) next.push_back({std::max(q.lo, e), q.hi, q.src + (std::max(q.lo, e) - q.lo)});
+      }
+      next.push_back({b, e, src[j]});
+      std::sort(next.begin(), next.end(), [](const Piece& x, const Piece& y) { return x.lo < y.lo; });
+      owned.swap(next);
+    }
+    int64_t at = 0;
+    for (const Piece& q : owned) {
+      if (q.lo > at) {
+        p->run_lo.push_back(at);
+        p->run_src.push_back(-1);
+      }
+      p->run_lo.push_back(q.lo);
+      p->run_src.push_back(q.src);
+      at = q.hi;
+    }
+    if (at < L) {
+      p->run_lo.push_back(at);
+      p->run_src.push_back(-1);
+    }
+    p->run_first.push_back((int)p->run_lo.size());
+  }
+}
+
 // The segment videos' tables (SyncPlan: det_end, item_*, run_*, stage_*), after ref_off and the chunk table.
 static void plan_segments(const SyncRequest& r, SyncPlan* p) {
   const auto& s = r.seg;
@@ -771,43 +820,7 @@ static void plan_segments(const SyncRequest& r, SyncPlan* p) {
   }
   p->item_start.push_back(p->item_start.empty() ? 0 : p->item_start.back());
   p->seg_frames = p->item_out.back();
-  // owned frames: a sweep in start order, each segment overwriting [begin, min(begin + len, L)) of the runs so far
-  p->run_first.assign(1, 0);
-  p->run_lo.clear();
-  p->run_src.clear();
-  for (int v : p->seg_video) {
-    const int i = p->seg_of[v];
-    const int64_t L = p->ref_off[v + 1] - p->ref_off[v];
-    struct Piece { int64_t lo, hi, src; };
-    std::vector<Piece> owned, next;
-    for (int64_t j = s.off[i]; j < s.off[i + 1]; ++j) {
-      const int64_t b = s.start[j] * (int64_t)r.sample_rate, e = std::min(b + seg_len[j - s.off[0]], L);
-      if (e <= b) continue;
-      next.clear();
-      for (const Piece& q : owned) {
-        if (q.lo < b) next.push_back({q.lo, std::min(q.hi, b), q.src});
-        if (q.hi > e) next.push_back({std::max(q.lo, e), q.hi, q.src + (std::max(q.lo, e) - q.lo)});
-      }
-      next.push_back({b, e, seg_scr[j - s.off[0]]});
-      std::sort(next.begin(), next.end(), [](const Piece& x, const Piece& y) { return x.lo < y.lo; });
-      owned.swap(next);
-    }
-    int64_t at = 0;
-    for (const Piece& q : owned) {
-      if (q.lo > at) {
-        p->run_lo.push_back(at);
-        p->run_src.push_back(-1);
-      }
-      p->run_lo.push_back(q.lo);
-      p->run_src.push_back(q.src);
-      at = q.hi;
-    }
-    if (at < L) {
-      p->run_lo.push_back(at);
-      p->run_src.push_back(-1);
-    }
-    p->run_first.push_back((int)p->run_lo.size());
-  }
+  plan_seg_runs(r, p, seg_scr.data() - (s.n > 0 ? s.off[0] : 0), seg_len.data() - (s.n > 0 ? s.off[0] : 0));
   // B2_HOST: the ranges the detector reads, merged
   std::vector<std::pair<int64_t, int64_t>> rg;
   for (int v = 0; v < V; ++v)
@@ -849,7 +862,12 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
   p->z_hi = r.energy.z_hi < 0 ? (3 * fpw) / 8 : r.energy.z_hi;
   p->ref_off.assign(V + 1, 0);
   if (r.ready.len) {   // ingested references: their lengths are the pushes' (no chunk table, nothing to detect)
-    for (int v = 0; v < V; ++v) p->ref_off[v + 1] = p->ref_off[v] + r.ready.len[v];
+    for (int v = 0; v < V; ++v)
+      p->ref_off[v + 1] = p->ref_off[v] + (!p->seg_of.empty() && p->seg_of[v] >= 0
+                                               ? seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate)
+                                               : r.ready.len[v]);
+    // segment videos: their runs point into the session's buffer, not into a scratch of this call
+    if (!p->seg_video.empty()) plan_seg_runs(r, p, r.ready.seg_at, r.ready.seg_len);
     return B2_OK;
   }
   // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length

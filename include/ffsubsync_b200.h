@@ -628,6 +628,34 @@ int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video /* [T] */, int
                           int memspace);
 int b2_ingest_abort(b2_handle h);
 
+/* ---- sampled segments in a session (--multi-segment-sync) ------------------------------------------------------
+ * MultiSegmentVideoSpeechTransformer.fit decodes only a few windows of each video (ffmpeg -ss start -t duration per
+ * segment, ffsubsync/speech_transformers.py:849-900) and skips a segment whose decode fails.  A session does that for
+ * segment videos next to audio videos: each segment's PCM is pushed on its own, the detector runs on it as it arrives
+ * (energy / ZCR restarts its windows and auditok its chunk loop at the segment's first sample), and the sync assembles
+ * the sparse reference on the device.  Let S_{v,j} be all bytes pushed to live (not dropped) segment j of video v,
+ * trailing odd byte dropped.  The sync call returns exactly what b2_sync_tracks_seg returns for the same tracks and
+ * arguments over the PCM of each audio video's pushes and each segment video's live S_{v,j} back to back in segment
+ * order, with the segment table seg_lo / seg_hi over those pieces and the dropped segments removed - b2_speech_output,
+ * B2_BEST_K_NO_SPEECH (a video whose segments were all dropped or never pushed included) and the label-0 rule of the
+ * search included.
+ * b2_ingest_segments      declares the segment videos: seg_video [P] (increasing), seg_total [P] (probed duration,
+ *                         seconds), seg_off [P+1], seg_start (whole seconds, increasing per video); the checks are
+ *                         b2_sync_tracks_seg's.  At most once per session, before any push to a listed video.
+ *                         b2_ingest_begin's expect_samples[v] of a segment video is the hint for each of its segments.
+ * b2_ingest_push_segments appends chunk i to segment segment[i] (counted within its video) of video video[i]; copies
+ *                         and enqueues as b2_ingest_push.  Segments and videos may interleave in any order.
+ *                         B2_ERR_BAD_ARG (the message names the chunk; nothing is pushed) for a video without segments,
+ *                         a segment out of range or a dropped segment; b2_ingest_push refuses a segment video.
+ * b2_ingest_drop_segment  discards a segment (what was pushed to it and any later push, refused): it takes no part in
+ *                         the reference and overwrites no earlier segment (the reference's "failed to extract segment").
+ * b2_ingest_windows gives a segment video the frames its live segments have fixed so far. */
+int b2_ingest_segments(b2_handle h, int P, const int32_t* seg_video /* [P] */, const double* seg_total /* [P] */,
+                       const int64_t* seg_off /* [P+1] */, const int64_t* seg_start);
+int b2_ingest_push_segments(b2_handle h, int n, const int32_t* video /* [n] */, const int64_t* segment /* [n] */,
+                            const void* const* bytes /* [n] */, const int64_t* n_bytes /* [n] */);
+int b2_ingest_drop_segment(b2_handle h, int video, int64_t segment);
+
 /* ---- synthetic PCM (bench / tests): counter-hash generator replayable in numpy -------------
  * oracle/vad_oracle.py:synth_pcm.  window_class: uint8 per 10 ms window (0 silence, 1 voiced,
  * 2 loud hiss), device or host per memspace; writes n_windows*fpw int16 samples. */
