@@ -24,9 +24,9 @@ STATUS_NAMES = {0: "B2_OK", -1: "B2_ERR_BAD_ARG", -2: "B2_ERR_CUDA", -3: "B2_ERR
 # every symbol declared in include/ffsubsync_b200.h (tests check the header against this list)
 EXPORTS = [
     "b2_version", "b2_create", "b2_destroy", "b2_set_stream", "b2_synchronize", "b2_last_error",
-    "b2_launch_count", "b2_vad_frames_per_window", "b2_vad_num_windows", "b2_vad_energy_zcr",
-    "b2_rasterize_lengths", "b2_rasterize", "b2_blend_signals", "b2_first_last_nonzero", "b2_align_batch",
-    "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
+    "b2_launch_count", "b2_vad_frames_per_window", "b2_vad_call_samples", "b2_vad_num_windows",
+    "b2_vad_energy_zcr", "b2_rasterize_lengths", "b2_rasterize", "b2_blend_signals", "b2_first_last_nonzero",
+    "b2_align_batch", "b2_reduce_ratios", "b2_sync_batch", "b2_synth_pcm", "b2_vad_stream_begin", "b2_vad_stream_push",
     "b2_vad_stream_windows", "b2_vad_stream_end", "b2_auditok_block_size", "b2_auditok_energy_floor",
     "b2_vad_auditok", "b2_capture_nominations", "b2_sync_tracks", "b2_sync_tracks_gss",
     "b2_sync_tracks_auditok", "b2_sync_tracks_subs", "b2_rasterize_pgs_lengths", "b2_rasterize_pgs",
@@ -76,6 +76,8 @@ def load() -> ctypes.CDLL:
         lib.b2_launch_count.argtypes = [_vp]
         lib.b2_launch_count.restype = _i64
         lib.b2_vad_frames_per_window.argtypes = [ctypes.c_int, ctypes.c_int]
+        lib.b2_vad_call_samples.argtypes = [ctypes.c_int, ctypes.c_int]
+        lib.b2_vad_call_samples.restype = _i64
         lib.b2_vad_num_windows.argtypes = [_i64, ctypes.c_int, ctypes.c_int]
         lib.b2_vad_num_windows.restype = _i64
         lib.b2_vad_energy_zcr.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -233,6 +235,19 @@ class Handle:
     # -- VAD ----------------------------------------------------------------------------------
     def frames_per_window(self, frame_rate: int, sample_rate: int) -> int:
         return int(self.lib.b2_vad_frames_per_window(frame_rate, sample_rate))
+
+    def energy_calls(self, pcm_off, frame_rate: int, sample_rate: int):
+        """The energy / ZCR detector calls of the reference's chunk loop over B signals (b2_vad_call_samples samples
+        each from every signal's start; one per signal where that is 0): (call_off [C+1], first [B+1]), signal b's
+        calls first[b] .. first[b+1]-1.  b2_vad_energy_zcr over call_off writes each signal's frames back to back,
+        signal b's from out_off[first[b]] on."""
+        pcm_off = _i64a(pcm_off)
+        call = int(self.lib.b2_vad_call_samples(frame_rate, sample_rate))
+        if call <= 0:
+            return pcm_off, np.arange(len(pcm_off), dtype=np.int64)
+        parts = [np.arange(a, b, call, dtype=np.int64) for a, b in zip(pcm_off[:-1], pcm_off[1:])]
+        first = np.concatenate([[0], np.cumsum([len(q) for q in parts])]).astype(np.int64)
+        return np.concatenate(parts + [pcm_off[-1:]]).astype(np.int64), first
 
     def vad_energy_zcr(self, pcm, pcm_off, frame_rate: int, sample_rate: int, non_speech_label: float,
                        energy_threshold: int, z_lo: int = -1, z_hi: int = -1, out=None,

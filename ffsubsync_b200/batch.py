@@ -210,7 +210,8 @@ class BatchSynchronizer:
         # MaxScoreAligner.__init__ (ffsubsync/aligners.py:98-101)
         self.max_offset_samples = None if max_offset_seconds is None else abs(int(max_offset_seconds * sample_rate))
         self.handle = _native.get_handle(device)
-        # auditok: samples per detector call, as VideoSpeechTransformer._chunks reads them
+        # auditok: samples per detector call, as VideoSpeechTransformer._chunks reads them (energy / ZCR: the library
+        # derives its calls from the rates, b2_vad_call_samples)
         self.chunk_samples = detector_chunk_bytes(frame_rate, sample_rate) // 2
 
     @property
@@ -486,8 +487,8 @@ class BatchSynchronizer:
 
     def _reference_lengths(self, pcm_off, refs=None, pgs=None, sig=None, seg=None) -> np.ndarray:
         """Each video's reference length [V] in the batched calls, from the library's length helpers: the detector's
-        windows (b2_vad_num_windows, or auditok_out_off's chunk loop), a text stream's b2_rasterize_lengths at ratio
-        1.0, a PGS list's b2_rasterize_pgs_lengths, a signal's stored length and a segment video's b2_segment_length."""
+        windows over the chunk loop (b2_vad_num_windows, or auditok_out_off), a text stream's b2_rasterize_lengths at
+        ratio 1.0, a PGS list's b2_rasterize_pgs_lengths, a signal's stored length and a segment video's b2_segment_length."""
         h = self.handle
         pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
         if self.auditok:
@@ -751,11 +752,13 @@ class BatchSynchronizer:
         mine = distributed.shard_candidates(K, rank, world)
         if self.auditok:   # b2_vad_auditok's float64 signal, rounded once to float32
             ref, ref_off = self._vad_auditok_device(pcm, pcm_off)
-        else:
+        else:   # over the chunk loop's detector calls, as the batched calls run it
+            calls, first = h.energy_calls(pcm_off, self.frame_rate, self.sample_rate)
             fpw = h.frames_per_window(self.frame_rate, self.sample_rate)
-            ref_off = np.concatenate([[0], np.cumsum((np.diff(pcm_off) + fpw - 1) // fpw)]).astype(np.int64)
+            call_out = np.concatenate([[0], np.cumsum((np.diff(calls) + fpw - 1) // fpw)]).astype(np.int64)
+            ref_off = call_out[first]
             ref = torch.empty(int(ref_off[-1]), dtype=torch.float32, device=dev)
-            h.vad_energy_zcr(pcm.data_ptr(), pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
+            h.vad_energy_zcr(pcm.data_ptr(), calls, self.frame_rate, self.sample_rate, self.non_speech_label,
                              self.energy_threshold, self.z_lo, self.z_hi, out=ref.data_ptr(),
                              memspace=_native.B2_DEVICE)
         k_loc = len(mine)
@@ -924,13 +927,13 @@ class BatchSynchronizer:
 
     def _reference_signals(self, pcm_host, pcm_off, refs=None, pgs=None, sig=None, seg=None):
         """The per-video reference signals the batched calls sync against, composed of public calls: the detector
-        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the videos' PCM, with subtitle references
-        (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0, and
+        (b2_vad_energy_zcr, or b2_vad_auditok rounded to float32) over the chunk loop's calls of the videos' PCM, with
+        subtitle references (refs, from _subs_refs) for a video that has one b2_rasterize of its stream at ratio 1.0 and level 1.0, and
         with PGS references (pgs, from _pgs_refs) for a video that has one b2_rasterize_pgs of its intervals, and with
         signal references (sig, from _sig_refs, on the host) for a video that has one DeserializeSpeechTransformer's
         rule at this synchroniser's label, in float64, rounded once to float32, and with segment references (seg, from
-        _seg_refs) for a video that has them the detector over each segment's samples as one signal (b2_vad_energy_zcr,
-        or b2_vad_auditok with the chunk loop rounded to float32), placed by MultiSegmentVideoSpeechTransformer.fit's
+        _seg_refs) for a video that has them the detector over each segment's samples as one signal (b2_vad_energy_zcr
+        or b2_vad_auditok rounded to float32, over the chunk loop), placed by MultiSegmentVideoSpeechTransformer.fit's
         rule (segment_oracle.assemble's, in start order) into int(total * sample_rate) + 2 frames of 0.0.
         Returns (float32 signals back to back, ref_off int64[V+1])."""
         h = self.handle
@@ -941,8 +944,7 @@ class BatchSynchronizer:
             det, det_off = h.vad_auditok(pcm_host, pcm_off, self.frame_rate, self.sample_rate, self.non_speech_label,
                                          chunk_samples=self.chunk_samples)
         else:
-            det, det_off = h.vad_energy_zcr(pcm_host, pcm_off, self.frame_rate, self.sample_rate,
-                                            self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+            det, det_off = self._vad_energy_host(pcm_host, pcm_off)
         if refs is None and pgs is None and sig is None and seg is None:
             return det.astype(np.float32), det_off
         parts = [det[det_off[v]: det_off[v + 1]].astype(np.float32) for v in range(V)]
@@ -976,8 +978,7 @@ class BatchSynchronizer:
                     d, d_off = h.vad_auditok(flat, p_off, self.frame_rate, self.sample_rate, self.non_speech_label,
                                              chunk_samples=self.chunk_samples)
                 else:
-                    d, d_off = h.vad_energy_zcr(flat, p_off, self.frame_rate, self.sample_rate,
-                                                self.non_speech_label, self.energy_threshold, self.z_lo, self.z_hi)
+                    d, d_off = self._vad_energy_host(flat, p_off)
                 L = int(float(total[i]) * self.sample_rate) + 2
                 x = np.zeros(L, dtype=np.float32)
                 for k, j in enumerate(js):
@@ -988,6 +989,15 @@ class BatchSynchronizer:
                 parts[v] = x
         off = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
         return (np.concatenate(parts) if parts else np.zeros(0, np.float32)), off
+
+    def _vad_energy_host(self, pcm_host, pcm_off):
+        """b2_vad_energy_zcr over the reference's chunk loop (each signal cut into its detector calls, as the batched
+        calls cut it).  Returns (float32 frames back to back, out_off int64[B+1])."""
+        h = self.handle
+        calls, first = h.energy_calls(pcm_off, self.frame_rate, self.sample_rate)
+        det, det_off = h.vad_energy_zcr(pcm_host, calls, self.frame_rate, self.sample_rate, self.non_speech_label,
+                                        self.energy_threshold, self.z_lo, self.z_hi)
+        return det, det_off[first]
 
     def _vad_auditok_device(self, pcm, pcm_off):
         """b2_vad_auditok over the videos of the CUDA tensor pcm (chunked as the batched calls chunk them), rounded

@@ -468,10 +468,15 @@ extern "C" int b2_vad_frames_per_window(int frame_rate, int sample_rate) {
   return vad_frames_per_window(frame_rate, sample_rate);
 }
 
+extern "C" int64_t b2_vad_call_samples(int frame_rate, int sample_rate) {
+  return energy_call_samples(frame_rate, sample_rate);
+}
+
 extern "C" int64_t b2_vad_num_windows(int64_t n_samples, int frame_rate, int sample_rate) {
   int fpw = b2_vad_frames_per_window(frame_rate, sample_rate);
   if (fpw <= 0 || n_samples < 0) return -1;
-  return (n_samples + fpw - 1) / fpw;  // len(range(0, n, fpw)), speech_transformers.py:169
+  // len(range(0, len, fpw)) per detector call (speech_transformers.py:169), summed over the chunk loop's calls
+  return chunked_num_windows(n_samples, fpw, energy_call_samples(frame_rate, sample_rate));
 }
 
 extern "C" int b2_vad_energy_zcr(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
@@ -1080,7 +1085,13 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
     return B2_OK;
   }
   const bool seg = !p.det_end.empty();
-  if (!p.auditok) {
+  if (!p.auditok && p.chunked) {   // energy / ZCR over the detector calls (never packed: plan_ref_format)
+    const ChunkTable& ch = p.ch;
+    const int c0 = ch.first[v0];
+    B2_TRY(b2i_vad_launch(h, b.pcm, ch.pcm.data() + c0, ch.first[v1] - c0, p.fpw, r.energy.non_speech_label,
+                          (int64_t)p.fpw * r.energy.energy_threshold, p.z_lo, p.z_hi, b.refsig, ch.out.data() + c0,
+                          nullptr, false, seg ? p.det_end.data() + c0 : nullptr));
+  } else if (!p.auditok) {
     // a packed sub-batch of signal (or segment) videos alone has no audio: the VAD has no tiles and is not asked
     // for bits
     bool audio = r.pcm_off[v1] > r.pcm_off[v0];
@@ -1942,7 +1953,7 @@ extern "C" int b2_ingest_begin(b2_handle h, int V, int frame_rate, int sample_ra
   s->det = det;
   s->V = V;
   s->streams.begin(V);
-  s->plan.begin(V, det.fpw, det.auditok, chunk_samples, energy_threshold_db);
+  s->plan.begin(V, det.fpw, det.auditok, det.call, energy_threshold_db);
   s->held.assign(V, {});
   s->at.assign(V, 0);
   s->cap.assign(V, 0);

@@ -2,7 +2,7 @@
 // audio video's, or one sampled segment's; IngestStreams below numbers them, and the planner's `video` index is that
 // stream number) arrives as pushes of any byte count; the planner cuts it into spans the detector can run on as they come:
 // every span starts on a window boundary and ends on one, or at the end of a detector call (auditok's chunk of
-// chunk_samples), so the windows of a span are exactly the windows the one-shot detector has over the same samples.
+// chunk_samples, energy / ZCR's energy_call_samples), so the windows of a span are exactly the windows the one-shot detector has over the same samples.
 // The samples of an unfinished window (and an odd trailing byte) are held back until the next push of that stream or
 // until finish().  No CUDA call happens here, so tests/host_emul/ingest_emul.cu runs the same code on the CPU.
 #pragma once
@@ -40,10 +40,12 @@ struct IngestPlanner {
   std::vector<int64_t> frames;   // frames the spans so far write
   std::vector<uint8_t> done;     // finish() ran
 
+  // chunk_samples: samples per detector call (SyncPlan::call: auditok's chunk_samples, or energy / ZCR's
+  // energy_call_samples, 0 where its calls divide into windows)
   void begin(int V, int fpw_, bool auditok_, int64_t chunk_samples, double db) {
     fpw = fpw_;
     auditok = auditok_;
-    chunk = auditok_ ? chunk_samples : 0;
+    chunk = chunk_samples;
     energy_threshold_db = db;
     bytes.assign(V, 0);
     base.assign(V, 0);

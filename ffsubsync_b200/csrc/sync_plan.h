@@ -224,6 +224,25 @@ static inline int vad_frames_per_window(int frame_rate, int sample_rate) {
   return (int)((1.0 / (double)sample_rate) * (double)frame_rate + 0.5);
 }
 
+// The reference's chunk loop reads (2 fr // sr) * 5000 samples per detector call (VideoSpeechTransformer._chunks:
+// (2 fr // sr) * 10000 bytes), and energy / ZCR restarts its window grid in every call, so a call that is not a whole
+// number of windows ends in a non-speech partial window and the next call's windows start on a new grid (22.05 kHz:
+// 2 205 000 samples of 221-sample windows).  The samples per call where that happens; 0 where the calls divide into
+// windows (8, 11.025, 12, 16, 24, 32, 44.1, 48, 96 kHz), since one call over the whole video then gives the same
+// frames.
+static inline int64_t energy_call_samples(int frame_rate, int sample_rate) {
+  const int fpw = vad_frames_per_window(frame_rate, sample_rate);
+  if (fpw <= 0) return 0;
+  const int64_t call = (2 * (int64_t)frame_rate / sample_rate) * 5000;
+  return call % fpw ? call : 0;
+}
+
+// Frames of a detector over n samples cut into calls of `call` samples (0: one call), windows of fpw
+static inline int64_t chunked_num_windows(int64_t n, int fpw, int64_t call) {
+  if (call <= 0) return (n + fpw - 1) / fpw;
+  return n / call * ((call + fpw - 1) / fpw) + (n % call + fpw - 1) / fpw;
+}
+
 static inline int auditok_block_size(int frame_rate, int sample_rate) {
   if (frame_rate <= 0 || sample_rate <= 0) return 0;
   // ADSFactory.ads(block_dur=1.0/sample_rate): int(sampling_rate * block_dur), speech_transformers.py:140;
@@ -440,6 +459,10 @@ struct SyncPlan {
   bool gss = false, auditok = false;
   bool any_subs = false;           // a video has a subtitle reference, text or PGS (levels 1 and 0, no PCM)
   int fpw = 0, z_lo = 0, z_hi = 0;
+  // Samples per detector call (0: one call per video): auditok's chunk_samples, or energy_call_samples.  The main
+  // detector launch runs over the chunk table ch when chunked: always for auditok, for energy / ZCR where call > 0.
+  int64_t call = 0;
+  bool chunked = false;
   // the reference's levels (B2CueSource::ref_label / ref_two_level)
   float label = 0.0f, ref_label = 0.0f;
   bool two_level = false;
@@ -453,7 +476,7 @@ struct SyncPlan {
   // a video's reference is not the detector's (text, PGS or signal): it has no PCM, its length comes from its
   // reference, and the tokenizer's table leaves it out.  Without signal videos this is any_subs.
   bool any_ref = false;
-  ChunkTable ch;                   // auditok
+  ChunkTable ch;                   // chunked
   int64_t auditok_e_min = 0;
   B2TokenizerParams tok{0.0, 0.0, 0.0, 0};
   std::vector<double> max_end;     // GSS: each track's largest cue end (its signal length at any ratio)
@@ -471,8 +494,8 @@ struct SyncPlan {
   std::vector<int64_t> det_end;
   // The detector launch over the sampled segments: item k reads the samples item_start[k] .. item_end[k] (absolute
   // in the call's pcm) and writes the scratch frames item_out[k] .. item_out[k+1]; item_tail[k] is auditok's energy
-  // floor of its short last block (0: none).  One item per segment for energy / ZCR, one per chunk of chunk_samples
-  // from the segment's first sample for auditok (the tokenizer restarts in every item).  item_first[v] .. item_first
+  // floor of its short last block (0: none).  One item per detector call of `call` samples from the segment's first
+  // sample (the window grid and auditok's tokenizer restart in every item), one per segment without calls.  item_first[v] .. item_first
   // [v+1]-1: the items of video v (none for other videos).  item_start has one spare entry (the vad launch's table
   // has n + 1 entries).  seg_frames: the scratch's size.
   std::vector<int64_t> item_start, item_end, item_out, item_tail;
@@ -521,14 +544,14 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
     p->cut = {0, V};
     return;
   }
-  // lane eligibility is decided on the tables the energy kernel reads: the videos, or auditok's chunks, and the
+  // lane eligibility is decided on the tables the energy kernel reads: the videos, or the detector calls, and the
   // sampled segments' items
   bool lane_ok;
   if (p->det_end.empty())
-    lane_ok = p->auditok ? env.lane_eligible(p->ch.pcm.data(), (int)p->ch.tail.size(), p->fpw)
+    lane_ok = p->chunked ? env.lane_eligible(p->ch.pcm.data(), (int)p->ch.tail.size(), p->fpw)
                          : env.lane_eligible(r.pcm_off, V, p->fpw);
   else
-    lane_ok = (p->auditok ? ranges_lane_ok(env, p->ch.pcm.data(), p->det_end.data(), (int)p->ch.tail.size(), p->fpw)
+    lane_ok = (p->chunked ? ranges_lane_ok(env, p->ch.pcm.data(), p->det_end.data(), (int)p->ch.tail.size(), p->fpw)
                           : audio_lane_ok(r, env, p, 0, V)) &&
               ranges_lane_ok(env, p->item_start.data(), p->item_end.data(), (int)p->item_end.size(), p->fpw);
   p->n_sub = 1;
@@ -556,8 +579,9 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // kernel, with no subtitle reference, whose chain takes the run path has its VAD write those bits, 32 to a word,
 // instead of the floats: 1/32 of the bytes written, and the chain reads bits instead of floats.  The chain's path
 // is decided here by the aligner's own functions on the chain's own inputs (align_path.h, as enqueue_chain passes
-// them), so the launcher reaches the same choice.  auditok, subtitle references, the lane-group kernel and the
-// FFT paths keep the float reference (text and PGS references alike).  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
+// them), so the launcher reaches the same choice.  auditok, energy / ZCR cut into detector calls (packed words hold
+// whole videos, not calls), subtitle references, the lane-group kernel and the FFT paths keep the float reference
+// (text and PGS references alike).  B2_REF_PACKED=0 keeps it everywhere (A/B knob).
 // Serialized signal references (b2_sync_tracks_sig) have the bits too: sig_ref_kernel writes them, so a sub-batch
 // whose videos are all signal videos or lane-eligible energy audio is packed like an audio one, with either
 // detector (auditok sub-batches qualify only when every video is a signal video).
@@ -578,7 +602,7 @@ static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPl
     const int v0 = p->cut[i], v1 = p->cut[i + 1];
     if (count(p->sub_video, v0, v1) || count(p->pgs_video, v0, v1)) continue;
     const bool all_sig = count(p->sig_video, v0, v1) + count(p->seg_video, v0, v1) == v1 - v0;
-    if (!all_sig && (p->auditok || !audio_lane_ok(r, env, p, v0, v1))) continue;
+    if (!all_sig && (p->chunked || !audio_lane_ok(r, env, p, v0, v1))) continue;
     const int t0 = p->trk_off[v0], nt = p->trk_off[v1] - t0;
     std::vector<int> chain_trk(v1 - v0 + 1);
     for (int v = v0; v <= v1; ++v) chain_trk[v - v0] = p->trk_off[v] - t0;
@@ -779,7 +803,7 @@ static void plan_segments(const SyncRequest& r, SyncPlan* p) {
   const auto& s = r.seg;
   const int V = r.V, fpw = p->fpw;
   // the main launch: every entry as before, a segment video's empty
-  if (p->auditok) {
+  if (p->chunked) {
     const int nc = (int)p->ch.tail.size();
     p->det_end.assign(p->ch.pcm.begin() + 1, p->ch.pcm.begin() + 1 + nc);
     for (int v : p->seg_video) p->det_end[p->ch.first[v]] = p->ch.pcm[p->ch.first[v]];
@@ -787,7 +811,8 @@ static void plan_segments(const SyncRequest& r, SyncPlan* p) {
     p->det_end.assign(r.pcm_off + 1, r.pcm_off + V + 1);
     for (int v : p->seg_video) p->det_end[v] = r.pcm_off[v];
   }
-  // the segments' items: energy one per segment, auditok one per chunk
+  // the segments' items: one per detector call of `call` samples from the segment's first sample (one per segment
+  // without calls)
   p->item_first.assign(V + 1, 0);
   p->item_out.assign(1, 0);
   p->item_start.clear();
@@ -801,7 +826,7 @@ static void plan_segments(const SyncRequest& r, SyncPlan* p) {
     for (int64_t j = i < 0 ? 0 : s.off[i]; i >= 0 && j < s.off[i + 1]; ++j) {
       const int64_t a = r.pcm_off[v] + s.lo[j], n = s.hi[j] - s.lo[j];
       seg_scr[j - s.off[0]] = p->item_out.back();
-      const int64_t step = !p->auditok || r.auditok.chunk_samples <= 0 ? (n > 0 ? n : 1) : r.auditok.chunk_samples;
+      const int64_t step = p->call > 0 ? p->call : (n > 0 ? n : 1);
       for (int64_t c = 0; c < n; c += step) {
         const int64_t len = std::min(step, n - c);
         p->item_start.push_back(a + c);
@@ -853,9 +878,12 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
       B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad tokenizer parameters", who);
     p->auditok_e_min = auditok_energy_floor(p->fpw, a.energy_threshold_db);
     p->tok = B2TokenizerParams{a.min_length, a.max_continuous_silence, a.non_speech_label, (long long)a.max_length};
+    p->call = a.chunk_samples;
   } else {
     p->fpw = vad_frames_per_window(r.frame_rate, r.sample_rate);
+    p->call = energy_call_samples(r.frame_rate, r.sample_rate);
   }
+  p->chunked = p->auditok || p->call > 0;
   const int fpw = p->fpw;
   if (fpw <= 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: bad frame_rate/sample_rate", who);
   p->z_lo = r.energy.z_lo < 0 ? 0 : r.energy.z_lo;
@@ -912,10 +940,11 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
     const int64_t n = r.pcm_off[v + 1] - r.pcm_off[v];
     if (n < 0) B2_FAIL(p, B2_ERR_BAD_ARG, "%s: pcm_off not monotone", who);
     if (p->any_ref && subs_len[v] >= 0) p->ref_off[v + 1] = p->ref_off[v] + subs_len[v];
-    else if (!p->auditok) p->ref_off[v + 1] = p->ref_off[v] + (n + fpw - 1) / fpw;
+    else if (!p->chunked) p->ref_off[v + 1] = p->ref_off[v] + (n + fpw - 1) / fpw;
   }
-  if (p->auditok) {
-    build_chunk_table(r.pcm_off, V, 0, fpw, r.auditok.chunk_samples, r.auditok.energy_threshold_db,
+  if (p->chunked) {
+    // energy / ZCR reads no tail floor (its partial window is non-speech): INFINITY makes them INT64_MAX, never met
+    build_chunk_table(r.pcm_off, V, 0, fpw, p->call, p->auditok ? r.auditok.energy_threshold_db : INFINITY,
                       p->any_ref ? subs_len.data() : nullptr, &p->ch);
     for (int v = 0; v < V; ++v) p->ref_off[v + 1] = p->ch.out[p->ch.first[v + 1]];
   }

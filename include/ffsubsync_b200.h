@@ -95,8 +95,16 @@ int64_t b2_launch_count(b2_handle h);
  * output length, labels, partial-window rule) called from the chunk loop :710-753.
  * Rule (this repo's detector, DESIGN.md): speech <=> sum x^2 >= fpw*energy_threshold and
  * z_lo <= #sign changes inside the window <= z_hi.  z_lo/z_hi < 0 select the defaults.
- * pcm: int16 mono samples of all B signals back to back (memspace); out: float per window. */
+ * pcm: int16 mono samples of all B signals back to back (memspace); out: float per window.
+ * b2_vad_energy_zcr is one detector call per signal: ceil(n / fpw) windows.  The reference's chunk loop calls the
+ * detector once per (2 frame_rate // sample_rate) * 5000 samples, and every call restarts the window grid; where that
+ * is not a whole number of windows (22.05 kHz: 2 205 000 samples of 221) each call ends in a non-speech partial
+ * window.  b2_vad_call_samples gives the samples per call there and 0 where the calls divide into windows (one call
+ * per video then gives the same frames).  The batched sync calls and the ingest session follow the chunk loop:
+ * b2_vad_num_windows is their reference length for a video of n_samples, the sum over its calls of ceil(len / fpw);
+ * b2_vad_energy_zcr over the calls as separate signals gives their frames. */
 int b2_vad_frames_per_window(int frame_rate, int sample_rate);
+int64_t b2_vad_call_samples(int frame_rate, int sample_rate);
 int64_t b2_vad_num_windows(int64_t n_samples, int frame_rate, int sample_rate);
 int b2_vad_energy_zcr(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
                       int frame_rate, int sample_rate, float non_speech_label,
@@ -211,7 +219,8 @@ int b2_reduce_ratios(b2_handle h, const double* score, const int32_t* offset,
 
 /* ---- the whole hot path for a batch of (video, subtitle) pairs -----------------------------
  * VAD on each pair's PCM -> rasterise its cues at K ratios -> align -> reduce
- * (ffsubsync/ffsubsync.py:637 + :196-235).  pcm and the outputs follow memspace; memspace may also be
+ * (ffsubsync/ffsubsync.py:637 + :196-235).  The VAD follows the reference's chunk loop: b2_vad_energy_zcr over each
+ * b2_vad_call_samples call of the PCM (over the whole PCM where that is 0), b2_vad_num_windows frames.  pcm and the outputs follow memspace; memspace may also be
  * B2_DEVICE_RESIDENT (see the enum): consecutive calls over resident PCM then overlap across the call boundary. */
 int b2_sync_batch(b2_handle h, const int16_t* pcm, const int64_t* pcm_off, int B,
                   int frame_rate, int sample_rate, float non_speech_label,
@@ -426,8 +435,9 @@ int b2_sync_tracks_sig(b2_handle h, const int16_t* pcm /* or NULL without audio 
  *                        (segments are slices of it) or only the decoded windows back to back.  Samples outside the
  *                        segments are never read, and B2_HOST copies only the segments (and the audio videos) to the
  *                        device.
- * Segment j writes what the call's detector returns for its samples taken as one signal - energy / ZCR:
- * ceil(n / fpw) frames, a trailing partial window non-speech; auditok: the chunk loop of chunk_samples from the
+ * Segment j writes what the call's detector returns for its samples taken as one signal - energy / ZCR: the chunk
+ * loop of b2_vad_call_samples from the segment's first sample (one call where that is 0), ceil(len / fpw) frames per
+ * call, a trailing partial window non-speech; auditok: the chunk loop of chunk_samples from the
  * segment's first sample, the tokenizer restarting in every chunk - to the frames [seg_start * sample_rate,
  * min(seg_start * sample_rate + len, L)) of a reference of L = int(seg_total * sample_rate) + 2 frames (float64
  * product, truncated), in increasing start order, so that a later segment overwrites an earlier one where they
@@ -554,7 +564,7 @@ int b2_capture_reference(b2_handle h, float* ref, int64_t capacity, int64_t* ref
 /* ---- speech output of the batched sync calls (--serialize-speech) ----------------------------
  * While set on a handle, every batched sync call (b2_sync_batch, b2_sync_tracks, _gss, _auditok, _subs, _pgs, _sig,
  * _seg) writes the reference signal of each listed video as float64: listed video i = videos[i] lands at
- * speech[speech_off[i] .. speech_off[i+1]), its length the call's own reference length (ceil(n/fpw) frames for
+ * speech[speech_off[i] .. speech_off[i+1]), its length the call's own reference length (b2_vad_num_windows frames for
  * energy / ZCR, the chunk loop's blocks for auditok, int(max_end*sr) + 2 for a text stream or PGS, int(seg_total*sr)
  * + 2 for segments, the stored length for a signal).  Each frame is the float32 frame the call aligned against,
  * widened: VideoSpeechTransformer's output rounded to float32 for detector videos, the rasterised stream for text,
@@ -586,8 +596,8 @@ int64_t b2_segment_length(double total_seconds, int sample_rate);
  * video's reference signal stays on the device - never its PCM.  A final call runs the batched sync chain over them.
  * Let P_v be all bytes pushed for video v, in push order, with a trailing odd byte dropped.  Whatever the cut of P_v
  * into pushes (1-byte and odd pushes, pushes that split a window or a detector call) and the interleaving:
- *   energy / ZCR   video v's reference is b2_vad_energy_zcr over P_v (ceil(n/fpw) windows, a partial last window
- *                  non-speech);
+ *   energy / ZCR   video v's reference is b2_vad_energy_zcr over each b2_vad_call_samples call of P_v (over P_v
+ *                  where that is 0), b2_vad_num_windows frames, a call's partial last window non-speech;
  *   auditok        it is b2_vad_auditok over P_v with chunk_samples, rounded once to float32: the tokenizer restarts
  *                  at every chunk_samples boundary of P_v wherever the pushes fell (read(n) on a pipe returns n bytes
  *                  until EOF, so the stream fixes the boundaries, not the caller);

@@ -8,7 +8,7 @@ batched calls write in increasing start order, so the later start wins where seg
 import numpy as np
 
 from . import auditok_oracle as au
-from . import vad_oracle as vo
+from . import chunk_oracle as co
 
 NO_SPEECH = ("Unable to detect speech in any sampled segment. "
              "Perhaps try specifying a different stream / track, or a different vad.")
@@ -39,11 +39,12 @@ def has_speech(x) -> bool:
 def detect(pcm, detector: str = "energy_zcr", sample_rate: int = 100, frame_rate: int = 16000,
            non_speech_label: float = 0.0, chunk_samples: int = 0, **params) -> np.ndarray:
     """The call's detector on one segment's int16 samples taken as one signal: energy / ZCR (vad_oracle; params:
-    energy_threshold, z_lo, z_hi), or auditok over the chunk loop of chunk_samples samples from the segment's first
-    sample (0: one call; params: energy_threshold in dB, min_length, max_length, max_continuous_silence)."""
+    energy_threshold, z_lo, z_hi) over the reference's chunk loop from the segment's first sample
+    (chunk_oracle.chunk_loop), or auditok over the chunk loop of chunk_samples samples from there (0: one call;
+    params: energy_threshold in dB, min_length, max_length, max_continuous_silence)."""
     pcm = np.asarray(pcm, dtype=np.int16)
     if detector == "energy_zcr":
-        return vo.energy_zcr_detect(pcm, sample_rate, frame_rate, non_speech_label, **params)
+        return co.chunk_loop("energy_zcr", pcm, frame_rate, sample_rate, non_speech_label, **params)
     step = chunk_samples if chunk_samples > 0 else max(len(pcm), 1)
     parts = [au.auditok_detect_fast(pcm[i:i + step].tobytes(), sample_rate, frame_rate, non_speech_label, **params)
              for i in range(0, len(pcm), step)]

@@ -121,6 +121,7 @@ int main(int argc, char** argv) {
     fprintf(o, "\n");
   };
   put("fpw", std::vector<int>{p.fpw, p.z_lo, p.z_hi});
+  put("call", std::vector<int64_t>{p.call, (int64_t)p.chunked});
   put("n_sub", std::vector<int>{p.n_sub, p.vad_sms});
   put("cut", p.cut);
   put("trk_off", p.trk_off);

@@ -71,15 +71,16 @@ def _random_ops(rng, V, fpw, chunk):
     return ops
 
 
-@pytest.mark.parametrize("auditok,fpw,chunk", [(False, 160, 0), (False, 480, 0), (True, 160, 0), (True, 160, 1600),
-                                               (True, 160, 1000), (True, 80, 333), (True, 480, 4800)])
+@pytest.mark.parametrize("auditok,fpw,chunk", [(False, 160, 0), (False, 480, 0), (False, 7, 30), (False, 221, 2205),
+                                               (True, 160, 0), (True, 160, 1600), (True, 160, 1000), (True, 80, 333),
+                                               (True, 480, 4800)])
 @pytest.mark.parametrize("seed", range(6))
 def test_spans_tile_the_stream_at_window_and_call_boundaries(auditok, fpw, chunk, seed):
     rng = np.random.RandomState(seed * 101 + fpw + chunk)
     V = 4
     ops = _random_ops(rng, V, fpw, chunk)
     per_op, frames, base = _run(V, fpw, auditok, chunk, ops)
-    c = chunk if auditok else 0
+    c = chunk   # energy / ZCR too: its calls where they do not divide into windows (b2_vad_call_samples)
     per_call = -(-c // fpw) if c > 0 else 0
     nbytes = [0] * V
     at = [0] * V                      # next sample each video's spans must start at
