@@ -1,11 +1,13 @@
 // CPU run of the batched sync calls' planner (ffsubsync_b200/csrc/sync_plan.h): the same plan_sync the five
 // b2_sync_* entry points call before they launch anything.  Test infrastructure (the build container has no
-// GPU); tests/test_plan_cpu.py and tests/test_auditok_sync_cpu.py drive it.
+// GPU); tests/test_plan_cpu.py, tests/test_plan_random_cpu.py and tests/test_auditok_sync_cpu.py
+// drive it.
 //
 // usage: plan_emul in.txt out.txt
 //   in : one field of the request per line, "name n v0 .. v(n-1)"; a missing array is a null pointer.
 //        Arrays: pcm_off track_video cue_start cue_end cue_off ratios ref_is_subs ref_cue_start ref_cue_end
-//        ref_cue_off.  Scalars (n = 1): who frame_rate sample_rate detector label energy_threshold z_lo z_hi
+//        ref_cue_off ref_is_pgs pgs_start pgs_end pgs_off ref_is_sig sig_off (the values x are not read: a
+//        dummy) seg_video seg_total seg_off seg_start seg_lo seg_hi.  Scalars (n = 1): who frame_rate sample_rate detector label energy_threshold z_lo z_hi
 //        auditok_label energy_threshold_db min_length max_length max_continuous_silence chunk_samples
 //        start_seconds max_offset_samples outputs (1: best_* given) all (1: all_* given) gss (1: the search
 //        runs) gss_ratio (1: given; default: gss) pcm (1: pcm given) sm_count subbatches vad_sms (as the
@@ -52,10 +54,10 @@ int main(int argc, char** argv) {
   };
   auto as_i = [](const std::string& s) { return strtoll(s.c_str(), nullptr, 10); };
   auto as_f = [](const std::string& s) { return strtod(s.c_str(), nullptr); };
-  i64s.reserve(8);
-  f64s.reserve(8);
-  i32s.reserve(2);
-  u8s.reserve(2);
+  i64s.reserve(16);
+  f64s.reserve(16);
+  i32s.reserve(4);
+  u8s.reserve(4);
   static int16_t pcm_dummy[8];
   static double d_dummy[1];
   static int32_t i_dummy[1];
@@ -104,6 +106,20 @@ int main(int argc, char** argv) {
   r.search = i64("gss") != 0;
   r.gss_ratio = i64("gss_ratio", r.search) ? d_dummy : nullptr;
   r.memspace = B2_HOST;
+  r.pgs.is_pgs = arr(u8s, "ref_is_pgs", as_i);
+  r.pgs.start_s = arr(f64s, "pgs_start", as_f);
+  r.pgs.end_s = arr(f64s, "pgs_end", as_f);
+  r.pgs.off = arr(i64s, "pgs_off", as_i);
+  r.sig.is_sig = arr(u8s, "ref_is_sig", as_i);
+  r.sig.off = arr(i64s, "sig_off", as_i);
+  r.sig.x = r.sig.off ? d_dummy : nullptr;
+  r.seg.video = arr(i32s, "seg_video", as_i);
+  r.seg.n = has("seg_video") ? (int)in["seg_video"].size() : 0;
+  r.seg.total = arr(f64s, "seg_total", as_f);
+  r.seg.off = arr(i64s, "seg_off", as_i);
+  r.seg.start = arr(i64s, "seg_start", as_i);
+  r.seg.lo = arr(i64s, "seg_lo", as_i);
+  r.seg.hi = arr(i64s, "seg_hi", as_i);
   g_lane = i64("lane") != 0;
   const std::string subbatches = has("subbatches") ? in["subbatches"][0] : "";
   const std::string vad_sms = has("vad_sms") ? in["vad_sms"][0] : "";
@@ -135,6 +151,10 @@ int main(int argc, char** argv) {
   put("tok_off", p.ch.tok_off);
   put("tok_end", p.ch.tok_end);
   put("tok_first", p.ch.tok_first);
+  put("pgs_video", p.pgs_video);
+  put("sig_video", p.sig_video);
+  put("seg_video", p.seg_video);
+  put("ref_packed", p.ref_packed);
   put("audio_samples", std::vector<int64_t>{p.audio_samples});
   fprintf(o, "two_level %d %.9g\n", (int)p.two_level, (double)p.ref_label);
   fclose(o);
