@@ -33,7 +33,7 @@ EXPORTS = [
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
     "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
     "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort", "b2_ingest_segments", "b2_ingest_push_segments",
-    "b2_ingest_drop_segment",
+    "b2_ingest_drop_segment", "b2_ingest_sync_refs",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -150,6 +150,7 @@ def load() -> ctypes.CDLL:
         lib.b2_ingest_windows.argtypes = [_vp, _vp]
         lib.b2_ingest_sync_tracks.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _f64, _i64,
                                               _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_ingest_sync_refs.argtypes = [_vp] + [_vp] * 12 + lib.b2_ingest_sync_tracks.argtypes[1:]
         lib.b2_ingest_abort.argtypes = [_vp]
         lib.b2_ingest_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
         lib.b2_ingest_push_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
@@ -820,16 +821,39 @@ class Handle:
     def ingest_sync_tracks(self, track_video, cue_start_s, cue_end_s, cue_keep, cue_off, ratios, start_seconds: float,
                            max_offset_samples: Optional[int], gss: bool = False, best_score=None, best_offset=None,
                            best_k=None, all_score=None, all_offset=None, gss_ratio=None, gss_evals=None,
-                           want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST):
+                           want_all: bool = False, want_evals: bool = False, memspace: int = B2_HOST,
+                           ref_is_subs=None, ref_cue_start_s=None, ref_cue_end_s=None, ref_cue_keep=None,
+                           ref_cue_off=None, ref_is_pgs=None, pgs_start_s=None, pgs_end_s=None, pgs_off=None,
+                           ref_is_sig=None, x=None, sig_off=None):
         """Flush, sync the tracks against the session's references and close it (b2_ingest_sync_tracks).  Outputs as
         for sync_tracks / sync_tracks_gss (memspace B2_HOST allocates them; B2_DEVICE takes device pointers).
+        The reference tables of sync_tracks_sig (text streams, PGS intervals, stored signals; x a float64 numpy array
+        under B2_HOST, a device pointer otherwise) give videos without pushes their references
+        (b2_ingest_sync_refs, called when any table is given).
         Returns (best_score, best_offset, best_k, all_score, all_offset), plus (gss_ratio, gss_evals) with gss."""
         track_video = np.ascontiguousarray(track_video, dtype=np.int32)
         cue_off = _i64a(cue_off)
         T = len(track_video)
+        V = getattr(self, "_ingest_V", 0)
+        tables = any(a is not None for a in (ref_is_subs, ref_cue_off, ref_is_pgs, pgs_off, ref_is_sig, sig_off))
+        name = "b2_ingest_sync_refs" if tables else "b2_ingest_sync_tracks"
         if len(cue_off) != T + 1:
             self.ingest_abort()
-            raise NativeError(-1, "b2_ingest_sync_tracks", "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+            raise NativeError(-1, name, "cue_off has %d entries for %d tracks" % (len(cue_off), T))
+        u8 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.uint8)   # noqa: E731
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)   # noqa: E731
+        ref_is_subs, ref_is_pgs, ref_is_sig = u8(ref_is_subs), u8(ref_is_pgs), u8(ref_is_sig)
+        ref_cue_off, pgs_off, sig_off = (None if a is None else _i64a(a) for a in (ref_cue_off, pgs_off, sig_off))
+        for what, a, n in (("ref_is_subs", ref_is_subs, V), ("ref_is_pgs", ref_is_pgs, V), ("ref_is_sig", ref_is_sig, V),
+                           ("ref_cue_off", ref_cue_off, V + 1), ("pgs_off", pgs_off, V + 1), ("sig_off", sig_off, V + 1)):
+            if a is not None and len(a) != n:
+                self.ingest_abort()
+                raise NativeError(-1, name, "%s has %d entries for %d videos" % (what, len(a), V))
+        ref_cue_start_s, ref_cue_end_s, pgs_start_s, pgs_end_s = (f64(a) for a in (ref_cue_start_s, ref_cue_end_s,
+                                                                                   pgs_start_s, pgs_end_s))
+        ref_cue_keep = u8(ref_cue_keep)
+        if x is not None and not isinstance(x, int):
+            x = f64(x)
         ratios = np.ascontiguousarray(ratios, dtype=np.float64)
         K = len(ratios)
         cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
@@ -847,13 +871,19 @@ class Handle:
             gss_evals = np.empty(T * GSS_EVALS, dtype=np.float64) if gss and want_evals else None
         elif gss and gss_ratio is None:
             self.ingest_abort()
-            raise ValueError("b2_ingest_sync_tracks with the search on device memory needs gss_ratio")
-        st = self.lib.b2_ingest_sync_tracks(
-            self.h, _ptr(track_video), T, _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off),
-            _ptr(ratios), K, float(start_seconds), _mask_width(max_offset_samples), _ptr(best_score),
-            _ptr(best_offset), _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
-            _ptr(gss_evals) if gss else None, memspace)
-        self._check(st, "b2_ingest_sync_tracks")
+            raise ValueError("%s with the search on device memory needs gss_ratio" % name)
+        args = (_ptr(track_video), T, _ptr(cue_start_s), _ptr(cue_end_s), _ptr(cue_keep), _ptr(cue_off), _ptr(ratios),
+                K, float(start_seconds), _mask_width(max_offset_samples), _ptr(best_score), _ptr(best_offset),
+                _ptr(best_k), _ptr(all_score), _ptr(all_offset), _ptr(gss_ratio) if gss else None,
+                _ptr(gss_evals) if gss else None, memspace)
+        if tables:
+            st = self.lib.b2_ingest_sync_refs(
+                self.h, _ptr(ref_is_subs), _ptr(ref_cue_start_s), _ptr(ref_cue_end_s), _ptr(ref_cue_keep),
+                _ptr(ref_cue_off), _ptr(ref_is_pgs), _ptr(pgs_start_s), _ptr(pgs_end_s), _ptr(pgs_off),
+                _ptr(ref_is_sig), _ptr(x), _ptr(sig_off), *args)
+        else:
+            st = self.lib.b2_ingest_sync_tracks(self.h, *args)
+        self._check(st, name)
         res = (best_score, best_offset, best_k, all_score, all_offset)
         return res + (gss_ratio, gss_evals) if gss else res
 

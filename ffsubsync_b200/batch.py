@@ -81,6 +81,10 @@ _PGS_ARGS = ("pgs_start", "pgs_end", "pgs_off", "pgs_video")
 _SIG_ARGS = ("sig", "sig_off", "sig_video")
 # keyword arguments of the sync methods that give videos sampled segments as reference (--multi-segment-sync)
 _SEG_ARGS = ("seg_video", "seg_total", "seg_off", "seg_start", "seg_lo", "seg_hi")
+# subtitle-file references (the reference's SUBTITLE_EXTENSIONS), which the batched calls do not take
+_SUBTITLE_EXTENSIONS = ("srt", "ass", "ssa", "sub")
+# sync_media: the segment field of a decoder job that probes a PGS stream instead of decoding audio
+_PGS_JOB = "pgs"
 _NO_SPEECH_MESSAGE = ("Unable to detect speech in any sampled segment. "
                       "Perhaps try specifying a different stream / track, or a different vad.")
 
@@ -227,12 +231,14 @@ class BatchSynchronizer:
             return refs, pgs
         return self._drop_text(V, refs, pgs[0] != 0), pgs
 
-    def _all_refs(self, V: int, streams: dict, on_device: bool):
+    def _all_refs(self, V: int, streams: dict, on_device: bool, seg=None):
         """(refs, pgs, sig, seg) of the keyword arguments: refs and pgs from _references, sig from _sig_refs, seg from
         _seg_refs.  A video with a signal and a text or PGS reference is refused: the reference tool's reference is a
         single file.  So is a video with segments and a PGS or signal reference; its text streams are dropped, since
-        sampling is audio-only (the reference drops a ``subs_then_`` prefix)."""
-        seg = self._seg_refs(V, {k: streams.pop(k) for k in _SEG_ARGS if k in streams})
+        sampling is audio-only (the reference drops a ``subs_then_`` prefix).  ``seg``: segment videos declared
+        elsewhere (an ingest session's (seg_video, seg_total)) in place of the segment keyword arguments."""
+        if seg is None:
+            seg = self._seg_refs(V, {k: streams.pop(k) for k in _SEG_ARGS if k in streams})
         sig = self._sig_refs(V, {k: streams.pop(k) for k in _SIG_ARGS if k in streams}, on_device)
         refs, pgs = self._references(V, streams)
         if seg is not None:
@@ -1016,11 +1022,14 @@ class BatchSynchronizer:
         detector runs on the device as it comes, so only the reference signals are ever held - not the videos'
         whole decodes.  The results equal the whole-PCM sync methods' over the same bytes.  expect_samples [V]: a
         sizing hint (e.g. ffprobe's duration times frame_rate); a longer video still fits.  The audio detector is
-        this synchroniser's (the one after ``subs_then_``); a session has no subtitle, PGS or signal references.
+        this synchroniser's (the one after ``subs_then_``).
         segments (``--multi-segment-sync``): dict(seg_video, seg_total, seg_off, seg_start), e.g. from
         ``ingest_segment_table``; those videos take their sampled segments' PCM (``push_segment``) and are synced
         against the sparse reference, as the sync methods with ``segment_table(..., piece_samples=...)`` over the
-        pieces pushed.  A segment video's expect_samples entry is the hint for each of its segments."""
+        pieces pushed.  A segment video's expect_samples entry is the hint for each of its segments.
+        Videos whose reference needs no audio - an embedded text stream with a ``subs_then_`` detector, PGS intervals,
+        a stored signal - take no pushes: their references are given to ``IngestSession.sync_tracks`` as the sync
+        methods' keyword arguments."""
         return IngestSession(self, V, expect_samples, segments)
 
 
@@ -1077,23 +1086,46 @@ class IngestSession:
         self.sync.handle.ingest_abort()
 
     def sync_tracks(self, track_video, cue_start, cue_end, cue_off, cue_keep=None, speech_video=None, out=None,
-                    all_out=None, want_all: bool = False):
+                    all_out=None, want_all: bool = False, **streams):
         """Sync track t (cue list cue_off[t] .. cue_off[t+1]) against video track_video[t] (non-decreasing) and close
         the session.  Without ``out``: what ``sync_host_tracks`` returns over the videos' PCM back to back.  With
         ``out`` (CUDA tensors best_score f64[T], best_offset i32[T], best_k i32[T], gss_ratio f64[T] with the search;
         ``all_out`` as for sync_device_tracks): what ``sync_device_tracks`` returns, with nothing synchronised.
         ``speech_video`` as there.  The golden-section search runs on the device only: outside its envelope the call
         raises (there is no PCM left to compose it from).  A segment video without a frame > 0 raises the reference's
-        ValueError on the host and gets ``best_k == B2_BEST_K_NO_SPEECH`` on the device, as the sync methods do."""
+        ValueError on the host and gets ``best_k == B2_BEST_K_NO_SPEECH`` on the device, as the sync methods do.
+        streams: the references of videos that took no pushes, as the sync methods take them - the embedded text
+        streams of a ``subs_then_`` detector (ref_cue_start, ref_cue_end, ref_cue_off, ref_stream_video and
+        ref_cue_content or ref_cue_keep), PGS intervals (pgs_start, pgs_end, pgs_off, pgs_video) and stored signals
+        (sig, sig_off, sig_video: a numpy array without ``out``, a CUDA tensor with it), combined by the same rules.
+        Segments are declared at ``ingest``, not here.  A video given such a reference that received pushed bytes is
+        refused (b2_ingest_sync_refs)."""
         s = self.sync
         h = s.handle
         pcm_off = np.concatenate([[0], np.cumsum(self._bytes // 2)]).astype(np.int64)
         on_device = out is not None
+        sig_in = streams.get("sig")
         try:
-            speech = s._speech_request(speech_video, pcm_off, seg=self._seg, on_device=on_device)
+            if any(streams.get(k) is not None for k in _SEG_ARGS):
+                raise ValueError("a session declares its segments at ingest(segments=...), not at sync_tracks")
+            refs, pgs, sig, _ = s._all_refs(self.V, streams, on_device, seg=self._seg)
+            speech = s._speech_request(speech_video, pcm_off, refs, pgs, sig, seg=self._seg, on_device=on_device)
         except Exception:
             self.abort()
             raise
+        tables = {}
+        if refs is not None:
+            tables.update(zip(("ref_is_subs", "ref_cue_start_s", "ref_cue_end_s", "ref_cue_keep", "ref_cue_off"), refs))
+        if pgs is not None:
+            tables.update(zip(("ref_is_pgs", "pgs_start_s", "pgs_end_s", "pgs_off"), pgs))
+        if sig is not None:
+            is_sig, x, voff = sig
+            tables.update(ref_is_sig=is_sig, x=x if isinstance(x, np.ndarray) else (x.data_ptr() if x.numel() else None),
+                          sig_off=voff)
+            if on_device and x is not sig_in:
+                # a converted copy: ready before the handle's stream reads it, and kept until the call is done
+                import torch
+                torch.cuda.current_stream(x.device).synchronize()
         cues = (track_video, cue_start, cue_end, cue_keep, cue_off, s.ratios, s.start_seconds, s.max_offset_samples)
         with s._speech_output(speech):
             if on_device:
@@ -1102,13 +1134,16 @@ class IngestSession:
                     ptrs["gss_ratio"] = out["gss_ratio"].data_ptr()
                 if all_out:
                     ptrs.update(all_score=all_out["score"].data_ptr(), all_offset=all_out["offset"].data_ptr())
-                h.ingest_sync_tracks(*cues, gss=s.gss, memspace=_native.B2_DEVICE, **ptrs)
+                h.ingest_sync_tracks(*cues, gss=s.gss, memspace=_native.B2_DEVICE, **ptrs, **tables)
             else:
-                res = h.ingest_sync_tracks(*cues, gss=s.gss, want_all=want_all, memspace=_native.B2_HOST)
+                res = h.ingest_sync_tracks(*cues, gss=s.gss, want_all=want_all, memspace=_native.B2_HOST, **tables)
         if on_device:
+            if sig is not None and sig[1] is not sig_in:
+                h.synchronize()
             if speech is not None:
                 out["speech"], out["speech_off"] = s._speech_result(speech)
             return out
+        s._raise_bad_signals(sig, res[2])
         s._raise_no_speech(self._seg, res[2], track_video)
         res = res[:6] if want_all else res[:3] + res[5:6]
         return res if speech is None else res + s._speech_result(speech)
@@ -1129,7 +1164,7 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
                max_decoders: int = 4, ffmpeg_path: Optional[str] = None, max_duration_seconds: Optional[float] = None,
                ref_stream: Optional[str] = None, expect_samples=None, speech_video=None, want_all: bool = False,
                multi_segment=False, segment_count: int = 8, segment_duration: int = 60,
-               skip_intro_outro: bool = False):
+               skip_intro_outro: bool = False, pgs_ref_stream=None, **streams):
     """``ffs movie.mkv -i a.srt ...`` for a library: decodes paths[v] with up to ``max_decoders`` ffmpeg processes at
     a time (VideoSpeechTransformer._build_ffmpeg_args: ``-ss`` from the synchroniser's start_seconds, ``-t`` from
     max_duration_seconds, ffmpeg_path, ref_stream), reads each pipe in the reference's 100 s ``read()`` calls on a
@@ -1141,7 +1176,22 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
     ``skip_intro_outro``) are decoded, each by its own ``ffmpeg -ss start -t segment_duration`` in the same pool.  A
     segment decoder that fails or cannot start is logged as the reference's "failed to extract segment" warning and
     the segment is dropped; a failing full-audio decoder aborts, as without segments.  The synchroniser's
-    start_seconds applies to the subtitle tracks only there."""
+    start_seconds applies to the subtitle tracks only there.
+    References that are not a video's audio (make_reference_pipe's order): such a video gets no decoder job.
+    - A path ending in ``npz`` / ``npy`` (the reference's ``_ref_format``) is a stored signal (``--serialize-speech``):
+      it is loaded with ``load_stored_speech`` and passed as ``sig``.  A subtitle file (``srt``, ``ass``, ``ssa``,
+      ``sub``) is refused with ValueError before anything starts: the batched calls have no subtitle-file references.
+    - ``pgs_ref_stream`` (``--pgs-ref-stream``): None, ``"auto"`` (the first PGS stream), one specifier (``"s:N"`` /
+      ``"0:s:N"``) for every video that is not a stored signal, or a list of V such entries (None: not PGS).  Each PGS
+      video's display intervals are probed with ffprobe (PGSSpeechTransformer._probe_intervals) as jobs of the same
+      pool; a failed probe, a stream without timings or intervals PGSSpeechTransformer.fit refuses (checked by fit's
+      own rasterisation before the sync) raise the reference's ValueError, with no fallback to audio.
+    - ``streams``: the embedded text streams of a ``subs_then_`` synchroniser, as the sync methods take them (their
+      extraction stays the caller's job); any other keyword is refused with TypeError before anything starts.  A video
+      that select_reference_streams gives a stream, and that is not a PGS or segment video, is not decoded.
+    The combinations follow the sync methods: PGS wins over text; a signal video with a PGS or text reference, and a
+    segment video with a PGS or signal reference, are refused; a segment video's text stream is dropped.  Returns what
+    ``sync_host_tracks`` returns over the decoded audio videos' PCM and the same references."""
     import queue
     import shutil
     import subprocess
@@ -1161,6 +1211,39 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
     if seg_videos and max_duration_seconds is not None:
         raise ValueError("max_duration_seconds limits a full decode; multi_segment decodes sampled segments of "
                          "segment_duration seconds instead")
+    from .speech_transformers import PGSSpeechTransformer, load_stored_speech
+    # PGS and signal references come from pgs_ref_stream and the paths, segments from multi_segment: streams holds the
+    # text streams alone, refused otherwise before any decoder starts
+    other = sorted(k for k in streams if k not in _STREAM_ARGS)
+    if other:
+        raise TypeError("sync_media takes embedded text streams as keyword arguments (%s), not %s; PGS references "
+                        "come from pgs_ref_stream, stored signals from .npz / .npy paths and segments from "
+                        "multi_segment" % (", ".join(_STREAM_ARGS), ", ".join(other)))
+    # the reference's choice by file type (make_reference_pipe: _ref_format is the name's last three characters)
+    for p in paths:
+        if str(p)[-3:] in _SUBTITLE_EXTENSIONS:
+            raise ValueError("%r is a subtitle file; the batched calls take no subtitle-file references" % str(p))
+    sig_videos = [v for v in range(V) if str(paths[v])[-3:] in ("npz", "npy")]
+    if pgs_ref_stream is None or isinstance(pgs_ref_stream, str):
+        pgs_spec = [None if v in sig_videos else pgs_ref_stream for v in range(V)]
+    else:
+        pgs_spec = list(pgs_ref_stream)
+        if len(pgs_spec) != V:
+            raise ValueError("pgs_ref_stream has %d entries for %d paths" % (len(pgs_spec), V))
+    pgs_videos = [v for v in range(V) if pgs_spec[v] is not None]
+    sigs = [np.asarray(load_stored_speech(paths[v]), dtype=np.float64).ravel() for v in sig_videos]
+    sig_kw = {}
+    if sig_videos:
+        sig_kw = dict(sig=np.concatenate(sigs), sig_video=np.array(sig_videos, np.int64),
+                      sig_off=np.concatenate([[0], np.cumsum([len(x) for x in sigs])]).astype(np.int64))
+    # the combinations, checked before anything starts (PGS intervals stand empty here): the text videos that stay
+    empty = np.zeros(0)
+    pgs_stand = dict(pgs_start=empty, pgs_end=empty, pgs_off=np.zeros(len(pgs_videos) + 1, np.int64),
+                     pgs_video=np.array(pgs_videos, np.int64)) if pgs_videos else {}
+    refs, _, _, _ = sync._all_refs(V, dict(streams, **pgs_stand, **sig_kw), on_device=False,
+                                   seg=(np.array(seg_videos, np.int32),) if seg_videos else None)
+    text_videos = [] if refs is None else [int(v) for v in np.flatnonzero(refs[0])]
+    no_audio = set(sig_videos) | set(pgs_videos) | set(text_videos)
 
     def ffmpeg_args(path, start_seconds, duration):
         return VideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate, frame_rate=sync.frame_rate,
@@ -1168,10 +1251,16 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
                                       ffmpeg_path=ffmpeg_path, ref_stream=ref_stream,
                                       max_duration_seconds=duration)._build_ffmpeg_args(path)
 
-    # the decoder jobs: (video, segment or None, ffmpeg arguments); a segment video has one job per segment
+    # the decoder jobs: (video, segment or None, ffmpeg arguments); a segment video has one job per segment, a PGS video
+    # one probe job (video, _PGS_JOB, its PGSSpeechTransformer)
     is_seg = set(seg_videos)
     jobs = [(v, None, ffmpeg_args(paths[v], sync.start_seconds, max_duration_seconds)) for v in range(V)
-            if v not in is_seg]
+            if v not in is_seg and v not in no_audio]
+    for v in pgs_videos:
+        spec = None if pgs_spec[v] == "auto" else pgs_spec[v]
+        jobs.append((v, _PGS_JOB, PGSSpeechTransformer(sample_rate=sync.sample_rate, start_seconds=sync.start_seconds,
+                                                       ffmpeg_path=ffmpeg_path, ref_stream=spec)))
+    pgs_intervals = {}
     segments = None
     if seg_videos:
         mst = MultiSegmentVideoSpeechTransformer(vad=sync.detector, sample_rate=sync.sample_rate,
@@ -1188,8 +1277,9 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
         expect = np.zeros(V, dtype=np.int64) if expect_samples is None else np.array(expect_samples, dtype=np.int64)
         expect[seg_videos] = int(round(segment_duration * sync.frame_rate))   # the hint of each segment
         expect_samples = expect
-    if jobs and shutil.which(jobs[0][2][0]) is None:
-        raise ValueError("cannot decode media: no ffmpeg binary found at %r" % jobs[0][2][0])
+    decoders = [j for j in jobs if j[1] is not _PGS_JOB]
+    if decoders and shutil.which(decoders[0][2][0]) is None:
+        raise ValueError("cannot decode media: no ffmpeg binary found at %r" % decoders[0][2][0])
     n_read = detector_chunk_bytes(sync.frame_rate, sync.sample_rate)
     n_workers = max(1, min(int(max_decoders), len(jobs)))
     chunks: "queue.Queue" = queue.Queue(maxsize=2 * n_workers)
@@ -1198,8 +1288,25 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
         todo.put(job)
     stop = threading.Event()
 
+    def probe(job: int):
+        """A PGS video's display intervals (PGSSpeechTransformer.fit before its raster) into pgs_intervals."""
+        v, _, t = jobs[job]
+        intervals = t._probe_intervals(paths[v])
+        if not intervals:
+            given = t._given_stream()
+            raise ValueError("No subtitle timings found in PGS stream {}.".format(given) if given is not None
+                             else "No subtitle timings found in the PGS intervals given.")
+        pgs_intervals[v] = intervals
+
     def decode(job: int):
-        """Pushes job's 100 s reads to `chunks`; returns why it failed (None: it did not)."""
+        """Pushes job's 100 s reads to `chunks` (a PGS job: probes its intervals); returns why it failed (None: it
+        did not)."""
+        if jobs[job][1] is _PGS_JOB:   # a failed probe is the reference's ValueError, handed back as it is
+            try:
+                probe(job)
+            except ValueError as e:
+                return e
+            return None
         proc = subprocess.Popen(jobs[job][2], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL)
         try:
             while not stop.is_set():
@@ -1243,6 +1350,8 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
                     session.push_segment(v, seg, data)
                 continue
             left -= 1
+            if isinstance(err, Exception):
+                raise err
             if err and seg is not None:   # one bad window must not sink the sync (speech_transformers.py:878-882)
                 start = int(segments["seg_start"][int(segments["seg_off"][seg_videos.index(v)]) + seg])
                 logger.warning("failed to extract segment at %ds: %s", start, err)
@@ -1260,8 +1369,23 @@ def sync_media(paths, sync: BatchSynchronizer, track_video, cue_start, cue_end, 
         raise
     for t in threads:
         t.join()
+    pgs_kw = {}
+    if pgs_videos:
+        # a list the probe returns can still be one PGSSpeechTransformer.fit refuses (a non-finite or too large time):
+        # fit's own rasterisation raises the reference's ValueError for it, before the sync
+        try:
+            for v, seg, t in jobs:
+                if seg is _PGS_JOB:
+                    t.fit(pgs_intervals[v])
+        except BaseException:
+            session.abort()
+            raise
+        iv = [np.asarray(pgs_intervals[v], dtype=np.float64).reshape(-1, 2) for v in pgs_videos]
+        pgs_kw = dict(pgs_start=np.concatenate([x[:, 0] for x in iv]), pgs_end=np.concatenate([x[:, 1] for x in iv]),
+                      pgs_off=np.concatenate([[0], np.cumsum([len(x) for x in iv])]).astype(np.int64),
+                      pgs_video=np.array(pgs_videos, np.int64))
     return session.sync_tracks(track_video, cue_start, cue_end, cue_off, cue_keep, speech_video=speech_video,
-                               want_all=want_all)
+                               want_all=want_all, **streams, **pgs_kw, **sig_kw)
 
 
 def select_reference_streams(V: int, cue_start, cue_end, cue_off, stream_video, start_seconds: float = 0.0,

@@ -1037,6 +1037,36 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
                         p.max_end.data() + t0, r.max_offset_samples, go);
 }
 
+// The references of the videos [v0, v1) that no detector writes and no PCM feeds, from the call's host tables: the
+// signal videos' (sig_ref_kernel: floats, or in a packed sub-batch the bits the VAD would write; it also resets and
+// sets their flags) and the text and PGS videos' (rasterised into their ranges).  The last part of the detector step
+// of the whole calls and of the ingest session's sync alike.
+static int written_refs(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
+                        bool ref_packed) {
+  // the videos of `list` in [v0, v1), relative to v0
+  auto in_range = [&](const std::vector<int>& list) {
+    std::vector<int> rel(std::lower_bound(list.begin(), list.end(), v0), std::lower_bound(list.begin(), list.end(), v1));
+    for (int& v : rel) v -= v0;
+    return rel;
+  };
+  const std::vector<int> sig(std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v0),
+                             std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v1));
+  if (!sig.empty())
+    B2_TRY(b2i_sig_ref_launch(h, b.sigx, r.sig.off, p.ref_off.data(), r.V, sig.data(), (int)sig.size(), p.label,
+                              ref_packed, b.refsig, b.first_bad));
+  if (!p.any_subs) return B2_OK;
+  const std::vector<int> subs = in_range(p.sub_video), pgs = in_range(p.pgs_video);
+  if (!subs.empty())
+    B2_TRY(b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
+                                 p.ref_off.data() + v0, v1 - v0, subs.data(), (int)subs.size(), r.sample_rate,
+                                 r.start_seconds, b.refsig));
+  if (!pgs.empty())
+    B2_TRY(b2i_raster_ref_launch(h, r.pgs.start_s, r.pgs.end_s, nullptr, r.pgs.off + v0, p.ref_off.data() + v0,
+                                 v1 - v0, pgs.data(), (int)pgs.size(), r.sample_rate, r.start_seconds, b.refsig,
+                                 true));
+  return B2_OK;
+}
+
 // The detector step of the videos [v0, v1), on whichever stream the handle launches on: the energy / ZCR VAD
 // into the reference-signal buffer, or for auditok the energy pass over the videos' chunks (label 0, every
 // crossing count accepted, a short last block judged on its own samples) writing its 0/1 flags there, then
@@ -1054,23 +1084,28 @@ static int enqueue_chain(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, con
 // With sampled segments (b2_sync_tracks_seg) a segment video is empty in the main launch (plan det_end); a second
 // detector launch reads only its segments' samples into the scratch (floats), and seg_ref_kernel writes its reference
 // from there, floats or bits, and resets and sets its speech flag.
-// With ingested references (b2_ingest_sync_tracks) the detector already ran as the PCM arrived: the step copies the
-// audio videos' references from the session's buffer to their ranges, one copy per run of videos stored back to back,
-// and seg_ref_kernel assembles the segment videos' ones from their segments' frames there.
+// With ingested references (b2_ingest_sync_tracks / _refs) the detector already ran as the PCM arrived: the step copies
+// the audio videos' references from the session's buffer to their ranges, one copy per run of videos stored back to
+// back, seg_ref_kernel assembles the segment videos' ones from their segments' frames there, and the signal, text and
+// PGS videos' ones are written from the call's tables as in the whole call (written_refs).
 static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const SyncBufs& b, int v0, int v1,
                   bool ref_packed) {
   // the segment videos [s0, s1) of p.seg_video lie in [v0, v1)
   const int s0 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v0) - p.seg_video.begin());
   const int s1 = (int)(std::lower_bound(p.seg_video.begin(), p.seg_video.end(), v1) - p.seg_video.begin());
   if (r.ready.len) {
-    auto is_seg = [&](int v) { return !p.seg_of.empty() && p.seg_of[v] >= 0; };
+    // a video whose reference is not its pushes' (segments, text, PGS, signal): none of its frames is copied
+    auto not_audio = [&](int v) {
+      auto has = [v](const std::vector<int>& list) { return std::binary_search(list.begin(), list.end(), v); };
+      return (!p.seg_of.empty() && p.seg_of[v] >= 0) || has(p.sub_video) || has(p.pgs_video) || has(p.sig_video);
+    };
     for (int v = v0; v < v1;) {
-      if (is_seg(v)) {
+      if (not_audio(v)) {
         ++v;
         continue;
       }
       int w = v + 1;
-      while (w < v1 && !is_seg(w) && r.ready.at[w] == r.ready.at[w - 1] + r.ready.len[w - 1]) ++w;
+      while (w < v1 && !not_audio(w) && r.ready.at[w] == r.ready.at[w - 1] + r.ready.len[w - 1]) ++w;
       const int64_t n = p.ref_off[w] - p.ref_off[v];
       if (n > 0)
         B2_CUDA(h, cudaMemcpyAsync(b.refsig + p.ref_off[v], r.ready.ref + r.ready.at[v], (size_t)n * 4,
@@ -1082,7 +1117,7 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
       B2_TRY(b2i_seg_ref_launch(h, r.ready.ref, p.ref_off.data(), p.seg_video.data() + s0, s1 - s0,
                                 p.run_first.data() + s0, p.run_lo.data(), p.run_src.data(), ref_packed, b.refsig,
                                 b.speech));
-    return B2_OK;
+    return p.any_ref ? written_refs(h, r, p, b, v0, v1, ref_packed) : B2_OK;
   }
   const bool seg = !p.det_end.empty();
   if (!p.auditok && p.chunked) {   // energy / ZCR over the detector calls (never packed: plan_ref_format)
@@ -1113,17 +1148,6 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
                                        ch.tok_end.data() + k0));
   }
   if (!p.any_ref) return B2_OK;
-  // the videos of `list` in [v0, v1), relative to v0
-  auto in_range = [&](const std::vector<int>& list) {
-    std::vector<int> rel(std::lower_bound(list.begin(), list.end(), v0), std::lower_bound(list.begin(), list.end(), v1));
-    for (int& v : rel) v -= v0;
-    return rel;
-  };
-  const std::vector<int> sig(std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v0),
-                             std::lower_bound(p.sig_video.begin(), p.sig_video.end(), v1));
-  if (!sig.empty())
-    B2_TRY(b2i_sig_ref_launch(h, b.sigx, r.sig.off, p.ref_off.data(), r.V, sig.data(), (int)sig.size(), p.label,
-                              ref_packed, b.refsig, b.first_bad));
   if (s1 > s0) {
     const int k0 = p.item_first[v0], nk = p.item_first[v1] - k0;
     if (nk > 0 && !p.auditok) {
@@ -1140,17 +1164,7 @@ static int detect(b2_ctx* h, const SyncRequest& r, const SyncPlan& p, const Sync
                               p.run_first.data() + s0, p.run_lo.data(), p.run_src.data(), ref_packed, b.refsig,
                               b.speech));
   }
-  if (!p.any_subs) return B2_OK;
-  const std::vector<int> subs = in_range(p.sub_video), pgs = in_range(p.pgs_video);
-  if (!subs.empty())
-    B2_TRY(b2i_raster_ref_launch(h, r.refs.cue_start_s, r.refs.cue_end_s, r.refs.cue_keep, r.refs.cue_off + v0,
-                                 p.ref_off.data() + v0, v1 - v0, subs.data(), (int)subs.size(), r.sample_rate,
-                                 r.start_seconds, b.refsig));
-  if (!pgs.empty())
-    B2_TRY(b2i_raster_ref_launch(h, r.pgs.start_s, r.pgs.end_s, nullptr, r.pgs.off + v0, p.ref_off.data() + v0,
-                                 v1 - v0, pgs.data(), (int)pgs.size(), r.sample_rate, r.start_seconds, b.refsig,
-                                 true));
-  return B2_OK;
+  return written_refs(h, r, p, b, v0, v1, ref_packed);
 }
 
 // Software pipeline over the plan's sub-batches of videos (sync_plan.h plan_cuts).  The VAD (HBM-bound) of every
@@ -2072,27 +2086,47 @@ extern "C" int b2_ingest_abort(b2_handle h) {
   return B2_OK;
 }
 
-extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, int T, const double* cue_start_s,
-                                     const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
-                                     const double* ratios, int K, double start_seconds, int64_t max_offset_samples,
-                                     double* best_score, int32_t* best_offset, int32_t* best_k, double* all_score,
-                                     int32_t* all_offset, double* gss_ratio, double* gss_evals, int memspace) {
+// b2_ingest_sync_refs: the reference tables in the order b2_sync_tracks_sig takes them (any group may be NULL), then
+// b2_ingest_sync_tracks' arguments; b2_ingest_sync_tracks is this call with every table NULL.
+extern "C" int b2_ingest_sync_refs(b2_handle h, const uint8_t* ref_is_subs, const double* ref_cue_start_s,
+                                   const double* ref_cue_end_s, const uint8_t* ref_cue_keep, const int64_t* ref_cue_off,
+                                   const uint8_t* ref_is_pgs, const double* pgs_start_s, const double* pgs_end_s,
+                                   const int64_t* pgs_off, const uint8_t* ref_is_sig, const double* x,
+                                   const int64_t* sig_off, const int32_t* track_video, int T, const double* cue_start_s,
+                                   const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                   const double* ratios, int K, double start_seconds, int64_t max_offset_samples,
+                                   double* best_score, int32_t* best_offset, int32_t* best_k, double* all_score,
+                                   int32_t* all_offset, double* gss_ratio, double* gss_evals, int memspace) {
   B2_ENTER(h);
-  B2Range range("b2_ingest_sync_tracks");
+  B2Range range("b2_ingest_sync_refs");
+  const bool tables = ref_is_subs || ref_cue_off || ref_is_pgs || pgs_off || ref_is_sig || sig_off;
+  // b2_ingest_sync_tracks keeps its own name in its messages
+  const char* who = tables ? "ingest_sync_refs" : "ingest_sync_tracks";
   IngestSession* s = h->ingest;
-  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: no open session on this handle");
+  if (!s || !s->active) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: no open session on this handle", who);
   // the session closes whatever the outcome
   struct Close {
     b2_ctx* h;
     IngestSession* s;
     ~Close() { ingest_release_ref(h, s); }
   } close{h, s};
-  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: null track_video");
-  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: gss_evals without gss_ratio");
+  if (T > 0 && !track_video) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: null track_video", who);
+  if (!gss_ratio && gss_evals) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: gss_evals without gss_ratio", who);
   if (memspace != B2_HOST && memspace != B2_DEVICE)
-    B2_FAIL(h, B2_ERR_BAD_ARG, "ingest_sync_tracks: memspace must be B2_HOST or B2_DEVICE");
-  B2_TRY(ingest_enqueue(h, s, 0, nullptr, nullptr, nullptr, true));
+    B2_FAIL(h, B2_ERR_BAD_ARG, "%s: memspace must be B2_HOST or B2_DEVICE", who);
+  if (ref_is_subs && !ref_cue_off) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: ref_is_subs without ref_cue_off", who);
+  if (ref_is_pgs && !pgs_off) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: ref_is_pgs without pgs_off", who);
+  if (ref_is_sig && !sig_off) B2_FAIL(h, B2_ERR_BAD_ARG, "%s: ref_is_sig without sig_off", who);
   const int V = s->V;
+  SyncRequest r = s->req;
+  r.who = gss_ratio ? (tables ? "ingest_sync_refs (search)" : "ingest_sync_tracks (search)") : who;
+  r.refs = {ref_is_subs, ref_cue_start_s, ref_cue_end_s, ref_cue_keep, V > 0 ? ref_cue_off : nullptr};
+  r.pgs = {ref_is_pgs, pgs_start_s, pgs_end_s, V > 0 ? pgs_off : nullptr};
+  r.sig = {ref_is_sig, x, V > 0 ? sig_off : nullptr};
+  // a reference video has no audio: P_v must be empty (plan_refs_check compares pcm_off, all equal in a session)
+  r.V = V;
+  if (const int st = ingest_refs_check(r, &s->streams, s->plan)) B2_FAIL(h, st, "%s", s->streams.err.c_str());
+  B2_TRY(ingest_enqueue(h, s, 0, nullptr, nullptr, nullptr, true));
   std::vector<int64_t> pcm_off(V + 1, 0);
   // the live segments' table: b2_sync_tracks_seg's, its sample ranges empty (the detector's output is on the
   // device), each segment's frames in the session's buffer
@@ -2109,8 +2143,6 @@ extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, in
     seg_off.push_back((int64_t)seg_start.size());
   }
   const std::vector<int64_t> no_range(seg_start.size() + 1, 0);
-  SyncRequest r = s->req;
-  r.who = gss_ratio ? "ingest_sync_tracks (search)" : "ingest_sync_tracks";
   r.pcm = nullptr;
   r.pcm_off = pcm_off.data();
   r.V = V;
@@ -2137,6 +2169,17 @@ extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, in
   if (ss.declared)
     r.seg = {P, ss.video.data(), ss.total.data(), seg_off.data(), seg_start.data(), no_range.data(), no_range.data()};
   return sync_run(h, _b2_fence_was_valid, r);
+}
+
+extern "C" int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video, int T, const double* cue_start_s,
+                                     const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                     const double* ratios, int K, double start_seconds, int64_t max_offset_samples,
+                                     double* best_score, int32_t* best_offset, int32_t* best_k, double* all_score,
+                                     int32_t* all_offset, double* gss_ratio, double* gss_evals, int memspace) {
+  return b2_ingest_sync_refs(h, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                             nullptr, nullptr, nullptr, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off,
+                             ratios, K, start_seconds, max_offset_samples, best_score, best_offset, best_k, all_score,
+                             all_offset, gss_ratio, gss_evals, memspace);
 }
 
 // ---- try_sync's epilogue (sync_output.cu) ----------------------------------------------------------------------

@@ -234,3 +234,19 @@ struct IngestStreams {
  private:
   char buf_[256];
 };
+
+// b2_ingest_sync_refs: a video given a text, PGS or signal reference (r.refs / r.pgs / r.sig, read as plan_refs_check
+// reads them) has no audio, so its stream must have taken no bytes; plan_refs_check cannot tell, since a session's
+// pcm_off is all zeros.  B2_ERR_BAD_ARG with st->err naming the first such video.
+static int ingest_refs_check(const SyncRequest& r, IngestStreams* st, const IngestPlanner& pl) {
+  for (int v = 0; v < r.V; ++v) {
+    const bool is_subs = r.refs.cue_off && r.refs.is_subs && r.refs.is_subs[v];
+    const bool is_pgs = r.pgs.off && r.pgs.is_pgs && r.pgs.is_pgs[v];
+    const bool is_sig = r.sig.off && r.sig.is_sig && r.sig.is_sig[v];
+    if ((is_subs || is_pgs || is_sig) && pl.bytes[v] > 0)
+      B2_FAIL(st, B2_ERR_BAD_ARG, "%s: video %d has a %s reference and received %lld pushed bytes; its audio is never "
+              "read, so it takes no pushes", r.who, v, is_sig ? "serialized signal" : is_pgs ? "PGS" : "text subtitle",
+              (long long)pl.bytes[v]);
+  }
+  return B2_OK;
+}

@@ -589,10 +589,12 @@ static void plan_cuts(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p)
 // signal videos (their chains take the run path only at label 0, where the reference has the levels 1.0 and 0.0).
 static void plan_ref_format(const SyncRequest& r, const SyncPipeEnv& env, SyncPlan* p) {
   p->ref_packed.assign(p->n_sub, 0);
-  // ingested audio references are floats; the run path packs them itself (ref_bits_kernel).  Segment videos' ones
-  // are assembled at sync by seg_ref_kernel, which writes bits as it does for b2_sync_tracks_seg.
-  if ((r.ready.len && p->seg_video.size() < (size_t)r.V) || (p->auditok && p->sig_video.empty() && p->seg_video.empty()) || !env.fused ||
-      (env.ref_packed && atoi(env.ref_packed) == 0))
+  // ingested audio references are floats; the run path packs them itself (ref_bits_kernel).  Segment and signal
+  // videos' ones are written at sync by seg_ref_kernel and sig_ref_kernel, which write bits as they do for
+  // b2_sync_tracks_seg / _sig; text and PGS ones are rasterised as floats there as in the whole call.
+  const size_t n_written = p->seg_video.size() + p->sig_video.size();
+  if ((r.ready.len && n_written < (size_t)r.V) || (p->auditok && p->sig_video.empty() && p->seg_video.empty()) ||
+      !env.fused || (env.ref_packed && atoi(env.ref_packed) == 0))
     return;
   // how many videos of `list` lie in [v0, v1)
   auto count = [](const std::vector<int>& list, int v0, int v1) {
@@ -864,6 +866,49 @@ static void plan_segments(const SyncRequest& r, SyncPlan* p) {
   }
 }
 
+// The lengths of the videos whose reference is not the detector's, in (*subs_len)[v] (-1: a detector video), and the
+// lists sub_video, pgs_video and sig_video; the cue and interval times are checked on the way.
+static int plan_ref_lengths(const SyncRequest& r, SyncPlan* p, std::vector<int64_t>* subs_len) {
+  const char* who = r.who;
+  const int V = r.V;
+  // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
+  // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
+  // the tracks' cues).  (*subs_len)[v] = -1: the video's reference is the detector's.
+  // PGS references: int(max_end * sample_rate) + 2 frames, the length b2_rasterize_pgs_lengths gives.
+  // Signal references: one frame per stored value, sig_off[v+1] - sig_off[v].
+  subs_len->assign(V, -1);
+  const uint8_t* is_subs = r.refs.cue_off ? r.refs.is_subs : nullptr;
+  const uint8_t* is_pgs = r.pgs.off ? r.pgs.is_pgs : nullptr;
+  if (is_subs && std::any_of(is_subs, is_subs + V, [](uint8_t x) { return x != 0; })) {
+    const double one = 1.0;
+    B2_TRY(cue_lengths(&p->err, who, "reference ", "bad reference cue list", r.refs.cue_start_s, r.refs.cue_end_s,
+                       r.refs.cue_off, V, &one, 1, r.start_seconds, r.sample_rate, subs_len->data()));
+    for (int v = 0; v < V; ++v) {
+      if (is_subs[v]) p->sub_video.push_back(v);
+      else (*subs_len)[v] = -1;
+    }
+  }
+  if (is_pgs) {
+    std::vector<int64_t> pgs_len(V);
+    B2_TRY(pgs_lengths(&p->err, who, "PGS ", r.pgs.start_s, r.pgs.end_s, r.pgs.off, V, r.sample_rate, true,
+                       r.start_seconds, is_pgs, pgs_len.data()));
+    for (int v = 0; v < V; ++v)
+      if (is_pgs[v]) {
+        p->pgs_video.push_back(v);
+        (*subs_len)[v] = pgs_len[v];
+      }
+  }
+  if (r.sig.off && r.sig.is_sig)
+    for (int v = 0; v < V; ++v)
+      if (r.sig.is_sig[v]) {
+        p->sig_video.push_back(v);
+        (*subs_len)[v] = r.sig.off[v + 1] - r.sig.off[v];
+      }
+  // Segment references: int(total * sample_rate) + 2 frames (speech_transformers.py:871)
+  for (int v : p->seg_video) (*subs_len)[v] = seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate);
+  return B2_OK;
+}
+
 // The detector's window size and arguments, and each video's reference length.
 static int plan_references(const SyncRequest& r, SyncPlan* p) {
   const char* who = r.who;
@@ -889,52 +934,16 @@ static int plan_references(const SyncRequest& r, SyncPlan* p) {
   p->z_lo = r.energy.z_lo < 0 ? 0 : r.energy.z_lo;
   p->z_hi = r.energy.z_hi < 0 ? (3 * fpw) / 8 : r.energy.z_hi;
   p->ref_off.assign(V + 1, 0);
-  if (r.ready.len) {   // ingested references: their lengths are the pushes' (no chunk table, nothing to detect)
+  std::vector<int64_t> subs_len;   // [V] with any_ref: each reference video's length, -1 for a detector video
+  if (p->any_ref) B2_TRY(plan_ref_lengths(r, p, &subs_len));
+  if (r.ready.len) {
+    // ingested references: an audio video's length is the pushes' (no chunk table, nothing to detect), a text, PGS,
+    // signal or segment video's its reference's, as in the whole call (its ready.len is not read)
     for (int v = 0; v < V; ++v)
-      p->ref_off[v + 1] = p->ref_off[v] + (!p->seg_of.empty() && p->seg_of[v] >= 0
-                                               ? seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate)
-                                               : r.ready.len[v]);
+      p->ref_off[v + 1] = p->ref_off[v] + (p->any_ref && subs_len[v] >= 0 ? subs_len[v] : r.ready.len[v]);
     // segment videos: their runs point into the session's buffer, not into a scratch of this call
     if (!p->seg_video.empty()) plan_seg_runs(r, p, r.ready.seg_at, r.ready.seg_len);
     return B2_OK;
-  }
-  // subtitle references: int(max_end * sample_rate) + 2 frames (speech_transformers.py:958-962), the length
-  // b2_rasterize gives at ratio 1.0; the lengths pass checks the cue times too (the same checks and messages as
-  // the tracks' cues).  subs_len[v] = -1: the video's reference is the detector's.
-  // PGS references: int(max_end * sample_rate) + 2 frames, the length b2_rasterize_pgs_lengths gives.
-  // Signal references: one frame per stored value, sig_off[v+1] - sig_off[v].
-  std::vector<int64_t> subs_len;
-  if (p->any_ref) {
-    subs_len.assign(V, -1);
-    const uint8_t* is_subs = r.refs.cue_off ? r.refs.is_subs : nullptr;
-    const uint8_t* is_pgs = r.pgs.off ? r.pgs.is_pgs : nullptr;
-    if (is_subs && std::any_of(is_subs, is_subs + V, [](uint8_t x) { return x != 0; })) {
-      const double one = 1.0;
-      B2_TRY(cue_lengths(&p->err, who, "reference ", "bad reference cue list", r.refs.cue_start_s, r.refs.cue_end_s,
-                         r.refs.cue_off, V, &one, 1, r.start_seconds, r.sample_rate, subs_len.data()));
-      for (int v = 0; v < V; ++v) {
-        if (is_subs[v]) p->sub_video.push_back(v);
-        else subs_len[v] = -1;
-      }
-    }
-    if (is_pgs) {
-      std::vector<int64_t> pgs_len(V);
-      B2_TRY(pgs_lengths(&p->err, who, "PGS ", r.pgs.start_s, r.pgs.end_s, r.pgs.off, V, r.sample_rate, true,
-                         r.start_seconds, is_pgs, pgs_len.data()));
-      for (int v = 0; v < V; ++v)
-        if (is_pgs[v]) {
-          p->pgs_video.push_back(v);
-          subs_len[v] = pgs_len[v];
-        }
-    }
-    if (r.sig.off && r.sig.is_sig)
-      for (int v = 0; v < V; ++v)
-        if (r.sig.is_sig[v]) {
-          p->sig_video.push_back(v);
-          subs_len[v] = r.sig.off[v + 1] - r.sig.off[v];
-        }
-    // Segment references: int(total * sample_rate) + 2 frames (speech_transformers.py:871)
-    for (int v : p->seg_video) subs_len[v] = seg_ref_length(r.seg.total[p->seg_of[v]], r.sample_rate);
   }
   for (int v = 0; v < V; ++v) {
     const int64_t n = r.pcm_off[v + 1] - r.pcm_off[v];

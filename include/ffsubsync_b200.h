@@ -636,6 +636,27 @@ int b2_ingest_sync_tracks(b2_handle h, const int32_t* track_video /* [T] */, int
                           double* all_score, int32_t* all_offset /* [T*K], [T*(K+1)] with the search, or NULL */,
                           double* gss_ratio /* [T] or NULL = grid only */, double* gss_evals /* [T*17] or NULL */,
                           int memspace);
+/* b2_ingest_sync_refs  b2_ingest_sync_tracks with references that need no audio: the reference tables of
+ *                     b2_sync_tracks_sig, in its order (text streams ref_is_subs .. ref_cue_off, PGS intervals
+ *                     ref_is_pgs .. pgs_off, stored signals ref_is_sig, x, sig_off; each group may be NULL), then
+ *                     b2_ingest_sync_tracks' arguments.  A reference video has no pushes (empty P_v).  The call
+ *                     returns exactly what b2_sync_tracks_seg returns for the same tracks, arguments and tables over
+ *                     the PCM P_0 ... P_{V-1} back to back with the session's segment table (as b2_ingest_sync_tracks
+ *                     builds it): b2_speech_output, B2_BEST_K_BAD_SIGNAL, B2_BEST_K_NO_SPEECH, the label / level / path
+ *                     rules and their B2_ERR_UNSUPPORTED refusals included.  B2_ERR_BAD_ARG for a text, PGS or signal
+ *                     video that received pushed bytes (the message names it), for a segment video given a reference,
+ *                     and for every table refusal of b2_sync_tracks_sig / _seg.  memspace covers the outputs and x:
+ *                     B2_HOST stages a host x, B2_DEVICE refuses one.  The tables are host arrays.  The session closes
+ *                     whatever the outcome; b2_ingest_sync_tracks is this call with every table NULL. */
+int b2_ingest_sync_refs(b2_handle h, const uint8_t* ref_is_subs /* [V] or NULL */, const double* ref_cue_start_s,
+                        const double* ref_cue_end_s, const uint8_t* ref_cue_keep, const int64_t* ref_cue_off /* [V+1] */,
+                        const uint8_t* ref_is_pgs /* [V] or NULL */, const double* pgs_start_s, const double* pgs_end_s,
+                        const int64_t* pgs_off /* [V+1] */, const uint8_t* ref_is_sig /* [V] or NULL */,
+                        const double* x, const int64_t* sig_off /* [V+1] */, const int32_t* track_video /* [T] */,
+                        int T, const double* cue_start_s, const double* cue_end_s, const uint8_t* cue_keep,
+                        const int64_t* cue_off /* [T+1] */, const double* ratios, int K, double start_seconds,
+                        int64_t max_offset_samples, double* best_score, int32_t* best_offset, int32_t* best_k /* [T] */,
+                        double* all_score, int32_t* all_offset, double* gss_ratio, double* gss_evals, int memspace);
 int b2_ingest_abort(b2_handle h);
 
 /* ---- sampled segments in a session (--multi-segment-sync) ------------------------------------------------------
