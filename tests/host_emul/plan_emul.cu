@@ -156,6 +156,14 @@ int main(int argc, char** argv) {
   put("seg_video", p.seg_video);
   put("ref_packed", p.ref_packed);
   put("audio_samples", std::vector<int64_t>{p.audio_samples});
+  put("det_end", p.det_end);
+  put("item_start", p.item_start);
+  put("item_end", p.item_end);
+  put("item_out", p.item_out);
+  put("item_tail", p.item_tail);
+  put("item_first", p.item_first);
+  put("stage_lo", p.stage_lo);
+  put("stage_hi", p.stage_hi);
   fprintf(o, "two_level %d %.9g\n", (int)p.two_level, (double)p.ref_label);
   fclose(o);
   return 0;

@@ -131,7 +131,8 @@ def _exact_result(exact, ref, sub, mos):
 
 def _call(handle, req, a, pcm, memspace, want_all, resident=False, keep=None):
     """One call of the request's entry point; returns host numpy (bs, bo, bk, a_s, a_o[, gss_ratio, gss_evals]),
-    or with `resident` the device tensors, unsynchronised."""
+    or with `resident` the device tensors, unsynchronised.  pcm: host int16 samples, or (device calls) the int
+    address of device samples that a["pcm_off"] indexes."""
     import torch
     from ffsubsync_b200 import _native as N
     e, T, K = req["entry"], len(req["tracks"]), len(req["ratios"])
@@ -141,7 +142,7 @@ def _call(handle, req, a, pcm, memspace, want_all, resident=False, keep=None):
     x = a.get("x")
     outs, dev = {}, {}
     if ms != N.B2_HOST:
-        dev = dict(pcm=torch.from_numpy(pcm).cuda() if len(pcm) else None,
+        dev = dict(pcm=None if isinstance(pcm, int) else torch.from_numpy(pcm).cuda() if len(pcm) else None,
                    best_score=torch.full((T,), 7.0, dtype=torch.float64, device="cuda"),
                    best_offset=torch.full((T,), 7, dtype=torch.int32, device="cuda"),
                    best_k=torch.full((T,), 7, dtype=torch.int32, device="cuda"))
@@ -157,7 +158,8 @@ def _call(handle, req, a, pcm, memspace, want_all, resident=False, keep=None):
         torch.cuda.synchronize()
         outs = {k: v.data_ptr() for k, v in dev.items() if k not in ("x", "pcm")}
         x = dev["x"].data_ptr() if dev.get("x") is not None else None
-        pcm = dev["pcm"].data_ptr() if dev["pcm"] is not None else None
+        if not isinstance(pcm, int):
+            pcm = dev["pcm"].data_ptr() if dev["pcm"] is not None else None
         if keep is not None:   # the tensors outlive calls that nothing synchronises
             keep.append(dev)
     common = dict(memspace=ms, want_all=want_all, **outs)

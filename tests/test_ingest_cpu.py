@@ -78,7 +78,12 @@ def _random_ops(rng, V, fpw, chunk):
 def test_spans_tile_the_stream_at_window_and_call_boundaries(auditok, fpw, chunk, seed):
     rng = np.random.RandomState(seed * 101 + fpw + chunk)
     V = 4
-    ops = _random_ops(rng, V, fpw, chunk)
+    check_spans(V, fpw, auditok, chunk, _random_ops(rng, V, fpw, chunk))
+
+
+def check_spans(V, fpw, auditok, chunk, ops):
+    """Runs ops through the planner and checks every span and completed call it returns against the stream's
+    window and call grid."""
     per_op, frames, base = _run(V, fpw, auditok, chunk, ops)
     c = chunk   # energy / ZCR too: its calls where they do not divide into windows (b2_vad_call_samples)
     per_call = -(-c // fpw) if c > 0 else 0
