@@ -33,7 +33,7 @@ EXPORTS = [
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
     "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
     "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort", "b2_ingest_segments", "b2_ingest_push_segments",
-    "b2_ingest_drop_segment", "b2_ingest_sync_refs",
+    "b2_ingest_drop_segment", "b2_ingest_sync_refs", "b2_split_tracks", "b2_apply_split",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -155,6 +155,10 @@ def load() -> ctypes.CDLL:
         lib.b2_ingest_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
         lib.b2_ingest_push_segments.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp]
         lib.b2_ingest_drop_segment.argtypes = [_vp, ctypes.c_int, _i64]
+        lib.b2_split_tracks.argtypes = [_vp, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
+                                        _vp, ctypes.c_int, _f64, _i64, _f64, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_apply_split.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _f64, _vp, _vp,
+                                       _vp, ctypes.c_int]
         _lib = lib
         return lib
 
@@ -939,6 +943,52 @@ class Handle:
             int(suppress is not None), 0.0 if suppress is None else float(suppress), *[_ptr(o) for o in outs],
             memspace)
         self._check(st, "b2_apply_sync")
+        return outs
+
+    def split_tracks(self, ref, ref_is_f64: bool, ref_off, track_video, cue_start_s, cue_end_s, cue_keep, cue_off,
+                     ratio, sample_rate: int, start_seconds: float, max_offset_samples, split_penalty: float,
+                     outs=None, memspace: int = B2_HOST):
+        """b2_split_tracks: per-segment offsets of the T = len(cue_off) - 1 tracks.  ref (float64 when ref_is_f64, else
+        float32) follows memspace; everything else but the outputs is host metadata (ratio: NaN skips a track).
+        B2_HOST: returns numpy (cue_offset i32 [cues], n_segments i32 [T], split_score f64 [T]).  B2_DEVICE: outs holds
+        those three device pointers in that order; enqueued on the handle's stream, returns outs."""
+        ref_off, cue_off = _i64a(ref_off), _i64a(cue_off)
+        V, T = len(ref_off) - 1, len(cue_off) - 1
+        track_video = np.ascontiguousarray(track_video, dtype=np.int32)
+        ratio = np.ascontiguousarray(ratio, dtype=np.float64)
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        keep = None if cue_keep is None else np.ascontiguousarray(cue_keep, dtype=np.uint8)
+        if memspace == B2_HOST:
+            ref = np.ascontiguousarray(ref, dtype=np.float64 if ref_is_f64 else np.float32)
+            n = int(cue_off[-1]) if T >= 0 else 0
+            outs = (np.zeros(n, np.int32), np.zeros(max(T, 0), np.int32), np.zeros(max(T, 0), np.float64))
+        st = self.lib.b2_split_tracks(
+            self.h, _ptr(ref), int(bool(ref_is_f64)), _ptr(ref_off), V, _ptr(track_video), T, _ptr(cue_start_s),
+            _ptr(cue_end_s), _ptr(keep), _ptr(cue_off), _ptr(ratio), int(sample_rate), float(start_seconds),
+            _mask_width(max_offset_samples), float(split_penalty), *[_ptr(o) for o in outs], memspace)
+        self._check(st, "b2_split_tracks")
+        return outs
+
+    def apply_split(self, ratio, n_segments, cue_offset, cue_start_s, cue_end_s, cue_off, sample_rate: int,
+                    apply_offset_seconds: float = 0.0, outs=None, memspace: int = B2_HOST):
+        """b2_apply_split: the synced cue times with each cue's own offset.  n_segments / cue_offset follow memspace;
+        ratio and the cue tables are host arrays.  B2_HOST: returns numpy (synced_start_us, synced_end_us, status).
+        B2_DEVICE: outs holds those three device pointers; enqueued on the handle's stream, returns outs."""
+        cue_off = _i64a(cue_off)
+        T = len(cue_off) - 1
+        ratio = np.ascontiguousarray(ratio, dtype=np.float64)
+        cue_start_s = np.ascontiguousarray(cue_start_s, dtype=np.float64)
+        cue_end_s = np.ascontiguousarray(cue_end_s, dtype=np.float64)
+        if memspace == B2_HOST:
+            n_segments = np.ascontiguousarray(n_segments, dtype=np.int32)
+            cue_offset = np.ascontiguousarray(cue_offset, dtype=np.int32)
+            n = int(cue_off[-1]) if T >= 0 else 0
+            outs = (np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(T, 0), np.int32))
+        st = self.lib.b2_apply_split(self.h, _ptr(ratio), _ptr(n_segments), _ptr(cue_offset), T, _ptr(cue_start_s),
+                                     _ptr(cue_end_s), _ptr(cue_off), int(sample_rate), float(apply_offset_seconds),
+                                     *[_ptr(o) for o in outs], memspace)
+        self._check(st, "b2_apply_split")
         return outs
 
     @contextlib.contextmanager

@@ -874,6 +874,105 @@ class BatchSynchronizer:
                                     suppress_output_if_offset_less_than))
         return dict(zip(("synced_start_us", "synced_end_us", "offset_seconds", "scale", "status"), outs))
 
+    # -- per-segment offsets with a split penalty (b2_split_tracks, b2_apply_split) ---------------------------------
+    def split_ratios(self, best_k, gss_ratio=None) -> np.ndarray:
+        """Each track's ratio from a sync call's best_k (host arrays): ratios[best_k], gss_ratio for best_k == K with
+        the search, NaN (skipped) for a track without an alignment."""
+        best_k = np.asarray(best_k, dtype=np.int64)
+        K = len(self.ratios)
+        r = np.full(len(best_k), np.nan)
+        grid = (best_k >= 0) & (best_k < K)
+        r[grid] = self.ratios[best_k[grid]]
+        if self.gss and gss_ratio is not None:
+            g = best_k == K
+            r[g] = np.asarray(gss_ratio, dtype=np.float64)[g]
+        return r
+
+    @staticmethod
+    def _split_refs(speech_off, track_video, speech_video):
+        """The tracks' indices into the written signals: speech_video lists the videos the sync call wrote (None: video
+        i is signal i).  ValueError for a track whose video has no signal."""
+        track_video = np.asarray(track_video, dtype=np.int64)
+        P = len(speech_off) - 1
+        listed = np.arange(P) if speech_video is None else np.asarray(speech_video, dtype=np.int64)
+        pos = {int(v): i for i, v in enumerate(listed)}
+        missing = sorted({int(v) for v in track_video if int(v) not in pos})
+        if missing:
+            raise ValueError("split needs the reference signals of videos %s: call the sync with speech_video covering "
+                             "them" % missing)
+        return np.array([pos[int(v)] for v in track_video], dtype=np.int32)
+
+    def split_tracks(self, out, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
+                     speech_video=None) -> dict:
+        """Per-segment offsets (b2_split_tracks) over the results of a device sync call made with ``speech_video``
+        (``out`` carries ``speech`` / ``speech_off``; pass the same speech_video here, None when it listed videos
+        0 .. P-1): each track's cue runs are cut into segments with their own offsets, a change of offset costing
+        ``split_penalty`` (+inf: one offset per track, the sync call's).  The tracks, cues and ratio are the sync
+        call's (ratio from best_k / gss_ratio).  Waits for the sync call to read best_k (and gss_ratio) back into the ratio
+        list, then enqueues the split on the handle's stream without synchronising.  Returns CUDA tensors ``cue_offset`` i32 per cue,
+        ``n_segments`` i32 and ``split_score`` f64 per track, and the host ``ratio`` (NaN: skipped track).
+        Departures a caller should know: the wait for best_k above (b2_split_tracks takes the ratios as host metadata,
+        so that a bad ratio is refused before anything runs); a video whose reference has a third level is not an
+        error here (the device call cannot stop after its level scan without a synchronisation) but gives its tracks
+        ``n_segments == -1``, NaN and offsets 0, which apply_split marks FAILED - split_tracks_host raises instead; and a
+        track with more than 16 384 kept cues is refused even when its cues make fewer runs (each run holds one)."""
+        import torch
+        if "speech" not in out:
+            raise ValueError("split_tracks needs the sync call's reference signals: call it with speech_video")
+        idx = self._split_refs(out["speech_off"], track_video, speech_video)
+        self.handle.synchronize()   # best_k is written on the handle's stream, which need not be torch's
+        ratio = self.split_ratios(out["best_k"].cpu().numpy(),
+                                  out["gss_ratio"].cpu().numpy() if self.gss else None)
+        dev = out["speech"].device
+        n, T = int(np.asarray(cue_off)[-1]), len(cue_off) - 1
+        res = {"cue_offset": torch.empty(max(n, 1), dtype=torch.int32, device=dev),
+               "n_segments": torch.empty(max(T, 1), dtype=torch.int32, device=dev),
+               "split_score": torch.empty(max(T, 1), dtype=torch.float64, device=dev)}
+        self.handle.split_tracks(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep,
+                                 cue_off, ratio, self.sample_rate, self.start_seconds, self.max_offset_samples,
+                                 split_penalty, outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
+        res = {"cue_offset": res["cue_offset"][:n], "n_segments": res["n_segments"][:T],
+               "split_score": res["split_score"][:T], "ratio": ratio}
+        return res
+
+    def split_tracks_host(self, res, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
+                          speech_video=None) -> dict:
+        """split_tracks over the tuple of a host sync call made with speech_video (best_score, best_offset, best_k
+        first, gss_ratio before the trailing (speech, speech_off) with the search).  Blocks; numpy results.  A reference
+        with a third level raises (NativeError, B2_ERR_UNSUPPORTED, naming the video and frame); more than 16 384 kept
+        cues in a track too."""
+        speech, speech_off = res[-2], res[-1]
+        idx = self._split_refs(speech_off, track_video, speech_video)
+        ratio = self.split_ratios(res[2], res[-3] if self.gss else None)
+        co, ns, sc = self.handle.split_tracks(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off,
+                                              ratio, self.sample_rate, self.start_seconds, self.max_offset_samples,
+                                              split_penalty, memspace=_native.B2_HOST)
+        return {"cue_offset": co, "n_segments": ns, "split_score": sc, "ratio": ratio}
+
+    def apply_split(self, split, cue_start, cue_end, cue_off, *,
+                    apply_offset_seconds: float = DEFAULT_APPLY_OFFSET_SECONDS) -> dict:
+        """try_sync's output step with each cue's own offset (b2_apply_split) over the dict split_tracks returned.
+        Enqueues one kernel without synchronising; returns CUDA tensors ``synced_start_us`` / ``synced_end_us`` int64
+        per cue and ``status`` i32 per track (WRITTEN | APPLIED, or FAILED for a skipped track)."""
+        import torch
+        dev = split["n_segments"].device
+        n, T = int(np.asarray(cue_off)[-1]), len(cue_off) - 1
+        res = {"synced_start_us": torch.empty(max(n, 1), dtype=torch.int64, device=dev),
+               "synced_end_us": torch.empty(max(n, 1), dtype=torch.int64, device=dev),
+               "status": torch.empty(max(T, 1), dtype=torch.int32, device=dev)}
+        self.handle.apply_split(split["ratio"], split["n_segments"].data_ptr(), split["cue_offset"].data_ptr(),
+                                cue_start, cue_end, cue_off, self.sample_rate, apply_offset_seconds,
+                                outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
+        return {"synced_start_us": res["synced_start_us"][:n], "synced_end_us": res["synced_end_us"][:n],
+                "status": res["status"][:T]}
+
+    def apply_split_host(self, split, cue_start, cue_end, cue_off, *,
+                         apply_offset_seconds: float = DEFAULT_APPLY_OFFSET_SECONDS) -> dict:
+        """apply_split over the numpy dict split_tracks_host returned.  Blocks; numpy results."""
+        outs = self.handle.apply_split(split["ratio"], split["n_segments"], split["cue_offset"], cue_start, cue_end,
+                                       cue_off, self.sample_rate, apply_offset_seconds, memspace=_native.B2_HOST)
+        return dict(zip(("synced_start_us", "synced_end_us", "status"), outs))
+
     def _gss_compose(self, pcm, pcm_off, track_video, cue_start, cue_end, cue_off, cue_keep=None, want_all=False,
                      refs=None, pgs=None, sig=None, seg=None, speech=None):
         """The golden-section search outside the envelope of the device-driven search, composed of public steps:

@@ -2264,3 +2264,135 @@ extern "C" int b2_apply_sync(b2_handle h, const double* best_score, const int32_
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
 }
+
+// ---- per-segment offsets with a split penalty (split.cu, sync_output.cu) ---------------------------------------
+extern "C" int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                               const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
+                               const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
+                               double start_seconds, int64_t max_offset_samples, double split_penalty,
+                               int32_t* cue_offset, int32_t* n_segments, double* split_score, int memspace) {
+  B2_ENTER(h);
+  if (V < 0 || T < 0 || !ref_off || !cue_off || (T && (!track_video || !ratio)))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "split: bad arguments (V %d, T %d, null table)", V, T);
+  if (memspace != B2_HOST && memspace != B2_DEVICE) B2_FAIL(h, B2_ERR_BAD_ARG, "split: memspace must be B2_HOST or B2_DEVICE");
+  if (std::isnan(split_penalty) || split_penalty < 0)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "split: split_penalty %g must be >= 0 (+inf: no splits)", split_penalty);
+  if (sample_rate <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: sample_rate %d <= 0", sample_rate);
+  if (ref_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: ref_off[0] %lld < 0", (long long)ref_off[0]);
+  for (int v = 0; v < V; ++v) {
+    if (ref_off[v + 1] < ref_off[v]) B2_FAIL(h, B2_ERR_BAD_ARG, "split: ref_off not monotone at video %d", v);
+    if (ref_off[v + 1] - ref_off[v] > 0x3fffffff)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "split: video %d: reference of %lld frames (at most 2^30 - 1)", v,
+              (long long)(ref_off[v + 1] - ref_off[v]));
+  }
+  if (cue_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: cue_off[0] %lld < 0", (long long)cue_off[0]);
+  for (int t = 0; t < T; ++t) {
+    if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "split: cue_off not monotone at track %d", t);
+    if (track_video[t] < 0 || track_video[t] >= V)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "split: track %d: video %d is outside [0, %d)", t, track_video[t], V);
+    if (!std::isnan(ratio[t]) && !ratio_ok(ratio[t]))
+      B2_FAIL(h, B2_ERR_BAD_ARG, "split: track %d: ratio %g is not a finite positive number (NaN skips)", t, ratio[t]);
+  }
+  if (T == 0) return B2_OK;
+  const int64_t c0 = cue_off[0], n = cue_off[T] - c0;
+  if (n && (!cue_start_s || !cue_end_s)) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null cue times");
+  if (!n_segments || !split_score || (n && !cue_offset)) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null output");
+  if (ref_off[V] > ref_off[0] && !ref) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null ref");
+  // the masks' lengths at each track's ratio (skipped tracks at 1.0), every cue time checked as b2_rasterize does
+  std::vector<double> r1(T);
+  for (int t = 0; t < T; ++t) r1[t] = std::isnan(ratio[t]) ? 1.0 : ratio[t];
+  std::vector<int64_t> len(T);
+  if (!(fabs(start_seconds) < B2_MAX_CUE_SECONDS) ||
+      rasterize_lengths(cue_start_s, cue_end_s, cue_off, T, r1.data(), 1, 1, sample_rate, len.data()) != B2_OK) {
+    int64_t at;
+    double val;
+    const char* why = bad_cue_input(cue_start_s, cue_end_s, cue_off, T, r1.data(), 1, 1, start_seconds, &at, &val);
+    B2_FAIL(h, B2_ERR_BAD_ARG, "split: %s (index %lld: %g)", why ? why : "bad cue list", (long long)at, val);
+  }
+  for (int t = 0; t < T; ++t)
+    if (len[t] > 0x3fffffff) B2_FAIL(h, B2_ERR_BAD_ARG, "split: track %d: mask of %lld frames", t, (long long)len[t]);
+  B2_CHECK_DEV(h, memspace, ref, "split: ref");
+  B2_CHECK_DEV(h, memspace, cue_offset, "split: cue_offset");
+  B2_CHECK_DEV(h, memspace, n_segments, "split: n_segments");
+  B2_CHECK_DEV(h, memspace, split_score, "split: split_score");
+  const size_t esz = ref_is_f64 ? 8 : 4;
+  if (memspace == B2_DEVICE)
+    return b2i_split_launch(h, ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
+                            cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
+                            false, nullptr, false, cue_offset, n_segments, split_score);
+  // B2_HOST: the reference staged in, outputs through the staging workspace (cue outputs at their absolute indices)
+  void *d_ref, *dout;
+  B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, ref, (size_t)ref_off[V] * esz, &d_ref));
+  const size_t Ts = (size_t)T;
+  B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_OUT, Ts * 12 + (size_t)n * 4 + 64, &dout));
+  double* d_sc = (double*)dout;
+  int32_t* d_ns = (int32_t*)(d_sc + Ts);
+  int32_t* d_co = d_ns + Ts;
+  B2_TRY(b2i_split_launch(h, d_ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
+                          cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
+                          true, ref, ref_is_f64 != 0, d_co - c0, d_ns, d_sc));
+  B2_TRY(copy_out(h, cue_offset + c0, d_co, (size_t)n * 4));
+  B2_TRY(copy_out(h, n_segments, d_ns, Ts * 4));
+  B2_TRY(copy_out(h, split_score, d_sc, Ts * 8));
+  B2_CUDA(h, cudaStreamSynchronize(h->stream));
+  return B2_OK;
+}
+
+extern "C" int b2_apply_split(b2_handle h, const double* ratio, const int32_t* n_segments, const int32_t* cue_offset,
+                              int T, const double* cue_start_s, const double* cue_end_s, const int64_t* cue_off,
+                              int sample_rate, double apply_offset_seconds, int64_t* synced_start_us,
+                              int64_t* synced_end_us, int32_t* status, int memspace) {
+  // Not B2_ENTER, as b2_apply_sync: a chain of resident sync calls stays valid across it
+  if (!h) return B2_ERR_BAD_ARG;
+  h->err.clear();
+  DeviceScope scope(h->device);
+  if (!scope.ok) return B2_ERR_CUDA;
+  if (T < 0 || !cue_off || (T && !ratio)) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: bad arguments (T %d)", T);
+  if (sample_rate <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: sample_rate %d <= 0", sample_rate);
+  if (!std::isfinite(apply_offset_seconds))
+    B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: apply_offset_seconds %g is not finite", apply_offset_seconds);
+  if (T == 0) return B2_OK;
+  if (!n_segments || !status) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: null n_segments / status");
+  if (cue_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: cue_off[0] %lld < 0", (long long)cue_off[0]);
+  double smax = 1.0;
+  for (int t = 0; t < T; ++t) {
+    if (cue_off[t + 1] < cue_off[t]) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: cue_off not monotone at track %d", t);
+    if (!std::isnan(ratio[t]) && !ratio_ok(ratio[t]))
+      B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: track %d: ratio %g is not a finite positive number", t, ratio[t]);
+    if (!std::isnan(ratio[t])) smax = std::max(smax, ratio[t]);
+  }
+  const int64_t c0 = cue_off[0], n = cue_off[T] - c0;
+  if (n && (!cue_start_s || !cue_end_s || !cue_offset)) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: null cue input");
+  if (n && (!synced_start_us || !synced_end_us)) B2_FAIL(h, B2_ERR_BAD_ARG, "apply_split: null synced_start_us / end_us");
+  // as b2_apply_sync: every output time is at most |t| * smax + 2^31 / sample_rate + |apply| in magnitude
+  const double t_max = (B2_MAX_CUE_SECONDS - 2147483648.0 / sample_rate - fabs(apply_offset_seconds)) / smax;
+  B2_CHECK_DEV(h, memspace, n_segments, "apply_split: n_segments");
+  B2_CHECK_DEV(h, memspace, status, "apply_split: status");
+  if (n) {
+    B2_CHECK_DEV(h, memspace, cue_offset, "apply_split: cue_offset");
+    B2_CHECK_DEV(h, memspace, synced_start_us, "apply_split: synced_start_us");
+    B2_CHECK_DEV(h, memspace, synced_end_us, "apply_split: synced_end_us");
+  }
+  const B2SyncRule rule = b2_sync_rule(sample_rate, apply_offset_seconds, 0, 0.0, 0.0, 0.0, 0, 0.0);
+  if (memspace == B2_DEVICE)
+    return b2i_apply_split_launch(h, ratio, n_segments, cue_offset, T, cue_start_s, cue_end_s, cue_off, t_max, rule,
+                                  synced_start_us, synced_end_us, status);
+  void *din, *dout;
+  const size_t Ts = (size_t)T;
+  B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_IN0, Ts * 4 + (size_t)n * 4 + 64, &din));
+  B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_OUT, (size_t)n * 16 + Ts * 4 + 64, &dout));
+  int32_t* d_ns = (int32_t*)din;
+  int32_t* d_co = d_ns + Ts;
+  B2_CUDA(h, cudaMemcpyAsync(d_ns, n_segments, Ts * 4, cudaMemcpyHostToDevice, h->stream));
+  if (n) B2_CUDA(h, cudaMemcpyAsync(d_co, cue_offset + c0, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
+  int64_t* d_su = (int64_t*)dout;
+  int64_t* d_eu = d_su + n;
+  int32_t* d_st = (int32_t*)(d_eu + n);
+  B2_TRY(b2i_apply_split_launch(h, ratio, d_ns, d_co - c0, T, cue_start_s, cue_end_s, cue_off, t_max, rule, d_su - c0,
+                                d_eu - c0, d_st));
+  B2_TRY(copy_out(h, synced_start_us + c0, d_su, (size_t)n * 8));
+  B2_TRY(copy_out(h, synced_end_us + c0, d_eu, (size_t)n * 8));
+  B2_TRY(copy_out(h, status, d_st, Ts * 4));
+  B2_CUDA(h, cudaStreamSynchronize(h->stream));
+  return B2_OK;
+}

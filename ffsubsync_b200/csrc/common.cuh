@@ -82,7 +82,7 @@ struct b2_ctx {
   // named grow-only workspaces
   enum { WS_STAGE_IN0, WS_STAGE_IN1, WS_STAGE_OUT, WS_META, WS_SPEC, WS_SCORES, WS_CAND,
          WS_SIG_REF, WS_SIG_REF2, WS_SIG_SUB, WS_MISC, WS_COUNTERS, WS_RUNS, WS_GSS, WS_GSS_OUT, WS_STAGE_SIG,
-         WS_SPEECH, WS_COUNT };
+         WS_SPEECH, WS_SPLIT, WS_COUNT };
   DeviceBuf ws[WS_COUNT];
   HostBuf pinned[4];
   cudaEvent_t pinned_ev[4] = {};   // recorded after the last async copy out of pinned[i]
@@ -342,3 +342,20 @@ int b2i_apply_sync_launch(b2_ctx* h, const double* d_bs, const int32_t* d_bo, co
                           const int64_t* cue_off, double t_max, const double* ratios, int K, const B2SyncRule& rule,
                           int64_t* d_start_us, int64_t* d_end_us, double* d_offset_seconds, double* d_scale,
                           int32_t* d_status);
+// Per-segment offsets of b2_split_tracks (K9s, split.cu) for T tracks against the reference frames d_ref (float64 when
+// ref_f64, else float32; DEVICE) of V videos at the HOST offsets ref_off [V+1].  Host arrays: track_video, the cue
+// lists (cue_off [T+1] absolute, also into d_cue_offset), ratio [T] (NaN = skipped) and len [T] (each track's mask
+// length at its ratio).  The caller has checked every argument.  refuse_three_levels: synchronise after the reference
+// scan and fail with B2_ERR_UNSUPPORTED for a video with a third level (h_ref: its host frames for the message, float64
+// when h_ref_f64, or null); otherwise that video's tracks get n_segments = -1.  Everything else is enqueued without a synchronisation.
+int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
+                     const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
+                     const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
+                     int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
+                     bool refuse_three_levels, const void* h_ref, bool h_ref_f64, int* d_cue_offset, int* d_n_segments,
+                     double* d_split_score);
+// b2_apply_split's kernel (sync_output.cu): n_segments / cue_offset / the outputs are DEVICE arrays, ratio [T] and the
+// cue tables HOST arrays (absolute cue indices, as for b2i_apply_sync_launch).
+int b2i_apply_split_launch(b2_ctx* h, const double* ratio, const int32_t* d_n_segments, const int32_t* d_cue_offset,
+                           int T, const double* cue_start, const double* cue_end, const int64_t* cue_off, double t_max,
+                           const B2SyncRule& rule, int64_t* d_start_us, int64_t* d_end_us, int32_t* d_status);

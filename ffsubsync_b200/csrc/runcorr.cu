@@ -30,35 +30,6 @@ struct RunStat {       // one (track, ratio) job of run_corr_kernel
   int arg;             // largest offset attaining mx
 };
 
-// Exclusive prefix sum over the CTA (blockDim.x a multiple of 32); *total = the sum.  sh: 33 ints.
-__device__ __forceinline__ int block_excl_scan(int v, int* sh, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, d);
-    if (lane >= d) x += y;
-  }
-  if (lane == 31) sh[warp] = x;
-  __syncthreads();
-  if (warp == 0) {
-    int s = lane < nw ? sh[lane] : 0;
-    const int own = s;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, s, d);
-      if (lane >= d) s += y;
-    }
-    sh[lane] = s - own;
-    if (lane == 31) sh[32] = s;
-  }
-  __syncthreads();
-  const int r = sh[warp] + x - v;
-  *total = sh[32];
-  __syncthreads();  // sh is reused by the next call
-  return r;
-}
-
 // Reference bits of one video per CTA: m = (r == 1.0f), packed 32 to a word with the count of the bits
 // below each word (rc_ref_entries layout: a zero guard word before, zero words up to index (R >> 5) + 1).
 // A warp turns 32 x 32 consecutive floats into 32 words with ballots (coalesced loads).
@@ -89,7 +60,7 @@ __global__ void __launch_bounds__(1024) ref_bits_kernel(const float* __restrict_
     }
     const int w = wb + lane;
     int tot;
-    const int ex = block_excl_scan(__popc(mine), sh, &tot);
+    const int ex = rc_block_excl_scan(__popc(mine), sh, &tot);
     if (w < n_words) q[w + 1] = make_uint2(mine, (uint32_t)(carry + ex));
     carry += tot;
   }
@@ -112,7 +83,7 @@ __global__ void __launch_bounds__(1024) ref_words_scan_kernel(const uint32_t* __
     const int w = w0 + threadIdx.x;
     const uint32_t mine = w < n_in ? __ldg(r + w) : 0u;
     int tot;
-    const int ex = block_excl_scan(__popc(mine), sh, &tot);
+    const int ex = rc_block_excl_scan(__popc(mine), sh, &tot);
     if (w < n_words) q[w + 1] = make_uint2(mine, (uint32_t)(carry + ex));
     carry += tot;
   }
@@ -161,34 +132,14 @@ __global__ void __launch_bounds__(kMaxThreads) run_corr_kernel(const SelJob* __r
   const int R = job.R, S = job.S;
   const uint32_t* bits = sub_bits + job.bits_off;
   // 1. runs of the mask: transitions at e in [0, S] (frames < 0 and >= S count as 0), in order
-  const int nws = S >> 5;
-  int n_end = 0;
-  for (int w0 = 0; w0 <= nws; w0 += nthr) {
-    const int w = w0 + tid;
-    uint32_t t = 0;
-    if (w <= nws) {
-      const int nb = S - 32 * w;  // valid bits of word w (> 0 except for w = S/32 when S % 32 == 0)
-      const uint32_t x = nb >= 32 ? __ldg(bits + w) : (nb > 0 ? __ldg(bits + w) & ((1u << nb) - 1u) : 0u);
-      const uint32_t prev = w > 0 ? __ldg(bits + w - 1) : 0u;  // word w-1 lies wholly below S
-      t = x ^ ((x << 1) | (prev >> 31));
-    }
-    int tot;
-    int idx = n_end + block_excl_scan(__popc(t), sh, &tot);
-    while (t) {
-      const int e = 32 * w + __ffs(t) - 1;
-      t &= t - 1;
-      if (idx < 2 * max_runs) (idx & 1 ? rb : ra)[idx >> 1] = e;
-      ++idx;
-    }
-    n_end += tot;
-  }
+  const int n_end = rc_decode_runs(bits, S, max_runs, ra, rb, sh);
   const int nr = min(n_end >> 1, max_runs);  // a run holds at least one cue: never cut here
   __syncthreads();
   for (int r0 = 0, carry = 0; r0 < nr; r0 += nthr) {
     const int r = r0 + tid;
     const int len = r < nr ? rb[r] - ra[r] : 0;
     int tot;
-    const int ex = block_excl_scan(len, sh, &tot);
+    const int ex = rc_block_excl_scan(len, sh, &tot);
     if (r < nr) rl[r] = carry + ex;
     carry += tot;
   }
@@ -258,7 +209,7 @@ __global__ void __launch_bounds__(kMaxThreads) run_corr_kernel(const SelJob* __r
   }
   int total;
   const int h = __popc(hit);
-  int rank = block_excl_scan(h, sh, &total);
+  int rank = rc_block_excl_scan(h, sh, &total);
   rank = total - rank - h;  // hits at larger offsets (higher threads)
   while (hit && rank < kCandMax) {
     const int i = 31 - __clz(hit);

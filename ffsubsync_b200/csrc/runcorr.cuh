@@ -155,6 +155,67 @@ RC_HD double rc_score(const uint2* q, int R, int S, const int* ra, const int* rb
   return (l.hi * c11 - c01) + (l.hia * c10 - l.alpha * c00);
 }
 
+#ifdef __CUDACC__
+// Exclusive prefix sum over the CTA (blockDim.x a multiple of 32); *total = the sum.  sh: 33 ints.
+__device__ __forceinline__ int rc_block_excl_scan(int v, int* sh, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, d);
+    if (lane >= d) x += y;
+  }
+  if (lane == 31) sh[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int s = lane < nw ? sh[lane] : 0;
+    const int own = s;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, s, d);
+      if (lane >= d) s += y;
+    }
+    sh[lane] = s - own;
+    if (lane == 31) sh[32] = s;
+  }
+  __syncthreads();
+  const int r = sh[warp] + x - v;
+  *total = sh[32];
+  __syncthreads();  // sh is reused by the next call
+  return r;
+}
+
+// The runs of an S-frame mask (bit i of bits = frame i): transitions at e in [0, S] (frames < 0 and >= S count
+// as 0), in order, the first max_runs runs to ra[r] (start) / rb[r] (end).  Returns the number of transitions
+// (twice the number of runs); the caller synchronises before reading ra / rb.
+__device__ __forceinline__ int rc_decode_runs(const uint32_t* __restrict__ bits, int S, int max_runs, int* ra,
+                                              int* rb, int* sh) {
+  const int tid = threadIdx.x, nthr = blockDim.x;
+  const int nws = S >> 5;
+  int n_end = 0;
+  for (int w0 = 0; w0 <= nws; w0 += nthr) {
+    const int w = w0 + tid;
+    uint32_t t = 0;
+    if (w <= nws) {
+      const int nb = S - 32 * w;  // valid bits of word w (> 0 except for w = S/32 when S % 32 == 0)
+      const uint32_t x = nb >= 32 ? __ldg(bits + w) : (nb > 0 ? __ldg(bits + w) & ((1u << nb) - 1u) : 0u);
+      const uint32_t prev = w > 0 ? __ldg(bits + w - 1) : 0u;  // word w-1 lies wholly below S
+      t = x ^ ((x << 1) | (prev >> 31));
+    }
+    int tot;
+    int idx = n_end + rc_block_excl_scan(__popc(t), sh, &tot);
+    while (t) {
+      const int e = 32 * w + __ffs(t) - 1;
+      t &= t - 1;
+      if (idx < 2 * max_runs) (idx & 1 ? rb : ra)[idx >> 1] = e;
+      ++idx;
+    }
+    n_end += tot;
+  }
+  return n_end;
+}
+#endif
+
 // Nomination margin epsilon of a job whose overlaps have at most n frames (n = min(R, S)).  With
 // c = max|s'| * max|r'| and u = 2^-53:
 //   rescore_kernel's float64 sum (fma per term, exact products, summation depth <= n + 25 including the

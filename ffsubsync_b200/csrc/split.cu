@@ -1,0 +1,403 @@
+// K9s: per-segment offsets with a split penalty over the reference signals of a finished batched sync call
+// (b2_split_tracks; objective and arithmetic in split.cuh, DESIGN.md section 4 "K9s").  The chain, all on the
+// handle's stream: split_ref_kernel (each video's two levels and its packed bits) -> raster_bits_kernel (the
+// tracks' masks at their own ratios) -> per track group split_dp_kernel (the programme, one CTA per track, a
+// switch word per unit and thread to the workspace) -> split_backtrack_kernel (the path, its score and the
+// per-cue offsets).
+#include <limits.h>
+#include <math.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+#include "job_plan.cuh"
+#include "split.cuh"
+
+using namespace split;
+
+namespace {
+
+struct SplitVideo {
+  long long ref_off;   // element offset of its frames
+  long long q_off;     // entry offset of its packed bits (rc_ref_entries(R) entries)
+  int R;
+};
+
+struct SplitLevel {
+  double beta;         // the level other than 1.0 (0.0 when every frame is 1.0)
+  long long bad;       // first frame with a third level (or a non-finite beta), -1 if none
+};
+
+struct SplitTrack {
+  long long q_off, bits_off, unit_base, dec_base;
+  long long c0, c1;    // cue range, relative to the uploaded cue arrays
+  double ratio;
+  float level;
+  int vid;             // index into the prepared videos
+  int R, S, o_lo, W, nthr, live;
+};
+
+// One CTA per video: beta = the first frame != 1.0, the first frame that is neither 1.0 nor beta, and the
+// run path's packed table (rc_ref_entries layout) of m = (r == 1.0), 32 x 32 frames per warp with ballots.
+template <typename T>
+__global__ void __launch_bounds__(1024) split_ref_kernel(const T* __restrict__ ref, const SplitVideo* __restrict__ vids,
+                                                         uint2* __restrict__ q_all, SplitLevel* __restrict__ lvl) {
+  __shared__ int sh[33];
+  __shared__ int s_first, s_bad;
+  const SplitVideo v = vids[blockIdx.x];
+  const T* r = ref + v.ref_off;
+  uint2* q = q_all + v.q_off;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    s_first = INT_MAX;
+    s_bad = INT_MAX;
+    q[0] = make_uint2(0u, 0u);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < v.R; i += blockDim.x)
+    if ((double)r[i] != 1.0) {  // a thread's first hit is its smallest
+      atomicMin(&s_first, i);
+      break;
+    }
+  __syncthreads();
+  const double beta = s_first < v.R ? (double)r[s_first] : 0.0;
+  if (threadIdx.x == 0 && s_first < v.R && !isfinite(beta)) atomicMin(&s_bad, s_first);
+  const int n_words = (v.R >> 5) + 2;  // words 0 .. (R >> 5) + 1
+  int carry = 0;
+  for (int w0 = 0; w0 < n_words; w0 += blockDim.x) {
+    const int wb = w0 + 32 * warp;  // this warp's 32 words
+    uint32_t mine = 0;
+#pragma unroll 4
+    for (int u = 0; u < 32; ++u) {
+      const long long i = 32LL * (wb + u) + lane;
+      const double x = i < v.R ? (double)__ldg(r + i) : 0.0;
+      if (i < v.R && x != 1.0 && x != beta) atomicMin(&s_bad, (int)i);
+      const uint32_t bal = __ballot_sync(0xffffffffu, i < v.R && x == 1.0);
+      if (lane == u) mine = bal;
+    }
+    const int w = wb + lane;
+    int tot;
+    const int ex = runcorr::rc_block_excl_scan(__popc(mine), sh, &tot);
+    if (w < n_words) q[w + 1] = make_uint2(mine, (uint32_t)(carry + ex));
+    carry += tot;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) lvl[blockIdx.x] = SplitLevel{beta, s_bad < v.R ? (long long)s_bad : -1LL};
+}
+
+// One CTA per track of the group: thread t owns the offsets o_lo + 32 t .. + 31.  Dynamic shared memory: 2 x
+// max_runs ints (run starts, ends).  Per unit j >= 1 each thread writes its switch word to
+// dec[dec_base + j * nthr + t], thread 0 the unit's argmax to arg[unit_base + j]; the runs go to runs[unit_base + r].
+template <int MAXT>
+__global__ void __launch_bounds__(MAXT) split_dp_kernel(const SplitTrack* __restrict__ trk, int t0,
+                                                        const uint2* __restrict__ q_all,
+                                                        const SplitLevel* __restrict__ lvl,
+                                                        const uint32_t* __restrict__ sub_bits, int max_runs,
+                                                        double penalty, uint32_t* __restrict__ dec,
+                                                        int* __restrict__ arg, int2* __restrict__ runs,
+                                                        int* __restrict__ n_units) {
+  extern __shared__ int rsm[];
+  int* ra = rsm;
+  int* rb = ra + max_runs;
+  __shared__ int sh[33];
+  __shared__ double smx[2][32];
+  __shared__ int sarg[2][32];
+  const int t = t0 + blockIdx.x, tid = threadIdx.x, nw = blockDim.x >> 5;
+  const SplitTrack k = trk[t];
+  if (!k.live || lvl[k.vid].bad >= 0) {
+    if (tid == 0) n_units[t] = k.live ? -1 : 0;
+    return;
+  }
+  const int n_end = runcorr::rc_decode_runs(sub_bits + k.bits_off, k.S, max_runs, ra, rb, sh);
+  const int nr = min(n_end >> 1, max_runs);
+  __syncthreads();
+  for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
+  if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  const int nu = nr > 0 ? nr : 1;
+  const uint2* q = q_all + k.q_off;
+  const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+  const int o0 = k.o_lo + kOffsetsPerThread * tid;
+  const int n_mine = max(0, min(kOffsetsPerThread, k.W - kOffsetsPerThread * tid));
+  double v[32];
+  double c = 0.0;
+  for (int j = 0; j < nu; ++j) {
+    const SpUnit u = sp_unit(ra, rb, nr, k.S, j);
+    double best = -INFINITY;
+    int barg = INT_MIN;
+    uint32_t d = 0;
+    if (n_mine > 0) d = sp_thread_step(q, k.R, u, o0, n_mine, j == 0, c, l, v, best, barg);
+    if (j > 0 && tid < k.nthr) dec[k.dec_base + (long long)j * k.nthr + tid] = d;
+    // unit maximum (ties: largest offset); the shared slots alternate so one barrier per unit suffices
+    for (int s = 16; s > 0; s >>= 1) {
+      const double ob = __shfl_xor_sync(0xffffffffu, best, s);
+      const int oa = __shfl_xor_sync(0xffffffffu, barg, s);
+      if (ob > best || (ob == best && oa > barg)) {
+        best = ob;
+        barg = oa;
+      }
+    }
+    if ((tid & 31) == 0) {
+      smx[j & 1][tid >> 5] = best;
+      sarg[j & 1][tid >> 5] = barg;
+    }
+    __syncthreads();
+    double mx = smx[j & 1][0];
+    int am = sarg[j & 1][0];
+    for (int w = 1; w < nw; ++w)
+      if (smx[j & 1][w] > mx || (smx[j & 1][w] == mx && sarg[j & 1][w] > am)) {
+        mx = smx[j & 1][w];
+        am = sarg[j & 1][w];
+      }
+    if (tid == 0) arg[k.unit_base + j] = am;
+    c = sp_sub(mx, penalty);
+  }
+  if (tid == 0) n_units[t] = nu;
+}
+
+// One CTA per track of the group: thread 0 walks the units back from the last unit's argmax (a set switch bit
+// sends unit j - 1 to its own argmax), then sums u_j(o_j) forwards; every thread then gives its cues the offset
+// of the unit holding their rasterised start frame, clamped into [0, S).
+struct SplitCues {
+  const double* start;
+  const double* end;
+  int sample_rate;
+  double start_seconds;
+};
+
+__global__ void __launch_bounds__(256) split_backtrack_kernel(const SplitTrack* __restrict__ trk, int t0,
+                                                              const uint2* __restrict__ q_all,
+                                                              const SplitLevel* __restrict__ lvl,
+                                                              const uint32_t* __restrict__ dec,
+                                                              const int* __restrict__ arg,
+                                                              const int2* __restrict__ runs,
+                                                              const int* __restrict__ n_units, int* unit_off,
+                                                              SplitCues cues, int* __restrict__ cue_offset,
+                                                              int* __restrict__ n_segments,
+                                                              double* __restrict__ split_score) {
+  __shared__ int s_nu;
+  const int t = t0 + blockIdx.x;
+  const SplitTrack k = trk[t];
+  if (threadIdx.x == 0) {
+    const int nu = n_units[t];
+    s_nu = nu;
+    if (nu <= 0) {
+      n_segments[t] = nu;
+      split_score[t] = NAN;
+    } else {
+      int* uo = unit_off + k.unit_base;
+      int o = arg[k.unit_base + nu - 1];
+      for (int j = nu - 1; j >= 0; --j) {
+        uo[j] = o;
+        if (j > 0) {
+          const int m = o - k.o_lo;
+          if ((dec[k.dec_base + (long long)j * k.nthr + (m >> 5)] >> (m & 31)) & 1u) o = arg[k.unit_base + j - 1];
+        }
+      }
+      const int nr = runs[k.unit_base].y == 0 ? 0 : nu;  // a run is never empty: (0, 0) marks none
+      const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+      const uint2* q = q_all + k.q_off;
+      double score = 0.0;
+      int seg = 1;
+      for (int j = 0; j < nu; ++j) {
+        SpUnit u;
+        if (nr == 0) {
+          u = SpUnit{0, 0, 0, k.S};
+        } else {
+          u.start = j == 0 ? 0 : runs[k.unit_base + j - 1].y;
+          u.a = runs[k.unit_base + j].x;
+          u.b = runs[k.unit_base + j].y;
+          u.end = j == nu - 1 ? k.S : u.b;
+        }
+        if (j > 0 && uo[j] != uo[j - 1]) ++seg;
+        score = sp_add(score, sp_unit_score(q, k.R, u, uo[j], l));
+      }
+      n_segments[t] = seg;
+      split_score[t] = score;
+    }
+  }
+  __syncthreads();
+  const int nu = s_nu;
+  for (long long i = k.c0 + threadIdx.x; i < k.c1; i += blockDim.x) {
+    int off = 0;
+    if (nu > 0) {
+      long long first, last;
+      b2_cue_bounds(cues.start[i], cues.end[i], k.ratio, cues.start_seconds, cues.sample_rate, k.S, first, last);
+      const int f = (int)(first < 0 ? 0 : (first > k.S - 1 ? k.S - 1 : first));
+      int lo = 0, hi = nu - 1;  // first unit whose run ends after f; the last unit when none does
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (runs[k.unit_base + mid].y > f) hi = mid;
+        else lo = mid + 1;
+      }
+      off = unit_off[k.unit_base + lo];
+    }
+    cue_offset[i] = off;
+  }
+}
+
+}  // namespace
+
+int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
+                     const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
+                     const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
+                     int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
+                     bool refuse_three_levels, const void* h_ref, bool h_ref_f64, int* d_cue_offset, int* d_n_segments,
+                     double* d_split_score) {
+  B2Range range("b2:split (split_ref, raster_bits, split_dp, split_backtrack)");
+  if (T <= 0) return B2_OK;
+  // ---- plan: videos, windows, workspace ----
+  std::vector<int> vid_of(V, -1);
+  std::vector<SplitVideo> vids;
+  std::vector<SplitTrack> trk(T);
+  std::vector<double> d_ratio_h(T, 1.0);
+  std::vector<long long> len_h(T, 0), unit_bound(T, 0);
+  long long q_total = 0, sig_words = 1, units = 0, max_cues = 0;
+  int max_runs = 1;
+  const long long c_base = cue_off[0];
+  for (int t = 0; t < T; ++t) {
+    SplitTrack& k = trk[t];
+    memset(&k, 0, sizeof(k));
+    k.c0 = cue_off[t] - c_base;
+    k.c1 = cue_off[t + 1] - c_base;
+    max_cues = std::max(max_cues, k.c1 - k.c0);
+    const int v = track_video[t];
+    const long long R = ref_off[v + 1] - ref_off[v];
+    if (std::isnan(ratio[t]) || R == 0) continue;  // skipped; an empty reference has no alignment
+    const B2JobPlan p = b2_plan_job(R, len[t], max_offset_samples, h->log2_quirk_mask);
+    if (p.kind != 0) continue;  // no offset survives the mask
+    const long long W = p.o_hi - p.o_lo + 1;
+    if (W > kMaxWindow)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: track %d: a window of %lld offsets is wider than %d (one CTA)", t, W,
+              kMaxWindow);
+    long long kept = 0;
+    for (long long c = cue_off[t]; c < cue_off[t + 1]; ++c) kept += cue_keep ? (cue_keep[c] != 0) : 1;
+    if (kept > kMaxRuns)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: track %d: %lld kept cues may make more than %d runs", t, kept, kMaxRuns);
+    if (vid_of[v] < 0) {
+      vid_of[v] = (int)vids.size();
+      vids.push_back(SplitVideo{(long long)ref_off[v], q_total, (int)R});
+      q_total += runcorr::rc_ref_entries((int)R);
+    }
+    k.live = 1;
+    k.vid = vid_of[v];
+    k.q_off = vids[k.vid].q_off;
+    k.R = (int)R;
+    k.S = (int)len[t];
+    k.o_lo = (int)p.o_lo;
+    k.W = (int)W;
+    k.nthr = (int)ceil_div64(W, kOffsetsPerThread);
+    k.ratio = ratio[t];
+    k.level = (float)std::min(1.0 / ratio[t], 1.0);
+    k.unit_base = units;
+    unit_bound[t] = std::max<long long>(kept, 1);
+    units += unit_bound[t];
+    max_runs = std::max<int>(max_runs, (int)kept);
+    sig_words = std::max<long long>(sig_words, (len[t] >> 5) + 2);
+    d_ratio_h[t] = ratio[t];
+    len_h[t] = len[t];
+  }
+  for (int t = 0; t < T; ++t) trk[t].bits_off = (long long)t * sig_words;
+  // track groups: the switch words of a group stay within kDecBudget words
+  const long long kDecBudget = 64LL << 20;
+  std::vector<int> group_first{0};
+  std::vector<int> group_thr;
+  long long dec_max = 1, dec_at = 0;
+  int thr = 32;
+  for (int t = 0; t < T; ++t) {
+    SplitTrack& k = trk[t];
+    const long long need = k.live ? unit_bound[t] * k.nthr : 0;
+    if (dec_at > 0 && dec_at + need > kDecBudget) {
+      group_first.push_back(t);
+      group_thr.push_back(thr);
+      dec_at = 0;
+      thr = 32;
+    }
+    k.dec_base = dec_at;
+    dec_at += need;
+    dec_max = std::max(dec_max, dec_at);
+    if (k.live) thr = std::max<int>(thr, (int)(32 * ceil_div64(k.nthr, 32)));
+  }
+  group_first.push_back(T);
+  group_thr.push_back(thr);
+
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~size_t(255); return o; };
+  const size_t nv = std::max<size_t>(vids.size(), 1), nunits = (size_t)std::max<long long>(units, 1);
+  const size_t o_q = take((size_t)std::max<long long>(q_total, 1) * 8), o_lvl = take(nv * sizeof(SplitLevel)),
+               o_bits = take((size_t)T * sig_words * 4), o_runs = take(nunits * 8), o_arg = take(nunits * 4),
+               o_uo = take(nunits * 4), o_nu = take((size_t)T * 4), o_dec = take((size_t)dec_max * 4);
+  void* d_ws;
+  B2_TRY(b2i_ws(h, b2_ctx::WS_SPLIT, at + 256, &d_ws));
+  char* base = (char*)d_ws;
+  uint2* q = (uint2*)(base + o_q);
+  SplitLevel* lvl = (SplitLevel*)(base + o_lvl);
+  uint32_t* bits = (uint32_t*)(base + o_bits);
+  int2* runs = (int2*)(base + o_runs);
+  int* arg = (int*)(base + o_arg);
+  int* uo = (int*)(base + o_uo);
+  int* nu = (int*)(base + o_nu);
+  uint32_t* dec = (uint32_t*)(base + o_dec);
+
+  const long long nc = cue_off[T] - c_base;
+  std::vector<long long> cue_rel(T + 1);
+  for (int t = 0; t <= T; ++t) cue_rel[t] = cue_off[t] - c_base;
+  MetaArena a;
+  B2_TRY(b2i_meta_begin(h, &a, (size_t)nc * 17 + (size_t)(T + 1) * 8 + (size_t)T * (sizeof(SplitTrack) + 16) +
+                                   vids.size() * sizeof(SplitVideo) + 1024));
+  B2CueDev cd;
+  cd.start = (const double*)b2i_meta_put(&a, cue_start + c_base, (size_t)nc * 8);
+  cd.end = (const double*)b2i_meta_put(&a, cue_end + c_base, (size_t)nc * 8);
+  cd.keep = cue_keep ? (const uint8_t*)b2i_meta_put(&a, cue_keep + c_base, (size_t)nc) : nullptr;
+  cd.cue_off = (const long long*)b2i_meta_put(&a, cue_rel.data(), (size_t)(T + 1) * 8);
+  cd.sample_rate = sample_rate;
+  cd.start_seconds = start_seconds;
+  const SplitTrack* d_trk = (const SplitTrack*)b2i_meta_put(&a, trk.data(), (size_t)T * sizeof(SplitTrack));
+  const double* d_ratio = (const double*)b2i_meta_put(&a, d_ratio_h.data(), (size_t)T * 8);
+  const long long* d_len = (const long long*)b2i_meta_put(&a, len_h.data(), (size_t)T * 8);
+  const SplitVideo* d_vids =
+      vids.empty() ? nullptr : (const SplitVideo*)b2i_meta_put(&a, vids.data(), vids.size() * sizeof(SplitVideo));
+  B2_TRY(b2i_meta_commit(&a));
+
+  if (!vids.empty()) {
+    if (ref_f64)
+      split_ref_kernel<double><<<(unsigned)vids.size(), 1024, 0, h->stream>>>((const double*)d_ref, d_vids, q, lvl);
+    else
+      split_ref_kernel<float><<<(unsigned)vids.size(), 1024, 0, h->stream>>>((const float*)d_ref, d_vids, q, lvl);
+    B2_CHECK_LAUNCH(h, "split_ref_kernel");
+    if (refuse_three_levels) {  // B2_HOST: a third level refuses the call before anything else runs
+      std::vector<SplitLevel> lv(vids.size());
+      B2_CUDA(h, cudaMemcpyAsync(lv.data(), lvl, vids.size() * sizeof(SplitLevel), cudaMemcpyDeviceToHost, h->stream));
+      B2_CUDA(h, cudaStreamSynchronize(h->stream));
+      for (int v = 0; v < V; ++v) {
+        if (vid_of[v] < 0 || lv[vid_of[v]].bad < 0) continue;
+        const long long f = lv[vid_of[v]].bad;
+        B2_FAIL(h, B2_ERR_UNSUPPORTED,
+                "split: video %d: frame %lld holds %g, a level other than 1.0 and %g (the reference must have two "
+                "finite levels)", v, f, !h_ref ? NAN : h_ref_f64 ? ((const double*)h_ref)[ref_off[v] + f] : (double)((const float*)h_ref)[ref_off[v] + f], lv[vid_of[v]].beta);
+      }
+    }
+  }
+  B2_TRY(b2i_raster_bits_dev_launch(h, cd, T, max_cues, d_ratio, d_len, sig_words, bits));
+  const size_t smem = (size_t)2 * max_runs * sizeof(int);
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const SplitCues sc{cd.start, cd.end, sample_rate, start_seconds};
+  for (size_t g = 0; g + 1 < group_first.size(); ++g) {
+    const int g0 = group_first[g], n = group_first[g + 1] - g0;
+    if (n <= 0) continue;
+    const int nthr = group_thr[g];
+    // 32 float64 values per thread: CTAs of up to 512 threads keep them in registers
+    if (nthr <= 512)
+      split_dp_kernel<512><<<(unsigned)n, (unsigned)nthr, smem, h->stream>>>(d_trk, g0, q, lvl, bits, max_runs,
+                                                                           penalty, dec, arg, runs, nu);
+    else
+      split_dp_kernel<1024><<<(unsigned)n, (unsigned)nthr, smem, h->stream>>>(d_trk, g0, q, lvl, bits, max_runs,
+                                                                            penalty, dec, arg, runs, nu);
+    B2_CHECK_LAUNCH(h, "split_dp_kernel");
+    // the kernel's cue indices are relative to c_base; d_cue_offset is indexed by absolute cue
+    split_backtrack_kernel<<<(unsigned)n, 256, 0, h->stream>>>(d_trk, g0, q, lvl, dec, arg, runs, nu, uo, sc,
+                                                              d_cue_offset + c_base, d_n_segments, d_split_score);
+    B2_CHECK_LAUNCH(h, "split_backtrack_kernel");
+  }
+  return B2_OK;
+}

@@ -1,0 +1,153 @@
+// Per-segment offsets with a split penalty (csrc/split.cu, DESIGN.md section 4 "K9s"): the arithmetic shared by
+// the kernels and their CPU emulation (tests/host_emul/split_emul.cu).
+//
+// A track's subtitle mask (S frames, runs [a_k, b_k) of 1s) is cut into units: unit j is the gap before run j
+// and run j, [start_j, end_j) with start_0 = 0, start_j = b_{j-1}, end_j = b_j, except that the last unit ends at
+// S (a mask without runs is one unit [0, S)).  At offset o (subtitle frame f meets reference frame f + o) unit j
+// contributes the run path's four-count score over its frames of the overlap [max(0, -o), min(S, R - o)):
+//     u_j(o) = (hi*c11 - c01) + (hia*c10 - alpha*c00)
+// with hi = 2*(double)level - 1, alpha = 2*beta - 1, hia = hi*alpha (runcorr.cuh's rc_levels).  With M(p) the
+// reference bits below p, p clamped to [0, R] (rc_ref_window):
+//     n_ov = |[start, end) n [-o, R - o)|,  mw = M(end + o) - M(start + o),
+//     uo   = |[a, b) n [-o, R - o)|,        um = M(b + o) - M(a + o)
+// (frames outside [0, R) have no reference bit), c11 = um, c01 = mw - um, c10 = uo - um,
+// c00 = n_ov - mw - uo + um.  The units' contributions add up to the whole track's score at o.
+// The programme over units j = 0 .. n-1 (lambda = split_penalty >= 0):
+//     V_0(o) = u_0(o),   V_j(o) = u_j(o) + max(V_{j-1}(o), M_{j-1} - lambda),   M_j = max_o V_j(o)
+// in float64 with every operation rounded on its own (no contraction): c = M_{j-1} - lambda, then the
+// switch decision c > V_{j-1}(o) (staying wins a tie), then u_j(o) + (switch ? c : V_{j-1}(o)).  The argmax of
+// each unit is its largest offset attaining M_j.  With +-1 signals (level 1, label 0) every value is an integer
+// below 2^53, so every cell is exact.
+#pragma once
+#include "runcorr.cuh"
+
+#ifdef __CUDACC__
+#define SP_HD __host__ __device__ __forceinline__
+#else
+#define SP_HD inline
+#endif
+
+namespace split {
+
+using runcorr::kOffsetsPerThread;
+constexpr int kMaxWindow = runcorr::kMaxWindow;  // offsets of one CTA
+constexpr int kMaxRuns = 16384;                  // runs of one track (shared memory of the run table)
+
+SP_HD double sp_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+SP_HD double sp_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+SP_HD double sp_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+struct SpLevels {
+  double hi, alpha, hia;
+};
+
+// level: the track's subtitle level (float)min(1/x, 1); beta: the reference's level other than 1.0
+SP_HD SpLevels sp_levels(float level, double beta) {
+  SpLevels l;
+  l.hi = sp_sub(sp_mul(2.0, (double)level), 1.0);
+  l.alpha = sp_sub(sp_mul(2.0, beta), 1.0);
+  l.hia = sp_mul(l.hi, l.alpha);
+  return l;
+}
+
+// Unit j of nr runs: [start, end) holding the run [a, b) (a = b = 0 for the one unit of a mask without runs)
+struct SpUnit {
+  int start, a, b, end;
+};
+
+SP_HD SpUnit sp_unit(const int* ra, const int* rb, int nr, int S, int j) {
+  SpUnit u;
+  if (nr == 0) {
+    u.start = 0;
+    u.a = 0;
+    u.b = 0;
+    u.end = S;
+    return u;
+  }
+  u.start = j == 0 ? 0 : rb[j - 1];
+  u.a = ra[j];
+  u.b = rb[j];
+  u.end = j == nr - 1 ? S : rb[j];
+  return u;
+}
+
+SP_HD int sp_overlap(int lo, int hi, int o, int R) {  // |[lo, hi) n [-o, R - o)|
+  const int x = lo > -o ? lo : -o;
+  const int y = hi < R - o ? hi : R - o;
+  return y > x ? y - x : 0;
+}
+
+// u_j(o) from the unit and the four reference prefixes M(start + o), M(a + o), M(b + o), M(end + o)
+SP_HD double sp_score(const SpUnit& u, int o, int R, int m_start, int m_a, int m_b, int m_end, const SpLevels& l) {
+  const int n_ov = sp_overlap(u.start, u.end, o, R);
+  if (n_ov == 0) return 0.0;
+  const int mw = m_end - m_start, um = m_b - m_a, uo = sp_overlap(u.a, u.b, o, R);
+  const double c11 = um, c01 = mw - um, c10 = uo - um, c00 = n_ov - mw - uo + um;
+  return sp_add(sp_sub(sp_mul(l.hi, c11), c01), sp_sub(sp_mul(l.hia, c10), sp_mul(l.alpha, c00)));
+}
+
+// u_j(o) at one offset (the backtrack's re-score of the chosen path)
+SP_HD double sp_unit_score(const uint2* q, int R, const SpUnit& u, int o, const SpLevels& l) {
+  using runcorr::rc_ref_prefix;
+  return sp_score(u, o, R, rc_ref_prefix(q, R, u.start + o), rc_ref_prefix(q, R, u.a + o),
+                  rc_ref_prefix(q, R, u.b + o), rc_ref_prefix(q, R, u.end + o), l);
+}
+
+// One thread's step of the programme over its offsets o0 .. o0 + n_mine - 1 (n_mine <= 32) for one unit:
+// the four prefixes of all 32 offsets come from one funnel-shifted window and one word prefix per endpoint.
+// first: unit 0 (V = u).  Otherwise c = M_{j-1} - lambda and bit i of the returned word is set when offset
+// o0 + i switched.  v[i] becomes V_j(o0 + i); best / barg: the thread's maximum and its largest offset.
+SP_HD uint32_t sp_thread_step(const uint2* q, int R, const SpUnit& u, int o0, int n_mine, bool first, double c,
+                              const SpLevels& l, double (&v)[32], double& best, int& barg) {
+  uint32_t w_s, w_a, w_b, w_e;
+  int p_s, p_a, p_b, p_e;
+  runcorr::rc_ref_window(q, R, u.start + o0, w_s, p_s);
+  runcorr::rc_ref_window(q, R, u.a + o0, w_a, p_a);
+  runcorr::rc_ref_window(q, R, u.b + o0, w_b, p_b);
+  runcorr::rc_ref_window(q, R, u.end + o0, w_e, p_e);
+  uint32_t dec = 0;
+  best = -INFINITY;
+  barg = -2147483647 - 1;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    if (i < n_mine) {
+      const uint32_t below = (1u << i) - 1u;
+      const double s = sp_score(u, o0 + i, R, p_s + runcorr::rc_popc(w_s & below), p_a + runcorr::rc_popc(w_a & below),
+                                p_b + runcorr::rc_popc(w_b & below), p_e + runcorr::rc_popc(w_e & below), l);
+      double x;
+      if (first) {
+        x = s;
+      } else {
+        const bool sw = c > v[i];
+        dec |= (uint32_t)sw << i;
+        x = sp_add(s, sw ? c : v[i]);
+      }
+      v[i] = x;
+      if (x >= best) {  // increasing offsets: ties go to the largest
+        best = x;
+        barg = o0 + i;
+      }
+    }
+  }
+  return dec;
+}
+
+}  // namespace split

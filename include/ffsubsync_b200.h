@@ -522,6 +522,49 @@ int b2_apply_sync(b2_handle h, const double* best_score, const int32_t* best_off
                   int64_t* synced_start_us, int64_t* synced_end_us, double* offset_seconds /* [T] */,
                   double* scale /* [T] */, int32_t* status /* [T] */, int memspace);
 
+/* ---- per-segment offsets with a split penalty, after any batched sync call ---------------------------------
+ * One offset per track (ffsubsync/aligners.py:24-86) fails when the video has a break the subtitles do not have, or
+ * the reverse.  This splits each track's cue runs into segments with their own offsets (DESIGN.md section 4 "K9s").
+ * Track t's mask is its kept cues rasterised at ratio[t] as the sync calls do (S frames, level (float)min(1/x, 1));
+ * unit j is the gap before its j-th run of 1s and that run (the leading gap in unit 0, the frames after the last run
+ * in the last unit; a mask without runs is one unit).  u_j(o) is unit j's four-count run-path score at offset o
+ * against the reference of video track_video[t] (levels 1.0 and one other finite value beta per video).  Over the
+ * window of offsets the aligner keeps for (R, S, max_offset_samples), the programme
+ *     V_0(o) = u_0(o),   V_j(o) = u_j(o) + max(V_{j-1}(o), max_o V_{j-1} - split_penalty)
+ * is solved in float64 with every operation rounded on its own; staying wins a tie, and among equal maxima the
+ * largest offset wins (the aligner's rule).  No cap on the number of splits, no order between adjacent segments'
+ * offsets, one ratio per track: split_penalty is the only knob, and +inf never switches.
+ *   ref            the videos' reference frames, float64 (ref_is_f64, what b2_speech_output writes) or float32, at
+ *                  ref_off [V+1] (host); in memspace.
+ *   ratio [T]      host: each track's ratio (ratios[best_k], or gss_ratio when best_k == K); NaN skips the track.
+ *   cue_*          host, as for b2_sync_tracks; cue_offset is indexed like the cues (absolute indices).
+ * Per track: n_segments (0 for a skipped track or one whose window is empty), split_score = the sum of u_j over the
+ * chosen path without penalties (NaN when skipped), and for every cue (kept or not) cue_offset = the offset of the
+ * unit holding its rasterised start frame clamped into [0, S) (0 when skipped).  memspace B2_HOST copies in and
+ * out and synchronises; B2_DEVICE enqueues on the handle's stream without a host synchronisation (behind the sync
+ * call that wrote the reference), and a video whose reference has a third level gives its tracks n_segments = -1,
+ * NaN and offsets 0 there, where B2_HOST refuses it with B2_ERR_UNSUPPORTED naming the video and frame.
+ * B2_ERR_UNSUPPORTED also for a window wider than 32768 offsets and a track with more than 16384 kept cues (each
+ * run holds one); B2_ERR_BAD_ARG for a NaN or negative split_penalty, a ratio that is not NaN or finite positive,
+ * a track_video entry outside [0, V), a non-monotone ref_off / cue_off, the cue checks of b2_rasterize and host
+ * pointers under B2_DEVICE. */
+int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off /* [V+1] */, int V,
+                    const int32_t* track_video /* [T] */, int T, const double* cue_start_s, const double* cue_end_s,
+                    const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */, const double* ratio /* [T] */,
+                    int sample_rate, double start_seconds, int64_t max_offset_samples, double split_penalty,
+                    int32_t* cue_offset, int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
+/* try_sync's output step (ffsubsync/ffsubsync.py:272-286, SubtitleScaler + SubtitleShifter) with each cue's own
+ * offset: for a track with n_segments > 0, cue i gets timedelta(seconds=t_i * ratio[t]) + timedelta(seconds=
+ * cue_offset[i] / sample_rate + apply_offset_seconds), each rounded half-to-even to the microsecond as b2_apply_sync
+ * rounds them, and status WRITTEN | APPLIED; other tracks are FAILED and keep their original times.  The quality gate
+ * and suppression do not apply.  ratio and the cue tables are host metadata; n_segments, cue_offset and the outputs
+ * follow memspace (B2_DEVICE: one kernel on the handle's stream, a chain of resident sync calls stays intact).
+ * B2_ERR_BAD_ARG as for b2_apply_sync. */
+int b2_apply_split(b2_handle h, const double* ratio /* [T] */, const int32_t* n_segments /* [T] */,
+                   const int32_t* cue_offset, int T, const double* cue_start_s, const double* cue_end_s,
+                   const int64_t* cue_off /* [T+1] */, int sample_rate, double apply_offset_seconds,
+                   int64_t* synced_start_us, int64_t* synced_end_us, int32_t* status /* [T] */, int memspace);
+
 /* ---- diagnostics for tests: the aligner's nomination stage ----------------------------------
  * Exposes the fp32 correlation the aligner nominates candidates from - the conv[] array of
  * ffsubsync/aligners.py:67-80 over the offsets that survive the mask, and the argmax of :45-48 before

@@ -1,0 +1,132 @@
+"""Cost of the per-segment offsets (b2_split_tracks) at the bench shape, alone and after the sync step it follows.
+
+    python tools/split_bench.py [--pairs 256] [--ratios 5] [--penalty 20] [--repeats 10] [--warmup 2]
+
+The workload is bench.py's (BASELINE configs[2]): 256 two-hour pairs (synth.make_pairs, about 1 200 cues each), K = 5,
++-60 s, PCM synthesised on the device.  Half the pairs get a planted 90 s cut in the middle: 9 000 windows of their
+video are removed halfway and the end padded with silence, so their subtitles after the cut sit 90 s later than the
+audio.  The sync step is BatchSynchronizer.sync_device with speech_video covering every video (the references the
+split reads); the split is split_tracks over its results.  Timed with CUDA events on one stream, after warm-up, in
+alternating repeats: the split alone over one sync step's results (including the read-back of best_k that forms the
+ratio list), and sync + split.  Reports DP cells (units x window offsets, summed over the tracks) per second of the
+split alone, the segment counts of the cut and uncut pairs at a few penalties, and the GPU's name, power limit and SM
+clock read in the same run.  Needs an H100.
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+from tracks_bench import FPW, FRAME_RATE, SAMPLE_RATE, gpu_info  # noqa: E402
+
+CUT = 9000   # windows of 10 ms: 90 s
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--pairs", type=int, default=256)
+    ap.add_argument("--ratios", type=int, default=5)
+    ap.add_argument("--penalty", type=float, default=20.0)
+    ap.add_argument("--repeats", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=2)
+    args = ap.parse_args()
+
+    import torch
+    from ffsubsync_b200 import _native
+    from ffsubsync_b200.batch import BatchSynchronizer
+    from ffsubsync_b200.synth import BENCH_RATIOS, make_pairs
+    from oracle import aligner_oracle as ao
+    from oracle import raster_oracle as ro
+
+    if not torch.cuda.is_available():
+        sys.exit("split_bench: no CUDA device (this measurement runs on the GPU only)")
+    info = gpu_info()
+    print(json.dumps(dict(info, event="gpu")), flush=True)
+    dev = torch.device("cuda", 0)
+    ratios = list(BENCH_RATIOS[: args.ratios])
+    B = args.pairs
+    stream = torch.cuda.Stream(device=dev)
+    torch.cuda.set_stream(stream)
+    bs = BatchSynchronizer(ratios, FRAME_RATE, SAMPLE_RATE, 0.0, max_offset_seconds=60)
+    bs.use_torch_stream()
+    h = bs.handle
+    pairs = make_pairs([13 + b for b in range(B)], 7200.0, ratios, handle=h)
+    wc = pairs.window_class.copy()
+    cut = np.zeros(B, bool)
+    for b in range(0, B, 2):   # the planted cut: the middle 90 s of the video removed
+        a, e = int(pairs.win_off[b]), int(pairs.win_off[b + 1])
+        mid = a + (e - a) // 2
+        wc[a:e] = np.concatenate([wc[a:mid], wc[mid + CUT:e], np.zeros(CUT, wc.dtype)])
+        cut[b] = True
+    n_win = int(pairs.win_off[-1])
+    cls_d = torch.from_numpy(wc).to(dev)
+    pcm = torch.empty(n_win * FPW, dtype=torch.int16, device=dev)
+    h.synth_pcm(cls_d.data_ptr(), n_win, FPW, 1234, out=pcm.data_ptr(), memspace=_native.B2_DEVICE)
+    del cls_d
+    pcm_off = pairs.win_off * FPW
+    cs, ce, co = pairs.cue_start, pairs.cue_end, pairs.cue_off
+    tv = np.arange(B, dtype=np.int32)
+    sv = np.arange(B)
+
+    def sync():
+        return bs.sync_device(pcm, pcm_off, cs, ce, co, speech_video=sv)
+
+    def split(out):
+        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=args.penalty)
+
+    def timed(fn, n):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(n):
+            fn()
+        e1.record(stream)
+        torch.cuda.synchronize(dev)
+        return e0.elapsed_time(e1) / n
+
+    out = sync()
+    for _ in range(args.warmup):
+        split(out)
+        split(sync())
+    torch.cuda.synchronize(dev)
+    split_ms, both_ms = [], []
+    for _ in range(args.repeats):   # alternating
+        split_ms.append(timed(lambda: split(out), 1))
+        both_ms.append(timed(lambda: split(sync()), 1))
+    res = split(out)
+    torch.cuda.synchronize(dev)
+    ns = res["n_segments"].cpu().numpy()
+    # DP cells: units (runs of the mask at the track's ratio, at least 1) x window offsets
+    ref_len = np.diff(out["speech_off"])
+    cells = 0
+    for t in range(B):
+        if np.isnan(res["ratio"][t]):
+            continue
+        mask = ro.rasterize(cs[co[t]:co[t + 1]], ce[co[t]:co[t + 1]], None, SAMPLE_RATE, 0.0, res["ratio"][t])[0] > 0
+        o_lo, o_hi = ao.offset_range(int(ref_len[t]), len(mask), bs.max_offset_samples)
+        cells += max(1, int(np.count_nonzero(np.diff(np.concatenate([[0], mask.astype(np.int8)])) == 1))) * \
+            max(0, o_hi - o_lo + 1)
+    med_split, med_both = float(np.median(split_ms)), float(np.median(both_ms))
+    # segments per pair at other penalties (the VAD reference is noisy: small penalties split on its noise too)
+    segs = {}
+    for pen in (args.penalty, 200.0, 2000.0, 20000.0):
+        n_s = bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen)["n_segments"].cpu().numpy()
+        segs[str(pen)] = dict(cut_median=float(np.median(n_s[cut])), uncut_median=float(np.median(n_s[~cut])),
+                              cut_two=int(np.sum(n_s[cut] == 2)), uncut_one=int(np.sum(n_s[~cut] == 1)))
+    print(json.dumps(dict(info, event="measure", pairs=B, K=len(ratios), penalty=args.penalty, cues=int(co[-1]),
+                          split_ms=round(med_split, 3), split_ms_all=[round(x, 3) for x in split_ms],
+                          sync_plus_split_ms=round(med_both, 3), sync_plus_split_ms_all=[round(x, 3) for x in both_ms],
+                          dp_cells=int(cells), dp_cells_per_s=round(cells / (med_split * 1e-3), 1),
+                          cut_pairs=int(cut.sum()), cut_pairs_with_two_segments=int(np.sum(ns[cut] == 2)),
+                          uncut_pairs_with_one_segment=int(np.sum(ns[~cut] == 1)), segments_by_penalty=segs)),
+          flush=True)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
