@@ -33,7 +33,7 @@ EXPORTS = [
     "b2_sync_tracks_pgs", "b2_capture_reference", "b2_sync_tracks_sig", "b2_apply_sync",
     "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
     "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort", "b2_ingest_segments", "b2_ingest_push_segments",
-    "b2_ingest_drop_segment", "b2_ingest_sync_refs", "b2_split_tracks", "b2_apply_split",
+    "b2_ingest_drop_segment", "b2_ingest_sync_refs", "b2_split_tracks", "b2_split_tracks_wide", "b2_apply_split",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -157,6 +157,7 @@ def load() -> ctypes.CDLL:
         lib.b2_ingest_drop_segment.argtypes = [_vp, ctypes.c_int, _i64]
         lib.b2_split_tracks.argtypes = [_vp, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
                                         _vp, ctypes.c_int, _f64, _i64, _f64, _vp, _vp, _vp, ctypes.c_int]
+        lib.b2_split_tracks_wide.argtypes = lib.b2_split_tracks.argtypes
         lib.b2_apply_split.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _f64, _vp, _vp,
                                        _vp, ctypes.c_int]
         _lib = lib
@@ -952,6 +953,21 @@ class Handle:
         float32) follows memspace; everything else but the outputs is host metadata (ratio: NaN skips a track).
         B2_HOST: returns numpy (cue_offset i32 [cues], n_segments i32 [T], split_score f64 [T]).  B2_DEVICE: outs holds
         those three device pointers in that order; enqueued on the handle's stream, returns outs."""
+        return self._split_tracks("b2_split_tracks", ref, ref_is_f64, ref_off, track_video, cue_start_s, cue_end_s,
+                                  cue_keep, cue_off, ratio, sample_rate, start_seconds, max_offset_samples,
+                                  split_penalty, outs, memspace)
+
+    def split_tracks_wide(self, ref, ref_is_f64: bool, ref_off, track_video, cue_start_s, cue_end_s, cue_keep, cue_off,
+                          ratio, sample_rate: int, start_seconds: float, max_offset_samples, split_penalty: float,
+                          outs=None, memspace: int = B2_HOST):
+        """b2_split_tracks_wide: split_tracks with windows of up to 16384 offsets per CTA of the widest thread-block
+        cluster the device co-schedules (262144 offsets at 16 CTAs); same arguments and results."""
+        return self._split_tracks("b2_split_tracks_wide", ref, ref_is_f64, ref_off, track_video, cue_start_s,
+                                  cue_end_s, cue_keep, cue_off, ratio, sample_rate, start_seconds, max_offset_samples,
+                                  split_penalty, outs, memspace)
+
+    def _split_tracks(self, name, ref, ref_is_f64, ref_off, track_video, cue_start_s, cue_end_s, cue_keep, cue_off,
+                      ratio, sample_rate, start_seconds, max_offset_samples, split_penalty, outs, memspace):
         ref_off, cue_off = _i64a(ref_off), _i64a(cue_off)
         V, T = len(ref_off) - 1, len(cue_off) - 1
         track_video = np.ascontiguousarray(track_video, dtype=np.int32)
@@ -963,11 +979,11 @@ class Handle:
             ref = np.ascontiguousarray(ref, dtype=np.float64 if ref_is_f64 else np.float32)
             n = int(cue_off[-1]) if T >= 0 else 0
             outs = (np.zeros(n, np.int32), np.zeros(max(T, 0), np.int32), np.zeros(max(T, 0), np.float64))
-        st = self.lib.b2_split_tracks(
+        st = getattr(self.lib, name)(
             self.h, _ptr(ref), int(bool(ref_is_f64)), _ptr(ref_off), V, _ptr(track_video), T, _ptr(cue_start_s),
             _ptr(cue_end_s), _ptr(keep), _ptr(cue_off), _ptr(ratio), int(sample_rate), float(start_seconds),
             _mask_width(max_offset_samples), float(split_penalty), *[_ptr(o) for o in outs], memspace)
-        self._check(st, "b2_split_tracks")
+        self._check(st, name)
         return outs
 
     def apply_split(self, ratio, n_segments, cue_offset, cue_start_s, cue_end_s, cue_off, sample_rate: int,

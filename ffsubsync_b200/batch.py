@@ -902,8 +902,15 @@ class BatchSynchronizer:
                              "them" % missing)
         return np.array([pos[int(v)] for v in track_video], dtype=np.int32)
 
+    def _split_window(self, split_max_offset_seconds):
+        """(Handle method, max_offset_samples) of a split: None keeps the sync window and b2_split_tracks; seconds
+        convert as max_offset_seconds does and go through b2_split_tracks_wide."""
+        if split_max_offset_seconds is None:
+            return self.handle.split_tracks, self.max_offset_samples
+        return self.handle.split_tracks_wide, abs(int(split_max_offset_seconds * self.sample_rate))
+
     def split_tracks(self, out, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                     speech_video=None) -> dict:
+                     speech_video=None, split_max_offset_seconds=None) -> dict:
         """Per-segment offsets (b2_split_tracks) over the results of a device sync call made with ``speech_video``
         (``out`` carries ``speech`` / ``speech_off``; pass the same speech_video here, None when it listed videos
         0 .. P-1): each track's cue runs are cut into segments with their own offsets, a change of offset costing
@@ -915,7 +922,11 @@ class BatchSynchronizer:
         so that a bad ratio is refused before anything runs); a video whose reference has a third level is not an
         error here (the device call cannot stop after its level scan without a synchronisation) but gives its tracks
         ``n_segments == -1``, NaN and offsets 0, which apply_split marks FAILED - split_tracks_host raises instead; and a
-        track with more than 16 384 kept cues is refused even when its cues make fewer runs (each run holds one)."""
+        track with more than 16 384 kept cues is refused even when its cues make fewer runs (each run holds one).
+        ``split_max_offset_seconds`` (None: the synchroniser's own max_offset_seconds) sets the window the segments'
+        offsets are searched in, up to about +-1 310 s at 100 Hz (b2_split_tracks_wide).  Every segment offset is
+        absolute and all segments share the window, so it must cover the sync offset plus the breaks before the last
+        segment: after a 5 min ad break the later cues need the sync offset plus 300 s."""
         import torch
         if "speech" not in out:
             raise ValueError("split_tracks needs the sync call's reference signals: call it with speech_video")
@@ -928,25 +939,27 @@ class BatchSynchronizer:
         res = {"cue_offset": torch.empty(max(n, 1), dtype=torch.int32, device=dev),
                "n_segments": torch.empty(max(T, 1), dtype=torch.int32, device=dev),
                "split_score": torch.empty(max(T, 1), dtype=torch.float64, device=dev)}
-        self.handle.split_tracks(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep,
-                                 cue_off, ratio, self.sample_rate, self.start_seconds, self.max_offset_samples,
-                                 split_penalty, outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
+        split, mos = self._split_window(split_max_offset_seconds)
+        split(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep, cue_off, ratio,
+              self.sample_rate, self.start_seconds, mos, split_penalty, outs=[t.data_ptr() for t in res.values()],
+              memspace=_native.B2_DEVICE)
         res = {"cue_offset": res["cue_offset"][:n], "n_segments": res["n_segments"][:T],
                "split_score": res["split_score"][:T], "ratio": ratio}
         return res
 
     def split_tracks_host(self, res, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                          speech_video=None) -> dict:
+                          speech_video=None, split_max_offset_seconds=None) -> dict:
         """split_tracks over the tuple of a host sync call made with speech_video (best_score, best_offset, best_k
         first, gss_ratio before the trailing (speech, speech_off) with the search).  Blocks; numpy results.  A reference
         with a third level raises (NativeError, B2_ERR_UNSUPPORTED, naming the video and frame); more than 16 384 kept
-        cues in a track too."""
+        cues in a track too.  ``split_max_offset_seconds`` as for split_tracks: an absolute window shared by all
+        segments, which must cover the sync offset plus the breaks before the last segment."""
         speech, speech_off = res[-2], res[-1]
         idx = self._split_refs(speech_off, track_video, speech_video)
         ratio = self.split_ratios(res[2], res[-3] if self.gss else None)
-        co, ns, sc = self.handle.split_tracks(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off,
-                                              ratio, self.sample_rate, self.start_seconds, self.max_offset_samples,
-                                              split_penalty, memspace=_native.B2_HOST)
+        split, mos = self._split_window(split_max_offset_seconds)
+        co, ns, sc = split(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off, ratio,
+                           self.sample_rate, self.start_seconds, mos, split_penalty, memspace=_native.B2_HOST)
         return {"cue_offset": co, "n_segments": ns, "split_score": sc, "ratio": ratio}
 
     def apply_split(self, split, cue_start, cue_end, cue_off, *,

@@ -2266,11 +2266,12 @@ extern "C" int b2_apply_sync(b2_handle h, const double* best_score, const int32_
 }
 
 // ---- per-segment offsets with a split penalty (split.cu, sync_output.cu) ---------------------------------------
-extern "C" int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
-                               const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
-                               const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
-                               double start_seconds, int64_t max_offset_samples, double split_penalty,
-                               int32_t* cue_offset, int32_t* n_segments, double* split_score, int memspace) {
+// b2_split_tracks and b2_split_tracks_wide: the same checks and outputs, wide: the wider envelope
+static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                        const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
+                        const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
+                        double start_seconds, int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
+                        int32_t* n_segments, double* split_score, int memspace, bool wide) {
   B2_ENTER(h);
   if (V < 0 || T < 0 || !ref_off || !cue_off || (T && (!track_video || !ratio)))
     B2_FAIL(h, B2_ERR_BAD_ARG, "split: bad arguments (V %d, T %d, null table)", V, T);
@@ -2319,7 +2320,7 @@ extern "C" int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, con
   if (memspace == B2_DEVICE)
     return b2i_split_launch(h, ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                             cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                            false, nullptr, false, cue_offset, n_segments, split_score);
+                            false, nullptr, false, wide, cue_offset, n_segments, split_score);
   // B2_HOST: the reference staged in, outputs through the staging workspace (cue outputs at their absolute indices)
   void *d_ref, *dout;
   B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, ref, (size_t)ref_off[V] * esz, &d_ref));
@@ -2330,12 +2331,33 @@ extern "C" int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, con
   int32_t* d_co = d_ns + Ts;
   B2_TRY(b2i_split_launch(h, d_ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                           cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                          true, ref, ref_is_f64 != 0, d_co - c0, d_ns, d_sc));
+                          true, ref, ref_is_f64 != 0, wide, d_co - c0, d_ns, d_sc));
   B2_TRY(copy_out(h, cue_offset + c0, d_co, (size_t)n * 4));
   B2_TRY(copy_out(h, n_segments, d_ns, Ts * 4));
   B2_TRY(copy_out(h, split_score, d_sc, Ts * 8));
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
+}
+
+extern "C" int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                               const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
+                               const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
+                               double start_seconds, int64_t max_offset_samples, double split_penalty,
+                               int32_t* cue_offset, int32_t* n_segments, double* split_score, int memspace) {
+  return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
+                      sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
+                      split_score, memspace, false);
+}
+
+extern "C" int b2_split_tracks_wide(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                                    const int32_t* track_video, int T, const double* cue_start_s,
+                                    const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                    const double* ratio, int sample_rate, double start_seconds,
+                                    int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
+                                    int32_t* n_segments, double* split_score, int memspace) {
+  return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
+                      sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
+                      split_score, memspace, true);
 }
 
 extern "C" int b2_apply_split(b2_handle h, const double* ratio, const int32_t* n_segments, const int32_t* cue_offset,

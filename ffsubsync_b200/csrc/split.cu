@@ -9,11 +9,14 @@
 
 #include <algorithm>
 
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 #include "job_plan.cuh"
 #include "split.cuh"
 
 using namespace split;
+namespace cg = cooperative_groups;
 
 namespace {
 
@@ -85,39 +88,58 @@ __global__ void __launch_bounds__(1024) split_ref_kernel(const T* __restrict__ r
   if (threadIdx.x == 0) lvl[blockIdx.x] = SplitLevel{beta, s_bad < v.R ? (long long)s_bad : -1LL};
 }
 
-// One CTA per track of the group: thread t owns the offsets o_lo + 32 t .. + 31.  Dynamic shared memory: 2 x
-// max_runs ints (run starts, ends).  Per unit j >= 1 each thread writes its switch word to
-// dec[dec_base + j * nthr + t], thread 0 the unit's argmax to arg[unit_base + j]; the runs go to runs[unit_base + r].
-template <int MAXT>
-__global__ void __launch_bounds__(MAXT) split_dp_kernel(const SplitTrack* __restrict__ trk, int t0,
-                                                        const uint2* __restrict__ q_all,
-                                                        const SplitLevel* __restrict__ lvl,
-                                                        const uint32_t* __restrict__ sub_bits, int max_runs,
-                                                        double penalty, uint32_t* __restrict__ dec,
-                                                        int* __restrict__ arg, int2* __restrict__ runs,
-                                                        int* __restrict__ n_units) {
+// One track per cluster of C CTAs (kCluster false: a plain launch, C = 1), the tracks order[g0 + cluster]: cluster
+// thread g = rank * blockDim.x + tid owns the offsets o_lo + 32 g .. + 31.  Every CTA decodes the runs into its own
+// dynamic shared memory (2 x max_runs ints: run starts, ends).  Per unit j >= 1 each thread writes its switch word to
+// dec[dec_base + j * nthr + g] (nthr: the track's threads over the whole cluster), rank 0's thread 0 the unit's
+// argmax to arg[unit_base + j]; rank 0 writes the runs to runs[unit_base + r].
+//
+// Barriers: the early exit depends on the track alone, so a cluster takes it as a whole, before any barrier or
+// shared-memory traffic.  Otherwise every CTA runs the same nu units (all decode the same runs), each with one
+// __syncthreads and one cluster barrier whether or not it owns offsets, then one final cluster barrier, so no CTA
+// exits while another may still read its slots.  CTA and cluster slots alternate between units: a slot written
+// at unit j + 2 was last read at unit j, before the barriers of unit j + 1.
+template <bool kCluster>
+__global__ void __launch_bounds__(kCtaThreads) split_dp_kernel(const SplitTrack* __restrict__ trk,
+                                                               const int* __restrict__ order, int g0,
+                                                               const uint2* __restrict__ q_all,
+                                                               const SplitLevel* __restrict__ lvl,
+                                                               const uint32_t* __restrict__ sub_bits, int max_runs,
+                                                               double penalty, uint32_t* __restrict__ dec,
+                                                               int* __restrict__ arg, int2* __restrict__ runs,
+                                                               int* __restrict__ n_units) {
   extern __shared__ int rsm[];
   int* ra = rsm;
   int* rb = ra + max_runs;
   __shared__ int sh[33];
-  __shared__ double smx[2][32];
-  __shared__ int sarg[2][32];
-  const int t = t0 + blockIdx.x, tid = threadIdx.x, nw = blockDim.x >> 5;
+  __shared__ double smx[2][kCtaThreads / 32];
+  __shared__ int sarg[2][kCtaThreads / 32];
+  __shared__ double cmx[2];
+  __shared__ int carg[2];
+  int C = 1, rank = 0;
+  if constexpr (kCluster) {
+    C = (int)cg::this_cluster().num_blocks();
+    rank = (int)cg::this_cluster().block_rank();
+  }
+  const int t = order[g0 + (int)blockIdx.x / C], tid = threadIdx.x, nw = blockDim.x >> 5;
   const SplitTrack k = trk[t];
   if (!k.live || lvl[k.vid].bad >= 0) {
-    if (tid == 0) n_units[t] = k.live ? -1 : 0;
+    if (rank == 0 && tid == 0) n_units[t] = k.live ? -1 : 0;
     return;
   }
   const int n_end = runcorr::rc_decode_runs(sub_bits + k.bits_off, k.S, max_runs, ra, rb, sh);
   const int nr = min(n_end >> 1, max_runs);
   __syncthreads();
-  for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
-  if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  if (rank == 0) {
+    for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
+    if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  }
   const int nu = nr > 0 ? nr : 1;
   const uint2* q = q_all + k.q_off;
   const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
-  const int o0 = k.o_lo + kOffsetsPerThread * tid;
-  const int n_mine = max(0, min(kOffsetsPerThread, k.W - kOffsetsPerThread * tid));
+  const int g = rank * (int)blockDim.x + tid;
+  const int o0 = k.o_lo + kOffsetsPerThread * g;
+  const int n_mine = max(0, min(kOffsetsPerThread, k.W - kOffsetsPerThread * g));
   double v[32];
   double c = 0.0;
   for (int j = 0; j < nu; ++j) {
@@ -126,16 +148,10 @@ __global__ void __launch_bounds__(MAXT) split_dp_kernel(const SplitTrack* __rest
     int barg = INT_MIN;
     uint32_t d = 0;
     if (n_mine > 0) d = sp_thread_step(q, k.R, u, o0, n_mine, j == 0, c, l, v, best, barg);
-    if (j > 0 && tid < k.nthr) dec[k.dec_base + (long long)j * k.nthr + tid] = d;
-    // unit maximum (ties: largest offset); the shared slots alternate so one barrier per unit suffices
-    for (int s = 16; s > 0; s >>= 1) {
-      const double ob = __shfl_xor_sync(0xffffffffu, best, s);
-      const int oa = __shfl_xor_sync(0xffffffffu, barg, s);
-      if (ob > best || (ob == best && oa > barg)) {
-        best = ob;
-        barg = oa;
-      }
-    }
+    if (j > 0 && g < k.nthr) dec[k.dec_base + (long long)j * k.nthr + g] = d;
+    // unit maximum (ties: largest offset): the warp, the CTA's warps, then the cluster's CTAs
+    for (int s = 16; s > 0; s >>= 1)
+      sp_merge(best, barg, __shfl_xor_sync(0xffffffffu, best, s), __shfl_xor_sync(0xffffffffu, barg, s));
     if ((tid & 31) == 0) {
       smx[j & 1][tid >> 5] = best;
       sarg[j & 1][tid >> 5] = barg;
@@ -143,15 +159,24 @@ __global__ void __launch_bounds__(MAXT) split_dp_kernel(const SplitTrack* __rest
     __syncthreads();
     double mx = smx[j & 1][0];
     int am = sarg[j & 1][0];
-    for (int w = 1; w < nw; ++w)
-      if (smx[j & 1][w] > mx || (smx[j & 1][w] == mx && sarg[j & 1][w] > am)) {
-        mx = smx[j & 1][w];
-        am = sarg[j & 1][w];
+    for (int w = 1; w < nw; ++w) sp_merge(mx, am, smx[j & 1][w], sarg[j & 1][w]);
+    if constexpr (kCluster) {
+      cg::cluster_group cl = cg::this_cluster();
+      if (tid == 0) {
+        cmx[j & 1] = mx;
+        carg[j & 1] = am;
       }
-    if (tid == 0) arg[k.unit_base + j] = am;
+      cl.sync();  // barrier.cluster arrive (release) / wait (acquire): the C slots are visible
+      mx = *cl.map_shared_rank(&cmx[j & 1], 0);
+      am = *cl.map_shared_rank(&carg[j & 1], 0);
+      for (int r = 1; r < C; ++r)
+        sp_merge(mx, am, *cl.map_shared_rank(&cmx[j & 1], r), *cl.map_shared_rank(&carg[j & 1], r));
+    }
+    if (rank == 0 && tid == 0) arg[k.unit_base + j] = am;
     c = sp_sub(mx, penalty);
   }
-  if (tid == 0) n_units[t] = nu;
+  if constexpr (kCluster) cg::this_cluster().sync();
+  if (rank == 0 && tid == 0) n_units[t] = nu;
 }
 
 // One CTA per track of the group: thread 0 walks the units back from the last unit's argmax (a set switch bit
@@ -237,14 +262,51 @@ __global__ void __launch_bounds__(256) split_backtrack_kernel(const SplitTrack* 
 
 }  // namespace
 
+// The widest cluster (CTAs) of split_dp_kernel at kCtaThreads threads and the largest run table that the device
+// co-schedules, from kMaxCluster down; queried once per handle.
+int b2i_split_max_cluster(b2_ctx* h) {
+  if (h->split_max_cluster > 0) return B2_OK;
+  const size_t smem = (size_t)2 * kMaxRuns * sizeof(int);
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  for (int C = kMaxCluster; C >= 1; --C) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)C);
+    cfg.blockDim = dim3((unsigned)kCtaThreads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = (unsigned)C;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    int n = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, split_dp_kernel<true>, &cfg);
+    if (e == cudaSuccess && n > 0) {
+      h->split_max_cluster = C;
+      return B2_OK;
+    }
+    (void)cudaGetLastError();  // a size the device refuses is an answer, not an error
+  }
+  B2_FAIL(h, B2_ERR_CUDA, "split: the device co-schedules no cluster of split_dp_kernel");
+}
+
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
                      const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
-                     bool refuse_three_levels, const void* h_ref, bool h_ref_f64, int* d_cue_offset, int* d_n_segments,
-                     double* d_split_score) {
+                     bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
+                     int* d_n_segments, double* d_split_score) {
   B2Range range("b2:split (split_ref, raster_bits, split_dp, split_backtrack)");
   if (T <= 0) return B2_OK;
+  // the envelope: b2_split_tracks up to kMaxWindow offsets (clusters of 1 or 2 CTAs), b2_split_tracks_wide up to
+  // the widest cluster of kCtaThreads-thread CTAs this device co-schedules
+  long long max_window = kMaxWindow;
+  if (wide) {
+    B2_TRY(b2i_split_max_cluster(h));
+    max_window = (long long)kCtaWindow * h->split_max_cluster;
+  }
   // ---- plan: videos, windows, workspace ----
   std::vector<int> vid_of(V, -1);
   std::vector<SplitVideo> vids;
@@ -266,9 +328,15 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     const B2JobPlan p = b2_plan_job(R, len[t], max_offset_samples, h->log2_quirk_mask);
     if (p.kind != 0) continue;  // no offset survives the mask
     const long long W = p.o_hi - p.o_lo + 1;
-    if (W > kMaxWindow)
-      B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: track %d: a window of %lld offsets is wider than %d (one CTA)", t, W,
-              kMaxWindow);
+    if (W > max_window) {
+      if (wide)
+        B2_FAIL(h, B2_ERR_UNSUPPORTED,
+                "split: track %d: a window of %lld offsets is wider than %lld (a cluster of %d CTAs of %d offsets, "
+                "the widest this device co-schedules)", t, W, max_window, h->split_max_cluster, kCtaWindow);
+      B2_FAIL(h, B2_ERR_UNSUPPORTED,
+              "split: track %d: a window of %lld offsets is wider than %d (b2_split_tracks_wide takes wider ones)", t,
+              W, kMaxWindow);
+    }
     long long kept = 0;
     for (long long c = cue_off[t]; c < cue_off[t + 1]; ++c) kept += cue_keep ? (cue_keep[c] != 0) : 1;
     if (kept > kMaxRuns)
@@ -297,28 +365,29 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     len_h[t] = len[t];
   }
   for (int t = 0; t < T; ++t) trk[t].bits_off = (long long)t * sig_words;
-  // track groups: the switch words of a group stay within kDecBudget words
+  // track groups: the switch words of a group stay within kDecBudget words; within a group the tracks are launched
+  // by cluster size C (cluster size is per launch), order[] listing each group's tracks by C
   const long long kDecBudget = 64LL << 20;
   std::vector<int> group_first{0};
-  std::vector<int> group_thr;
   long long dec_max = 1, dec_at = 0;
-  int thr = 32;
+  std::vector<int> ncta(T, 1), order(T);
   for (int t = 0; t < T; ++t) {
     SplitTrack& k = trk[t];
     const long long need = k.live ? unit_bound[t] * k.nthr : 0;
     if (dec_at > 0 && dec_at + need > kDecBudget) {
       group_first.push_back(t);
-      group_thr.push_back(thr);
       dec_at = 0;
-      thr = 32;
     }
     k.dec_base = dec_at;
     dec_at += need;
     dec_max = std::max(dec_max, dec_at);
-    if (k.live) thr = std::max<int>(thr, (int)(32 * ceil_div64(k.nthr, 32)));
+    if (k.live) ncta[t] = (int)ceil_div64(k.W, kCtaWindow);
+    order[t] = t;
   }
   group_first.push_back(T);
-  group_thr.push_back(thr);
+  for (size_t g = 0; g + 1 < group_first.size(); ++g)
+    std::stable_sort(order.begin() + group_first[g], order.begin() + group_first[g + 1],
+                     [&](int a, int b) { return ncta[a] < ncta[b]; });
 
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~size_t(255); return o; };
@@ -343,7 +412,7 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   for (int t = 0; t <= T; ++t) cue_rel[t] = cue_off[t] - c_base;
   MetaArena a;
   B2_TRY(b2i_meta_begin(h, &a, (size_t)nc * 17 + (size_t)(T + 1) * 8 + (size_t)T * (sizeof(SplitTrack) + 16) +
-                                   vids.size() * sizeof(SplitVideo) + 1024));
+                                   vids.size() * sizeof(SplitVideo) + (size_t)T * 4 + 1024));
   B2CueDev cd;
   cd.start = (const double*)b2i_meta_put(&a, cue_start + c_base, (size_t)nc * 8);
   cd.end = (const double*)b2i_meta_put(&a, cue_end + c_base, (size_t)nc * 8);
@@ -354,6 +423,7 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   const SplitTrack* d_trk = (const SplitTrack*)b2i_meta_put(&a, trk.data(), (size_t)T * sizeof(SplitTrack));
   const double* d_ratio = (const double*)b2i_meta_put(&a, d_ratio_h.data(), (size_t)T * 8);
   const long long* d_len = (const long long*)b2i_meta_put(&a, len_h.data(), (size_t)T * 8);
+  const int* d_order = (const int*)b2i_meta_put(&a, order.data(), (size_t)T * 4);
   const SplitVideo* d_vids =
       vids.empty() ? nullptr : (const SplitVideo*)b2i_meta_put(&a, vids.data(), vids.size() * sizeof(SplitVideo));
   B2_TRY(b2i_meta_commit(&a));
@@ -379,21 +449,42 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   }
   B2_TRY(b2i_raster_bits_dev_launch(h, cd, T, max_cues, d_ratio, d_len, sig_words, bits));
   const size_t smem = (size_t)2 * max_runs * sizeof(int);
-  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   const SplitCues sc{cd.start, cd.end, sample_rate, start_seconds};
   for (size_t g = 0; g + 1 < group_first.size(); ++g) {
     const int g0 = group_first[g], n = group_first[g + 1] - g0;
     if (n <= 0) continue;
-    const int nthr = group_thr[g];
-    // 32 float64 values per thread: CTAs of up to 512 threads keep them in registers
-    if (nthr <= 512)
-      split_dp_kernel<512><<<(unsigned)n, (unsigned)nthr, smem, h->stream>>>(d_trk, g0, q, lvl, bits, max_runs,
-                                                                           penalty, dec, arg, runs, nu);
-    else
-      split_dp_kernel<1024><<<(unsigned)n, (unsigned)nthr, smem, h->stream>>>(d_trk, g0, q, lvl, bits, max_runs,
-                                                                            penalty, dec, arg, runs, nu);
-    B2_CHECK_LAUNCH(h, "split_dp_kernel");
+    for (int i = g0; i < g0 + n;) {
+      const int C = ncta[order[i]];
+      int e = i;
+      while (e < g0 + n && ncta[order[e]] == C) ++e;
+      if (C == 1) {  // one CTA of the bucket's widest track's threads
+        int thr = 32;
+        for (int x = i; x < e; ++x) thr = std::max<int>(thr, (int)(32 * ceil_div64(trk[order[x]].nthr, 32)));
+        split_dp_kernel<false><<<(unsigned)(e - i), (unsigned)thr, smem, h->stream>>>(
+            d_trk, d_order, i, q, lvl, bits, max_runs, penalty, dec, arg, runs, nu);
+      } else {  // CTAs of kCtaThreads threads: CTA r of a track owns its offsets r * kCtaWindow ..
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)((e - i) * C));
+        cfg.blockDim = dim3((unsigned)kCtaThreads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = h->stream;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = (unsigned)C;
+        at[0].val.clusterDim.y = 1;
+        at[0].val.clusterDim.z = 1;
+        cfg.attrs = at;
+        cfg.numAttrs = 1;
+        B2_CUDA(h, cudaLaunchKernelEx(&cfg, split_dp_kernel<true>, d_trk, (const int*)d_order, i, (const uint2*)q,
+                                      (const SplitLevel*)lvl, (const uint32_t*)bits, max_runs, penalty, dec, arg, runs,
+                                      nu));
+      }
+      B2_CHECK_LAUNCH(h, "split_dp_kernel");
+      i = e;
+    }
     // the kernel's cue indices are relative to c_base; d_cue_offset is indexed by absolute cue
     split_backtrack_kernel<<<(unsigned)n, 256, 0, h->stream>>>(d_trk, g0, q, lvl, dec, arg, runs, nu, uo, sc,
                                                               d_cue_offset + c_base, d_n_segments, d_split_score);

@@ -1,5 +1,5 @@
 // Per-segment offsets with a split penalty (csrc/split.cu, DESIGN.md section 4 "K9s"): the arithmetic shared by
-// the kernels and their CPU emulation (tests/host_emul/split_emul.cu).
+// the kernels and their CPU emulations (tests/host_emul/split_emul.cu, split_cluster_emul.cu).
 //
 // A track's subtitle mask (S frames, runs [a_k, b_k) of 1s) is cut into units: unit j is the gap before run j
 // and run j, [start_j, end_j) with start_0 = 0, start_j = b_{j-1}, end_j = b_j, except that the last unit ends at
@@ -30,8 +30,13 @@
 namespace split {
 
 using runcorr::kOffsetsPerThread;
-constexpr int kMaxWindow = runcorr::kMaxWindow;  // offsets of one CTA
+constexpr int kMaxWindow = runcorr::kMaxWindow;  // b2_split_tracks' envelope
 constexpr int kMaxRuns = 16384;                  // runs of one track (shared memory of the run table)
+// A track is one thread-block cluster of C CTAs of at most kCtaThreads threads (32 float64 V each stay in registers
+// at 128 registers a thread); cluster thread g = rank * blockDim + tid owns the offsets o_lo + 32 g .. + 31.
+constexpr int kCtaThreads = 512;
+constexpr int kCtaWindow = kOffsetsPerThread * kCtaThreads;  // offsets of one CTA: C = ceil(W / kCtaWindow)
+constexpr int kMaxCluster = 16;                              // non-portable past 8
 
 SP_HD double sp_add(double a, double b) {
 #ifdef __CUDA_ARCH__
@@ -148,6 +153,15 @@ SP_HD uint32_t sp_thread_step(const uint2* q, int R, const SpUnit& u, int o0, in
     }
   }
   return dec;
+}
+
+// One step of the unit maximum over candidates (warp lanes, a CTA's warps, a cluster's CTAs): the larger value, and
+// among equal values the larger offset, so the merge gives np.argmax over the reversed window in any order.
+SP_HD void sp_merge(double& best, int& barg, double ob, int oa) {
+  if (ob > best || (ob == best && oa > barg)) {
+    best = ob;
+    barg = oa;
+  }
 }
 
 }  // namespace split

@@ -544,7 +544,7 @@ int b2_apply_sync(b2_handle h, const double* best_score, const int32_t* best_off
  * out and synchronises; B2_DEVICE enqueues on the handle's stream without a host synchronisation (behind the sync
  * call that wrote the reference), and a video whose reference has a third level gives its tracks n_segments = -1,
  * NaN and offsets 0 there, where B2_HOST refuses it with B2_ERR_UNSUPPORTED naming the video and frame.
- * B2_ERR_UNSUPPORTED also for a window wider than 32768 offsets and a track with more than 16384 kept cues (each
+ * B2_ERR_UNSUPPORTED also for a window wider than 32768 offsets (b2_split_tracks_wide below goes further) and a track with more than 16384 kept cues (each
  * run holds one); B2_ERR_BAD_ARG for a NaN or negative split_penalty, a ratio that is not NaN or finite positive,
  * a track_video entry outside [0, V), a non-monotone ref_off / cue_off, the cue checks of b2_rasterize and host
  * pointers under B2_DEVICE. */
@@ -553,6 +553,17 @@ int b2_split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t*
                     const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */, const double* ratio /* [T] */,
                     int sample_rate, double start_seconds, int64_t max_offset_samples, double split_penalty,
                     int32_t* cue_offset, int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
+/* b2_split_tracks with a wider envelope: the same arguments, outputs, memspaces and refusals, but windows of up to
+ * 16384 x C offsets, C the widest thread-block cluster of 512-thread CTAs the device co-schedules (at most 16:
+ * 262144 offsets, +-1310 s at 100 Hz; the refusal names the limit).  The window is absolute and shared by all of a
+ * track's segments, so it must cover the sync offset plus the breaks before the last segment.  Results equal
+ * b2_split_tracks' bit for bit wherever both run. */
+int b2_split_tracks_wide(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off /* [V+1] */, int V,
+                         const int32_t* track_video /* [T] */, int T, const double* cue_start_s,
+                         const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */,
+                         const double* ratio /* [T] */, int sample_rate, double start_seconds,
+                         int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
+                         int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
 /* try_sync's output step (ffsubsync/ffsubsync.py:272-286, SubtitleScaler + SubtitleShifter) with each cue's own
  * offset: for a track with n_segments > 0, cue i gets timedelta(seconds=t_i * ratio[t]) + timedelta(seconds=
  * cue_offset[i] / sample_rate + apply_offset_seconds), each rounded half-to-even to the microsecond as b2_apply_sync

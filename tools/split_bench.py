@@ -1,6 +1,7 @@
 """Cost of the per-segment offsets (b2_split_tracks) at the bench shape, alone and after the sync step it follows.
 
     python tools/split_bench.py [--pairs 256] [--ratios 5] [--penalty 20] [--repeats 10] [--warmup 2]
+                                [--split-max-offset-seconds S]
 
 The workload is bench.py's (BASELINE configs[2]): 256 two-hour pairs (synth.make_pairs, about 1 200 cues each), K = 5,
 +-60 s, PCM synthesised on the device.  Half the pairs get a planted 90 s cut in the middle: 9 000 windows of their
@@ -11,6 +12,13 @@ alternating repeats: the split alone over one sync step's results (including the
 ratio list), and sync + split.  Reports DP cells (units x window offsets, summed over the tracks) per second of the
 split alone, the segment counts of the cut and uncut pairs at a few penalties, and the GPU's name, power limit and SM
 clock read in the same run.  Needs an H100.
+
+--split-max-offset-seconds (default: the sync window, +-60 s) sets the split's own window
+(split_tracks(split_max_offset_seconds=...), b2_split_tracks_wide): the second half of a cut pair needs
+true_offset - 9000 frames, which the +-60 s window cannot hold for any of the bench's seeds.  The run then also
+reports the CTAs per track's cluster (ceil(window / 16 384)), and, per penalty, how many cut pairs come back as exactly
+two segments at true_offset and true_offset - 9000 with the break in the middle cue, and how many uncut pairs stay
+whole.
 """
 import argparse
 import json
@@ -35,6 +43,7 @@ def main():
     ap.add_argument("--penalty", type=float, default=20.0)
     ap.add_argument("--repeats", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--split-max-offset-seconds", type=float, default=None)
     args = ap.parse_args()
 
     import torch
@@ -77,8 +86,9 @@ def main():
     def sync():
         return bs.sync_device(pcm, pcm_off, cs, ce, co, speech_video=sv)
 
-    def split(out):
-        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=args.penalty)
+    def split(out, pen=args.penalty):
+        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
+                               split_max_offset_seconds=args.split_max_offset_seconds)
 
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -103,22 +113,41 @@ def main():
     ns = res["n_segments"].cpu().numpy()
     # DP cells: units (runs of the mask at the track's ratio, at least 1) x window offsets
     ref_len = np.diff(out["speech_off"])
+    mos = bs.max_offset_samples if args.split_max_offset_seconds is None else \
+        abs(int(args.split_max_offset_seconds * SAMPLE_RATE))
     cells = 0
+    ctas = set()
     for t in range(B):
         if np.isnan(res["ratio"][t]):
             continue
         mask = ro.rasterize(cs[co[t]:co[t + 1]], ce[co[t]:co[t + 1]], None, SAMPLE_RATE, 0.0, res["ratio"][t])[0] > 0
-        o_lo, o_hi = ao.offset_range(int(ref_len[t]), len(mask), bs.max_offset_samples)
+        o_lo, o_hi = ao.offset_range(int(ref_len[t]), len(mask), mos)
         cells += max(1, int(np.count_nonzero(np.diff(np.concatenate([[0], mask.astype(np.int8)])) == 1))) * \
             max(0, o_hi - o_lo + 1)
+        ctas.add(-(-max(0, o_hi - o_lo + 1) // 16384))
     med_split, med_both = float(np.median(split_ms)), float(np.median(both_ms))
     # segments per pair at other penalties (the VAD reference is noisy: small penalties split on its noise too)
+    # a cut pair is found when its cues take true_offset before the middle of the video and true_offset - CUT after
+    # it (cues are rasterised at the pair's ratio; the cut sits at the middle window of the video)
     segs = {}
     for pen in (args.penalty, 200.0, 2000.0, 20000.0):
-        n_s = bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen)["n_segments"].cpu().numpy()
+        r = split(out, pen)
+        n_s, c_o = r["n_segments"].cpu().numpy(), r["cue_offset"].cpu().numpy()
+        found = 0
+        for b in np.flatnonzero(cut):
+            if n_s[b] != 2 or np.isnan(r["ratio"][b]):
+                continue
+            o = c_o[co[b]:co[b + 1]]
+            t0 = int(pairs.true_offset[b])
+            before = np.flatnonzero(o == t0)
+            after = np.flatnonzero(o == t0 - CUT)
+            found += int(len(before) + len(after) == len(o) and len(before) and len(after)
+                         and before.max() < after.min())
         segs[str(pen)] = dict(cut_median=float(np.median(n_s[cut])), uncut_median=float(np.median(n_s[~cut])),
-                              cut_two=int(np.sum(n_s[cut] == 2)), uncut_one=int(np.sum(n_s[~cut] == 1)))
+                              cut_two=int(np.sum(n_s[cut] == 2)), uncut_one=int(np.sum(n_s[~cut] == 1)),
+                              cut_two_at_true_offsets=found)
     print(json.dumps(dict(info, event="measure", pairs=B, K=len(ratios), penalty=args.penalty, cues=int(co[-1]),
+                          split_max_offset_samples=mos, cluster_ctas=sorted(ctas),
                           split_ms=round(med_split, 3), split_ms_all=[round(x, 3) for x in split_ms],
                           sync_plus_split_ms=round(med_both, 3), sync_plus_split_ms_all=[round(x, 3) for x in both_ms],
                           dp_cells=int(cells), dp_cells_per_s=round(cells / (med_split * 1e-3), 1),
