@@ -902,15 +902,20 @@ class BatchSynchronizer:
                              "them" % missing)
         return np.array([pos[int(v)] for v in track_video], dtype=np.int32)
 
-    def _split_window(self, split_max_offset_seconds):
-        """(Handle method, max_offset_samples) of a split: None keeps the sync window and b2_split_tracks; seconds
-        convert as max_offset_seconds does and go through b2_split_tracks_wide."""
+    def _split_window(self, split_max_offset_seconds, max_segments=None):
+        """(Handle method, max_offset_samples, arguments after split_penalty) of a split: None keeps the sync window
+        and b2_split_tracks; seconds convert as max_offset_seconds does and go through b2_split_tracks_wide.  An integer
+        max_segments goes through b2_split_tracks_capped at either window."""
+        mos = self.max_offset_samples if split_max_offset_seconds is None else \
+            abs(int(split_max_offset_seconds * self.sample_rate))
+        if max_segments is not None:
+            return self.handle.split_tracks_capped, mos, (int(max_segments),)
         if split_max_offset_seconds is None:
-            return self.handle.split_tracks, self.max_offset_samples
-        return self.handle.split_tracks_wide, abs(int(split_max_offset_seconds * self.sample_rate))
+            return self.handle.split_tracks, mos, ()
+        return self.handle.split_tracks_wide, mos, ()
 
     def split_tracks(self, out, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                     speech_video=None, split_max_offset_seconds=None) -> dict:
+                     speech_video=None, split_max_offset_seconds=None, max_segments=None) -> dict:
         """Per-segment offsets (b2_split_tracks) over the results of a device sync call made with ``speech_video``
         (``out`` carries ``speech`` / ``speech_off``; pass the same speech_video here, None when it listed videos
         0 .. P-1): each track's cue runs are cut into segments with their own offsets, a change of offset costing
@@ -926,7 +931,10 @@ class BatchSynchronizer:
         ``split_max_offset_seconds`` (None: the synchroniser's own max_offset_seconds) sets the window the segments'
         offsets are searched in, up to about +-1 310 s at 100 Hz (b2_split_tracks_wide).  Every segment offset is
         absolute and all segments share the window, so it must cover the sync offset plus the breaks before the last
-        segment: after a 5 min ad break the later cues need the sync offset plus 300 s."""
+        segment: after a 5 min ad break the later cues need the sync offset plus 300 s.
+        ``max_segments`` (None: no cap, the calls above) caps each track at that many segments (b2_split_tracks_capped,
+        1 .. 16, at most 8 at +-150 s on an H100) and adds ``split_profile``, a (T, max_segments) f64 tensor: column k
+        is the track's best penalised objective with at most k + 1 segments (NaN for a track n_segments <= 0 marks)."""
         import torch
         if "speech" not in out:
             raise ValueError("split_tracks needs the sync call's reference signals: call it with speech_video")
@@ -939,28 +947,32 @@ class BatchSynchronizer:
         res = {"cue_offset": torch.empty(max(n, 1), dtype=torch.int32, device=dev),
                "n_segments": torch.empty(max(T, 1), dtype=torch.int32, device=dev),
                "split_score": torch.empty(max(T, 1), dtype=torch.float64, device=dev)}
-        split, mos = self._split_window(split_max_offset_seconds)
+        if max_segments is not None:
+            res["split_profile"] = torch.empty((max(T, 1), max(int(max_segments), 1)), dtype=torch.float64, device=dev)
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments)
         split(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep, cue_off, ratio,
-              self.sample_rate, self.start_seconds, mos, split_penalty, outs=[t.data_ptr() for t in res.values()],
-              memspace=_native.B2_DEVICE)
+              self.sample_rate, self.start_seconds, mos, split_penalty, *cap,
+              outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
         res = {"cue_offset": res["cue_offset"][:n], "n_segments": res["n_segments"][:T],
-               "split_score": res["split_score"][:T], "ratio": ratio}
+               "split_score": res["split_score"][:T], "ratio": ratio,
+               **({} if max_segments is None else {"split_profile": res["split_profile"][:T]})}
         return res
 
     def split_tracks_host(self, res, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                          speech_video=None, split_max_offset_seconds=None) -> dict:
+                          speech_video=None, split_max_offset_seconds=None, max_segments=None) -> dict:
         """split_tracks over the tuple of a host sync call made with speech_video (best_score, best_offset, best_k
         first, gss_ratio before the trailing (speech, speech_off) with the search).  Blocks; numpy results.  A reference
         with a third level raises (NativeError, B2_ERR_UNSUPPORTED, naming the video and frame); more than 16 384 kept
         cues in a track too.  ``split_max_offset_seconds`` as for split_tracks: an absolute window shared by all
-        segments, which must cover the sync offset plus the breaks before the last segment."""
+        segments, which must cover the sync offset plus the breaks before the last segment.  ``max_segments`` as for
+        split_tracks: the result gains ``split_profile``, a (T, max_segments) numpy array."""
         speech, speech_off = res[-2], res[-1]
         idx = self._split_refs(speech_off, track_video, speech_video)
         ratio = self.split_ratios(res[2], res[-3] if self.gss else None)
-        split, mos = self._split_window(split_max_offset_seconds)
-        co, ns, sc = split(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off, ratio,
-                           self.sample_rate, self.start_seconds, mos, split_penalty, memspace=_native.B2_HOST)
-        return {"cue_offset": co, "n_segments": ns, "split_score": sc, "ratio": ratio}
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments)
+        outs = split(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off, ratio, self.sample_rate,
+                     self.start_seconds, mos, split_penalty, *cap, memspace=_native.B2_HOST)
+        return dict(zip(("cue_offset", "n_segments", "split_score", "split_profile"), outs), ratio=ratio)
 
     def apply_split(self, split, cue_start, cue_end, cue_off, *,
                     apply_offset_seconds: float = DEFAULT_APPLY_OFFSET_SECONDS) -> dict:

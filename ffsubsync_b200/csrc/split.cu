@@ -3,7 +3,8 @@
 // handle's stream: split_ref_kernel (each video's two levels and its packed bits) -> raster_bits_kernel (the
 // tracks' masks at their own ratios) -> per track group split_dp_kernel (the programme, one CTA per track, a
 // switch word per unit and thread to the workspace) -> split_backtrack_kernel (the path, its score and the
-// per-cue offsets).
+// per-cue offsets).  b2_split_tracks_capped (at most N segments) runs split_capped_dp_kernel (N layers of the
+// programme on one cluster per track) and split_capped_backtrack_kernel in the last two places.
 #include <limits.h>
 #include <math.h>
 
@@ -189,6 +190,55 @@ struct SplitCues {
   double start_seconds;
 };
 
+// split_capped_backtrack_kernel's epilogue, the lines split_backtrack_kernel below runs inline (kept there as they
+// were, so that kernel's code does not change).  The path uo[0 .. nu - 1] of a track: its segment count and the sum
+// of u_j(uo[j]) (one thread)
+__device__ __forceinline__ void split_path_score(const SplitTrack& k, int t, int nu, const int* uo, const uint2* q_all,
+                                                 const SplitLevel* lvl, const int2* runs, int* n_segments,
+                                                 double* split_score) {
+  const int nr = runs[k.unit_base].y == 0 ? 0 : nu;  // a run is never empty: (0, 0) marks none
+  const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+  const uint2* q = q_all + k.q_off;
+  double score = 0.0;
+  int seg = 1;
+  for (int j = 0; j < nu; ++j) {
+    SpUnit u;
+    if (nr == 0) {
+      u = SpUnit{0, 0, 0, k.S};
+    } else {
+      u.start = j == 0 ? 0 : runs[k.unit_base + j - 1].y;
+      u.a = runs[k.unit_base + j].x;
+      u.b = runs[k.unit_base + j].y;
+      u.end = j == nu - 1 ? k.S : u.b;
+    }
+    if (j > 0 && uo[j] != uo[j - 1]) ++seg;
+    score = sp_add(score, sp_unit_score(q, k.R, u, uo[j], l));
+  }
+  n_segments[t] = seg;
+  split_score[t] = score;
+}
+
+// Every cue of the track (all threads of the CTA): the offset of the unit holding its rasterised start frame
+__device__ __forceinline__ void split_cue_offsets(const SplitTrack& k, int nu, const int2* runs, const int* unit_off,
+                                                  const SplitCues& cues, int* cue_offset) {
+  for (long long i = k.c0 + threadIdx.x; i < k.c1; i += blockDim.x) {
+    int off = 0;
+    if (nu > 0) {
+      long long first, last;
+      b2_cue_bounds(cues.start[i], cues.end[i], k.ratio, cues.start_seconds, cues.sample_rate, k.S, first, last);
+      const int f = (int)(first < 0 ? 0 : (first > k.S - 1 ? k.S - 1 : first));
+      int lo = 0, hi = nu - 1;  // first unit whose run ends after f; the last unit when none does
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (runs[k.unit_base + mid].y > f) hi = mid;
+        else lo = mid + 1;
+      }
+      off = unit_off[k.unit_base + lo];
+    }
+    cue_offset[i] = off;
+  }
+}
+
 __global__ void __launch_bounds__(256) split_backtrack_kernel(const SplitTrack* __restrict__ trk, int t0,
                                                               const uint2* __restrict__ q_all,
                                                               const SplitLevel* __restrict__ lvl,
@@ -260,15 +310,154 @@ __global__ void __launch_bounds__(256) split_backtrack_kernel(const SplitTrack* 
   }
 }
 
-}  // namespace
+// b2_split_tracks_capped (at most N segments): one track per cluster of N x C CTAs, C = ceil(W / kCtaWindow) as for
+// split_dp_kernel<true> (C = 1: CTAs of the bucket's widest track's threads).  CTA rank r runs layer kl = r / C (kl:
+// the switches allowed so far) over window part p = r % C, part thread g = p * blockDim.x + tid owning the offsets
+// o_lo + 32 g .. + 31 with the unchanged sp_thread_step.  Layer 0 never switches (c = -inf); layer kl >= 1 switches to
+// c = M_{j-1,kl-1} - penalty.  Per unit j each CTA publishes its maximum in an alternating slot; after the cluster
+// barrier it merges its own layer's C slots (the unit's argmax, which part 0 writes to arg[(unit_base + j) * N + kl])
+// and layer kl - 1's C slots (its next c), each in rank order.  Switch words go to
+// dec[dec_base + (j * N + kl) * nthr + g]; part 0 of layer kl writes the last unit's maximum to profile[t * N + kl].
+//
+// Barriers as split_dp_kernel<true>: the early exit depends on the track alone and comes before any barrier; then every
+// CTA (past the window or in a layer the track cannot reach alike) runs the decode's barriers and, per unit, one
+// __syncthreads and one cluster barrier, and one final cluster barrier.  A slot written at unit j + 2 was last read
+// (by its own layer and the layer above) at unit j, before the barriers of unit j + 1.
+__global__ void __launch_bounds__(kCtaThreads) split_capped_dp_kernel(const SplitTrack* __restrict__ trk,
+                                                                      const int* __restrict__ order, int g0, int N,
+                                                                      const uint2* __restrict__ q_all,
+                                                                      const SplitLevel* __restrict__ lvl,
+                                                                      const uint32_t* __restrict__ sub_bits,
+                                                                      int max_runs, double penalty,
+                                                                      uint32_t* __restrict__ dec,
+                                                                      int* __restrict__ arg, int2* __restrict__ runs,
+                                                                      int* __restrict__ n_units,
+                                                                      double* __restrict__ profile) {
+  extern __shared__ int rsm[];
+  int* ra = rsm;
+  int* rb = ra + max_runs;
+  __shared__ int sh[33];
+  __shared__ double smx[2][kCtaThreads / 32];
+  __shared__ int sarg[2][kCtaThreads / 32];
+  __shared__ double cmx[2];
+  __shared__ int carg[2];
+  cg::cluster_group cl = cg::this_cluster();
+  const int NC = (int)cl.num_blocks(), rank = (int)cl.block_rank(), C = NC / N;
+  const int layer = rank / C, part = rank - layer * C;
+  const int t = order[g0 + (int)blockIdx.x / NC], tid = threadIdx.x, nw = blockDim.x >> 5;
+  const SplitTrack k = trk[t];
+  if (!k.live || lvl[k.vid].bad >= 0) {
+    if (rank == 0 && tid < N) profile[(long long)t * N + tid] = NAN;  // N <= kMaxSegments <= 32 <= blockDim.x
+    if (rank == 0 && tid == 0) n_units[t] = k.live ? -1 : 0;
+    return;
+  }
+  const int n_end = runcorr::rc_decode_runs(sub_bits + k.bits_off, k.S, max_runs, ra, rb, sh);
+  const int nr = min(n_end >> 1, max_runs);
+  __syncthreads();
+  if (rank == 0) {
+    for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
+    if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  }
+  const int nu = nr > 0 ? nr : 1;
+  const uint2* q = q_all + k.q_off;
+  const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+  const int g = part * (int)blockDim.x + tid;
+  const int o0 = k.o_lo + kOffsetsPerThread * g;
+  const int n_mine = max(0, min(kOffsetsPerThread, k.W - kOffsetsPerThread * g));
+  const int own = layer * C;  // the first rank of this layer (the layer below: own - C)
+  double v[32];
+  double c = -INFINITY;
+  for (int j = 0; j < nu; ++j) {
+    const SpUnit u = sp_unit(ra, rb, nr, k.S, j);
+    double best = -INFINITY;
+    int barg = INT_MIN;
+    uint32_t d = 0;
+    if (n_mine > 0) d = sp_thread_step(q, k.R, u, o0, n_mine, j == 0, c, l, v, best, barg);
+    if (j > 0 && g < k.nthr) dec[k.dec_base + ((long long)j * N + layer) * k.nthr + g] = d;
+    for (int s = 16; s > 0; s >>= 1)
+      sp_merge(best, barg, __shfl_xor_sync(0xffffffffu, best, s), __shfl_xor_sync(0xffffffffu, barg, s));
+    if ((tid & 31) == 0) {
+      smx[j & 1][tid >> 5] = best;
+      sarg[j & 1][tid >> 5] = barg;
+    }
+    __syncthreads();
+    double mx = smx[j & 1][0];
+    int am = sarg[j & 1][0];
+    for (int w = 1; w < nw; ++w) sp_merge(mx, am, smx[j & 1][w], sarg[j & 1][w]);
+    if (tid == 0) {
+      cmx[j & 1] = mx;
+      carg[j & 1] = am;
+    }
+    cl.sync();  // barrier.cluster arrive (release) / wait (acquire): the N x C slots are visible
+    if (part == 0 && tid == 0) {
+      mx = *cl.map_shared_rank(&cmx[j & 1], own);
+      am = *cl.map_shared_rank(&carg[j & 1], own);
+      for (int r = 1; r < C; ++r)
+        sp_merge(mx, am, *cl.map_shared_rank(&cmx[j & 1], own + r), *cl.map_shared_rank(&carg[j & 1], own + r));
+      arg[(k.unit_base + j) * N + layer] = am;
+      if (j == nu - 1) profile[(long long)t * N + layer] = mx;
+    }
+    if (layer > 0) {
+      mx = *cl.map_shared_rank(&cmx[j & 1], own - C);
+      am = *cl.map_shared_rank(&carg[j & 1], own - C);
+      for (int r = 1; r < C; ++r)
+        sp_merge(mx, am, *cl.map_shared_rank(&cmx[j & 1], own - C + r), *cl.map_shared_rank(&carg[j & 1], own - C + r));
+      c = sp_sub(mx, penalty);
+    }
+  }
+  cl.sync();
+  if (rank == 0 && tid == 0) n_units[t] = nu;
+}
 
-// The widest cluster (CTAs) of split_dp_kernel at kCtaThreads threads and the largest run table that the device
-// co-schedules, from kMaxCluster down; queried once per handle.
-int b2i_split_max_cluster(b2_ctx* h) {
-  if (h->split_max_cluster > 0) return B2_OK;
+// The capped path: thread 0 walks back from the top layer's last argmax, a set switch bit at (layer kl, unit j) sending
+// unit j - 1 to layer kl - 1's argmax; the score and the cue offsets as split_backtrack_kernel.
+__global__ void __launch_bounds__(256) split_capped_backtrack_kernel(const SplitTrack* __restrict__ trk, int t0, int N,
+                                                                     const uint2* __restrict__ q_all,
+                                                                     const SplitLevel* __restrict__ lvl,
+                                                                     const uint32_t* __restrict__ dec,
+                                                                     const int* __restrict__ arg,
+                                                                     const int2* __restrict__ runs,
+                                                                     const int* __restrict__ n_units, int* unit_off,
+                                                                     SplitCues cues, int* __restrict__ cue_offset,
+                                                                     int* __restrict__ n_segments,
+                                                                     double* __restrict__ split_score) {
+  __shared__ int s_nu;
+  const int t = t0 + blockIdx.x;
+  const SplitTrack k = trk[t];
+  if (threadIdx.x == 0) {
+    const int nu = n_units[t];
+    s_nu = nu;
+    if (nu <= 0) {
+      n_segments[t] = nu;
+      split_score[t] = NAN;
+    } else {
+      int* uo = unit_off + k.unit_base;
+      int kl = N - 1;
+      int o = arg[(k.unit_base + nu - 1) * N + kl];
+      for (int j = nu - 1; j >= 0; --j) {
+        uo[j] = o;
+        if (j > 0 && kl > 0) {
+          const int m = o - k.o_lo;
+          if ((dec[k.dec_base + ((long long)j * N + kl) * k.nthr + (m >> 5)] >> (m & 31)) & 1u) {
+            --kl;
+            o = arg[(k.unit_base + j - 1) * N + kl];
+          }
+        }
+      }
+      split_path_score(k, t, nu, uo, q_all, lvl, runs, n_segments, split_score);
+    }
+  }
+  __syncthreads();
+  split_cue_offsets(k, s_nu, runs, unit_off, cues, cue_offset);
+}
+
+// The widest cluster (CTAs, from kMaxCluster down) of kernel at kCtaThreads threads and the largest run table that
+// the device co-schedules, into *out.
+template <typename Kernel>
+int split_query_cluster(b2_ctx* h, Kernel kernel, const char* name, int* out) {
   const size_t smem = (size_t)2 * kMaxRuns * sizeof(int);
-  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  B2_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   for (int C = kMaxCluster; C >= 1; --C) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)C);
@@ -282,14 +471,28 @@ int b2i_split_max_cluster(b2_ctx* h) {
     cfg.attrs = at;
     cfg.numAttrs = 1;
     int n = 0;
-    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, split_dp_kernel<true>, &cfg);
+    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg);
     if (e == cudaSuccess && n > 0) {
-      h->split_max_cluster = C;
+      *out = C;
       return B2_OK;
     }
     (void)cudaGetLastError();  // a size the device refuses is an answer, not an error
   }
-  B2_FAIL(h, B2_ERR_CUDA, "split: the device co-schedules no cluster of split_dp_kernel");
+  B2_FAIL(h, B2_ERR_CUDA, "split: the device co-schedules no cluster of %s", name);
+}
+
+}  // namespace
+
+// The widest clusters of split_dp_kernel and of split_capped_dp_kernel (each queried for its own kernel) that the
+// device co-schedules; once per handle.
+int b2i_split_max_cluster(b2_ctx* h) {
+  if (h->split_max_cluster > 0) return B2_OK;
+  return split_query_cluster(h, split_dp_kernel<true>, "split_dp_kernel", &h->split_max_cluster);
+}
+
+int b2i_split_capped_max_cluster(b2_ctx* h) {
+  if (h->split_capped_max_cluster > 0) return B2_OK;
+  return split_query_cluster(h, split_capped_dp_kernel, "split_capped_dp_kernel", &h->split_capped_max_cluster);
 }
 
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
@@ -297,13 +500,20 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
                      bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
-                     int* d_n_segments, double* d_split_score) {
+                     int* d_n_segments, double* d_split_score, int max_segments, double* d_profile) {
   B2Range range("b2:split (split_ref, raster_bits, split_dp, split_backtrack)");
   if (T <= 0) return B2_OK;
   // the envelope: b2_split_tracks up to kMaxWindow offsets (clusters of 1 or 2 CTAs), b2_split_tracks_wide up to
-  // the widest cluster of kCtaThreads-thread CTAs this device co-schedules
+  // the widest cluster of kCtaThreads-thread CTAs this device co-schedules, b2_split_tracks_capped up to N x C CTAs
+  // of the widest cluster of split_capped_dp_kernel
+  const bool capped = max_segments > 0;
+  const int N = capped ? max_segments : 1;
   long long max_window = kMaxWindow;
-  if (wide) {
+  if (capped) {
+    if (N > kMaxSegments) B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: max_segments %d is more than %d", N, kMaxSegments);
+    B2_TRY(b2i_split_capped_max_cluster(h));
+    max_window = (long long)kCtaWindow * (h->split_capped_max_cluster / N);
+  } else if (wide) {
     B2_TRY(b2i_split_max_cluster(h));
     max_window = (long long)kCtaWindow * h->split_max_cluster;
   }
@@ -329,6 +539,11 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     if (p.kind != 0) continue;  // no offset survives the mask
     const long long W = p.o_hi - p.o_lo + 1;
     if (W > max_window) {
+      if (capped)
+        B2_FAIL(h, B2_ERR_UNSUPPORTED,
+                "split: track %d: a window of %lld offsets is wider than %lld at %d segments (%d segments x %lld CTAs of "
+                "%d offsets; %d CTAs make the widest cluster this device co-schedules)", t, W, max_window, N, N,
+                (long long)ceil_div64(W, kCtaWindow), kCtaWindow, h->split_capped_max_cluster);
       if (wide)
         B2_FAIL(h, B2_ERR_UNSUPPORTED,
                 "split: track %d: a window of %lld offsets is wider than %lld (a cluster of %d CTAs of %d offsets, "
@@ -366,14 +581,15 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   }
   for (int t = 0; t < T; ++t) trk[t].bits_off = (long long)t * sig_words;
   // track groups: the switch words of a group stay within kDecBudget words; within a group the tracks are launched
-  // by cluster size C (cluster size is per launch), order[] listing each group's tracks by C
+  // by cluster size C (cluster size is per launch), order[] listing each group's tracks by C.  Capped: N layers of
+  // switch words per unit.
   const long long kDecBudget = 64LL << 20;
   std::vector<int> group_first{0};
   long long dec_max = 1, dec_at = 0;
   std::vector<int> ncta(T, 1), order(T);
   for (int t = 0; t < T; ++t) {
     SplitTrack& k = trk[t];
-    const long long need = k.live ? unit_bound[t] * k.nthr : 0;
+    const long long need = k.live ? unit_bound[t] * k.nthr * N : 0;
     if (dec_at > 0 && dec_at + need > kDecBudget) {
       group_first.push_back(t);
       dec_at = 0;
@@ -393,7 +609,7 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~size_t(255); return o; };
   const size_t nv = std::max<size_t>(vids.size(), 1), nunits = (size_t)std::max<long long>(units, 1);
   const size_t o_q = take((size_t)std::max<long long>(q_total, 1) * 8), o_lvl = take(nv * sizeof(SplitLevel)),
-               o_bits = take((size_t)T * sig_words * 4), o_runs = take(nunits * 8), o_arg = take(nunits * 4),
+               o_bits = take((size_t)T * sig_words * 4), o_runs = take(nunits * 8), o_arg = take(nunits * N * 4),
                o_uo = take(nunits * 4), o_nu = take((size_t)T * 4), o_dec = take((size_t)dec_max * 4);
   void* d_ws;
   B2_TRY(b2i_ws(h, b2_ctx::WS_SPLIT, at + 256, &d_ws));
@@ -453,6 +669,45 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   const SplitCues sc{cd.start, cd.end, sample_rate, start_seconds};
+  if (capped) {
+    B2_CUDA(h, cudaFuncSetAttribute(split_capped_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2_CUDA(h, cudaFuncSetAttribute(split_capped_dp_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    for (size_t g = 0; g + 1 < group_first.size(); ++g) {
+      const int g0 = group_first[g], n = group_first[g + 1] - g0;
+      if (n <= 0) continue;
+      for (int i = g0; i < g0 + n;) {
+        const int C = ncta[order[i]];
+        int e = i;
+        while (e < g0 + n && ncta[order[e]] == C) ++e;
+        int thr = kCtaThreads;  // C = 1: CTAs of the bucket's widest track's threads
+        if (C == 1) {
+          thr = 32;
+          for (int x = i; x < e; ++x) thr = std::max<int>(thr, (int)(32 * ceil_div64(trk[order[x]].nthr, 32)));
+        }
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)((e - i) * N * C));
+        cfg.blockDim = dim3((unsigned)thr);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = h->stream;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = (unsigned)(N * C);
+        at[0].val.clusterDim.y = 1;
+        at[0].val.clusterDim.z = 1;
+        cfg.attrs = at;
+        cfg.numAttrs = 1;
+        B2_CUDA(h, cudaLaunchKernelEx(&cfg, split_capped_dp_kernel, d_trk, (const int*)d_order, i, N, (const uint2*)q,
+                                      (const SplitLevel*)lvl, (const uint32_t*)bits, max_runs, penalty, dec, arg, runs,
+                                      nu, d_profile));
+        B2_CHECK_LAUNCH(h, "split_capped_dp_kernel");
+        i = e;
+      }
+      split_capped_backtrack_kernel<<<(unsigned)n, 256, 0, h->stream>>>(
+          d_trk, g0, N, q, lvl, dec, arg, runs, nu, uo, sc, d_cue_offset + c_base, d_n_segments, d_split_score);
+      B2_CHECK_LAUNCH(h, "split_capped_backtrack_kernel");
+    }
+    return B2_OK;
+  }
   for (size_t g = 0; g + 1 < group_first.size(); ++g) {
     const int g0 = group_first[g], n = group_first[g + 1] - g0;
     if (n <= 0) continue;

@@ -37,6 +37,9 @@ constexpr int kMaxRuns = 16384;                  // runs of one track (shared me
 constexpr int kCtaThreads = 512;
 constexpr int kCtaWindow = kOffsetsPerThread * kCtaThreads;  // offsets of one CTA: C = ceil(W / kCtaWindow)
 constexpr int kMaxCluster = 16;                              // non-portable past 8
+// b2_split_tracks_capped: at most kMaxSegments layers, one cluster of N x C CTAs per track (N x C <= the widest
+// cluster of split_capped_dp_kernel the device co-schedules)
+constexpr int kMaxSegments = 16;
 
 SP_HD double sp_add(double a, double b) {
 #ifdef __CUDA_ARCH__

@@ -564,6 +564,25 @@ int b2_split_tracks_wide(b2_handle h, const void* ref, int ref_is_f64, const int
                          const double* ratio /* [T] */, int sample_rate, double start_seconds,
                          int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
                          int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
+/* b2_split_tracks_wide with at most max_segments segments per track (DESIGN.md section 4 "K9s", the capped
+ * programme).  Layer k = 0 .. N-1 (N = max_segments) counts the switches allowed so far:
+ *     V_{0,k}(o) = u_0(o),   V_{j,0}(o) = u_j(o) + V_{j-1,0}(o),
+ *     V_{j,k}(o) = u_j(o) + max(V_{j-1,k}(o), M_{j-1,k-1} - split_penalty)  (k >= 1),   M_{j,k} = max_o V_{j,k}(o)
+ * with b2_split_tracks' rounding, tie and argmax rules.  cue_offset, n_segments (<= N) and split_score come from the
+ * top layer's path; a track with at most N units gets b2_split_tracks_wide's results bit for bit, and N = 1 its
+ * results at split_penalty = +inf.  split_profile [T x N] (f64, in memspace): split_profile[t*N + k] = the best
+ * penalised objective with at most k+1 segments, M_{last,k} (at split_penalty 0 the best plain score per segment
+ * count); NaN for a skipped track, an empty window or (B2_DEVICE) a three-level reference.  Refusals: those of
+ * b2_split_tracks_wide; B2_ERR_BAD_ARG for max_segments < 1; B2_ERR_UNSUPPORTED for max_segments > 16 and for a
+ * track whose N x ceil(window / 16384) CTAs exceed the widest cluster the device co-schedules for this kernel (16 on
+ * an H100: +-60 s at 100 Hz up to N = 16, +-150 s up to N = 8), the message naming the widest window at that N. */
+int b2_split_tracks_capped(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off /* [V+1] */, int V,
+                           const int32_t* track_video /* [T] */, int T, const double* cue_start_s,
+                           const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */,
+                           const double* ratio /* [T] */, int sample_rate, double start_seconds,
+                           int64_t max_offset_samples, double split_penalty, int max_segments, int32_t* cue_offset,
+                           int32_t* n_segments /* [T] */, double* split_score /* [T] */,
+                           double* split_profile /* [T x max_segments] */, int memspace);
 /* try_sync's output step (ffsubsync/ffsubsync.py:272-286, SubtitleScaler + SubtitleShifter) with each cue's own
  * offset: for a track with n_segments > 0, cue i gets timedelta(seconds=t_i * ratio[t]) + timedelta(seconds=
  * cue_offset[i] / sample_rate + apply_offset_seconds), each rounded half-to-even to the microsecond as b2_apply_sync

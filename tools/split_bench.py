@@ -1,7 +1,7 @@
 """Cost of the per-segment offsets (b2_split_tracks) at the bench shape, alone and after the sync step it follows.
 
     python tools/split_bench.py [--pairs 256] [--ratios 5] [--penalty 20] [--repeats 10] [--warmup 2]
-                                [--split-max-offset-seconds S]
+                                [--split-max-offset-seconds S] [--max-segments N]
 
 The workload is bench.py's (BASELINE configs[2]): 256 two-hour pairs (synth.make_pairs, about 1 200 cues each), K = 5,
 +-60 s, PCM synthesised on the device.  Half the pairs get a planted 90 s cut in the middle: 9 000 windows of their
@@ -19,6 +19,11 @@ true_offset - 9000 frames, which the +-60 s window cannot hold for any of the be
 reports the CTAs per track's cluster (ceil(window / 16 384)), and, per penalty, how many cut pairs come back as exactly
 two segments at true_offset and true_offset - 9000 with the break in the middle cue, and how many uncut pairs stay
 whole.
+
+--max-segments N also times the capped split (split_tracks(max_segments=N), b2_split_tracks_capped) alternating with the
+uncapped one in the same repeats, and reports under "capped": its median time, per penalty 0, 20, 200 and 2 000 the
+cut pairs found as exactly two segments at true_offset and true_offset - 9000 and the uncut pairs that stay whole, and
+at penalty 0 the quantiles of split_profile[:, 1] - split_profile[:, 0] over cut and over uncut pairs (N >= 2).
 """
 import argparse
 import json
@@ -44,6 +49,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--split-max-offset-seconds", type=float, default=None)
+    ap.add_argument("--max-segments", type=int, default=None)
     args = ap.parse_args()
 
     import torch
@@ -90,6 +96,10 @@ def main():
         return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
                                split_max_offset_seconds=args.split_max_offset_seconds)
 
+    def split_capped(out, pen=args.penalty):
+        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
+                               split_max_offset_seconds=args.split_max_offset_seconds, max_segments=args.max_segments)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
@@ -99,15 +109,20 @@ def main():
         torch.cuda.synchronize(dev)
         return e0.elapsed_time(e1) / n
 
+    capped = args.max_segments is not None
     out = sync()
     for _ in range(args.warmup):
         split(out)
         split(sync())
+        if capped:
+            split_capped(out)
     torch.cuda.synchronize(dev)
-    split_ms, both_ms = [], []
+    split_ms, both_ms, capped_ms = [], [], []
     for _ in range(args.repeats):   # alternating
         split_ms.append(timed(lambda: split(out), 1))
         both_ms.append(timed(lambda: split(sync()), 1))
+        if capped:
+            capped_ms.append(timed(lambda: split_capped(out), 1))
     res = split(out)
     torch.cuda.synchronize(dev)
     ns = res["n_segments"].cpu().numpy()
@@ -146,13 +161,43 @@ def main():
         segs[str(pen)] = dict(cut_median=float(np.median(n_s[cut])), uncut_median=float(np.median(n_s[~cut])),
                               cut_two=int(np.sum(n_s[cut] == 2)), uncut_one=int(np.sum(n_s[~cut] == 1)),
                               cut_two_at_true_offsets=found)
+    extra = {}
+    if capped:
+        csegs = {}
+        for pen in (0.0, 20.0, 200.0, 2000.0):
+            r = split_capped(out, pen)
+            n_s, c_o = r["n_segments"].cpu().numpy(), r["cue_offset"].cpu().numpy()
+            found = 0
+            for b in np.flatnonzero(cut):
+                if n_s[b] != 2:
+                    continue
+                o = c_o[co[b]:co[b + 1]]
+                t0 = int(pairs.true_offset[b])
+                before, after = np.flatnonzero(o == t0), np.flatnonzero(o == t0 - CUT)
+                found += int(len(before) + len(after) == len(o) and len(before) and len(after)
+                             and before.max() < after.min())
+            csegs[str(pen)] = dict(cut_two_at_true_offsets=found, uncut_one=int(np.sum(n_s[~cut] == 1)),
+                                   cut_two=int(np.sum(n_s[cut] == 2)), segments_hist=np.bincount(
+                                       np.maximum(n_s, 0), minlength=args.max_segments + 1).tolist())
+            if pen == 0.0 and args.max_segments >= 2:
+                prof = r["split_profile"].cpu().numpy()
+                gain = prof[:, 1] - prof[:, 0]
+                q = [0.0, 0.05, 0.25, 0.5, 0.75, 0.95, 1.0]
+                ok = ~np.isnan(gain)
+                gains = dict(quantiles=q, cut=np.quantile(gain[cut & ok], q).round(1).tolist(),
+                             uncut=np.quantile(gain[~cut & ok], q).round(1).tolist())
+        extra = dict(capped=dict(max_segments=args.max_segments, split_ms=round(float(np.median(capped_ms)), 3),
+                                 split_ms_all=[round(x, 3) for x in capped_ms],
+                                 ratio_to_uncapped=round(float(np.median(capped_ms)) / med_split, 2),
+                                 segments_by_penalty=csegs, **({"profile_gain_at_penalty_0": gains}
+                                                               if args.max_segments >= 2 else {})))
     print(json.dumps(dict(info, event="measure", pairs=B, K=len(ratios), penalty=args.penalty, cues=int(co[-1]),
                           split_max_offset_samples=mos, cluster_ctas=sorted(ctas),
                           split_ms=round(med_split, 3), split_ms_all=[round(x, 3) for x in split_ms],
                           sync_plus_split_ms=round(med_both, 3), sync_plus_split_ms_all=[round(x, 3) for x in both_ms],
                           dp_cells=int(cells), dp_cells_per_s=round(cells / (med_split * 1e-3), 1),
                           cut_pairs=int(cut.sum()), cut_pairs_with_two_segments=int(np.sum(ns[cut] == 2)),
-                          uncut_pairs_with_one_segment=int(np.sum(ns[~cut] == 1)), segments_by_penalty=segs)),
+                          uncut_pairs_with_one_segment=int(np.sum(ns[~cut] == 1)), segments_by_penalty=segs, **extra)),
           flush=True)
     return 0
 
