@@ -902,20 +902,35 @@ class BatchSynchronizer:
                              "them" % missing)
         return np.array([pos[int(v)] for v in track_video], dtype=np.int32)
 
-    def _split_window(self, split_max_offset_seconds, max_segments=None):
+    @staticmethod
+    def _split_direction(max_segments, split_direction):
+        """Refuses a split_direction other than None, +1 and -1, and one combined with max_segments."""
+        if split_direction is None:
+            return
+        if isinstance(split_direction, bool) or split_direction not in (1, -1):
+            raise ValueError("split_direction must be None, +1 (offsets only grow) or -1 (only shrink), not %r"
+                             % (split_direction,))
+        if max_segments is not None:
+            raise ValueError("split_direction and max_segments cannot be combined")
+
+    def _split_window(self, split_max_offset_seconds, max_segments=None, split_direction=None):
         """(Handle method, max_offset_samples, arguments after split_penalty) of a split: None keeps the sync window
         and b2_split_tracks; seconds convert as max_offset_seconds does and go through b2_split_tracks_wide.  An integer
-        max_segments goes through b2_split_tracks_capped at either window."""
+        max_segments goes through b2_split_tracks_capped at either window, a split_direction of +-1 through
+        b2_split_tracks_directed."""
         mos = self.max_offset_samples if split_max_offset_seconds is None else \
             abs(int(split_max_offset_seconds * self.sample_rate))
         if max_segments is not None:
             return self.handle.split_tracks_capped, mos, (int(max_segments),)
+        if split_direction is not None:
+            return self.handle.split_tracks_directed, mos, (int(split_direction),)
         if split_max_offset_seconds is None:
             return self.handle.split_tracks, mos, ()
         return self.handle.split_tracks_wide, mos, ()
 
     def split_tracks(self, out, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                     speech_video=None, split_max_offset_seconds=None, max_segments=None) -> dict:
+                     speech_video=None, split_max_offset_seconds=None, max_segments=None,
+                     split_direction=None) -> dict:
         """Per-segment offsets (b2_split_tracks) over the results of a device sync call made with ``speech_video``
         (``out`` carries ``speech`` / ``speech_off``; pass the same speech_video here, None when it listed videos
         0 .. P-1): each track's cue runs are cut into segments with their own offsets, a change of offset costing
@@ -934,8 +949,14 @@ class BatchSynchronizer:
         segment: after a 5 min ad break the later cues need the sync offset plus 300 s.
         ``max_segments`` (None: no cap, the calls above) caps each track at that many segments (b2_split_tracks_capped,
         1 .. 16, at most 8 at +-150 s on an H100) and adds ``split_profile``, a (T, max_segments) f64 tensor: column k
-        is the track's best penalised objective with at most k + 1 segments (NaN for a track n_segments <= 0 marks)."""
+        is the track's best penalised objective with at most k + 1 segments (NaN for a track n_segments <= 0 marks).
+        ``split_direction`` (None: either way, the calls above) makes the offsets move one way only along the track
+        (b2_split_tracks_directed, at either window; same results): +1 when the video has breaks the subtitles lack
+        (ad breaks, an intermission: every break moves the later cues later), -1 when the subtitles have content the
+        video lacks (a cut release, a recap pruned from the video: later cues move earlier).  It cannot be combined
+        with ``max_segments`` (ValueError, as for any value other than None, +1 and -1)."""
         import torch
+        self._split_direction(max_segments, split_direction)
         if "speech" not in out:
             raise ValueError("split_tracks needs the sync call's reference signals: call it with speech_video")
         idx = self._split_refs(out["speech_off"], track_video, speech_video)
@@ -949,7 +970,7 @@ class BatchSynchronizer:
                "split_score": torch.empty(max(T, 1), dtype=torch.float64, device=dev)}
         if max_segments is not None:
             res["split_profile"] = torch.empty((max(T, 1), max(int(max_segments), 1)), dtype=torch.float64, device=dev)
-        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments)
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction)
         split(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep, cue_off, ratio,
               self.sample_rate, self.start_seconds, mos, split_penalty, *cap,
               outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
@@ -959,17 +980,20 @@ class BatchSynchronizer:
         return res
 
     def split_tracks_host(self, res, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
-                          speech_video=None, split_max_offset_seconds=None, max_segments=None) -> dict:
+                          speech_video=None, split_max_offset_seconds=None, max_segments=None,
+                          split_direction=None) -> dict:
         """split_tracks over the tuple of a host sync call made with speech_video (best_score, best_offset, best_k
         first, gss_ratio before the trailing (speech, speech_off) with the search).  Blocks; numpy results.  A reference
         with a third level raises (NativeError, B2_ERR_UNSUPPORTED, naming the video and frame); more than 16 384 kept
         cues in a track too.  ``split_max_offset_seconds`` as for split_tracks: an absolute window shared by all
         segments, which must cover the sync offset plus the breaks before the last segment.  ``max_segments`` as for
-        split_tracks: the result gains ``split_profile``, a (T, max_segments) numpy array."""
+        split_tracks: the result gains ``split_profile``, a (T, max_segments) numpy array.  ``split_direction`` as for
+        split_tracks: +1 for ad breaks or an intermission in the video, -1 for a cut video or a pruned recap."""
+        self._split_direction(max_segments, split_direction)
         speech, speech_off = res[-2], res[-1]
         idx = self._split_refs(speech_off, track_video, speech_video)
         ratio = self.split_ratios(res[2], res[-3] if self.gss else None)
-        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments)
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction)
         outs = split(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off, ratio, self.sample_rate,
                      self.start_seconds, mos, split_penalty, *cap, memspace=_native.B2_HOST)
         return dict(zip(("cue_offset", "n_segments", "split_score", "split_profile"), outs), ratio=ratio)

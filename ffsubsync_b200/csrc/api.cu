@@ -2266,14 +2266,16 @@ extern "C" int b2_apply_sync(b2_handle h, const double* best_score, const int32_
 }
 
 // ---- per-segment offsets with a split penalty (split.cu, sync_output.cu) ---------------------------------------
-// b2_split_tracks, b2_split_tracks_wide and b2_split_tracks_capped: the same checks and outputs, wide: the wider
-// envelope; max_segments > 0 (capped, wide set): at most that many segments and split_profile [T x max_segments]
+// b2_split_tracks, b2_split_tracks_wide, b2_split_tracks_capped and b2_split_tracks_directed: the same checks and
+// outputs, wide: the wider envelope; max_segments > 0 (capped, wide set): at most that many segments and
+// split_profile [T x max_segments]; directed (wide set): offsets monotone in direction +1 or -1
 static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
                         const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
                         const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
                         double start_seconds, int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
                         int32_t* n_segments, double* split_score, int memspace, bool wide, bool capped = false,
-                        int max_segments = 0, double* split_profile = nullptr) {
+                        int max_segments = 0, double* split_profile = nullptr, bool directed = false,
+                        int direction = 0) {
   B2_ENTER(h);
   if (V < 0 || T < 0 || !ref_off || !cue_off || (T && (!track_video || !ratio)))
     B2_FAIL(h, B2_ERR_BAD_ARG, "split: bad arguments (V %d, T %d, null table)", V, T);
@@ -2281,6 +2283,8 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   if (std::isnan(split_penalty) || split_penalty < 0)
     B2_FAIL(h, B2_ERR_BAD_ARG, "split: split_penalty %g must be >= 0 (+inf: no splits)", split_penalty);
   if (capped && max_segments < 1) B2_FAIL(h, B2_ERR_BAD_ARG, "split: max_segments %d must be >= 1", max_segments);
+  if (directed && direction != 1 && direction != -1)
+    B2_FAIL(h, B2_ERR_BAD_ARG, "split: direction %d must be +1 (offsets only grow) or -1 (only shrink)", direction);
   if (sample_rate <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: sample_rate %d <= 0", sample_rate);
   if (ref_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: ref_off[0] %lld < 0", (long long)ref_off[0]);
   for (int v = 0; v < V; ++v) {
@@ -2326,7 +2330,8 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   if (memspace == B2_DEVICE)
     return b2i_split_launch(h, ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                             cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                            false, nullptr, false, wide, cue_offset, n_segments, split_score, N, split_profile);
+                            false, nullptr, false, wide, cue_offset, n_segments, split_score, N, split_profile,
+                            directed ? direction : 0);
   // B2_HOST: the reference staged in, outputs through the staging workspace (cue outputs at their absolute indices)
   void *d_ref, *dout;
   B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, ref, (size_t)ref_off[V] * esz, &d_ref));
@@ -2338,7 +2343,7 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   int32_t* d_co = d_ns + Ts;
   B2_TRY(b2i_split_launch(h, d_ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                           cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                          true, ref, ref_is_f64 != 0, wide, d_co - c0, d_ns, d_sc, N, d_pr));
+                          true, ref, ref_is_f64 != 0, wide, d_co - c0, d_ns, d_sc, N, d_pr, directed ? direction : 0));
   B2_TRY(copy_out(h, cue_offset + c0, d_co, (size_t)n * 4));
   B2_TRY(copy_out(h, n_segments, d_ns, Ts * 4));
   B2_TRY(copy_out(h, split_score, d_sc, Ts * 8));
@@ -2378,6 +2383,17 @@ extern "C" int b2_split_tracks_capped(b2_handle h, const void* ref, int ref_is_f
   return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
                       sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
                       split_score, memspace, true, true, max_segments, split_profile);
+}
+
+extern "C" int b2_split_tracks_directed(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                                        const int32_t* track_video, int T, const double* cue_start_s,
+                                        const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                        const double* ratio, int sample_rate, double start_seconds,
+                                        int64_t max_offset_samples, double split_penalty, int direction,
+                                        int32_t* cue_offset, int32_t* n_segments, double* split_score, int memspace) {
+  return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
+                      sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
+                      split_score, memspace, true, false, 0, nullptr, true, direction);
 }
 
 extern "C" int b2_apply_split(b2_handle h, const double* ratio, const int32_t* n_segments, const int32_t* cue_offset,

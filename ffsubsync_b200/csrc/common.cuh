@@ -69,6 +69,7 @@ struct b2_ctx {
   int64_t launches = 0;
   int split_max_cluster = 0;     // widest split_dp_kernel cluster the device co-schedules (0: not queried yet)
   int split_capped_max_cluster = 0;  // the same for split_capped_dp_kernel
+  int split_directed_max_cluster = 0;  // the same for split_directed_dp_kernel (both directions)
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
   int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
   B2Capture capture;             // set by b2_capture_nominations (tests)
@@ -353,16 +354,21 @@ int b2i_apply_sync_launch(b2_ctx* h, const double* d_bs, const int32_t* d_bo, co
 // wide: b2_split_tracks_wide's envelope (h->split_max_cluster CTAs per track) instead of b2_split_tracks' 32768 offsets.
 // max_segments > 0: b2_split_tracks_capped (at most that many segments, clusters of max_segments x C CTAs up to
 // h->split_capped_max_cluster; wide must be set) and d_profile [T x max_segments] (DEVICE) gets each layer's maximum.
+// direction +1 / -1: b2_split_tracks_directed (offsets only grow / only shrink along the track; clusters up to
+// h->split_directed_max_cluster; wide must be set, max_segments 0).
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
                      const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
                      bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
-                     int* d_n_segments, double* d_split_score, int max_segments = 0, double* d_profile = nullptr);
+                     int* d_n_segments, double* d_split_score, int max_segments = 0, double* d_profile = nullptr,
+                     int direction = 0);
 // Sets h->split_max_cluster (split.cu) if it is not set yet.
 int b2i_split_max_cluster(b2_ctx* h);
 // Sets h->split_capped_max_cluster (split.cu) if it is not set yet.
 int b2i_split_capped_max_cluster(b2_ctx* h);
+// Sets h->split_directed_max_cluster (split.cu) if it is not set yet.
+int b2i_split_directed_max_cluster(b2_ctx* h);
 // b2_apply_split's kernel (sync_output.cu): n_segments / cue_offset / the outputs are DEVICE arrays, ratio [T] and the
 // cue tables HOST arrays (absolute cue indices, as for b2i_apply_sync_launch).
 int b2i_apply_split_launch(b2_ctx* h, const double* ratio, const int32_t* d_n_segments, const int32_t* d_cue_offset,

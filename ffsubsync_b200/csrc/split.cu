@@ -4,11 +4,14 @@
 // tracks' masks at their own ratios) -> per track group split_dp_kernel (the programme, one CTA per track, a
 // switch word per unit and thread to the workspace) -> split_backtrack_kernel (the path, its score and the
 // per-cue offsets).  b2_split_tracks_capped (at most N segments) runs split_capped_dp_kernel (N layers of the
-// programme on one cluster per track) and split_capped_backtrack_kernel in the last two places.
+// programme on one cluster per track) and split_capped_backtrack_kernel in the last two places;
+// b2_split_tracks_directed (offsets monotone in one direction) split_directed_dp_kernel and
+// split_directed_backtrack_kernel.
 #include <limits.h>
 #include <math.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include <cooperative_groups.h>
 
@@ -451,6 +454,175 @@ __global__ void __launch_bounds__(256) split_capped_backtrack_kernel(const Split
   split_cue_offsets(k, s_nu, runs, unit_off, cues, cue_offset);
 }
 
+// b2_split_tracks_directed (offsets only grow, kDir = +1, or only shrink, kDir = -1, along the track): split_dp_kernel's
+// layout, launch and barriers with sp_thread_step_dir.  The step of unit j needs, per thread, the maximum of V_{j-1}
+// over the offsets before its own (kDir = -1: after them), so each unit ends with a cluster-wide exclusive scan of the
+// thread maxima in offset order: a warp scan with shuffles, the warps' totals through alternating shared slots after
+// the unit's __syncthreads (every thread takes the warps before its own), the CTAs' totals through alternating
+// distributed-shared-memory slots after the unit's cluster barrier (rank r takes the ranks before it, kDir = -1 after
+// it).  Per unit j >= 1 each thread writes its switch word to dec[dec_base + 2 j nthr + g] and its record word (the
+// records of V_{j-1}) to dec[dec_base + (2 j + 1) nthr + g]; rank 0's thread 0 writes the last unit's argmax (the
+// warps' and CTAs' maxima merged with sp_merge at that unit only) to arg[unit_base + nu - 1].  Barriers as
+// split_dp_kernel: the early exit is the track's, then per unit one __syncthreads and one cluster barrier in every
+// CTA, owning offsets or not, and one final cluster barrier.
+template <int kDir, bool kCluster>
+__global__ void __launch_bounds__(kCtaThreads) split_directed_dp_kernel(const SplitTrack* __restrict__ trk,
+                                                                        const int* __restrict__ order, int g0,
+                                                                        const uint2* __restrict__ q_all,
+                                                                        const SplitLevel* __restrict__ lvl,
+                                                                        const uint32_t* __restrict__ sub_bits,
+                                                                        int max_runs, double penalty,
+                                                                        uint32_t* __restrict__ dec,
+                                                                        int* __restrict__ arg, int2* __restrict__ runs,
+                                                                        int* __restrict__ n_units) {
+  extern __shared__ int rsm[];
+  int* ra = rsm;
+  int* rb = ra + max_runs;
+  __shared__ int sh[33];
+  __shared__ double smx[2][kCtaThreads / 32];
+  __shared__ int sarg[2][kCtaThreads / 32];
+  __shared__ double cmx[2];
+  __shared__ int carg[2];
+  int C = 1, rank = 0;
+  if constexpr (kCluster) {
+    C = (int)cg::this_cluster().num_blocks();
+    rank = (int)cg::this_cluster().block_rank();
+  }
+  const int t = order[g0 + (int)blockIdx.x / C], tid = threadIdx.x, nw = blockDim.x >> 5;
+  const int lane = tid & 31, warp = tid >> 5;
+  const SplitTrack k = trk[t];
+  if (!k.live || lvl[k.vid].bad >= 0) {
+    if (rank == 0 && tid == 0) n_units[t] = k.live ? -1 : 0;
+    return;
+  }
+  const int n_end = runcorr::rc_decode_runs(sub_bits + k.bits_off, k.S, max_runs, ra, rb, sh);
+  const int nr = min(n_end >> 1, max_runs);
+  __syncthreads();
+  if (rank == 0) {
+    for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
+    if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  }
+  const int nu = nr > 0 ? nr : 1;
+  const uint2* q = q_all + k.q_off;
+  const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+  const int g = rank * (int)blockDim.x + tid;
+  const int o0 = k.o_lo + kOffsetsPerThread * g;
+  const int n_mine = max(0, min(kOffsetsPerThread, k.W - kOffsetsPerThread * g));
+  double v[32];
+  double p = -INFINITY;  // the maximum of V_{j-1} over the offsets on the kDir side behind this thread's
+  for (int j = 0; j < nu; ++j) {
+    const SpUnit u = sp_unit(ra, rb, nr, k.S, j);
+    double best = -INFINITY;
+    int barg = INT_MIN;
+    uint32_t d = 0, rec = 0;
+    if (n_mine > 0) d = sp_thread_step_dir<kDir>(q, k.R, u, o0, n_mine, j == 0, p, penalty, l, v, best, barg, rec);
+    if (j > 0 && g < k.nthr) {
+      uint32_t* w = dec + k.dec_base + 2LL * j * k.nthr + g;
+      w[0] = d;
+      w[k.nthr] = rec;
+    }
+    // exclusive scan of the thread maxima in the direction's order: lanes ...
+    double incl = best;
+    for (int s = 1; s < 32; s <<= 1) {
+      const double y = kDir > 0 ? __shfl_up_sync(0xffffffffu, incl, s) : __shfl_down_sync(0xffffffffu, incl, s);
+      if (kDir > 0 ? lane >= s : lane + s < 32) incl = y > incl ? y : incl;
+    }
+    double ex = kDir > 0 ? __shfl_up_sync(0xffffffffu, incl, 1) : __shfl_down_sync(0xffffffffu, incl, 1);
+    if (lane == (kDir > 0 ? 0 : 31)) ex = -INFINITY;
+    const bool last = j == nu - 1;  // the same in every thread of the cluster
+    if (last)
+      for (int s = 16; s > 0; s >>= 1)
+        sp_merge(best, barg, __shfl_xor_sync(0xffffffffu, best, s), __shfl_xor_sync(0xffffffffu, barg, s));
+    if (lane == (kDir > 0 ? 31 : 0)) {  // the lane holding the warp's total (and, at the last unit, its argmax)
+      smx[j & 1][warp] = incl;
+      sarg[j & 1][warp] = barg;
+    }
+    __syncthreads();
+    // ... the warps ...
+    for (int w = kDir > 0 ? 0 : warp + 1; w < (kDir > 0 ? warp : nw); ++w) {
+      const double x = smx[j & 1][w];
+      ex = x > ex ? x : ex;
+    }
+    double mx = -INFINITY;
+    int am = INT_MIN;
+    if (tid == 0)
+      for (int w = 0; w < nw; ++w) sp_merge(mx, am, smx[j & 1][w], sarg[j & 1][w]);
+    // ... and the CTAs
+    if constexpr (kCluster) {
+      cg::cluster_group cl = cg::this_cluster();
+      if (tid == 0) {
+        cmx[j & 1] = mx;
+        carg[j & 1] = am;
+      }
+      cl.sync();  // barrier.cluster arrive (release) / wait (acquire): the C slots are visible
+      for (int r = kDir > 0 ? 0 : rank + 1; r < (kDir > 0 ? rank : C); ++r) {
+        const double x = *cl.map_shared_rank(&cmx[j & 1], r);
+        ex = x > ex ? x : ex;
+      }
+      if (last && rank == 0 && tid == 0)
+        for (int r = 1; r < C; ++r)
+          sp_merge(mx, am, *cl.map_shared_rank(&cmx[j & 1], r), *cl.map_shared_rank(&carg[j & 1], r));
+    }
+    if (last && rank == 0 && tid == 0) arg[k.unit_base + j] = am;
+    p = ex;
+  }
+  if constexpr (kCluster) cg::this_cluster().sync();
+  if (rank == 0 && tid == 0) n_units[t] = nu;
+}
+
+// The directed path: thread 0 walks back from the last unit's argmax; a set switch bit at (j, o) sends unit j - 1 to
+// the nearest record of V_{j-1} behind o (dir = +1: the largest record below o, -1: the smallest above), which is the
+// argmax of V_{j-1} over that side with ties to the largest offset.  The score and the cue offsets as
+// split_backtrack_kernel.
+__global__ void __launch_bounds__(256) split_directed_backtrack_kernel(const SplitTrack* __restrict__ trk, int t0,
+                                                                       int dir, const uint2* __restrict__ q_all,
+                                                                       const SplitLevel* __restrict__ lvl,
+                                                                       const uint32_t* __restrict__ dec,
+                                                                       const int* __restrict__ arg,
+                                                                       const int2* __restrict__ runs,
+                                                                       const int* __restrict__ n_units, int* unit_off,
+                                                                       SplitCues cues, int* __restrict__ cue_offset,
+                                                                       int* __restrict__ n_segments,
+                                                                       double* __restrict__ split_score) {
+  __shared__ int s_nu;
+  const int t = t0 + blockIdx.x;
+  const SplitTrack k = trk[t];
+  if (threadIdx.x == 0) {
+    const int nu = n_units[t];
+    s_nu = nu;
+    if (nu <= 0) {
+      n_segments[t] = nu;
+      split_score[t] = NAN;
+    } else {
+      int* uo = unit_off + k.unit_base;
+      int m = arg[k.unit_base + nu - 1] - k.o_lo;
+      for (int j = nu - 1; j >= 0; --j) {
+        uo[j] = k.o_lo + m;
+        if (j > 0) {
+          const uint32_t* w = dec + k.dec_base + 2LL * j * k.nthr;
+          if ((w[m >> 5] >> (m & 31)) & 1u) {  // a switch has a record behind it: the scans stop inside the window
+            const uint32_t* rw = w + k.nthr;
+            if (dir > 0) {
+              int i = (m - 1) >> 5;
+              uint32_t b = rw[i] & ((2u << ((m - 1) & 31)) - 1u);  // bits <= m - 1
+              while (b == 0) b = rw[--i];
+              m = 32 * i + 31 - __clz(b);
+            } else {
+              int i = (m + 1) >> 5;
+              uint32_t b = rw[i] & ~((1u << ((m + 1) & 31)) - 1u);  // bits >= m + 1
+              while (b == 0) b = rw[++i];
+              m = 32 * i + __ffs(b) - 1;
+            }
+          }
+        }
+      }
+      split_path_score(k, t, nu, uo, q_all, lvl, runs, n_segments, split_score);
+    }
+  }
+  __syncthreads();
+  split_cue_offsets(k, s_nu, runs, unit_off, cues, cue_offset);
+}
+
 // The widest cluster (CTAs, from kMaxCluster down) of kernel at kCtaThreads threads and the largest run table that
 // the device co-schedules, into *out.
 template <typename Kernel>
@@ -495,17 +667,29 @@ int b2i_split_capped_max_cluster(b2_ctx* h) {
   return split_query_cluster(h, split_capped_dp_kernel, "split_capped_dp_kernel", &h->split_capped_max_cluster);
 }
 
+// split_directed_dp_kernel's widest cluster: the narrower of its two directions' (the same code but for the order of
+// the walk and the scan).
+int b2i_split_directed_max_cluster(b2_ctx* h) {
+  if (h->split_directed_max_cluster > 0) return B2_OK;
+  int up = 0, down = 0;
+  B2_TRY(split_query_cluster(h, split_directed_dp_kernel<1, true>, "split_directed_dp_kernel<1>", &up));
+  B2_TRY(split_query_cluster(h, split_directed_dp_kernel<-1, true>, "split_directed_dp_kernel<-1>", &down));
+  h->split_directed_max_cluster = std::min(up, down);
+  return B2_OK;
+}
+
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
                      const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
                      bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
-                     int* d_n_segments, double* d_split_score, int max_segments, double* d_profile) {
+                     int* d_n_segments, double* d_split_score, int max_segments, double* d_profile, int direction) {
   B2Range range("b2:split (split_ref, raster_bits, split_dp, split_backtrack)");
   if (T <= 0) return B2_OK;
   // the envelope: b2_split_tracks up to kMaxWindow offsets (clusters of 1 or 2 CTAs), b2_split_tracks_wide up to
   // the widest cluster of kCtaThreads-thread CTAs this device co-schedules, b2_split_tracks_capped up to N x C CTAs
-  // of the widest cluster of split_capped_dp_kernel
+  // of the widest cluster of split_capped_dp_kernel, b2_split_tracks_directed up to the widest cluster of
+  // split_directed_dp_kernel
   const bool capped = max_segments > 0;
   const int N = capped ? max_segments : 1;
   long long max_window = kMaxWindow;
@@ -513,6 +697,9 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     if (N > kMaxSegments) B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: max_segments %d is more than %d", N, kMaxSegments);
     B2_TRY(b2i_split_capped_max_cluster(h));
     max_window = (long long)kCtaWindow * (h->split_capped_max_cluster / N);
+  } else if (direction != 0) {
+    B2_TRY(b2i_split_directed_max_cluster(h));
+    max_window = (long long)kCtaWindow * h->split_directed_max_cluster;
   } else if (wide) {
     B2_TRY(b2i_split_max_cluster(h));
     max_window = (long long)kCtaWindow * h->split_max_cluster;
@@ -544,6 +731,11 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
                 "split: track %d: a window of %lld offsets is wider than %lld at %d segments (%d segments x %lld CTAs of "
                 "%d offsets; %d CTAs make the widest cluster this device co-schedules)", t, W, max_window, N, N,
                 (long long)ceil_div64(W, kCtaWindow), kCtaWindow, h->split_capped_max_cluster);
+      if (direction != 0)
+        B2_FAIL(h, B2_ERR_UNSUPPORTED,
+                "split: track %d: a window of %lld offsets is wider than %lld (a cluster of %d CTAs of %d offsets, "
+                "the widest of the directed split this device co-schedules)", t, W, max_window,
+                h->split_directed_max_cluster, kCtaWindow);
       if (wide)
         B2_FAIL(h, B2_ERR_UNSUPPORTED,
                 "split: track %d: a window of %lld offsets is wider than %lld (a cluster of %d CTAs of %d offsets, "
@@ -582,14 +774,15 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   for (int t = 0; t < T; ++t) trk[t].bits_off = (long long)t * sig_words;
   // track groups: the switch words of a group stay within kDecBudget words; within a group the tracks are launched
   // by cluster size C (cluster size is per launch), order[] listing each group's tracks by C.  Capped: N layers of
-  // switch words per unit.
+  // switch words per unit; directed: a switch word and a record word per unit.
   const long long kDecBudget = 64LL << 20;
+  const int words = capped ? N : direction != 0 ? 2 : 1;
   std::vector<int> group_first{0};
   long long dec_max = 1, dec_at = 0;
   std::vector<int> ncta(T, 1), order(T);
   for (int t = 0; t < T; ++t) {
     SplitTrack& k = trk[t];
-    const long long need = k.live ? unit_bound[t] * k.nthr * N : 0;
+    const long long need = k.live ? unit_bound[t] * k.nthr * words : 0;
     if (dec_at > 0 && dec_at + need > kDecBudget) {
       group_first.push_back(t);
       dec_at = 0;
@@ -707,6 +900,56 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
       B2_CHECK_LAUNCH(h, "split_capped_backtrack_kernel");
     }
     return B2_OK;
+  }
+  if (direction != 0) {
+    // the launches of split_dp_kernel below with the directed kernel of direction D
+    auto run = [&](auto dir) -> int {
+      constexpr int D = decltype(dir)::value;
+      B2_CUDA(h, cudaFuncSetAttribute(split_directed_dp_kernel<D, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+      B2_CUDA(h, cudaFuncSetAttribute(split_directed_dp_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+      B2_CUDA(h, cudaFuncSetAttribute(split_directed_dp_kernel<D, true>,
+                                      cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      for (size_t g = 0; g + 1 < group_first.size(); ++g) {
+        const int g0 = group_first[g], n = group_first[g + 1] - g0;
+        if (n <= 0) continue;
+        for (int i = g0; i < g0 + n;) {
+          const int C = ncta[order[i]];
+          int e = i;
+          while (e < g0 + n && ncta[order[e]] == C) ++e;
+          if (C == 1) {  // one CTA of the bucket's widest track's threads
+            int thr = 32;
+            for (int x = i; x < e; ++x) thr = std::max<int>(thr, (int)(32 * ceil_div64(trk[order[x]].nthr, 32)));
+            split_directed_dp_kernel<D, false><<<(unsigned)(e - i), (unsigned)thr, smem, h->stream>>>(
+                d_trk, d_order, i, q, lvl, bits, max_runs, penalty, dec, arg, runs, nu);
+          } else {
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3((unsigned)((e - i) * C));
+            cfg.blockDim = dim3((unsigned)kCtaThreads);
+            cfg.dynamicSmemBytes = smem;
+            cfg.stream = h->stream;
+            cudaLaunchAttribute at[1];
+            at[0].id = cudaLaunchAttributeClusterDimension;
+            at[0].val.clusterDim.x = (unsigned)C;
+            at[0].val.clusterDim.y = 1;
+            at[0].val.clusterDim.z = 1;
+            cfg.attrs = at;
+            cfg.numAttrs = 1;
+            B2_CUDA(h, cudaLaunchKernelEx(&cfg, split_directed_dp_kernel<D, true>, d_trk, (const int*)d_order, i,
+                                          (const uint2*)q, (const SplitLevel*)lvl, (const uint32_t*)bits, max_runs,
+                                          penalty, dec, arg, runs, nu));
+          }
+          B2_CHECK_LAUNCH(h, "split_directed_dp_kernel");
+          i = e;
+        }
+        split_directed_backtrack_kernel<<<(unsigned)n, 256, 0, h->stream>>>(
+            d_trk, g0, D, q, lvl, dec, arg, runs, nu, uo, sc, d_cue_offset + c_base, d_n_segments, d_split_score);
+        B2_CHECK_LAUNCH(h, "split_directed_backtrack_kernel");
+      }
+      return B2_OK;
+    };
+    return direction > 0 ? run(std::integral_constant<int, 1>{}) : run(std::integral_constant<int, -1>{});
   }
   for (size_t g = 0; g + 1 < group_first.size(); ++g) {
     const int g0 = group_first[g], n = group_first[g + 1] - g0;

@@ -1,5 +1,6 @@
 // Per-segment offsets with a split penalty (csrc/split.cu, DESIGN.md section 4 "K9s"): the arithmetic shared by
-// the kernels and their CPU emulations (tests/host_emul/split_emul.cu, split_cluster_emul.cu).
+// the kernels and their CPU emulations (tests/host_emul/split_emul.cu, split_cluster_emul.cu, split_capped_emul.cu,
+// split_directed_emul.cu).
 //
 // A track's subtitle mask (S frames, runs [a_k, b_k) of 1s) is cut into units: unit j is the gap before run j
 // and run j, [start_j, end_j) with start_0 = 0, start_j = b_{j-1}, end_j = b_j, except that the last unit ends at
@@ -155,6 +156,58 @@ SP_HD uint32_t sp_thread_step(const uint2* q, int R, const SpUnit& u, int o0, in
       }
     }
   }
+  return dec;
+}
+
+// The directed programme (b2_split_tracks_directed, direction kDir = +1 or -1): a switch at o may only come from an
+// offset on the kDir side behind it,
+//     P_{j-1}(o) = max { V_{j-1}(o') : o' < o }  (kDir = +1; o' > o for kDir = -1, -inf when empty)
+//     c = P_{j-1}(o) - lambda,   switch = c > V_{j-1}(o),   V_j(o) = u_j(o) + (switch ? c : V_{j-1}(o))
+// with the rounding of sp_thread_step.  p: the exclusive prefix (kDir = -1: suffix) maximum of V_{j-1} over the
+// offsets before o0 (after o0 + n_mine - 1); the thread walks its offsets in the direction's order with a running
+// maximum of the old values.  Bit i of rec is set when V_{j-1}(o0 + i) is a record: >= everything before it
+// (kDir = +1), > everything after it (kDir = -1); a switch's source is the nearest record behind it.  Bit i of the
+// returned word is set when o0 + i switched; best / barg as sp_thread_step.
+template <int kDir>
+SP_HD uint32_t sp_thread_step_dir(const uint2* q, int R, const SpUnit& u, int o0, int n_mine, bool first, double p,
+                                  double penalty, const SpLevels& l, double (&v)[32], double& best, int& barg,
+                                  uint32_t& rec) {
+  uint32_t w_s, w_a, w_b, w_e;
+  int p_s, p_a, p_b, p_e;
+  runcorr::rc_ref_window(q, R, u.start + o0, w_s, p_s);
+  runcorr::rc_ref_window(q, R, u.a + o0, w_a, p_a);
+  runcorr::rc_ref_window(q, R, u.b + o0, w_b, p_b);
+  runcorr::rc_ref_window(q, R, u.end + o0, w_e, p_e);
+  uint32_t dec = 0, rb = 0;
+  best = -INFINITY;
+  barg = -2147483647 - 1;
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    const int i = kDir > 0 ? k : 31 - k;
+    if (i < n_mine) {
+      const uint32_t below = (1u << i) - 1u;
+      const double s = sp_score(u, o0 + i, R, p_s + runcorr::rc_popc(w_s & below), p_a + runcorr::rc_popc(w_a & below),
+                                p_b + runcorr::rc_popc(w_b & below), p_e + runcorr::rc_popc(w_e & below), l);
+      double x;
+      if (first) {
+        x = s;
+      } else {
+        const double old = v[i];
+        rb |= (uint32_t)(kDir > 0 ? old >= p : old > p) << i;
+        const double c = sp_sub(p, penalty);
+        const bool sw = c > old;
+        dec |= (uint32_t)sw << i;
+        x = sp_add(s, sw ? c : old);
+        p = old > p ? old : p;
+      }
+      v[i] = x;
+      if (kDir > 0 ? x >= best : x > best) {  // ties go to the largest offset in either walk
+        best = x;
+        barg = o0 + i;
+      }
+    }
+  }
+  rec = rb;
   return dec;
 }
 

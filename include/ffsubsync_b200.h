@@ -583,6 +583,24 @@ int b2_split_tracks_capped(b2_handle h, const void* ref, int ref_is_f64, const i
                            int64_t max_offset_samples, double split_penalty, int max_segments, int32_t* cue_offset,
                            int32_t* n_segments /* [T] */, double* split_score /* [T] */,
                            double* split_profile /* [T x max_segments] */, int memspace);
+/* b2_split_tracks_wide with segment offsets that only move one way along the track (DESIGN.md section 4 "K9s", the
+ * directed programme).  direction = +1: offsets only grow (the video has breaks the subtitles lack: ad breaks, an
+ * intermission); -1: offsets only shrink (the subtitles have content the video lacks: a cut release, a pruned recap).
+ * A switch at offset o may only come from an offset o' < o (+1) or o' > o (-1):
+ *     P_{j-1}(o) = max { V_{j-1}(o') : o' on that side of o }  (-inf when empty),
+ *     V_j(o) = u_j(o) + max(V_{j-1}(o), P_{j-1}(o) - split_penalty)
+ * with b2_split_tracks' rounding, tie (staying wins) and argmax rules; a switch's source is the argmax of V_{j-1} over
+ * that side, the largest offset among equal maxima.  The path is monotone in the direction, and at split_penalty =
+ * +inf every output equals b2_split_tracks_wide's.  Outputs, memspaces, three-level handling and the 16 384-cue limit
+ * are b2_split_tracks_wide's.  Refusals: those of b2_split_tracks_wide; B2_ERR_BAD_ARG for a direction other than
+ * +-1; B2_ERR_UNSUPPORTED for a window wider than 16 384 offsets x the widest cluster of this call's kernel the
+ * device co-schedules (16 CTAs, 262 144 offsets, on an H100), the message naming the limit. */
+int b2_split_tracks_directed(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off /* [V+1] */, int V,
+                             const int32_t* track_video /* [T] */, int T, const double* cue_start_s,
+                             const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */,
+                             const double* ratio /* [T] */, int sample_rate, double start_seconds,
+                             int64_t max_offset_samples, double split_penalty, int direction, int32_t* cue_offset,
+                             int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
 /* try_sync's output step (ffsubsync/ffsubsync.py:272-286, SubtitleScaler + SubtitleShifter) with each cue's own
  * offset: for a track with n_segments > 0, cue i gets timedelta(seconds=t_i * ratio[t]) + timedelta(seconds=
  * cue_offset[i] / sample_rate + apply_offset_seconds), each rounded half-to-even to the microsecond as b2_apply_sync

@@ -1,7 +1,7 @@
 """Cost of the per-segment offsets (b2_split_tracks) at the bench shape, alone and after the sync step it follows.
 
     python tools/split_bench.py [--pairs 256] [--ratios 5] [--penalty 20] [--repeats 10] [--warmup 2]
-                                [--split-max-offset-seconds S] [--max-segments N]
+                                [--split-max-offset-seconds S] [--max-segments N] [--split-direction {-1,1}]
 
 The workload is bench.py's (BASELINE configs[2]): 256 two-hour pairs (synth.make_pairs, about 1 200 cues each), K = 5,
 +-60 s, PCM synthesised on the device.  Half the pairs get a planted 90 s cut in the middle: 9 000 windows of their
@@ -24,6 +24,12 @@ whole.
 uncapped one in the same repeats, and reports under "capped": its median time, per penalty 0, 20, 200 and 2 000 the
 cut pairs found as exactly two segments at true_offset and true_offset - 9000 and the uncut pairs that stay whole, and
 at penalty 0 the quantiles of split_profile[:, 1] - split_profile[:, 0] over cut and over uncut pairs (N >= 2).
+
+--split-direction D also times the directed split (split_tracks(split_direction=D), b2_split_tracks_directed) alternating
+with the undirected one in the same repeats, and reports under "directed": its median time, and for both directions
+(-1 fits the cut pairs: their later cues sit 90 s earlier) at penalties 0, 20, 200, 2 000 and 20 000 the cut pairs found
+as exactly two segments at true_offset and true_offset - 9000, the uncut pairs that stay whole, and the median segment
+count of each group.
 """
 import argparse
 import json
@@ -50,6 +56,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--split-max-offset-seconds", type=float, default=None)
     ap.add_argument("--max-segments", type=int, default=None)
+    ap.add_argument("--split-direction", type=int, choices=(-1, 1), default=None)
     args = ap.parse_args()
 
     import torch
@@ -100,6 +107,10 @@ def main():
         return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
                                split_max_offset_seconds=args.split_max_offset_seconds, max_segments=args.max_segments)
 
+    def split_directed(out, pen=args.penalty, d=args.split_direction):
+        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
+                               split_max_offset_seconds=args.split_max_offset_seconds, split_direction=d)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
@@ -110,19 +121,24 @@ def main():
         return e0.elapsed_time(e1) / n
 
     capped = args.max_segments is not None
+    directed = args.split_direction is not None
     out = sync()
     for _ in range(args.warmup):
         split(out)
         split(sync())
         if capped:
             split_capped(out)
+        if directed:
+            split_directed(out)
     torch.cuda.synchronize(dev)
-    split_ms, both_ms, capped_ms = [], [], []
+    split_ms, both_ms, capped_ms, directed_ms = [], [], [], []
     for _ in range(args.repeats):   # alternating
         split_ms.append(timed(lambda: split(out), 1))
         both_ms.append(timed(lambda: split(sync()), 1))
         if capped:
             capped_ms.append(timed(lambda: split_capped(out), 1))
+        if directed:
+            directed_ms.append(timed(lambda: split_directed(out), 1))
     res = split(out)
     torch.cuda.synchronize(dev)
     ns = res["n_segments"].cpu().numpy()
@@ -191,6 +207,30 @@ def main():
                                  ratio_to_uncapped=round(float(np.median(capped_ms)) / med_split, 2),
                                  segments_by_penalty=csegs, **({"profile_gain_at_penalty_0": gains}
                                                                if args.max_segments >= 2 else {})))
+    if directed:
+        dsegs = {}
+        for d in (-1, 1):
+            for pen in (0.0, 20.0, 200.0, 2000.0, 20000.0):
+                r = split_directed(out, pen, d)
+                n_s, c_o = r["n_segments"].cpu().numpy(), r["cue_offset"].cpu().numpy()
+                found = 0
+                for b in np.flatnonzero(cut):
+                    if n_s[b] != 2:
+                        continue
+                    o = c_o[co[b]:co[b + 1]]
+                    t0 = int(pairs.true_offset[b])
+                    before, after = np.flatnonzero(o == t0), np.flatnonzero(o == t0 - CUT)
+                    found += int(len(before) + len(after) == len(o) and len(before) and len(after)
+                                 and before.max() < after.min())
+                dsegs["%+d@%s" % (d, pen)] = dict(cut_two_at_true_offsets=found,
+                                                  uncut_one=int(np.sum(n_s[~cut] == 1)),
+                                                  cut_median=float(np.median(n_s[cut])),
+                                                  uncut_median=float(np.median(n_s[~cut])))
+        extra["directed"] = dict(split_direction=args.split_direction,
+                                 split_ms=round(float(np.median(directed_ms)), 3),
+                                 split_ms_all=[round(x, 3) for x in directed_ms],
+                                 ratio_to_undirected=round(float(np.median(directed_ms)) / med_split, 2),
+                                 segments_by_direction_and_penalty=dsegs)
     print(json.dumps(dict(info, event="measure", pairs=B, K=len(ratios), penalty=args.penalty, cues=int(co[-1]),
                           split_max_offset_samples=mos, cluster_ctas=sorted(ctas),
                           split_ms=round(med_split, 3), split_ms_all=[round(x, 3) for x in split_ms],
