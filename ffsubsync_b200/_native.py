@@ -34,7 +34,7 @@ EXPORTS = [
     "b2_sync_tracks_seg", "b2_speech_output", "b2_segment_length", "b2_ingest_begin", "b2_ingest_push",
     "b2_ingest_windows", "b2_ingest_sync_tracks", "b2_ingest_abort", "b2_ingest_segments", "b2_ingest_push_segments",
     "b2_ingest_drop_segment", "b2_ingest_sync_refs", "b2_split_tracks", "b2_split_tracks_wide", "b2_split_tracks_capped",
-    "b2_split_tracks_directed", "b2_apply_split",
+    "b2_split_tracks_directed", "b2_split_tracks_breaks", "b2_apply_split",
 ]
 B2_DETECTOR_ENERGY_ZCR, B2_DETECTOR_AUDITOK = 0, 1   # b2_sync_tracks_subs: the detector of the audio videos
 B2_BEST_K_BAD_SIGNAL = -2   # best_k of the tracks of a video whose stored signal leaves its domain (b2_sync_tracks_sig)
@@ -163,6 +163,8 @@ def load() -> ctypes.CDLL:
                                                                                     ctypes.c_int])
         lib.b2_split_tracks_directed.argtypes = (lib.b2_split_tracks.argtypes[:16] + [ctypes.c_int] +
                                                  lib.b2_split_tracks.argtypes[16:])
+        lib.b2_split_tracks_breaks.argtypes = (lib.b2_split_tracks.argtypes[:16] + [_vp, ctypes.c_int, _vp, _vp, _vp,
+                                                                                    _vp, ctypes.c_int])
         lib.b2_apply_split.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _f64, _vp, _vp,
                                        _vp, ctypes.c_int]
         _lib = lib
@@ -990,9 +992,20 @@ class Handle:
                                   cue_end_s, cue_keep, cue_off, ratio, sample_rate, start_seconds, max_offset_samples,
                                   split_penalty, outs, memspace, direction=direction)
 
+    def split_tracks_breaks(self, ref, ref_is_f64: bool, ref_off, track_video, cue_start_s, cue_end_s, cue_keep,
+                            cue_off, ratio, sample_rate: int, start_seconds: float, max_offset_samples,
+                            split_penalty: float, breaks, outs=None, memspace: int = B2_HOST):
+        """b2_split_tracks_breaks: split_tracks_wide along the stated breaks (a sequence of +1 / -1, the i-th break of a
+        path moving the offset that way).  B2_HOST: returns numpy (cue_offset i32 [cues], n_segments i32 [T],
+        split_score f64 [T], split_profile f64 [T, len(breaks) + 1]).  B2_DEVICE: outs holds those four device pointers
+        in that order; enqueued on the handle's stream, returns outs."""
+        return self._split_tracks("b2_split_tracks_breaks", ref, ref_is_f64, ref_off, track_video, cue_start_s,
+                                  cue_end_s, cue_keep, cue_off, ratio, sample_rate, start_seconds, max_offset_samples,
+                                  split_penalty, outs, memspace, breaks=breaks)
+
     def _split_tracks(self, name, ref, ref_is_f64, ref_off, track_video, cue_start_s, cue_end_s, cue_keep, cue_off,
                       ratio, sample_rate, start_seconds, max_offset_samples, split_penalty, outs, memspace,
-                      max_segments=None, direction=None):
+                      max_segments=None, direction=None, breaks=None):
         ref_off, cue_off = _i64a(ref_off), _i64a(cue_off)
         V, T = len(ref_off) - 1, len(cue_off) - 1
         track_video = np.ascontiguousarray(track_video, dtype=np.int32)
@@ -1006,9 +1019,14 @@ class Handle:
             outs = (np.zeros(n, np.int32), np.zeros(max(T, 0), np.int32), np.zeros(max(T, 0), np.float64))
             if max_segments is not None:
                 outs += (np.zeros((max(T, 0), max(int(max_segments), 1)), np.float64),)
+            if breaks is not None:
+                outs += (np.zeros((max(T, 0), len(breaks) + 1), np.float64),)
         cap = () if max_segments is None else (int(max_segments),)
         if direction is not None:
             cap += (int(direction),)
+        if breaks is not None:
+            brk = np.ascontiguousarray(breaks, dtype=np.int32)
+            cap += (_ptr(brk), len(brk))
         st = getattr(self.lib, name)(
             self.h, _ptr(ref), int(bool(ref_is_f64)), _ptr(ref_off), V, _ptr(track_video), T, _ptr(cue_start_s),
             _ptr(cue_end_s), _ptr(keep), _ptr(cue_off), _ptr(ratio), int(sample_rate), float(start_seconds),

@@ -904,7 +904,8 @@ class BatchSynchronizer:
 
     @staticmethod
     def _split_direction(max_segments, split_direction):
-        """Refuses a split_direction other than None, +1 and -1, and one combined with max_segments."""
+        """Refuses a split_direction other than None, +1 and -1, and one combined with max_segments (at most N
+        segments in direction d are split_breaks=(d,) * (N - 1))."""
         if split_direction is None:
             return
         if isinstance(split_direction, bool) or split_direction not in (1, -1):
@@ -913,13 +914,35 @@ class BatchSynchronizer:
         if max_segments is not None:
             raise ValueError("split_direction and max_segments cannot be combined")
 
-    def _split_window(self, split_max_offset_seconds, max_segments=None, split_direction=None):
+    @staticmethod
+    def _split_breaks(max_segments, split_direction, split_breaks):
+        """split_breaks as a tuple of +-1 ints (None stays None).  Refuses an empty sequence, bools, entries other than
+        +1 and -1, and split_breaks combined with max_segments or split_direction."""
+        if split_breaks is None:
+            return None
+        if isinstance(split_breaks, (str, bytes)) or not hasattr(split_breaks, "__len__"):
+            raise ValueError("split_breaks must be a sequence of +1 / -1, not %r" % (split_breaks,))
+        out = []
+        for d in split_breaks:
+            if isinstance(d, (bool, np.bool_)) or not isinstance(d, (int, np.integer)) or d not in (1, -1):
+                raise ValueError("split_breaks entries must be +1 (the offset grows) or -1 (it shrinks), not %r"
+                                 % (d,))
+            out.append(int(d))
+        if not out:
+            raise ValueError("split_breaks must state at least one break")
+        if max_segments is not None or split_direction is not None:
+            raise ValueError("split_breaks cannot be combined with max_segments or split_direction")
+        return tuple(out)
+
+    def _split_window(self, split_max_offset_seconds, max_segments=None, split_direction=None, split_breaks=None):
         """(Handle method, max_offset_samples, arguments after split_penalty) of a split: None keeps the sync window
         and b2_split_tracks; seconds convert as max_offset_seconds does and go through b2_split_tracks_wide.  An integer
         max_segments goes through b2_split_tracks_capped at either window, a split_direction of +-1 through
-        b2_split_tracks_directed."""
+        b2_split_tracks_directed, a split_breaks tuple through b2_split_tracks_breaks."""
         mos = self.max_offset_samples if split_max_offset_seconds is None else \
             abs(int(split_max_offset_seconds * self.sample_rate))
+        if split_breaks is not None:
+            return self.handle.split_tracks_breaks, mos, (split_breaks,)
         if max_segments is not None:
             return self.handle.split_tracks_capped, mos, (int(max_segments),)
         if split_direction is not None:
@@ -930,7 +953,7 @@ class BatchSynchronizer:
 
     def split_tracks(self, out, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
                      speech_video=None, split_max_offset_seconds=None, max_segments=None,
-                     split_direction=None) -> dict:
+                     split_direction=None, split_breaks=None) -> dict:
         """Per-segment offsets (b2_split_tracks) over the results of a device sync call made with ``speech_video``
         (``out`` carries ``speech`` / ``speech_off``; pass the same speech_video here, None when it listed videos
         0 .. P-1): each track's cue runs are cut into segments with their own offsets, a change of offset costing
@@ -954,9 +977,17 @@ class BatchSynchronizer:
         (b2_split_tracks_directed, at either window; same results): +1 when the video has breaks the subtitles lack
         (ad breaks, an intermission: every break moves the later cues later), -1 when the subtitles have content the
         video lacks (a cut release, a recap pruned from the video: later cues move earlier).  It cannot be combined
-        with ``max_segments`` (ValueError, as for any value other than None, +1 and -1)."""
+        with ``max_segments`` (ValueError, as for any value other than None, +1 and -1); ``split_breaks`` says both.
+        ``split_breaks`` (None: the calls above) states the breaks a user knows of, in track order: a sequence of 1 to
+        15 entries of +1 / -1, e.g. ``(-1,)`` for one cut or ``(1, 1, 1)`` for up to three ad breaks
+        (b2_split_tracks_breaks, at either window).  A track gets at most that many breaks, its i-th break moving the
+        offset the i-th way, and the result gains ``split_profile``, a (T, len(split_breaks) + 1) f64 tensor: column m
+        is the track's best penalised objective with exactly m breaks (-inf when none fits, NaN for a track
+        n_segments <= 0 marks).  ValueError for an empty sequence, bools, other entries, and with ``max_segments`` or
+        ``split_direction``."""
         import torch
         self._split_direction(max_segments, split_direction)
+        split_breaks = self._split_breaks(max_segments, split_direction, split_breaks)
         if "speech" not in out:
             raise ValueError("split_tracks needs the sync call's reference signals: call it with speech_video")
         idx = self._split_refs(out["speech_off"], track_video, speech_video)
@@ -970,30 +1001,35 @@ class BatchSynchronizer:
                "split_score": torch.empty(max(T, 1), dtype=torch.float64, device=dev)}
         if max_segments is not None:
             res["split_profile"] = torch.empty((max(T, 1), max(int(max_segments), 1)), dtype=torch.float64, device=dev)
-        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction)
+        if split_breaks is not None:
+            res["split_profile"] = torch.empty((max(T, 1), len(split_breaks) + 1), dtype=torch.float64, device=dev)
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction, split_breaks)
         split(out["speech"].data_ptr(), True, out["speech_off"], idx, cue_start, cue_end, cue_keep, cue_off, ratio,
               self.sample_rate, self.start_seconds, mos, split_penalty, *cap,
               outs=[t.data_ptr() for t in res.values()], memspace=_native.B2_DEVICE)
         res = {"cue_offset": res["cue_offset"][:n], "n_segments": res["n_segments"][:T],
                "split_score": res["split_score"][:T], "ratio": ratio,
-               **({} if max_segments is None else {"split_profile": res["split_profile"][:T]})}
+               **({} if "split_profile" not in res else {"split_profile": res["split_profile"][:T]})}
         return res
 
     def split_tracks_host(self, res, track_video, cue_start, cue_end, cue_off, cue_keep=None, *, split_penalty: float,
                           speech_video=None, split_max_offset_seconds=None, max_segments=None,
-                          split_direction=None) -> dict:
+                          split_direction=None, split_breaks=None) -> dict:
         """split_tracks over the tuple of a host sync call made with speech_video (best_score, best_offset, best_k
         first, gss_ratio before the trailing (speech, speech_off) with the search).  Blocks; numpy results.  A reference
         with a third level raises (NativeError, B2_ERR_UNSUPPORTED, naming the video and frame); more than 16 384 kept
         cues in a track too.  ``split_max_offset_seconds`` as for split_tracks: an absolute window shared by all
         segments, which must cover the sync offset plus the breaks before the last segment.  ``max_segments`` as for
         split_tracks: the result gains ``split_profile``, a (T, max_segments) numpy array.  ``split_direction`` as for
-        split_tracks: +1 for ad breaks or an intermission in the video, -1 for a cut video or a pruned recap."""
+        split_tracks: +1 for ad breaks or an intermission in the video, -1 for a cut video or a pruned recap.
+        ``split_breaks`` as for split_tracks: the result gains ``split_profile``, a (T, len(split_breaks) + 1) numpy
+        array."""
         self._split_direction(max_segments, split_direction)
+        split_breaks = self._split_breaks(max_segments, split_direction, split_breaks)
         speech, speech_off = res[-2], res[-1]
         idx = self._split_refs(speech_off, track_video, speech_video)
         ratio = self.split_ratios(res[2], res[-3] if self.gss else None)
-        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction)
+        split, mos, cap = self._split_window(split_max_offset_seconds, max_segments, split_direction, split_breaks)
         outs = split(speech, True, speech_off, idx, cue_start, cue_end, cue_keep, cue_off, ratio, self.sample_rate,
                      self.start_seconds, mos, split_penalty, *cap, memspace=_native.B2_HOST)
         return dict(zip(("cue_offset", "n_segments", "split_score", "split_profile"), outs), ratio=ratio)

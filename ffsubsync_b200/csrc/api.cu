@@ -2266,16 +2266,17 @@ extern "C" int b2_apply_sync(b2_handle h, const double* best_score, const int32_
 }
 
 // ---- per-segment offsets with a split penalty (split.cu, sync_output.cu) ---------------------------------------
-// b2_split_tracks, b2_split_tracks_wide, b2_split_tracks_capped and b2_split_tracks_directed: the same checks and
-// outputs, wide: the wider envelope; max_segments > 0 (capped, wide set): at most that many segments and
-// split_profile [T x max_segments]; directed (wide set): offsets monotone in direction +1 or -1
+// b2_split_tracks, b2_split_tracks_wide, b2_split_tracks_capped, b2_split_tracks_directed and b2_split_tracks_breaks:
+// the same checks and outputs, wide: the wider envelope; max_segments > 0 (capped, wide set): at most that many segments and
+// split_profile [T x max_segments]; directed (wide set): offsets monotone in direction +1 or -1; broken (wide set):
+// at most n_breaks breaks in the stated directions and split_profile [T x (n_breaks + 1)]
 static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
                         const int32_t* track_video, int T, const double* cue_start_s, const double* cue_end_s,
                         const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, int sample_rate,
                         double start_seconds, int64_t max_offset_samples, double split_penalty, int32_t* cue_offset,
                         int32_t* n_segments, double* split_score, int memspace, bool wide, bool capped = false,
                         int max_segments = 0, double* split_profile = nullptr, bool directed = false,
-                        int direction = 0) {
+                        int direction = 0, bool broken = false, const int32_t* breaks = nullptr, int n_breaks = 0) {
   B2_ENTER(h);
   if (V < 0 || T < 0 || !ref_off || !cue_off || (T && (!track_video || !ratio)))
     B2_FAIL(h, B2_ERR_BAD_ARG, "split: bad arguments (V %d, T %d, null table)", V, T);
@@ -2285,6 +2286,16 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   if (capped && max_segments < 1) B2_FAIL(h, B2_ERR_BAD_ARG, "split: max_segments %d must be >= 1", max_segments);
   if (directed && direction != 1 && direction != -1)
     B2_FAIL(h, B2_ERR_BAD_ARG, "split: direction %d must be +1 (offsets only grow) or -1 (only shrink)", direction);
+  if (broken) {
+    if (n_breaks < 1 || !breaks)
+      B2_FAIL(h, B2_ERR_BAD_ARG, "split: n_breaks %d must be >= 1 (with a breaks list)", n_breaks);
+    for (int i = 0; i < n_breaks; ++i)
+      if (breaks[i] != 1 && breaks[i] != -1)
+        B2_FAIL(h, B2_ERR_BAD_ARG, "split: breaks[%d] = %d must be +1 (the offset grows) or -1 (it shrinks)", i,
+                breaks[i]);
+    if (n_breaks > 15)  // split::kMaxBreaks: 16 layers of split_breaks_dp_kernel
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: %d breaks is more than 15", n_breaks);
+  }
   if (sample_rate <= 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: sample_rate %d <= 0", sample_rate);
   if (ref_off[0] < 0) B2_FAIL(h, B2_ERR_BAD_ARG, "split: ref_off[0] %lld < 0", (long long)ref_off[0]);
   for (int v = 0; v < V; ++v) {
@@ -2305,7 +2316,7 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   const int64_t c0 = cue_off[0], n = cue_off[T] - c0;
   if (n && (!cue_start_s || !cue_end_s)) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null cue times");
   if (!n_segments || !split_score || (n && !cue_offset)) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null output");
-  if (capped && !split_profile) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null split_profile");
+  if ((capped || broken) && !split_profile) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null split_profile");
   if (ref_off[V] > ref_off[0] && !ref) B2_FAIL(h, B2_ERR_BAD_ARG, "split: null ref");
   // the masks' lengths at each track's ratio (skipped tracks at 1.0), every cue time checked as b2_rasterize does
   std::vector<double> r1(T);
@@ -2324,30 +2335,31 @@ static int split_tracks(b2_handle h, const void* ref, int ref_is_f64, const int6
   B2_CHECK_DEV(h, memspace, cue_offset, "split: cue_offset");
   B2_CHECK_DEV(h, memspace, n_segments, "split: n_segments");
   B2_CHECK_DEV(h, memspace, split_score, "split: split_score");
-  if (capped) B2_CHECK_DEV(h, memspace, split_profile, "split: split_profile");
-  const int N = capped ? max_segments : 0;
+  if (capped || broken) B2_CHECK_DEV(h, memspace, split_profile, "split: split_profile");
+  const int N = capped ? max_segments : broken ? n_breaks + 1 : 0;  // profile columns
   const size_t esz = ref_is_f64 ? 8 : 4;
   if (memspace == B2_DEVICE)
     return b2i_split_launch(h, ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                             cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                            false, nullptr, false, wide, cue_offset, n_segments, split_score, N, split_profile,
-                            directed ? direction : 0);
+                            false, nullptr, false, wide, cue_offset, n_segments, split_score, capped ? N : 0,
+                            split_profile, directed ? direction : 0, breaks, broken ? n_breaks : 0);
   // B2_HOST: the reference staged in, outputs through the staging workspace (cue outputs at their absolute indices)
   void *d_ref, *dout;
   B2_TRY(stage_in(h, b2_ctx::WS_STAGE_IN0, ref, (size_t)ref_off[V] * esz, &d_ref));
   const size_t Ts = (size_t)T;
   B2_TRY(b2i_ws(h, b2_ctx::WS_STAGE_OUT, Ts * 12 + Ts * N * 8 + (size_t)n * 4 + 64, &dout));
   double* d_sc = (double*)dout;
-  double* d_pr = d_sc + Ts;  // [T x N] (capped)
+  double* d_pr = d_sc + Ts;  // [T x N] (capped, breaks)
   int32_t* d_ns = (int32_t*)(d_pr + Ts * N);
   int32_t* d_co = d_ns + Ts;
   B2_TRY(b2i_split_launch(h, d_ref, ref_is_f64 != 0, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep,
                           cue_off, ratio, len.data(), sample_rate, start_seconds, max_offset_samples, split_penalty,
-                          true, ref, ref_is_f64 != 0, wide, d_co - c0, d_ns, d_sc, N, d_pr, directed ? direction : 0));
+                          true, ref, ref_is_f64 != 0, wide, d_co - c0, d_ns, d_sc, capped ? N : 0, d_pr,
+                          directed ? direction : 0, breaks, broken ? n_breaks : 0));
   B2_TRY(copy_out(h, cue_offset + c0, d_co, (size_t)n * 4));
   B2_TRY(copy_out(h, n_segments, d_ns, Ts * 4));
   B2_TRY(copy_out(h, split_score, d_sc, Ts * 8));
-  if (capped) B2_TRY(copy_out(h, split_profile, d_pr, Ts * N * 8));
+  if (capped || broken) B2_TRY(copy_out(h, split_profile, d_pr, Ts * N * 8));
   B2_CUDA(h, cudaStreamSynchronize(h->stream));
   return B2_OK;
 }
@@ -2394,6 +2406,18 @@ extern "C" int b2_split_tracks_directed(b2_handle h, const void* ref, int ref_is
   return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
                       sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
                       split_score, memspace, true, false, 0, nullptr, true, direction);
+}
+
+extern "C" int b2_split_tracks_breaks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off, int V,
+                                      const int32_t* track_video, int T, const double* cue_start_s,
+                                      const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off,
+                                      const double* ratio, int sample_rate, double start_seconds,
+                                      int64_t max_offset_samples, double split_penalty, const int32_t* breaks,
+                                      int n_breaks, int32_t* cue_offset, int32_t* n_segments, double* split_score,
+                                      double* split_profile, int memspace) {
+  return split_tracks(h, ref, ref_is_f64, ref_off, V, track_video, T, cue_start_s, cue_end_s, cue_keep, cue_off, ratio,
+                      sample_rate, start_seconds, max_offset_samples, split_penalty, cue_offset, n_segments,
+                      split_score, memspace, true, false, 0, split_profile, false, 0, true, breaks, n_breaks);
 }
 
 extern "C" int b2_apply_split(b2_handle h, const double* ratio, const int32_t* n_segments, const int32_t* cue_offset,

@@ -70,6 +70,7 @@ struct b2_ctx {
   int split_max_cluster = 0;     // widest split_dp_kernel cluster the device co-schedules (0: not queried yet)
   int split_capped_max_cluster = 0;  // the same for split_capped_dp_kernel
   int split_directed_max_cluster = 0;  // the same for split_directed_dp_kernel (both directions)
+  int split_breaks_max_cluster[8] = {};  // the same for split_breaks_dp_kernel<16, 10, 8, 6, 5, 4, 3, 2>
   uint64_t log2_quirk_mask = 0;  // bit k set: CPython's ceil(math.log(2**k, 2)) == k + 1
   int vad_partition_sms = 0;     // > 0: the lane-per-window VAD runs at most this many CTAs (one per SM)
   B2Capture capture;             // set by b2_capture_nominations (tests)
@@ -356,19 +357,25 @@ int b2i_apply_sync_launch(b2_ctx* h, const double* d_bs, const int32_t* d_bo, co
 // h->split_capped_max_cluster; wide must be set) and d_profile [T x max_segments] (DEVICE) gets each layer's maximum.
 // direction +1 / -1: b2_split_tracks_directed (offsets only grow / only shrink along the track; clusters up to
 // h->split_directed_max_cluster; wide must be set, max_segments 0).
+// n_breaks > 0: b2_split_tracks_breaks (breaks [n_breaks] of +1 / -1, HOST, checked; clusters up to
+// h->split_breaks_max_cluster for the kernel's layer count; wide must be set, max_segments and direction 0) and
+// d_profile [T x (n_breaks + 1)] (DEVICE) gets each exact break count's maximum.
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
                      const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
                      bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
                      int* d_n_segments, double* d_split_score, int max_segments = 0, double* d_profile = nullptr,
-                     int direction = 0);
+                     int direction = 0, const int32_t* breaks = nullptr, int n_breaks = 0);
 // Sets h->split_max_cluster (split.cu) if it is not set yet.
 int b2i_split_max_cluster(b2_ctx* h);
 // Sets h->split_capped_max_cluster (split.cu) if it is not set yet.
 int b2i_split_capped_max_cluster(b2_ctx* h);
 // Sets h->split_directed_max_cluster (split.cu) if it is not set yet.
 int b2i_split_directed_max_cluster(b2_ctx* h);
+// Sets h->split_breaks_max_cluster for split_breaks_dp_kernel<kM> (kM = 32 / (n_breaks + 1) offsets a thread;
+// split.cu) if it is not set yet.
+int b2i_split_breaks_max_cluster(b2_ctx* h, int kM);
 // b2_apply_split's kernel (sync_output.cu): n_segments / cue_offset / the outputs are DEVICE arrays, ratio [T] and the
 // cue tables HOST arrays (absolute cue indices, as for b2i_apply_sync_launch).
 int b2i_apply_split_launch(b2_ctx* h, const double* ratio, const int32_t* d_n_segments, const int32_t* d_cue_offset,

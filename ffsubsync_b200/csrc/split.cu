@@ -623,6 +623,236 @@ __global__ void __launch_bounds__(256) split_directed_backtrack_kernel(const Spl
   split_cue_offsets(k, s_nu, runs, unit_off, cues, cue_offset);
 }
 
+// b2_split_tracks_breaks (breaks d_1 .. d_nb, nb + 1 <= kL = 32 / kM layers): the layers live inside the thread and the
+// offsets are spread over the cluster.  Cluster thread g = rank * blockDim.x + tid owns the kM offsets o_lo + kM g ..
+// and all layers' V for them in registers (kL x kM <= 32 doubles), so C = ceil(W / (kM kCtaThreads)); every launch is a
+// cluster launch (C = 1: one CTA of the bucket's widest track's threads).  Per unit each thread runs
+// sp_thread_step_breaks, then each layer m >= 1 needs the maximum of V_{j,m-1} over the offsets on the d_m side of its
+// own for the next unit: per layer, an exclusive scan of the thread maxima in d_m's order, lanes by shuffles, the
+// warps' totals through alternating shared slots after the unit's __syncthreads, the CTAs' totals through alternating
+// distributed-shared-memory slots after the unit's cluster barrier.  Per unit j >= 1 each thread writes its switch word
+// to dec[dec_base + 2 j nthr + g] and its record word to dec[dec_base + (2 j + 1) nthr + g] (bit m kM + i: layer m,
+// offset i).  At the last unit each layer's maximum and its largest argmax (sp_merge over lanes, warps and CTAs) go to
+// profile[t (nb + 1) + m] and arg[(unit_base + nu - 1)(nb + 1) + m].
+//
+// Barriers as split_dp_kernel<true>: the early exit depends on the track alone and comes before any barrier; then every
+// CTA, owning offsets or not, runs the decode's barriers, per unit one __syncthreads and one cluster barrier, and one
+// final cluster barrier.  A slot written at unit j + 2 was last read at unit j, before the barriers of unit j + 1.
+template <int kM>
+__global__ void __launch_bounds__(kCtaThreads) split_breaks_dp_kernel(const SplitTrack* __restrict__ trk,
+                                                                      const int* __restrict__ order, int g0,
+                                                                      const uint2* __restrict__ q_all,
+                                                                      const SplitLevel* __restrict__ lvl,
+                                                                      const uint32_t* __restrict__ sub_bits,
+                                                                      int max_runs, double penalty, int nb, uint32_t up,
+                                                                      uint32_t* __restrict__ dec,
+                                                                      int* __restrict__ arg, int2* __restrict__ runs,
+                                                                      int* __restrict__ n_units,
+                                                                      double* __restrict__ profile) {
+  constexpr int kL = 32 / kM, kW = kCtaThreads / 32;
+  extern __shared__ int rsm[];
+  int* ra = rsm;
+  int* rb = ra + max_runs;
+  __shared__ int sh[33];
+  __shared__ double smx[2][kL][kW];  // the warps' scan totals per layer
+  __shared__ double cmx[2][kL];      // the CTA's
+  __shared__ double lmx[kL][kW];     // the last unit's maxima and argmaxes: the warps' ...
+  __shared__ int larg[kL][kW];
+  __shared__ double lcmx[kL];        // ... and the CTA's
+  __shared__ int lcarg[kL];
+  cg::cluster_group cl = cg::this_cluster();
+  const int C = (int)cl.num_blocks(), rank = (int)cl.block_rank();
+  const int t = order[g0 + (int)blockIdx.x / C], tid = threadIdx.x, nw = blockDim.x >> 5;
+  const int lane = tid & 31, warp = tid >> 5, L = nb + 1;
+  const SplitTrack k = trk[t];
+  if (!k.live || lvl[k.vid].bad >= 0) {
+    if (rank == 0 && tid < L) profile[(long long)t * L + tid] = NAN;  // L <= 16 <= blockDim.x
+    if (rank == 0 && tid == 0) n_units[t] = k.live ? -1 : 0;
+    return;
+  }
+  const int n_end = runcorr::rc_decode_runs(sub_bits + k.bits_off, k.S, max_runs, ra, rb, sh);
+  const int nr = min(n_end >> 1, max_runs);
+  __syncthreads();
+  if (rank == 0) {
+    for (int r = tid; r < nr; r += blockDim.x) runs[k.unit_base + r] = make_int2(ra[r], rb[r]);
+    if (nr == 0 && tid == 0) runs[k.unit_base] = make_int2(0, 0);  // no run: the one unit [0, S)
+  }
+  const int nu = nr > 0 ? nr : 1;
+  const uint2* q = q_all + k.q_off;
+  const SpLevels l = sp_levels(k.level, lvl[k.vid].beta);
+  const int g = rank * (int)blockDim.x + tid;
+  const int o0 = k.o_lo + kM * g;
+  const int n_mine = max(0, min(kM, k.W - kM * g));
+  double v[kL][kM];
+  double p[kL];
+#pragma unroll
+  for (int m = 0; m < kL; ++m) {
+    p[m] = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < kM; ++i) v[m][i] = -INFINITY;
+  }
+  for (int j = 0; j < nu; ++j) {
+    const SpUnit u = sp_unit(ra, rb, nr, k.S, j);
+    uint32_t d = 0, rec = 0;
+    if (n_mine > 0) sp_thread_step_breaks<kL, kM>(q, k.R, u, o0, n_mine, j == 0, nb, up, p, penalty, l, v, d, rec);
+    if (j > 0 && g < k.nthr) {
+      uint32_t* w = dec + k.dec_base + 2LL * j * k.nthr + g;
+      w[0] = d;
+      w[k.nthr] = rec;
+    }
+    // per layer m >= 1: the exclusive scan of the thread maxima of layer m - 1 in d_m's order, lanes ...
+#pragma unroll
+    for (int m = 1; m < kL; ++m) {
+      if (m > nb) continue;
+      const bool fwd = (up >> m) & 1u;
+      double incl = v[m - 1][0];
+#pragma unroll
+      for (int i = 1; i < kM; ++i) incl = v[m - 1][i] > incl ? v[m - 1][i] : incl;
+      for (int s = 1; s < 32; s <<= 1) {
+        const double y = __shfl_sync(0xffffffffu, incl, fwd ? lane - s : lane + s);
+        if (fwd ? lane >= s : lane + s < 32) incl = y > incl ? y : incl;
+      }
+      const double ex = __shfl_sync(0xffffffffu, incl, fwd ? lane - 1 : lane + 1);
+      p[m] = lane == (fwd ? 0 : 31) ? -INFINITY : ex;
+      if (lane == (fwd ? 31 : 0)) smx[j & 1][m][warp] = incl;  // the lane holding the warp's total
+    }
+    const bool last = j == nu - 1;  // the same in every thread of the cluster
+    if (last) {
+#pragma unroll
+      for (int m = 0; m < kL; ++m) {
+        if (m > nb) continue;
+        double best = -INFINITY;
+        int barg = INT_MIN;
+#pragma unroll
+        for (int i = 0; i < kM; ++i)
+          if (i < n_mine && v[m][i] >= best) {  // increasing offsets: ties go to the largest
+            best = v[m][i];
+            barg = o0 + i;
+          }
+        for (int s = 16; s > 0; s >>= 1)
+          sp_merge(best, barg, __shfl_xor_sync(0xffffffffu, best, s), __shfl_xor_sync(0xffffffffu, barg, s));
+        if (lane == 0) {
+          lmx[m][warp] = best;
+          larg[m][warp] = barg;
+        }
+      }
+    }
+    __syncthreads();
+    // ... the warps ...
+#pragma unroll
+    for (int m = 1; m < kL; ++m) {
+      if (m > nb) continue;
+      const bool fwd = (up >> m) & 1u;
+      double ex = p[m];
+      for (int w = fwd ? 0 : warp + 1; w < (fwd ? warp : nw); ++w) {
+        const double x = smx[j & 1][m][w];
+        ex = x > ex ? x : ex;
+      }
+      p[m] = ex;
+    }
+    if (tid < L) {  // thread m: layer m's CTA scan total (m >= 1; at the last unit also its maximum and argmax)
+      if (tid > 0) {
+        double mx = -INFINITY;
+        for (int w = 0; w < nw; ++w) mx = smx[j & 1][tid][w] > mx ? smx[j & 1][tid][w] : mx;
+        cmx[j & 1][tid] = mx;
+      }
+      if (last) {
+        double lm = -INFINITY;
+        int la = INT_MIN;
+        for (int w = 0; w < nw; ++w) sp_merge(lm, la, lmx[tid][w], larg[tid][w]);
+        lcmx[tid] = lm;
+        lcarg[tid] = la;
+      }
+    }
+    cl.sync();  // barrier.cluster arrive (release) / wait (acquire): the C slots are visible
+    // ... and the CTAs
+#pragma unroll
+    for (int m = 1; m < kL; ++m) {
+      if (m > nb) continue;
+      const bool fwd = (up >> m) & 1u;
+      double ex = p[m];
+      for (int r = fwd ? 0 : rank + 1; r < (fwd ? rank : C); ++r) {
+        const double x = *cl.map_shared_rank(&cmx[j & 1][m], r);
+        ex = x > ex ? x : ex;
+      }
+      p[m] = ex;
+    }
+    if (last && rank == 0 && tid < L) {
+      double lm = lcmx[tid];
+      int la = lcarg[tid];
+      for (int r = 1; r < C; ++r) sp_merge(lm, la, *cl.map_shared_rank(&lcmx[tid], r), *cl.map_shared_rank(&lcarg[tid], r));
+      profile[(long long)t * L + tid] = lm;
+      arg[(k.unit_base + j) * L + tid] = la;
+    }
+  }
+  cl.sync();
+  if (rank == 0 && tid == 0) n_units[t] = nu;
+}
+
+// The path along stated breaks: thread 0 starts at the overall maximum of the last unit over (layer, offset), ties to
+// the largest offset and then the smallest layer; a set switch bit at (j, m, o) sends unit j - 1 to layer m - 1 at the
+// nearest record of V_{j-1,m-1} on the d_m side of o (up: bit m set when d_m = +1), which is the argmax of V_{j-1,m-1}
+// over that side with ties to the largest offset.  The score and the cue offsets as split_backtrack_kernel.
+__global__ void __launch_bounds__(256) split_breaks_backtrack_kernel(const SplitTrack* __restrict__ trk, int t0, int nb,
+                                                                     uint32_t up, int kM,
+                                                                     const uint2* __restrict__ q_all,
+                                                                     const SplitLevel* __restrict__ lvl,
+                                                                     const uint32_t* __restrict__ dec,
+                                                                     const int* __restrict__ arg,
+                                                                     const double* __restrict__ profile,
+                                                                     const int2* __restrict__ runs,
+                                                                     const int* __restrict__ n_units, int* unit_off,
+                                                                     SplitCues cues, int* __restrict__ cue_offset,
+                                                                     int* __restrict__ n_segments,
+                                                                     double* __restrict__ split_score) {
+  __shared__ int s_nu;
+  const int t = t0 + blockIdx.x;
+  const SplitTrack k = trk[t];
+  if (threadIdx.x == 0) {
+    const int nu = n_units[t];
+    s_nu = nu;
+    if (nu <= 0) {
+      n_segments[t] = nu;
+      split_score[t] = NAN;
+    } else {
+      const int L = nb + 1;
+      const int* a = arg + (k.unit_base + nu - 1) * L;
+      const double* pr = profile + (long long)t * L;
+      int ml = 0;  // the end: the largest maximum, then the largest offset, then the smallest layer
+      for (int m = 1; m < L; ++m)
+        if (pr[m] > pr[ml] || (pr[m] == pr[ml] && a[m] > a[ml])) ml = m;
+      int* uo = unit_off + k.unit_base;
+      int x = a[ml] - k.o_lo;  // window index of the offset
+      const uint32_t mask = (1u << kM) - 1u;  // kM <= 16
+      for (int j = nu - 1; j >= 0; --j) {
+        uo[j] = k.o_lo + x;
+        if (j > 0 && ml > 0) {
+          const uint32_t* w = dec + k.dec_base + 2LL * j * k.nthr;
+          const int sh = ml * kM;
+          if ((w[x / kM] >> (sh + x % kM)) & 1u) {  // a switch has a record behind it: the scans stop in the window
+            const uint32_t* rw = w + k.nthr;
+            if ((up >> ml) & 1u) {
+              int i = (x - 1) / kM;
+              uint32_t b = (rw[i] >> sh) & mask & ((2u << ((x - 1) % kM)) - 1u);  // bits <= x - 1
+              while (b == 0) b = (rw[--i] >> sh) & mask;
+              x = kM * i + 31 - __clz(b);
+            } else {
+              int i = (x + 1) / kM;
+              uint32_t b = (rw[i] >> sh) & mask & ~((1u << ((x + 1) % kM)) - 1u);  // bits >= x + 1
+              while (b == 0) b = (rw[++i] >> sh) & mask;
+              x = kM * i + __ffs(b) - 1;
+            }
+            --ml;
+          }
+        }
+      }
+      split_path_score(k, t, nu, uo, q_all, lvl, runs, n_segments, split_score);
+    }
+  }
+  __syncthreads();
+  split_cue_offsets(k, s_nu, runs, unit_off, cues, cue_offset);
+}
+
 // The widest cluster (CTAs, from kMaxCluster down) of kernel at kCtaThreads threads and the largest run table that
 // the device co-schedules, into *out.
 template <typename Kernel>
@@ -678,22 +908,56 @@ int b2i_split_directed_max_cluster(b2_ctx* h) {
   return B2_OK;
 }
 
+// split_breaks_dp_kernel's offsets per thread for nb breaks: the most that leave room for nb + 1 layers of them in 32
+// registers' worth of doubles (8 instantiations), and the index of that instantiation
+static int split_breaks_offsets(int nb) { return 32 / (nb + 1); }
+static int split_breaks_shape(int kM) {
+  return kM >= 16 ? 0 : kM >= 10 ? 1 : kM >= 8 ? 2 : kM >= 6 ? 3 : kM >= 5 ? 4 : kM >= 4 ? 5 : kM >= 3 ? 6 : 7;
+}
+
+// The widest cluster of split_breaks_dp_kernel<kM> (each instantiation queried for itself); once per handle and kM.
+int b2i_split_breaks_max_cluster(b2_ctx* h, int kM) {
+  int* out = &h->split_breaks_max_cluster[split_breaks_shape(kM)];
+  if (*out > 0) return B2_OK;
+  switch (kM) {
+    case 16: return split_query_cluster(h, split_breaks_dp_kernel<16>, "split_breaks_dp_kernel<16>", out);
+    case 10: return split_query_cluster(h, split_breaks_dp_kernel<10>, "split_breaks_dp_kernel<10>", out);
+    case 8: return split_query_cluster(h, split_breaks_dp_kernel<8>, "split_breaks_dp_kernel<8>", out);
+    case 6: return split_query_cluster(h, split_breaks_dp_kernel<6>, "split_breaks_dp_kernel<6>", out);
+    case 5: return split_query_cluster(h, split_breaks_dp_kernel<5>, "split_breaks_dp_kernel<5>", out);
+    case 4: return split_query_cluster(h, split_breaks_dp_kernel<4>, "split_breaks_dp_kernel<4>", out);
+    case 3: return split_query_cluster(h, split_breaks_dp_kernel<3>, "split_breaks_dp_kernel<3>", out);
+    default: return split_query_cluster(h, split_breaks_dp_kernel<2>, "split_breaks_dp_kernel<2>", out);
+  }
+}
+
 int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* ref_off, int V,
                      const int32_t* track_video, int T, const double* cue_start, const double* cue_end,
                      const uint8_t* cue_keep, const int64_t* cue_off, const double* ratio, const int64_t* len,
                      int sample_rate, double start_seconds, int64_t max_offset_samples, double penalty,
                      bool refuse_three_levels, const void* h_ref, bool h_ref_f64, bool wide, int* d_cue_offset,
-                     int* d_n_segments, double* d_split_score, int max_segments, double* d_profile, int direction) {
+                     int* d_n_segments, double* d_split_score, int max_segments, double* d_profile, int direction,
+                     const int32_t* breaks, int n_breaks) {
   B2Range range("b2:split (split_ref, raster_bits, split_dp, split_backtrack)");
   if (T <= 0) return B2_OK;
   // the envelope: b2_split_tracks up to kMaxWindow offsets (clusters of 1 or 2 CTAs), b2_split_tracks_wide up to
   // the widest cluster of kCtaThreads-thread CTAs this device co-schedules, b2_split_tracks_capped up to N x C CTAs
   // of the widest cluster of split_capped_dp_kernel, b2_split_tracks_directed up to the widest cluster of
-  // split_directed_dp_kernel
-  const bool capped = max_segments > 0;
-  const int N = capped ? max_segments : 1;
+  // split_directed_dp_kernel, b2_split_tracks_breaks up to the widest cluster of split_breaks_dp_kernel<kM> of
+  // kCtaThreads x kM offsets a CTA
+  const bool capped = max_segments > 0, broken = n_breaks > 0;
+  const int N = capped ? max_segments : broken ? n_breaks + 1 : 1;
+  const int per_thread = broken ? split_breaks_offsets(n_breaks) : kOffsetsPerThread;  // offsets a thread owns
+  const int cta_window = kCtaThreads * per_thread;
+  uint32_t up = 0;  // bit m: d_m = +1
+  for (int m = 1; m <= n_breaks; ++m) up |= (uint32_t)(breaks[m - 1] > 0) << m;
   long long max_window = kMaxWindow;
-  if (capped) {
+  if (broken) {
+    if (n_breaks > kMaxBreaks)
+      B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: %d breaks is more than %d", n_breaks, kMaxBreaks);
+    B2_TRY(b2i_split_breaks_max_cluster(h, per_thread));
+    max_window = (long long)cta_window * h->split_breaks_max_cluster[split_breaks_shape(per_thread)];
+  } else if (capped) {
     if (N > kMaxSegments) B2_FAIL(h, B2_ERR_UNSUPPORTED, "split: max_segments %d is more than %d", N, kMaxSegments);
     B2_TRY(b2i_split_capped_max_cluster(h));
     max_window = (long long)kCtaWindow * (h->split_capped_max_cluster / N);
@@ -726,6 +990,11 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     if (p.kind != 0) continue;  // no offset survives the mask
     const long long W = p.o_hi - p.o_lo + 1;
     if (W > max_window) {
+      if (broken)
+        B2_FAIL(h, B2_ERR_UNSUPPORTED,
+                "split: track %d: a window of %lld offsets is wider than %lld, the widest at %d breaks (a cluster of %lld "
+                "CTAs of %d offsets, %d offsets a thread; the widest cluster of this kernel the device "
+                "co-schedules)", t, W, max_window, n_breaks, max_window / cta_window, cta_window, per_thread);
       if (capped)
         B2_FAIL(h, B2_ERR_UNSUPPORTED,
                 "split: track %d: a window of %lld offsets is wider than %lld at %d segments (%d segments x %lld CTAs of "
@@ -760,7 +1029,7 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     k.S = (int)len[t];
     k.o_lo = (int)p.o_lo;
     k.W = (int)W;
-    k.nthr = (int)ceil_div64(W, kOffsetsPerThread);
+    k.nthr = (int)ceil_div64(W, per_thread);
     k.ratio = ratio[t];
     k.level = (float)std::min(1.0 / ratio[t], 1.0);
     k.unit_base = units;
@@ -774,9 +1043,10 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   for (int t = 0; t < T; ++t) trk[t].bits_off = (long long)t * sig_words;
   // track groups: the switch words of a group stay within kDecBudget words; within a group the tracks are launched
   // by cluster size C (cluster size is per launch), order[] listing each group's tracks by C.  Capped: N layers of
-  // switch words per unit; directed: a switch word and a record word per unit.
+  // switch words per unit; directed: a switch word and a record word per unit; breaks: a switch word and a record
+  // word per unit, each holding all layers' bits of the thread's 32 / (n + 1) offsets.
   const long long kDecBudget = 64LL << 20;
-  const int words = capped ? N : direction != 0 ? 2 : 1;
+  const int words = capped ? N : (direction != 0 || broken) ? 2 : 1;
   std::vector<int> group_first{0};
   long long dec_max = 1, dec_at = 0;
   std::vector<int> ncta(T, 1), order(T);
@@ -790,7 +1060,7 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
     k.dec_base = dec_at;
     dec_at += need;
     dec_max = std::max(dec_max, dec_at);
-    if (k.live) ncta[t] = (int)ceil_div64(k.W, kCtaWindow);
+    if (k.live) ncta[t] = (int)ceil_div64(k.W, cta_window);
     order[t] = t;
   }
   group_first.push_back(T);
@@ -862,6 +1132,61 @@ int b2i_split_launch(b2_ctx* h, const void* d_ref, bool ref_f64, const int64_t* 
   B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   B2_CUDA(h, cudaFuncSetAttribute(split_dp_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   const SplitCues sc{cd.start, cd.end, sample_rate, start_seconds};
+  if (broken) {
+    // cluster launches of split_breaks_dp_kernel<KM> by cluster size (C = 1: the bucket's widest track's threads)
+    auto run = [&](auto offsets) -> int {
+      constexpr int KM = decltype(offsets)::value;
+      B2_CUDA(h, cudaFuncSetAttribute(split_breaks_dp_kernel<KM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+      B2_CUDA(h, cudaFuncSetAttribute(split_breaks_dp_kernel<KM>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      for (size_t g = 0; g + 1 < group_first.size(); ++g) {
+        const int g0 = group_first[g], n = group_first[g + 1] - g0;
+        if (n <= 0) continue;
+        for (int i = g0; i < g0 + n;) {
+          const int C = ncta[order[i]];
+          int e = i;
+          while (e < g0 + n && ncta[order[e]] == C) ++e;
+          int thr = kCtaThreads;
+          if (C == 1) {
+            thr = 32;
+            for (int x = i; x < e; ++x) thr = std::max<int>(thr, (int)(32 * ceil_div64(trk[order[x]].nthr, 32)));
+          }
+          cudaLaunchConfig_t cfg = {};
+          cfg.gridDim = dim3((unsigned)((e - i) * C));
+          cfg.blockDim = dim3((unsigned)thr);
+          cfg.dynamicSmemBytes = smem;
+          cfg.stream = h->stream;
+          cudaLaunchAttribute at[1];
+          at[0].id = cudaLaunchAttributeClusterDimension;
+          at[0].val.clusterDim.x = (unsigned)C;
+          at[0].val.clusterDim.y = 1;
+          at[0].val.clusterDim.z = 1;
+          cfg.attrs = at;
+          cfg.numAttrs = 1;
+          B2_CUDA(h, cudaLaunchKernelEx(&cfg, split_breaks_dp_kernel<KM>, d_trk, (const int*)d_order, i,
+                                        (const uint2*)q, (const SplitLevel*)lvl, (const uint32_t*)bits, max_runs,
+                                        penalty, n_breaks, up, dec, arg, runs, nu, d_profile));
+          B2_CHECK_LAUNCH(h, "split_breaks_dp_kernel");
+          i = e;
+        }
+        split_breaks_backtrack_kernel<<<(unsigned)n, 256, 0, h->stream>>>(
+            d_trk, g0, n_breaks, up, KM, q, lvl, dec, arg, d_profile, runs, nu, uo, sc, d_cue_offset + c_base,
+            d_n_segments, d_split_score);
+        B2_CHECK_LAUNCH(h, "split_breaks_backtrack_kernel");
+      }
+      return B2_OK;
+    };
+    switch (per_thread) {
+      case 16: return run(std::integral_constant<int, 16>{});
+      case 10: return run(std::integral_constant<int, 10>{});
+      case 8: return run(std::integral_constant<int, 8>{});
+      case 6: return run(std::integral_constant<int, 6>{});
+      case 5: return run(std::integral_constant<int, 5>{});
+      case 4: return run(std::integral_constant<int, 4>{});
+      case 3: return run(std::integral_constant<int, 3>{});
+      default: return run(std::integral_constant<int, 2>{});
+    }
+  }
   if (capped) {
     B2_CUDA(h, cudaFuncSetAttribute(split_capped_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     B2_CUDA(h, cudaFuncSetAttribute(split_capped_dp_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));

@@ -1,6 +1,6 @@
 // Per-segment offsets with a split penalty (csrc/split.cu, DESIGN.md section 4 "K9s"): the arithmetic shared by
 // the kernels and their CPU emulations (tests/host_emul/split_emul.cu, split_cluster_emul.cu, split_capped_emul.cu,
-// split_directed_emul.cu).
+// split_directed_emul.cu, split_breaks_emul.cu).
 //
 // A track's subtitle mask (S frames, runs [a_k, b_k) of 1s) is cut into units: unit j is the gap before run j
 // and run j, [start_j, end_j) with start_0 = 0, start_j = b_{j-1}, end_j = b_j, except that the last unit ends at
@@ -209,6 +209,115 @@ SP_HD uint32_t sp_thread_step_dir(const uint2* q, int R, const SpUnit& u, int o0
   }
   rec = rb;
   return dec;
+}
+
+// The programme along stated breaks (b2_split_tracks_breaks, breaks d_1 .. d_n, each +1 or -1, 1 <= n <= kMaxBreaks):
+// layer m holds the paths with exactly m breaks, the i-th break moving the offset strictly up (d_i = +1) or down (-1),
+//     V_{0,0} = u_0,  V_{0,m} = -inf (m >= 1);  V_{j,0} = u_j + V_{j-1,0}  (layer 0 never switches)
+//     c = P^{d_m}_{j-1,m-1}(o) - lambda,   V_{j,m}(o) = u_j(o) + (c > V_{j-1,m}(o) ? c : V_{j-1,m}(o))  (m >= 1)
+// with P^{+1} the exclusive prefix maximum over o' < o, P^{-1} the exclusive suffix maximum over o' > o (-inf when
+// empty), each operation rounded on its own as in sp_thread_step_dir.  A break's source is the nearest record of
+// V_{j-1,m-1} on the d_m side (sp_thread_step_dir's record rule), so no row is stored.
+constexpr int kMaxBreaks = 15;
+
+// One cell of a layer m >= 1 in the walk of its break (kUp: d_m = +1): old = V_{j-1,m-1}(o), cur = V_{j-1,m}(o) becomes
+// V_{j,m}(o); pm, the maximum of V_{j-1,m-1} behind o, takes old in.  bit: the cell's bit in the switch and record words.
+template <bool kUp>
+SP_HD void sp_break_cell(double s, double old, double& cur, double& pm, double penalty, int bit, uint32_t& d,
+                         uint32_t& r) {
+  r |= (uint32_t)(kUp ? old >= pm : old > pm) << bit;
+  const double c = sp_sub(pm, penalty);
+  const bool sw = c > cur;
+  d |= (uint32_t)sw << bit;
+  cur = sp_add(s, sw ? c : cur);
+  pm = old > pm ? old : pm;
+}
+
+// One thread's step over its kM offsets o0 .. o0 + n_mine - 1 for all layers 0 .. nb (nb + 1 <= kL, kL x kM <= 32) of
+// one unit: u_j is scored once per offset, then the layers are updated from the top down (layer m reads the old values
+// of layer m - 1), each walking the offsets in its break's order; layer 0 (which never switches, and whose old values
+// only layer 1 reads) is updated inside layer 1's walk.  With two layers that walk is the only one and scores u_j
+// itself.  up: bit m set when d_m = +1.  p[m] (m >= 1): the maximum of V_{j-1,m-1} over the offsets on the d_m side
+// behind this thread's.  first: unit 0.  v[m][i] = V_{j,m}(o0 + i); offsets past n_mine and layers past nb keep -inf.
+// Bit m * kM + i of sw is set when o0 + i switched into layer m, of rec when V_{j-1,m-1}(o0 + i) is a record on the d_m
+// side (>= all before it for +1, > all after it for -1).
+template <int kL, int kM>
+SP_HD void sp_thread_step_breaks(const uint2* q, int R, const SpUnit& u, int o0, int n_mine, bool first, int nb,
+                                 uint32_t up, const double (&p)[kL], double penalty, const SpLevels& l,
+                                 double (&v)[kL][kM], uint32_t& sw, uint32_t& rec) {
+  static_assert(kL * kM <= 32, "one bit per layer and offset");
+  constexpr bool kStore = kL > 2;  // more than one walk reads u_j
+  uint32_t w_s, w_a, w_b, w_e;
+  int p_s, p_a, p_b, p_e;
+  runcorr::rc_ref_window(q, R, u.start + o0, w_s, p_s);
+  runcorr::rc_ref_window(q, R, u.a + o0, w_a, p_a);
+  runcorr::rc_ref_window(q, R, u.b + o0, w_b, p_b);
+  runcorr::rc_ref_window(q, R, u.end + o0, w_e, p_e);
+  auto score = [&](int i) {
+    const uint32_t below = (1u << i) - 1u;
+    return sp_score(u, o0 + i, R, p_s + runcorr::rc_popc(w_s & below), p_a + runcorr::rc_popc(w_a & below),
+                    p_b + runcorr::rc_popc(w_b & below), p_e + runcorr::rc_popc(w_e & below), l);
+  };
+  double s[kStore ? kM : 1];
+  if constexpr (kStore) {
+#pragma unroll
+    for (int i = 0; i < kM; ++i) s[i] = i < n_mine ? score(i) : 0.0;
+  }
+  uint32_t d = 0, r = 0;
+  if (first) {
+#pragma unroll
+    for (int i = 0; i < kM; ++i) {
+      if (i < n_mine) {
+        if constexpr (kStore) v[0][i] = s[i];
+        else v[0][i] = score(i);
+      }
+    }
+    sw = 0;
+    rec = 0;
+    return;
+  }
+  if constexpr (kStore) {
+#pragma unroll
+    for (int m = kL - 1; m >= 2; --m) {
+      if (m > nb) continue;
+      double pm = p[m];
+      if ((up >> m) & 1u) {  // both walks unrolled, so every register index is a constant
+#pragma unroll
+        for (int i = 0; i < kM; ++i)
+          if (i < n_mine) sp_break_cell<true>(s[i], v[m - 1][i], v[m][i], pm, penalty, m * kM + i, d, r);
+      } else {
+#pragma unroll
+        for (int i = kM - 1; i >= 0; --i)
+          if (i < n_mine) sp_break_cell<false>(s[i], v[m - 1][i], v[m][i], pm, penalty, m * kM + i, d, r);
+      }
+    }
+  }
+  double pm = p[1];  // layer 1 (nb >= 1), then layer 0 at each offset once layer 1 has read its old value
+  if (up & 2u) {
+#pragma unroll
+    for (int i = 0; i < kM; ++i) {
+      if (i < n_mine) {
+        double si;
+        if constexpr (kStore) si = s[i];
+        else si = score(i);
+        sp_break_cell<true>(si, v[0][i], v[1][i], pm, penalty, kM + i, d, r);
+        v[0][i] = sp_add(si, v[0][i]);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int i = kM - 1; i >= 0; --i) {
+      if (i < n_mine) {
+        double si;
+        if constexpr (kStore) si = s[i];
+        else si = score(i);
+        sp_break_cell<false>(si, v[0][i], v[1][i], pm, penalty, kM + i, d, r);
+        v[0][i] = sp_add(si, v[0][i]);
+      }
+    }
+  }
+  sw = d;
+  rec = r;
 }
 
 // One step of the unit maximum over candidates (warp lanes, a CTA's warps, a cluster's CTAs): the larger value, and

@@ -601,6 +601,32 @@ int b2_split_tracks_directed(b2_handle h, const void* ref, int ref_is_f64, const
                              const double* ratio /* [T] */, int sample_rate, double start_seconds,
                              int64_t max_offset_samples, double split_penalty, int direction, int32_t* cue_offset,
                              int32_t* n_segments /* [T] */, double* split_score /* [T] */, int memspace);
+/* b2_split_tracks_wide along stated breaks (DESIGN.md section 4 "K9s", the programme along breaks): breaks [n_breaks]
+ * (HOST) lists d_1 .. d_n, each +1 (that break moves the offset up: an ad break, an intermission) or -1 (down: a cut,
+ * a pruned recap), 1 <= n <= 15.  A path may have m <= n breaks, and its i-th break (in track order) moves the offset
+ * strictly in direction d_i.  Layer m holds the paths with exactly m breaks:
+ *     V_{0,0} = u_0,  V_{0,m} = -inf (m >= 1),  V_{j,0}(o) = u_j(o) + V_{j-1,0}(o),
+ *     V_{j,m}(o) = u_j(o) + max(V_{j-1,m}(o), P^{d_m}_{j-1,m-1}(o) - split_penalty)  (m >= 1)
+ * with P^{+1} the maximum over o' < o, P^{-1} over o' > o (-inf when empty), and b2_split_tracks' rounding and tie
+ * (staying wins) rules.  The path ends at the largest V_{last,m}(o) over (m, o), ties to the largest offset and then
+ * the smallest m; a break's source is the argmax of V_{j-1,m-1} over the d_m side, the largest offset among equal
+ * maxima.  cue_offset, n_segments (= m + 1) and split_score come from that path.  split_profile [T x (n + 1)] (f64,
+ * in memspace): split_profile[t*(n+1) + m] = max_o V_{last,m}(o), the best penalised objective with exactly m breaks
+ * following d_1 .. d_m (-inf when no such path fits the window or the units, NaN for a track whose n_segments is
+ * <= 0).  At split_penalty = +inf every output equals b2_split_tracks_wide's, with split_profile[t*(n+1)] finite and
+ * the other columns -inf.  Outputs, memspaces, three-level handling and the 16 384-cue limit are b2_split_tracks_wide's.
+ * Refusals: those of b2_split_tracks_wide; B2_ERR_BAD_ARG for n_breaks < 1 or an entry other than +-1;
+ * B2_ERR_UNSUPPORTED for n_breaks > 15 and for a window wider than this call's envelope at that n: 512 x 32 / L
+ * offsets a CTA (L = the smallest of 2, 4, 8, 16 holding n + 1 layers) x the widest cluster of the kernel for L the
+ * device co-schedules, the message naming the limit. */
+int b2_split_tracks_breaks(b2_handle h, const void* ref, int ref_is_f64, const int64_t* ref_off /* [V+1] */, int V,
+                           const int32_t* track_video /* [T] */, int T, const double* cue_start_s,
+                           const double* cue_end_s, const uint8_t* cue_keep, const int64_t* cue_off /* [T+1] */,
+                           const double* ratio /* [T] */, int sample_rate, double start_seconds,
+                           int64_t max_offset_samples, double split_penalty, const int32_t* breaks /* [n_breaks] */,
+                           int n_breaks, int32_t* cue_offset, int32_t* n_segments /* [T] */,
+                           double* split_score /* [T] */, double* split_profile /* [T x (n_breaks + 1)] */,
+                           int memspace);
 /* try_sync's output step (ffsubsync/ffsubsync.py:272-286, SubtitleScaler + SubtitleShifter) with each cue's own
  * offset: for a track with n_segments > 0, cue i gets timedelta(seconds=t_i * ratio[t]) + timedelta(seconds=
  * cue_offset[i] / sample_rate + apply_offset_seconds), each rounded half-to-even to the microsecond as b2_apply_sync

@@ -2,6 +2,7 @@
 
     python tools/split_bench.py [--pairs 256] [--ratios 5] [--penalty 20] [--repeats 10] [--warmup 2]
                                 [--split-max-offset-seconds S] [--max-segments N] [--split-direction {-1,1}]
+                                [--split-breaks D1,D2,..]
 
 The workload is bench.py's (BASELINE configs[2]): 256 two-hour pairs (synth.make_pairs, about 1 200 cues each), K = 5,
 +-60 s, PCM synthesised on the device.  Half the pairs get a planted 90 s cut in the middle: 9 000 windows of their
@@ -30,6 +31,15 @@ with the undirected one in the same repeats, and reports under "directed": its m
 (-1 fits the cut pairs: their later cues sit 90 s earlier) at penalties 0, 20, 200, 2 000 and 20 000 the cut pairs found
 as exactly two segments at true_offset and true_offset - 9000, the uncut pairs that stay whole, and the median segment
 count of each group.
+
+--split-breaks D1,D2,.. (each +1 or -1, e.g. -1 or +1,+1,+1) also times the split along those breaks
+(split_tracks(split_breaks=...), b2_split_tracks_breaks) alternating with the others in the same repeats, and, unless
+they are given, the capped split at N = len(breaks) + 1 and the directed one in the first break's direction, for the
+cost beside them.  It reports under "breaks": its median time and its ratio to the plain, capped and directed calls'
+medians; per penalty 0, 20, 200, 2 000 and 20 000 the cut pairs found as exactly two segments at true_offset and
+true_offset - 9000, the uncut pairs that stay whole, the median segment count of each group and the histogram of
+segment counts; and, per penalty, the quantiles of split_profile[:, 1] - split_profile[:, 0] over cut and over uncut
+pairs.
 """
 import argparse
 import json
@@ -57,7 +67,15 @@ def main():
     ap.add_argument("--split-max-offset-seconds", type=float, default=None)
     ap.add_argument("--max-segments", type=int, default=None)
     ap.add_argument("--split-direction", type=int, choices=(-1, 1), default=None)
+    ap.add_argument("--split-breaks", type=str, default=None)
     args = ap.parse_args()
+    brk = None
+    if args.split_breaks is not None:
+        brk = tuple(int(x) for x in args.split_breaks.split(","))
+        if args.max_segments is None:
+            args.max_segments = len(brk) + 1
+        if args.split_direction is None:
+            args.split_direction = brk[0]
 
     import torch
     from ffsubsync_b200 import _native
@@ -111,6 +129,10 @@ def main():
         return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
                                split_max_offset_seconds=args.split_max_offset_seconds, split_direction=d)
 
+    def split_breaks(out, pen=args.penalty):
+        return bs.split_tracks(out, tv, cs, ce, co, split_penalty=pen,
+                               split_max_offset_seconds=args.split_max_offset_seconds, split_breaks=brk)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
@@ -130,8 +152,10 @@ def main():
             split_capped(out)
         if directed:
             split_directed(out)
+        if brk is not None:
+            split_breaks(out)
     torch.cuda.synchronize(dev)
-    split_ms, both_ms, capped_ms, directed_ms = [], [], [], []
+    split_ms, both_ms, capped_ms, directed_ms, breaks_ms = [], [], [], [], []
     for _ in range(args.repeats):   # alternating
         split_ms.append(timed(lambda: split(out), 1))
         both_ms.append(timed(lambda: split(sync()), 1))
@@ -139,6 +163,8 @@ def main():
             capped_ms.append(timed(lambda: split_capped(out), 1))
         if directed:
             directed_ms.append(timed(lambda: split_directed(out), 1))
+        if brk is not None:
+            breaks_ms.append(timed(lambda: split_breaks(out), 1))
     res = split(out)
     torch.cuda.synchronize(dev)
     ns = res["n_segments"].cpu().numpy()
@@ -231,6 +257,38 @@ def main():
                                  split_ms_all=[round(x, 3) for x in directed_ms],
                                  ratio_to_undirected=round(float(np.median(directed_ms)) / med_split, 2),
                                  segments_by_direction_and_penalty=dsegs)
+    if brk is not None:
+        bsegs, bgain = {}, {}
+        q = [0.0, 0.05, 0.25, 0.5, 0.75, 0.95, 1.0]
+        for pen in (0.0, 20.0, 200.0, 2000.0, 20000.0):
+            r = split_breaks(out, pen)
+            n_s, c_o = r["n_segments"].cpu().numpy(), r["cue_offset"].cpu().numpy()
+            found = 0
+            for b in np.flatnonzero(cut):
+                if n_s[b] != 2:
+                    continue
+                o = c_o[co[b]:co[b + 1]]
+                t0 = int(pairs.true_offset[b])
+                before, after = np.flatnonzero(o == t0), np.flatnonzero(o == t0 - CUT)
+                found += int(len(before) + len(after) == len(o) and len(before) and len(after)
+                             and before.max() < after.min())
+            bsegs[str(pen)] = dict(cut_two_at_true_offsets=found, uncut_one=int(np.sum(n_s[~cut] == 1)),
+                                   cut_median=float(np.median(n_s[cut])), uncut_median=float(np.median(n_s[~cut])),
+                                   segments_hist=np.bincount(np.maximum(n_s, 0), minlength=len(brk) + 2).tolist())
+            prof = r["split_profile"].cpu().numpy()
+            gain = prof[:, 1] - prof[:, 0]
+            ok = np.isfinite(gain)
+            bgain[str(pen)] = dict(cut=np.quantile(gain[cut & ok], q).round(1).tolist() if (cut & ok).any() else [],
+                                   uncut=np.quantile(gain[~cut & ok], q).round(1).tolist() if (~cut & ok).any() else [],
+                                   not_finite=int(np.sum(~ok)))
+        med_b = float(np.median(breaks_ms))
+        extra["breaks"] = dict(split_breaks=list(brk), split_ms=round(med_b, 3),
+                               split_ms_all=[round(x, 3) for x in breaks_ms],
+                               ratio_to_plain=round(med_b / med_split, 2),
+                               ratio_to_capped=round(med_b / float(np.median(capped_ms)), 2),
+                               ratio_to_directed=round(med_b / float(np.median(directed_ms)), 2),
+                               segments_by_penalty=bsegs,
+                               profile_gain_quantiles=q, profile_gain_by_penalty=bgain)
     print(json.dumps(dict(info, event="measure", pairs=B, K=len(ratios), penalty=args.penalty, cues=int(co[-1]),
                           split_max_offset_samples=mos, cluster_ctas=sorted(ctas),
                           split_ms=round(med_split, 3), split_ms_all=[round(x, 3) for x in split_ms],
